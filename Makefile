@@ -1,5 +1,5 @@
 # Build / test entry points (reference: Makefile:40-90 + .github/workflows/main.yml). The real build logic lives in
-# distributed_llama_b200/_build.py (g++ for the host library and native front ends, nvcc -gencode arch=compute_100a,code=sm_100a
+# distributed_llama_b200/_build.py (g++ for the host library and native front ends, nvcc -gencode arch=compute_90a,code=sm_90a
 # for the CUDA library); these targets only name the common invocations.
 PY ?= python
 
@@ -15,7 +15,7 @@ native: build
 test:             ## CPU tests (formats, tokenizer, converters, apps, native API server, reference-binary parity)
 	$(PY) -m pytest tests -q -m "not gpu"
 
-test-gpu:         ## needs a B200
+test-gpu:         ## needs an H100
 	$(PY) -m pytest tests -q -m gpu
 
 bench:
@@ -24,7 +24,7 @@ bench:
 smoke:
 	$(PY) -c "import __graft_entry__ as g; g.build(); g.smoke()"
 
-sanitize:         ## compute-sanitizer memcheck over every kernel family (needs a B200)
+sanitize:         ## compute-sanitizer memcheck over every kernel family (needs an H100)
 	bash tools/sanitize.sh memcheck
 
 clean:

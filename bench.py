@@ -1,15 +1,16 @@
 #!/usr/bin/env python
-"""Headline benchmark: batch-1 decode tokens/s (+ prefill TTFT) of Llama-3.1-8B q40, tensor-parallel over N B200s.
+"""Headline benchmark: batch-1 decode tokens/s (+ prefill TTFT) of Llama-3.1-8B q40, tensor-parallel over N H100s.
 
     python bench.py --gpus 1 --steps 64 --warmup 8
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 4 --master-addr 127.0.0.1 --master-port 29501 \
         bench.py --gpus 4 --steps 64 --warmup 8
-    python bench.py --impl reference --gpus 1 --steps 32 --warmup 3     # unmodified reference (CPU build, TCP loopback)
+    python bench.py --impl reference --gpus 1 --steps 32 --warmup 3     # unmodified reference (CPU build in oracle/_ref, TCP loopback)
+    python bench.py --gpus 1 --steps 64 --warmup 8 --dump-outputs out/  # also writes the last timed step's outputs as .npy
 
 Metric definition follows the reference's own benchmark mode (`dllama inference`, src/dllama.cpp:76-115): one "step"
 is one generated token of a single sequence (forward of 1 token through all layers + sampling); `value` is the
 whole-job tokens/s. The model is random-init in the real `.m` layout (no network for checkpoints); weights (4.5 GB) are
-far larger than L2 (126 MB) so every step streams them from HBM — no L2 flush is needed between steps.
+far larger than the H100's L2 (50 MB) so every step streams them from HBM — no L2 flush is needed between steps.
 """
 from __future__ import annotations
 
@@ -109,6 +110,13 @@ class ClockSampler:
         return {"sm_mhz": med, "sm_max_mhz": max_clock or None, "reasons": sorted(reasons), "samples": len(clocks)}
 
 
+def dump_outputs(out_dir: str, tokens):
+    """What the timed decode returned to its caller: the greedy token ids of the timed steps, in order (float64)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "tokens.npy"), np.asarray(tokens, dtype=np.float64))
+
+
 # ------------------------------------------------------------------------------------------------------------
 def run_ours(args):
     import torch
@@ -187,6 +195,8 @@ def run_ours(args):
     e.record()
     barrier()
     dev_ms = max_over_ranks(s.elapsed_time(e))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, toks)
     # long-context decode: the same step at position 2048 (the KV rows below it hold whatever the cache was initialised with —
     # only the attention cost over 2048 positions is of interest)
     extra = {}
@@ -245,7 +255,9 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm = peaks.get("hbm_gbs", 6650.0)
+        hbm, hbm_source = peaks.get("hbm_gbs"), "measured"
+        if not hbm:
+            hbm, hbm_source = 3350.0, "H100 SXM data sheet"
         out = {
             "metric": "decode tokens/sec (batch-1 sequence, greedy) + prefill TTFT, Llama-3.1-8B q40" if args.model == "llama-3.1-8b"
                       else f"decode tokens/sec + prefill TTFT, {args.model} q40",
@@ -254,13 +266,14 @@ def run_ours(args):
             "vs_baseline": round(value / base, 2), "dtype": "q40 weights, q80 activations (int8 dp4a), bf16 KV, f32 accum",
             "data": "synthetic (random-init weights in .m layout, synthetic prompt)",
             "config": {"model": args.model, "global_batch": 1, "seq_len": args.prompt_len + steps, "prompt_len": args.prompt_len,
-                       "parallelism": f"tp{args.gpus}", "decode_path": "persistent megakernel" if (eng.mega and eng.mega_active) else "multi-kernel PDL chain", "l2_policy": "weights per step (%.2f GB/GPU) >> 126 MB L2, no flush needed" % (weight_bytes / 1e9),
+                       "parallelism": f"tp{args.gpus}", "decode_path": "persistent megakernel" if (eng.mega and eng.mega_active) else "multi-kernel PDL chain", "l2_policy": "weights per step (%.2f GB/GPU) >> 50 MB L2, no flush needed" % (weight_bytes / 1e9),
                        "baseline_ref": "reference published Llama-2-7B q40 ms/token on %d x RPi 4B (report.pdf)" % args.gpus},
             "ttft_ms": round(ttft_ms, 3), "prefill_tokens_per_s": round(args.prompt_len / ttft_ms * 1e3, 1),
             "e2e": {"value": round(steps / e2e_ms * 1e3, 2), "unit": "tokens/s", "h2d_bytes_per_step": 8, "d2h_bytes_per_step": 4},
             "gpu_launches": eng.launches_per_decode_step * steps,
             "hbm_roofline": {"weight_bytes_per_step_per_gpu": weight_bytes, "achieved_gbs": round(weight_bytes / ms_per_step / 1e6, 1),
-                             "frac_of_measured_hbm": round(weight_bytes / ms_per_step / 1e6 / hbm, 3)},
+                             "frac_of_peak_hbm": round(weight_bytes / ms_per_step / 1e6 / hbm, 3), "peak_hbm_gbs": hbm,
+                             "peak_hbm_source": hbm_source},
             "clocks": clocks, "tokens_agree": e2e_tokens == toks, "impl": "ours",
             "tokens_sha": hashlib.sha1(",".join(map(str, toks[:16])).encode()).hexdigest()[:16],   # first 16 greedy tokens: TP=N must equal TP=1
             "load_s": round(load_s, 2), "bytes_uploaded_per_rank": int(sess.weights.bytes_uploaded),
@@ -274,24 +287,10 @@ def run_ours(args):
 
 # ------------------------------------------------------------------------------------------------------------
 def ref_binary():
-    src = os.path.join(ROOT, "baseline", "_ref", "distributed-llama")
-    exe = os.path.join(src, "dllama")
-    if not os.path.isdir(src):
-        if os.path.isdir("/root/reference"):
-            os.makedirs(os.path.dirname(src), exist_ok=True)
-            shutil.copytree("/root/reference", src)
-            subprocess.run(["chmod", "-R", "u+w", src])
-        else:
-            return None, "reference sources not present under baseline/_ref"
-    # always (re)build on the box we run on: the reference Makefile uses -march=native
-    stamp = os.path.join(src, ".built_on")
-    host_id = open("/proc/cpuinfo").read().split("model name")[1].split("\n")[0] if os.path.exists("/proc/cpuinfo") else "?"
-    if not os.path.exists(exe) or not os.path.exists(stamp) or open(stamp).read() != host_id:
-        subprocess.run(["make", "clean"], cwd=src, stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
-        r = subprocess.run(["make", "dllama", f"-j{os.cpu_count() or 4}"], cwd=src, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-        if r.returncode != 0 or not os.path.exists(exe):
-            return None, "reference build failed: " + r.stdout[-300:].replace("\n", " ")
-        open(stamp, "w").write(host_id)
+    """The reference's `dllama`, built beforehand into oracle/_ref (oracle/README.md); this script never builds it."""
+    exe = os.path.join(ROOT, "oracle", "_ref", "dllama")
+    if not os.access(exe, os.X_OK):
+        return None, "reference binary not present (oracle/_ref/dllama, see oracle/README.md)"
     return exe, None
 
 
@@ -360,7 +359,7 @@ def _run_reference_once(exe, args, model_path, tok_path, n, threads, steps, warm
 
 
 def run_reference(args):
-    """Reference arm: the UNMODIFIED reference tree (baseline/_ref/distributed-llama), built with its own Makefile, driven through
+    """Reference arm: the UNMODIFIED reference (oracle/_ref/dllama), built with its own Makefile, driven through
     its own CLI. The only thing chosen here is how it is launched: `--nthreads` is swept over the power-of-two counts that fit the
     physical cores available to each of the n processes (short probe runs), processes are pinned to disjoint CPU sets, and the
     best configuration is then timed on the full step count."""
@@ -440,6 +439,8 @@ def main():
     ap.add_argument("--max-seq-len", type=int, default=4096)
     ap.add_argument("--ref-timeout", type=int, default=1500)
     ap.add_argument("--decode-path", default="mega", choices=["multi", "mega"], help="multi-kernel PDL chain or persistent megakernel")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed run returned (DIR/tokens.npy) for output comparison")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

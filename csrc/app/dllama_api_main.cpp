@@ -1,5 +1,5 @@
 // `dllama-api-native`: the OpenAI-style HTTP server of the reference (src/dllama-api.cpp:602-632) as a native binary on one
-// B200 — api_server.cpp (HTTP, JSON, NaiveCache, templates, stop detection) over NativeEngine. Multi-GPU serving: ./dllama-api --gpus N.
+// GPU — api_server.cpp (HTTP, JSON, NaiveCache, templates, stop detection) over NativeEngine. Multi-GPU serving: ./dllama-api --gpus N.
 #include <chrono>
 #include <cstdio>
 #include <cstring>

@@ -306,7 +306,7 @@ int main(int argc, char **argv) {
         if (job.nRanks > 1)
             std::printf("🔗 %u GPUs (one process each), all-reduce inside the kernels over %s\n", job.nRanks,
                         app.engine.multicast() ? "the NVSwitch multicast mapping (multimem.st)" : "NVLink peer memory");
-        std::printf("🧠 GPU %d: sm_100a kernels, %s decode; %.2f GB of weights uploaded%s\n", a.gpuIndex,
+        std::printf("🧠 GPU %d: sm_90a kernels, %s decode; %.2f GB of weights uploaded%s\n", a.gpuIndex,
                     app.engine.persistentKernel() ? "persistent-kernel" : "multi-kernel", app.engine.bytesUploaded() / 1e9,
                     job.nRanks > 1 ? " by this rank" : "");
         std::printf("💿 Weights loaded\n");

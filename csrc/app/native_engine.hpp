@@ -1,5 +1,5 @@
 // Python-free runtime of one GPU: maps a `.m` file, uploads + re-tiles the q40 weights, owns the device buffers and drives the
-// engine in _cuda.so (persistent decode kernel, tcgen05 prefill, CUDA-graph greedy loop).
+// engine in _cuda.so (persistent decode kernel, tensor-core prefill, CUDA-graph greedy loop).
 //
 // Role in the reference: loadLlmNetWeight + NnExecutor/NnCpuDevice set-up + RootLlmInference (src/llm.cpp:614-669,
 // src/nn/nn-cpu.cpp:41-148, src/app.cpp:168-208) for the single-node case. The tensor-parallel launcher (one process per GPU,

@@ -1,26 +1,28 @@
-// Prompt-chunk (prefill) attention on the 5th-generation tensor cores: S = Q.K^T and O = P.V are tcgen05.mma instructions with
-// the accumulators in tensor memory; K and V tiles stream from the bf16 head-major KV cache through TMA tensor maps.
+// Prompt-chunk (prefill) attention on the Hopper tensor cores: S = Q.K^T and O = P.V are wgmma.mma_async instructions with the
+// accumulators in registers; K and V tiles stream from the bf16 head-major KV cache through TMA tensor maps.
 //
 // Work item (one CTA) = one KV head x one query tile. The `kvMul` query heads that share the KV head (GQA) are packed on the
 // MMA M dimension: a tile holds tq = 128 / kvMul consecutive prompt tokens x kvMul heads = up to 128 query rows, so every K / V
 // tile fetched from the cache is used by all heads of the group. KV is walked in tiles of 128 positions, causal inside the chunk
 // (row of token t sees positions <= p0 + t). Two passes over the KV tiles keep the kernel free of accumulator rescaling:
-//   pass 1: S tiles -> per-row running maximum m and normaliser l (registers of the softmax warps)
-//   pass 2: S tiles again -> P = exp2(S - m) as bf16 into shared memory (canonical K-major SWIZZLE_128B tile) -> O += P.V
-// Warp roles: 0 = TMA producer, 1 = MMA issuer (one elected lane), 2 = TMEM allocator, 4..7 = softmax / epilogue (thread = query
-// row = TMEM lane). S is double-buffered in TMEM so QK^T of tile j+1 overlaps the softmax of tile j.
+//   pass 1: S tiles -> per-row running maximum m and normaliser l
+//   pass 2: S tiles again -> P = exp2(S - m) as bf16 registers (the A operand of the next wgmma) -> O += P.V
+// Warp roles: 0 = TMA producer; warps 4..7 and 8..11 = two consumer warpgroups, each owning 64 query rows of the tile (wgmma M = 64).
+// Each 128-position KV tile is processed as two halves of 64 positions (S half = 32 registers a thread).
 //
 // Replaces (reference): OP_MULTIHEAD_ATT over a prompt chunk, multiheadAtt_F32 + softmax_F32 per (head, batch row)
 // (src/nn/nn-cpu-ops.cpp:753-788,1260-1286) and the round-1 fallback that ran the decode kernel once per (head, token).
 #include <cuda.h>
 
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace dl {
 namespace {
 
-constexpr int kApThreads = 256;
+constexpr int kApThreads = 384;
 constexpr uint32_t kApAtomBytes = 16384;   // one [128 rows x 64 bf16] SWIZZLE_128B atom column
+constexpr uint32_t kApConsumerWarps = 8;
 
 __device__ __forceinline__ uint32_t apAddr(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void apBarInit(uint64_t *b, uint32_t c) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(apAddr(b)), "r"(c) : "memory"); }
@@ -39,45 +41,9 @@ __device__ __forceinline__ void apTmaLoad2d(void *dst, const CUtensorMap *map, u
                  "l"(reinterpret_cast<uint64_t>(map)), "r"(apAddr(bar)), "r"(c0), "r"(c1)
                  : "memory");
 }
-__device__ __forceinline__ void apFenceAfter() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void apFenceBefore() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void apUmma(uint32_t tmemD, uint64_t descA, uint64_t descB, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmemD), "l"(descA),
-        "l"(descB), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void apCommit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(apAddr(bar)) : "memory");
-}
-__device__ __forceinline__ void apTmemLoad32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, "
-        "%20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// one lane of a converged warp; the predicate form keeps the enclosed tcgen05 operands in uniform registers
-__device__ __forceinline__ bool apElectOne() {
-    uint32_t p;
-    asm volatile("{\n.reg .pred P;\nelect.sync _|P, 0xffffffff;\nselp.u32 %0, 1, 0, P;\n}\n" : "=r"(p));
-    return p != 0;
-}
-
-// Shared-memory matrix descriptors (sm_100 version 1, SWIZZLE_128B).
-//   K-major  : rows of 128 B (64 bf16 along K), 8-row groups 1024 B apart (SBO); LBO is fixed to 1 for swizzled K-major tiles.
-//   MN-major : rows of 128 B hold 64 consecutive M/N elements of ONE k index; 8 consecutive k rows form a 1024 B group (SBO);
-//              the next 64 M/N elements live `lboBytes` further (LBO). This is the natural layout of a V tile [pos][headDim].
-__device__ __forceinline__ uint64_t apDescK(uint32_t addr) {
-    return (uint64_t)((addr >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ uint64_t apDescMN(uint32_t addr, uint32_t lboBytes) {
-    return (uint64_t)((addr >> 4) & 0x3fffu) | ((uint64_t)((lboBytes >> 4) & 0x3fffu) << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+__device__ __forceinline__ uint32_t apPack(float lo, float hi) {
+    __nv_bfloat162 b = __floats2bfloat162_rn(lo, hi);
+    return *reinterpret_cast<uint32_t *>(&b);
 }
 
 struct AttnPrefillKArgs {
@@ -101,14 +67,10 @@ __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __gri
     uint8_t *Qs = smem;                                  // [NA][128 rows][128 B]
     uint8_t *Ks = Qs + kTileBytes;                       // [2][NA][128][128 B]
     uint8_t *Vs = Ks + 2 * kTileBytes;                   // [2][NA][128][128 B]
-    uint8_t *Ps = Vs + 2 * kTileBytes;                   // [2 atoms][128 rows][128 B]: P tile 128 x 128 bf16
-    uint64_t *bars = reinterpret_cast<uint64_t *>(Ps + 2 * kApAtomBytes);
-    uint64_t *qReady = bars, *kFull = bars + 1, *kEmpty = bars + 3, *vFull = bars + 5, *vEmpty = bars + 7, *sFull = bars + 9,
-             *sEmpty = bars + 11, *pFull = bars + 13, *pEmpty = bars + 14, *oFull = bars + 15;
-    uint32_t *tmemBasePtr = reinterpret_cast<uint32_t *>(bars + 16);
+    uint64_t *bars = reinterpret_cast<uint64_t *>(Vs + 2 * kTileBytes);
+    uint64_t *kFull = bars, *kEmpty = bars + 2, *vFull = bars + 4, *vEmpty = bars + 6;
 
-    // warp index via shuffle = warp-uniform for the compiler: the role branches become uniform control flow and the tcgen05 / TMA
-    // operands stay in uniform registers (with tid >> 5 every UTCHMMA sat in an ELECT + R2UR.BROADCAST + BRA.U.ANY loop, ~100 clocks)
+    // warp index via shuffle = warp-uniform for the compiler: the role branches become uniform control flow
     const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
     const uint32_t item = blockIdx.x;
     const uint32_t kvh = item / a.nQTiles, qt = item - kvh * a.nQTiles;
@@ -120,25 +82,14 @@ __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __gri
 
     pdlLaunchDependents();
     if (tid == 0) {
-        apBarInit(qReady, 4);
         for (int i = 0; i < 2; i++) {
-            apBarInit(&kFull[i], 1); apBarInit(&kEmpty[i], 1);
-            apBarInit(&vFull[i], 1); apBarInit(&vEmpty[i], 1);
-            apBarInit(&sFull[i], 1); apBarInit(&sEmpty[i], 4);
+            apBarInit(&kFull[i], 1); apBarInit(&kEmpty[i], kApConsumerWarps);
+            apBarInit(&vFull[i], 1); apBarInit(&vEmpty[i], kApConsumerWarps);
         }
-        apBarInit(pFull, 4); apBarInit(pEmpty, 1); apBarInit(oFull, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(apAddr(tmemBasePtr)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    apFenceBefore();
     __syncthreads();
-    apFenceAfter();
     pdlWait();   // q rows and the new K/V rows come from the rope kernel before this one
-    const uint32_t tmemBase = __shfl_sync(0xffffffffu, *tmemBasePtr, 0);
-    const uint32_t tmemO = tmemBase + 256;             // S0: cols [0,128), S1: [128,256), O: [256, 256 + HD)
 
     if (warp == 0) {
         // ================================ TMA producer ================================
@@ -159,63 +110,15 @@ __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __gri
                 }
             }
         }
-    } else if (warp == 1) {
-        // ================================ MMA issuer ================================
-        // instruction descriptors: D = f32, A = B = bf16, M = 128; S: N = 128, both operands K-major; PV: N = HD, B (= V) MN-major
-        const uint32_t idescS = (1u << 4) | (1u << 7) | (1u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-        const uint32_t idescPV = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 16) | (((uint32_t)HD >> 3) << 17) | ((128u >> 4) << 24);
-        apBarWait(qReady, 0);
-        apFenceAfter();
-        uint32_t itK = 0, itS = 0;
-        auto issueS = [&]() {
-            const uint32_t st = itK & 1, ph = (itK >> 1) & 1, sb = itS & 1, sph = (itS >> 1) & 1;
-            apBarWait(&kFull[st], ph);
-            apBarWait(&sEmpty[sb], sph ^ 1);
-            apFenceAfter();
-            if (apElectOne()) {
-#pragma unroll
-                for (uint32_t c = 0; c < NA; c++) {
-                    const uint64_t dq = apDescK(apAddr(Qs + c * kApAtomBytes));
-                    const uint64_t dk = apDescK(apAddr(Ks + st * kTileBytes + c * kApAtomBytes));
-#pragma unroll
-                    for (uint32_t k = 0; k < 4; k++) apUmma(tmemBase + sb * 128, dq + 2 * k, dk + 2 * k, idescS, (c | k) != 0 ? 1u : 0u);
-                }
-                apCommit(&kEmpty[st]);
-                apCommit(&sFull[sb]);
-            }
-            __syncwarp();
-            itK++; itS++;
-        };
-        for (uint32_t j = 0; j < nKv; j++) issueS();           // pass 1: statistics only
-        issueS();                                              // pass 2: S(0)
-        for (uint32_t j = 0; j < nKv; j++) {
-            if (j + 1 < nKv) issueS();                         // S(j+1) overlaps the softmax of tile j
-            const uint32_t vs = j & 1;
-            apBarWait(pFull, j & 1);
-            apBarWait(&vFull[vs], (j >> 1) & 1);
-            apFenceAfter();
-            if (apElectOne()) {
-#pragma unroll
-                for (uint32_t kk = 0; kk < 8; kk++) {              // 8 slices of 16 KV positions
-                    const uint64_t dp = apDescK(apAddr(Ps + (kk >> 2) * kApAtomBytes)) + 2 * (kk & 3);
-                    const uint64_t dv = apDescMN(apAddr(Vs + vs * kTileBytes + kk * 2048), kApAtomBytes);
-                    apUmma(tmemO, dp, dv, idescPV, (j | kk) != 0 ? 1u : 0u);
-                }
-                apCommit(&vEmpty[vs]);
-                apCommit(pEmpty);
-                if (j == nKv - 1) apCommit(oFull);
-            }
-            __syncwarp();
-        }
     } else if (warp >= 4) {
-        // ================================ softmax / epilogue (thread = query row) ================================
-        const uint32_t q = (uint32_t)warp - 4, row = q * 32 + lane;
-        // ---- Q tile: f32 -> scaled bf16, canonical K-major SWIZZLE_128B layout ----
+        // ============================ consumer warpgroup g: query rows [64g, 64g + 64) ============================
+        const uint32_t g = (uint32_t)(warp - 4) >> 2, qw = (uint32_t)(warp - 4) & 3;
+        // ---- Q rows of this warpgroup: f32 -> scaled bf16, canonical K-major SWIZZLE_128B layout ----
         {
             constexpr uint32_t CPR = HD / 8;           // 16-byte chunks (8 elements) per row
             constexpr uint32_t RPI = 32 / CPR;         // rows per warp iteration
             const uint32_t cc = lane % CPR;
-            for (uint32_t r0 = q * 32; r0 < q * 32 + 32; r0 += RPI) {
+            for (uint32_t r0 = 64 * g + 16 * qw; r0 < 64 * g + 16 * qw + 16; r0 += RPI) {
                 const uint32_t r = r0 + lane / CPR;
                 uint4 packed = make_uint4(0u, 0u, 0u, 0u);
                 if (r < rowsValid) {
@@ -223,120 +126,136 @@ __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __gri
                     const float4 *src = reinterpret_cast<const float4 *>(a.qkv + (size_t)(t0 + ti) * a.qkvStride + (size_t)(kvh * a.kvMul + hi) * HD + cc * 8);
                     const float4 v0 = __ldg(src), v1 = __ldg(src + 1);
                     const float s = a.scaleLog2;
-                    __nv_bfloat162 b0 = __floats2bfloat162_rn(v0.x * s, v0.y * s), b1 = __floats2bfloat162_rn(v0.z * s, v0.w * s);
-                    __nv_bfloat162 b2 = __floats2bfloat162_rn(v1.x * s, v1.y * s), b3 = __floats2bfloat162_rn(v1.z * s, v1.w * s);
-                    packed = make_uint4(*reinterpret_cast<uint32_t *>(&b0), *reinterpret_cast<uint32_t *>(&b1), *reinterpret_cast<uint32_t *>(&b2),
-                                        *reinterpret_cast<uint32_t *>(&b3));
+                    packed = make_uint4(apPack(v0.x * s, v0.y * s), apPack(v0.z * s, v0.w * s), apPack(v1.x * s, v1.y * s), apPack(v1.z * s, v1.w * s));
                 }
                 *reinterpret_cast<uint4 *>(Qs + (cc >> 3) * kApAtomBytes + r * 128 + (((cc & 7) ^ (r & 7)) << 4)) = packed;
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) apBarArrive(qReady);
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
+            wgBarrier(1 + g);
         }
-        const bool rowOk = row < rowsValid;
-        const uint32_t ti = row / a.kvMul, hi = row - ti * a.kvMul;
-        const uint32_t rowPos = a.p0 + t0 + ti;          // last visible position of this row
-        const uint32_t laneAddr = (q * 32u) << 16;
-        float m = -INFINITY, l = 0.f;
-        uint32_t itS = 0;
+        // this thread's two accumulator rows (fragment rows lane / 4 and lane / 4 + 8 of the warp's 16)
+        bool rowOk[2];
+        uint32_t rowPos[2];   // last visible position of the row
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const uint32_t row = 64 * g + 16 * qw + (lane >> 2) + 8 * h;
+            rowOk[h] = row < rowsValid;
+            rowPos[h] = a.p0 + t0 + row / a.kvMul;
+        }
+        const uint32_t qAddr = apAddr(Qs) + g * 8192;          // rows 64g.. start 64 x 128 B into every atom
+        const uint32_t colBase = 2 * (lane & 3);
+        // S half-tile [64 rows x 64 positions] = Q . K^T, K rows [half * 64, half * 64 + 64) of the stage
+        auto computeS = [&](float (&s)[32], uint32_t kAddr) {
+            wgFence();
+#pragma unroll
+            for (uint32_t c = 0; c < NA; c++)
+#pragma unroll
+                for (uint32_t k = 0; k < 4; k++)
+                    wgmmaSS<0>(s, wgDesc(qAddr + c * kApAtomBytes) + 2 * k, wgDesc(kAddr + c * kApAtomBytes) + 2 * k, (c | k) != 0 ? 1u : 0u);
+            wgCommit();
+            wgWait<0>();
+            wgFenceAcc(s);
+        };
+        // causal mask in place (masked -> -inf); fragment element 4i + 2h + e = (row h, position pos0 + 8i + colBase + e)
+        auto maskS = [&](float (&s)[32], uint32_t pos0) {
+#pragma unroll
+            for (int i = 0; i < 8; i++)
+#pragma unroll
+                for (int h = 0; h < 2; h++)
+#pragma unroll
+                    for (int e = 0; e < 2; e++) {
+                        const bool vis = rowOk[h] && pos0 + 8 * i + colBase + e <= rowPos[h];
+                        if (!vis) s[4 * i + 2 * h + e] = -INFINITY;
+                    }
+        };
+        float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+        uint32_t itK = 0;
         // ---- pass 1: row maximum and normaliser ----
-        for (uint32_t j = 0; j < nKv; j++, itS++) {
-            const uint32_t sb = itS & 1, sph = (itS >> 1) & 1;
-            apBarWait(&sFull[sb], sph);
-            apFenceAfter();
+        for (uint32_t j = 0; j < nKv; j++, itK++) {
+            const uint32_t st = itK & 1, ph = (itK >> 1) & 1;
+            apBarWait(&kFull[st], ph);
 #pragma unroll 1
-            for (uint32_t c0 = 0; c0 < 128; c0 += 32) {
-                uint32_t r[32];
-                apTmemLoad32(tmemBase + laneAddr + sb * 128 + c0, r);
-                const uint32_t pos0 = j * 128 + c0;
-                float cm = -INFINITY;
+            for (uint32_t half = 0; half < 2; half++) {
+                float s[32];
+                computeS(s, apAddr(Ks + st * kTileBytes) + half * 8192);
+                maskS(s, j * 128 + half * 64);
 #pragma unroll
-                for (int i = 0; i < 32; i++) {
-                    const bool vis = rowOk && pos0 + i <= rowPos;
-                    const float s = vis ? __uint_as_float(r[i]) : -INFINITY;
-                    r[i] = __float_as_uint(s);
-                    cm = fmaxf(cm, s);
-                }
-                const float mNew = fmaxf(m, cm);
-                if (mNew > -INFINITY) {
+                for (int h = 0; h < 2; h++) {
+                    float cm = -INFINITY;
+#pragma unroll
+                    for (int i = 0; i < 8; i++) cm = fmaxf(cm, fmaxf(s[4 * i + 2 * h], s[4 * i + 2 * h + 1]));
+                    cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 1));
+                    cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, 2));   // the 4 lanes of a row
+                    const float mNew = fmaxf(m[h], cm);
                     float acc = 0.f;
+                    if (mNew > -INFINITY) {
 #pragma unroll
-                    for (int i = 0; i < 32; i++) acc += exp2f(__uint_as_float(r[i]) - mNew);
-                    l = l * exp2f(m - mNew) + acc;
-                    m = mNew;
+                        for (int i = 0; i < 8; i++) acc += exp2f(s[4 * i + 2 * h] - mNew) + exp2f(s[4 * i + 2 * h + 1] - mNew);
+                    }
+                    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+                    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+                    if (mNew > -INFINITY) {
+                        l[h] = l[h] * exp2f(m[h] - mNew) + acc;
+                        m[h] = mNew;
+                    }
                 }
             }
-            apFenceBefore();
             __syncwarp();
-            if (lane == 0) apBarArrive(&sEmpty[sb]);
+            if (lane == 0) apBarArrive(&kEmpty[st]);
         }
-        // ---- pass 2: P tiles ----
-        for (uint32_t j = 0; j < nKv; j++, itS++) {
-            const uint32_t sb = itS & 1, sph = (itS >> 1) & 1;
-            apBarWait(&sFull[sb], sph);
-            if (j > 0) apBarWait(pEmpty, (j - 1) & 1);     // P.V of the previous tile has consumed the P buffer
-            apFenceAfter();
+        // ---- pass 2: P = exp2(S - m) -> O += P.V ----
+        const float mP[2] = {m[0] > -INFINITY ? m[0] : 0.f, m[1] > -INFINITY ? m[1] : 0.f};   // rows without a visible position: P = 0
+        float o[NA][32];
+        for (uint32_t j = 0; j < nKv; j++, itK++) {
+            const uint32_t st = itK & 1, ph = (itK >> 1) & 1, vs = j & 1, vph = (j >> 1) & 1;
+            apBarWait(&kFull[st], ph);
+            apBarWait(&vFull[vs], vph);
 #pragma unroll 1
-            for (uint32_t c0 = 0; c0 < 128; c0 += 32) {
-                uint32_t r[32];
-                apTmemLoad32(tmemBase + laneAddr + sb * 128 + c0, r);
-                const uint32_t pos0 = j * 128 + c0;
-                uint32_t pk[16];
+            for (uint32_t half = 0; half < 2; half++) {
+                float s[32];
+                computeS(s, apAddr(Ks + st * kTileBytes) + half * 8192);
+                maskS(s, j * 128 + half * 64);
+                uint32_t pa[4][4];   // A fragments of 4 k-steps of 16 positions
 #pragma unroll
-                for (int i = 0; i < 16; i++) {
-                    const bool v0 = rowOk && pos0 + 2 * i <= rowPos, v1 = rowOk && pos0 + 2 * i + 1 <= rowPos;
-                    const float p0 = v0 ? exp2f(__uint_as_float(r[2 * i]) - m) : 0.f;
-                    const float p1 = v1 ? exp2f(__uint_as_float(r[2 * i + 1]) - m) : 0.f;
-                    __nv_bfloat162 b = __floats2bfloat162_rn(p0, p1);
-                    pk[i] = *reinterpret_cast<uint32_t *>(&b);
-                }
-                // 32 columns = 4 chunks of 8 columns; column chunk index inside the 64-wide atom: ((c0 % 64) / 8 + i)
-                uint8_t *prow = Ps + (c0 >> 6) * kApAtomBytes + row * 128;
+                for (int kk = 0; kk < 4; kk++)
 #pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    const uint32_t chunk = ((c0 & 63) >> 3) + i;
-                    *reinterpret_cast<uint4 *>(prow + ((chunk ^ (row & 7)) << 4)) = make_uint4(pk[4 * i], pk[4 * i + 1], pk[4 * i + 2], pk[4 * i + 3]);
-                }
+                    for (int x = 0; x < 4; x++) {
+                        const int i = 2 * kk + (x >> 1), h = x & 1;   // a0: (i = 2kk, row), a1: (2kk, row + 8), a2: (2kk + 1, row), a3: (2kk + 1, row + 8)
+                        pa[kk][x] = apPack(exp2f(s[4 * i + 2 * h] - mP[h]), exp2f(s[4 * i + 2 * h + 1] - mP[h]));
+                    }
+                wgFence();
+#pragma unroll
+                for (int kk = 0; kk < 4; kk++)
+#pragma unroll
+                    for (uint32_t n = 0; n < NA; n++) {
+                        const uint32_t vAddr = apAddr(Vs + vs * kTileBytes + n * kApAtomBytes) + (half * 64 + kk * 16) * 128;
+                        wgmmaRS(o[n], pa[kk], wgDesc(vAddr, kApAtomBytes), (j | half | kk) != 0 ? 1u : 0u);
+                    }
+                wgCommit();
+                wgWait<0>();
+#pragma unroll
+                for (uint32_t n = 0; n < NA; n++) wgFenceAcc(o[n]);
             }
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            apFenceBefore();
             __syncwarp();
             if (lane == 0) {
-                apBarArrive(&sEmpty[sb]);
-                apBarArrive(pFull);
+                apBarArrive(&kEmpty[st]);
+                apBarArrive(&vEmpty[vs]);
             }
         }
         // ---- epilogue: O / l -> bf16 ----
-        apBarWait(oFull, 0);
-        apFenceAfter();
-        const float invL = l > 0.f ? 1.f / l : 0.f;
-        __nv_bfloat16 *orow = a.out + (size_t)(t0 + ti) * a.outStride + (size_t)(kvh * a.kvMul + hi) * HD;
-#pragma unroll 1
-        for (uint32_t c0 = 0; c0 < (uint32_t)HD; c0 += 32) {
-            uint32_t r[32];
-            apTmemLoad32(tmemO + laneAddr + c0, r);
-            if (rowOk) {
 #pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    uint32_t w[4];
+        for (int h = 0; h < 2; h++) {
+            if (!rowOk[h]) continue;
+            const uint32_t row = 64 * g + 16 * qw + (lane >> 2) + 8 * h;
+            const uint32_t ti = row / a.kvMul, hi = row - ti * a.kvMul;
+            const float invL = l[h] > 0.f ? 1.f / l[h] : 0.f;
+            __nv_bfloat16 *orow = a.out + (size_t)(t0 + ti) * a.outStride + (size_t)(kvh * a.kvMul + hi) * HD;
 #pragma unroll
-                    for (int k = 0; k < 4; k++) {
-                        __nv_bfloat162 b = __floats2bfloat162_rn(__uint_as_float(r[8 * i + 2 * k]) * invL, __uint_as_float(r[8 * i + 2 * k + 1]) * invL);
-                        w[k] = *reinterpret_cast<uint32_t *>(&b);
-                    }
-                    *reinterpret_cast<uint4 *>(orow + c0 + 8 * i) = make_uint4(w[0], w[1], w[2], w[3]);
-                }
-            }
+            for (uint32_t n = 0; n < NA; n++)
+#pragma unroll
+                for (int i = 0; i < 8; i++)
+                    *reinterpret_cast<uint32_t *>(orow + n * 64 + 8 * i + colBase) = apPack(o[n][4 * i + 2 * h] * invL, o[n][4 * i + 2 * h + 1] * invL);
         }
-        apFenceBefore();
-    }
-
-    apFenceBefore();
-    __syncthreads();
-    if (warp == 2) {
-        apFenceAfter();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemBase), "r"(512u) : "memory");
     }
 }
 
@@ -367,7 +286,7 @@ bool apCacheMap(CUtensorMap *map, const void *cache, uint32_t hd, uint64_t rows)
 
 template <int HD>
 int apLaunch(const CUtensorMap &mk, const CUtensorMap &mv, const AttnPrefillKArgs &k, uint32_t grid, cudaStream_t stream, bool pdl) {
-    constexpr size_t smemBytes = (size_t)(HD / 64) * kApAtomBytes * 5 + 2 * kApAtomBytes + 256 + 1024;
+    constexpr size_t smemBytes = (size_t)(HD / 64) * kApAtomBytes * 5 + 256 + 1024;
     static bool configured = false;
     if (!configured) {
         DL_CUDA_CHECK(cudaFuncSetAttribute(attnPrefillTcKernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));

@@ -1,4 +1,4 @@
-// Grid-barrier micro-benchmark (tools/microbench_barrier.py): the persistent decode kernel spends ~1-2 us per software grid
+// Grid-barrier micro-benchmark (tools/microbench_barrier.py): the persistent decode kernel spends microseconds per software grid
 // barrier, 5 barriers per layer. This kernel times candidate implementations under the same launch shape (one CTA per SM,
 // 16 consumer warps + 1 producer warp, optional concurrent bulk-copy weight stream) so the choice is made on measurements.
 #include "kernels.h"

@@ -1,5 +1,5 @@
-// Shared device helpers for the sm_100a kernels: PTX wrappers (PDL, cache-hinted loads, mbarrier, TMA,
-// tcgen05), warp reductions and the device weight layout description.
+// Shared device helpers for the sm_90a kernels: PTX wrappers (PDL, cache-hinted loads, mbarrier, TMA),
+// warp reductions and the device weight layout description.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -58,7 +58,7 @@ __device__ __forceinline__ void pdlLaunchDependents() { asm volatile("griddepcon
 __device__ __forceinline__ void pdlWait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // ---- cache-hinted global loads ----------------------------------------------------------------------
-// Weights are streamed exactly once per token: bypass L1 (sm_100a ptxas only accepts L2::evict_first on 256-bit loads).
+// Weights are streamed exactly once per token: bypass L1.
 __device__ __forceinline__ uint4 ldgStream16(const void *p) {
     uint4 r;
     asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"

@@ -49,7 +49,7 @@ struct Engine {
     unsigned int **flagUcDev = nullptr;
     uint32_t vocabLimit = 0;     // 0 = none; otherwise the greedy arg-max ignores vocabulary rows >= vocabLimit
     bool prefillFusedAr = false; // TP prefill: GEMM + all-reduce in one kernel (DL_PREFILL_FUSED_AR=1) instead of GEMM, then all-reduce kernel
-    bool tcAttn = true;          // prefill attention on tcgen05 (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
+    bool tcAttn = true;          // prefill attention on the tensor cores (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
     bool fusedAttn = true, fusedArgmax = true, useTma = true;   // debugging switches (DL_NO_FUSED_ATTN / DL_NO_FUSED_ARGMAX / DL_NO_TMA)
 };
 

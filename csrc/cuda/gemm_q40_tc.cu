@@ -1,36 +1,44 @@
-// Prefill GEMM on the 5th-generation tensor cores: out[T][d] = act_bf16[T][n] · dequant(W_q40[d][n])^T, T <= 256.
+// Prefill GEMM on the Hopper tensor cores: out[T][d] = act_bf16[T][n] · dequant(W_q40[d][n])^T, T <= 256.
 //
 // Reference path replaced: batched OP_MATMUL via llamafile tinyBLAS (Q40×Q80 on CPU vector units,
 // src/nn/nn-cpu-ops.cpp:1120-1136, src/nn/llamafile/sgemm.cpp:455-783) for the 32-token prefill chunks.
 //
-// sm_100a design (swap-AB: the 128 weight rows fill the UMMA M dimension, the tokens sit on N):
-//   warp 0      TMA producer   — activations tile [nTile tokens x 64 k] per stage via cp.async.bulk.tensor (SWIZZLE_128B)
-//   warp 1      MMA issuer     — one elected lane issues 4 x tcgen05.mma (M=128, N=nTile, K=16, bf16 -> f32 TMEM) per stage,
-//                                tcgen05.commit releases the stage / publishes the accumulator
-//   warp 2      TMEM allocator — 2 accumulator buffers (epilogue of tile i overlaps the MMAs of tile i+1)
-//   warps 4-7   epilogue       — tcgen05.ld (32 lanes x 16 columns), fused residual-add / SwiGLU / store
+// sm_90a design (swap-AB: the 128 weight rows of a tile are the wgmma M dimension, two m64 halves; the tokens sit on N):
+//   warp 0      TMA producer   — activations tile [64 tokens x 64 k] per stage via cp.async.bulk.tensor (SWIZZLE_128B)
+//   warps 4-7   MMA + epilogue — one warpgroup issues 2 x 4 wgmma.mma_async (m64n64k16, bf16 -> f32 registers) per stage,
+//                                releases the stage once the group before it has retired (wgmma.wait_group 1), and after the
+//                                last stage runs the fused residual-add / SwiGLU / store epilogue from its registers
 //   warps 8-15  dequant        — q40 nibbles + fp16 scale -> bf16, written straight into the canonical K-major
-//                                SWIZZLE_128B UMMA tile in shared memory (generic proxy), fence.proxy.async, mbarrier arrive.
+//                                SWIZZLE_128B wgmma tile in shared memory (generic proxy), fence.proxy.async, mbarrier arrive.
 //                                This is the "q40 dequant fused into the GEMM prologue": the weights are never materialised
 //                                in bf16 in global memory, HBM traffic stays at 4.5 bits/weight.
-// Persistent CTAs loop over 128-row tiles; all synchronisation is mbarrier based (no __syncthreads in the main loop).
+// A work item is one 128-row tile x one tile of up to 64 tokens (the f32 accumulator of 128 x 64 is 64 registers per consumer
+// thread); chunks of more than 64 tokens are several token tiles of the same row tile, handled by neighbouring CTAs so the
+// second read of the weights hits L2. Persistent CTAs loop over work items; all synchronisation is mbarrier based.
 #include <cuda.h>
 #include <cstdlib>
 
 #include "kernels.h"
+#include "wgmma.cuh"
 
 namespace dl {
 
 constexpr int kGmBlockM = 128;
 constexpr int kGmBlockK = 64;
+constexpr int kGmTokTile = 64;                 // tokens per work item = wgmma N
 constexpr int kGmThreads = 512;
 constexpr int kGmDeqWarps = 8;
 constexpr int kGmMaxStages = 8;
 constexpr int kGmMaxBStages = 12;
+constexpr int kGmConsumerWarps = 4;
+// accumulator staging for the epilogue: per consumer warp 32 rows x 16 tokens f32, row stride 17 (conflict-free row reads)
+constexpr int kGmStgStride = 17;
+constexpr int kGmStgBytes = kGmConsumerWarps * 32 * kGmStgStride * 4;
 // DL_GEMM_DEBUG bit 9 (512): CTA 0 records %clock64 stamps of its pipeline events (tools/trace_gemm.py)
 __device__ unsigned long long gGemmTrace[4096];
-__device__ __forceinline__ unsigned long long gmClock() { unsigned long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)); return t; }   // activation-tile ring of the TMA-staged variant
+__device__ __forceinline__ unsigned long long gmClock() { unsigned long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)); return t; }
 constexpr int kGmATileBytes = kGmBlockM * kGmBlockK * 2;   // 16 KB
+constexpr int kGmBTileBytes = kGmTokTile * kGmBlockK * 2;  // 8 KB
 
 enum { GEPI_STORE_F32 = 0, GEPI_RESIDUAL = 1, GEPI_SWIGLU_BF16 = 2, GEPI_STORE_BF16 = 3, GEPI_RESIDUAL_AR = 4 };
 
@@ -38,27 +46,25 @@ struct GemmArgs {
     const uint32_t *qs;
     const __half *scales;
     uint32_t d, n;        // weight rows / columns
-    uint32_t T, nTile;    // tokens, tokens rounded up to 16
+    uint32_t T;           // tokens (grouped mode: the most tokens one group can have)
     void *out;
     uint32_t outStride;   // elements between tokens
-    uint32_t stages, tmemCols;
+    uint32_t stages;
     uint32_t bStages;      // TMA-staged variant: depth of the activation-tile ring (decoupled from the A-tile ring), in MMA steps
-    uint32_t kPair;        // TMA-staged variant: 64-wide k-blocks per MMA step (1 or 2): one barrier round + one commit per step
     uint32_t splitK;       // TMA-staged variant: K is cut into splitK ranges handled by different CTAs (work item = tile x split)
     float *splitScratch;   // [splitK][T][d] f32 partial accumulators
     uint32_t clusterSplit;  // TMA-staged variant: the splitK CTAs of a row tile form a thread-block cluster and reduce over distributed shared memory
-    unsigned int *splitCounters;   // [nTilesM * 4][2], zero-initialised, self-resetting (arrived / done, per 32-row quarter of a tile)
+    unsigned int *splitCounters;   // [row tiles x token tiles x 4][2], zero-initialised, self-resetting (arrived / done, per consumer warp)
     ArArgs ar;             // GEPI_RESIDUAL_AR: tensor-parallel all-reduce fused into the epilogue (LL words over peer memory)
     uint32_t rawStages;    // TMA-staged variant: depth of the raw q40 ring (2 or 3)
     // DL_GEMM_DEBUG (timing experiments and the pipeline trace of the TMA-staged variant; never set in production):
-    //   1 skip the proxy fence · 2 skip the A-tile stores · 4 release raw stages late · 8 epilogue waits without back-off
-    //   16 one k-slice per MMA step (kPair = 1) · 32 issue no MMAs after the first · 64 no q40 -> bf16 conversion (32 | 64 = the
-    //   data-movement skeleton) · 256 contiguous raw loads (wrong results) · 512 CTA 0 records %clock64 stamps (tools/trace_gemm.py)
+    //   1 skip the proxy fence · 2 skip the A-tile stores · 4 release raw stages late
+    //   64 no q40 -> bf16 conversion · 256 contiguous raw loads (wrong results) · 512 CTA 0 records %clock64 stamps (tools/trace_gemm.py)
     uint32_t debugFlags;
     uint32_t act;          // gate activation of GEPI_SWIGLU_BF16 (gHiddenAct)
     // Grouped (mixture-of-experts) mode, TMA-staged variant only: the weight matrix is nGroups stacked [grpRows][n] matrices, the
     // activation / output rows are sorted by group; group g owns rows [grpOffset[g], grpOffset[g] + grpCount[g]) (device arrays
-    // written by moeSortKernel). Row tile t belongs to group t / grpTiles; groups without tokens are skipped by every warp role.
+    // written by moeSortKernel). Row tile t belongs to group t / grpTiles; token tiles without tokens are skipped by every warp role.
     const int *grpCount, *grpOffset;
     uint32_t grpTiles, grpRows, nGroups;
 };
@@ -75,16 +81,6 @@ __device__ __forceinline__ void gmBarWait(uint64_t *b, uint32_t parity) {
         "{\n.reg .pred p;\nGM_WAIT:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n@p bra GM_DONE;\nbra GM_WAIT;\nGM_DONE:\n}\n" ::"r"(sAddr(b)),
         "r"(parity)
         : "memory");
-}
-// Wait used by warps that idle for a whole tile (epilogue): back off between probes so the spinning warp does not take issue
-// slots from the dequantisation warps that share its scheduler.
-__device__ __forceinline__ void gmBarWaitIdle(uint64_t *b, uint32_t parity) {
-    uint32_t done = 0;
-    while (true) {
-        asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(done) : "r"(sAddr(b)), "r"(parity) : "memory");
-        if (done) break;
-        __nanosleep(256);
-    }
 }
 __device__ __forceinline__ void tmaLoad2d(void *dst, const CUtensorMap *map, uint32_t c0, uint32_t c1, uint64_t *bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(sAddr(dst)),
@@ -112,35 +108,49 @@ __device__ __forceinline__ void clusterSync() {
     asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// one lane of a converged warp (elect.sync): the predicate form keeps the enclosed tcgen05 operands uniform
-__device__ __forceinline__ bool electOne() {
-    uint32_t p;
-    asm volatile("{\n.reg .pred P;\nelect.sync _|P, 0xffffffff;\nselp.u32 %0, 1, 0, P;\n}\n" : "=r"(p));
-    return p != 0;
+// ---- accumulator of one consumer warpgroup: rows [0, 64) in acc0, [64, 128) in acc1, 64 tokens ----------------------------
+// The epilogue works row-wise: lane l of consumer warp q owns tile row gmRow(q, l) = 16q + (l & 15) + 64 (l >> 4), i.e. the 32 rows
+// whose accumulator fragments the warp holds. gmLoadAcc transposes 16 token columns of those rows through the warp's staging
+// buffer so every lane gets its row's 16 values.
+__device__ __forceinline__ uint32_t gmRow(uint32_t q, uint32_t lane) { return 16u * q + (lane & 15u) + 64u * (lane >> 4); }
+
+template <int CI>
+__device__ __forceinline__ void gmStageSlab(float *stgW, const float (&acc)[32], uint32_t lane) {
+    const uint32_t r = lane >> 2, c = 2u * (lane & 3u);
+#pragma unroll
+    for (int ii = 0; ii < 2; ii++) {
+        const int i = 2 * CI + ii;   // 8-token column group of the fragment
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            float *dst = stgW + (r + 8 * h) * kGmStgStride + ii * 8 + c;
+            dst[0] = acc[4 * i + 2 * h];
+            dst[1] = acc[4 * i + 2 * h + 1];
+        }
+    }
 }
-__device__ __forceinline__ void tcFenceAfter() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcFenceBefore() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma(uint32_t tmemD, uint64_t descA, uint64_t descB, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\ntcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n" ::"r"(tmemD), "l"(descA),
-        "l"(descB), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void ummaCommit(uint64_t *bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(sAddr(bar)) : "memory");
-}
-__device__ __forceinline__ void tmemLoad16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void gmLoadAcc(float *stgW, const float (&acc0)[32], const float (&acc1)[32], uint32_t lane, uint32_t c0,
+                                          uint32_t (&r)[16]) {
+    __syncwarp();
+    switch (c0 >> 4) {
+        case 0: gmStageSlab<0>(stgW, acc0, lane); gmStageSlab<0>(stgW + 16 * kGmStgStride, acc1, lane); break;
+        case 1: gmStageSlab<1>(stgW, acc0, lane); gmStageSlab<1>(stgW + 16 * kGmStgStride, acc1, lane); break;
+        case 2: gmStageSlab<2>(stgW, acc0, lane); gmStageSlab<2>(stgW + 16 * kGmStgStride, acc1, lane); break;
+        default: gmStageSlab<3>(stgW, acc0, lane); gmStageSlab<3>(stgW + 16 * kGmStgStride, acc1, lane); break;
+    }
+    __syncwarp();
+#pragma unroll
+    for (int j = 0; j < 16; j++) r[j] = __float_as_uint(stgW[lane * kGmStgStride + j]);
 }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (8-row groups 1024 B apart), sm_100 descriptor version 1.
-__device__ __forceinline__ uint64_t makeSmemDesc(uint32_t smemAddrBytes) {
-    return (uint64_t)((smemAddrBytes >> 4) & 0x3fffu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// One k-slice (64 wide) of the 128 x 64 tile: 4 x 2 wgmma (K = 16 each, +32 B per slice inside the swizzle atom; rows 64..127 of
+// the A tile start 8 KB in).
+__device__ __forceinline__ void gmMmaSlice(float (&acc0)[32], float (&acc1)[32], uint64_t descA, uint64_t descB, bool first) {
+#pragma unroll
+    for (uint32_t k = 0; k < kGmBlockK / 16; k++) {
+        const uint32_t accum = (first && k == 0) ? 0u : 1u;
+        wgmmaSS<0>(acc0, descA + 2 * k, descB + 2 * k, accum);
+        wgmmaSS<0>(acc1, descA + (8192 >> 4) + 2 * k, descB + 2 * k, accum);
+    }
 }
 
 template <int EPI>
@@ -148,129 +158,109 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcKernel(const __grid_co
     extern __shared__ __align__(1024) uint8_t smemRaw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smemRaw) + 1023) & ~(uintptr_t)1023);
     // warp index through a shuffle: tells the compiler it is warp-uniform, so the role branches below are uniform control flow and
-    // the tcgen05 / TMA operands (descriptors, barrier addresses) stay in uniform registers. With `tid >> 5` every UTCHMMA / UTCBAR
-    // was wrapped in an ELECT + 5x R2UR.BROADCAST + BRA.U.ANY loop: ~100 clocks per instruction on the single MMA-issuing thread,
-    // which paced the whole k-loop (tools/trace_gemm.py: 480-650 clocks to issue 4 MMAs + 2 commits).
+    // the wgmma / TMA operands (descriptors, barrier addresses) stay in uniform registers.
     const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-    const uint32_t nTile = a.nTile;
-    const uint32_t bTileBytes = nTile * 128;
-    const uint32_t stageBytes = kGmATileBytes + bTileBytes;
+    const uint32_t stageBytes = kGmATileBytes + kGmBTileBytes;
     uint64_t *fullBar = reinterpret_cast<uint64_t *>(smem + (size_t)a.stages * stageBytes);
     uint64_t *emptyBar = fullBar + kGmMaxStages;
-    uint64_t *tmemFull = emptyBar + kGmMaxStages;     // [2]
-    uint64_t *tmemEmpty = tmemFull + 2;               // [2]
-    uint32_t *tmemBasePtr = reinterpret_cast<uint32_t *>(tmemEmpty + 2);
+    float *stg = reinterpret_cast<float *>(reinterpret_cast<uint8_t *>(fullBar) + 512);
 
     const uint32_t nblk = a.n / 32;
     const uint32_t nkb = a.n / kGmBlockK;
     const uint32_t nTilesM = (a.d + kGmBlockM - 1) / kGmBlockM;
+    const uint32_t nTT = (a.T + kGmTokTile - 1) / kGmTokTile;
+    const uint32_t nItems = nTilesM * nTT;   // item = row tile x token tile
 
     pdlLaunchDependents();
     if (tid == 0) {
         for (uint32_t s = 0; s < a.stages; s++) {
             gmBarInit(&fullBar[s], 1 + kGmDeqWarps);
-            gmBarInit(&emptyBar[s], 1);
-        }
-        for (int i = 0; i < 2; i++) {
-            gmBarInit(&tmemFull[i], 1);
-            gmBarInit(&tmemEmpty[i], 4);
+            gmBarInit(&emptyBar[s], kGmConsumerWarps);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sAddr(tmemBasePtr)), "r"(a.tmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcFenceBefore();
     __syncthreads();
-    tcFenceAfter();
-    const uint32_t tmemBase = __shfl_sync(0xffffffffu, *tmemBasePtr, 0);   // warp-uniform for the compiler
     pdlWait();   // activations (and the residual stream) come from the predecessor kernel
 
     if (warp == 0) {
         // ===================== TMA producer: activation tiles =====================
         if (lane == 0) {
             uint32_t it = 0;
-            for (uint32_t tile = blockIdx.x; tile < nTilesM; tile += gridDim.x) {
+            for (uint32_t item = blockIdx.x; item < nItems; item += gridDim.x) {
+                const uint32_t tok0 = (item % nTT) * kGmTokTile;
                 for (uint32_t kb = 0; kb < nkb; kb++, it++) {
                     const uint32_t s = it % a.stages, ph = (it / a.stages) & 1;
                     gmBarWait(&emptyBar[s], ph ^ 1);
-                    gmBarExpectTx(&fullBar[s], bTileBytes);
-                    tmaLoad2d(smem + (size_t)s * stageBytes + kGmATileBytes, &tmapB, kb * kGmBlockK, 0, &fullBar[s]);
+                    gmBarExpectTx(&fullBar[s], kGmBTileBytes);
+                    tmaLoad2d(smem + (size_t)s * stageBytes + kGmATileBytes, &tmapB, kb * kGmBlockK, tok0, &fullBar[s]);
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((nTile >> 3) << 17) | ((uint32_t)(kGmBlockM >> 4) << 24);
-        uint32_t it = 0, tcount = 0;
-        for (uint32_t tile = blockIdx.x; tile < nTilesM; tile += gridDim.x, tcount++) {
-            const uint32_t acc = tcount & 1, accPh = (tcount >> 1) & 1;
-            gmBarWait(&tmemEmpty[acc], accPh ^ 1);
-            tcFenceAfter();
-            const uint32_t tmemD = tmemBase + acc * nTile;
-            for (uint32_t kb = 0; kb < nkb; kb++, it++) {
-                const uint32_t s = it % a.stages, ph = (it / a.stages) & 1;
-                gmBarWait(&fullBar[s], ph);
-                tcFenceAfter();
-                const uint32_t aAddr = sAddr(smem + (size_t)s * stageBytes);
-                const uint64_t descA = makeSmemDesc(aAddr);
-                const uint64_t descB = makeSmemDesc(aAddr + kGmATileBytes);
-                if (electOne()) {
-#pragma unroll
-                    for (uint32_t k = 0; k < kGmBlockK / 16; k++)
-                        umma(tmemD, descA + 2 * k, descB + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);   // +32 B per K=16 slice
-                    ummaCommit(&emptyBar[s]);
-                    if (kb == nkb - 1) ummaCommit(&tmemFull[acc]);
-                }
-                __syncwarp();
             }
         }
     } else if (warp >= 4 && warp < 8) {
-        // ===================== epilogue =====================
-        const uint32_t q = warp - 4;
-        uint32_t tcount = 0;
-        for (uint32_t tile = blockIdx.x; tile < nTilesM; tile += gridDim.x, tcount++) {
-            const uint32_t acc = tcount & 1, accPh = (tcount >> 1) & 1;
-            gmBarWait(&tmemFull[acc], accPh);
-            tcFenceAfter();
-            const uint32_t f = tile * kGmBlockM + q * 32 + lane;     // output feature owned by this thread (= TMEM lane)
+        // ===================== MMA + epilogue (one warpgroup) =====================
+        const uint32_t q = warp - 4, row = gmRow(q, lane);
+        float *stgW = stg + q * 32 * kGmStgStride;
+        float acc0[32], acc1[32];
+        uint32_t it = 0;
+        for (uint32_t item = blockIdx.x; item < nItems; item += gridDim.x) {
+            const uint32_t tile = item / nTT, tok0 = (item % nTT) * kGmTokTile;
+            const uint32_t Teff = min(a.T - tok0, (uint32_t)kGmTokTile);
+            uint32_t prev = 0;
+            for (uint32_t kb = 0; kb < nkb; kb++, it++) {
+                const uint32_t s = it % a.stages, ph = (it / a.stages) & 1;
+                gmBarWait(&fullBar[s], ph);
+                const uint32_t aAddr = sAddr(smem + (size_t)s * stageBytes);
+                wgFence();
+                gmMmaSlice(acc0, acc1, wgDesc(aAddr), wgDesc(aAddr + kGmATileBytes), kb == 0);
+                wgCommit();
+                wgWait<1>();   // the stage before this one has been read by the tensor cores
+                if (kb > 0) {
+                    __syncwarp();
+                    if (lane == 0) gmBarArrive(&emptyBar[prev]);
+                }
+                prev = s;
+            }
+            wgWait<0>();
+            wgFenceAcc(acc0);
+            wgFenceAcc(acc1);
+            __syncwarp();
+            if (lane == 0) gmBarArrive(&emptyBar[prev]);
+            const uint32_t f = tile * kGmBlockM + row;     // output feature owned by this thread
             const bool fOk = f < a.d;
-            for (uint32_t c0 = 0; c0 < nTile; c0 += 16) {
+            for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
                 uint32_t r[16];
                 float resid[16];
                 if (EPI == GEPI_RESIDUAL) {   // issue all residual loads of the 16-column group before any store (no serialised RMW chain)
 #pragma unroll
                     for (int j = 0; j < 16; j++)
-                        resid[j] = (c0 + j < a.T && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(c0 + j) * a.outStride + f) : 0.f;
+                        resid[j] = (c0 + j < Teff && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(tok0 + c0 + j) * a.outStride + f) : 0.f;
                 }
-                tmemLoad16(tmemBase + ((q * 32u) << 16) + acc * nTile + c0, r);
+                gmLoadAcc(stgW, acc0, acc1, lane, c0, r);
 #pragma unroll
                 for (int j = 0; j < 16; j++) {
                     const uint32_t tok = c0 + j;
+                    const size_t orow = (size_t)(tok0 + tok) * a.outStride;
                     const float v = __uint_as_float(r[j]);
                     if (EPI == GEPI_SWIGLU_BF16) {
                         const float other = __shfl_xor_sync(0xffffffffu, v, 1);   // rows (2i, 2i+1) = (gate_i, up_i)
-                        if (tok < a.T && fOk && !(lane & 1))
-                            reinterpret_cast<__nv_bfloat16 *>(a.out)[(size_t)tok * a.outStride + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
-                    } else if (tok < a.T && fOk) {
-                        if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[(size_t)tok * a.outStride + f] = v;
-                        if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[(size_t)tok * a.outStride + f] = v + resid[j];
-                        if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[(size_t)tok * a.outStride + f] = __float2bfloat16_rn(v);
+                        if (tok < Teff && fOk && !(lane & 1))
+                            reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
+                    } else if (tok < Teff && fOk) {
+                        if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[orow + f] = v;
+                        if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[orow + f] = v + resid[j];
+                        if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + f] = __float2bfloat16_rn(v);
                     }
                 }
             }
-            tcFenceBefore();
-            __syncwarp();
-            if (lane == 0) gmBarArrive(&tmemEmpty[acc]);
         }
     } else if (warp >= 8) {
-        // ===================== dequant: q40 -> bf16 UMMA tile =====================
+        // ===================== dequant: q40 -> bf16 wgmma tile =====================
         const uint32_t dt = tid - 256;
         const uint32_t row = dt & 127, b = dt >> 7;                 // 128 rows x 2 quant blocks per 64-wide k slice
         const uint32_t swz = row & 7;
         uint32_t it = 0;
-        for (uint32_t tile = blockIdx.x; tile < nTilesM; tile += gridDim.x) {
+        for (uint32_t item = blockIdx.x; item < nItems; item += gridDim.x) {
+            const uint32_t tile = item / nTT;
             const uint32_t rowG = tile * kGmBlockM + row;
             const bool ok = rowG < a.d;
             const uint4 *qrow = reinterpret_cast<const uint4 *>(a.qs) + (size_t)rowG * nblk + b;
@@ -330,13 +320,6 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcKernel(const __grid_co
             }
         }
     }
-
-    tcFenceBefore();
-    __syncthreads();
-    if (warp == 2) {
-        tcFenceAfter();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemBase), "r"(a.tmemCols) : "memory");
-    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -357,59 +340,49 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
     extern __shared__ __align__(1024) uint8_t smemRaw[];
     uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smemRaw) + 1023) & ~(uintptr_t)1023);
     const int tid = threadIdx.x, lane = tid & 31, warp = __shfl_sync(0xffffffffu, tid >> 5, 0);   // see gemmQ40TcKernel
-    const uint32_t nTile = a.nTile;
-    const uint32_t bTileBytes = nTile * 128;
-    // Two independent rings: A tiles (dequantised weights, written by the dequant warps) and B tiles (activations, TMA). Round 1
-    // kept them in one stage; with 64+ tokens only 4 such stages fit, i.e. ONE A tile per dequant group, so every group had to
-    // wait for the MMA of its previous tile before converting the next (ncu: dequant warps 50 % in long-scoreboard waits, tensor
-    // pipe 10 %). Now the A ring is 8 deep (2 per group) whatever the token count.
+    // Two independent rings: A tiles (dequantised weights, written by the dequant warps) and B tiles (activations, TMA). With one
+    // combined stage only one A tile per dequant group fits, so every group would wait for the MMA of its previous tile before
+    // converting the next; the A ring is 8 deep (2 per group) where shared memory allows.
     uint8_t *bBase = smem + (size_t)a.stages * kGmATileBytes;
-    uint8_t *rawBase = bBase + (size_t)a.bStages * a.kPair * bTileBytes;        // [rawStages][18 KB], 1024-aligned (all tiles are multiples of 1 KB)
+    uint8_t *rawBase = bBase + (size_t)a.bStages * kGmBTileBytes;        // [rawStages][18 KB], 1024-aligned (all tiles are multiples of 1 KB)
     uint64_t *fullBar = reinterpret_cast<uint64_t *>(rawBase + (size_t)a.rawStages * kGmRawStageBytes);   // A tile converted
     uint64_t *emptyBar = fullBar + kGmMaxStages;                                                            // A tile consumed
     uint64_t *bFull = emptyBar + kGmMaxStages;
-    uint64_t *bEmpty = bFull + kGmMaxBStages;
-    uint64_t *tmemFull = bEmpty + kGmMaxBStages;
-    uint64_t *tmemEmpty = tmemFull + 2;
-    uint64_t *rawFull = tmemEmpty + 2;
+    uint64_t *rawFull = bFull + kGmMaxBStages;
     uint64_t *rawEmpty = rawFull + kGmRawStagesMax;
-    uint32_t *tmemBasePtr = reinterpret_cast<uint32_t *>(rawEmpty + kGmRawStagesMax);
-    uint64_t *freeBar = rawEmpty + kGmRawStagesMax + 1;   // [4 source ranks][4 epilogue warps]: "the rings of rank r are free" (cluster split-K)
-    uint64_t *dataBar = freeBar + 16;                     // [4 epilogue warps]: every peer has delivered its partial sums for my tokens
+    uint64_t *freeBar = rawEmpty + kGmRawStagesMax;   // [4 source ranks][4 consumer warps]: "the rings of rank r are free" (cluster split-K)
+    uint64_t *dataBar = freeBar + 16;                 // [4 consumer warps]: every peer has delivered its partial sums for my tokens
+    float *stg = reinterpret_cast<float *>(reinterpret_cast<uint8_t *>(fullBar) + 1024);
 
     const uint32_t nkb = a.n / kGmBlockK;
     const uint32_t nkq = (a.n + kGmRawK - 1) / kGmRawK;
     const uint32_t nTilesM = a.grpCount ? a.nGroups * a.grpTiles : (a.d + kGmBlockM - 1) / kGmBlockM;
+    const uint32_t nTT = (a.T + kGmTokTile - 1) / kGmTokTile;
     const uint32_t splitK = a.splitK;
-    const uint32_t nItems = nTilesM * splitK;
-    // work item -> (row tile, K range in 256-wide raw chunks); consecutive items share a tile
+    const uint32_t nItems = nTilesM * nTT * splitK;
+    // work item -> (row tile, token tile, K range in 256-wide raw chunks); consecutive items share a row tile
     auto kqBegin = [&](uint32_t ks) { return (uint32_t)(((uint64_t)ks * nkq) / splitK); };
-    // grouped mode: (tile) -> weight row of the tile's first row, first activation/output row, number of valid tokens
+    auto itemTile = [&](uint32_t item) { return item / (splitK * nTT); };
+    auto itemTT = [&](uint32_t item) { return (item / splitK) % nTT; };
     // a.stages is 4 or 8 (tmaGeometry): stage / phase of the A ring by shift and mask; the raw and B rings (arbitrary depth) keep
     // incremental (stage, parity) counters — a runtime `%` or `/` is a ~25-instruction I2F/MUFU.RCP sequence per use
     const uint32_t aMask = a.stages - 1, aShift = a.stages == 8 ? 3u : 2u;
-    // MMA step = kPair adjacent k-slices (A-ring slots 2p, 2p+1 are adjacent in shared memory) sharing one full / empty barrier
-    // pair, indexed by slot >> pShift; the phase of a slot and of its step are the same bit of the slice counter.
-    const uint32_t pShift = a.kPair == 2 ? 1u : 0u;
     const bool grouped = a.grpCount != nullptr;
+    // grouped mode: (tile) -> weight row of the tile's first row; (tile, token tile) -> first activation/output row, valid tokens
     auto tileRow0 = [&](uint32_t tile) { return grouped ? (tile / a.grpTiles) * a.grpRows + (tile % a.grpTiles) * kGmBlockM : tile * kGmBlockM; };
-    auto tileTokens = [&](uint32_t tile) { return grouped ? (uint32_t)__ldg(a.grpCount + tile / a.grpTiles) : a.T; };
-    auto tileTok0 = [&](uint32_t tile) { return grouped ? (uint32_t)__ldg(a.grpOffset + tile / a.grpTiles) : 0u; };
+    auto tileTokens = [&](uint32_t tile, uint32_t tt) -> uint32_t {
+        const uint32_t total = grouped ? (uint32_t)__ldg(a.grpCount + tile / a.grpTiles) : a.T, t0 = tt * kGmTokTile;
+        return total > t0 ? min(total - t0, (uint32_t)kGmTokTile) : 0u;
+    };
+    auto tileTok0 = [&](uint32_t tile, uint32_t tt) { return (grouped ? (uint32_t)__ldg(a.grpOffset + tile / a.grpTiles) : 0u) + tt * kGmTokTile; };
 
     pdlLaunchDependents();
     if (tid == 0) {
         for (uint32_t s = 0; s < a.stages; s++) {
-            gmBarInit(&fullBar[s], 2 * a.kPair);   // the dequant warps that fill the step's k-slices (indexed by step slot: s < stages / kPair used)
-            gmBarInit(&emptyBar[s], 1);
+            gmBarInit(&fullBar[s], 2);   // the two dequant warps of the group that fills the slice
+            gmBarInit(&emptyBar[s], kGmConsumerWarps);
         }
-        for (uint32_t s = 0; s < a.bStages; s++) {
-            gmBarInit(&bFull[s], 1);
-            gmBarInit(&bEmpty[s], 1);
-        }
-        for (int i = 0; i < 2; i++) {
-            gmBarInit(&tmemFull[i], 1);
-            gmBarInit(&tmemEmpty[i], 4);
-        }
+        for (uint32_t s = 0; s < a.bStages; s++) gmBarInit(&bFull[s], 1);
         for (uint32_t i = 0; i < a.rawStages; i++) {
             gmBarInit(&rawFull[i], 1);
             gmBarInit(&rawEmpty[i], kGmDeqWarps);
@@ -420,23 +393,16 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sAddr(tmemBasePtr)), "r"(a.tmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tcFenceBefore();
     __syncthreads();
     if (a.clusterSplit) clusterSync();   // no peer may arrive on (or write into) this CTA before its barriers exist
-    tcFenceAfter();
-    const uint32_t tmemBase = __shfl_sync(0xffffffffu, *tmemBasePtr, 0);   // warp-uniform for the compiler
 
     if (warp == 3) {
         // ===================== raw weight producer (weights are constants: no dependency wait) =====================
         if (lane == 0) {
             uint32_t rs = 0, ph = 0;
             for (uint32_t item = blockIdx.x; item < nItems; item += gridDim.x) {
-                const uint32_t tile = item / splitK, ks = item - tile * splitK;
-                if (grouped && tileTokens(tile) == 0) continue;
+                const uint32_t tile = itemTile(item), ks = item % splitK;
+                if (tileTokens(tile, itemTT(item)) == 0) continue;
                 const uint32_t wRow = tileRow0(tile);
                 for (uint32_t kq = kqBegin(ks); kq < kqBegin(ks + 1); kq++) {
                     gmBarWait(&rawEmpty[rs], ph ^ 1);
@@ -446,8 +412,8 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                         tmaLoad2d(dst, &tmapQ, 0, (tile * nkq + kq) * kGmBlockM, &rawFull[rs]);
                         tmaLoad2d(dst + kGmRawQsBytes, &tmapS, 0, (tile * nkq + kq) * kGmBlockM, &rawFull[rs]);
                     } else {
-                    tmaLoad2d(dst, &tmapQ, kq * 128, wRow, &rawFull[rs]);                 // nibbles: 128 B per row
-                    tmaLoad2d(dst + kGmRawQsBytes, &tmapS, kq * 16, wRow, &rawFull[rs]);   // scales: 16 B per row
+                        tmaLoad2d(dst, &tmapQ, kq * 128, wRow, &rawFull[rs]);                 // nibbles: 128 B per row
+                        tmaLoad2d(dst + kGmRawQsBytes, &tmapS, kq * 16, wRow, &rawFull[rs]);   // scales: 16 B per row
                     }
                     if (++rs == a.rawStages) { rs = 0; ph ^= 1u; }
                 }
@@ -459,133 +425,111 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
         if (lane == 0) {
             uint32_t it = 0, sbP = 0;
             for (uint32_t item = blockIdx.x; item < nItems; item += gridDim.x) {
-                const uint32_t ks = item % splitK;
-                if (grouped && tileTokens(item / splitK) == 0) continue;
-                const uint32_t tok0 = tileTok0(item / splitK);
-                for (uint32_t kb = kqBegin(ks) * 4; kb < min(kqBegin(ks + 1) * 4, nkb); kb += a.kPair, it++) {
-                    // `it` counts MMA steps. B stage s was last read by the MMAs of step it - bStages; their completion is already
-                    // signalled on the A ring's emptyBar (one tcgen05.commit per step: the issuing warp paces the k-loop, every
-                    // instruction it does not execute counts). bStages <= stages / kPair, so that phase cannot have been overtaken.
+                const uint32_t ks = item % splitK, tile = itemTile(item), tt = itemTT(item);
+                if (tileTokens(tile, tt) == 0) continue;
+                const uint32_t tok0 = tileTok0(tile, tt);
+                for (uint32_t kb = kqBegin(ks) * 4; kb < min(kqBegin(ks + 1) * 4, nkb); kb++, it++) {
+                    // `it` counts k-slices. B stage s was last read by the MMAs of slice it - bStages; their completion is already
+                    // signalled on the A ring's emptyBar. bStages <= stages, so that phase cannot have been overtaken.
                     const uint32_t s = sbP;
                     if (it >= a.bStages) {
-                        const uint32_t j = (it - a.bStages) << pShift;      // first k-slice of that step
-                        gmBarWait(&emptyBar[(j & aMask) >> pShift], (j >> aShift) & 1);
+                        const uint32_t j = it - a.bStages;
+                        gmBarWait(&emptyBar[j & aMask], (j >> aShift) & 1);
                     }
-                    gmBarExpectTx(&bFull[s], bTileBytes * a.kPair);
-                    for (uint32_t h = 0; h < a.kPair; h++)
-                        tmaLoad2d(bBase + ((size_t)s * a.kPair + h) * bTileBytes, &tmapB, (kb + h) * kGmBlockK, tok0, &bFull[s]);
+                    gmBarExpectTx(&bFull[s], kGmBTileBytes);
+                    tmaLoad2d(bBase + (size_t)s * kGmBTileBytes, &tmapB, kb * kGmBlockK, tok0, &bFull[s]);
                     if (++sbP == a.bStages) sbP = 0;
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // One k-block costs this warp ~650 clocks (two barrier probes of ~75 clocks, four UTCHMMA, two UTCBAR, ~100 instructions of
-        // descriptor / phase arithmetic) against 4 x 32 clocks of tensor-core work at N = 64: the k-loop is paced by this warp, not
-        // by the dequant groups or the rings (tools/trace_gemm.py). A second issuing warp (alternate k-blocks, own accumulator)
-        // hung the kernel on the first tile, see experiments/README.md.
-        const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((nTile >> 3) << 17) | ((uint32_t)(kGmBlockM >> 4) << 24);
-        uint32_t itBase = 0, tcount = 0, sbM = 0, phbM = 0;
+    } else if (warp >= 4 && warp < 8) {
+        // ===================== MMA + epilogue (one warpgroup) =====================
+        pdlWait();   // the residual stream is read-modify-written
+        const uint32_t q = warp - 4, row = gmRow(q, lane);
+        float *stgW = stg + q * 32 * kGmStgStride;
+        float acc0[32], acc1[32];
+        auto loadAcc = [&](uint32_t c0, uint32_t (&r)[16]) { gmLoadAcc(stgW, acc0, acc1, lane, c0, r); };
+        uint32_t itBase = 0, sbM = 0, phbM = 0;
         for (uint32_t item = blockIdx.x; item < nItems; item += gridDim.x) {
-            const uint32_t ks = item % splitK;
-            if (grouped && tileTokens(item / splitK) == 0) continue;
-            const uint32_t tc = tcount++;
+            const uint32_t ks = item % splitK, tile = itemTile(item), tt = itemTT(item);
+            const uint32_t Teff = tileTokens(tile, tt);
+            if (Teff == 0) continue;
             const uint32_t kb0 = kqBegin(ks) * 4, kb1 = min(kqBegin(ks + 1) * 4, nkb);
-            const uint32_t acc = tc & 1, accPh = (tc >> 1) & 1;
-            gmBarWait(&tmemEmpty[acc], accPh ^ 1);
-            tcFenceAfter();
-            const uint32_t tmemD = tmemBase + acc * nTile;
-            for (uint32_t kb = kb0; kb < kb1; kb += a.kPair) {
+            uint32_t prevSlot = 0;
+            for (uint32_t kb = kb0; kb < kb1; kb++) {
                 const uint32_t it = itBase + (kb - kb0);                 // k-slice counter of the step's first slice
                 const uint32_t s = it & aMask, ph = (it >> aShift) & 1;
                 const uint32_t sb = sbM, phb = phbM;
                 if (++sbM == a.bStages) { sbM = 0; phbM ^= 1u; }
-                const bool trc = (a.debugFlags & 512u) && blockIdx.x == 0 && lane == 0 && it < 256;
+                const bool trc = (a.debugFlags & 512u) && blockIdx.x == 0 && q == 0 && lane == 0 && it < 256;
                 if (trc) gGemmTrace[it * 4 + 0] = gmClock();
                 gmBarWait(&bFull[sb], phb);
                 if (trc) gGemmTrace[it * 4 + 1] = gmClock();
-                gmBarWait(&fullBar[s >> pShift], ph);
+                gmBarWait(&fullBar[s], ph);
                 if (trc) gGemmTrace[it * 4 + 2] = gmClock();
-                tcFenceAfter();
-                const uint64_t descA = makeSmemDesc(sAddr(smem + (size_t)s * kGmATileBytes));
-                const uint64_t descB = makeSmemDesc(sAddr(bBase + (size_t)sb * a.kPair * bTileBytes));
-                if (electOne()) {
-#pragma unroll
-                    for (uint32_t k = 0; k < kGmBlockK / 16; k++)
-                        if (!(a.debugFlags & 32u) || (kb == kb0 && k == 0)) umma(tmemD, descA + 2 * k, descB + 2 * k, idesc, (kb != kb0 || k != 0) ? 1u : 0u);
-                    if (a.kPair == 2) {
-                        // second k-slice of the step: next A slot (+16 KB) and the second half of the B stage (descriptor address units: 16 B)
-                        const uint64_t descA2 = descA + (kGmATileBytes >> 4), descB2 = descB + (bTileBytes >> 4);
-#pragma unroll
-                        for (uint32_t k = 0; k < kGmBlockK / 16; k++) umma(tmemD, descA2 + 2 * k, descB2 + 2 * k, idesc, 1u);
-                    }
-                    ummaCommit(&emptyBar[s >> pShift]);
-                    if (kb + a.kPair >= kb1) ummaCommit(&tmemFull[acc]);
+                const uint64_t descA = wgDesc(sAddr(smem + (size_t)s * kGmATileBytes));
+                const uint64_t descB = wgDesc(sAddr(bBase + (size_t)sb * kGmBTileBytes));
+                wgFence();
+                gmMmaSlice(acc0, acc1, descA, descB, kb == kb0);
+                wgCommit();
+                wgWait<1>();   // the previous slice's tiles have been read by the tensor cores: release them
+                if (kb != kb0) {
+                    __syncwarp();
+                    if (lane == 0) gmBarArrive(&emptyBar[prevSlot]);
                 }
+                prevSlot = s;
                 if (trc) gGemmTrace[it * 4 + 3] = gmClock();
-                __syncwarp();
             }
+            wgWait<0>();
+            wgFenceAcc(acc0);
+            wgFenceAcc(acc1);
+            __syncwarp();
+            if (lane == 0) gmBarArrive(&emptyBar[prevSlot]);
             itBase += kb1 - kb0;
-        }
-    } else if (warp >= 4 && warp < 8) {
-        // ===================== epilogue =====================
-        pdlWait();   // the residual stream is read-modify-written
-        const uint32_t q = warp - 4;
-        // accumulator columns [c0, c0 + 16) of this warp's 32 rows
-        auto loadAcc = [&](uint32_t acc, uint32_t c0, uint32_t (&r)[16]) { tmemLoad16(tmemBase + ((q * 32u) << 16) + acc * nTile + c0, r); };
-        uint32_t tcount = 0;
-        for (uint32_t item = blockIdx.x; item < nItems; item += gridDim.x) {
-            const uint32_t tile = item / splitK, ks = item - tile * splitK;
-            const uint32_t Teff = tileTokens(tile);
-            if (grouped && Teff == 0) continue;
-            const uint32_t tc = tcount++;
-            const uint32_t acc = tc & 1, accPh = (tc >> 1) & 1;
-            if (a.debugFlags & 8u) gmBarWait(&tmemFull[acc], accPh); else gmBarWaitIdle(&tmemFull[acc], accPh);
-            tcFenceAfter();
             // grouped mode: f is the feature index inside the group's matrix, output rows start at the group's first sorted row
-            const uint32_t f = (grouped ? (tile % a.grpTiles) * kGmBlockM : tile * kGmBlockM) + q * 32 + lane;
+            const uint32_t f = (grouped ? (tile % a.grpTiles) * kGmBlockM : tile * kGmBlockM) + row;
             const bool fOk = f < (grouped ? a.grpRows : a.d);
-            const uint32_t rowOff = tileTok0(tile);
+            const uint32_t rowOff = tileTok0(tile, tt);
             if (splitK > 1 && a.clusterSplit) {
-                // ---- split-K inside a thread-block cluster: the splitK CTAs of this row tile are the ranks of one cluster (rank = ks).
+                // ---- split-K inside a thread-block cluster: the splitK CTAs of this work item are the ranks of one cluster (rank = ks).
                 // Rank r reduces the tokens [r * per, (r + 1) * per): every other rank stores its partial sums for those tokens
                 // straight into r's shared memory (st.shared::cluster into the A ring, which is idle once r's accumulator is
                 // complete) and arrives on r's mbarrier; r adds them in rank order (deterministic) to its own accumulator columns and
                 // runs the epilogue. No global scratch, no MEMBAR.GPU, no atomics: two DSMEM hops instead of three L2 round trips.
-                const uint32_t per = ((a.T + splitK - 1) / splitK + 15u) & ~15u;      // 16-token granularity = one tcgen05.ld
-                const uint32_t row = q * 32 + lane;
+                const uint32_t per = ((Teff + splitK - 1) / splitK + 15u) & ~15u;     // 16-token granularity = one gmLoadAcc
                 const uint32_t recvLocal = sAddr(smem);                                // float recv[splitK - 1][per][128] in the A ring
                 if (lane == 0)
                     for (uint32_t p = 0; p < splitK; p++)
                         if (p != ks) arriveRemote(mapaShared(sAddr(&freeBar[ks * 4 + q]), p));   // my MMAs are done: my rings may be overwritten
                 for (uint32_t dp = 1; dp < splitK; dp++) {
                     const uint32_t p = (ks + dp) % splitK;                             // staggered order: not everybody hits rank 0 first
-                    const uint32_t pBeg = p * per, pEnd = min(a.T, pBeg + per);
+                    const uint32_t pBeg = p * per, pEnd = min(Teff, pBeg + per);
                     gmBarWaitCluster(&freeBar[p * 4 + q], 0);
                     const uint32_t slot = ks < p ? ks : ks - 1;                        // my place among p's splitK - 1 sources, in rank order
                     const uint32_t dstBase = mapaShared(recvLocal + (slot * per * kGmBlockM + row) * 4u, p);
                     for (uint32_t c0 = pBeg; c0 < pEnd; c0 += 16) {
                         uint32_t r[16];
-                        loadAcc(acc, c0, r);
+                        loadAcc(c0, r);
 #pragma unroll
                         for (int j = 0; j < 16; j++)
                             if (c0 + j < pEnd) stClusterF32(dstBase + (c0 + j - pBeg) * (kGmBlockM * 4u), __uint_as_float(r[j]));
                     }
                     arriveRemote(mapaShared(sAddr(&dataBar[q]), p));                   // every lane: its own stores are released
                 }
-                const uint32_t tBeg = ks * per, tEnd = min(a.T, tBeg + per);
+                const uint32_t tBeg = ks * per, tEnd = min(Teff, tBeg + per);
                 gmBarWaitCluster(&dataBar[q], 0);
                 const float *recv = reinterpret_cast<const float *>(smem);
                 for (uint32_t c0 = tBeg; c0 < tEnd; c0 += 16) {
                     uint32_t own[16];
-                    loadAcc(acc, c0, own);
+                    loadAcc(c0, own);
                     float resid[16];
 #pragma unroll
                     for (int j = 0; j < 16; j++)
-                        resid[j] = (EPI == GEPI_RESIDUAL && c0 + j < tEnd && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(c0 + j) * a.outStride + f) : 0.f;
+                        resid[j] = (EPI == GEPI_RESIDUAL && c0 + j < tEnd && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(rowOff + c0 + j) * a.outStride + f) : 0.f;
 #pragma unroll
                     for (int j = 0; j < 16; j++) {
                         const uint32_t tok = c0 + j;
+                        const size_t orow = (size_t)(rowOff + tok) * a.outStride;
                         float v = 0.f;
                         for (uint32_t r = 0; r < splitK; r++) {                        // rank order, own partial at position ks
                             if (r == ks) v += __uint_as_float(own[j]);
@@ -594,38 +538,32 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                         if (EPI == GEPI_SWIGLU_BF16) {
                             const float other = __shfl_xor_sync(0xffffffffu, v, 1);
                             if (fOk && tok < tEnd && !(lane & 1))
-                                reinterpret_cast<__nv_bfloat16 *>(a.out)[(size_t)tok * a.outStride + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
+                                reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
                         } else if (fOk && tok < tEnd) {
-                            if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[(size_t)tok * a.outStride + f] = v;
-                            if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[(size_t)tok * a.outStride + f] = resid[j] + v;
-                            if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[(size_t)tok * a.outStride + f] = __float2bfloat16_rn(v);
+                            if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[orow + f] = v;
+                            if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[orow + f] = resid[j] + v;
+                            if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + f] = __float2bfloat16_rn(v);
                         }
                     }
                 }
-                tcFenceBefore();
-                __syncwarp();
-                if (lane == 0) gmBarArrive(&tmemEmpty[acc]);
                 continue;
             }
             if (splitK > 1) {
-                // ---- split-K: park the partial accumulator; once all splits of this 32-row quarter have arrived, every split reduces
-                // its own share of the tokens (fixed summation order -> deterministic). All splits of a tile are co-resident (one item
-                // per CTA, nItems <= SMs), so the wait cannot deadlock; the reduce is latency-bound (a dependent L2 round trip per
-                // round of 8 tokens), which is why it is spread over the splits instead of left to the last arriver.
+                // ---- split-K: park the partial accumulator; once all splits of this warp's 32 rows have arrived, every split reduces
+                // its own share of the tokens (fixed summation order -> deterministic). All splits of a work item are co-resident
+                // (one item per CTA, nItems <= SMs), so the wait cannot deadlock; the reduce is latency-bound (a dependent L2 round
+                // trip per round of 8 tokens), which is why it is spread over the splits instead of left to the last arriver.
                 float *mineS = a.splitScratch + (size_t)ks * a.T * a.d;
-                for (uint32_t c0 = 0; c0 < nTile; c0 += 16) {
+                for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
                     uint32_t r[16];
-                    loadAcc(acc, c0, r);
+                    loadAcc(c0, r);
 #pragma unroll
                     for (int j = 0; j < 16; j++)
-                        if (c0 + j < a.T && fOk) mineS[(size_t)(c0 + j) * a.d + f] = __uint_as_float(r[j]);
+                        if (c0 + j < Teff && fOk) mineS[(size_t)(rowOff + c0 + j) * a.d + f] = __uint_as_float(r[j]);
                 }
-                tcFenceBefore();
-                __syncwarp();
-                if (lane == 0) gmBarArrive(&tmemEmpty[acc]);
                 __threadfence();
                 __syncwarp();
-                unsigned int *ctr = a.splitCounters + (size_t)(tile * 4 + q) * 2;   // [0]: splits arrived, [1]: splits done reducing
+                unsigned int *ctr = a.splitCounters + (size_t)((tile * nTT + tt) * 4 + q) * 2;   // [0]: splits arrived, [1]: splits done reducing
                 if (lane == 0) {
                     atomicAdd(ctr, 1u);
                     unsigned int seen = 0, spins = 0;
@@ -635,7 +573,7 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                     } while (seen < splitK && ++spins < (1u << 24));
                 }
                 __syncwarp();
-                const uint32_t per = (a.T + splitK - 1) / splitK, tBeg = ks * per, tEnd = min(a.T, tBeg + per);
+                const uint32_t per = (Teff + splitK - 1) / splitK, tBeg = ks * per, tEnd = min(Teff, tBeg + per);
                 for (uint32_t tok0 = tBeg; tok0 < tEnd; tok0 += 8) {
                     // 8 tokens x up to 4 splits (+ 8 residual values) are loaded before any arithmetic: ~40 loads in flight per thread
                     float part[8][4], res[8];
@@ -644,23 +582,24 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                         const bool ok = fOk && tok0 + j < tEnd;
 #pragma unroll
                         for (int k2 = 0; k2 < 4; k2++)
-                            part[j][k2] = (ok && (uint32_t)k2 < splitK) ? __ldcg(a.splitScratch + ((size_t)k2 * a.T + tok0 + j) * a.d + f) : 0.f;
-                        res[j] = (EPI == GEPI_RESIDUAL && ok) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(tok0 + j) * a.outStride + f) : 0.f;
+                            part[j][k2] = (ok && (uint32_t)k2 < splitK) ? __ldcg(a.splitScratch + ((size_t)k2 * a.T + rowOff + tok0 + j) * a.d + f) : 0.f;
+                        res[j] = (EPI == GEPI_RESIDUAL && ok) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(rowOff + tok0 + j) * a.outStride + f) : 0.f;
                     }
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
                         const uint32_t tok = tok0 + j;
+                        const size_t orow = (size_t)(rowOff + tok) * a.outStride;
                         float v = 0.f;
 #pragma unroll
                         for (int k2 = 0; k2 < 4; k2++) v += part[j][k2];          // fixed order -> deterministic
                         if (EPI == GEPI_SWIGLU_BF16) {
                             const float other = __shfl_xor_sync(0xffffffffu, v, 1);
                             if (fOk && tok < tEnd && !(lane & 1))
-                                reinterpret_cast<__nv_bfloat16 *>(a.out)[(size_t)tok * a.outStride + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
+                                reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
                         } else if (fOk && tok < tEnd) {
-                            if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[(size_t)tok * a.outStride + f] = v;
-                            if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[(size_t)tok * a.outStride + f] = res[j] + v;
-                            if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[(size_t)tok * a.outStride + f] = __float2bfloat16_rn(v);
+                            if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[orow + f] = v;
+                            if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[orow + f] = res[j] + v;
+                            if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + f] = __float2bfloat16_rn(v);
                         }
                     }
                 }
@@ -672,31 +611,28 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                 continue;
             }
             if (EPI == GEPI_RESIDUAL_AR) {
-                // ---- GEMM + all-reduce in one kernel: the accumulator tile goes from TMEM straight into LL words of
-                // every rank's slot[myRank] (NVLink peer stores, 256 B per warp store); after the TMEM buffer is released
-                // the same threads poll the slots of all source ranks for their (token, feature) cells, sum them in rank
-                // order, add the residual and clear the words.
+                // ---- GEMM + all-reduce in one kernel: the accumulator tile goes from registers straight into LL words of
+                // every rank's slot[myRank] (NVLink peer stores); then the same threads poll the slots of all source ranks for their
+                // (token, feature) cells, sum them in rank order, add the residual and clear the words.
                 const ArArgs &ar = a.ar;
                 const size_t slotBase = (size_t)(ar.parity * ar.nRanks + ar.rank) * ar.slotStride;
-                for (uint32_t c0 = 0; c0 < nTile; c0 += 16) {
+                for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
                     uint32_t r[16];
-                    loadAcc(acc, c0, r);
+                    loadAcc(c0, r);
 #pragma unroll
                     for (int j = 0; j < 16; j++) {
-                        const uint32_t tok = c0 + j;
-                        if (tok < a.T && fOk) {
+                        const uint32_t tok = rowOff + c0 + j;
+                        if (c0 + j < Teff && fOk) {
                             const size_t off = slotBase + (size_t)tok * ar.dim + f;
 #pragma unroll 1
                             for (uint32_t p = 0; p < ar.nRanks; p++) stLL(ar.slots[(ar.rank + p) % ar.nRanks] + off, r[j], 1u);
                         }
                     }
                 }
-                tcFenceBefore();
-                __syncwarp();
-                if (lane == 0) gmBarArrive(&tmemEmpty[acc]);
                 if (fOk) {
                     uint64_t *mine = ar.slots[ar.rank];
-                    for (uint32_t tok0 = 0; tok0 < a.T; tok0 += 16) {
+                    for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
+                        const uint32_t tok0 = rowOff + c0;
                         float sum[16];
 #pragma unroll
                         for (int j = 0; j < 16; j++) sum[j] = 0.f;
@@ -708,19 +644,19 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                                 all = true;
 #pragma unroll
                                 for (int j = 0; j < 16; j++) {
-                                    v[j] = (tok0 + j < a.T) ? ldLL(base + (size_t)(tok0 + j) * ar.dim) : make_uint2(0u, 1u);
+                                    v[j] = (c0 + j < Teff) ? ldLL(base + (size_t)(tok0 + j) * ar.dim) : make_uint2(0u, 1u);
                                     all = all && v[j].y != 0u;
                                 }
                             } while (!all);
 #pragma unroll
                             for (int j = 0; j < 16; j++) {
                                 sum[j] += __uint_as_float(v[j].x);
-                                if (tok0 + j < a.T) stLL(base + (size_t)(tok0 + j) * ar.dim, 0u, 0u);
+                                if (c0 + j < Teff) stLL(base + (size_t)(tok0 + j) * ar.dim, 0u, 0u);
                             }
                         }
 #pragma unroll
                         for (int j = 0; j < 16; j++) {
-                            if (tok0 + j < a.T) {
+                            if (c0 + j < Teff) {
                                 float *o = reinterpret_cast<float *>(a.out) + (size_t)(tok0 + j) * a.outStride + f;
                                 *o = __ldcg(o) + sum[j];
                             }
@@ -729,8 +665,7 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                 }
                 continue;
             }
-            for (uint32_t c0 = 0; c0 < nTile; c0 += 16) {
-                if (grouped && c0 >= Teff) break;   // warp-uniform: the remaining columns belong to other groups
+            for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
                 uint32_t r[16];
                 float resid[16];
                 if (EPI == GEPI_RESIDUAL) {   // issue all residual loads of the 16-column group before any store (no serialised RMW chain)
@@ -738,7 +673,7 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                     for (int j = 0; j < 16; j++)
                         resid[j] = (c0 + j < Teff && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(rowOff + c0 + j) * a.outStride + f) : 0.f;
                 }
-                loadAcc(acc, c0, r);
+                loadAcc(c0, r);
 #pragma unroll
                 for (int j = 0; j < 16; j++) {
                     const uint32_t tok = c0 + j;
@@ -755,12 +690,9 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                     }
                 }
             }
-            tcFenceBefore();
-            __syncwarp();
-            if (lane == 0) gmBarArrive(&tmemEmpty[acc]);
         }
     } else if (warp >= 8) {
-        // ===================== dequant: shared-memory q40 chunk -> bf16 UMMA tile =====================
+        // ===================== dequant: shared-memory q40 chunk -> bf16 wgmma tile =====================
         // Four groups of two warps; group g converts the g-th 64-wide k-slice of every 256-wide raw chunk, so four A tiles
         // are being converted concurrently and the load -> convert -> store -> proxy-fence latency of one slice overlaps
         // with the others (one group per slice instead of all eight warps serialising on every slice).
@@ -772,7 +704,7 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
         uint32_t itR = 0, rsD = 0, rphD = 0;
         for (uint32_t item = blockIdx.x; item < nItems; item += gridDim.x) {
             const uint32_t ks = item % splitK;
-            if (grouped && tileTokens(item / splitK) == 0) continue;
+            if (tileTokens(itemTile(item), itemTT(item)) == 0) continue;
             for (uint32_t kq = kqBegin(ks); kq < kqBegin(ks + 1); kq++, itR++) {
                 const uint32_t rs = rsD, rph = rphD;
                 if (++rsD == a.rawStages) { rsD = 0; rphD ^= 1u; }
@@ -803,7 +735,7 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                 const uint32_t itA = itR * 4 + grp;
                 const uint32_t s = itA & aMask, ph = (itA >> aShift) & 1;
                 if (trd) tq[2] = gmClock();
-                gmBarWait(&emptyBar[s >> pShift], ph ^ 1);
+                gmBarWait(&emptyBar[s], ph ^ 1);
                 if (trd) tq[3] = gmClock();
                 uint8_t *aTile = smem + (size_t)s * kGmATileBytes;
 #pragma unroll
@@ -838,18 +770,11 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                 __syncwarp();
                 if (trd) tq[5] = gmClock();
                 if (lane == 0) {
-                    gmBarArrive(&fullBar[s >> pShift]);
+                    gmBarArrive(&fullBar[s]);
                     if (lateRelease) gmBarArrive(&rawEmpty[rs]);
                 }
             }
         }
-    }
-
-    tcFenceBefore();
-    __syncthreads();
-    if (warp == 2) {
-        tcFenceAfter();
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmemBase), "r"(a.tmemCols) : "memory");
     }
 }
 
@@ -912,30 +837,26 @@ static bool encode2d(EncodeTiledFn enc, CUtensorMap *map, CUtensorMapDataType ty
 // Shared-memory geometry of the TMA-staged variant: A ring (multiple of 4: each dequant group always revisits its own stages),
 // B ring (>= 2 activation tiles), raw q40 ring. Returns the dynamic shared-memory size, 0 if nothing fits.
 static size_t tmaGeometry(GemmArgs &a) {
-    const size_t bTile = (size_t)a.nTile * 128;
-    const size_t budget = 227 * 1024 - 1024 - 1024;   // 1 KB alignment slack + 1 KB of mbarriers
-    // Candidates in order of preference: {k-slices per MMA step, A slices, raw stages, minimum B steps}. Two slices per step halve the
-    // barrier probes / commits of the issuing warp (it paces the k-loop at <= 128 tokens); then the deeper A ring (two slices per
-    // dequant group), then >= 4 k-slices of activations in flight (2 measured ~15 % slower, more than 4 gains nothing).
-    static const uint32_t cand[9][4] = {{2, 8, 3, 2}, {2, 8, 2, 2}, {2, 4, 3, 2}, {1, 8, 3, 4}, {1, 8, 2, 4}, {1, 4, 3, 4}, {1, 4, 2, 4}, {1, 8, 2, 2}, {1, 4, 2, 2}};
-    if (const char *ea = getenv("DL_GEMM_GEOM")) {   // experiment: "kPair,A,raw,B"
-        unsigned gp = 0, ga = 0, gr = 0, gb = 0;
-        if (sscanf(ea, "%u,%u,%u,%u", &gp, &ga, &gr, &gb) == 4 && (gp == 1 || gp == 2) && (ga == 4 || ga == 8) && gr >= 2 && gr <= (unsigned)kGmRawStagesMax &&
-            gb >= 2 && gb <= ga / gp) {
-            const size_t need = (size_t)ga * kGmATileBytes + (size_t)gr * kGmRawStageBytes + gb * gp * bTile;
-            if (need <= budget) { a.kPair = gp; a.stages = ga; a.rawStages = gr; a.bStages = gb; return need + 1024 + 1024; }
+    const size_t bTile = kGmBTileBytes;
+    const size_t budget = 227 * 1024 - 1024 - 1024 - kGmStgBytes;   // 1 KB alignment slack + 1 KB of mbarriers + epilogue staging
+    // Candidates in order of preference: {A slices, raw stages, minimum B slices}: the deeper A ring (two slices per dequant group)
+    // first, then >= 4 k-slices of activations in flight.
+    static const uint32_t cand[6][3] = {{8, 3, 4}, {8, 2, 4}, {4, 3, 4}, {4, 2, 4}, {8, 2, 2}, {4, 2, 2}};
+    if (const char *ea = getenv("DL_GEMM_GEOM")) {   // experiment: "A,raw,B"
+        unsigned ga = 0, gr = 0, gb = 0;
+        if (sscanf(ea, "%u,%u,%u", &ga, &gr, &gb) == 3 && (ga == 4 || ga == 8) && gr >= 2 && gr <= (unsigned)kGmRawStagesMax && gb >= 2 && gb <= ga) {
+            const size_t need = (size_t)ga * kGmATileBytes + (size_t)gr * kGmRawStageBytes + gb * bTile;
+            if (need <= budget) { a.stages = ga; a.rawStages = gr; a.bStages = gb; return need + 1024 + 1024 + kGmStgBytes; }
         }
     }
-    for (int i = 0; i < 9; i++) {
-        const uint32_t kp = cand[i][0], nA = cand[i][1], nRaw = cand[i][2], minB = cand[i][3];
-        if (kp == 2 && (a.debugFlags & 16u)) continue;
-        const size_t fixed = (size_t)nA * kGmATileBytes + (size_t)nRaw * kGmRawStageBytes, bStage = kp * bTile;
-        if (fixed + minB * bStage > budget) continue;
-        size_t nb = (budget - fixed) / bStage;
-        const size_t cap = kp == 2 ? nA / 2 : 4;      // released through the A ring's barriers: never deeper than it (in steps)
-        if (nb > cap) nb = cap;
-        a.kPair = kp; a.stages = nA; a.rawStages = nRaw; a.bStages = (uint32_t)nb;
-        return fixed + nb * bStage + 1024 + 1024;
+    for (int i = 0; i < 6; i++) {
+        const uint32_t nA = cand[i][0], nRaw = cand[i][1], minB = cand[i][2];
+        const size_t fixed = (size_t)nA * kGmATileBytes + (size_t)nRaw * kGmRawStageBytes;
+        if (fixed + minB * bTile > budget) continue;
+        size_t nb = (budget - fixed) / bTile;
+        if (nb > 4) nb = 4;      // released through the A ring's barriers: never deeper than it
+        a.stages = nA; a.rawStages = nRaw; a.bStages = (uint32_t)nb;
+        return fixed + nb * bTile + 1024 + 1024 + kGmStgBytes;
     }
     return 0;
 }
@@ -955,16 +876,11 @@ int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t
     GemmArgs a{};
     a.act = gHiddenAct;
     a.qs = (const uint32_t *)qs; a.scales = (const __half *)scales; a.d = d; a.n = n; a.T = T;
-    a.nTile = (T + 15) / 16 * 16;
     a.out = out; a.outStride = outStride;
     if (ar) a.ar = *ar;
     { const char *dbg = getenv("DL_GEMM_DEBUG"); a.debugFlags = dbg ? (uint32_t)atoi(dbg) : 0u; }
-    uint32_t cols = 32;
-    while (cols < 2 * a.nTile) cols *= 2;
-    a.tmemCols = cols;
-    const size_t stageBytes = kGmATileBytes + (size_t)a.nTile * 128;
-    const size_t budget = 227 * 1024 - 1024 - 512;
-    size_t rawBytes = 0;
+    const size_t stageBytes = kGmATileBytes + kGmBTileBytes;
+    const size_t budget = 227 * 1024 - 1024 - 512 - kGmStgBytes;
     uint32_t stages = 0;
     size_t tmaSmem = 0;
     if (tma) {
@@ -982,10 +898,10 @@ int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t
         if (stages < 2) return -3;
     }
     a.stages = stages;
-    const size_t smemBytes = tma ? tmaSmem : stages * stageBytes + rawBytes + 1024 + 512;
+    const size_t smemBytes = tma ? tmaSmem : stages * stageBytes + 1024 + 512 + kGmStgBytes;
 
     CUtensorMap mapB, mapQ, mapS;
-    if (!encode2d(enc, &mapB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, act, n, T, (uint64_t)actStride * 2, kGmBlockK, a.nTile, CU_TENSOR_MAP_SWIZZLE_128B))
+    if (!encode2d(enc, &mapB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, act, n, T, (uint64_t)actStride * 2, kGmBlockK, kGmTokTile, CU_TENSOR_MAP_SWIZZLE_128B))
         return -4;
     if (tma) {
         if (a.debugFlags & 256u) {
@@ -997,26 +913,26 @@ int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t
         }
     }
     const uint32_t nTilesM = (d + kGmBlockM - 1) / kGmBlockM;
+    const uint32_t nTT = (T + kGmTokTile - 1) / kGmTokTile;
     a.splitK = 1;
     if (tma && epi != GEPI_RESIDUAL_AR) {
-        // small-d matrices (qkv, wo, w2) leave most SMs idle with one CTA per 128-row tile: cut K so that ~all SMs get an item
+        // small-d matrices (qkv, wo, w2) leave most SMs idle with one CTA per work item: cut K so that ~all SMs get an item
         const uint32_t nkq = n / 256;
-        uint32_t sk = (uint32_t)numSms / nTilesM;
-        // The k-loop of one CTA is latency-bound (~290 ns per 64 of K whatever the number of busy SMs), so idle SMs are worth a
-        // split even at K = 4096; the cooperative reduce costs a few us. At most 4 splits (reduce register budget), every split
-        // keeps >= 4 raw chunks (1024 of K), and all items must be co-resident (the reduce waits for its sibling splits).
+        uint32_t sk = (uint32_t)numSms / (nTilesM * nTT);
+        // The k-loop of one CTA is latency-bound, so idle SMs are worth a split even at K = 4096; the cooperative reduce costs a
+        // few us. At most 4 splits (reduce register budget), every split keeps >= 4 raw chunks (1024 of K), and all items must be
+        // co-resident (the reduce waits for its sibling splits).
         if (sk > 4) sk = 4;
         if (sk > nkq / 4) sk = nkq / 4;
         // reduce over distributed shared memory (thread-block cluster) when the receive buffer ((sk - 1) x per x 128 f32) fits into the
-        // idle A ring: ~4 us cheaper than the global-scratch reduce (wo 30.7 -> 26.6 us, w2 43.0 -> 38.9 us at T = 64)
+        // idle A ring: two DSMEM hops instead of the global-scratch round trips
         const char *clEnv = getenv("DL_GEMM_CLUSTER");
         auto clusterFits = [&](uint32_t k) {
-            const uint32_t per = ((T + k - 1) / k + 15u) & ~15u;
-            // clusters of 2 or 4 only: clusters of 3 measured much slower (qkv 43.1 vs 32.8 us unsplit), presumably placement inside a GPC
+            const uint32_t per = ((min(T, (uint32_t)kGmTokTile) + k - 1) / k + 15u) & ~15u;
+            // clusters of 2 or 4 only (a power of two divides the GPC evenly)
             return (k == 2 || k == 4) && (size_t)(k - 1) * per * kGmBlockM * 4 <= (size_t)a.stages * kGmATileBytes && !(clEnv && clEnv[0] == '0');
         };
-        // K < 8192 with fewer than 4 splits (d = 6144: 48 tiles, 3 splits) does not pay: 29.5 vs 29.6 us with the global-scratch reduce,
-        // 43.1 vs 32.8 us with clusters of 3 (T = 64)
+        // K < 8192 with fewer than 4 splits does not pay for the reduce
         if (nkq < 32 && sk < 4) sk = 1;
         if (const char *f = getenv("DL_GEMM_SPLITK")) { const uint32_t want = (uint32_t)atoi(f); if (want >= 1 && want < sk) sk = want; }
         if (sk >= 2) {
@@ -1030,13 +946,13 @@ int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t
                 DL_CUDA_CHECK(cudaMalloc(&gSplitCounters, 4096 * sizeof(unsigned int)));
                 DL_CUDA_CHECK(cudaMemset(gSplitCounters, 0, 4096 * sizeof(unsigned int)));
             }
-            if (nTilesM * 8 <= 4096) {
+            if (nTilesM * nTT * 8 <= 4096) {
                 a.splitK = sk; a.splitScratch = gSplitScratch; a.splitCounters = gSplitCounters;
                 a.clusterSplit = clusterFits(sk) ? 1u : 0u;
             }
         }
     }
-    const uint32_t nItems = nTilesM * a.splitK;
+    const uint32_t nItems = nTilesM * nTT * a.splitK;
     const int grid = (int)(nItems < (uint32_t)numSms ? nItems : (uint32_t)numSms);
     const CUtensorMap *pq = tma ? &mapQ : nullptr, *ps = tma ? &mapS : nullptr;
     switch (epi) {
@@ -1063,20 +979,16 @@ int gemmQ40TcGrouped(int epi, const void *qs, const void *scales, uint32_t nGrou
     GemmArgs a{};
     a.act = gHiddenAct;
     a.qs = (const uint32_t *)qs; a.scales = (const __half *)scales; a.d = nGroups * grpRows; a.n = n; a.T = maxTokens;
-    a.nTile = (maxTokens + 15) / 16 * 16;
     a.out = out; a.outStride = outStride;
     a.grpCount = grpCount; a.grpOffset = grpOffset; a.grpRows = grpRows; a.grpTiles = (grpRows + kGmBlockM - 1) / kGmBlockM; a.nGroups = nGroups;
     a.splitK = 1;
-    uint32_t cols = 32;
-    while (cols < 2 * a.nTile) cols *= 2;
-    a.tmemCols = cols;
     const size_t smemBytes = tmaGeometry(a);
     if (!smemBytes) return 1;
     CUtensorMap mapB, mapQ, mapS;
-    if (!encode2d(enc, &mapB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, act, n, rowsTotal, (uint64_t)actStride * 2, kGmBlockK, a.nTile, CU_TENSOR_MAP_SWIZZLE_128B)) return -4;
+    if (!encode2d(enc, &mapB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, act, n, rowsTotal, (uint64_t)actStride * 2, kGmBlockK, kGmTokTile, CU_TENSOR_MAP_SWIZZLE_128B)) return -4;
     if (!encode2d(enc, &mapQ, CU_TENSOR_MAP_DATA_TYPE_UINT8, qs, n / 2, a.d, n / 2, 128, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_128B)) return -7;
     if (!encode2d(enc, &mapS, CU_TENSOR_MAP_DATA_TYPE_UINT8, scales, n / 16, a.d, n / 16, 16, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_NONE)) return -8;
-    const uint32_t nItems = nGroups * a.grpTiles;
+    const uint32_t nItems = nGroups * a.grpTiles * ((maxTokens + kGmTokTile - 1) / kGmTokTile);
     const int grid = (int)(nItems < (uint32_t)numSms ? nItems : (uint32_t)numSms);
     switch (epi) {
         case GEPI_STORE_F32: return launchGemm<GEPI_STORE_F32>(mapB, &mapQ, &mapS, a, grid, smemBytes, stream, false);

@@ -6,7 +6,7 @@
 //   CAST(f32->q80) + MATMUL + [all-gather + MERGE_ADD residual]      src/llm.cpp:385-411, :533-566
 //   ... + SILU + MUL (SwiGLU)                                        src/llm.cpp:509-532
 // The integer math is the reference's Q80×Q40 contract (nn-cpu-ops.cpp:231-449: int8 dot per 32-block, scaled
-// by d_w·d_x); everything else about the kernel is Blackwell-specific:
+// by d_w·d_x); everything else about the kernel is specific to the GPU:
 //   * one persistent CTA per SM (512 threads); each CTA owns a contiguous, pair-aligned row tile, so the
 //     per-SM byte share of the weight stream is equal to within one row pair;
 //   * a warp-step = (row, 32-block segment): lanes read 512 contiguous bytes of nibbles, U steps are issued

@@ -90,7 +90,7 @@ struct AttnArgs {
 };
 int launchAttnDecode(const AttnArgs &a, int nb, cudaStream_t stream, bool pdl);
 
-// Prompt-chunk attention on tcgen05 (attn_prefill_tc.cu): T consecutive tokens at positions p0.., causal, GQA heads packed on MMA-M.
+// Prompt-chunk attention on the tensor cores (attn_prefill_tc.cu, wgmma): T consecutive tokens at positions p0.., causal, GQA heads packed on MMA-M.
 struct AttnPrefillArgs {
     const float *qkv;            // [T][qkvStride] f32, q rows already normalised + rotated; K/V of the chunk already in the cache
     uint32_t qkvStride;
@@ -204,7 +204,7 @@ struct MegaArgs {
 
 int launchMegaDecode(MegaArgs m, int numSms, cudaStream_t stream);
 
-// tcgen05 prefill GEMM (gemm_q40_tc.cu)
+// tensor-core prefill GEMM (gemm_q40_tc.cu, wgmma)
 enum { GEPI_STORE_F32_ = 0, GEPI_RESIDUAL_ = 1, GEPI_SWIGLU_BF16_ = 2, GEPI_STORE_BF16_ = 3 };
 int gemmQ40Tc(int epi, const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride, uint32_t T,
               void *out, uint32_t outStride, int numSms, cudaStream_t stream, bool pdl);

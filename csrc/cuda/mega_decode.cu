@@ -1,6 +1,6 @@
 // Persistent single-token decode kernel: one launch per generated token for dense models (Llama / Qwen3).
 //
-// The multi-kernel decode path pays ~3 µs of grid-completion latency at each of its 161 kernel boundaries and restarts the
+// The multi-kernel decode path pays a grid-completion latency at each of its 161 kernel boundaries and restarts the
 // weight stream at every launch. Here one CTA per SM stays resident for the whole token:
 //   * warp 16 (producer) walks the list of all weight matrices of the token and streams this CTA's row tile of each one
 //     through a single shared-memory ring with cp.async.bulk + mbarriers. It never synchronises with the phases — only
@@ -9,10 +9,10 @@
 //     W1|W3 GEMV + SwiGLU | W2 GEMV + residual] -> logits GEMV + arg-max, separated by software grid barriers.
 //   * Every vector that crosses a phase boundary (x, q|k|v, z, h) travels as LL words: 8-byte {f32 payload, epoch} stores that
 //     L2 delivers atomically. The barrier therefore needs NO memory fence (a relaxed arrive + relaxed poll): it only orders
-//     control flow, and a consumer that finds a word with a stale epoch simply re-reads it. Measured on B200 with the weight
-//     stream running (profiles/barrier_microbench.txt): fenced barrier 2.2 us, relaxed 0.9 us — MEMBAR.GPU queues behind the
-//     ~180 KB of bulk-copy reads each SM keeps in flight. Round 1 tried LL words *instead of* barriers and lost (every thread
-//     polling during the arrival skew floods L2, experiments/README.md); here the poll starts only after the arrival counter
+//     control flow, and a consumer that finds a word with a stale epoch simply re-reads it. With the weight stream running a
+//     fenced barrier costs more than a relaxed one (tools/microbench_barrier.py): MEMBAR.GPU queues behind the
+//     bulk-copy reads each SM keeps in flight. LL words *instead of* barriers lose (every thread
+//     polling during the arrival skew floods L2); here the poll starts only after the arrival counter
 //     says the stores have been issued, so it almost always succeeds on the first read.
 //   * tensor-parallel runs use the same LL-word protocol between GPUs in the WO / W2 epilogues (one multimem.st through the
 //     NVSwitch multicast mapping reaches every rank; unicast peer stores when no multicast object exists) and the cross-rank
@@ -190,8 +190,8 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
             }
             float ss = 0.f;
             // NB: issuing the LL loads of several float4 before checking any epoch (one L2 round trip instead of one per value) was
-            // measured and rejected: the extra live registers push the 96-register kernel (17 warps are allocated as 20) into spilling
-            // inside the dp4a main loop (w13 main loop 8.0 -> 11.0 us per layer).
+            // rejected: the extra live registers push the 96-register kernel (17 warps are allocated as 20) into spilling
+            // inside the dp4a main loop.
 #pragma unroll
             for (int k = 0; k < kMaxVec; k++) {
                 const uint32_t i = vecBase + k * kConsumerThreads + tid;
@@ -351,7 +351,7 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
                 SpinGuard g(m.abortFlag);
                 const bool timeIt = m.syncNs && blockIdx.x == 0 && tid == 0;     // "Sync" time of the CLI lines: wait for the peers' partial sums
                 const uint64_t tSync0 = timeIt ? globalTimerNs() : 0;
-                // (requesting the N words in batches of 4 before examining them measured 1092 vs 1145 tok/s at N = 8: kept sequential)
+                // (requesting the N words in batches of 4 before examining them was slower at N = 8: kept sequential)
                 for (uint32_t sr = 0; sr < ar.nRanks; sr++) {
                     uint64_t *w = mine + (size_t)(arParity * ar.nRanks + sr) * ar.slotStride + rowBase + r;
                     uint2 v2 = ldLL(w);
@@ -710,8 +710,8 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
             bool wrapped = false;   // every stage has been filled once: from now on wait for the consumers to free it
             // Pacing: at most `maxInflight` fills are outstanding at any time. The ring (capacity) still runs up to nStages
             // fills ahead of the consumers, but a freshly drained ring is refilled by a short pipeline of requests instead of
-            // one 180 KB burst per SM: 26 MB of queued bulk reads chip-wide put ~1-4 us of queueing delay in front of every
-            // latency-critical load (barrier polls, activation vectors) at the L2 slices (profiles/barrier_microbench.txt).
+            // one ring-sized burst per SM: tens of MB of queued bulk reads chip-wide put microseconds of queueing delay in front
+            // of every latency-critical load (barrier polls, activation vectors) at the L2 slices (tools/microbench_barrier.py).
             RingPos landed{0u, 0u};
             uint32_t nIssued = 0, nLanded = 0;
             const uint32_t maxInflight = m.maxInflight ? m.maxInflight : m.nStages;

@@ -1,4 +1,4 @@
-// Mixture-of-experts feed-forward over a prompt chunk (T tokens): routing -> token sort by expert -> grouped tcgen05 GEMMs ->
+// Mixture-of-experts feed-forward over a prompt chunk (T tokens): routing -> token sort by expert -> grouped tensor-core GEMMs ->
 // weighted combine (+ tensor/expert-parallel all-reduce over peer memory).
 //
 // Reference: the MoE branch of buildLlmNet (src/llm.cpp:425-499) run at nBatches = 32: REPEAT_Z, gate MATMUL, SOFTMAX, MOE_GATE, per

@@ -87,7 +87,7 @@ DL_EXPORT int dl_repack_q40(const void *src, uint64_t srcRowPitch, uint64_t srcC
                      (__half *)dstScales, dstRowStride, dstRowOffset, headDim};
     const uint64_t total = (uint64_t)rows * blocksPerRow;
     if (total == 0) return 0;
-    const int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int grid = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     dl::repackQ40Kernel<<<grid, 256, 0, stream>>>(a);
     DL_CUDA_CHECK(cudaGetLastError());
     return 0;
@@ -97,7 +97,7 @@ DL_EXPORT int dl_dequant_device_q40(const void *qs, const void *scales, uint32_t
                                     cudaStream_t stream) {
     const uint64_t total = (uint64_t)rows * blocksPerRow;
     if (total == 0) return 0;
-    const int grid = (int)((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+    const int grid = (int)((total + 255) / 256 < 132 * 16 ? (total + 255) / 256 : 132 * 16);
     dl::dequantDeviceQ40Kernel<<<grid, 256, 0, stream>>>((const uint32_t *)qs, (const __half *)scales, rows, blocksPerRow, out);
     DL_CUDA_CHECK(cudaGetLastError());
     return 0;

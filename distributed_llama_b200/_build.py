@@ -1,10 +1,10 @@
 """In-tree builder for the two native libraries.
 
 * ``_host``  – pybind11 module (g++ only): formats, codecs, slicers, tokenizer, sampler.
-* ``_cuda``  – plain C-ABI shared library (nvcc, sm_100a only): kernels, engine runtime, peer-memory comm.
+* ``_cuda``  – plain C-ABI shared library (nvcc, sm_90a only): kernels, engine runtime, peer-memory comm.
   Loaded through ctypes so the kernels carry no torch/pybind dependency and compile in seconds.
 
-Artifacts are written next to this file (git-ignored, but shipped to the GPU box by gpurun).
+Artifacts are written next to this file (git-ignored).
 A source hash is stored beside each artifact so stale builds are rebuilt and fresh ones are reused.
 """
 from __future__ import annotations
@@ -23,7 +23,7 @@ REPO_DIR = PKG_DIR.parent
 CSRC = REPO_DIR / "csrc"
 _lock = threading.Lock()
 
-NVCC_ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+NVCC_ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def _hash_sources(files, extra: str = "") -> str:

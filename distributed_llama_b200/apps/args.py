@@ -1,7 +1,7 @@
 """Command-line flags of `dllama` / `dllama-api` — same surface as the reference parser (src/app.cpp:24-135):
 `--key value` pairs, first positional = mode, `--workers` variadic, `--help/-h/--usage` short-circuit, unknown flags
 are an error. Flags that only make sense for the CPU/TCP design (`--nthreads`, `--net-turbo`, `--gpu-index`,
-`--gpu-segments`, `--workers host:port`) are accepted for drop-in compatibility; on the B200 build the worker set is
+`--gpu-segments`, `--workers host:port`) are accepted for drop-in compatibility; on the GPU build the worker set is
 the torch.distributed world (one process per GPU), so `--workers` only has to name as many entries as there are ranks-1.
 """
 from __future__ import annotations
@@ -35,7 +35,7 @@ class AppArgs:
     gpu_index: int = -1
     gpu_segments: Optional[str] = None
     benchmark: bool = False
-    # B200 build extras
+    # GPU build extras
     gpus: int = 0            # spawn this many local ranks (0 = use the current torch.distributed world / single GPU)
     moe_mode: str = "auto"   # tp | ep | auto
 
@@ -120,7 +120,7 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
 USAGE = """Usage: dllama {inference|chat|perplexity|worker} {--model <path>} {--tokenizer <path>}
         [--prompt <text>] [--steps <n>] [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>]
         [--temperature <temp>] [--topp <t>] [--seed <s>] [--chat-template {llama2|llama3|deepSeek3|chatml}]
-        [--gpus <n>]                      run tensor-parallel on n local B200s (spawns one process per GPU)
+        [--gpus <n>]                      run tensor-parallel on n local GPUs (spawns one process per GPU)
         [--workers <ip:port> ...] [--nthreads <n>] [--net-turbo {0|1}] [--gpu-index <i>] [--gpu-segments <a:b>]
                                           accepted for compatibility with the reference CLI
 """

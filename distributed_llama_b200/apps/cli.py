@@ -188,7 +188,7 @@ def worker(args: AppArgs) -> None:
 
 
 def _respawn_with_torchrun(argv: List[str], gpus: int) -> int:
-    """`--gpus N`: start root + N-1 workers as N local processes (the B200 analogue of examples/n-workers.sh)."""
+    """`--gpus N`: start root + N-1 workers as N local processes (the GPU analogue of examples/n-workers.sh)."""
     port = 29500 + (os.getpid() % 2000)
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={gpus}", "--master-addr", "127.0.0.1",
            "--master-port", str(port), "-m", "distributed_llama_b200.apps.cli"] + argv

@@ -1,6 +1,6 @@
 """Root/worker application runtime (reference: runInferenceApp / runWorkerApp, src/app.cpp:232-365).
 
-Process model on the B200 box: one process per GPU. Rank 0 is the *root* (tokenizer, sampler, user I/O), ranks >= 1 are
+Process model on a multi-GPU node: one process per GPU. Rank 0 is the *root* (tokenizer, sampler, user I/O), ranks >= 1 are
 *workers*: they hold their tensor-parallel weight slices and mirror every forward the root issues. Control flows as the
 reference's 8-byte LlmControlPacket {position, batchSize} (src/app.hpp:46-49) — here extended with an opcode and passed through a
 shared-memory channel with heartbeats (parallel/control.py; torch.distributed broadcasts only when the ranks span hosts);
@@ -78,8 +78,9 @@ class RootInference:
         self.header = sess.header
         self.eval_ms = 0.0
         self._ctl = torch.zeros(4, dtype=torch.int64, device=sess.device) if (comm is not None and chan is None) else None
-        self._pin_out = torch.zeros(1, dtype=torch.int32).pin_memory() if torch.cuda.is_available() else None
-        self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory() if torch.cuda.is_available() else None
+        on_gpu = torch.device(sess.device).type == "cuda"   # the session's device, not whether the machine has a GPU
+        self._pin_out = torch.zeros(1, dtype=torch.int32).pin_memory() if on_gpu else None
+        self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory() if on_gpu else None
 
     def _send(self, op: int, pos: int, tokens: Sequence[int]):
         if self.comm is None:
@@ -106,7 +107,7 @@ class RootInference:
 
     def forward_greedy(self, token: int, pos: int) -> int:
         self._send(OP_STEP_GREEDY, pos, [token])
-        if self._pin_in is None:          # no CUDA device (CPU-side protocol tests)
+        if self._pin_in is None:          # session on the CPU (protocol tests)
             self.eng._set_inputs([token], pos)
             self.eng.run_decode_step()
             return int(self.eng.tokens[0])
@@ -123,7 +124,7 @@ class RootInference:
     # ---- sampling on the device: the logits never leave the GPUs (csrc/cuda/sampler.cu) ----
     @property
     def device_sampling(self) -> bool:
-        return torch.cuda.is_available() and not getattr(self.eng, "_parts", False) and os.environ.get("DL_HOST_SAMPLER") is None
+        return self._pin_in is not None and not getattr(self.eng, "_parts", False) and os.environ.get("DL_HOST_SAMPLER") is None
 
     def seed(self, seed: int) -> None:
         self._send(OP_SEED, 0, [seed & 0x7FFFFFFF, (seed >> 31) & 0x7FFFFFFF, (seed >> 62) & 0x3])
@@ -239,7 +240,7 @@ def run_inference_app(args: AppArgs, handler: Callable[[AppContext], None]) -> N
         req = H.required_device_bytes(header, n_nodes, 2)
         print(f"📀 RequiredMemory: {req // (1024 * 1024)} MB")
         name = torch.cuda.get_device_name(sess.device)
-        print(f"🧠 GPU: {name} x{n_nodes} (sm_100a kernels; tensor parallel over NVLink peer memory)")
+        print(f"🧠 GPU: {name} x{n_nodes} (sm_90a kernels; tensor parallel over NVLink peer memory)")
         print("💿 Weights loaded")
     inf = RootInference(sess, comm, chan)
     ctx = AppContext(args=args, sess=sess, inference=inf, tokenizer=tok, sampler=sess.sampler, header=header)

@@ -1,4 +1,4 @@
-"""ctypes binding of the sm_100a kernel/runtime library (csrc/cuda -> distributed_llama_b200/_cuda.so).
+"""ctypes binding of the sm_90a kernel/runtime library (csrc/cuda -> distributed_llama_b200/_cuda.so).
 
 The library is torch-free: tensors cross the boundary as raw device pointers + the current CUDA stream handle.
 If the library is missing on a machine with a GPU we build it; failures are loud (no eager fallback).

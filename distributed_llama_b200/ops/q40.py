@@ -93,7 +93,7 @@ def gemv_q40(w: DeviceQ40, x: torch.Tensor, *, pro: int, epi: int, out: torch.Te
 
 def gemm_q40_tc(w: DeviceQ40, act: torch.Tensor, *, epi: int, out: torch.Tensor, num_sms: int = 0, pdl: bool = False,
                 variant: str = "auto") -> torch.Tensor:
-    """tcgen05 prefill GEMM. act: bf16 [T, n] (T <= 256); out: [T, d] f32 (STORE/RESIDUAL), bf16 [T, d/2] (SWIGLU) or bf16 [T, d]."""
+    """Tensor-core (wgmma) prefill GEMM. act: bf16 [T, n] (T <= 256); out: [T, d] f32 (STORE/RESIDUAL), bf16 [T, d/2] (SWIGLU) or bf16 [T, d]."""
     assert act.dtype == torch.bfloat16 and act.is_cuda and act.stride(1) == 1
     if num_sms == 0:
         num_sms = torch.cuda.get_device_properties(act.device).multi_processor_count

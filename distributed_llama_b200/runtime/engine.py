@@ -240,7 +240,7 @@ class Engine:
 
     def prefill(self, tokens: Sequence[int], start_pos: int = 0, want_logits: bool = True) -> Optional[torch.Tensor]:
         """Feeds a prompt; returns the logits row of its last token (device tensor). Single GPU: chunks of up to 256 tokens
-        on the tcgen05 GEMM path. Tensor parallel: chunks of up to max_batch tokens on the GEMV path (fused all-reduce)."""
+        on the tensor-core GEMM path. Tensor parallel: chunks of up to max_batch tokens on the GEMV path (fused all-reduce)."""
         tokens = list(tokens)
         if start_pos + len(tokens) > self.seq_len:
             raise ValueError("position beyond the context length")

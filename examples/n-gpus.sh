@@ -1,5 +1,5 @@
 #!/bin/bash
-# Start root + workers on N local B200s in one command (the analogue of the reference's examples/n-workers.sh, which
+# Start root + workers on N local GPUs in one command (the analogue of the reference's examples/n-workers.sh, which
 # spawns N TCP workers in `screen`): here every rank is a torchrun-managed process bound to one GPU.
 #
 #   N=8 MODEL=model.m TOKENIZER=tok.t bash examples/n-gpus.sh inference --prompt "Hello" --steps 64

@@ -7,7 +7,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box via gpurun)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

@@ -1,4 +1,4 @@
-"""tcgen05 prompt-chunk attention (csrc/cuda/attn_prefill_tc.cu) vs a plain PyTorch f32 reference of the same op:
+"""Tensor-core prompt-chunk attention (csrc/cuda/attn_prefill_tc.cu) vs a plain PyTorch f32 reference of the same op:
 causal softmax(q.k^T / sqrt(hd)).v over a bf16 head-major KV cache, GQA, chunk of T tokens starting at position p0."""
 import math
 

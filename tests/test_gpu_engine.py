@@ -60,7 +60,7 @@ def test_graph_decode_equals_eager(tmp_models):
 
 @pytest.mark.parametrize("name", ["tiny-llama31", "tiny-qwen3", "tiny-qwen3-moe"])
 def test_tensor_core_prefill_matches_oracle(tmp_models, name):
-    """Prompt chunks > 8 tokens run on the tcgen05 GEMM path (bf16 activations); later decode steps read its KV cache."""
+    """Prompt chunks > 8 tokens run on the tensor-core GEMM path (bf16 activations); later decode steps read its KV cache."""
     mf, eng, oracle = _setup(tmp_models, name)
     toks = [(7 * i + 3) % 500 + 1 for i in range(45)]
     ref = oracle.forward(toks, 0)

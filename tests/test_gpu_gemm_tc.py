@@ -1,4 +1,4 @@
-"""tcgen05 prefill GEMM (q40 dequant fused into the prologue) vs a plain PyTorch f32 reference."""
+"""Tensor-core prefill GEMM (q40 dequant fused into the prologue) vs a plain PyTorch f32 reference."""
 import numpy as np
 import pytest
 import torch
@@ -10,10 +10,11 @@ from test_gpu_kernels import _rand_q40, _device_q40   # noqa: E402
 
 @pytest.mark.parametrize("variant", ["ldg", "tma"])
 @pytest.mark.parametrize("d,n,T", [(256, 256, 16), (128, 64, 1), (384, 512, 17), (6144, 4096, 64), (4096, 14336, 64),
-                                   (1024, 1792, 200), (2048, 4096, 256), (1000, 2176, 33), (28672, 4096, 100), (4096, 4096, 192)])
+                                   (1024, 1792, 200), (2048, 4096, 256), (1000, 2176, 33), (28672, 4096, 100), (4096, 4096, 192),
+                                   (4096, 14336, 128)])
 def test_gemm_store_f32(d, n, T, variant):
-    if variant == "tma" and (n % 256 or T > 208):
-        pytest.skip("TMA-staged variant needs n % 256 == 0 and room for 4 pipeline stages")
+    if variant == "tma" and n % 256:
+        pytest.skip("TMA-staged variant needs n % 256 == 0")
     from distributed_llama_b200 import ops
     raw, wq = _rand_q40(d, n, seed=5)
     w = _device_q40(raw, d, n)
@@ -26,6 +27,24 @@ def test_gemm_store_f32(d, n, T, variant):
     err = (out - ref).abs().max().item()
     scale = ref.abs().max().item()
     assert err < 0.02 * scale + 1e-3, (err, scale)
+
+
+@pytest.mark.parametrize("cluster", ["1", "0"])
+def test_gemm_split_k_over_token_tiles(cluster, monkeypatch):
+    """Llama-3.1-8B w2 at a 128-token chunk: split-K over 2 token tiles, reduced inside a thread-block cluster or (cluster = 0)
+    through the global scratch; residual epilogue."""
+    from distributed_llama_b200 import ops
+    monkeypatch.setenv("DL_GEMM_CLUSTER", cluster)
+    d, n, T = 4096, 14336, 128
+    raw, wq = _rand_q40(d, n, seed=8)
+    w = _device_q40(raw, d, n)
+    torch.manual_seed(4)
+    act = torch.randn(T, n, device="cuda").bfloat16()
+    x = torch.randn(T, d, device="cuda")
+    ref = x + act.float() @ torch.from_numpy(wq).cuda().T
+    ops.gemm_q40_tc(w, act, epi=ops.GEPI_RESIDUAL, out=x, variant="tma")
+    torch.cuda.synchronize()
+    assert (x - ref).abs().max().item() < 0.02 * ref.abs().max().item() + 1e-3
 
 
 def test_gemm_residual_and_swiglu():

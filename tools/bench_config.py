@@ -89,11 +89,13 @@ if rank == 0:
         peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm = peaks.get("hbm_gbs", 6650.0)
+    hbm, hbm_source = peaks.get("hbm_gbs"), "measured"
+    if not hbm:
+        hbm, hbm_source = 3350.0, "H100 SXM data sheet"
     print(json.dumps({"model": args.model, "n_gpus": world, "decode_tok_s": round(1000.0 / ms, 1), "ms_per_step": round(ms, 4), "decode_pos": pos0,
                       "ttft_ms": round(min(ttft[1:]), 3), "prompt_len": args.prompt_len, "decode_path": "persistent megakernel" if (eng.mega and eng.mega_active) else "multi-kernel",
                       "moe_mode": W.moe_mode, "weight_bytes_streamed_per_step_per_gpu": int(wb),
-                      "frac_of_measured_hbm": round(wb / ms / 1e6 / hbm, 3), "weights_init_s": round(load_s, 1),
+                      "frac_of_peak_hbm": round(wb / ms / 1e6 / hbm, 3), "peak_hbm_gbs": hbm, "peak_hbm_source": hbm_source, "weights_init_s": round(load_s, 1),
                       "data": "random-init device weights (no file), synthetic prompt"}), flush=True)
 if world > 1:
     dist.barrier()

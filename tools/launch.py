@@ -4,7 +4,7 @@
     python tools/launch.py <model> [-skip-run] [-skip-script] [-y] [--gpus N]
 
 Same role as the reference's launch.py (launch.py:17-195): model table keyed by name (multi-part files are concatenated),
-resumable download with retries, `run_<model>.sh` generation. The run script starts this repo's `dllama` on N local B200s
+resumable download with retries, `run_<model>.sh` generation. The run script starts this repo's `dllama` on N local GPUs
 instead of building the CPU binary.
 """
 from __future__ import annotations

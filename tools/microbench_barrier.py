@@ -15,7 +15,7 @@ lib.dl_bench_grid_barrier.restype = C.c_int
 sms = torch.cuda.get_device_properties(0).multi_processor_count
 stream_buf = torch.empty(1 << 30, dtype=torch.uint8, device="cuda")
 names = {0: "red.release + ld.acquire poll (shipped)", 1: "relaxed red/poll, no fence (lower bound, not a data barrier)",
-         2: "per-CTA flag lines, warp polls 148 lines", 3: "8 group counters, 8 pollers", 4: "fence + relaxed red, relaxed polls + fence",
+         2: "per-CTA flag lines, warp polls one line per CTA", 3: "8 group counters, 8 pollers", 4: "fence + relaxed red, relaxed polls + fence",
          5: "flag words in one array, warp polls with 16-byte loads"}
 iters = 1000
 for traffic in (0, 1):

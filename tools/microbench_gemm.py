@@ -1,4 +1,4 @@
-"""tcgen05 prefill GEMM microbenchmark at Llama-3.1-8B shapes (CUDA events, weights >> L2 between shapes)."""
+"""Tensor-core prefill GEMM microbenchmark at Llama-3.1-8B shapes (CUDA events, weights >> L2 between shapes)."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

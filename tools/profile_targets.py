@@ -1,4 +1,4 @@
-"""Small driver for ncu captures: loads the 8B synthetic model, runs one prefill (tcgen05 GEMM path) and a few decode steps."""
+"""Small driver for ncu captures: loads the 8B synthetic model, runs one prefill (tensor-core GEMM path) and a few decode steps."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,5 +1,5 @@
-"""compute-sanitizer workload at the real Llama-3.1-8B shapes (random-init device weights): one tcgen05 prefill chunk (GEMMs with
-paired k-slices + cooperative split-K, tensor-core attention, PDL chain) and three tokens of the persistent decode kernel.
+"""compute-sanitizer workload at the real Llama-3.1-8B shapes (random-init device weights): one tensor-core prefill chunk (GEMMs with
+cooperative split-K, tensor-core attention, PDL chain) and three tokens of the persistent decode kernel.
     compute-sanitizer --tool memcheck python tools/sanitize_8b.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

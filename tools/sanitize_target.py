@@ -1,4 +1,4 @@
-"""Workload for compute-sanitizer (tools/sanitize.sh): tiny synthetic models through every kernel family — tcgen05 prefill,
+"""Workload for compute-sanitizer (tools/sanitize.sh): tiny synthetic models through every kernel family — tensor-core prefill,
 persistent decode kernel, multi-kernel PDL decode path, MoE router + routed GEMVs, dense f32 weights."""
 import os
 import sys

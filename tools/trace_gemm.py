@@ -1,4 +1,4 @@
-"""Pipeline timeline of the prefill GEMM (CTA 0): where the MMA issuer and one dequant group spend their cycles.
+"""Pipeline timeline of the prefill GEMM (CTA 0): where the MMA warpgroup (warp 4) and one dequant group spend their cycles.
 Needs DL_GEMM_DEBUG=512 (set here). Output: per-k-block stamps in SM clocks relative to the first event."""
 import ctypes as C, os, sys
 os.environ["DL_GEMM_DEBUG"] = str(512 | int(os.environ.get("DL_GEMM_DEBUG", "0")))
@@ -27,7 +27,7 @@ t = np.array(buf[:], dtype=np.int64)
 mma = t[:1024].reshape(256, 4)[:64]
 dq = t[1024:1024 + 4 * 64 * 8].reshape(4, 64, 8)[:, :16, :6]
 t0 = min(mma[0, 0], dq[:, 0, 0].min())
-print("MMA issuer, per k-block: start  +waitB  +waitA  +issue   (period)")
+print("MMA warpgroup, per k-block: start  +waitB  +waitA  +issue+release   (period)")
 prev = None
 for i in range(64):
     s, b, a_, e = mma[i] - t0
