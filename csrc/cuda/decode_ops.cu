@@ -603,3 +603,37 @@ int launchArgmaxAdvance(const float *logits, uint32_t vocab, int *tokenOut, int 
 }
 
 }  // namespace dl
+
+// Stand-alone entry points for the unit tests (tests/test_gpu_decode_attn.py): each fills the argument struct and calls the
+// launcher without programmatic dependent launch. Pointers are device pointers; caches are bf16 [nKvHeads][seqLen][headDim].
+DL_EXPORT int dl_rope_kv(float *qkv, uint32_t qkvStride, const int *pos, const float *rope, const float *qNorm, const float *kNorm,
+                         float eps, uint32_t nHeads, uint32_t nKvHeads, uint32_t headDim, uint32_t seqLen, void *kCache, void *vCache,
+                         int nb, cudaStream_t stream) {
+    dl::RopeKvArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos; a.rope = rope; a.qNorm = qNorm; a.kNorm = kNorm; a.eps = eps;
+    a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen;
+    a.kCache = (__nv_bfloat16 *)kCache; a.vCache = (__nv_bfloat16 *)vCache;
+    return dl::launchRopeKv(a, nb, stream, false);
+}
+
+DL_EXPORT int dl_attn_decode(const float *qkv, uint32_t qkvStride, const int *pos, const void *kCache, const void *vCache, uint32_t nHeads,
+                             uint32_t nKvHeads, uint32_t headDim, uint32_t seqLen, uint32_t nSplits, float *partial, unsigned int *counters,
+                             float *out, uint32_t outStride, void *outBf16, int nb, cudaStream_t stream) {
+    dl::AttnArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos;
+    a.kCache = (const __nv_bfloat16 *)kCache; a.vCache = (const __nv_bfloat16 *)vCache;
+    a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
+    a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride; a.outBf16 = (__nv_bfloat16 *)outBf16;
+    return dl::launchAttnDecode(a, nb, stream, false);
+}
+
+DL_EXPORT int dl_attn_fused(const float *qkv, const int *pos, const float *rope, const float *qNorm, const float *kNorm, float eps,
+                            void *kCache, void *vCache, uint32_t nHeads, uint32_t nKvHeads, uint32_t headDim, uint32_t seqLen,
+                            uint32_t nSplits, float *partial, unsigned int *counters, float *out, cudaStream_t stream) {
+    dl::AttnFusedArgs a{};
+    a.qkv = qkv; a.pos = pos; a.rope = rope; a.qNorm = qNorm; a.kNorm = kNorm; a.eps = eps;
+    a.kCache = (__nv_bfloat16 *)kCache; a.vCache = (__nv_bfloat16 *)vCache;
+    a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
+    a.partial = partial; a.counters = counters; a.out = out;
+    return dl::launchAttnFused(a, stream, false);
+}

@@ -53,25 +53,32 @@ class _TensorWriter:
                 x = self.rng.standard_normal((rows, n), dtype=np.float32) * np.float32(std)
                 self._emit(quants.quantize(float_type, x))
 
-    def norm(self, n: int):
-        x = (1.0 + 0.1 * self.rng.standard_normal(n, dtype=np.float32)).astype(np.float32)
+    def norm(self, n: int, gain: float = 1.0):
+        x = (1.0 + 0.1 * self.rng.standard_normal(n, dtype=np.float32)).astype(np.float32) * np.float32(gain)
         self._emit(x)
 
 
-def write_synthetic_model(path: str, cfg: ModelConfig, weights_float_type: int = quants.F_Q40, seed: int = 1234) -> int:
-    """Writes a random-weight model file for `cfg`; returns the file size in bytes."""
+def write_synthetic_model(path: str, cfg: ModelConfig, weights_float_type: int = quants.F_Q40, seed: int = 1234,
+                          attn_gain: float = 1.0) -> int:
+    """Writes a random-weight model file for `cfg`; returns the file size in bytes.
+
+    `attn_gain` scales the attention scores: it multiplies the std of the q and k matrices, or, for models with QK-norm
+    (where the norm weights set the score scale), the q/k norm weights. It draws no extra random numbers: every other
+    tensor is the same for any gain, and the default of 1.0 leaves the whole file unchanged."""
     tmp = path + ".tmp"
     head_dim = cfg.head_dim or cfg.dim // cfg.n_heads
     q_dim, kv_dim = head_dim * cfg.n_heads, head_dim * cfg.n_kv_heads
     ff = cfg.moe_hidden_dim if cfg.arch_type == ARCH_QWEN3_MOE else cfg.hidden_dim
     wt = weights_float_type
+    qk_norm = cfg.arch_type in (ARCH_QWEN3, ARCH_QWEN3_MOE)
+    qk_std = (1.0 if qk_norm else attn_gain) / np.sqrt(cfg.dim)
     with open(tmp, "wb") as f:
         write_model_header(f, cfg.header_params(wt))
         w = _TensorWriter(f, seed)
         w.matrix(quants.F_32, cfg.vocab_size, cfg.dim, std=1.0)
         for _ in range(cfg.n_layers):
-            w.matrix(wt, q_dim, cfg.dim)
-            w.matrix(wt, kv_dim, cfg.dim)
+            w.matrix(wt, q_dim, cfg.dim, std=qk_std)
+            w.matrix(wt, kv_dim, cfg.dim, std=qk_std)
             w.matrix(wt, kv_dim, cfg.dim)
             w.matrix(wt, cfg.dim, q_dim, std=0.5 / np.sqrt(q_dim))
             if cfg.n_experts > 0:
@@ -84,9 +91,9 @@ def write_synthetic_model(path: str, cfg: ModelConfig, weights_float_type: int =
                 w.matrix(wt, ff, cfg.dim)
                 w.matrix(wt, cfg.dim, ff, std=0.5 / np.sqrt(ff))
                 w.matrix(wt, ff, cfg.dim)
-            if cfg.arch_type in (ARCH_QWEN3, ARCH_QWEN3_MOE):
-                w.norm(head_dim)
-                w.norm(head_dim)
+            if qk_norm:
+                w.norm(head_dim, attn_gain)
+                w.norm(head_dim, attn_gain)
             w.norm(cfg.dim)
             w.norm(cfg.dim)
         w.norm(cfg.dim)

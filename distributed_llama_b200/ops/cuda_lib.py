@@ -62,6 +62,12 @@ def lib() -> C.CDLL:
     L.dl_rmsnorm_bf16.restype = i32
     L.dl_attn_prefill_tc.argtypes = [vp, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
     L.dl_attn_prefill_tc.restype = i32
+    L.dl_rope_kv.argtypes = [vp, u32, vp, vp, vp, vp, f32, u32, u32, u32, u32, vp, vp, i32, vp]
+    L.dl_rope_kv.restype = i32
+    L.dl_attn_decode.argtypes = [vp, u32, vp, vp, vp, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp, i32, vp]
+    L.dl_attn_decode.restype = i32
+    L.dl_attn_fused.argtypes = [vp, vp, vp, vp, vp, f32, vp, vp, u32, u32, u32, u32, u32, vp, vp, vp, vp]
+    L.dl_attn_fused.restype = i32
     L.dl_engine_create.argtypes = [C.POINTER(EngineConfig)]
     L.dl_engine_create.restype = vp
     L.dl_engine_destroy.argtypes = [vp]

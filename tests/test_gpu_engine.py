@@ -89,6 +89,7 @@ def test_persistent_decode_kernel(tmp_models, name):
     eng_m.enable_mega()
     eng_m.prefill(prompt[:-1], 0, want_logits=False)
     lg_m = eng_m.step(prompt[-1], len(prompt) - 1).clone()
+    assert eng_m.mega_active        # otherwise the comparison below would check the multi-kernel path against itself
     eng_c = _setup(tmp_models, name)[1]
     eng_c.enable_mega(False)
     eng_c.prefill(prompt[:-1], 0, want_logits=False)
@@ -99,6 +100,7 @@ def test_persistent_decode_kernel(tmp_models, name):
         e.enable_mega()
         e.prefill(prompt[:-1], 0, want_logits=False)
         toks = e.decode_greedy(prompt[-1], len(prompt) - 1, 40, use_graph=use_graph)
+        assert e.mega_active
         agree = sum(a == b for a, b in zip(toks, ref_toks))
         assert agree >= 36, (toks, ref_toks)
 
