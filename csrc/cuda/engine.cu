@@ -37,7 +37,7 @@ struct Engine {
     uint2 *megaX = nullptr, *megaQkv = nullptr, *megaZ = nullptr, *megaH = nullptr;   // LL vectors of the persistent kernel
     unsigned int *megaSeq = nullptr;
     unsigned int *abortHost = nullptr, *abortDev = nullptr;   // mapped pinned word: device wait loops report a blown spin budget here
-    uint32_t megaInflight = 2;         // DL_MEGA_INFLIGHT: producer pacing of the persistent kernel (0 = unpaced)
+    uint32_t megaInflight = 1;         // DL_MEGA_INFLIGHT: producer pacing of the persistent kernel (0 = unpaced; DESIGN.md §7)
     uint32_t megaCtas = 0;             // DL_MEGA_CTAS: grid size override of the persistent kernel (0 = one CTA per SM)
     bool useMega = false;
     bool lastDecodeMega = false, megaFallbackWarned = false;   // did the last single-token forward run on the persistent kernel?
@@ -140,6 +140,7 @@ static int engineDecodeMega(Engine &e, bool greedyAdvance, cudaStream_t stream) 
     m.trace = e.trace;
     m.traceCtas = e.traceAllCtas ? c.numSms : 1u;
     m.traceStride = e.traceAllCtas ? (uint32_t)(((size_t)e.traceCap * 4) / c.numSms) : 0u;
+    m.traceProdSlot = (e.trace && m.traceStride >= megaTraceRowSlots(c.nLayers)) ? megaTraceProdSlot(c.nLayers) : 0u;
     if (e.comm.nRanks > 1) fillAr(e, m.ar, 0);
     return launchMegaDecode(m, (int)(e.megaCtas ? e.megaCtas : c.numSms), stream);
 }

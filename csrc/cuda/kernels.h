@@ -199,8 +199,15 @@ struct MegaArgs {
     uint32_t act, vocabLimit;    // see GemvArgs
     uint64_t *trace;
     uint32_t traceCtas, traceStride;   // CTAs 0..traceCtas-1 record their phase stamps at trace[cta * traceStride + slot]
+    uint32_t traceProdSlot;      // != 0: first producer slot of a CTA's trace row (megaTraceProdSlot; all-CTA tracing only)
     ArArgs ar;
 };
+
+// Trace row of one CTA of the persistent kernel: 18 * nLayers + 5 consumer phase stamps, then (from this slot on, 8-aligned) two
+// producer counters per weight phase k = 4 * layer + {QKV, WO, W1|W3, W2}, k = 4 * nLayers for the logits: at 2k the ns the
+// producer waited for a free ring stage, at 2k + 1 the ns it waited on the in-flight cap.
+inline uint32_t megaTraceProdSlot(uint32_t nLayers) { return (18 * nLayers + 5 + 7) / 8 * 8; }
+inline uint32_t megaTraceRowSlots(uint32_t nLayers) { return megaTraceProdSlot(nLayers) + 2 * (4 * nLayers + 1); }
 
 int launchMegaDecode(MegaArgs m, int numSms, cudaStream_t stream);
 

@@ -145,6 +145,44 @@ __device__ __forceinline__ void megaTile(const MegaPhase &P, uint32_t &pairBegin
     tileRows = 2 * (P.pairsQ + (b < P.pairsRem ? 1u : 0u));
 }
 
+// The producer's position in the token's weight stream: weight phase k (4 * layer + {QKV, WO, W1|W3, W2}, 4 * nLayers = logits)
+// and row offset r0 inside this CTA's tile of it. Phases in which this CTA owns no rows are skipped, exactly as the consumers'
+// main loops run zero fills there. One step of the cursor = one ring fill.
+struct FillCursor {
+    uint32_t k, r0;
+    uint32_t tileRows, rowBase, SR, rowQsBytes, rowScBytes;
+    const uint8_t *qs, *sc;
+
+    __device__ __forceinline__ bool valid(const MegaArgs &m) const { return k <= 4 * m.nLayers; }
+    // settle on the first phase >= k in which this CTA owns rows (r0 = 0)
+    __device__ __forceinline__ void enter(const MegaArgs &m) {
+        for (r0 = 0; k <= 4 * m.nLayers; k++) {
+            const uint32_t l = k >> 2, w = k & 3;
+            const MegaPhase &P = m.ph[l == m.nLayers ? (uint32_t)MP_LOGITS : w];
+            uint32_t pairBegin;
+            megaTile(P, pairBegin, tileRows);
+            if (tileRows == 0) continue;
+            rowBase = pairBegin * 2; SR = P.stageRows;
+            rowQsBytes = P.nblk * 16; rowScBytes = P.nblk * 2;
+            if (l == m.nLayers) { qs = m.wclsQs; sc = m.wclsSc; }
+            else {
+                const MegaLayer &L = m.layers[l];
+                qs = w == MP_QKV ? L.qkvQs : w == MP_WO ? L.woQs : w == MP_W13 ? L.w13Qs : L.w2Qs;
+                sc = w == MP_QKV ? L.qkvSc : w == MP_WO ? L.woSc : w == MP_W13 ? L.w13Sc : L.w2Sc;
+            }
+            return;
+        }
+    }
+    __device__ __forceinline__ void next(const MegaArgs &m) {
+        r0 += SR;
+        if (r0 >= tileRows) { k++; enter(m); }
+    }
+    // source ranges of the current fill
+    __device__ __forceinline__ uint32_t rows() const { return min(SR, tileRows - r0); }
+    __device__ __forceinline__ const uint8_t *qsSrc() const { return qs + (uint64_t)(rowBase + r0) * rowQsBytes; }
+    __device__ __forceinline__ const uint8_t *scSrc() const { return sc + (uint64_t)(rowBase + r0) * rowScBytes; }
+};
+
 // One GEMV phase on the consumer warps.
 // `in` / inEpoch: LL vector consumed by the prologue; `outW` / outEpoch: LL vector produced by the epilogue (EPI_RESIDUAL: the
 // residual stream itself, read-modify-written on the rows this CTA owns); `outF`: plain f32 output of the logits phase.
@@ -715,38 +753,55 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
             RingPos landed{0u, 0u};
             uint32_t nIssued = 0, nLanded = 0;
             const uint32_t maxInflight = m.maxInflight ? m.maxInflight : m.nStages;
-            auto stream = [&](const uint8_t *qs, const uint8_t *sc, const MegaPhase &P) {
-                const uint32_t rowQsBytes = P.nblk * 16, rowScBytes = P.nblk * 2;
-                uint32_t pairBegin, tileRows;
-                megaTile(P, pairBegin, tileRows);
-                const uint32_t rowBase = pairBegin * 2, SR = P.stageRows;
-                for (uint32_t r0 = 0; r0 < tileRows; r0 += SR) {
-                    const uint32_t st = pr.st;
-                    if (wrapped) mbarWait(&sm.emptyBar[st], pr.par ^ 1u);
-                    while (nIssued - nLanded >= maxInflight) {
-                        mbarWait(&sm.fullBar[landed.st], landed.par);
-                        landed.advance(m.nStages);
-                        nLanded++;
-                    }
-                    nIssued++;
-                    const uint32_t rows = min(SR, tileRows - r0);
-                    const uint32_t bq = rows * rowQsBytes, bs = rows * rowScBytes;
-                    uint8_t *dst = sm.ring + st * m.stageBytes;
-                    mbarExpectTx(&sm.fullBar[st], bq + bs);
-                    tmaBulkLoad(dst, qs + (uint64_t)(rowBase + r0) * rowQsBytes, bq, &sm.fullBar[st], policy);
-                    tmaBulkLoad(dst + SR * rowQsBytes, sc + (uint64_t)(rowBase + r0) * rowScBytes, bs, &sm.fullBar[st], policy);
-                    pr.advance(m.nStages);
-                    if (pr.st == 0) wrapped = true;
+            auto waitLanded = [&]() {
+                while (nIssued - nLanded >= maxInflight) {
+                    mbarWait(&sm.fullBar[landed.st], landed.par);
+                    landed.advance(m.nStages);
+                    nLanded++;
                 }
             };
-            for (uint32_t l = 0; l < m.nLayers; l++) {
-                const MegaLayer &L = m.layers[l];
-                stream(L.qkvQs, L.qkvSc, m.ph[MP_QKV]);
-                stream(L.woQs, L.woSc, m.ph[MP_WO]);
-                stream(L.w13Qs, L.w13Sc, m.ph[MP_W13]);
-                stream(L.w2Qs, L.w2Sc, m.ph[MP_W2]);
+            // All-CTA tracing: per weight phase, the ns spent waiting for a free stage (ring full) and on the in-flight cap.
+            uint64_t *prodTrace = (m.trace && m.traceProdSlot && blockIdx.x < m.traceCtas)
+                                      ? m.trace + (size_t)blockIdx.x * m.traceStride + m.traceProdSlot : nullptr;
+            uint64_t fullNs = 0, capNs = 0;
+            FillCursor cur;
+            cur.k = 0;
+            cur.enter(m);
+            if (prodTrace)   // leading phases without rows here
+                for (uint32_t kk = 0; kk < cur.k && kk <= 4 * m.nLayers; kk++) prodTrace[2 * kk] = prodTrace[2 * kk + 1] = 0u;
+            while (cur.valid(m)) {
+                const uint32_t st = pr.st;
+                if (prodTrace) {
+                    const uint64_t t0 = globalTimerNs();
+                    if (wrapped) mbarWait(&sm.emptyBar[st], pr.par ^ 1u);
+                    const uint64_t t1 = globalTimerNs();
+                    waitLanded();
+                    const uint64_t t2 = globalTimerNs();
+                    fullNs += t1 - t0;
+                    capNs += t2 - t1;
+                } else {
+                    if (wrapped) mbarWait(&sm.emptyBar[st], pr.par ^ 1u);
+                    waitLanded();
+                }
+                nIssued++;
+                const uint32_t rows = cur.rows();
+                const uint32_t bq = rows * cur.rowQsBytes, bs = rows * cur.rowScBytes;
+                uint8_t *dst = sm.ring + st * m.stageBytes;
+                mbarExpectTx(&sm.fullBar[st], bq + bs);
+                tmaBulkLoad(dst, cur.qsSrc(), bq, &sm.fullBar[st], policy);
+                tmaBulkLoad(dst + cur.SR * cur.rowQsBytes, cur.scSrc(), bs, &sm.fullBar[st], policy);
+                pr.advance(m.nStages);
+                if (pr.st == 0) wrapped = true;
+                const uint32_t k = cur.k;
+                cur.next(m);
+                if (prodTrace && cur.k != k) {   // last fill of phase k issued; phases skipped on the way (no rows here) waited 0 ns
+                    for (uint32_t kk = k; kk < cur.k && kk <= 4 * m.nLayers; kk++) {
+                        prodTrace[2 * kk] = kk == k ? fullNs : 0u;
+                        prodTrace[2 * kk + 1] = kk == k ? capNs : 0u;
+                    }
+                    fullNs = capNs = 0;
+                }
             }
-            stream(m.wclsQs, m.wclsSc, m.ph[MP_LOGITS]);
         }
         return;
     }

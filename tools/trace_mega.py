@@ -8,6 +8,7 @@ from distributed_llama_b200.api import InferenceSession
 
 args = [a for a in sys.argv[1:] if not a.startswith("--")]
 ALL = "--all" in sys.argv          # every CTA records its stamps: barrier skew analysis
+SAVE = next((a.split("=", 1)[1] for a in sys.argv[1:] if a.startswith("--save=")), None)   # --all: also write the stamps (us) as .npy
 model = args[0] if args else "llama-3.1-8b"
 comm = None
 rank = int(os.environ.get("RANK", "0"))
@@ -75,7 +76,24 @@ if ALL:
         dur = np.stack([T[:, i + 1] - T[:, i] for i in idx], 1).mean(1)
         order = np.argsort(dur)
         print(f"  {ph}: per-CTA mean {dur.mean():.2f} us, min {dur.min():.2f} (cta {order[0]}), max {dur.max():.2f} (cta {order[-1]}), p90 {np.percentile(dur, 90):.2f}")
-    np.save(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out", "trace_all.npy"), T)
+    # producer stalls (csrc/cuda/kernels.h megaTraceProdSlot): per weight phase k = 4 * layer + {QKV, WO, W1|W3, W2} (k = 4L: logits),
+    # ns the producer waited for a free ring stage ("ring full") and on the in-flight cap
+    raw = eng.trace_buf.cpu().numpy().reshape(-1)[: eng.num_sms * eng.trace_stride].reshape(eng.num_sms, eng.trace_stride)
+    p0 = (18 * L + 5 + 7) // 8 * 8
+    P = raw[:, p0: p0 + 2 * (4 * L + 1)].astype(np.float64).reshape(eng.num_sms, 4 * L + 1, 2) / 1e3   # us
+    full, cap = P[:, :, 0], P[:, :, 1]
+    print(f"producer stalls (us per CTA, mean over {eng.num_sms} CTAs; per phase: mean over layers):")
+    print(f"{'phase':8s} {'ring full':>10s} {'inflight cap':>13s}")
+    for j, nm in enumerate(("qkv", "wo", "w13", "w2")):
+        print(f"{nm:8s} {full[:, j:4 * L:4].mean():10.2f} {cap[:, j:4 * L:4].mean():13.2f}")
+    print(f"{'logits':8s} {full[:, 4 * L].mean():10.2f} {cap[:, 4 * L].mean():13.2f}")
+    fl = full[:, :4 * L].reshape(eng.num_sms, L, 4).sum(2).mean(0)
+    cl_ = cap[:, :4 * L].reshape(eng.num_sms, L, 4).sum(2).mean(0)
+    print(f"per layer total: ring full {fl.mean():.2f} us (min {fl.min():.2f}, max {fl.max():.2f}), "
+          f"inflight cap {cl_.mean():.2f} us (min {cl_.min():.2f}, max {cl_.max():.2f})")
+    print(f"per token: ring full {full.sum(1).mean():.1f} us, inflight cap {cap.sum(1).mean():.1f} us; step {T.max():.1f} us")
+    if SAVE:
+        np.save(SAVE, T)
     sys.exit(0)
 st = eng.trace_buf.cpu().numpy().reshape(-1)
 st = st[st != 0].astype(np.float64)
