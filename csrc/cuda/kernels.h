@@ -205,7 +205,7 @@ struct MegaArgs {
 
 // Trace row of one CTA of the persistent kernel: 18 * nLayers + 5 consumer phase stamps, then (from this slot on, 8-aligned) two
 // producer counters per weight phase k = 4 * layer + {QKV, WO, W1|W3, W2}, k = 4 * nLayers for the logits: at 2k the ns the
-// producer waited for a free ring stage, at 2k + 1 the ns it waited on the in-flight cap.
+// producer waited for a free ring stage, at 2k + 1 the ns it waited on the in-flight cap. A layer's K/V fills count towards its QKV phase.
 inline uint32_t megaTraceProdSlot(uint32_t nLayers) { return (18 * nLayers + 5 + 7) / 8 * 8; }
 inline uint32_t megaTraceRowSlots(uint32_t nLayers) { return megaTraceProdSlot(nLayers) + 2 * (4 * nLayers + 1); }
 

@@ -3,10 +3,12 @@
 // The multi-kernel decode path pays a grid-completion latency at each of its 161 kernel boundaries and restarts the
 // weight stream at every launch. Here one CTA per SM stays resident for the whole token:
 //   * warp 16 (producer) walks the list of all weight matrices of the token and streams this CTA's row tile of each one
-//     through a single shared-memory ring with cp.async.bulk + mbarriers. It never synchronises with the phases — only
-//     ring space limits it — so the HBM stream runs continuously across phase boundaries and layers.
-//   * warps 0-15 (consumers) execute the phases embedding -> per layer [QKV GEMV | attention | WO GEMV + residual |
-//     W1|W3 GEMV + SwiGLU | W2 GEMV + residual] -> logits GEMV + arg-max, separated by software grid barriers.
+//     through a single shared-memory ring with cp.async.bulk + mbarriers; between a layer's QKV and WO fills it streams the
+//     cached K/V rows of this CTA's attention items the same way. It never synchronises with the phases — only ring space
+//     limits it — so the HBM stream runs continuously across phase boundaries and layers.
+//   * warps 0-15 (consumers) execute the phases embedding -> per layer [QKV GEMV, attention | WO GEMV + residual |
+//     W1|W3 GEMV + SwiGLU | W2 GEMV + residual] -> logits GEMV + arg-max, separated by software grid barriers (none between
+//     QKV and attention: attention polls the q|k|v words of its own heads).
 //   * Every vector that crosses a phase boundary (x, q|k|v, z, h) travels as LL words: 8-byte {f32 payload, epoch} stores that
 //     L2 delivers atomically. The barrier therefore needs NO memory fence (a relaxed arrive + relaxed poll): it only orders
 //     control flow, and a consumer that finds a word with a stale epoch simply re-reads it. With the weight stream running a
@@ -37,7 +39,7 @@ static uint32_t megaStageRows(uint32_t n, uint32_t stageBytes) {
 struct MegaSmem {
     uint8_t *ring;
     uint4 *planeA, *planeB;
-    float *dxs, *dx8, *partial, *red, *rope;
+    float *dxs, *dx8, *partial, *red, *rope, *qHand;
     uint64_t *fullBar, *emptyBar;
 };
 
@@ -181,6 +183,31 @@ struct FillCursor {
     __device__ __forceinline__ uint32_t rows() const { return min(SR, tileRows - r0); }
     __device__ __forceinline__ const uint8_t *qsSrc() const { return qs + (uint64_t)(rowBase + r0) * rowQsBytes; }
     __device__ __forceinline__ const uint8_t *scSrc() const { return sc + (uint64_t)(rowBase + r0) * rowScBytes; }
+};
+
+// Attention work items: (head, split) pairs dealt round-robin to the CTAs (item blockIdx.x, + gridDim.x, ...). The producer derives
+// the K/V fills of this CTA from the same rule as the consumers, so both must come from here.
+constexpr uint32_t kKvChunk = kConsumerWarps * 4;   // cached K/V rows per ring fill: warp w takes rows 4w..4w+3
+constexpr uint32_t kKvInflight = 2;                  // producer pacing of the K/V fills (the weight fills: MegaArgs::maxInflight)
+// Effective split count: grows with the position (read on the device, so a replayed graph follows it), capped at nSplits.
+__device__ __forceinline__ uint32_t attnSplits(const MegaArgs &m, uint32_t nPos) {
+    uint32_t eff = (nPos + 255) / 256;
+    if (eff > m.nSplits) eff = m.nSplits;
+    if (eff < 1) eff = 1;
+    return eff;
+}
+struct AttnItem {
+    uint32_t h, split, kvh, begin, end, cachedEnd;   // cached rows [begin, cachedEnd) come through the ring
+    bool ownsNew;                                     // the split that ends at the new position also takes this token's k/v
+    __device__ __forceinline__ AttnItem(const MegaArgs &m, uint32_t item, uint32_t nPos, uint32_t eff) {
+        h = item / eff; split = item - h * eff;
+        kvh = h / (m.nHeads / m.nKvHeads);
+        const uint32_t chunk = (nPos + eff - 1) / eff;
+        begin = split * chunk;
+        end = min(begin + chunk, nPos);
+        ownsNew = end == nPos;
+        cachedEnd = ownsNew ? end - 1 : end;
+    }
 };
 
 // One GEMV phase on the consumer warps.
@@ -492,16 +519,18 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
     }
 }
 
-// Attention phase: work items (head, split) are dealt round-robin to the CTAs; the 16 consumer warps of a CTA share the
-// positions of one item. Same math as attnFusedKernel (decode_ops.cu).
+// Attention phase: work items (head, split) are dealt round-robin to the CTAs (AttnItem); the 16 consumer warps of a CTA share
+// the positions of one item. Same math as attnFusedKernel (decode_ops.cu). The cached K/V rows of an item arrive through the ring,
+// kKvChunk rows per fill (the producer issues them between this layer's QKV and WO fills), warp w takes rows 4w..4w+3 of each.
+// The q|k|v words are polled by warp 0 alone, and q is handed to the other warps through shared memory: this phase follows the
+// QKV epilogue without a grid barrier, so the poll covers the other CTAs' arrival skew.
 template <int HD>
-__device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaLayer &L, int p, int tid, uint32_t inEpoch, uint32_t outEpoch) {
+__device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaLayer &L, int p, int tid, uint32_t inEpoch, uint32_t outEpoch,
+                             RingPos &ring) {
     constexpr int DPL = HD / 32;
     const int lane = tid & 31, warp = tid >> 5;
     const uint32_t nPos = (uint32_t)p + 1;
-    uint32_t eff = (nPos + 255) / 256;
-    if (eff > m.nSplits) eff = m.nSplits;
-    if (eff < 1) eff = 1;
+    const uint32_t eff = attnSplits(m, nPos);
     const uint32_t kvMul = m.nHeads / m.nKvHeads;
     const uint32_t qDim = m.nHeads * HD, kvDim = m.nKvHeads * HD;
     float *sAcc = sm.partial;                 // [16][HD]
@@ -529,30 +558,14 @@ __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaL
         }
     };
     for (uint32_t item = blockIdx.x; item < m.nHeads * eff; item += gridDim.x) {
-        const uint32_t h = item / eff, split = item - h * eff;
-        const uint32_t kvh = h / kvMul;
-        const uint32_t chunk = (nPos + eff - 1) / eff;
-        const uint32_t begin = split * chunk;
-        const uint32_t end = min(begin + chunk, nPos);
-        const bool ownsNew = end == nPos;
-        const uint32_t cachedEnd = ownsNew ? end - 1 : end;
+        const AttnItem it(m, item, nPos, eff);
+        const uint32_t h = it.h, split = it.split, kvh = it.kvh, cachedEnd = it.cachedEnd;
+        const bool ownsNew = it.ownsNew;
         __nv_bfloat16 *kHead = L.kCache + (size_t)kvh * m.seqLen * HD;
         __nv_bfloat16 *vHead = L.vCache + (size_t)kvh * m.seqLen * HD;
-        const __nv_bfloat16 *kBase = kHead + lane * DPL;
-        const __nv_bfloat16 *vBase = vHead + lane * DPL;
         constexpr int UN = 4;
+        static_assert(kConsumerWarps * UN == kKvChunk, "one ring fill of K/V rows = one batch of the 16 warps");
         using RawT = typename std::conditional<DPL == 4, uint2, uint32_t>::type;   // DPL bf16 values of one cache row
-        RawT kRaw[UN], vRaw[UN];
-        auto loadBatch = [&](uint32_t s0) {
-#pragma unroll
-            for (int u = 0; u < UN; u++) {
-                const uint32_t s = s0 + u;
-                if (s < cachedEnd) {
-                    kRaw[u] = *reinterpret_cast<const RawT *>(kBase + (size_t)s * HD);
-                    vRaw[u] = *reinterpret_cast<const RawT *>(vBase + (size_t)s * HD);
-                }
-            }
-        };
         auto unpack = [&](const RawT &r, float (&o)[DPL]) {
             if constexpr (DPL == 4) {
                 const float2 a0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&r.x));
@@ -563,15 +576,12 @@ __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaL
                 o[0] = a0.x; o[1] = a0.y;
             }
         };
-        // Everything that does not depend on this layer's q is requested first: the first batch of cached K/V rows (and, on the warp
-        // that owns the new position, the raw k/v words) are in flight while q is polled — one L2 round trip instead of three.
-        uint32_t s0 = begin + warp * UN;
-        loadBatch(s0);
+        // On the item that owns the new position, warp 0 requests the raw k/v words before it polls q: one L2 round trip, not two.
         const bool newRow = ownsNew && warp == 0;
         const uint2 *ksrc = m.qkvW + qDim + (size_t)kvh * HD + lane * DPL;
         const uint2 *vsrc = m.qkvW + qDim + kvDim + (size_t)kvh * HD + lane * DPL;
         float q[DPL], kn[DPL], vn[DPL];
-        {
+        if (warp == 0) {
             const uint2 *src = m.qkvW + (size_t)h * HD + lane * DPL;
             if constexpr (DPL == 4) {
                 uint4 ka0, ka1, va0, va1;
@@ -597,6 +607,13 @@ __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaL
                     for (int i = 0; i < DPL; i++) { kn[i] = ldWwait(ksrc + i, inEpoch, m.abortFlag); vn[i] = ldWwait(vsrc + i, inEpoch, m.abortFlag); }
                 }
             }
+#pragma unroll
+            for (int i = 0; i < DPL; i++) sm.qHand[lane * DPL + i] = q[i];
+        }
+        consumerBarrier();   // (the other warps read the previous item's q before that item's merge barriers)
+        if (warp != 0) {
+#pragma unroll
+            for (int i = 0; i < DPL; i++) q[i] = sm.qHand[lane * DPL + i];
         }
         normRope(q, L.qNorm);
         const float scale = rsqrtf((float)HD);
@@ -630,18 +647,27 @@ __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaL
 #pragma unroll
             for (int i = 0; i < DPL; i++) acc[i] = vn[i];
         }
-        for (; s0 < cachedEnd; s0 += kConsumerWarps * UN) {
+        // one ring fill per kKvChunk cached rows: K rows at the start of the stage, V rows kKvChunk rows further
+        for (uint32_t c0 = it.begin; c0 < cachedEnd; c0 += kKvChunk) {
+            const uint32_t st = ring.st;
+            const __nv_bfloat16 *sK = reinterpret_cast<const __nv_bfloat16 *>(sm.ring + st * m.stageBytes) + warp * UN * HD + lane * DPL;
+            const __nv_bfloat16 *sV = sK + kKvChunk * HD;
+            const uint32_t cur = c0 + warp * UN;
+            mbarWait(&sm.fullBar[st], ring.par);
             float kf[UN][DPL], vf[UN][DPL];
 #pragma unroll
             for (int u = 0; u < UN; u++) {
-                if (s0 + u < cachedEnd) { unpack(kRaw[u], kf[u]); unpack(vRaw[u], vf[u]); }
-                else {
+                if (cur + u < cachedEnd) {
+                    unpack(*reinterpret_cast<const RawT *>(sK + u * HD), kf[u]);
+                    unpack(*reinterpret_cast<const RawT *>(sV + u * HD), vf[u]);
+                } else {
 #pragma unroll
                     for (int i = 0; i < DPL; i++) { kf[u][i] = 0.f; vf[u][i] = 0.f; }
                 }
             }
-            const uint32_t cur = s0;
-            if (s0 + kConsumerWarps * UN < cachedEnd) loadBatch(s0 + kConsumerWarps * UN);   // next batch in flight during the math
+            __syncwarp();
+            if (lane == 0) mbarArrive(&sm.emptyBar[st]);   // the rows are in registers: release the stage before the math
+            ring.advance(m.nStages);
             float sc[UN];
 #pragma unroll
             for (int u = 0; u < UN; u++) {
@@ -727,7 +753,8 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
     sm.partial = sm.dx8 + m.planeBlocks;
     sm.red = sm.partial + m.partialFloats;
     sm.rope = sm.red + 32;                                              // [128] rotary (cos, sin) pairs of this token's position
-    sm.fullBar = reinterpret_cast<uint64_t *>(sm.rope + 128);
+    sm.qHand = sm.rope + 128;                                           // [128] attention: q of the item, polled by warp 0
+    sm.fullBar = reinterpret_cast<uint64_t *>(sm.qHand + 128);
     sm.emptyBar = sm.fullBar + kMaxStages;
 
     if (tid == 0) {
@@ -737,8 +764,11 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
+    // The position: read by every thread before the CTA's first barrier, since CTA 0 advances it at the end of the launch.
+    int p = m.pos[0];
+    if (p < 0) p = 0;
+    if ((uint32_t)p >= m.seqLen) p = m.seqLen - 1;
     __syncthreads();
-    const uint32_t qDim = m.nHeads * m.headDim, kvDim = m.nKvHeads * m.headDim, qkvDim = qDim + 2 * kvDim;
 
     if (warp == kConsumerWarps) {
         // =============================== producer: every weight matrix of the token, back to back ===============================
@@ -753,55 +783,89 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
             RingPos landed{0u, 0u};
             uint32_t nIssued = 0, nLanded = 0;
             const uint32_t maxInflight = m.maxInflight ? m.maxInflight : m.nStages;
-            auto waitLanded = [&]() {
-                while (nIssued - nLanded >= maxInflight) {
+            // K/V fills may have kKvInflight fills in flight (DESIGN.md §7): they are requested while the consumers still work on
+            // QKV / W2, and their rows are cache reads of the kvMul q heads of a group rather than part of the weight stream.
+            const uint32_t kvInflight = min(max(maxInflight, kKvInflight), m.nStages);
+            auto waitLanded = [&](uint32_t cap) {
+                while (nIssued - nLanded >= cap) {
                     mbarWait(&sm.fullBar[landed.st], landed.par);
                     landed.advance(m.nStages);
                     nLanded++;
                 }
             };
-            // All-CTA tracing: per weight phase, the ns spent waiting for a free stage (ring full) and on the in-flight cap.
+            // All-CTA tracing: per weight phase, the ns spent waiting for a free stage (ring full) and on the in-flight cap, summed in
+            // registers and stored once the fills move on to a later phase (phases without fills here store 0). The K/V fills of a
+            // layer count towards its QKV phase.
             uint64_t *prodTrace = (m.trace && m.traceProdSlot && blockIdx.x < m.traceCtas)
                                       ? m.trace + (size_t)blockIdx.x * m.traceStride + m.traceProdSlot : nullptr;
             uint64_t fullNs = 0, capNs = 0;
-            FillCursor cur;
-            cur.k = 0;
-            cur.enter(m);
-            if (prodTrace)   // leading phases without rows here
-                for (uint32_t kk = 0; kk < cur.k && kk <= 4 * m.nLayers; kk++) prodTrace[2 * kk] = prodTrace[2 * kk + 1] = 0u;
-            while (cur.valid(m)) {
+            uint32_t traceK = 0;
+            auto traceTo = [&](uint32_t k) {
+                for (; traceK < k; traceK++) {
+                    prodTrace[2 * traceK] = fullNs;
+                    prodTrace[2 * traceK + 1] = capNs;
+                    fullNs = capNs = 0;
+                }
+            };
+            // one ring fill: wait for a free stage and for the in-flight count to drop under `cap`, then `copy(stage, full barrier)`
+            auto fill = [&](uint32_t phaseK, uint32_t cap, uint32_t bytes, auto &&copy) {
                 const uint32_t st = pr.st;
                 if (prodTrace) {
+                    traceTo(phaseK);
                     const uint64_t t0 = globalTimerNs();
                     if (wrapped) mbarWait(&sm.emptyBar[st], pr.par ^ 1u);
                     const uint64_t t1 = globalTimerNs();
-                    waitLanded();
+                    waitLanded(cap);
                     const uint64_t t2 = globalTimerNs();
                     fullNs += t1 - t0;
                     capNs += t2 - t1;
                 } else {
                     if (wrapped) mbarWait(&sm.emptyBar[st], pr.par ^ 1u);
-                    waitLanded();
+                    waitLanded(cap);
                 }
                 nIssued++;
-                const uint32_t rows = cur.rows();
-                const uint32_t bq = rows * cur.rowQsBytes, bs = rows * cur.rowScBytes;
-                uint8_t *dst = sm.ring + st * m.stageBytes;
-                mbarExpectTx(&sm.fullBar[st], bq + bs);
-                tmaBulkLoad(dst, cur.qsSrc(), bq, &sm.fullBar[st], policy);
-                tmaBulkLoad(dst + cur.SR * cur.rowQsBytes, cur.scSrc(), bs, &sm.fullBar[st], policy);
+                mbarExpectTx(&sm.fullBar[st], bytes);
+                copy(sm.ring + st * m.stageBytes, &sm.fullBar[st]);
                 pr.advance(m.nStages);
                 if (pr.st == 0) wrapped = true;
-                const uint32_t k = cur.k;
-                cur.next(m);
-                if (prodTrace && cur.k != k) {   // last fill of phase k issued; phases skipped on the way (no rows here) waited 0 ns
-                    for (uint32_t kk = k; kk < cur.k && kk <= 4 * m.nLayers; kk++) {
-                        prodTrace[2 * kk] = kk == k ? fullNs : 0u;
-                        prodTrace[2 * kk + 1] = kk == k ? capNs : 0u;
+            };
+            // K/V fills of layer l: this CTA's attention items (AttnItem, the consumers' rule), one fill per kKvChunk cached rows,
+            // each fill = the K rows and the V rows (both contiguous in the head-major cache). Rows written by earlier launches only.
+            const uint64_t kvPolicy = policyEvictNormal();   // a K/V row is read by the kvMul q heads of its group
+            const uint32_t nPos = (uint32_t)p + 1, eff = attnSplits(m, nPos);
+            auto kvFills = [&](uint32_t l) {
+                const MegaLayer &L = m.layers[l];
+                for (uint32_t item = blockIdx.x; item < m.nHeads * eff; item += gridDim.x) {
+                    const AttnItem it(m, item, nPos, eff);
+                    const __nv_bfloat16 *kHead = L.kCache + (size_t)it.kvh * m.seqLen * HD;
+                    const __nv_bfloat16 *vHead = L.vCache + (size_t)it.kvh * m.seqLen * HD;
+                    for (uint32_t c0 = it.begin; c0 < it.cachedEnd; c0 += kKvChunk) {
+                        const uint32_t bytes = min(kKvChunk, it.cachedEnd - c0) * HD * 2;
+                        fill(4 * l + MP_QKV, kvInflight, 2 * bytes, [&](uint8_t *dst, uint64_t *bar) {
+                            tmaBulkLoad(dst, kHead + (size_t)c0 * HD, bytes, bar, kvPolicy);
+                            tmaBulkLoad(dst + kKvChunk * HD * 2, vHead + (size_t)c0 * HD, bytes, bar, kvPolicy);
+                        });
                     }
-                    fullNs = capNs = 0;
                 }
+            };
+            FillCursor cur;
+            cur.k = 0;
+            cur.enter(m);
+            uint32_t kvLayer = 0;   // next layer whose K/V fills are due
+            for (;;) {
+                const bool more = cur.valid(m);
+                // the consumers take a layer's K/V fills after its QKV fills and before any later phase's
+                while (kvLayer < m.nLayers && (!more || cur.k > 4 * kvLayer)) kvFills(kvLayer++);
+                if (!more) break;
+                const uint32_t rows = cur.rows();
+                const uint32_t bq = rows * cur.rowQsBytes, bs = rows * cur.rowScBytes;
+                fill(cur.k, maxInflight, bq + bs, [&](uint8_t *dst, uint64_t *bar) {
+                    tmaBulkLoad(dst, cur.qsSrc(), bq, bar, policy);
+                    tmaBulkLoad(dst + cur.SR * cur.rowQsBytes, cur.scSrc(), bs, bar, policy);
+                });
+                cur.next(m);
             }
+            if (prodTrace) traceTo(4 * m.nLayers + 1);
         }
         return;
     }
@@ -815,9 +879,6 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
     // Epochs of the LL vectors: launch sequence number (device resident, bumped by CTA 0 at the end of every launch) x 1024 +
     // phase index. Phase indices: 0 = embedding; layer l: 1+5l QKV, 2+5l attention, 3+5l WO, 4+5l W1|W3, 5+5l W2.
     const uint32_t seqBase = __ldcg(m.launchSeq) << 10;
-    int p = m.pos[0];
-    if (p < 0) p = 0;
-    if ((uint32_t)p >= m.seqLen) p = m.seqLen - 1;
     if (tid < HD) sm.rope[tid] = m.rope[(size_t)p * HD + tid];
     // embedding: every CTA writes the rows of the residual stream it owns in the WO / W2 phases (same thread -> same rows, so
     // the residual read-modify-write never depends on another CTA's store)
@@ -846,9 +907,9 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
         stamp();
         megaGemv<PRO_RMSNORM_, EPI_STORE_>(m, sm, m.ph[MP_QKV], xA, e0, L.norm0, m.qkvW, e0 + 1, nullptr, 0, ring, tid, slot);
         stamp();
-        llBarrier();
+        // no barrier: attention polls the q|k|v words it needs, CTAs without an attention item go on to the next barrier
         stamp();
-        megaAttention<HD>(m, sm, L, p, tid, e0 + 1, e0 + 2);
+        megaAttention<HD>(m, sm, L, p, tid, e0 + 1, e0 + 2, ring);
         stamp();
         llBarrier();
         stamp();
@@ -898,12 +959,13 @@ int launchMegaDecode(MegaArgs m, int numSms, cudaStream_t stream) {
     }
     m.partialFloats = (partial + 3) / 4 * 4;
     m.planeBlocks = maxN / 32;
-    const size_t fixedBytes = (size_t)m.planeBlocks * (16 + 16 + 4 + 4) + (size_t)m.partialFloats * 4 + 32 * 4 + 128 * 4 + 2 * kMaxStages * 8 + 256;
+    const size_t fixedBytes = (size_t)m.planeBlocks * (16 + 16 + 4 + 4) + (size_t)m.partialFloats * 4 + 32 * 4 + 2 * 128 * 4 + 2 * kMaxStages * 8 + 256;
     const size_t budget = 226 * 1024;
     // stage must hold >= 4 rows of the widest matrix
     const uint32_t maxRowBytes = (maxN / 32) * 18;
     uint32_t stageBytes = 36 * 1024;
     if (maxRowBytes * 4 > stageBytes) stageBytes = (maxRowBytes * 4 + 127) / 128 * 128;
+    if (2 * kKvChunk * m.headDim * 2 > stageBytes) return 1;   // a K/V fill: kKvChunk bf16 rows of K and of V
     if (fixedBytes + 2 * (size_t)stageBytes > budget) return 1;
     uint32_t stages = (uint32_t)((budget - fixedBytes) / stageBytes);
     if (stages > (uint32_t)kMaxStages) stages = kMaxStages;

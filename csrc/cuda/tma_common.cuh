@@ -38,6 +38,11 @@ __device__ __forceinline__ uint64_t policyEvictFirst() {
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
     return p;
 }
+__device__ __forceinline__ uint64_t policyEvictNormal() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
 __device__ __forceinline__ void tmaBulkLoad(void *dst, const void *src, uint32_t bytes, uint64_t *bar, uint64_t policy) {
     asm volatile(
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(smemAddr(dst)),

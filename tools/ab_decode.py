@@ -4,9 +4,12 @@ round, checks that every run produced the same greedy tokens and prints median /
     python tools/ab_decode.py                                   # DL_MEGA_INFLIGHT=2 (the previous pacing) vs the default
     python tools/ab_decode.py --rounds 5 --variant DL_MEGA_INFLIGHT=2 --variant DL_MEGA_INFLIGHT=3 --variant ''
     python tools/ab_decode.py --variant 'DL_MEGA_INFLIGHT=2 DL_MEGA_CTAS=128' --variant ''
+    python tools/ab_decode.py --variant @ab_checkouts/parent --variant ''      # another checkout of the code vs this tree
 
 A variant is a space-separated list of NAME=VALUE settings; '' is the default environment. Every variant variable is removed from
-the environment of the runs that do not set it.
+the environment of the runs that do not set it. An item @DIR runs bench.py of the checkout at DIR (relative to this tree, e.g. a
+`git archive` of another commit unpacked under the git-ignored ab_checkouts/) instead of this tree's; every checkout builds its
+native libraries in place before the first round.
 """
 import argparse
 import io
@@ -23,12 +26,16 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def parse_variant(spec: str) -> dict:
-    env = {}
+def parse_variant(spec: str):
+    """-> (environment settings, checkout root)"""
+    env, root = {}, ROOT
     for item in spec.split():
+        if item.startswith("@"):
+            root = os.path.join(ROOT, item[1:])
+            continue
         k, _, v = item.partition("=")
         env[k] = v
-    return env
+    return env, root
 
 
 def gpu_info() -> str:
@@ -48,22 +55,29 @@ def main():
     ap.add_argument("--json", metavar="FILE", default=None, help="also write every run's result line to FILE")
     args = ap.parse_args()
     specs = args.variant if args.variant else ["DL_MEGA_INFLIGHT=2", ""]
-    variants = [parse_variant(s) for s in specs]
+    parsed = [parse_variant(s) for s in specs]
+    variants = [env for env, _ in parsed]
+    roots = [root for _, root in parsed]
     names = [s if s else "(default)" for s in specs]
     knobs = set().union(*variants)
     print(gpu_info(), flush=True)
+    for root in dict.fromkeys(roots):
+        r = subprocess.run([sys.executable, os.path.join(root, "__graft_entry__.py")], capture_output=True, text=True, cwd=root)
+        if r.returncode != 0:
+            sys.stderr.write(r.stdout[-3000:] + r.stderr[-3000:])
+            raise SystemExit(f"build failed in {root}")
 
     results = {n: [] for n in names}
     tokens = []   # (variant, round, tokens.npy bytes)
     with tempfile.TemporaryDirectory() as tmp:
         for rnd in range(args.rounds):
-            for name, var in zip(names, variants):
+            for name, var, root in zip(names, variants, roots):
                 env = {k: v for k, v in os.environ.items() if k not in knobs}
                 env.update(var)
                 out = os.path.join(tmp, f"r{rnd}_{len(tokens)}")
-                cmd = [sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", str(args.steps), "--warmup",
+                cmd = [sys.executable, os.path.join(root, "bench.py"), "--gpus", "1", "--steps", str(args.steps), "--warmup",
                        str(args.warmup), "--dump-outputs", out]
-                r = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=ROOT)
+                r = subprocess.run(cmd, env=env, capture_output=True, text=True, cwd=root)
                 lines = [ln for ln in r.stdout.splitlines() if ln.startswith("{")]
                 if r.returncode != 0 or not lines:
                     sys.stderr.write(r.stderr[-3000:])

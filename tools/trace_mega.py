@@ -1,4 +1,9 @@
-"""Phase timeline of the persistent decode kernel (one %globaltimer stamp at every phase start on CTA 0)."""
+"""Phase timeline of the persistent decode kernel (one %globaltimer stamp at every phase start on CTA 0).
+
+    python tools/trace_mega.py [model] [--all] [--pos=N] [--save=FILE]
+
+--pos=N traces the step at position N (default 63, the position after the 64-token prompt; the context is sized to fit it).
+"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -9,6 +14,7 @@ from distributed_llama_b200.api import InferenceSession
 args = [a for a in sys.argv[1:] if not a.startswith("--")]
 ALL = "--all" in sys.argv          # every CTA records its stamps: barrier skew analysis
 SAVE = next((a.split("=", 1)[1] for a in sys.argv[1:] if a.startswith("--save=")), None)   # --all: also write the stamps (us) as .npy
+POS = int(next((a.split("=", 1)[1] for a in sys.argv[1:] if a.startswith("--pos=")), 63))
 model = args[0] if args else "llama-3.1-8b"
 comm = None
 rank = int(os.environ.get("RANK", "0"))
@@ -22,16 +28,16 @@ if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         ensure_model(model)
     dist.barrier()
 m, t = ensure_model(model)
-sess = InferenceSession(m, t, max_seq_len=2048, comm=comm)
+sess = InferenceSession(m, t, max_seq_len=max(2048, POS + 64), comm=comm)
 eng = sess.engine
 eng.enable_trace(4096, all_ctas=ALL)
 eng.enable_mega()
 prompt = [(7 * i + 3) % 1000 + 1 for i in range(64)]
 eng.prefill(prompt[:-1], 0, want_logits=False)
-eng.decode_greedy(prompt[-1], 63, 8)
+eng.decode_greedy(prompt[-1], POS, 8)
 torch.cuda.synchronize()
 eng.trace_buf.zero_()
-eng.decode_greedy(prompt[-1], 63, 1)
+eng.decode_greedy(prompt[-1], POS, 1)
 torch.cuda.synchronize()
 if rank != 0:
     sys.exit(0)
@@ -43,7 +49,7 @@ if ALL:
     nst = len(names) + 1
     T = eng.trace_buf.cpu().numpy().reshape(-1)[: eng.num_sms * eng.trace_stride].reshape(eng.num_sms, eng.trace_stride)[:, :nst].astype(np.float64)
     T = (T - T.min()) / 1e3          # us, common origin
-    print(f"all-CTA trace: {eng.num_sms} CTAs x {nst} stamps; step = {T.max():.1f} us")
+    print(f"all-CTA trace at position {POS}: {eng.num_sms} CTAs x {nst} stamps; step = {T.max():.1f} us")
     # interval i spans stamps i..i+1; for a barrier interval the start stamp is the CTA's arrival and the end stamp its release
     stats = {}
     late = {}
@@ -77,7 +83,7 @@ if ALL:
         order = np.argsort(dur)
         print(f"  {ph}: per-CTA mean {dur.mean():.2f} us, min {dur.min():.2f} (cta {order[0]}), max {dur.max():.2f} (cta {order[-1]}), p90 {np.percentile(dur, 90):.2f}")
     # producer stalls (csrc/cuda/kernels.h megaTraceProdSlot): per weight phase k = 4 * layer + {QKV, WO, W1|W3, W2} (k = 4L: logits),
-    # ns the producer waited for a free ring stage ("ring full") and on the in-flight cap
+    # ns the producer waited for a free ring stage ("ring full") and on the in-flight cap; the qkv row includes the layer's K/V fills
     raw = eng.trace_buf.cpu().numpy().reshape(-1)[: eng.num_sms * eng.trace_stride].reshape(eng.num_sms, eng.trace_stride)
     p0 = (18 * L + 5 + 7) // 8 * 8
     P = raw[:, p0: p0 + 2 * (4 * L + 1)].astype(np.float64).reshape(eng.num_sms, 4 * L + 1, 2) / 1e3   # us
