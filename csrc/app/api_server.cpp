@@ -135,12 +135,69 @@ uint32_t NaiveCache::resolveDeltaPrompt(std::vector<ChatItem> &messages) {
     return 0;
 }
 
-std::string chunkJson(const std::string *delta, bool stop) {
+std::string chunkJson(const std::string *delta, bool stop, uint32_t index) {
     std::string s = "{\"id\": \"cmpl-c0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
-                    ", \"model\": \"Distributed Model\", \"choices\": [{\"index\": 0, \"finish_reason\": " + (stop ? "\"stop\"" : "\"\"");
+                    ", \"model\": \"Distributed Model\", \"choices\": [{\"index\": " + std::to_string(index) + ", \"finish_reason\": " +
+                    (stop ? "\"stop\"" : "\"\"");
     if (!stop) s += ", \"delta\": {\"role\": \"assistant\", \"content\": " + jsonEscape(delta ? *delta : std::string()) + "}";
     s += "}]}";
     return s;
+}
+
+// ---- several completions of one prompt ------------------------------------------------------------------------------------
+
+std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t token, uint32_t P, uint32_t n, int maxTokens, uint32_t seqLen,
+                                             Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken) {
+    if (n < 1 || n > kMaxChoices) throw std::runtime_error("n must be between 1 and 8");
+    std::vector<std::vector<int32_t>> out(n);
+    const uint32_t C = P + 1 < seqLen ? (seqLen - 1 - P) / n : 0;
+    const uint32_t limit = maxTokens <= 0 ? C : std::min<uint32_t>((uint32_t)maxTokens, C);
+    if (limit == 0) return out;
+    // today's single-sequence path from P for the choices in [first, last]; they all see the same tokens
+    const auto single = [&](Sampler &smp, uint32_t first, uint32_t last) {
+        int32_t tok = token;
+        uint32_t pos = P;
+        std::vector<bool> done(n, false);
+        uint32_t nDone = 0;
+        while (out[first].size() < limit) {
+            tok = backend.next(tok, pos++, smp);
+            for (uint32_t i = first; i <= last; i++) {
+                if (done[i]) continue;
+                out[i].push_back(tok);
+                if (onToken(i, tok)) { done[i] = true; nDone++; }
+            }
+            if (nDone == last - first + 1) break;
+        }
+    };
+    if (n == 1 || sampler.temperature() == 0.f) {   // greedy choices are all equal: one run
+        single(sampler, 0, n - 1);
+        return out;
+    }
+    const float T = sampler.temperature(), topp = sampler.topp();
+    std::vector<uint64_t> seeds(n);
+    for (uint32_t i = 0; i < n; i++) seeds[i] = choiceSeed(baseSeed, i);
+    if (!backend.batchedChoices(n)) {
+        const uint64_t saved = backend.saveSampler();
+        for (uint32_t i = 0; i < n; i++) {
+            Sampler smp(sampler.vocabSize(), T, topp, seeds[i]);
+            single(smp, i, i);
+        }
+        backend.restoreSampler(saved);
+        return out;
+    }
+    backend.seedChoices(seeds);
+    std::vector<int32_t> last = backend.choicesFirst(token, P, n, T, topp);
+    uint32_t active = (1u << n) - 1u;
+    for (uint32_t j = 0;; j++) {
+        for (uint32_t i = 0; i < n; i++) {
+            if (!((active >> i) & 1u)) continue;
+            out[i].push_back(last[i]);
+            if (onToken(i, last[i]) || out[i].size() >= limit) active &= ~(1u << i);
+        }
+        if (!active) break;
+        last = backend.choicesStep(last, P, C, j, active, T, topp);
+    }
+    return out;
 }
 
 // ---- completion -----------------------------------------------------------------------------------------------------------
@@ -178,7 +235,16 @@ void ApiServer::complete(HttpRequest &req) {
     const int maxTokens = (int)body.numberOr("max_tokens", -1);
     sampler_.setTemperature((float)body.numberOr("temperature", cfg_.temperature));
     sampler_.setTopp((float)body.numberOr("top_p", cfg_.topp));
-    if (const JsonValue *s = body.find("seed")) if (s->kind == JsonValue::Number) sampler_.setSeed((uint64_t)s->num);
+    uint32_t nChoices = 1;
+    if (const JsonValue *v = body.find("n")) {
+        if (v->kind != JsonValue::Number || v->num != (double)(int64_t)v->num || v->num < 1 || v->num > kMaxChoices)
+            throw std::runtime_error("'n' must be an integer from 1 to 8");
+        nChoices = (uint32_t)v->num;
+    }
+    bool seeded = false;
+    if (const JsonValue *s = body.find("seed")) if (s->kind == JsonValue::Number) { sampler_.setSeed((uint64_t)s->num); seeded = true; }
+    // several completions: choice i uses choiceSeed(base, i); without a seed the base is drawn from the advancing generator
+    const uint64_t baseSeed = seeded ? sampler_.seed() : (nChoices > 1 ? sampler_.nextSeed() : 0);
 
     const uint32_t seqLen = backend_.seqLen();
     const uint32_t startPos = cache_.resolveDeltaPrompt(messages);
@@ -189,6 +255,10 @@ void ApiServer::complete(HttpRequest &req) {
     const uint32_t promptEnd = std::min(startPos + nPrompt - 1, seqLen);
     const uint32_t maxPred = maxTokens > 0 ? std::min(promptEnd + (uint32_t)maxTokens, seqLen) : seqLen;
     for (const ChatItem &m : messages) cache_.push(promptEnd, m);
+    if (nChoices > 1) {
+        completeChoices(req, nChoices, stream, g.publicPrompt, tokens, startPos, promptEnd, maxTokens, baseSeed);
+        return;
+    }
 
     std::string buffer;
     if (stream) req.writeStreamStart();
@@ -234,6 +304,55 @@ void ApiServer::complete(HttpRequest &req) {
                       "}, \"finish_reason\": \"stop\"}]}");
     }
     std::printf("🔶\n");
+}
+
+// n completions of one prompt: the prompt is prefilled once and the cache keeps only the prompt messages, so a follow-up that
+// quotes any one choice re-uses the prompt.
+void ApiServer::completeChoices(HttpRequest &req, uint32_t n, bool stream, const std::string &publicPrompt, const std::vector<int32_t> &tokens,
+                                uint32_t startPos, uint32_t promptEnd, int maxTokens, uint64_t baseSeed) {
+    std::vector<EosDetector> dets(n, EosDetector(tok_.data().eosIds, stops_, maxLen(stops_), maxLen(stops_)));
+    std::vector<std::string> pending(n), buffers(n);
+    if (stream) req.writeStreamStart();
+    if (!publicPrompt.empty())
+        for (uint32_t i = 0; i < n; i++) {
+            if (stream) req.writeStreamChunk("data: " + chunkJson(&publicPrompt, false, i) + "\r\n\r\n");
+            buffers[i] += publicPrompt;
+        }
+    const uint32_t nPref = promptEnd - startPos;
+    backend_.prefill(std::vector<int32_t>(tokens.begin(), tokens.begin() + nPref), startPos);
+    const int32_t token = nPref < tokens.size() ? tokens[nPref] : tokens.back();
+    const auto onToken = [&](uint32_t i, int32_t t) {
+        const std::string piece = tok_.decodeWith(pending[i], t);
+        const EosDetectorResult kind = dets[i].append(t, piece);
+        if (kind == NOT_EOS || kind == EOS) {
+            const std::string delta = dets[i].getDelta();
+            if (!delta.empty()) {
+                if (stream) req.writeStreamChunk("data: " + chunkJson(&delta, false, i) + "\r\n\r\n");
+                buffers[i] += delta;
+            }
+            dets[i].reset();
+        }
+        return kind == EOS;
+    };
+    const std::vector<std::vector<int32_t>> out = runChoices(backend_, token, promptEnd, n, maxTokens, backend_.seqLen(), sampler_, baseSeed, onToken);
+    std::printf("(%u choices)🔶\n", n);
+    if (stream) {
+        for (uint32_t i = 0; i < n; i++) req.writeStreamChunk("data: " + chunkJson(nullptr, true, i) + "\r\n\r\n");
+        req.writeStreamChunk("data: [DONE]");
+        req.writeStreamEnd();
+        return;
+    }
+    uint32_t nCompletion = 0;
+    for (const auto &o : out) nCompletion += (uint32_t)o.size();
+    const uint32_t nPrompt = (uint32_t)tokens.size();
+    std::string choices;
+    for (uint32_t i = 0; i < n; i++)
+        choices += std::string(i ? ", " : "") + "{\"index\": " + std::to_string(i) + ", \"message\": {\"role\": \"assistant\", \"content\": " +
+                   jsonEscape(buffers[i]) + "}, \"finish_reason\": \"stop\"}";
+    req.writeJson("{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
+                  ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
+                  ", \"prompt_tokens\": " + std::to_string(nPrompt) + ", \"total_tokens\": " + std::to_string(nPrompt + nCompletion) +
+                  "}, \"choices\": [" + choices + "]}");
 }
 
 void ApiServer::models(HttpRequest &req) const {

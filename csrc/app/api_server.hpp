@@ -4,6 +4,7 @@
 // JSON / template / stop-detector plumbing can be exercised without a GPU (tests/native/api_stub_main.cpp).
 #pragma once
 #include <cstdint>
+#include <functional>
 #include <map>
 #include <string>
 #include <vector>
@@ -20,7 +21,27 @@ struct InferenceBackend {
     virtual void setVocabLimit(uint32_t) {}   // greedy decoding never returns ids >= limit (tokenizer vocabulary)
     virtual void prefill(const std::vector<int32_t> &tokens, uint32_t pos) = 0;
     virtual int32_t next(int32_t token, uint32_t pos, Sampler &sampler) = 0;   // greedy on the device when temperature == 0
+    // Several completions of one prompt (runChoices). Without a batched path the choices run one after another through next().
+    virtual bool batchedChoices(uint32_t /*n*/) const { return false; }
+    virtual void seedChoices(const std::vector<uint64_t> & /*seeds*/) {}
+    // first tokens of n choices, all drawn from the logits of `token` at P
+    virtual std::vector<int32_t> choicesFirst(int32_t /*token*/, uint32_t /*P*/, uint32_t /*n*/, float /*temperature*/, float /*topp*/) { return {}; }
+    // one batched step: choice b feeds tokens[b] at rotary position P + 1 + j, cache row P + 1 + b * C + j (active choices only)
+    virtual std::vector<int32_t> choicesStep(const std::vector<int32_t> & /*tokens*/, uint32_t /*P*/, uint32_t /*C*/, uint32_t /*j*/,
+                                             uint32_t /*activeMask*/, float /*temperature*/, float /*topp*/) { return {}; }
+    // the sequential path re-seeds the single-sequence generator per choice; these keep its stream across the request
+    virtual uint64_t saveSampler() { return 0; }
+    virtual void restoreSampler(uint64_t /*saved*/) {}
 };
+
+constexpr uint32_t kMaxChoices = 8;   // the engine's widest batch: one row per choice
+
+// n completions of the prompt whose last token `token` sits at P (everything before it prefilled); choice i draws with
+// choiceSeed(baseSeed, i), its j-th token has rotary position P + 1 + j and cache row P + 1 + i * C + j with
+// C = (seqLen - 1 - P) / n, and it stops after min(maxTokens, C) tokens (maxTokens <= 0: C). onToken(i, token) returns true
+// when choice i is finished. Same rules as distributed_llama_b200.api.run_choices.
+std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t token, uint32_t P, uint32_t n, int maxTokens, uint32_t seqLen,
+                                             Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken);
 
 struct HttpRequest {
     int fd = -1;
@@ -53,7 +74,7 @@ private:
     std::vector<Item> items_;
 };
 
-std::string chunkJson(const std::string *delta, bool stop);   // one streamed `chat.completion` chunk
+std::string chunkJson(const std::string *delta, bool stop, uint32_t index = 0);   // one streamed `chat.completion` chunk
 
 struct ApiConfig {
     std::string host = "0.0.0.0", modelName = "model", chatTemplate;
@@ -67,6 +88,8 @@ class ApiServer {
 public:
     ApiServer(InferenceBackend &backend, Tokenizer &tokenizer, const ApiConfig &cfg);
     void complete(HttpRequest &req);
+    void completeChoices(HttpRequest &req, uint32_t n, bool stream, const std::string &publicPrompt, const std::vector<int32_t> &tokens,
+                         uint32_t startPos, uint32_t promptEnd, int maxTokens, uint64_t baseSeed);
     void models(HttpRequest &req) const;
     void serve();          // accept loop
 private:

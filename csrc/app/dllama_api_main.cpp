@@ -34,6 +34,18 @@ struct EngineBackend : InferenceBackend {
         std::memcpy(tmp.data(), logits, tmp.size() * sizeof(float));
         return sampler.sample(tmp.data());
     }
+    // choices: one batched step per token on dense models; the sequential fallback (MoE) keeps the device generator's stream
+    bool batchedChoices(uint32_t n) const override { return e.supportsChoices(n); }
+    void seedChoices(const std::vector<uint64_t> &seeds) override { tp.seedChoices(seeds); }
+    std::vector<int32_t> choicesFirst(int32_t token, uint32_t P, uint32_t n, float temperature, float topp) override {
+        return tp.choicesFirst(token, P, n, temperature, topp);
+    }
+    std::vector<int32_t> choicesStep(const std::vector<int32_t> &tokens, uint32_t P, uint32_t C, uint32_t j, uint32_t activeMask, float temperature,
+                                     float topp) override {
+        return tp.choicesStep(tokens, P, C, j, activeMask, temperature, topp);
+    }
+    uint64_t saveSampler() override { return e.nRanks() > 1 ? tp.samplerState() : 0; }
+    void restoreSampler(uint64_t saved) override { if (e.nRanks() > 1) tp.restoreSampler(saved); }
 };
 
 const char *kUsage =

@@ -419,6 +419,48 @@ int32_t NativeEngine::stepSampled(int32_t token, uint32_t pos, float temperature
     return next;
 }
 
+uint64_t NativeEngine::samplerState() { return (uint64_t)dl_engine_sampler_state(impl_->engine); }
+
+void NativeEngine::seedChoiceSamplers(const std::vector<uint64_t> &seeds) {
+    std::vector<unsigned long long> s(seeds.begin(), seeds.end());
+    engCheck(dl_engine_sampler_seed_rows(impl_->engine, s.data(), (int)s.size()), "dl_engine_sampler_seed_rows");
+}
+
+static uint32_t choiceBatch(uint32_t n) { uint32_t nb = 1; while (nb < n) nb *= 2; return nb; }
+
+std::vector<int32_t> NativeEngine::choicesFirst(int32_t token, uint32_t P, uint32_t n, float temperature, float topp) {
+    if (!supportsChoices(n) || P >= seqLen_) throw std::runtime_error("choices: unsupported batch or position");
+    Impl &I = *impl_;
+    setInputs(&token, 1, P, false);
+    forward(1, 1, false);
+    const uint32_t nb = choiceBatch(n), mask = ((1u << nb) - 1u) & ~((1u << n) - 1u);
+    engCheck(dl_engine_sample_rows(I.engine, (int)nb, mask, temperature, topp, 1, I.stream), "dl_engine_sample_rows");
+    std::vector<int32_t> out(n);
+    cudaCheck(cudaMemcpyAsync(out.data(), I.tokens, n * 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(tokens)");
+    cudaCheck(cudaStreamSynchronize(I.stream), "choicesFirst");
+    if (dl_engine_aborted(I.engine)) throw std::runtime_error("device-side wait timed out: a tensor-parallel peer stopped responding");
+    return out;
+}
+
+std::vector<int32_t> NativeEngine::choicesStep(const std::vector<int32_t> &tokens, uint32_t P, uint32_t C, uint32_t j, uint32_t activeMask,
+                                               float temperature, float topp) {
+    const uint32_t n = (uint32_t)tokens.size(), nb = choiceBatch(n);
+    if (!supportsChoices(n) || C < 1 || j >= C || (uint64_t)P + 1 + (uint64_t)n * C > seqLen_) throw std::runtime_error("choices: rows beyond the context");
+    Impl &I = *impl_;
+    std::vector<int32_t> t(tokens), p(nb, (int32_t)(P + 1 + j));
+    t.resize(nb, 0);
+    const uint32_t mask = ~activeMask & ((1u << nb) - 1u);
+    cudaCheck(cudaMemcpyAsync(I.tokens, t.data(), nb * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(tokens)");
+    cudaCheck(cudaMemcpyAsync(I.pos, p.data(), nb * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(pos)");
+    engCheck(dl_engine_choices_forward(I.engine, (int)nb, P, C, j, mask, I.stream), "dl_engine_choices_forward");
+    engCheck(dl_engine_sample_rows(I.engine, (int)nb, mask, temperature, topp, 0, I.stream), "dl_engine_sample_rows");
+    std::vector<int32_t> out(n);
+    cudaCheck(cudaMemcpyAsync(out.data(), I.tokens, n * 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(tokens)");
+    cudaCheck(cudaStreamSynchronize(I.stream), "choicesStep");
+    if (dl_engine_aborted(I.engine)) throw std::runtime_error("device-side wait timed out: a tensor-parallel peer stopped responding");
+    return out;
+}
+
 uint64_t NativeEngine::syncNs() const { return nRanks_ > 1 ? (uint64_t)dl_engine_sync_ns(impl_->engine) : 0; }
 
 void NativeEngine::linkBytes(uint32_t nTokens, uint64_t &sent, uint64_t &received) const {

@@ -50,6 +50,14 @@ public:
     // rank must have called seedSampler with the same seed; under tensor parallelism every rank draws the same token.
     void seedSampler(uint64_t seed);
     int32_t stepSampled(int32_t token, uint32_t pos, float temperature, float topp);
+    uint64_t samplerState();   // single-sequence generator state: seedSampler(samplerState()) continues its stream
+    // Several completions of one prompt (csrc/cuda/choices.cu), dense models, n <= 8: generators of the batched sampler (separate
+    // from the single-sequence one), first draws from the logits of `token` at P, one batched step (see InferenceBackend).
+    bool supportsChoices(uint32_t n) const { return n >= 1 && n <= maxBatch_ && h_.nExperts == 0; }
+    void seedChoiceSamplers(const std::vector<uint64_t> &seeds);
+    std::vector<int32_t> choicesFirst(int32_t token, uint32_t P, uint32_t n, float temperature, float topp);
+    std::vector<int32_t> choicesStep(const std::vector<int32_t> &tokens, uint32_t P, uint32_t C, uint32_t j, uint32_t activeMask, float temperature,
+                                     float topp);
     // n greedy steps back to back on the device without host round trips; returns the generated tokens.
     std::vector<int32_t> decodeGreedy(int32_t firstToken, uint32_t pos, uint32_t nSteps);
     void synchronize();

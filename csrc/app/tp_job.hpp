@@ -23,7 +23,8 @@
 
 namespace dl {
 
-enum : uint32_t { TP_OP_PREFILL = 1, TP_OP_STEP_GREEDY = 2, TP_OP_STEP_SAMPLED = 3, TP_OP_EXIT = 4, TP_OP_SEED = 5 };
+enum : uint32_t { TP_OP_PREFILL = 1, TP_OP_STEP_GREEDY = 2, TP_OP_STEP_SAMPLED = 3, TP_OP_EXIT = 4, TP_OP_SEED = 5,
+                  TP_OP_CHOICES_SEED = 6, TP_OP_CHOICES_FIRST = 7, TP_OP_CHOICES_STEP = 8 };
 constexpr uint32_t kTpMaxRanks = 8, kTpCtrlTokens = 256;
 
 struct TpControl {
@@ -111,7 +112,8 @@ struct TpJob {   // one process's view of the job
 struct TpEngine {
     NativeEngine &engine;
     TpJob &job;
-    uint64_t seedGen = ~0ull;
+    uint64_t seedGen = ~0ull, seedOf = 0;   // (generation, seed) of the sampler the device generator was last seeded for
+    uint64_t savedGen = ~0ull, savedSeed = 0;
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos) {
         for (size_t i = 0; i < tokens.size(); i += 192) {   // one control packet per tensor-core chunk
             const uint32_t n = (uint32_t)std::min<size_t>(192, tokens.size() - i);
@@ -125,15 +127,53 @@ struct TpEngine {
     }
     // temperature / top-p on the device (the logits stay sharded); `sampler` only supplies the parameters and the seed
     int32_t stepSampled(int32_t token, uint32_t pos, Sampler &sampler, float topp) {
-        if (sampler.seedGeneration() != seedGen) {
+        if (sampler.seedGeneration() != seedGen || sampler.seed() != seedOf) {
             seedGen = sampler.seedGeneration();
+            seedOf = sampler.seed();
             job.issue(TP_OP_SEED, nullptr, 0, 0, 0.f, 0.f, sampler.seed());
             engine.seedSampler(sampler.seed());
         }
         job.issue(TP_OP_STEP_SAMPLED, &token, 1, pos, sampler.temperature(), topp);
         return engine.stepSampled(token, pos, sampler.temperature(), topp);
     }
+    // the single-sequence generator's state, and re-seeding every rank with it (sequential choices re-seed it per choice)
+    uint64_t samplerState() {
+        savedGen = seedGen; savedSeed = seedOf;
+        return seedGen == ~0ull ? 0 : engine.samplerState();
+    }
+    void restoreSampler(uint64_t state) {
+        seedGen = savedGen; seedOf = savedSeed;
+        if (seedGen == ~0ull) return;   // never seeded before the request: the next sampled step seeds afresh
+        job.issue(TP_OP_SEED, nullptr, 0, 0, 0.f, 0.f, state);
+        engine.seedSampler(state);
+    }
+    // choices: seeds travel as (lo, hi) token pairs; step packets carry [C, j, activeMask, tokens...]
+    void seedChoices(const std::vector<uint64_t> &seeds) {
+        std::vector<int32_t> w;
+        for (uint64_t s : seeds) { w.push_back((int32_t)(uint32_t)s); w.push_back((int32_t)(uint32_t)(s >> 32)); }
+        job.issue(TP_OP_CHOICES_SEED, w.data(), (uint32_t)w.size(), 0);
+        engine.seedChoiceSamplers(seeds);
+    }
+    std::vector<int32_t> choicesFirst(int32_t token, uint32_t P, uint32_t n, float temperature, float topp) {
+        const int32_t w[2] = {token, (int32_t)n};
+        job.issue(TP_OP_CHOICES_FIRST, w, 2, P, temperature, topp);
+        return engine.choicesFirst(token, P, n, temperature, topp);
+    }
+    std::vector<int32_t> choicesStep(const std::vector<int32_t> &tokens, uint32_t P, uint32_t C, uint32_t j, uint32_t activeMask, float temperature,
+                                     float topp) {
+        std::vector<int32_t> w = {(int32_t)C, (int32_t)j, (int32_t)activeMask};
+        w.insert(w.end(), tokens.begin(), tokens.end());
+        job.issue(TP_OP_CHOICES_STEP, w.data(), (uint32_t)w.size(), P, temperature, topp);
+        return engine.choicesStep(tokens, P, C, j, activeMask, temperature, topp);
+    }
 };
+
+// Seeds of a TP_OP_CHOICES_SEED packet.
+inline std::vector<uint64_t> tpChoiceSeeds(const int32_t *w, uint32_t n) {
+    std::vector<uint64_t> seeds;
+    for (uint32_t i = 0; i + 1 < n; i += 2) seeds.push_back((uint64_t)(uint32_t)w[i] | ((uint64_t)(uint32_t)w[i + 1] << 32));
+    return seeds;
+}
 
 // ranks >= 1: mirror the root's engine calls until TP_OP_EXIT (reference: runWorkerApp, src/app.cpp:306-365). Returns the exit code.
 inline int tpWorkerMain(const std::string &model, const std::string &tokenizer, uint32_t maxSeqLen, int gpuIndex, TpJob &job) {
@@ -154,6 +194,11 @@ inline int tpWorkerMain(const std::string &model, const std::string &tokenizer, 
             else if (c.op == TP_OP_STEP_GREEDY) engine.stepGreedy(c.tokens[0], c.pos);
             else if (c.op == TP_OP_STEP_SAMPLED) engine.stepSampled(c.tokens[0], c.pos, c.temperature, c.topp);
             else if (c.op == TP_OP_SEED) engine.seedSampler(c.seed);
+            else if (c.op == TP_OP_CHOICES_SEED) engine.seedChoiceSamplers(tpChoiceSeeds(c.tokens, c.n));
+            else if (c.op == TP_OP_CHOICES_FIRST) engine.choicesFirst(c.tokens[0], c.pos, (uint32_t)c.tokens[1], c.temperature, c.topp);
+            else if (c.op == TP_OP_CHOICES_STEP)
+                engine.choicesStep(std::vector<int32_t>(c.tokens + 3, c.tokens + c.n), c.pos, (uint32_t)c.tokens[0], (uint32_t)c.tokens[1],
+                                   (uint32_t)c.tokens[2], c.temperature, c.topp);
             job.ctl->ack[job.rank].store(mine, std::memory_order_release);
         }
         job.ctl->ack[job.rank].store(mine, std::memory_order_release);

@@ -56,12 +56,14 @@ __global__ void __launch_bounds__(128) ropeKvKernel(RopeKvArgs a) {
         const float x1 = v.x * cs.y + v.y * cs.x;
         v.x = x0; v.y = x1;
     }
+    const uint32_t cacheRow = (uint32_t)p + t * a.rowStride;
+    const bool inactive = t < 32 && ((a.inactiveMask >> t) & 1u);
     if (isQ) {
         reinterpret_cast<float2 *>(row)[j] = v;
-    } else {
+    } else if (!inactive && cacheRow < a.seqLen) {
         const uint32_t kvh = isK ? head - a.nHeads : head - a.nHeads - a.nKvHeads;
         __nv_bfloat16 *cache = isK ? a.kCache : a.vCache;
-        __nv_bfloat162 *dst = reinterpret_cast<__nv_bfloat162 *>(cache + ((size_t)kvh * a.seqLen + p) * hd);
+        __nv_bfloat162 *dst = reinterpret_cast<__nv_bfloat162 *>(cache + ((size_t)kvh * a.seqLen + cacheRow) * hd);
         dst[j] = __floats2bfloat162_rn(v.x, v.y);
     }
 }

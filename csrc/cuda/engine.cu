@@ -145,13 +145,18 @@ static int engineDecodeMega(Engine &e, bool greedyAdvance, cudaStream_t stream) 
     return launchMegaDecode(m, (int)(e.megaCtas ? e.megaCtas : c.numSms), stream);
 }
 
-// logitsMode: 0 = none (prefill chunk), 1 = logits of the last token in the batch into logits[0], 2 = all tokens
-static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, cudaStream_t stream) {
+// Geometry of a choices step (see choices.cu): nb rows at rotary position P + 1 + j, row b stored at P + 1 + b * C + j.
+struct ChoiceStep { uint32_t P, C, j, inactiveMask; };
+
+// logitsMode: 0 = none (prefill chunk), 1 = logits of the last token in the batch into logits[0], 2 = all tokens.
+// ch: a choices step instead of a batch of consecutive tokens (logitsMode 2, dense layers only).
+static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, cudaStream_t stream, const ChoiceStep *ch = nullptr) {
     const EngineConfig &c = e.cfg;
     const bool pdl = c.usePdl != 0;
     const uint32_t qDim = c.nHeads * c.headDim, kvDim = c.nKvHeads * c.headDim, qkvDim = qDim + 2 * kvDim;
     if (nb < 1 || (uint32_t)nb > c.maxBatch || (nb & (nb - 1))) return -10;
     e.lastDecodeMega = false;
+    if (ch && (c.nExperts > 0 || logitsMode != 2 || greedyAdvance)) return -14;
     if (nb == 1 && logitsMode == 1 && e.useMega) {
         const int r = engineDecodeMega(e, greedyAdvance, stream);
         if (r != 1) { e.lastDecodeMega = r == 0; return r; }
@@ -172,7 +177,20 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
         a.qs = (const uint32_t *)L.qkvQs; a.scales = (const __half *)L.qkvSc; a.d = qkvDim; a.n = c.dim;
         a.in = e.g.x; a.inStride = c.dim; a.normW = L.norm0; a.eps = c.eps; a.out = e.g.qkv; a.outStride = qkvDim; a.trace = nextTrace();
         DL_TRY(gemvSel(e, PRO_RMSNORM_, EPI_STORE_, nb, a, c.numSms, stream, pdl));
-        if (nb == 1 && e.fusedAttn) {
+        if (ch) {
+            // 2+3. qk-norm + rope + K/V append at the choices' own rows, then attention over the shared prompt + own rows
+            RopeKvArgs r{};
+            r.qkv = e.g.qkv; r.qkvStride = qkvDim; r.pos = e.g.pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
+            r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = c.seqLen;
+            r.kCache = (__nv_bfloat16 *)L.kCache; r.vCache = (__nv_bfloat16 *)L.vCache; r.rowStride = ch->C; r.inactiveMask = ch->inactiveMask;
+            DL_TRY(launchRopeKv(r, nb, stream, pdl));
+            ChoiceAttnArgs t{};
+            t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.kCache = r.kCache; t.vCache = r.vCache;
+            t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.seqLen = c.seqLen; t.nSplits = c.nSplits;
+            t.B = (uint32_t)nb; t.P = ch->P; t.C = ch->C; t.j = ch->j; t.inactiveMask = ch->inactiveMask;
+            t.partial = e.g.attnPartial; t.counters = e.g.attnCounters; t.out = e.g.z; t.outStride = qDim;
+            DL_TRY(launchChoiceAttn(t, stream, pdl));
+        } else if (nb == 1 && e.fusedAttn) {
             // 2+3. qk-norm + rope + kv append + attention in one launch
             AttnFusedArgs f{};
             f.qkv = e.g.qkv; f.pos = e.g.pos; f.rope = e.g.rope; f.qNorm = L.qNorm; f.kNorm = L.kNorm; f.eps = c.eps;
@@ -344,6 +362,9 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
 
 using dl::Engine;
 
+// rngState: [0] = single-sequence generator, [kChoiceRngSlots + b] = generator of choice b
+constexpr uint32_t kChoiceRngSlots = 8;
+
 DL_EXPORT void *dl_engine_create(const dl::EngineConfig *cfg) {
     Engine *e = new Engine();
     e->cfg = *cfg;
@@ -453,12 +474,11 @@ DL_EXPORT int dl_engine_aborted(void *h) {
 
 // Seeds the device-resident xorshift* generator (same stream of coins as the host Sampler for the same seed) and allocates the
 // sampler scratch. Under tensor parallelism every rank must call this with the same seed.
-DL_EXPORT int dl_engine_sampler_seed(void *h, unsigned long long seed) {
-    Engine *e = (Engine *)h;
+static int ensureSampler(Engine *e) {
     const dl::EngineConfig &c = e->cfg;
     if (!e->rngState) {
-        DL_CUDA_CHECK(cudaMalloc(&e->rngState, 64));
-        DL_CUDA_CHECK(cudaMalloc(&e->probScratch, ((size_t)c.vocab * (c.nRanks ? c.nRanks : 1) + 16) * sizeof(float)));
+        DL_CUDA_CHECK(cudaMalloc(&e->rngState, 2 * kChoiceRngSlots * sizeof(unsigned long long)));
+        DL_CUDA_CHECK(cudaMalloc(&e->probScratch, ((size_t)c.maxBatch * c.vocab * (c.nRanks ? c.nRanks : 1) + 16) * sizeof(float)));
         DL_CUDA_CHECK(cudaMalloc(&e->gatherEpoch, 64));
         DL_CUDA_CHECK(cudaMemset(e->gatherEpoch, 0, 64));
         DL_CUDA_CHECK(cudaMalloc(&e->gatherBlockCounter, 64));
@@ -476,9 +496,23 @@ DL_EXPORT int dl_engine_sampler_seed(void *h, unsigned long long seed) {
             DL_CUDA_CHECK(cudaMemcpy(e->flagUcDev, f, sizeof(f), cudaMemcpyHostToDevice));
         }
     }
+    return 0;
+}
+
+DL_EXPORT int dl_engine_sampler_seed(void *h, unsigned long long seed) {
+    Engine *e = (Engine *)h;
+    DL_TRY(ensureSampler(e));
     if (seed == 0) seed = 0x9E3779B97F4A7C15ull;   // xorshift state must not be zero
     DL_CUDA_CHECK(cudaMemcpy(e->rngState, &seed, sizeof(seed), cudaMemcpyHostToDevice));
     return 0;
+}
+
+// Current state of the single-sequence generator (0 before the first seeding). Seeding with it continues the same stream.
+DL_EXPORT unsigned long long dl_engine_sampler_state(void *h) {
+    Engine *e = (Engine *)h;
+    unsigned long long v = 0;
+    if (e->rngState && cudaMemcpy(&v, e->rngState, sizeof(v), cudaMemcpyDeviceToHost) != cudaSuccess) return 0ull;
+    return v;
 }
 
 // Samples the next token from the logits of the last forward (logitsMode 1) on the device: tokens[0] <- sample, pos[0]++, history.
@@ -502,6 +536,43 @@ DL_EXPORT int dl_engine_sample(void *h, float temperature, float topp, cudaStrea
     DL_TRY(dl::launchLogitsGather(e->g.logits, c.vocab, c.rank, nR, gatherMc, e->gatherUcDev, flagMc, e->flagUcDev, e->gatherBlockCounter, stream));
     return dl::launchSample(gatherLocal, e->probScratch, n, temperature, topp, e->rngState, e->g.tokens, e->g.pos, e->g.history, c.seqLen, flagLocal,
                             e->gatherEpoch, nR, stream);
+}
+
+// Seeds the n <= 8 generators of the batched sampler. They are separate from the single-sequence generator of dl_engine_sample,
+// which keeps its stream. Every rank must pass the same seeds.
+DL_EXPORT int dl_engine_sampler_seed_rows(void *h, const unsigned long long *seeds, int n) {
+    Engine *e = (Engine *)h;
+    if (n < 1 || n > (int)kChoiceRngSlots) return -51;
+    DL_TRY(ensureSampler(e));
+    unsigned long long s[kChoiceRngSlots];
+    for (int i = 0; i < n; i++) s[i] = seeds[i] ? seeds[i] : 0x9E3779B97F4A7C15ull;
+    DL_CUDA_CHECK(cudaMemcpy(e->rngState + kChoiceRngSlots, s, n * sizeof(unsigned long long), cudaMemcpyHostToDevice));
+    return 0;
+}
+
+// nb draws into tokens[0..nb), row b with batched-sampler generator b. firstStep: every row draws from the logits row of the last single-token
+// forward (logits[0]); otherwise row b draws from logits[b] of a choices forward. Rows set in inactiveMask draw nothing.
+// Tensor parallel: the vocabulary slices of the rows are gathered first and every rank draws the same tokens.
+DL_EXPORT int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, float temperature, float topp, int firstStep, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    const dl::EngineConfig &c = e->cfg;
+    if (!e->rngState) return -50;
+    if (nb < 1 || (uint32_t)nb > c.maxBatch || nb > (int)kChoiceRngSlots) return -10;
+    const uint32_t nR = e->comm.nRanks > 1 ? e->comm.nRanks : 1;
+    const uint32_t full = c.vocab * nR;
+    const uint32_t n = (e->vocabLimit && e->vocabLimit < full) ? e->vocabLimit : full;
+    const uint32_t rows = firstStep ? 1u : (uint32_t)nb;
+    if (nR == 1)
+        return dl::launchSampleRows(e->g.logits, firstStep ? 0u : c.vocab, e->probScratch, n, temperature, topp, e->rngState + kChoiceRngSlots, e->g.tokens, nb,
+                                    inactiveMask, nullptr, nullptr, 1, stream);
+    uint8_t *mine = (uint8_t *)e->comm.arena[e->comm.rank];
+    float *gatherLocal = (float *)(mine + e->comm.gatherOff);
+    unsigned int *flagLocal = (unsigned int *)(mine + e->comm.flagsOff);
+    float *gatherMc = e->comm.mcArena ? (float *)((uint8_t *)e->comm.mcArena + e->comm.gatherOff) : nullptr;
+    unsigned int *flagMc = e->comm.mcArena ? (unsigned int *)((uint8_t *)e->comm.mcArena + e->comm.flagsOff) : nullptr;
+    DL_TRY(dl::launchLogitsGather(e->g.logits, c.vocab, c.rank, nR, gatherMc, e->gatherUcDev, flagMc, e->flagUcDev, e->gatherBlockCounter, stream, rows));
+    return dl::launchSampleRows(gatherLocal, firstStep ? 0u : full, e->probScratch, n, temperature, topp, e->rngState + kChoiceRngSlots, e->g.tokens, nb, inactiveMask,
+                                flagLocal, e->gatherEpoch, nR, stream);
 }
 
 DL_EXPORT int dl_engine_set_comm(void *h, const dl::CommPtrs *p) {
@@ -584,6 +655,14 @@ DL_EXPORT int dl_engine_forward_part(void *h, int nb, uint32_t layer, int part, 
         return dl::gemvSel(e, dl::PRO_PLAIN_, dl::EPI_STORE_, nb, a, c.numSms, stream, false);
     }
     return -2;
+}
+
+// One choices step: nb (power of two, <= maxBatch) tokens staged in tokens[0..nb) with pos[0..nb) = P + 1 + j. Row b attends to
+// the prompt rows [0, P] and its own rows [P + 1 + b * C, P + 1 + b * C + j] and appends its K/V at P + 1 + b * C + j; rows set
+// in inactiveMask (finished choices, batch padding) write no K/V. Logits of all nb rows land in logits[0..nb).
+DL_EXPORT int dl_engine_choices_forward(void *h, int nb, uint32_t P, uint32_t C, uint32_t j, uint32_t inactiveMask, cudaStream_t stream) {
+    const dl::ChoiceStep ch{P, C, j, inactiveMask};
+    return dl::engineForward(*(Engine *)h, nb, 2, false, stream, &ch);
 }
 
 DL_EXPORT int dl_engine_prefill(void *h, uint32_t T, uint32_t p0, int wantLogits, cudaStream_t stream) {

@@ -90,6 +90,11 @@ int dl_engine_mega_active(void *h);   // 1 if the last single-token forward ran 
 unsigned long long dl_engine_sync_ns(void *h);
 int dl_engine_sampler_seed(void *h, unsigned long long seed);
 int dl_engine_sample(void *h, float temperature, float topp, cudaStream_t stream);   // after a forward with logitsMode 1
+// choices (several completions of one prompt, csrc/cuda/choices.cu): generators 0..n-1, batched draws, one choices forward
+int dl_engine_sampler_seed_rows(void *h, const unsigned long long *seeds, int n);   // separate from the single-sequence generator
+unsigned long long dl_engine_sampler_state(void *h);   // single-sequence generator state (seed with it to continue the stream)
+int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, float temperature, float topp, int firstStep, cudaStream_t stream);
+int dl_engine_choices_forward(void *h, int nb, uint32_t P, uint32_t C, uint32_t j, uint32_t inactiveMask, cudaStream_t stream);
 int dl_engine_set_trace(void *h, uint64_t *buf, uint32_t capLaunches);
 int dl_engine_set_trace_all(void *h, int allCtas);
 uint32_t dl_engine_num_sms(void *h);

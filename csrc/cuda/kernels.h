@@ -73,8 +73,29 @@ struct RopeKvArgs {
     uint32_t nHeads, nKvHeads, headDim, seqLen;
     __nv_bfloat16 *kCache;
     __nv_bfloat16 *vCache;
+    // Choice steps (several sequences at one rotary position): token t stores its K/V row at pos[t] + t * rowStride, and tokens
+    // whose bit is set in inactiveMask store nothing. Both 0 for a plain batch of consecutive tokens.
+    uint32_t rowStride, inactiveMask;
 };
 int launchRopeKv(const RopeKvArgs &a, int nb, cudaStream_t stream, bool pdl);
+
+// Attention of B choices that share the prompt rows [0, P] of the cache (choices.cu). Query row b (choice b, rotary position
+// P + 1 + j, already normalised and rotated by ropeKvKernel) attends to [0, P] and to its own rows [P + 1 + b * C, P + 1 + b * C + j].
+// A CTA owns (KV head, prefix split) and serves all B * nHeads / nKvHeads query rows of that head, so each prefix row is read
+// once per step. The last split also runs the per-choice suffixes; the last CTA to finish merges the splits.
+struct ChoiceAttnArgs {
+    const float *qkv;
+    uint32_t qkvStride;
+    const __nv_bfloat16 *kCache, *vCache;
+    uint32_t nHeads, nKvHeads, headDim, seqLen, nSplits;
+    uint32_t B, P, C, j;
+    uint32_t inactiveMask;   // rows whose bit is set skip their suffix; their output is not meaningful
+    float *partial;          // >= B * nHeads * nSplits * (headDim + 2) floats
+    unsigned int *counters;  // [nKvHeads], zero-initialised, self-resetting
+    float *out;              // [B][outStride], head h at columns h * headDim
+    uint32_t outStride;
+};
+int launchChoiceAttn(const ChoiceAttnArgs &a, cudaStream_t stream, bool pdl);
 
 struct AttnArgs {
     const float *qkv;
@@ -153,7 +174,12 @@ int launchSample(const float *logits, float *probs, uint32_t n, float temperatur
                  int *history, uint32_t historyCap, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
                  cudaStream_t stream);
 int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t nRanks, float *gatherMc, float *const *gatherUcDev,
-                       unsigned int *flagMc, unsigned int *const *flagUcDev, unsigned int *blockCounter, cudaStream_t stream);
+                       unsigned int *flagMc, unsigned int *const *flagUcDev, unsigned int *blockCounter, cudaStream_t stream, uint32_t rows = 1);
+// B draws, one CTA per row: row b reads logits + b * logitsStride (0: every row draws from the same logits), uses rng[b] and writes
+// tokenOut[b]. Rows whose bit is set in inactiveMask draw nothing and keep their generator state. No position advance.
+int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
+                     int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
+                     cudaStream_t stream);
 
 // Persistent decode kernel (mega_decode.cu)
 struct MegaLayer {

@@ -37,6 +37,8 @@ struct SampleArgs {
     unsigned int *gatherEpoch;     // device counter of completed gathers (the kernel advances it)
     uint32_t nRanks;
     int *debugOut;             // optional [4]: {last index in order?, ...} unused by the product path
+    // batched draws (grid B, one CTA per row): row b reads logits + b * logitsStride, probs + b * probsStride, rng[b], tokenOut[b]
+    uint32_t logitsStride, probsStride, inactiveMask;
 };
 
 __device__ float blockMax(float v, float *red) {
@@ -169,13 +171,19 @@ __global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
     __shared__ int sInt[8];
     __shared__ float sCoin;
     const uint32_t n = a.n;
+    const uint32_t row = blockIdx.x;
+    if (row < 32 && ((a.inactiveMask >> row) & 1u)) return;
+    a.logits += (size_t)row * a.logitsStride;
+    a.probs += (size_t)row * a.probsStride;
+    a.rng += row;
+    a.tokenOut += row;
     if (a.gatherFlag && a.nRanks > 1) {
         if (threadIdx.x == 0) {
             const unsigned int want = (*a.gatherEpoch + 1u) * a.nRanks;
             unsigned int v;
             uint32_t spins = 0;
             do { asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a.gatherFlag) : "memory"); } while ((int)(v - want) < 0 && ++spins < (1u << 28));
-            *a.gatherEpoch += 1u;
+            if (gridDim.x == 1) *a.gatherEpoch += 1u;   // batched draws: epochAdvanceKernel runs after the grid
         }
         __syncthreads();
     }
@@ -242,14 +250,18 @@ __global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
     }
 }
 
-// Copies this rank's vocabulary slice into the gather buffer of every rank and signals its arrival.
+__global__ void epochAdvanceKernel(unsigned int *gatherEpoch) { *gatherEpoch += 1u; }
+
+// Copies this rank's vocabulary slice of `rows` logits rows ([rows][v0], local) into the gather buffer of every rank
+// ([rows][nRanks * v0]) and signals its arrival.
 __global__ void __launch_bounds__(256) logitsGatherKernel(const float *local, uint32_t v0, uint32_t rank, uint32_t nRanks, float *gatherMc,
                                                            float *const *gatherUc, unsigned int *flagMc, unsigned int *const *flagUc,
-                                                           unsigned int *blockCounter) {
+                                                           unsigned int *blockCounter, uint32_t rows) {
     const uint32_t nVec = v0 / 4;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nVec; i += gridDim.x * blockDim.x) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nVec * rows; i += gridDim.x * blockDim.x) {
         const float4 v = reinterpret_cast<const float4 *>(local)[i];
-        const size_t off = (size_t)rank * v0 + (size_t)i * 4;
+        const uint32_t row = i / nVec;
+        const size_t off = ((size_t)row * nRanks + rank) * v0 + (size_t)(i - row * nVec) * 4;
         if (gatherMc) {
             asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(gatherMc + off), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
         } else {
@@ -284,10 +296,27 @@ int launchSample(const float *logits, float *probs, uint32_t n, float temperatur
 }
 
 int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t nRanks, float *gatherMc, float *const *gatherUcDev,
-                       unsigned int *flagMc, unsigned int *const *flagUcDev, unsigned int *blockCounter, cudaStream_t stream) {
-    if (v0 % 4) return -1;
-    logitsGatherKernel<<<32, 256, 0, stream>>>(local, v0, rank, nRanks, gatherMc, gatherUcDev, flagMc, flagUcDev, blockCounter);
+                       unsigned int *flagMc, unsigned int *const *flagUcDev, unsigned int *blockCounter, cudaStream_t stream, uint32_t rows) {
+    if (v0 % 4 || rows < 1) return -1;
+    logitsGatherKernel<<<32, 256, 0, stream>>>(local, v0, rank, nRanks, gatherMc, gatherUcDev, flagMc, flagUcDev, blockCounter, rows);
     DL_CUDA_CHECK(cudaGetLastError());
+    return 0;
+}
+
+int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
+                     int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
+                     cudaStream_t stream) {
+    if (n < 2 || temperature <= 0.f || B < 1 || B > 32) return -1;
+    SampleArgs a{};
+    a.logits = logits; a.probs = probs; a.n = n; a.temperature = temperature; a.topp = topp; a.rng = rng; a.tokenOut = tokenOut;
+    a.gatherFlag = gatherFlag; a.gatherEpoch = gatherEpoch; a.nRanks = nRanks;
+    a.logitsStride = logitsStride; a.probsStride = n; a.inactiveMask = inactiveMask;
+    sampleKernel<<<B, kSampThreads, 0, stream>>>(a);
+    DL_CUDA_CHECK(cudaGetLastError());
+    if (gatherFlag && nRanks > 1 && B > 1) {
+        epochAdvanceKernel<<<1, 1, 0, stream>>>(gatherEpoch);
+        DL_CUDA_CHECK(cudaGetLastError());
+    }
     return 0;
 }
 
@@ -297,4 +326,12 @@ int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t 
 DL_EXPORT int dl_sample_logits(const float *logits, float *probsScratch, uint32_t n, float temperature, float topp, unsigned long long *rngState,
                                int *tokenOut, cudaStream_t stream) {
     return dl::launchSample(logits, probsScratch, n, temperature, topp, rngState, tokenOut, nullptr, nullptr, 0, nullptr, nullptr, 1, stream);
+}
+
+// Stand-alone entry for tests: B draws from logits rows (device f32, row b at logits + b * logitsStride; 0 = all rows from one row),
+// with the generators rngState[0..B) (device u64) and B * n floats of scratch.
+DL_EXPORT int dl_sample_rows(const float *logits, uint32_t logitsStride, float *probsScratch, uint32_t n, float temperature, float topp,
+                             unsigned long long *rngState, int *tokenOut, uint32_t B, uint32_t inactiveMask, cudaStream_t stream) {
+    return dl::launchSampleRows(logits, logitsStride, probsScratch, n, temperature, topp, rngState, tokenOut, B, inactiveMask, nullptr, nullptr, 1,
+                                stream);
 }

@@ -172,6 +172,14 @@ PYBIND11_MODULE(_host, m) {
         .def_property_readonly("eos_ids", [](const Tokenizer &t) { return t.data().eosIds; })
         .def_property_readonly("chat_template", [](const Tokenizer &t) { return asBytes(t.data().chatTemplate); });
 
+    // Streaming decoder state of one sequence over a shared tokenizer (the choices of one request each keep their own).
+    struct TokenDecoder { std::string pending; };
+    py::class_<TokenDecoder>(m, "TokenDecoder")
+        .def(py::init<>())
+        .def("decode", [](TokenDecoder &d, const Tokenizer &t, int32_t token) { return asBytes(t.decodeWith(d.pending, token)); })
+        .def("reset", [](TokenDecoder &d) { d.pending.clear(); });
+    m.def("choice_seed", &choiceSeed, py::arg("seed"), py::arg("index"));
+
     py::class_<Rng>(m, "Rng")
         .def(py::init<uint64_t>())
         .def("next_u32", &Rng::nextU32)
@@ -186,6 +194,7 @@ PYBIND11_MODULE(_host, m) {
             return s.sample(copy.mutable_data());
         })
         .def("next_coin", &Sampler::nextCoin)
+        .def("next_seed", &Sampler::nextSeed)
         .def("set_temperature", &Sampler::setTemperature)
         .def("set_topp", &Sampler::setTopp)
         .def("set_seed", &Sampler::setSeed)

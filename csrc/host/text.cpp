@@ -207,22 +207,22 @@ std::vector<int32_t> Tokenizer::encode(const std::string &text, bool isStart, bo
     return toks;
 }
 
-std::string Tokenizer::decode(int32_t token) {
+std::string Tokenizer::decodeWith(std::string &pending, int32_t token) const {
     if (token == d_.bosId) return std::string();
     if (isEos(token)) {
         std::string rest;
-        rest.swap(pending_);
+        rest.swap(pending);
         return rest;
     }
     if (token < 0 || (size_t)token >= d_.vocab.size()) throw std::runtime_error("Tokenizer: token id out of range");
-    pending_ += d_.vocab[token];
+    pending += d_.vocab[token];
 
     static const char kReplacement[] = "\xEF\xBF\xBD";
     std::string out;
-    size_t i = 0, committed = 0;   // bytes [0, committed) of pending_ are fully consumed
-    const size_t n = pending_.size();
+    size_t i = 0, committed = 0;   // bytes [0, committed) of pending are fully consumed
+    const size_t n = pending.size();
     while (i < n) {
-        const unsigned char c = (unsigned char)pending_[i];
+        const unsigned char c = (unsigned char)pending[i];
         size_t need;
         if (c <= 0x7f) need = 0;
         else if (c >= 0xc0 && c <= 0xdf) need = 1;
@@ -230,9 +230,9 @@ std::string Tokenizer::decode(int32_t token) {
         else if (c >= 0xf0 && c <= 0xf7) need = 3;
         else { out += kReplacement; i++; committed = i; continue; }   // stray continuation / invalid lead
         size_t have = 0;
-        while (have < need && i + 1 + have < n && (((unsigned char)pending_[i + 1 + have]) & 0xc0) == 0x80) have++;
+        while (have < need && i + 1 + have < n && (((unsigned char)pending[i + 1 + have]) & 0xc0) == 0x80) have++;
         if (have == need) {
-            out.append(pending_, i, need + 1);
+            out.append(pending, i, need + 1);
             i += need + 1;
             committed = i;
         } else if (i + 1 + have < n) {
@@ -244,9 +244,11 @@ std::string Tokenizer::decode(int32_t token) {
             break;   // incomplete tail: wait for more bytes
         }
     }
-    pending_.erase(0, committed);
+    pending.erase(0, committed);
     return out;
 }
+
+std::string Tokenizer::decode(int32_t token) { return decodeWith(pending_, token); }
 
 // ---- RNG / sampler ---------------------------------------------------------------------------------
 

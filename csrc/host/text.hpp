@@ -40,6 +40,8 @@ public:
     // Invalid sequences are replaced by U+FFFD. BOS yields "", EOS flushes whatever is pending.
     std::string decode(int32_t token);
     void resetDecoder() { pending_.clear(); }
+    // The same streaming decode with the caller's pending bytes: one state per sequence (the choices of one request).
+    std::string decodeWith(std::string &pending, int32_t token) const;
     bool isEos(int32_t token) const;
     std::string describe() const;   // the "📄 ..." lines
 
@@ -57,6 +59,16 @@ private:
     std::string pending_;
 };
 
+// Seed of choice i of a request for several completions: choice 0 keeps the request's seed (so it draws what a one-completion
+// request draws), the others get a splitmix64 mix of (seed, i). The host and device samplers, and both servers, use this.
+inline uint64_t choiceSeed(uint64_t seed, uint32_t i) {
+    if (i == 0) return seed;
+    uint64_t z = seed + 0x9E3779B97F4A7C15ull * (uint64_t)i;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
 // xorshift* generator shared by the host and (by passing the drawn coin) the device sampler.
 struct Rng {
     uint64_t state;
@@ -72,6 +84,9 @@ public:
     Sampler(uint32_t vocabSize, float temperature, float topp, uint64_t seed);
     int32_t sample(float *logits);          // modifies logits in place (temperature, softmax)
     float nextCoin() { return rng_.nextF32(); }
+    // A fresh 64-bit seed drawn from this sampler's generator (advances it): the base seed of a request for several
+    // completions that names no seed, so that repeated requests differ.
+    uint64_t nextSeed() { const uint64_t hi = rng_.nextU32(); return (hi << 32) | rng_.nextU32(); }
     void setTemperature(float t) { temperature_ = t; }
     void setTopp(float p) { topp_ = p; }
     void setSeed(uint64_t s) { rng_.state = s; seed_ = s; seedGeneration_++; }

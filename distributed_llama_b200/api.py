@@ -9,6 +9,7 @@ src/app.cpp:232-304).
 """
 from __future__ import annotations
 
+import os
 import time
 from dataclasses import dataclass
 from typing import Callable, List, Optional, Sequence
@@ -26,6 +27,77 @@ class GenerationStats:
     n_generated: int = 0
     prefill_ms: float = 0.0
     decode_ms: float = 0.0
+
+
+MAX_CHOICES = 8   # the engine's widest batch: one row per choice
+
+
+def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: int, sampler, base_seed: int,
+                on_token: Callable[[int, int], bool]) -> List[List[int]]:
+    """Generates n completions of one prompt whose last token `token` sits at position P, everything before it prefilled.
+
+    Choice i draws with an xorshift* generator seeded with choice_seed(base_seed, i); its j-th token has rotary position
+    P + 1 + j and its K/V row is P + 1 + i*C + j with C = (seq_len - 1 - P) // n, so the choices share the rest of the context
+    window and each stops after min(max_tokens, C) tokens. Rows up to P-1 are never written; row P is written by the forward
+    of `token` (once on the batched path, once per choice, with the same values, on the sequential path). The single-sequence
+    generator continues its stream afterwards. on_token(i, tok) is called for every generated token and returns True when
+    choice i is finished (end of sequence or stop string). `backend` provides next_token_at(token, pos, sampler),
+    forget_device_seed(), save_sampler() / restore_sampler(saved), and for the batched path batched_choices(n),
+    seed_choices(seeds), choices_first(token, P, n, T, topp) and choices_step(tokens, P, C, j, active, T, topp)
+    (InferenceSession and apps.runtime.RootInference). Returns each choice's tokens."""
+    H = host()
+    if not 1 <= n <= MAX_CHOICES:
+        raise ValueError(f"n must be between 1 and {MAX_CHOICES}")
+    C = (seq_len - 1 - P) // n
+    limit = C if max_tokens <= 0 else min(max_tokens, C)
+    out: List[List[int]] = [[] for _ in range(n)]
+    if limit <= 0:
+        return out
+
+    def single(smp, choices):
+        # today's single-sequence path from P; rows past P belong to this sequence until the next one overwrites them
+        tok, pos, done = token, P, set()
+        while len(out[choices[0]]) < limit:
+            tok = backend.next_token_at(tok, pos, smp)
+            pos += 1
+            for i in choices:
+                if i not in done:
+                    out[i].append(tok)
+                    if on_token(i, tok):
+                        done.add(i)
+            if len(done) == len(choices):
+                break
+
+    if n == 1 or sampler.temperature == 0.0:
+        # greedy choices are all equal: one run
+        single(sampler, list(range(n)))
+        return out
+    T, topp = sampler.temperature, sampler.topp
+    seeds = [H.choice_seed(base_seed, i) for i in range(n)]
+    if not backend.batched_choices(n):
+        saved = backend.save_sampler()
+        try:
+            for i in range(n):
+                backend.forget_device_seed()
+                single(H.Sampler(sampler.vocab_size, T, topp, seeds[i]), [i])
+        finally:
+            backend.restore_sampler(saved)
+        return out
+    backend.seed_choices(seeds)
+    last = backend.choices_first(token, P, n, T, topp)
+    active = [True] * n
+    j = 0
+    while True:
+        for i in range(n):
+            if active[i]:
+                out[i].append(last[i])
+                if on_token(i, last[i]) or len(out[i]) >= limit:
+                    active[i] = False
+        if not any(active):
+            break
+        last = backend.choices_step(last, P, C, j, active, T, topp)
+        j += 1
+    return out
 
 
 class InferenceSession:
@@ -100,6 +172,63 @@ class InferenceSession:
             return int(self._pin_out[0])
         lg = self.forward_logits(token)
         return int(self.sampler.sample(lg.float().cpu().numpy()))
+
+    # ---- several completions of one prompt ----
+    def next_token_at(self, token: int, pos: int, sampler) -> int:
+        """next_token at an explicit position with an explicit sampler (the choices' sequential path)."""
+        saved = self.sampler
+        self.pos, self.sampler = pos, sampler
+        try:
+            return self.next_token(token)
+        finally:
+            self.sampler = saved
+
+    def forget_device_seed(self):
+        self._dev_seeded = None
+
+    def save_sampler(self):
+        key = self._dev_seeded
+        return key, (self.engine.sampler_state() if key is not None else 0)
+
+    def restore_sampler(self, saved):
+        key, state = saved
+        if key is not None:
+            self.engine.seed_sampler(state)
+        self._dev_seeded = key
+
+    def batched_choices(self, n: int) -> bool:
+        return self.device.type == "cuda" and self.engine.supports_choices(n) and os.environ.get("DL_HOST_SAMPLER") is None
+
+    def seed_choices(self, seeds: Sequence[int]):
+        self.engine.seed_choice_samplers(seeds)
+
+    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float) -> List[int]:
+        return self.engine.choices_first(token, P, n, temperature, topp)
+
+    def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
+                     topp: float) -> List[int]:
+        return self.engine.choices_step(tokens, P, C, j, active, temperature, topp)
+
+    def generate_choices(self, prompt: str, n: int, max_tokens: int, seed: Optional[int] = None) -> List[str]:
+        """n completions of `prompt`, each at most max_tokens tokens (and at most its share of the remaining context, see
+        run_choices), with the session's temperature and top-p. Choice i is seeded with choice_seed(seed, i); without a seed
+        the base seed is drawn from the session's sampler, so repeated calls differ. The prompt is prefilled once."""
+        assert self.tokenizer is not None
+        H = host()
+        toks = self.tokenizer.encode(prompt, True, True)
+        self.prefill(toks[:-1])
+        P = self.pos
+        decoders = [H.TokenDecoder() for _ in range(n)]
+        pieces: List[List[bytes]] = [[] for _ in range(n)]
+
+        def on_token(i: int, tok: int) -> bool:
+            pieces[i].append(decoders[i].decode(self.tokenizer, tok))
+            return bool(self.tokenizer.is_eos(tok))
+
+        base = self.sampler.next_seed() if seed is None else seed
+        run_choices(self, toks[-1], P, n, max_tokens, self.engine.seq_len, self.sampler, base, on_token)
+        self.pos = P + 1
+        return [b"".join(p).decode("utf-8", errors="replace") for p in pieces]
 
     # ---- text level ----
     def generate(self, prompt: str, steps: int, on_piece: Optional[Callable[[str], None]] = None) -> str:

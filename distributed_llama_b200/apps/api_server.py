@@ -15,6 +15,7 @@ import time
 from typing import Dict, List, Optional, Tuple
 
 from .. import host
+from ..api import MAX_CHOICES, run_choices
 from .args import AppArgs, parse_args
 from .cli import make_chat_tools
 from .runtime import AppContext, run_inference_app
@@ -112,8 +113,16 @@ class HttpRequest:
         self._send(b"0000\r\n\r\n")
 
 
-def chunk_json(delta: Optional[str], stop: bool) -> str:
-    choice = {"index": 0, "finish_reason": "stop" if stop else ""}
+def parse_n(body: dict) -> int:
+    """The request's `n` (completions of one prompt): absent means 1; anything but an integer in 1..MAX_CHOICES is refused."""
+    n = body.get("n", 1)
+    if isinstance(n, bool) or not isinstance(n, int) or not 1 <= n <= MAX_CHOICES:
+        raise ValueError(f"'n' must be an integer from 1 to {MAX_CHOICES}")
+    return n
+
+
+def chunk_json(delta: Optional[str], stop: bool, index: int = 0) -> str:
+    choice = {"index": index, "finish_reason": "stop" if stop else ""}
     if not stop:
         choice["delta"] = {"role": "assistant", "content": delta}
     return json.dumps({"id": "cmpl-c0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
@@ -131,6 +140,7 @@ class ApiServer:
         ctx, H = self.ctx, self.H
         tok, inf, h, smp = ctx.tokenizer, ctx.inference, ctx.header, ctx.sampler
         body = req.json or {}
+        n_choices = parse_n(body)
         messages = [(m["role"], m["content"]) for m in body["messages"]]
         stream = bool(body.get("stream", False))
         max_tokens = int(body.get("max_tokens", -1))
@@ -138,6 +148,8 @@ class ApiServer:
         smp.set_topp(float(body.get("top_p", ctx.args.topp)))
         if "seed" in body:
             smp.set_seed(int(body["seed"]))
+        # several completions: choice i uses choice_seed(base, i); without a seed the base is drawn from the advancing generator
+        base_seed = smp.seed if "seed" in body else (smp.next_seed() if n_choices > 1 else 0)
         delta_prompt, start_pos = self.cache.resolve_delta_prompt(list(messages))
         content, public = self.gen.generate(delta_prompt, True)
         print(f"🔹{content.decode('utf-8', errors='replace')}🔸", end="")
@@ -147,6 +159,9 @@ class ApiServer:
         max_pred = min(prompt_end + max_tokens, h.seq_len) if max_tokens > 0 else h.seq_len
         for m in delta_prompt:
             self.cache.push(prompt_end, m)
+        if n_choices > 1:
+            self._complete_choices(req, n_choices, stream, public, tokens, start_pos, prompt_end, max_tokens, n_prompt, base_seed)
+            return
         buffer = ""
         if stream:
             req.write_stream_start()
@@ -195,6 +210,57 @@ class ApiServer:
                 "usage": {"completion_tokens": n_completion, "prompt_tokens": n_prompt, "total_tokens": n_prompt + n_completion},
                 "choices": [{"index": 0, "message": {"role": "assistant", "content": buffer}, "finish_reason": "stop"}]}))
         print("🔶")
+
+    def _complete_choices(self, req: HttpRequest, n: int, stream: bool, public: bytes, tokens, start_pos: int, prompt_end: int,
+                          max_tokens: int, n_prompt: int, base_seed: int):
+        """n completions of one prompt (api.run_choices): the prompt is prefilled once and the cache keeps only the prompt
+        messages, so a follow-up that quotes any one choice reuses the prompt."""
+        ctx, H = self.ctx, self.H
+        tok, inf, h = ctx.tokenizer, ctx.inference, ctx.header
+        eos_ids = list(tok.eos_ids)
+        stops = [tok.piece(i) for i in eos_ids]
+        pad = max((len(x) for x in stops), default=0)
+        dets = [H.EosDetector(eos_ids, stops, pad, pad) for _ in range(n)]
+        decoders = [H.TokenDecoder() for _ in range(n)]
+        buffers = [""] * n
+        if stream:
+            req.write_stream_start()
+        if public:
+            p = public.decode("utf-8", errors="replace")
+            for i in range(n):
+                if stream:
+                    req.write_stream_chunk("data: " + chunk_json(p, False, i) + "\r\n\r\n")
+                buffers[i] += p
+        n_pref = prompt_end - start_pos
+        inf.prefill(tokens[:n_pref], start_pos)
+        token = tokens[n_pref] if n_pref < len(tokens) else tokens[-1]
+
+        def on_token(i: int, t: int) -> bool:
+            piece = decoders[i].decode(tok, t)
+            kind = dets[i].append(t, piece)
+            if kind in (H.NOT_EOS, H.EOS):
+                delta = dets[i].get_delta()
+                if delta:
+                    d = delta.decode("utf-8", errors="replace")
+                    if stream:
+                        req.write_stream_chunk("data: " + chunk_json(d, False, i) + "\r\n\r\n")
+                    buffers[i] += d
+                dets[i].reset()
+            return kind == H.EOS
+
+        out = run_choices(inf, token, prompt_end, n, max_tokens, h.seq_len, ctx.sampler, base_seed, on_token)
+        print(f"({n} choices)🔶")
+        if stream:
+            for i in range(n):
+                req.write_stream_chunk("data: " + chunk_json(None, True, i) + "\r\n\r\n")
+            req.write_stream_chunk("data: [DONE]")
+            req.write_stream_end()
+            return
+        n_completion = sum(len(o) for o in out)
+        req.write_json(json.dumps({
+            "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
+            "usage": {"completion_tokens": n_completion, "prompt_tokens": n_prompt, "total_tokens": n_prompt + n_completion},
+            "choices": [{"index": i, "message": {"role": "assistant", "content": buffers[i]}, "finish_reason": "stop"} for i in range(n)]}))
 
     def models(self, req: HttpRequest):
         name = self.ctx.args.model.replace("\\", "/").split("/")[-1]

@@ -21,6 +21,33 @@ from ..api import InferenceSession
 from .args import AppArgs
 
 OP_STOP, OP_PREFILL, OP_STEP_LOGITS, OP_STEP_GREEDY, OP_DECODE_N, OP_STEP_SAMPLE, OP_SEED = 0, 1, 2, 3, 4, 5, 6
+OP_CHOICES_SEED, OP_CHOICES_FIRST, OP_CHOICES_STEP = 7, 8, 9
+
+
+def _split_seed(seed: int) -> List[int]:
+    return [seed & 0x7FFFFFFF, (seed >> 31) & 0x7FFFFFFF, (seed >> 62) & 0x3]
+
+
+def _join_seed(w: Sequence[int]) -> int:
+    return w[0] | (w[1] << 31) | (w[2] << 62)
+
+
+def _active_mask(active: Sequence[bool]) -> int:
+    return sum(1 << i for i, a in enumerate(active) if a)
+
+
+def _active_list(mask: int, n: int) -> List[bool]:
+    return [bool((mask >> i) & 1) for i in range(n)]
+
+
+def _f32_bits(*xs: float) -> List[int]:
+    import struct
+    return list(struct.unpack(f"<{len(xs)}i", struct.pack(f"<{len(xs)}f", *xs)))
+
+
+def _bits_f32(*xs: int) -> List[float]:
+    import struct
+    return list(struct.unpack(f"<{len(xs)}f", struct.pack(f"<{len(xs)}i", *xs)))
 
 
 def world():
@@ -127,7 +154,7 @@ class RootInference:
         return self._pin_in is not None and not getattr(self.eng, "_parts", False) and os.environ.get("DL_HOST_SAMPLER") is None
 
     def seed(self, seed: int) -> None:
-        self._send(OP_SEED, 0, [seed & 0x7FFFFFFF, (seed >> 31) & 0x7FFFFFFF, (seed >> 62) & 0x3])
+        self._send(OP_SEED, 0, _split_seed(seed))
         self.eng.seed_sampler(seed)
 
     def forward_sampled(self, token: int, pos: int, temperature: float, topp: float) -> int:
@@ -151,6 +178,39 @@ class RootInference:
                 self._seeded = (sampler.seed, sampler.seed_generation)
             return self.forward_sampled(token, pos, sampler.temperature, sampler.topp)
         return int(sampler.sample(self.forward_logits(token, pos).float().cpu().numpy()))
+
+    # ---- several completions of one prompt (api.run_choices); workers mirror every batched step ----
+    def next_token_at(self, token: int, pos: int, sampler) -> int:
+        return self.next_token(token, pos, sampler)
+
+    def forget_device_seed(self):
+        self._seeded = None
+
+    def save_sampler(self):
+        key = getattr(self, "_seeded", None)
+        return key, (self.eng.sampler_state() if key is not None and self.device_sampling else 0)
+
+    def restore_sampler(self, saved):
+        key, state = saved
+        if key is not None and self.device_sampling:
+            self.seed(state)
+        self._seeded = key
+
+    def batched_choices(self, n: int) -> bool:
+        return self.device_sampling and self.eng.supports_choices(n)
+
+    def seed_choices(self, seeds: Sequence[int]) -> None:
+        self._send(OP_CHOICES_SEED, 0, [w for s in seeds for w in _split_seed(s)])
+        self.eng.seed_choice_samplers(seeds)
+
+    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float) -> List[int]:
+        self._send(OP_CHOICES_FIRST, P, [token, n] + _f32_bits(temperature, topp))
+        return self.eng.choices_first(token, P, n, temperature, topp)
+
+    def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
+                     topp: float) -> List[int]:
+        self._send(OP_CHOICES_STEP, P, [C, j, _active_mask(active)] + _f32_bits(temperature, topp) + list(tokens))
+        return self.eng.choices_step(tokens, P, C, j, active, temperature, topp)
 
     def decode_greedy(self, token: int, pos: int, n_steps: int) -> List[int]:
         """n greedy steps with the token fed back on the device (no host round trip per step): one control packet for all."""
@@ -196,7 +256,17 @@ def worker_loop(sess: InferenceSession, comm, chan=None) -> None:
         elif op == OP_DECODE_N:
             eng.decode_greedy(toks[0], pos, toks[1])
         elif op == OP_SEED:
-            eng.seed_sampler(toks[0] | (toks[1] << 31) | (toks[2] << 62))
+            eng.seed_sampler(_join_seed(toks))
+        elif op == OP_CHOICES_SEED:
+            eng.seed_choice_samplers([_join_seed(toks[i:i + 3]) for i in range(0, len(toks), 3)])
+        elif op == OP_CHOICES_FIRST:
+            temperature, topp = _bits_f32(toks[2], toks[3])
+            eng.choices_first(toks[0], pos, toks[1], temperature, topp)
+        elif op == OP_CHOICES_STEP:
+            C, j, mask = toks[0], toks[1], toks[2]
+            temperature, topp = _bits_f32(toks[3], toks[4])
+            tokens = toks[5:]
+            eng.choices_step(tokens, pos, C, j, _active_list(mask, len(tokens)), temperature, topp)
         elif op == OP_STEP_SAMPLE:
             import struct
             temperature, topp = struct.unpack("<ff", struct.pack("<ii", toks[1], toks[2]))

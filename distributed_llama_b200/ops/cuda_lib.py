@@ -110,6 +110,20 @@ def lib() -> C.CDLL:
     L.dl_engine_sample.restype = i32
     L.dl_sample_logits.argtypes = [vp, vp, u32, f32, f32, vp, vp, vp]
     L.dl_sample_logits.restype = i32
+    L.dl_sample_rows.argtypes = [vp, u32, vp, u32, f32, f32, vp, vp, u32, u32, vp]
+    L.dl_sample_rows.restype = i32
+    L.dl_choice_attn.argtypes = [vp, u32, vp, vp, vp, vp, f32, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
+    L.dl_choice_attn.restype = i32
+    L.dl_choice_attn_only.argtypes = [vp, u32, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
+    L.dl_choice_attn_only.restype = i32
+    L.dl_engine_sampler_state.argtypes = [vp]
+    L.dl_engine_sampler_state.restype = C.c_uint64
+    L.dl_engine_sampler_seed_rows.argtypes = [vp, C.POINTER(C.c_uint64), i32]
+    L.dl_engine_sampler_seed_rows.restype = i32
+    L.dl_engine_sample_rows.argtypes = [vp, i32, u32, f32, f32, i32, vp]
+    L.dl_engine_sample_rows.restype = i32
+    L.dl_engine_choices_forward.argtypes = [vp, i32, u32, u32, u32, u32, vp]
+    L.dl_engine_choices_forward.restype = i32
     L.dl_engine_sync_ns.argtypes = [vp]
     L.dl_engine_sync_ns.restype = C.c_uint64
     L.dl_engine_mega_active.argtypes = [vp]

@@ -165,6 +165,72 @@ class Engine:
         self.forward_batch([token], pos, logits_mode=1)
         cl.check(self._lib.dl_engine_sample(self._h, float(temperature), float(topp), cl.stream_ptr()), "engine_sample")
 
+    # -- choices: several completions of one prompt, one row per choice (csrc/cuda/choices.cu) --
+    def supports_choices(self, n: int) -> bool:
+        """True if n choices can run as one batched step: dense layers, kernel-fused collectives, n <= max_batch."""
+        return 1 <= n <= min(8, self.max_batch) and self.w.header.n_experts == 0 and not self._parts
+
+    @staticmethod
+    def _choice_batch(n: int, active: Optional[Sequence[bool]] = None):
+        """(rows padded to a power of two, bit mask of the inactive rows: finished choices and padding)."""
+        nb = 1
+        while nb < n:
+            nb *= 2
+        mask = 0
+        for b in range(nb):
+            if b >= n or (active is not None and not active[b]):
+                mask |= 1 << b
+        return nb, mask
+
+    def seed_choice_samplers(self, seeds: Sequence[int]):
+        """Seeds generator i of the batched sampler with seeds[i]; the single-sequence generator keeps its stream."""
+        arr = (C.c_uint64 * len(seeds))(*[int(s) & 0xFFFFFFFFFFFFFFFF for s in seeds])
+        cl.check(self._lib.dl_engine_sampler_seed_rows(self._h, arr, len(seeds)), "engine_sampler_seed_rows")
+        self._sampler_ready = True
+
+    def sample_choices_first(self, n: int, temperature: float, topp: float) -> None:
+        """After a single-token forward at the prompt end: choice i draws its first token from that logits row with generator i.
+        The draws land in tokens[:n]."""
+        nb, mask = self._choice_batch(n)
+        cl.check(self._lib.dl_engine_sample_rows(self._h, nb, mask, float(temperature), float(topp), 1, cl.stream_ptr()), "engine_sample_rows")
+
+    def choices_forward(self, tokens: Sequence[int], P: int, C: int, j: int, active: Optional[Sequence[bool]] = None) -> None:
+        """One choices step: choice b feeds tokens[b] at rotary position P + 1 + j, attends to the prompt rows [0, P] and its own
+        rows [P + 1 + b*C, P + 1 + b*C + j], and stores its K/V at the last of those. Inactive choices write nothing.
+        Logits of every row land in logits[:len(tokens)]."""
+        n = len(tokens)
+        nb, mask = self._choice_batch(n, active)
+        if not self.supports_choices(n):
+            raise ValueError("batched choices need dense layers, kernel-fused collectives and n <= max_batch")
+        if C < 1 or j >= C or P + 1 + n * C > self.seq_len:
+            raise ValueError("choice rows beyond the context length")
+        self.tokens[:nb].copy_(torch.tensor(list(tokens) + [0] * (nb - n), dtype=torch.int32))
+        self.pos[:nb].fill_(P + 1 + j)
+        cl.check(self._lib.dl_engine_choices_forward(self._h, nb, P, C, j, mask, cl.stream_ptr()), "engine_choices_forward")
+
+    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float) -> List[int]:
+        """Forward of the prompt's last token at P, then choice i draws its first token from that row with generator i."""
+        self.forward_batch([token], P, logits_mode=1)
+        self.sample_choices_first(n, temperature, topp)
+        out = self.tokens[:n].tolist()
+        self.check_abort()
+        return out
+
+    def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
+                     topp: float) -> List[int]:
+        """choices_forward, then every active row draws its next token with its own generator. Returns the draws (inactive
+        rows: whatever tokens[] held)."""
+        self.choices_forward(tokens, P, C, j, active)
+        nb, mask = self._choice_batch(len(tokens), active)
+        cl.check(self._lib.dl_engine_sample_rows(self._h, nb, mask, float(temperature), float(topp), 0, cl.stream_ptr()), "engine_sample_rows")
+        out = self.tokens[:len(tokens)].tolist()
+        self.check_abort()
+        return out
+
+    def sampler_state(self) -> int:
+        """State of the single-sequence device generator (0 before the first seeding); seed_sampler(state) continues its stream."""
+        return int(self._lib.dl_engine_sampler_state(self._h))
+
     # -- traffic / synchronisation accounting (reference: NnNetwork::getStats + executor sync timers, src/dllama.cpp:59-66) --
     def sync_ns(self) -> int:
         """Cumulative ns the decode kernel waited for peer ranks inside its fused all-reduces (0 on one GPU)."""
