@@ -151,7 +151,8 @@ std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t 
     if (n < 1 || n > kMaxChoices) throw std::runtime_error("n must be between 1 and 8");
     std::vector<std::vector<int32_t>> out(n);
     const uint32_t C = P + 1 < seqLen ? (seqLen - 1 - P) / n : 0;
-    const uint32_t limit = maxTokens <= 0 ? C : std::min<uint32_t>((uint32_t)maxTokens, C);
+    uint32_t limit = n == 1 ? (P < seqLen ? seqLen - P : 0) : C;
+    if (maxTokens > 0) limit = std::min<uint32_t>((uint32_t)maxTokens, limit);
     if (limit == 0) return out;
     // today's single-sequence path from P for the choices in [first, last]; they all see the same tokens
     const auto single = [&](Sampler &smp, uint32_t first, uint32_t last) {
@@ -219,13 +220,15 @@ ApiServer::ApiServer(InferenceBackend &backend, Tokenizer &tokenizer, const ApiC
     : backend_(backend), tok_(tokenizer), cfg_(cfg), sampler_(std::min<uint32_t>(backend.vocabSize(), tokenizer.vocabSize()), cfg.temperature, cfg.topp, cfg.seed),
       stops_(stopPieces(tokenizer)),
       gen_(cfg.chatTemplate.empty() ? TEMPLATE_UNKNOWN : parseChatTemplateType(cfg.chatTemplate), tokenizer.data().chatTemplate,
-           stops_.empty() ? std::string() : stops_[0]),
-      det_(tokenizer.data().eosIds, stops_, maxLen(stops_), maxLen(stops_)) {
+           stops_.empty() ? std::string() : stops_[0]) {
     backend_.setVocabLimit(tokenizer.vocabSize());
     std::printf("⭐ Chat template: %s\n", chatTemplateTypeName(gen_.type()));
     for (const std::string &s : stops_) std::printf("🛑 Stop: %s\n", s.c_str());
 }
 
+// n completions of one prompt (runChoices; n = 1 without `n`): the prompt is prefilled once. After one completion the cache
+// keeps its answer too; after several it keeps only the prompt messages, so a follow-up that quotes any one choice re-uses the
+// prompt.
 void ApiServer::complete(HttpRequest &req) {
     if (!req.hasJson || !req.json.isObject()) throw std::runtime_error("request body must be a JSON object");
     const JsonValue &body = req.json;
@@ -235,16 +238,16 @@ void ApiServer::complete(HttpRequest &req) {
     const int maxTokens = (int)body.numberOr("max_tokens", -1);
     sampler_.setTemperature((float)body.numberOr("temperature", cfg_.temperature));
     sampler_.setTopp((float)body.numberOr("top_p", cfg_.topp));
-    uint32_t nChoices = 1;
+    uint32_t n = 1;
     if (const JsonValue *v = body.find("n")) {
         if (v->kind != JsonValue::Number || v->num != (double)(int64_t)v->num || v->num < 1 || v->num > kMaxChoices)
             throw std::runtime_error("'n' must be an integer from 1 to 8");
-        nChoices = (uint32_t)v->num;
+        n = (uint32_t)v->num;
     }
     bool seeded = false;
     if (const JsonValue *s = body.find("seed")) if (s->kind == JsonValue::Number) { sampler_.setSeed((uint64_t)s->num); seeded = true; }
     // several completions: choice i uses choiceSeed(base, i); without a seed the base is drawn from the advancing generator
-    const uint64_t baseSeed = seeded ? sampler_.seed() : (nChoices > 1 ? sampler_.nextSeed() : 0);
+    const uint64_t baseSeed = seeded ? sampler_.seed() : (n > 1 ? sampler_.nextSeed() : 0);
 
     const uint32_t seqLen = backend_.seqLen();
     const uint32_t startPos = cache_.resolveDeltaPrompt(messages);
@@ -253,76 +256,21 @@ void ApiServer::complete(HttpRequest &req) {
     const std::vector<int32_t> tokens = tok_.encode(g.content, startPos == 0, true);
     const uint32_t nPrompt = (uint32_t)tokens.size();
     const uint32_t promptEnd = std::min(startPos + nPrompt - 1, seqLen);
-    const uint32_t maxPred = maxTokens > 0 ? std::min(promptEnd + (uint32_t)maxTokens, seqLen) : seqLen;
     for (const ChatItem &m : messages) cache_.push(promptEnd, m);
-    if (nChoices > 1) {
-        completeChoices(req, nChoices, stream, g.publicPrompt, tokens, startPos, promptEnd, maxTokens, baseSeed);
-        return;
-    }
 
-    std::string buffer;
-    if (stream) req.writeStreamStart();
-    if (!g.publicPrompt.empty()) {
-        if (stream) req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false) + "\r\n\r\n");
-        buffer += g.publicPrompt;
-    }
-    uint32_t pos = startPos;
-    const uint32_t n = promptEnd - pos;
-    backend_.prefill(std::vector<int32_t>(tokens.begin(), tokens.begin() + n), pos);
-    pos += n;
-    int32_t token = n < tokens.size() ? tokens[n] : tokens.back();
-    tok_.resetDecoder();
-    det_.reset();
-    while (pos < maxPred) {
-        token = backend_.next(token, pos, sampler_);
-        const std::string piece = tok_.decode(token);
-        const EosDetectorResult kind = det_.append(token, piece);
-        if (!piece.empty()) { std::printf("%s", piece.c_str()); std::fflush(stdout); }
-        if (kind == NOT_EOS || kind == EOS) {
-            const std::string delta = det_.getDelta();
-            if (!delta.empty()) {
-                if (stream) req.writeStreamChunk("data: " + chunkJson(&delta, false) + "\r\n\r\n");
-                buffer += delta;
-            }
-            det_.reset();
-        }
-        pos++;
-        if (kind == EOS) break;
-    }
-    if (pos == seqLen) cache_.clear();
-    else cache_.push(pos, {"assistant", buffer});
-    if (stream) {
-        req.writeStreamChunk("data: " + chunkJson(nullptr, true) + "\r\n\r\n");
-        req.writeStreamChunk("data: [DONE]");
-        req.writeStreamEnd();
-    } else {
-        const uint32_t nCompletion = pos - promptEnd;
-        req.writeJson("{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
-                      ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
-                      ", \"prompt_tokens\": " + std::to_string(nPrompt) + ", \"total_tokens\": " + std::to_string(nPrompt + nCompletion) +
-                      "}, \"choices\": [{\"index\": 0, \"message\": {\"role\": \"assistant\", \"content\": " + jsonEscape(buffer) +
-                      "}, \"finish_reason\": \"stop\"}]}");
-    }
-    std::printf("🔶\n");
-}
-
-// n completions of one prompt: the prompt is prefilled once and the cache keeps only the prompt messages, so a follow-up that
-// quotes any one choice re-uses the prompt.
-void ApiServer::completeChoices(HttpRequest &req, uint32_t n, bool stream, const std::string &publicPrompt, const std::vector<int32_t> &tokens,
-                                uint32_t startPos, uint32_t promptEnd, int maxTokens, uint64_t baseSeed) {
     std::vector<EosDetector> dets(n, EosDetector(tok_.data().eosIds, stops_, maxLen(stops_), maxLen(stops_)));
-    std::vector<std::string> pending(n), buffers(n);
-    if (stream) req.writeStreamStart();
-    if (!publicPrompt.empty())
-        for (uint32_t i = 0; i < n; i++) {
-            if (stream) req.writeStreamChunk("data: " + chunkJson(&publicPrompt, false, i) + "\r\n\r\n");
-            buffers[i] += publicPrompt;
-        }
+    std::vector<std::string> pending(n), buffers(n, g.publicPrompt);
+    if (stream) {
+        req.writeStreamStart();
+        if (!g.publicPrompt.empty())
+            for (uint32_t i = 0; i < n; i++) req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false, i) + "\r\n\r\n");
+    }
     const uint32_t nPref = promptEnd - startPos;
     backend_.prefill(std::vector<int32_t>(tokens.begin(), tokens.begin() + nPref), startPos);
     const int32_t token = nPref < tokens.size() ? tokens[nPref] : tokens.back();
     const auto onToken = [&](uint32_t i, int32_t t) {
         const std::string piece = tok_.decodeWith(pending[i], t);
+        if (n == 1 && !piece.empty()) { std::printf("%s", piece.c_str()); std::fflush(stdout); }
         const EosDetectorResult kind = dets[i].append(t, piece);
         if (kind == NOT_EOS || kind == EOS) {
             const std::string delta = dets[i].getDelta();
@@ -334,25 +282,31 @@ void ApiServer::completeChoices(HttpRequest &req, uint32_t n, bool stream, const
         }
         return kind == EOS;
     };
-    const std::vector<std::vector<int32_t>> out = runChoices(backend_, token, promptEnd, n, maxTokens, backend_.seqLen(), sampler_, baseSeed, onToken);
-    std::printf("(%u choices)🔶\n", n);
+    const std::vector<std::vector<int32_t>> out = runChoices(backend_, token, promptEnd, n, maxTokens, seqLen, sampler_, baseSeed, onToken);
+    if (n == 1) {
+        const uint32_t end = promptEnd + (uint32_t)out[0].size();
+        if (end == seqLen) cache_.clear();
+        else cache_.push(end, {"assistant", buffers[0]});
+    }
     if (stream) {
         for (uint32_t i = 0; i < n; i++) req.writeStreamChunk("data: " + chunkJson(nullptr, true, i) + "\r\n\r\n");
         req.writeStreamChunk("data: [DONE]");
         req.writeStreamEnd();
-        return;
+    } else {
+        uint32_t nCompletion = 0;
+        std::string choices;
+        for (uint32_t i = 0; i < n; i++) {
+            nCompletion += (uint32_t)out[i].size();
+            choices += std::string(i ? ", " : "") + "{\"index\": " + std::to_string(i) + ", \"message\": {\"role\": \"assistant\", \"content\": " +
+                       jsonEscape(buffers[i]) + "}, \"finish_reason\": \"stop\"}";
+        }
+        req.writeJson("{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
+                      ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
+                      ", \"prompt_tokens\": " + std::to_string(nPrompt) + ", \"total_tokens\": " + std::to_string(nPrompt + nCompletion) +
+                      "}, \"choices\": [" + choices + "]}");
     }
-    uint32_t nCompletion = 0;
-    for (const auto &o : out) nCompletion += (uint32_t)o.size();
-    const uint32_t nPrompt = (uint32_t)tokens.size();
-    std::string choices;
-    for (uint32_t i = 0; i < n; i++)
-        choices += std::string(i ? ", " : "") + "{\"index\": " + std::to_string(i) + ", \"message\": {\"role\": \"assistant\", \"content\": " +
-                   jsonEscape(buffers[i]) + "}, \"finish_reason\": \"stop\"}";
-    req.writeJson("{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
-                  ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
-                  ", \"prompt_tokens\": " + std::to_string(nPrompt) + ", \"total_tokens\": " + std::to_string(nPrompt + nCompletion) +
-                  "}, \"choices\": [" + choices + "]}");
+    if (n == 1) std::printf("🔶\n");
+    else std::printf("(%u choices)🔶\n", n);
 }
 
 void ApiServer::models(HttpRequest &req) const {

@@ -1,7 +1,7 @@
 // Native `dllama-api`: blocking HTTP/1.1 server with the reference's routes (src/dllama-api.cpp:43-632, src/api-types.hpp):
 //   POST /v1/chat/completions (JSON body; JSON response or SSE-style chunked stream), GET /v1/models, OPTIONS * (CORS), else 404.
 // One request at a time over one KV sequence with NaiveCache prefix re-use. The inference side is an interface so the HTTP /
-// JSON / template / stop-detector plumbing can be exercised without a GPU (tests/native/api_stub_main.cpp).
+// JSON / template / stop-detector plumbing can be exercised without a GPU (tests/native/api_choices_stub_main.cpp).
 #pragma once
 #include <cstdint>
 #include <functional>
@@ -38,8 +38,9 @@ constexpr uint32_t kMaxChoices = 8;   // the engine's widest batch: one row per 
 
 // n completions of the prompt whose last token `token` sits at P (everything before it prefilled); choice i draws with
 // choiceSeed(baseSeed, i), its j-th token has rotary position P + 1 + j and cache row P + 1 + i * C + j with
-// C = (seqLen - 1 - P) / n, and it stops after min(maxTokens, C) tokens (maxTokens <= 0: C). onToken(i, token) returns true
-// when choice i is finished. Same rules as distributed_llama_b200.api.run_choices.
+// C = (seqLen - 1 - P) / n, and it stops after min(maxTokens, C) tokens (maxTokens <= 0: C). A single completion (n = 1) is the
+// single-sequence loop of the CLIs instead: it stops after min(maxTokens, seqLen - P) tokens, so it may fill the context up to
+// its last row. onToken(i, token) returns true when choice i is finished. Same rules as distributed_llama_b200.api.run_choices.
 std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t token, uint32_t P, uint32_t n, int maxTokens, uint32_t seqLen,
                                              Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken);
 
@@ -88,8 +89,6 @@ class ApiServer {
 public:
     ApiServer(InferenceBackend &backend, Tokenizer &tokenizer, const ApiConfig &cfg);
     void complete(HttpRequest &req);
-    void completeChoices(HttpRequest &req, uint32_t n, bool stream, const std::string &publicPrompt, const std::vector<int32_t> &tokens,
-                         uint32_t startPos, uint32_t promptEnd, int maxTokens, uint64_t baseSeed);
     void models(HttpRequest &req) const;
     void serve();          // accept loop
 private:
@@ -100,7 +99,6 @@ private:
     NaiveCache cache_;
     std::vector<std::string> stops_;
     ChatTemplateGenerator gen_;
-    EosDetector det_;
 };
 
 }  // namespace dl

@@ -2,7 +2,6 @@
 // GPU — api_server.cpp (HTTP, JSON, NaiveCache, templates, stop detection) over NativeEngine. Multi-GPU serving: ./dllama-api --gpus N.
 #include <chrono>
 #include <cstdio>
-#include <cstring>
 #include <ctime>
 #include <stdexcept>
 #include <string>
@@ -21,19 +20,12 @@ namespace {
 struct EngineBackend : InferenceBackend {
     NativeEngine &e;
     TpEngine tp;              // announces every engine call to the worker ranks of a --gpus N job (no-op on one GPU)
-    std::vector<float> tmp;
-    EngineBackend(NativeEngine &engine, TpJob &job) : e(engine), tp{engine, job}, tmp(engine.header().vocabSize) {}
+    EngineBackend(NativeEngine &engine, TpJob &job) : e(engine), tp{engine, job} {}
     uint32_t seqLen() const override { return e.seqLen(); }
     uint32_t vocabSize() const override { return e.header().vocabSize; }
     void setVocabLimit(uint32_t limit) override { e.setVocabLimit(limit); }
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos) override { if (!tokens.empty()) tp.prefill(tokens, pos); }
-    int32_t next(int32_t token, uint32_t pos, Sampler &sampler) override {
-        if (sampler.temperature() == 0.f) return tp.stepGreedy(token, pos);
-        if (e.nRanks() > 1) return tp.stepSampled(token, pos, sampler, sampler.topp());   // device sampler: the logits stay sharded
-        const float *logits = e.step(token, pos);
-        std::memcpy(tmp.data(), logits, tmp.size() * sizeof(float));
-        return sampler.sample(tmp.data());
-    }
+    int32_t next(int32_t token, uint32_t pos, Sampler &sampler) override { return tp.next(token, pos, sampler); }
     // choices: one batched step per token on dense models; the sequential fallback (MoE) keeps the device generator's stream
     bool batchedChoices(uint32_t n) const override { return e.supportsChoices(n); }
     void seedChoices(const std::vector<uint64_t> &seeds) override { tp.seedChoices(seeds); }

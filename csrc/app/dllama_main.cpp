@@ -109,13 +109,7 @@ struct App {
 
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos) { tp.prefill(tokens, pos); }
 
-    int32_t next(int32_t token, uint32_t pos) {
-        if (sampler.temperature() == 0.f) return tp.stepGreedy(token, pos);
-        if (job.nRanks > 1) return tp.stepSampled(token, pos, sampler, args.topp);   // logits stay sharded on the devices
-        const float *logits = engine.step(token, pos);
-        std::vector<float> tmp(logits, logits + std::min<uint32_t>(tokenizer.vocabSize(), engine.header().vocabSize));
-        return sampler.sample(tmp.data());
-    }
+    int32_t next(int32_t token, uint32_t pos) { return tp.next(token, pos, sampler); }
 };
 
 void inference(App &app) {

@@ -114,6 +114,7 @@ struct TpEngine {
     TpJob &job;
     uint64_t seedGen = ~0ull, seedOf = 0;   // (generation, seed) of the sampler the device generator was last seeded for
     uint64_t savedGen = ~0ull, savedSeed = 0;
+    std::vector<float> hostLogits = {};     // the host sampler's copy of the logits (one GPU)
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos) {
         for (size_t i = 0; i < tokens.size(); i += 192) {   // one control packet per tensor-core chunk
             const uint32_t n = (uint32_t)std::min<size_t>(192, tokens.size() - i);
@@ -125,16 +126,25 @@ struct TpEngine {
         job.issue(TP_OP_STEP_GREEDY, &token, 1, pos);
         return engine.stepGreedy(token, pos);
     }
+    // One generated token with the sampler's settings: greedy on the device, temperature / top-p on the device under tensor
+    // parallelism (the logits stay sharded), or the host sampler on the logits copied back from one GPU.
+    int32_t next(int32_t token, uint32_t pos, Sampler &sampler) {
+        if (sampler.temperature() == 0.f) return stepGreedy(token, pos);
+        if (engine.nRanks() > 1) return stepSampled(token, pos, sampler);
+        const float *logits = engine.step(token, pos);
+        hostLogits.assign(logits, logits + sampler.vocabSize());
+        return sampler.sample(hostLogits.data());
+    }
     // temperature / top-p on the device (the logits stay sharded); `sampler` only supplies the parameters and the seed
-    int32_t stepSampled(int32_t token, uint32_t pos, Sampler &sampler, float topp) {
+    int32_t stepSampled(int32_t token, uint32_t pos, Sampler &sampler) {
         if (sampler.seedGeneration() != seedGen || sampler.seed() != seedOf) {
             seedGen = sampler.seedGeneration();
             seedOf = sampler.seed();
             job.issue(TP_OP_SEED, nullptr, 0, 0, 0.f, 0.f, sampler.seed());
             engine.seedSampler(sampler.seed());
         }
-        job.issue(TP_OP_STEP_SAMPLED, &token, 1, pos, sampler.temperature(), topp);
-        return engine.stepSampled(token, pos, sampler.temperature(), topp);
+        job.issue(TP_OP_STEP_SAMPLED, &token, 1, pos, sampler.temperature(), sampler.topp());
+        return engine.stepSampled(token, pos, sampler.temperature(), sampler.topp());
     }
     // the single-sequence generator's state, and re-seeding every rank with it (sequential choices re-seed it per choice)
     uint64_t samplerState() {

@@ -38,10 +38,12 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
 
     Choice i draws with an xorshift* generator seeded with choice_seed(base_seed, i); its j-th token has rotary position
     P + 1 + j and its K/V row is P + 1 + i*C + j with C = (seq_len - 1 - P) // n, so the choices share the rest of the context
-    window and each stops after min(max_tokens, C) tokens. Rows up to P-1 are never written; row P is written by the forward
+    window and each stops after min(max_tokens, C) tokens (max_tokens <= 0: C). A single completion (n = 1) is the
+    single-sequence loop of `generate` and the CLIs instead: it stops after min(max_tokens, seq_len - P) tokens, so it may fill
+    the context up to its last row. Rows up to P-1 are never written; row P is written by the forward
     of `token` (once on the batched path, once per choice, with the same values, on the sequential path). The single-sequence
     generator continues its stream afterwards. on_token(i, tok) is called for every generated token and returns True when
-    choice i is finished (end of sequence or stop string). `backend` provides next_token_at(token, pos, sampler),
+    choice i is finished (end of sequence or stop string). `backend` provides next_token(token, pos, sampler),
     forget_device_seed(), save_sampler() / restore_sampler(saved), and for the batched path batched_choices(n),
     seed_choices(seeds), choices_first(token, P, n, T, topp) and choices_step(tokens, P, C, j, active, T, topp)
     (InferenceSession and apps.runtime.RootInference). Returns each choice's tokens."""
@@ -49,7 +51,9 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     if not 1 <= n <= MAX_CHOICES:
         raise ValueError(f"n must be between 1 and {MAX_CHOICES}")
     C = (seq_len - 1 - P) // n
-    limit = C if max_tokens <= 0 else min(max_tokens, C)
+    limit = seq_len - P if n == 1 else C
+    if max_tokens > 0:
+        limit = min(max_tokens, limit)
     out: List[List[int]] = [[] for _ in range(n)]
     if limit <= 0:
         return out
@@ -58,7 +62,7 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
         # today's single-sequence path from P; rows past P belong to this sequence until the next one overwrites them
         tok, pos, done = token, P, set()
         while len(out[choices[0]]) < limit:
-            tok = backend.next_token_at(tok, pos, smp)
+            tok = backend.next_token(tok, pos, smp)
             pos += 1
             for i in choices:
                 if i not in done:
@@ -143,9 +147,13 @@ class InferenceSession:
         self.pos += 1
         return lg
 
-    def next_token(self, token: int) -> int:
-        """One decode step with host-visible result: H2D (token,pos) from pinned memory, forward + sampling, D2H."""
-        if self.sampler.temperature == 0.0:
+    def next_token(self, token: int, pos: Optional[int] = None, sampler=None) -> int:
+        """One decode step with host-visible result: H2D (token,pos) from pinned memory, forward + sampling, D2H. `pos` and
+        `sampler` default to the session's own; run_choices passes its own, as it does to apps.runtime.RootInference."""
+        if pos is not None:
+            self.pos = pos
+        smp = self.sampler if sampler is None else sampler
+        if smp.temperature == 0.0:
             self._pin_in[0] = token
             self._pin_in[1] = self.pos
             eng = self.engine
@@ -160,29 +168,20 @@ class InferenceSession:
         eng = self.engine
         if self.device.type == "cuda" and not getattr(eng, "_parts", False):
             # temperature / top-p on the device (csrc/cuda/sampler.cu): only the sampled token crosses PCIe
-            gen = (self.sampler.seed, self.sampler.seed_generation)
+            gen = (smp.seed, smp.seed_generation)
             if self._dev_seeded != gen:
-                eng.seed_sampler(self.sampler.seed)
+                eng.seed_sampler(smp.seed)
                 self._dev_seeded = gen
-            eng.step_sampled(token, self.pos, self.sampler.temperature, self.sampler.topp)
+            eng.step_sampled(token, self.pos, smp.temperature, smp.topp)
             self._pin_out.copy_(eng.tokens[:1], non_blocking=True)
             torch.cuda.current_stream().synchronize()
             eng.check_abort()
             self.pos += 1
             return int(self._pin_out[0])
         lg = self.forward_logits(token)
-        return int(self.sampler.sample(lg.float().cpu().numpy()))
+        return int(smp.sample(lg.float().cpu().numpy()))
 
     # ---- several completions of one prompt ----
-    def next_token_at(self, token: int, pos: int, sampler) -> int:
-        """next_token at an explicit position with an explicit sampler (the choices' sequential path)."""
-        saved = self.sampler
-        self.pos, self.sampler = pos, sampler
-        try:
-            return self.next_token(token)
-        finally:
-            self.sampler = saved
-
     def forget_device_seed(self):
         self._dev_seeded = None
 

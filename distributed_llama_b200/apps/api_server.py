@@ -133,14 +133,21 @@ class ApiServer:
     def __init__(self, ctx: AppContext):
         self.ctx = ctx
         self.cache = NaiveCache()
-        self.gen, self.det = make_chat_tools(ctx)
+        self.gen, _ = make_chat_tools(ctx)
         self.H = host()
+        eos_ids = list(ctx.tokenizer.eos_ids)
+        stops = [ctx.tokenizer.piece(i) for i in eos_ids]
+        pad = max((len(x) for x in stops), default=0)
+        self.detector_args = (eos_ids, stops, pad, pad)
 
     def complete(self, req: HttpRequest):
+        """n completions of one prompt (api.run_choices; n = 1 without `n`): the prompt is prefilled once. After one completion
+        the cache keeps its answer too; after several it keeps only the prompt messages, so a follow-up that quotes any one
+        choice reuses the prompt."""
         ctx, H = self.ctx, self.H
         tok, inf, h, smp = ctx.tokenizer, ctx.inference, ctx.header, ctx.sampler
         body = req.json or {}
-        n_choices = parse_n(body)
+        n = parse_n(body)
         messages = [(m["role"], m["content"]) for m in body["messages"]]
         stream = bool(body.get("stream", False))
         max_tokens = int(body.get("max_tokens", -1))
@@ -149,94 +156,32 @@ class ApiServer:
         if "seed" in body:
             smp.set_seed(int(body["seed"]))
         # several completions: choice i uses choice_seed(base, i); without a seed the base is drawn from the advancing generator
-        base_seed = smp.seed if "seed" in body else (smp.next_seed() if n_choices > 1 else 0)
+        base_seed = smp.seed if "seed" in body else (smp.next_seed() if n > 1 else 0)
         delta_prompt, start_pos = self.cache.resolve_delta_prompt(list(messages))
         content, public = self.gen.generate(delta_prompt, True)
         print(f"🔹{content.decode('utf-8', errors='replace')}🔸", end="")
         tokens = tok.encode(content, start_pos == 0, True)
         n_prompt = len(tokens)
         prompt_end = min(start_pos + n_prompt - 1, h.seq_len)
-        max_pred = min(prompt_end + max_tokens, h.seq_len) if max_tokens > 0 else h.seq_len
         for m in delta_prompt:
             self.cache.push(prompt_end, m)
-        if n_choices > 1:
-            self._complete_choices(req, n_choices, stream, public, tokens, start_pos, prompt_end, max_tokens, n_prompt, base_seed)
-            return
-        buffer = ""
-        if stream:
-            req.write_stream_start()
-        if public:
-            p = public.decode("utf-8", errors="replace")
-            if stream:
-                req.write_stream_chunk("data: " + chunk_json(p, False) + "\r\n\r\n")
-            buffer += p
-        pos = start_pos
-        n = prompt_end - pos
-        inf.prefill(tokens[:n], pos)
-        pos += n
-        token = tokens[n] if n < len(tokens) else tokens[-1]
-        tok.reset_decoder()
-        self.det.reset()
-        greedy = smp.temperature == 0.0
-        while pos < max_pred:
-            token = inf.next_token(token, pos, smp)
-            piece = tok.decode(token)
-            kind = self.det.append(token, piece)
-            if piece:
-                print(piece.decode("utf-8", errors="replace"), end="", flush=True)
-            if kind in (H.NOT_EOS, H.EOS):
-                delta = self.det.get_delta()
-                if delta:
-                    d = delta.decode("utf-8", errors="replace")
-                    if stream:
-                        req.write_stream_chunk("data: " + chunk_json(d, False) + "\r\n\r\n")
-                    buffer += d
-                self.det.reset()
-            pos += 1
-            if kind == H.EOS:
-                break
-        if pos == h.seq_len:
-            self.cache.clear()
-        else:
-            self.cache.push(pos, ("assistant", buffer))
-        if stream:
-            req.write_stream_chunk("data: " + chunk_json(None, True) + "\r\n\r\n")
-            req.write_stream_chunk("data: [DONE]")
-            req.write_stream_end()
-        else:
-            n_completion = pos - prompt_end
-            req.write_json(json.dumps({
-                "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
-                "usage": {"completion_tokens": n_completion, "prompt_tokens": n_prompt, "total_tokens": n_prompt + n_completion},
-                "choices": [{"index": 0, "message": {"role": "assistant", "content": buffer}, "finish_reason": "stop"}]}))
-        print("🔶")
-
-    def _complete_choices(self, req: HttpRequest, n: int, stream: bool, public: bytes, tokens, start_pos: int, prompt_end: int,
-                          max_tokens: int, n_prompt: int, base_seed: int):
-        """n completions of one prompt (api.run_choices): the prompt is prefilled once and the cache keeps only the prompt
-        messages, so a follow-up that quotes any one choice reuses the prompt."""
-        ctx, H = self.ctx, self.H
-        tok, inf, h = ctx.tokenizer, ctx.inference, ctx.header
-        eos_ids = list(tok.eos_ids)
-        stops = [tok.piece(i) for i in eos_ids]
-        pad = max((len(x) for x in stops), default=0)
-        dets = [H.EosDetector(eos_ids, stops, pad, pad) for _ in range(n)]
+        dets = [H.EosDetector(*self.detector_args) for _ in range(n)]
         decoders = [H.TokenDecoder() for _ in range(n)]
-        buffers = [""] * n
+        p = public.decode("utf-8", errors="replace")
+        buffers = [p] * n
         if stream:
             req.write_stream_start()
-        if public:
-            p = public.decode("utf-8", errors="replace")
-            for i in range(n):
-                if stream:
+            if p:
+                for i in range(n):
                     req.write_stream_chunk("data: " + chunk_json(p, False, i) + "\r\n\r\n")
-                buffers[i] += p
         n_pref = prompt_end - start_pos
         inf.prefill(tokens[:n_pref], start_pos)
         token = tokens[n_pref] if n_pref < len(tokens) else tokens[-1]
 
         def on_token(i: int, t: int) -> bool:
             piece = decoders[i].decode(tok, t)
+            if n == 1 and piece:
+                print(piece.decode("utf-8", errors="replace"), end="", flush=True)
             kind = dets[i].append(t, piece)
             if kind in (H.NOT_EOS, H.EOS):
                 delta = dets[i].get_delta()
@@ -248,19 +193,26 @@ class ApiServer:
                 dets[i].reset()
             return kind == H.EOS
 
-        out = run_choices(inf, token, prompt_end, n, max_tokens, h.seq_len, ctx.sampler, base_seed, on_token)
-        print(f"({n} choices)🔶")
+        out = run_choices(inf, token, prompt_end, n, max_tokens, h.seq_len, smp, base_seed, on_token)
+        if n == 1:
+            end = prompt_end + len(out[0])
+            if end == h.seq_len:
+                self.cache.clear()
+            else:
+                self.cache.push(end, ("assistant", buffers[0]))
         if stream:
             for i in range(n):
                 req.write_stream_chunk("data: " + chunk_json(None, True, i) + "\r\n\r\n")
             req.write_stream_chunk("data: [DONE]")
             req.write_stream_end()
-            return
-        n_completion = sum(len(o) for o in out)
-        req.write_json(json.dumps({
-            "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
-            "usage": {"completion_tokens": n_completion, "prompt_tokens": n_prompt, "total_tokens": n_prompt + n_completion},
-            "choices": [{"index": i, "message": {"role": "assistant", "content": buffers[i]}, "finish_reason": "stop"} for i in range(n)]}))
+        else:
+            n_completion = sum(len(o) for o in out)
+            req.write_json(json.dumps({
+                "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
+                "usage": {"completion_tokens": n_completion, "prompt_tokens": n_prompt, "total_tokens": n_prompt + n_completion},
+                "choices": [{"index": i, "message": {"role": "assistant", "content": b}, "finish_reason": "stop"}
+                            for i, b in enumerate(buffers)]}))
+        print("🔶" if n == 1 else f"({n} choices)🔶")
 
     def models(self, req: HttpRequest):
         name = self.ctx.args.model.replace("\\", "/").split("/")[-1]

@@ -180,9 +180,6 @@ class RootInference:
         return int(sampler.sample(self.forward_logits(token, pos).float().cpu().numpy()))
 
     # ---- several completions of one prompt (api.run_choices); workers mirror every batched step ----
-    def next_token_at(self, token: int, pos: int, sampler) -> int:
-        return self.next_token(token, pos, sampler)
-
     def forget_device_seed(self):
         self._seeded = None
 

@@ -1,8 +1,8 @@
-// CPU-only harness for the `n` (several completions) path of csrc/app/api_server.cpp: the real HTTP / JSON / chat-template / stop-detector / NaiveCache code over a
-// deterministic fake model (next token = a fixed function of (token, position); emits EOS after `--eos-after` tokens). With a
+// CPU-only harness for csrc/app/api_server.cpp: the real HTTP / JSON / chat-template / stop-detector / NaiveCache code over a
+// deterministic fake model (next token = a fixed function of (token, position); emits EOS after `eos-after` tokens). With a
 // temperature above 0 the token also depends on the sampler's seed, so the choices of an `n` request differ, and EOS comes
-// `--eos-after` positions after the prefilled prompt, so every choice of the sequential path gets the same length.
-// Prints "POS <start> <n>" for every prefill so the test can check the prefix re-use of NaiveCache.
+// `eos-after` positions after the prefilled prompt, so every choice of the sequential path gets the same length.
+// Prints "POS <start> <n>" for every prefill so the tests can check the prefix re-use of NaiveCache.
 #include <cstdio>
 #include <cstdlib>
 #include <string>
@@ -33,12 +33,12 @@ struct StubBackend : InferenceBackend {
 };
 
 int main(int argc, char **argv) {
-    if (argc < 4) { std::fprintf(stderr, "usage: api_stub <tokenizer.t> <port> <max-requests> [eos-after]\n"); return 2; }
+    if (argc < 4) { std::fprintf(stderr, "usage: api_stub <tokenizer.t> <port> <max-requests> [eos-after] [seq-len]\n"); return 2; }
     Tokenizer tok(argv[1]);
     StubBackend b;
     b.vocab = tok.vocabSize();
     b.regular = tok.regularVocabSize();
-    b.seq = 4096;
+    b.seq = argc > 5 ? (uint32_t)std::atoi(argv[5]) : 4096;
     b.eos = tok.data().eosIds.at(0);
     b.eosAfter = argc > 4 ? (uint32_t)std::atoi(argv[4]) : 12;
     ApiConfig cfg;

@@ -1,5 +1,5 @@
 """Native API server (csrc/app/api_server.cpp) end to end on CPU: real sockets, HTTP parsing, JSON in/out, chat template, stop
-detection, SSE streaming and NaiveCache prefix re-use over a deterministic stub model (tests/native/api_stub_main.cpp)."""
+detection, SSE streaming and NaiveCache prefix re-use over a deterministic stub model (tests/native/api_choices_stub_main.cpp)."""
 import http.client
 import json
 import os
@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 def stub(tmp_path_factory):
     d = tmp_path_factory.mktemp("api_stub")
     exe = str(d / "api_stub")
-    srcs = [os.path.join(ROOT, "tests", "native", "api_stub_main.cpp"), os.path.join(ROOT, "csrc", "app", "api_server.cpp"),
+    srcs = [os.path.join(ROOT, "tests", "native", "api_choices_stub_main.cpp"), os.path.join(ROOT, "csrc", "app", "api_server.cpp"),
             os.path.join(ROOT, "csrc", "host", "text.cpp")]
     subprocess.run(["g++", "-O1", "-std=c++17", "-Wall", "-Wno-sign-compare", *srcs, "-o", exe], check=True)
     from distributed_llama_b200.models.synthetic import write_synthetic_tokenizer
