@@ -629,6 +629,15 @@ DL_EXPORT int dl_attn_decode(const float *qkv, uint32_t qkvStride, const int *po
     return dl::launchAttnDecode(a, nb, stream, false);
 }
 
+// Router of T tokens (tests/test_gpu_moe.py): logits [T][nExperts], expertIdx / expertWeight [T][k]; counter [T] zeroed, self-resetting.
+DL_EXPORT int dl_moe_router(const float *x, const float *normW, const float *gate, float eps, uint32_t dim, uint32_t nExperts, uint32_t k,
+                            float *logits, unsigned int *counter, int *expertIdx, float *expertWeight, int T, cudaStream_t stream) {
+    dl::RouterArgs a{};
+    a.x = x; a.normW = normW; a.gate = gate; a.eps = eps; a.dim = dim; a.nExperts = nExperts; a.k = k;
+    a.logits = logits; a.counter = counter; a.expertIdx = expertIdx; a.expertWeight = expertWeight;
+    return dl::launchMoeRouter(a, T, stream, false);
+}
+
 DL_EXPORT int dl_attn_fused(const float *qkv, const int *pos, const float *rope, const float *qNorm, const float *kNorm, float eps,
                             void *kCache, void *vCache, uint32_t nHeads, uint32_t nKvHeads, uint32_t headDim, uint32_t seqLen,
                             uint32_t nSplits, float *partial, unsigned int *counters, float *out, cudaStream_t stream) {

@@ -91,34 +91,66 @@ static int gemvSel(const Engine &e, int pro, int epi, int nb, const GemvArgs &a,
     return e.useTma ? gemvQ40Auto(pro, epi, nb, a, numSms, stream, pdl) : gemvQ40(pro, epi, nb, a, numSms, stream, pdl);
 }
 
-// Mixture-of-experts feed-forward of one token: router -> k x (W1|W3 -> silu*up) -> k x W2; the weighted expert sum is
-// *added* to `out` (the residual stream, or a zeroed partial buffer on the NCCL path), all-reduced in the epilogue if asked.
+// Mixture-of-experts feed-forward of one token, all buffers explicit (the engine's and those of tests/test_gpu_moe.py).
+struct MoeDecodeArgs {
+    const float *x;                       // [dim] residual stream (router and W1|W3 input)
+    float *out;                           // [dim] the weighted expert sum is added here
+    const float *norm, *gate;             // ffn rms-norm weight [dim], router gate [nExperts][dim] f32
+    const void *w13Qs, *w13Sc, *w2Qs, *w2Sc;   // [nLocal][2*ff][dim] gate/up interleaved, [nLocal][dim][ff]
+    uint32_t dim, ff, nExperts, k, firstLocal, nLocal;
+    float eps;
+    float *routerLogits;                  // [nExperts]
+    unsigned int *routerCounter;          // [1], zero-initialised, self-resetting
+    int *expertIdx;                       // [k]
+    float *expertWeight;                  // [k]
+    float *h;                             // [k][ff] SwiGLU output per routing slot
+    float *moeScratch;                    // [k][dim] weighted per-slot products
+    unsigned int *moeCounters;            // [numSms / k], zero-initialised, self-resetting
+    uint32_t numSms;                      // CTAs per routing slot = numSms / k (at least 1)
+    uint64_t *trace13, *trace2;
+    ArArgs ar;                            // nRanks > 1: all-reduce in the W2 epilogue
+};
+
+// router -> k x (W1|W3 -> silu*up) -> k x W2; the weighted expert sum is *added* to `out`.
+static int moeDecodeFfn(const MoeDecodeArgs &m, cudaStream_t stream, bool pdl) {
+    RouterArgs ro{};
+    ro.x = m.x; ro.normW = m.norm; ro.gate = m.gate; ro.eps = m.eps; ro.dim = m.dim; ro.nExperts = m.nExperts;
+    ro.k = m.k; ro.logits = m.routerLogits; ro.counter = m.routerCounter; ro.expertIdx = m.expertIdx; ro.expertWeight = m.expertWeight;
+    DL_TRY(launchMoeRouter(ro, 1, stream, pdl));
+    const uint32_t perSlot = m.numSms / m.k > 0 ? m.numSms / m.k : 1;
+    GemvArgs a{};
+    a.qs = (const uint32_t *)m.w13Qs; a.scales = (const __half *)m.w13Sc; a.d = 2 * m.ff; a.n = m.dim;
+    a.in = m.x; a.inStride = m.dim; a.normW = m.norm; a.eps = m.eps; a.out = m.h; a.outStride = m.ff; a.trace = m.trace13;
+    a.moeCtasPerSlot = perSlot; a.kActive = m.k; a.expertIdx = m.expertIdx; a.outSlotStride = m.ff;
+    a.expertQsStride = (uint64_t)2 * m.ff * (m.dim / 8); a.expertScaleStride = (uint64_t)2 * m.ff * (m.dim / 32);
+    a.moeFirstExpert = m.firstLocal; a.moeNumLocal = m.nLocal;
+    { const int r = gemvQ40Tma(PRO_RMSNORM_, EPI_SWIGLU_, 1, a, (int)m.numSms, stream, pdl); if (r != 0) return r == 1 ? -31 : r; }
+    a = GemvArgs{};
+    a.qs = (const uint32_t *)m.w2Qs; a.scales = (const __half *)m.w2Sc; a.d = m.dim; a.n = m.ff;
+    a.in = m.h; a.inStride = m.ff; a.inSlotStride = m.ff; a.out = m.out; a.outStride = m.dim; a.trace = m.trace2;
+    a.moeCtasPerSlot = perSlot; a.kActive = m.k; a.expertIdx = m.expertIdx; a.expertWeight = m.expertWeight;
+    a.expertQsStride = (uint64_t)m.dim * (m.ff / 8); a.expertScaleStride = (uint64_t)m.dim * (m.ff / 32);
+    a.moeFirstExpert = m.firstLocal; a.moeNumLocal = m.nLocal; a.moeScratch = m.moeScratch; a.moeCounters = m.moeCounters;
+    a.ar = m.ar;
+    { const int r = gemvQ40Tma(PRO_PLAIN_, EPI_MOE_DOWN_, 1, a, (int)m.numSms, stream, pdl); if (r != 0) return r == 1 ? -32 : r; }
+    return 0;
+}
+
+// Mixture-of-experts feed-forward of the engine's token: the weighted expert sum is *added* to `out` (the residual stream, or a
+// zeroed partial buffer on the NCCL path), all-reduced in the epilogue if asked.
 static int runMoe(Engine &e, const LayerPtrs &L, float *out, bool fusedAr, uint64_t *trace13, uint64_t *trace2, cudaStream_t stream,
                   bool pdl) {
     const EngineConfig &c = e.cfg;
     if (c.wType != 0) return -34;   // expert-indexed kernels exist for q40 matrices only
-    RouterArgs ro{};
-    ro.x = e.g.x; ro.normW = L.norm1; ro.gate = L.moeGate; ro.eps = c.eps; ro.dim = c.dim; ro.nExperts = c.nExperts;
-    ro.k = c.nActiveExperts; ro.logits = e.g.routerLogits; ro.counter = e.g.routerCounter; ro.expertIdx = e.g.expertIdx;
-    ro.expertWeight = e.g.expertWeight;
-    DL_TRY(launchMoeRouter(ro, 1, stream, pdl));
-    const uint32_t perSlot = c.numSms / c.nActiveExperts > 0 ? c.numSms / c.nActiveExperts : 1;
-    GemvArgs a{};
-    a.qs = (const uint32_t *)L.w13Qs; a.scales = (const __half *)L.w13Sc; a.d = 2 * c.ffDim; a.n = c.dim;
-    a.in = e.g.x; a.inStride = c.dim; a.normW = L.norm1; a.eps = c.eps; a.out = e.g.h; a.outStride = c.ffDim; a.trace = trace13;
-    a.moeCtasPerSlot = perSlot; a.kActive = c.nActiveExperts; a.expertIdx = e.g.expertIdx; a.outSlotStride = c.ffDim;
-    a.expertQsStride = (uint64_t)2 * c.ffDim * (c.dim / 8); a.expertScaleStride = (uint64_t)2 * c.ffDim * (c.dim / 32);
-    a.moeFirstExpert = c.moeFirstExpert; a.moeNumLocal = c.moeNumLocal;
-    { const int r = gemvQ40Tma(PRO_RMSNORM_, EPI_SWIGLU_, 1, a, c.numSms, stream, pdl); if (r != 0) return r == 1 ? -31 : r; }
-    a = GemvArgs{};
-    a.qs = (const uint32_t *)L.w2Qs; a.scales = (const __half *)L.w2Sc; a.d = c.dim; a.n = c.ffDim;
-    a.in = e.g.h; a.inStride = c.ffDim; a.inSlotStride = c.ffDim; a.out = out; a.outStride = c.dim; a.trace = trace2;
-    a.moeCtasPerSlot = perSlot; a.kActive = c.nActiveExperts; a.expertIdx = e.g.expertIdx; a.expertWeight = e.g.expertWeight;
-    a.expertQsStride = (uint64_t)c.dim * (c.ffDim / 8); a.expertScaleStride = (uint64_t)c.dim * (c.ffDim / 32);
-    a.moeFirstExpert = c.moeFirstExpert; a.moeNumLocal = c.moeNumLocal; a.moeScratch = e.g.moeScratch; a.moeCounters = e.g.moeCounters;
-    if (fusedAr) fillAr(e, a.ar, 1);
-    { const int r = gemvQ40Tma(PRO_PLAIN_, EPI_MOE_DOWN_, 1, a, c.numSms, stream, pdl); if (r != 0) return r == 1 ? -32 : r; }
-    return 0;
+    MoeDecodeArgs m{};
+    m.x = e.g.x; m.out = out; m.norm = L.norm1; m.gate = L.moeGate;
+    m.w13Qs = L.w13Qs; m.w13Sc = L.w13Sc; m.w2Qs = L.w2Qs; m.w2Sc = L.w2Sc;
+    m.dim = c.dim; m.ff = c.ffDim; m.nExperts = c.nExperts; m.k = c.nActiveExperts; m.firstLocal = c.moeFirstExpert; m.nLocal = c.moeNumLocal;
+    m.eps = c.eps; m.routerLogits = e.g.routerLogits; m.routerCounter = e.g.routerCounter; m.expertIdx = e.g.expertIdx;
+    m.expertWeight = e.g.expertWeight; m.h = e.g.h; m.moeScratch = e.g.moeScratch; m.moeCounters = e.g.moeCounters; m.numSms = c.numSms;
+    m.trace13 = trace13; m.trace2 = trace2;
+    if (fusedAr) fillAr(e, m.ar, 1);
+    return moeDecodeFfn(m, stream, pdl);
 }
 
 // One token through the persistent kernel (dense models, nb == 1). Returns 1 when the shape is not supported.
@@ -663,6 +695,22 @@ DL_EXPORT int dl_engine_forward_part(void *h, int nb, uint32_t layer, int part, 
 DL_EXPORT int dl_engine_choices_forward(void *h, int nb, uint32_t P, uint32_t C, uint32_t j, uint32_t inactiveMask, cudaStream_t stream) {
     const dl::ChoiceStep ch{P, C, j, inactiveMask};
     return dl::engineForward(*(Engine *)h, nb, 2, false, stream, &ch);
+}
+
+// Decode mixture-of-experts feed-forward of one token on one rank (tests/test_gpu_moe.py): the engine's launch sequence with the
+// caller's buffers (see MoeDecodeArgs) and the gate activation passed explicitly (0 = SiLU, 1 = GELU). No programmatic dependent launch.
+DL_EXPORT int dl_moe_decode_ffn(const float *x, float *out, const float *norm, const float *gate, const void *w13Qs, const void *w13Sc,
+                                const void *w2Qs, const void *w2Sc, uint32_t dim, uint32_t ff, uint32_t nExperts, uint32_t k,
+                                uint32_t firstLocal, uint32_t nLocal, float eps, float *routerLogits, unsigned int *routerCounter,
+                                int *expertIdx, float *expertWeight, float *hOut, float *moeScratch, unsigned int *moeCounters,
+                                uint32_t numSms, uint32_t hiddenAct, cudaStream_t stream) {
+    dl::MoeDecodeArgs m{};
+    m.x = x; m.out = out; m.norm = norm; m.gate = gate; m.w13Qs = w13Qs; m.w13Sc = w13Sc; m.w2Qs = w2Qs; m.w2Sc = w2Sc;
+    m.dim = dim; m.ff = ff; m.nExperts = nExperts; m.k = k; m.firstLocal = firstLocal; m.nLocal = nLocal; m.eps = eps;
+    m.routerLogits = routerLogits; m.routerCounter = routerCounter; m.expertIdx = expertIdx; m.expertWeight = expertWeight;
+    m.h = hOut; m.moeScratch = moeScratch; m.moeCounters = moeCounters; m.numSms = numSms;
+    const dl::HiddenActScope act(hiddenAct);
+    return dl::moeDecodeFfn(m, stream, false);
 }
 
 DL_EXPORT int dl_engine_prefill(void *h, uint32_t T, uint32_t p0, int wantLogits, cudaStream_t stream) {

@@ -1053,6 +1053,16 @@ DL_EXPORT int dl_gemm_q40_tc(int epi, const void *qs, const void *scales, uint32
     return dl::gemmQ40TcV(epi, qs, scales, d, n, act, actStride, T, out, outStride, numSms, stream, pdl != 0, variant, nullptr);
 }
 
+// Grouped mode for the unit tests (tests/test_gpu_moe.py): gemmQ40TcGrouped with caller-provided device arrays grpCount /
+// grpOffset [nGroups] and the gate activation of GEPI_SWIGLU_BF16 passed explicitly (0 = SiLU, 1 = GELU).
+DL_EXPORT int dl_gemm_q40_tc_grouped(int epi, const void *qs, const void *scales, uint32_t nGroups, uint32_t grpRows, uint32_t n, const void *act,
+                                     uint32_t actStride, uint32_t rowsTotal, uint32_t maxTokens, const int *grpCount, const int *grpOffset,
+                                     void *out, uint32_t outStride, int numSms, uint32_t hiddenAct, cudaStream_t stream) {
+    const dl::HiddenActScope a(hiddenAct);
+    return dl::gemmQ40TcGrouped(epi, qs, scales, nGroups, grpRows, n, act, actStride, rowsTotal, maxTokens, grpCount, grpOffset, out,
+                                outStride, numSms, stream);
+}
+
 DL_EXPORT int dl_rmsnorm_bf16(const float *x, uint32_t xStride, const float *w, void *y, uint32_t yStride, uint32_t n, float eps,
                               uint32_t T, cudaStream_t stream) {
     return dl::launchRmsNormBf16(x, xStride, w, y, yStride, n, eps, T, stream);

@@ -11,6 +11,14 @@ enum { EPI_STORE_ = 0, EPI_RESIDUAL_ = 1, EPI_SWIGLU_ = 2, EPI_ARGMAX_ = 3, EPI_
 constexpr int kMaxRanks = 8;
 extern uint32_t gHiddenAct;   // process-wide gate activation (0 = SiLU, 1 = GELU), set by dl_engine_create from the model header
 
+// Sets gHiddenAct for the launches of one stand-alone entry point and restores the engine's value afterwards (the launchers read
+// it on the host when they fill the kernel arguments).
+struct HiddenActScope {
+    uint32_t saved;
+    explicit HiddenActScope(uint32_t act) : saved(gHiddenAct) { gHiddenAct = act; }
+    ~HiddenActScope() { gHiddenAct = saved; }
+};
+
 struct ArArgs {
     uint32_t nRanks, rank, parity, maxCtas;
     uint32_t slotStride;          // words per (parity, source rank) slot = maxBatch * dim

@@ -6,6 +6,8 @@
 // (token, expert) pair. Here the (token, expert) pairs of the whole chunk are sorted by expert so every expert's weights are read
 // once per chunk and multiplied on the tensor cores (gemmQ40TcGrouped): dispatch = a gather into expert-sorted rows, combine = a
 // deterministic weighted sum per token in routing-slot order, pushed to every rank through LL words when experts are sharded.
+#include <algorithm>
+
 #include "kernels.h"
 
 namespace dl {
@@ -138,13 +140,17 @@ struct MoeScratch {
     unsigned int *routerCounter = nullptr;
     __nv_bfloat16 *xs = nullptr, *hs = nullptr;
     float *ys = nullptr;
-    size_t capPairs = 0, capDim = 0, capFf = 0, capExperts = 0;
+    size_t capPairs = 0, capDim = 0, capFf = 0, capExperts = 0, capTokens = 0;
 };
 MoeScratch gMoe;
 
+// The router scratch is [T][nExperts] logits + [T] counters, so the token count is a capacity of its own: a chunk with more
+// tokens but fewer pairs per token (smaller k) than an earlier one must still reallocate. Capacities only grow.
 int moeEnsureScratch(uint32_t nPairs, uint32_t dim, uint32_t ff, uint32_t nExperts, uint32_t T) {
     MoeScratch &m = gMoe;
-    if (nPairs <= m.capPairs && dim <= m.capDim && ff <= m.capFf && nExperts <= m.capExperts) return 0;
+    if (nPairs <= m.capPairs && dim <= m.capDim && ff <= m.capFf && nExperts <= m.capExperts && T <= m.capTokens) return 0;
+    nPairs = std::max(nPairs, (uint32_t)m.capPairs); dim = std::max(dim, (uint32_t)m.capDim); ff = std::max(ff, (uint32_t)m.capFf);
+    nExperts = std::max(nExperts, (uint32_t)m.capExperts); T = std::max(T, (uint32_t)m.capTokens);
     for (void *p : {(void *)m.count, (void *)m.offset, (void *)m.slotOfPair, (void *)m.tokenOfSlot, (void *)m.totalRows, (void *)m.expertIdx,
                     (void *)m.expertWeight, (void *)m.routerLogits, (void *)m.routerCounter, (void *)m.xs, (void *)m.hs, (void *)m.ys})
         if (p) cudaFree(p);
@@ -159,7 +165,7 @@ int moeEnsureScratch(uint32_t nPairs, uint32_t dim, uint32_t ff, uint32_t nExper
     DL_CUDA_CHECK(cudaMalloc(&m.xs, (P + 256) * dim * 2)); DL_CUDA_CHECK(cudaMemset(m.xs, 0, (P + 256) * dim * 2));
     DL_CUDA_CHECK(cudaMalloc(&m.hs, (P + 256) * ff * 2)); DL_CUDA_CHECK(cudaMemset(m.hs, 0, (P + 256) * ff * 2));
     DL_CUDA_CHECK(cudaMalloc(&m.ys, P * dim * 4));
-    m.capPairs = nPairs; m.capDim = dim; m.capFf = ff; m.capExperts = nExperts;
+    m.capPairs = nPairs; m.capDim = dim; m.capFf = ff; m.capExperts = nExperts; m.capTokens = T;
     return 0;
 }
 
@@ -198,3 +204,21 @@ int moePrefillFfn(const MoePrefillArgs &a, cudaStream_t stream) {
 }
 
 }  // namespace dl
+
+// Stand-alone entry point for the unit tests (tests/test_gpu_moe.py): moePrefillFfn on one rank, with the gate activation passed
+// explicitly (0 = SiLU, 1 = GELU) instead of the one of the last engine created. The routing the call used (expert id and weight
+// of every pair, [T][k]) is copied to expertIdxOut / expertWeightOut.
+DL_EXPORT int dl_moe_prefill_ffn(float *x, void *xnScratch, const float *norm, const float *gate, const void *w13Qs, const void *w13Sc,
+                                 const void *w2Qs, const void *w2Sc, uint32_t T, uint32_t dim, uint32_t ff, uint32_t nExperts, uint32_t k,
+                                 uint32_t firstLocal, uint32_t nLocal, float eps, int numSms, uint32_t hiddenAct, int *expertIdxOut,
+                                 float *expertWeightOut, cudaStream_t stream) {
+    dl::MoePrefillArgs a{};
+    a.x = x; a.xnScratch = xnScratch; a.norm = norm; a.gate = gate; a.w13Qs = w13Qs; a.w13Sc = w13Sc; a.w2Qs = w2Qs; a.w2Sc = w2Sc;
+    a.T = T; a.dim = dim; a.ff = ff; a.nExperts = nExperts; a.k = k; a.firstLocal = firstLocal; a.nLocal = nLocal; a.eps = eps; a.numSms = numSms;
+    const dl::HiddenActScope act(hiddenAct);
+    const int r = dl::moePrefillFfn(a, stream);
+    if (r != 0) return r;
+    DL_CUDA_CHECK(cudaMemcpyAsync(expertIdxOut, dl::gMoe.expertIdx, (size_t)T * k * sizeof(int), cudaMemcpyDeviceToDevice, stream));
+    DL_CUDA_CHECK(cudaMemcpyAsync(expertWeightOut, dl::gMoe.expertWeight, (size_t)T * k * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+    return 0;
+}

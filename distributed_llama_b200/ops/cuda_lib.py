@@ -68,6 +68,14 @@ def lib() -> C.CDLL:
     L.dl_attn_decode.restype = i32
     L.dl_attn_fused.argtypes = [vp, vp, vp, vp, vp, f32, vp, vp, u32, u32, u32, u32, u32, vp, vp, vp, vp]
     L.dl_attn_fused.restype = i32
+    L.dl_moe_router.argtypes = [vp, vp, vp, f32, u32, u32, u32, vp, vp, vp, vp, i32, vp]
+    L.dl_moe_router.restype = i32
+    L.dl_gemm_q40_tc_grouped.argtypes = [i32, vp, vp, u32, u32, u32, vp, u32, u32, u32, vp, vp, vp, u32, i32, u32, vp]
+    L.dl_gemm_q40_tc_grouped.restype = i32
+    L.dl_moe_prefill_ffn.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, u32, u32, u32, u32, u32, f32, i32, u32, vp, vp, vp]
+    L.dl_moe_prefill_ffn.restype = i32
+    L.dl_moe_decode_ffn.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, u32, u32, u32, u32, f32, vp, vp, vp, vp, vp, vp, vp, u32, u32, vp]
+    L.dl_moe_decode_ffn.restype = i32
     L.dl_engine_create.argtypes = [C.POINTER(EngineConfig)]
     L.dl_engine_create.restype = vp
     L.dl_engine_destroy.argtypes = [vp]
