@@ -154,6 +154,7 @@ std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t 
     uint32_t limit = n == 1 ? (P < seqLen ? seqLen - P : 0) : C;
     if (maxTokens > 0) limit = std::min<uint32_t>((uint32_t)maxTokens, limit);
     if (limit == 0) return out;
+    sampler.beginCompletion();
     // today's single-sequence path from P for the choices in [first, last]; they all see the same tokens
     const auto single = [&](Sampler &smp, uint32_t first, uint32_t last) {
         int32_t tok = token;
@@ -180,13 +181,15 @@ std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t 
     if (!backend.batchedChoices(n)) {
         const uint64_t saved = backend.saveSampler();
         for (uint32_t i = 0; i < n; i++) {
-            Sampler smp(sampler.vocabSize(), T, topp, seeds[i]);
+            Sampler smp(sampler.vocabSize(), T, topp, seeds[i]);   // a fresh sampler: its own counts, from zero
+            smp.setControls(sampler.presencePenalty(), sampler.frequencyPenalty(), sampler.logitBias());
             single(smp, i, i);
         }
         backend.restoreSampler(saved);
         return out;
     }
     backend.seedChoices(seeds);
+    backend.choiceControls(sampler, n);
     std::vector<int32_t> last = backend.choicesFirst(token, P, n, T, topp);
     uint32_t active = (1u << n) - 1u;
     for (uint32_t j = 0;; j++) {
@@ -214,7 +217,39 @@ int maxLen(const std::vector<std::string> &v) {
     for (const std::string &s : v) m = std::max(m, s.size());
     return (int)m;
 }
+float boundedNumber(const JsonValue &v, double limit, const char *what) {
+    if (v.kind != JsonValue::Number || !(v.num >= -limit && v.num <= limit))
+        throw std::runtime_error(std::string("'") + what + "' must be a number from " + std::to_string((int)-limit) + " to " + std::to_string((int)limit));
+    return (float)v.num;
+}
+// The request's sampling controls; same rules as distributed_llama_b200.apps.api_server.parse_controls: penalties are numbers in
+// [-2, 2] (absent: the server's defaults); logit_bias is an object of at most 100 entries whose keys are decimal token ids in
+// [0, vocab) without leading zeros and whose values are numbers in [-100, 100]. A repeated key keeps its last value.
+void parseControls(const JsonValue &body, uint32_t vocab, float &presence, float &frequency, std::vector<std::pair<int32_t, float>> &bias) {
+    if (const JsonValue *v = body.find("presence_penalty")) presence = boundedNumber(*v, kMaxPenalty, "presence_penalty");
+    if (const JsonValue *v = body.find("frequency_penalty")) frequency = boundedNumber(*v, kMaxPenalty, "frequency_penalty");
+    bias.clear();
+    const JsonValue *b = body.find("logit_bias");
+    if (!b) return;
+    if (!b->isObject()) throw std::runtime_error("'logit_bias' must be an object");
+    std::map<int32_t, float> byId;
+    for (const auto &kv : b->obj) {
+        const std::string &k = kv.first;
+        bool ok = !k.empty() && k.size() <= 10 && (k[0] != '0' || k.size() == 1);
+        for (char c : k) ok = ok && c >= '0' && c <= '9';
+        if (!ok || std::stoull(k) >= vocab) throw std::runtime_error("'logit_bias' keys must be token ids below the vocabulary size");
+        byId[(int32_t)std::stoull(k)] = boundedNumber(kv.second, kMaxLogitBias, "logit_bias");
+    }
+    if (byId.size() > kMaxLogitBiasEntries) throw std::runtime_error("'logit_bias' has more than 100 entries");
+    bias.assign(byId.begin(), byId.end());
+}
 }  // namespace
+
+float parsePenalty(const std::string &flag, const std::string &value) {
+    const float v = std::stof(value);
+    if (!(v >= -kMaxPenalty && v <= kMaxPenalty)) throw std::runtime_error(flag + " must be from -2 to 2");
+    return v;
+}
 
 ApiServer::ApiServer(InferenceBackend &backend, Tokenizer &tokenizer, const ApiConfig &cfg)
     : backend_(backend), tok_(tokenizer), cfg_(cfg), sampler_(std::min<uint32_t>(backend.vocabSize(), tokenizer.vocabSize()), cfg.temperature, cfg.topp, cfg.seed),
@@ -244,6 +279,10 @@ void ApiServer::complete(HttpRequest &req) {
             throw std::runtime_error("'n' must be an integer from 1 to 8");
         n = (uint32_t)v->num;
     }
+    float presence = cfg_.presencePenalty, frequency = cfg_.frequencyPenalty;
+    std::vector<std::pair<int32_t, float>> bias;
+    parseControls(body, sampler_.vocabSize(), presence, frequency, bias);
+    sampler_.setControls(presence, frequency, bias);
     bool seeded = false;
     if (const JsonValue *s = body.find("seed")) if (s->kind == JsonValue::Number) { sampler_.setSeed((uint64_t)s->num); seeded = true; }
     // several completions: choice i uses choiceSeed(base, i); without a seed the base is drawn from the advancing generator

@@ -24,6 +24,8 @@ struct InferenceBackend {
     // Several completions of one prompt (runChoices). Without a batched path the choices run one after another through next().
     virtual bool batchedChoices(uint32_t /*n*/) const { return false; }
     virtual void seedChoices(const std::vector<uint64_t> & /*seeds*/) {}
+    // the sampler's controls for the batched choices, each choice's counts from zero
+    virtual void choiceControls(const Sampler & /*sampler*/, uint32_t /*n*/) {}
     // first tokens of n choices, all drawn from the logits of `token` at P
     virtual std::vector<int32_t> choicesFirst(int32_t /*token*/, uint32_t /*P*/, uint32_t /*n*/, float /*temperature*/, float /*topp*/) { return {}; }
     // one batched step: choice b feeds tokens[b] at rotary position P + 1 + j, cache row P + 1 + b * C + j (active choices only)
@@ -40,7 +42,8 @@ constexpr uint32_t kMaxChoices = 8;   // the engine's widest batch: one row per 
 // choiceSeed(baseSeed, i), its j-th token has rotary position P + 1 + j and cache row P + 1 + i * C + j with
 // C = (seqLen - 1 - P) / n, and it stops after min(maxTokens, C) tokens (maxTokens <= 0: C). A single completion (n = 1) is the
 // single-sequence loop of the CLIs instead: it stops after min(maxTokens, seqLen - P) tokens, so it may fill the context up to
-// its last row. onToken(i, token) returns true when choice i is finished. Same rules as distributed_llama_b200.api.run_choices.
+// its last row. onToken(i, token) returns true when choice i is finished. The sampler's controls apply to every choice, each with
+// its own counts from zero. Same rules as distributed_llama_b200.api.run_choices.
 std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t token, uint32_t P, uint32_t n, int maxTokens, uint32_t seqLen,
                                              Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken);
 
@@ -77,10 +80,14 @@ private:
 
 std::string chunkJson(const std::string *delta, bool stop, uint32_t index = 0);   // one streamed `chat.completion` chunk
 
+// A --presence-penalty / --frequency-penalty value: a number in [-kMaxPenalty, kMaxPenalty] (throws otherwise).
+float parsePenalty(const std::string &flag, const std::string &value);
+
 struct ApiConfig {
     std::string host = "0.0.0.0", modelName = "model", chatTemplate;
     int port = 9990;
     float temperature = 0.8f, topp = 0.9f;
+    float presencePenalty = 0.f, frequencyPenalty = 0.f;   // defaults of the request fields
     uint64_t seed = 0;
     int maxRequests = 0;   // 0 = serve forever
 };

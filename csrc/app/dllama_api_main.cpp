@@ -29,6 +29,7 @@ struct EngineBackend : InferenceBackend {
     // choices: one batched step per token on dense models; the sequential fallback (MoE) keeps the device generator's stream
     bool batchedChoices(uint32_t n) const override { return e.supportsChoices(n); }
     void seedChoices(const std::vector<uint64_t> &seeds) override { tp.seedChoices(seeds); }
+    void choiceControls(const Sampler &sampler, uint32_t n) override { tp.choiceControls(sampler, n); }
     std::vector<int32_t> choicesFirst(int32_t token, uint32_t P, uint32_t n, float temperature, float topp) override {
         return tp.choicesFirst(token, P, n, temperature, topp);
     }
@@ -42,7 +43,8 @@ struct EngineBackend : InferenceBackend {
 
 const char *kUsage =
     "Usage: dllama-api-native --model <path> --tokenizer <path> [--host <addr>] [--port <p>] [--max-seq-len <n>]\n"
-    "        [--temperature <t>] [--topp <p>] [--seed <s>] [--chat-template {llama2|llama3|deepSeek3|chatml}] [--gpu-index <i>]\n"
+    "        [--temperature <t>] [--topp <p>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]\n"
+    "        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--gpu-index <i>]\n"
     "        [--gpus <n>]   tensor parallel over n GPUs: a supervisor forks one process per GPU (rank 0 serves HTTP) and restarts\n"
     "                       the whole job 3 s after any rank fails\n";
 
@@ -85,6 +87,8 @@ int main(int argc, char **argv) {
             else if (name == "--max-seq-len") maxSeqLen = (uint32_t)std::stoul(v);
             else if (name == "--temperature") cfg.temperature = std::stof(v);
             else if (name == "--topp") cfg.topp = std::stof(v);
+            else if (name == "--presence-penalty") cfg.presencePenalty = parsePenalty(name, v);
+            else if (name == "--frequency-penalty") cfg.frequencyPenalty = parsePenalty(name, v);
             else if (name == "--seed") cfg.seed = std::stoull(v);
             else if (name == "--chat-template") cfg.chatTemplate = v;
             else if (name == "--gpu-index") gpu = std::max(0, std::stoi(v));

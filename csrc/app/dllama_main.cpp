@@ -30,6 +30,7 @@
 #include <vector>
 
 #include "../host/text.hpp"
+#include "api_server.hpp"
 #include "native_engine.hpp"
 #include "tp_job.hpp"
 
@@ -42,6 +43,7 @@ struct Args {
     bool hasPrompt = false, help = false;
     uint32_t steps = 0, maxSeqLen = 0;
     float temperature = 0.8f, topp = 0.9f;
+    float presencePenalty = 0.f, frequencyPenalty = 0.f;
     uint64_t seed = (uint64_t)std::time(nullptr);
     int gpuIndex = 0;
     uint32_t gpus = 1;
@@ -49,7 +51,8 @@ struct Args {
 
 const char *kUsage =
     "Usage: dllama-native {inference|perplexity|chat} --model <path> --tokenizer <path>\n"
-    "        [--prompt <text>] [--steps <n>] [--temperature <t>] [--topp <p>] [--seed <s>] [--max-seq-len <n>]\n"
+    "        [--prompt <text>] [--steps <n>] [--temperature <t>] [--topp <p>] [--presence-penalty <p>] [--frequency-penalty <f>]\n"
+    "        [--seed <s>] [--max-seq-len <n>]\n"
     "        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--buffer-float-type q80] [--gpu-index <i>]\n"
     "        [--gpus <n>]   tensor parallel over GPUs gpu-index .. gpu-index + n - 1 of this machine (one process per GPU)\n"
     "        (accepted for drop-in compatibility and ignored: --nthreads --net-turbo --gpu-segments --workers --host --port)\n";
@@ -74,6 +77,8 @@ Args parse(int argc, char **argv) {
         else if (name == "--steps") a.steps = (uint32_t)std::stoul(value);
         else if (name == "--temperature") a.temperature = std::stof(value);
         else if (name == "--topp") a.topp = std::stof(value);
+        else if (name == "--presence-penalty") a.presencePenalty = parsePenalty(name, value);
+        else if (name == "--frequency-penalty") a.frequencyPenalty = parsePenalty(name, value);
         else if (name == "--seed") a.seed = std::stoull(value);
         else if (name == "--max-seq-len") a.maxSeqLen = (uint32_t)std::stoul(value);
         else if (name == "--chat-template") a.chatTemplate = value;
@@ -105,6 +110,7 @@ struct App {
           sampler(std::min<uint32_t>(tokenizer.vocabSize(), engine.header().vocabSize), a.temperature, a.topp, a.seed), tp{engine, j} {
         // sampling ranges over the tokenizer's vocabulary (reference src/app.cpp:243-246); padded embedding rows never win
         engine.setVocabLimit(tokenizer.vocabSize());
+        sampler.setControls(a.presencePenalty, a.frequencyPenalty, {});
     }
 
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos) { tp.prefill(tokens, pos); }
@@ -140,6 +146,7 @@ void inference(App &app) {
     std::fflush(stdout);
     int32_t token = tokens[pos];
     app.tokenizer.resetDecoder();
+    app.sampler.beginCompletion();
     const uint32_t maxPos = std::min(h.seqLen, a.steps);
     uint32_t nPred = 0;
     while (pos < maxPos) {
@@ -227,6 +234,7 @@ void chat(App &app) {
         int32_t token = n < tokens.size() ? tokens[n] : tokens.back();
         app.tokenizer.resetDecoder();
         det.reset();
+        app.sampler.beginCompletion();
         std::printf("\n🤖 Assistant\n");
         if (!g.publicPrompt.empty()) std::printf("%s", g.publicPrompt.c_str());
         while (pos < h.seqLen) {

@@ -421,6 +421,15 @@ int32_t NativeEngine::stepSampled(int32_t token, uint32_t pos, float temperature
 
 uint64_t NativeEngine::samplerState() { return (uint64_t)dl_engine_sampler_state(impl_->engine); }
 
+void NativeEngine::setSamplingControls(float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias, uint32_t rowMask) {
+    std::vector<int32_t> ids;
+    std::vector<float> vals;
+    for (const auto &b : bias) { ids.push_back(b.first); vals.push_back(b.second); }
+    engCheck(dl_engine_set_sampling_controls(impl_->engine, presence, frequency, ids.data(), vals.data(), (int)ids.size(), rowMask,
+                                             impl_->stream),
+             "dl_engine_set_sampling_controls");
+}
+
 void NativeEngine::seedChoiceSamplers(const std::vector<uint64_t> &seeds) {
     std::vector<unsigned long long> s(seeds.begin(), seeds.end());
     engCheck(dl_engine_sampler_seed_rows(impl_->engine, s.data(), (int)s.size()), "dl_engine_sampler_seed_rows");

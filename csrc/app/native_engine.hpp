@@ -51,6 +51,10 @@ public:
     void seedSampler(uint64_t seed);
     int32_t stepSampled(int32_t token, uint32_t pos, float temperature, float topp);
     uint64_t samplerState();   // single-sequence generator state: seedSampler(samplerState()) continues its stream
+    // Presence / frequency penalties and logit bias ((id, value) pairs) of the following device draws; zeroes the count rows in
+    // rowMask (bit 0: stepSampled, bit 1 + i: choice i). All zero: off. With controls on, stepSampled and the choices steps accept
+    // temperature 0 (arg-max of the controlled logits). Every rank must make the same call.
+    void setSamplingControls(float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias, uint32_t rowMask);
     // Several completions of one prompt (csrc/cuda/choices.cu), dense models, n <= 8: generators of the batched sampler (separate
     // from the single-sequence one), first draws from the logits of `token` at P, one batched step (see InferenceBackend).
     bool supportsChoices(uint32_t n) const { return n >= 1 && n <= maxBatch_ && h_.nExperts == 0; }

@@ -12,6 +12,7 @@
 #include <chrono>
 #include <csignal>
 #include <cstdio>
+#include <cstring>
 #include <ctime>
 #include <new>
 #include <stdexcept>
@@ -24,7 +25,8 @@
 namespace dl {
 
 enum : uint32_t { TP_OP_PREFILL = 1, TP_OP_STEP_GREEDY = 2, TP_OP_STEP_SAMPLED = 3, TP_OP_EXIT = 4, TP_OP_SEED = 5,
-                  TP_OP_CHOICES_SEED = 6, TP_OP_CHOICES_FIRST = 7, TP_OP_CHOICES_STEP = 8 };
+                  TP_OP_CHOICES_SEED = 6, TP_OP_CHOICES_FIRST = 7, TP_OP_CHOICES_STEP = 8,
+                  TP_OP_CONTROLS = 9 };   // penalties in (temperature, topp), count-row mask in pos, tokens = (id, bias bits) pairs
 constexpr uint32_t kTpMaxRanks = 8, kTpCtrlTokens = 256;
 
 struct TpControl {
@@ -115,6 +117,7 @@ struct TpEngine {
     uint64_t seedGen = ~0ull, seedOf = 0;   // (generation, seed) of the sampler the device generator was last seeded for
     uint64_t savedGen = ~0ull, savedSeed = 0;
     std::vector<float> hostLogits = {};     // the host sampler's copy of the logits (one GPU)
+    uint64_t controlsGen = 0;               // completion generation whose controls the devices hold for stepSampled (0: off)
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos) {
         for (size_t i = 0; i < tokens.size(); i += 192) {   // one control packet per tensor-core chunk
             const uint32_t n = (uint32_t)std::min<size_t>(192, tokens.size() - i);
@@ -128,8 +131,9 @@ struct TpEngine {
     }
     // One generated token with the sampler's settings: greedy on the device, temperature / top-p on the device under tensor
     // parallelism (the logits stay sharded), or the host sampler on the logits copied back from one GPU.
+    // Greedy with sampling controls is the arg-max of the controlled logits (device sampler or host sampler), not the fused arg-max.
     int32_t next(int32_t token, uint32_t pos, Sampler &sampler) {
-        if (sampler.temperature() == 0.f) return stepGreedy(token, pos);
+        if (sampler.temperature() == 0.f && !sampler.controlsActive()) return stepGreedy(token, pos);
         if (engine.nRanks() > 1) return stepSampled(token, pos, sampler);
         const float *logits = engine.step(token, pos);
         hostLogits.assign(logits, logits + sampler.vocabSize());
@@ -137,7 +141,12 @@ struct TpEngine {
     }
     // temperature / top-p on the device (the logits stay sharded); `sampler` only supplies the parameters and the seed
     int32_t stepSampled(int32_t token, uint32_t pos, Sampler &sampler) {
-        if (sampler.seedGeneration() != seedGen || sampler.seed() != seedOf) {
+        const uint64_t gen = sampler.controlsActive() ? sampler.completionGeneration() : 0;
+        if (gen != controlsGen) {   // a new completion: count row 0 starts from zero
+            setControls(sampler, 1u);
+            controlsGen = gen;
+        }
+        if (sampler.temperature() != 0.f && (sampler.seedGeneration() != seedGen || sampler.seed() != seedOf)) {
             seedGen = sampler.seedGeneration();
             seedOf = sampler.seed();
             job.issue(TP_OP_SEED, nullptr, 0, 0, 0.f, 0.f, sampler.seed());
@@ -145,6 +154,23 @@ struct TpEngine {
         }
         job.issue(TP_OP_STEP_SAMPLED, &token, 1, pos, sampler.temperature(), sampler.topp());
         return engine.stepSampled(token, pos, sampler.temperature(), sampler.topp());
+    }
+    void setControls(const Sampler &sampler, uint32_t rowMask) {
+        std::vector<int32_t> w;
+        for (const auto &b : sampler.logitBias()) {
+            uint32_t bits;
+            std::memcpy(&bits, &b.second, 4);
+            w.push_back(b.first);
+            w.push_back((int32_t)bits);
+        }
+        job.issue(TP_OP_CONTROLS, w.data(), (uint32_t)w.size(), rowMask, sampler.presencePenalty(), sampler.frequencyPenalty());
+        engine.setSamplingControls(sampler.presencePenalty(), sampler.frequencyPenalty(), sampler.logitBias(), rowMask);
+    }
+    // the batched choices' controls (count rows 1..n zeroed)
+    void choiceControls(const Sampler &sampler, uint32_t n) {
+        if (!sampler.controlsActive() && controlsGen == 0) return;
+        setControls(sampler, ((1u << n) - 1u) << 1);
+        controlsGen = sampler.controlsActive() ? ~0ull : 0;   // row 0's counts are not this sampler's
     }
     // the single-sequence generator's state, and re-seeding every rank with it (sequential choices re-seed it per choice)
     uint64_t samplerState() {
@@ -178,6 +204,17 @@ struct TpEngine {
     }
 };
 
+// Bias pairs of a TP_OP_CONTROLS packet.
+inline std::vector<std::pair<int32_t, float>> tpControlBias(const int32_t *w, uint32_t n) {
+    std::vector<std::pair<int32_t, float>> bias;
+    for (uint32_t i = 0; i + 1 < n; i += 2) {
+        float v;
+        std::memcpy(&v, &w[i + 1], 4);
+        bias.push_back({w[i], v});
+    }
+    return bias;
+}
+
 // Seeds of a TP_OP_CHOICES_SEED packet.
 inline std::vector<uint64_t> tpChoiceSeeds(const int32_t *w, uint32_t n) {
     std::vector<uint64_t> seeds;
@@ -204,6 +241,7 @@ inline int tpWorkerMain(const std::string &model, const std::string &tokenizer, 
             else if (c.op == TP_OP_STEP_GREEDY) engine.stepGreedy(c.tokens[0], c.pos);
             else if (c.op == TP_OP_STEP_SAMPLED) engine.stepSampled(c.tokens[0], c.pos, c.temperature, c.topp);
             else if (c.op == TP_OP_SEED) engine.seedSampler(c.seed);
+            else if (c.op == TP_OP_CONTROLS) engine.setSamplingControls(c.temperature, c.topp, tpControlBias(c.tokens, c.n), c.pos);
             else if (c.op == TP_OP_CHOICES_SEED) engine.seedChoiceSamplers(tpChoiceSeeds(c.tokens, c.n));
             else if (c.op == TP_OP_CHOICES_FIRST) engine.choicesFirst(c.tokens[0], c.pos, (uint32_t)c.tokens[1], c.temperature, c.topp);
             else if (c.op == TP_OP_CHOICES_STEP)

@@ -48,6 +48,12 @@ struct Engine {
     float **gatherUcDev = nullptr;
     unsigned int **flagUcDev = nullptr;
     uint32_t vocabLimit = 0;     // 0 = none; otherwise the greedy arg-max ignores vocabulary rows >= vocabLimit
+    // sampling controls (dl_engine_set_sampling_controls), allocated on first use: count rows [1 + kChoiceRngSlots][vocabFull]
+    // (row 0: single sequence, row 1 + b: choice b) and a dense bias [vocabFull]
+    uint32_t *ctlCounts = nullptr;
+    float *ctlBias = nullptr;
+    bool ctlActive = false, ctlBiasActive = false;
+    float ctlPresence = 0.f, ctlFrequency = 0.f;
     bool prefillFusedAr = false; // TP prefill: GEMM + all-reduce in one kernel (DL_PREFILL_FUSED_AR=1) instead of GEMM, then all-reduce kernel
     bool tcAttn = true;          // prefill attention on the tensor cores (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
     bool fusedAttn = true, fusedArgmax = true, useTma = true;   // debugging switches (DL_NO_FUSED_ATTN / DL_NO_FUSED_ARGMAX / DL_NO_TMA)
@@ -425,6 +431,8 @@ DL_EXPORT void dl_engine_destroy(void *h) {
     if (e->megaCounter) cudaFree(e->megaCounter);
     for (void *q : {(void *)e->megaX, (void *)e->megaX2, (void *)e->megaQkv, (void *)e->megaZ, (void *)e->megaH, (void *)e->megaSeq}) if (q) cudaFree(q);
     if (e->abortHost) cudaFreeHost(e->abortHost);
+    if (e->ctlCounts) cudaFree(e->ctlCounts);
+    if (e->ctlBias) cudaFree(e->ctlBias);
     delete e;
 }
 
@@ -547,9 +555,55 @@ DL_EXPORT unsigned long long dl_engine_sampler_state(void *h) {
     return v;
 }
 
+// The sampling controls of the following draws: presence and frequency penalties and a logit bias given as nBias (id, value) pairs
+// (ids in [0, V), V = the sampled vocabulary). Zeroes the count rows set in rowMask (bit 0: single sequence, bit 1 + b: choice b),
+// so call it at the start of every completion. All zero (and no bias) switches the controls off: the draws are exactly those
+// without controls. Under tensor parallelism every rank makes the same call and keeps identical counts. The uploads run on `stream`
+// (the stream of the draws) and are complete when the call returns.
+DL_EXPORT int dl_engine_set_sampling_controls(void *h, float presence, float frequency, const int32_t *ids, const float *vals, int nBias,
+                                              uint32_t rowMask, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    const uint32_t full = e->cfg.vocab * (e->comm.nRanks > 1 ? e->comm.nRanks : 1);
+    const uint32_t n = (e->vocabLimit && e->vocabLimit < full) ? e->vocabLimit : full;
+    const uint32_t rows = 1 + kChoiceRngSlots;
+    if (nBias < 0 || (rowMask >> rows) != 0) return -52;
+    for (int i = 0; i < nBias; i++) if (ids[i] < 0 || (uint32_t)ids[i] >= n) return -53;
+    e->ctlActive = false;   // set again only once every buffer below is in place
+    if (presence == 0.f && frequency == 0.f && nBias == 0) return 0;
+    DL_TRY(ensureSampler(e));
+    if (!e->ctlCounts) {
+        DL_CUDA_CHECK(cudaMalloc(&e->ctlCounts, (size_t)rows * full * sizeof(uint32_t)));
+        DL_CUDA_CHECK(cudaMemsetAsync(e->ctlCounts, 0, (size_t)rows * full * sizeof(uint32_t), stream));
+    }
+    if (!e->ctlBias) DL_CUDA_CHECK(cudaMalloc(&e->ctlBias, (size_t)full * sizeof(float)));
+    std::vector<float> bias;
+    if (nBias > 0) {
+        bias.assign(full, 0.f);
+        for (int i = 0; i < nBias; i++) bias[ids[i]] = vals[i];
+        DL_CUDA_CHECK(cudaMemcpyAsync(e->ctlBias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
+    }
+    for (uint32_t r = 0; r < rows; r++)
+        if ((rowMask >> r) & 1u) DL_CUDA_CHECK(cudaMemsetAsync(e->ctlCounts + (size_t)r * full, 0, (size_t)full * sizeof(uint32_t), stream));
+    DL_CUDA_CHECK(cudaStreamSynchronize(stream));   // `bias` is a host temporary
+    e->ctlPresence = presence;
+    e->ctlFrequency = frequency;
+    e->ctlBiasActive = nBias > 0;
+    e->ctlActive = true;
+    return 0;
+}
+
+// The active controls for draws whose row 0 uses count row `firstRow` (null: none).
+static const dl::SampleControls *activeControls(const Engine *e, uint32_t firstRow, dl::SampleControls &ctl) {
+    if (!e->ctlActive) return nullptr;
+    const uint32_t full = e->cfg.vocab * (e->comm.nRanks > 1 ? e->comm.nRanks : 1);
+    ctl = dl::SampleControls{e->ctlBiasActive ? e->ctlBias : nullptr, e->ctlCounts + (size_t)firstRow * full, full, e->ctlPresence, e->ctlFrequency};
+    return &ctl;
+}
+
 // Samples the next token from the logits of the last forward (logitsMode 1) on the device: tokens[0] <- sample, pos[0]++, history.
 // Tensor parallel: the vocabulary slices are first gathered into every rank's arena (peer / multicast stores, no NCCL); every rank
-// then draws the same token from its own copy of the generator.
+// then draws the same token from its own copy of the generator. With sampling controls active, temperature 0 draws the arg-max of
+// the controlled logits.
 DL_EXPORT int dl_engine_sample(void *h, float temperature, float topp, cudaStream_t stream) {
     Engine *e = (Engine *)h;
     const dl::EngineConfig &c = e->cfg;
@@ -557,9 +611,11 @@ DL_EXPORT int dl_engine_sample(void *h, float temperature, float topp, cudaStrea
     const uint32_t nR = e->comm.nRanks > 1 ? e->comm.nRanks : 1;
     const uint32_t full = c.vocab * nR;
     const uint32_t n = (e->vocabLimit && e->vocabLimit < full) ? e->vocabLimit : full;
+    dl::SampleControls ctlArgs;
+    const dl::SampleControls *ctl = activeControls(e, 0, ctlArgs);
     if (nR == 1)
         return dl::launchSample(e->g.logits, e->probScratch, n, temperature, topp, e->rngState, e->g.tokens, e->g.pos, e->g.history, c.seqLen,
-                                nullptr, nullptr, 1, stream);
+                                nullptr, nullptr, 1, stream, ctl);
     uint8_t *mine = (uint8_t *)e->comm.arena[e->comm.rank];
     float *gatherLocal = (float *)(mine + e->comm.gatherOff);
     unsigned int *flagLocal = (unsigned int *)(mine + e->comm.flagsOff);
@@ -567,7 +623,7 @@ DL_EXPORT int dl_engine_sample(void *h, float temperature, float topp, cudaStrea
     unsigned int *flagMc = e->comm.mcArena ? (unsigned int *)((uint8_t *)e->comm.mcArena + e->comm.flagsOff) : nullptr;
     DL_TRY(dl::launchLogitsGather(e->g.logits, c.vocab, c.rank, nR, gatherMc, e->gatherUcDev, flagMc, e->flagUcDev, e->gatherBlockCounter, stream));
     return dl::launchSample(gatherLocal, e->probScratch, n, temperature, topp, e->rngState, e->g.tokens, e->g.pos, e->g.history, c.seqLen, flagLocal,
-                            e->gatherEpoch, nR, stream);
+                            e->gatherEpoch, nR, stream, ctl);
 }
 
 // Seeds the n <= 8 generators of the batched sampler. They are separate from the single-sequence generator of dl_engine_sample,
@@ -594,9 +650,11 @@ DL_EXPORT int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, floa
     const uint32_t full = c.vocab * nR;
     const uint32_t n = (e->vocabLimit && e->vocabLimit < full) ? e->vocabLimit : full;
     const uint32_t rows = firstStep ? 1u : (uint32_t)nb;
+    dl::SampleControls ctlArgs;
+    const dl::SampleControls *ctl = activeControls(e, 1, ctlArgs);
     if (nR == 1)
         return dl::launchSampleRows(e->g.logits, firstStep ? 0u : c.vocab, e->probScratch, n, temperature, topp, e->rngState + kChoiceRngSlots, e->g.tokens, nb,
-                                    inactiveMask, nullptr, nullptr, 1, stream);
+                                    inactiveMask, nullptr, nullptr, 1, stream, ctl);
     uint8_t *mine = (uint8_t *)e->comm.arena[e->comm.rank];
     float *gatherLocal = (float *)(mine + e->comm.gatherOff);
     unsigned int *flagLocal = (unsigned int *)(mine + e->comm.flagsOff);
@@ -604,7 +662,7 @@ DL_EXPORT int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, floa
     unsigned int *flagMc = e->comm.mcArena ? (unsigned int *)((uint8_t *)e->comm.mcArena + e->comm.flagsOff) : nullptr;
     DL_TRY(dl::launchLogitsGather(e->g.logits, c.vocab, c.rank, nR, gatherMc, e->gatherUcDev, flagMc, e->flagUcDev, e->gatherBlockCounter, stream, rows));
     return dl::launchSampleRows(gatherLocal, firstStep ? 0u : full, e->probScratch, n, temperature, topp, e->rngState + kChoiceRngSlots, e->g.tokens, nb, inactiveMask,
-                                flagLocal, e->gatherEpoch, nR, stream);
+                                flagLocal, e->gatherEpoch, nR, stream, ctl);
 }
 
 DL_EXPORT int dl_engine_set_comm(void *h, const dl::CommPtrs *p) {

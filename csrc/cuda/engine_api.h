@@ -90,6 +90,10 @@ int dl_engine_mega_active(void *h);   // 1 if the last single-token forward ran 
 unsigned long long dl_engine_sync_ns(void *h);
 int dl_engine_sampler_seed(void *h, unsigned long long seed);
 int dl_engine_sample(void *h, float temperature, float topp, cudaStream_t stream);   // after a forward with logitsMode 1
+// presence / frequency penalties and logit bias of the following draws; zeroes the count rows in rowMask (bit 0: single sequence,
+// bit 1 + b: choice b). All zero: off.
+int dl_engine_set_sampling_controls(void *h, float presence, float frequency, const int32_t *ids, const float *vals, int nBias, uint32_t rowMask,
+                                    cudaStream_t stream);
 // choices (several completions of one prompt, csrc/cuda/choices.cu): generators 0..n-1, batched draws, one choices forward
 int dl_engine_sampler_seed_rows(void *h, const unsigned long long *seeds, int n);   // separate from the single-sequence generator
 unsigned long long dl_engine_sampler_state(void *h);   // single-sequence generator state (seed with it to continue the stream)

@@ -178,16 +178,26 @@ int launchArgmaxAdvance(const float *logits, uint32_t vocab, int *tokenOut, int 
                         cudaStream_t stream, bool pdl);   // single rank only: the index is local to `logits`
 
 // Device-side temperature / top-p sampler and the logits gather that feeds it under tensor parallelism (sampler.cu)
+// Optional per-request controls, applied to every logit before temperature (float32, round to nearest, no contraction):
+//   x = l[t] + bias[t] (bias non-null); if c[t] > 0: x = x - c[t] * frequency, then x = x - presence.
+// counts row b (counts + b * countsStride) holds how often row b has drawn each token; every draw increments it. With controls
+// the temperature may be 0: the token is then the arg-max of the transformed logits (lowest index among ties).
+struct SampleControls {
+    const float *bias;        // [n] or null
+    uint32_t *counts;         // [rows][countsStride] or null
+    uint32_t countsStride;
+    float presence, frequency;
+};
 int launchSample(const float *logits, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng, int *tokenOut, int *pos,
                  int *history, uint32_t historyCap, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                 cudaStream_t stream);
+                 cudaStream_t stream, const SampleControls *controls = nullptr);
 int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t nRanks, float *gatherMc, float *const *gatherUcDev,
                        unsigned int *flagMc, unsigned int *const *flagUcDev, unsigned int *blockCounter, cudaStream_t stream, uint32_t rows = 1);
 // B draws, one CTA per row: row b reads logits + b * logitsStride (0: every row draws from the same logits), uses rng[b] and writes
 // tokenOut[b]. Rows whose bit is set in inactiveMask draw nothing and keep their generator state. No position advance.
 int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
                      int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                     cudaStream_t stream);
+                     cudaStream_t stream, const SampleControls *controls = nullptr);
 
 // Persistent decode kernel (mega_decode.cu)
 struct MegaLayer {

@@ -39,7 +39,18 @@ struct SampleArgs {
     int *debugOut;             // optional [4]: {last index in order?, ...} unused by the product path
     // batched draws (grid B, one CTA per row): row b reads logits + b * logitsStride, probs + b * probsStride, rng[b], tokenOut[b]
     uint32_t logitsStride, probsStride, inactiveMask;
+    SampleControls ctl;        // bias / penalties (kernels.h); row b counts at ctl.counts + b * ctl.countsStride
 };
+
+// The controls' transform of one logit (kernels.h); explicit roundings because the library is built with --use_fast_math.
+__device__ __forceinline__ float controlled(const SampleControls &c, float x, uint32_t i) {
+    if (c.bias) x = __fadd_rn(x, c.bias[i]);
+    if (c.counts) {
+        const uint32_t k = c.counts[i];
+        if (k > 0) x = __fsub_rn(__fsub_rn(x, __fmul_rn((float)k, c.frequency)), c.presence);
+    }
+    return x;
+}
 
 __device__ float blockMax(float v, float *red) {
     v = warpMax(v);
@@ -164,39 +175,16 @@ __device__ Found radixFind(const SampleArgs &a, float inv, float cutoff, unsigne
     return Found{sInt[2], base + need * fStar};
 }
 
-__global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
-    __shared__ float red[32];
-    __shared__ unsigned long long hist[256];
-    __shared__ unsigned long long scratch[64];
-    __shared__ int sInt[8];
-    __shared__ float sCoin;
+// Temperature / top-p draw from src (logits, or the transformed logits under controls) whose maximum after division by T is m.
+__device__ int drawSampled(const SampleArgs &a, const float *src, float m, unsigned long long *hist, unsigned long long *scratch, int *sInt,
+                           float *sCoin) {
     const uint32_t n = a.n;
-    const uint32_t row = blockIdx.x;
-    if (row < 32 && ((a.inactiveMask >> row) & 1u)) return;
-    a.logits += (size_t)row * a.logitsStride;
-    a.probs += (size_t)row * a.probsStride;
-    a.rng += row;
-    a.tokenOut += row;
-    if (a.gatherFlag && a.nRanks > 1) {
-        if (threadIdx.x == 0) {
-            const unsigned int want = (*a.gatherEpoch + 1u) * a.nRanks;
-            unsigned int v;
-            uint32_t spins = 0;
-            do { asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a.gatherFlag) : "memory"); } while ((int)(v - want) < 0 && ++spins < (1u << 28));
-            if (gridDim.x == 1) *a.gatherEpoch += 1u;   // batched draws: epochAdvanceKernel runs after the grid
-        }
-        __syncthreads();
-    }
-    // softmax statistics (IEEE division / shared exp / integer normaliser: the host sampler computes the very same numbers)
-    float m = -INFINITY;
-    for (uint32_t i = threadIdx.x; i < n; i += kSampThreads) m = fmaxf(m, __fdiv_rn(a.logits[i], a.temperature));
-    m = blockMax(m, red);
     // per-thread sums over contiguous chunks (index order), combined by a fixed tree
     const uint32_t chunk = (n + kSampThreads - 1) / kSampThreads;
     const uint32_t lo = threadIdx.x * chunk, hi = min(lo + chunk, n);
     unsigned long long sFix = 0;
     for (uint32_t i = lo; i < hi; i++) {
-        const float e = expNeg(__fsub_rn(__fdiv_rn(a.logits[i], a.temperature), m));
+        const float e = expNeg(__fsub_rn(__fdiv_rn(src[i], a.temperature), m));
         a.probs[i] = e;
         sFix += toFix(e);
     }
@@ -208,12 +196,11 @@ __global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
         st ^= st >> 12; st ^= st << 25; st ^= st >> 27;
         *a.rng = st;
         const uint32_t u = (uint32_t)((st * 0x2545F4914F6CDD1Dull) >> 32);
-        sCoin = (float)(u >> 8) * 5.9604644775390625e-8f;   // / 2^24, exact
+        *sCoin = (float)(u >> 8) * 5.9604644775390625e-8f;   // / 2^24, exact
         sInt[2] = (int)n - 1;
     }
     __syncthreads();
-    const float coin = sCoin;
-    int token;
+    const float coin = *sCoin;
     if (a.topp <= 0.f || a.topp >= 1.f) {
         // multinomial walk in index order
         unsigned long long mine = 0;
@@ -229,19 +216,69 @@ __global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
             }
         }
         __syncthreads();
-        token = sInt[2];
-    } else {
-        const float cutoff = __fdiv_rn(1.0f - a.topp, (float)(n - 1));
-        const Found cut = radixFind(a, inv, cutoff, toFix(a.topp), hist, scratch, sInt);
-        // r = coin * cumulative (the reference multiplies the float prefix sum)
-        const float cumulative = __fdiv_rn((float)cut.prefix, kFix);
-        const unsigned long long r = toFix(coin * cumulative);
+        return sInt[2];
+    }
+    const float cutoff = __fdiv_rn(1.0f - a.topp, (float)(n - 1));
+    const Found cut = radixFind(a, inv, cutoff, toFix(a.topp), hist, scratch, sInt);
+    // r = coin * cumulative (the reference multiplies the float prefix sum)
+    const float cumulative = __fdiv_rn((float)cut.prefix, kFix);
+    const unsigned long long r = toFix(coin * cumulative);
+    __syncthreads();
+    return radixFind(a, inv, cutoff, r, hist, scratch, sInt).index;
+}
+
+__global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
+    __shared__ float red[32];
+    __shared__ unsigned long long hist[256];
+    __shared__ unsigned long long scratch[64];
+    __shared__ int sInt[8];
+    __shared__ float sCoin;
+    const uint32_t n = a.n;
+    const uint32_t row = blockIdx.x;
+    if (row < 32 && ((a.inactiveMask >> row) & 1u)) return;
+    a.logits += (size_t)row * a.logitsStride;
+    a.probs += (size_t)row * a.probsStride;
+    a.rng += row;
+    a.tokenOut += row;
+    if (a.ctl.counts) a.ctl.counts += (size_t)row * a.ctl.countsStride;
+    if (a.gatherFlag && a.nRanks > 1) {
+        if (threadIdx.x == 0) {
+            const unsigned int want = (*a.gatherEpoch + 1u) * a.nRanks;
+            unsigned int v;
+            uint32_t spins = 0;
+            do { asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(a.gatherFlag) : "memory"); } while ((int)(v - want) < 0 && ++spins < (1u << 28));
+            if (gridDim.x == 1) *a.gatherEpoch += 1u;   // batched draws: epochAdvanceKernel runs after the grid
+        }
         __syncthreads();
-        const Found pick = radixFind(a, inv, cutoff, r, hist, scratch, sInt);
-        token = pick.index;
+    }
+    // With controls the max pass stores the transformed logits in probs, and the later passes read them from there: counts and
+    // bias are read once per logit.
+    const bool ctl = a.ctl.bias || a.ctl.counts;
+    const bool greedy = a.temperature == 0.f;   // reached with controls only (the launchers refuse it otherwise)
+    const float *src = ctl ? a.probs : a.logits;
+    // softmax statistics (IEEE division / shared exp / integer normaliser: the host sampler computes the very same numbers)
+    float m = -INFINITY;
+    for (uint32_t i = threadIdx.x; i < n; i += kSampThreads) {
+        float x = a.logits[i];
+        if (ctl) { x = controlled(a.ctl, x, i); a.probs[i] = x; }
+        m = fmaxf(m, greedy ? x : __fdiv_rn(x, a.temperature));
+    }
+    m = blockMax(m, red);
+    int token;
+    if (greedy) {   // arg-max: the lowest index holding the maximum
+        if (threadIdx.x == 0) sInt[3] = (int)n - 1;
+        __syncthreads();
+        for (uint32_t i = threadIdx.x; i < n; i += kSampThreads) {
+            if (src[i] == m) { atomicMin(&sInt[3], (int)i); break; }
+        }
+        __syncthreads();
+        token = sInt[3];
+    } else {
+        token = drawSampled(a, src, m, hist, scratch, sInt, &sCoin);
     }
     if (threadIdx.x == 0) {
         a.tokenOut[0] = token;
+        if (a.ctl.counts) a.ctl.counts[token] += 1u;
         if (a.pos) {
             const int p = a.pos[0] + 1;
             a.pos[0] = p;
@@ -285,11 +322,12 @@ __global__ void __launch_bounds__(256) logitsGatherKernel(const float *local, ui
 
 int launchSample(const float *logits, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng, int *tokenOut, int *pos,
                  int *history, uint32_t historyCap, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                 cudaStream_t stream) {
-    if (n < 2 || temperature <= 0.f) return -1;
+                 cudaStream_t stream, const SampleControls *controls) {
+    if (n < 2 || !(temperature > 0.f || (temperature == 0.f && controls))) return -1;
     SampleArgs a{};
     a.logits = logits; a.probs = probs; a.n = n; a.temperature = temperature; a.topp = topp; a.rng = rng; a.tokenOut = tokenOut; a.pos = pos;
     a.history = history; a.historyCap = historyCap; a.gatherFlag = gatherFlag; a.gatherEpoch = gatherEpoch; a.nRanks = nRanks;
+    if (controls) a.ctl = *controls;
     sampleKernel<<<1, kSampThreads, 0, stream>>>(a);
     DL_CUDA_CHECK(cudaGetLastError());
     return 0;
@@ -305,12 +343,13 @@ int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t 
 
 int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
                      int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                     cudaStream_t stream) {
-    if (n < 2 || temperature <= 0.f || B < 1 || B > 32) return -1;
+                     cudaStream_t stream, const SampleControls *controls) {
+    if (n < 2 || !(temperature > 0.f || (temperature == 0.f && controls)) || B < 1 || B > 32) return -1;
     SampleArgs a{};
     a.logits = logits; a.probs = probs; a.n = n; a.temperature = temperature; a.topp = topp; a.rng = rng; a.tokenOut = tokenOut;
     a.gatherFlag = gatherFlag; a.gatherEpoch = gatherEpoch; a.nRanks = nRanks;
     a.logitsStride = logitsStride; a.probsStride = n; a.inactiveMask = inactiveMask;
+    if (controls) a.ctl = *controls;
     sampleKernel<<<B, kSampThreads, 0, stream>>>(a);
     DL_CUDA_CHECK(cudaGetLastError());
     if (gatherFlag && nRanks > 1 && B > 1) {
@@ -334,4 +373,14 @@ DL_EXPORT int dl_sample_rows(const float *logits, uint32_t logitsStride, float *
                              unsigned long long *rngState, int *tokenOut, uint32_t B, uint32_t inactiveMask, cudaStream_t stream) {
     return dl::launchSampleRows(logits, logitsStride, probsScratch, n, temperature, topp, rngState, tokenOut, B, inactiveMask, nullptr, nullptr, 1,
                                 stream);
+}
+
+// dl_sample_rows with sampling controls (kernels.h: SampleControls): bias (device f32 [n], may be null), counts (device u32, row b at
+// counts + b * countsStride, may be null; every draw increments it) and the two penalties. Temperature 0 draws the arg-max.
+DL_EXPORT int dl_sample_rows_controlled(const float *logits, uint32_t logitsStride, float *probsScratch, uint32_t n, float temperature, float topp,
+                                        unsigned long long *rngState, int *tokenOut, uint32_t B, uint32_t inactiveMask, const float *bias,
+                                        uint32_t *counts, uint32_t countsStride, float presence, float frequency, cudaStream_t stream) {
+    const dl::SampleControls ctl{bias, counts, countsStride, presence, frequency};
+    return dl::launchSampleRows(logits, logitsStride, probsScratch, n, temperature, topp, rngState, tokenOut, B, inactiveMask, nullptr, nullptr, 1,
+                                stream, &ctl);
 }

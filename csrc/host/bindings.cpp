@@ -193,6 +193,25 @@ PYBIND11_MODULE(_host, m) {
             F32Array copy = logits.attr("copy")().cast<F32Array>();
             return s.sample(copy.mutable_data());
         })
+        .def("set_controls", [](Sampler &s, float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias) {
+            s.setControls(presence, frequency, bias);
+        }, py::arg("presence_penalty"), py::arg("frequency_penalty"), py::arg("logit_bias") = std::vector<std::pair<int32_t, float>>{})
+        .def("begin_completion", &Sampler::beginCompletion)
+        .def("apply_controls", [](const Sampler &s, F32Array logits) {
+            if ((uint32_t)logits.size() < s.vocabSize()) throw std::invalid_argument("Sampler: logits shorter than vocab size");
+            F32Array copy = logits.attr("copy")().cast<F32Array>();
+            s.applyControls(copy.mutable_data());
+            return copy;
+        })
+        .def_property_readonly("controls_active", &Sampler::controlsActive)
+        .def_property_readonly("presence_penalty", &Sampler::presencePenalty)
+        .def_property_readonly("frequency_penalty", &Sampler::frequencyPenalty)
+        .def_property_readonly("logit_bias", &Sampler::logitBias)
+        .def_property_readonly("counts", [](const Sampler &s) {
+            const std::vector<uint32_t> &c = s.counts();
+            return py::array_t<uint32_t>((py::ssize_t)c.size(), c.data());
+        })
+        .def_property_readonly("completion_generation", &Sampler::completionGeneration)
         .def("next_coin", &Sampler::nextCoin)
         .def("next_seed", &Sampler::nextSeed)
         .def("set_temperature", &Sampler::setTemperature)

@@ -3,6 +3,7 @@
 #include "../common/dl_expf.h"
 
 #include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -271,10 +272,59 @@ void softmaxInPlace(float *x, size_t n) {
     for (size_t i = 0; i < n; i++) x[i] *= inv;
 }
 
+static uint64_t nextCompletionGeneration() {
+    static std::atomic<uint64_t> next{1};
+    return next.fetch_add(1);
+}
+
 Sampler::Sampler(uint32_t vocabSize, float temperature, float topp, uint64_t seed)
-    : vocabSize_(vocabSize), temperature_(temperature), topp_(topp), rng_(seed), seed_(seed) {}
+    : vocabSize_(vocabSize), temperature_(temperature), topp_(topp), rng_(seed), seed_(seed), completion_(nextCompletionGeneration()) {}
+
+void Sampler::setControls(float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias) {
+    for (const auto &b : bias)
+        if (b.first < 0 || (uint32_t)b.first >= vocabSize_) throw std::invalid_argument("logit_bias: token id outside the vocabulary");
+    presence_ = presence;
+    frequency_ = frequency;
+    bias_ = bias;
+    biasDense_.clear();
+    if (!bias_.empty()) {
+        biasDense_.assign(vocabSize_, 0.f);
+        for (const auto &b : bias_) biasDense_[b.first] = b.second;
+    }
+    if (!controlsActive()) counts_.clear();
+    else counts_.assign(vocabSize_, 0u);
+    completion_ = nextCompletionGeneration();
+}
+
+void Sampler::beginCompletion() {
+    std::fill(counts_.begin(), counts_.end(), 0u);
+    completion_ = nextCompletionGeneration();
+}
+
+// Built without FMA (-O2, no -march): every step rounds to float32 as the device's __fadd_rn / __fmul_rn / __fsub_rn do.
+void Sampler::applyControls(float *logits) const {
+    const bool bias = !biasDense_.empty(), counted = !counts_.empty();
+    for (uint32_t i = 0; i < vocabSize_; i++) {
+        float x = logits[i];
+        if (bias) x = x + biasDense_[i];
+        if (counted && counts_[i] > 0) {
+            const float pen = (float)counts_[i] * frequency_;
+            x = x - pen;
+            x = x - presence_;
+        }
+        logits[i] = x;
+    }
+}
 
 int32_t Sampler::sample(float *logits) {
+    if (!controlsActive()) return draw(logits);
+    applyControls(logits);
+    const int32_t token = draw(logits);
+    counts_[token]++;
+    return token;
+}
+
+int32_t Sampler::draw(float *logits) {
     const int n = (int)vocabSize_;
     if (temperature_ == 0.0f) {
         int best = 0;

@@ -79,10 +79,35 @@ struct Rng {
 
 void softmaxInPlace(float *x, size_t n);
 
+// Limits of the sampling controls (presence / frequency penalties and logit bias): both API servers refuse requests beyond them.
+// One tensor-parallel control packet carries every bias entry.
+constexpr float kMaxPenalty = 2.0f;
+constexpr float kMaxLogitBias = 100.0f;
+constexpr uint32_t kMaxLogitBiasEntries = 100;
+
 class Sampler {
 public:
     Sampler(uint32_t vocabSize, float temperature, float topp, uint64_t seed);
-    int32_t sample(float *logits);          // modifies logits in place (temperature, softmax)
+    // Modifies logits in place (controls, temperature, softmax). With controls active, counts the drawn token.
+    int32_t sample(float *logits);
+    // Sampling controls of the following draws (presence / frequency penalty, logit bias as (id, value) pairs, ids < vocabSize).
+    // Before temperature every logit becomes, in float32 without contraction: x = l + bias (if any bias is given), then, for a
+    // token this completion has drawn c > 0 times, x = x - c * frequency, then x = x - presence. The device sampler
+    // (csrc/cuda/sampler.cu) computes the same numbers. All zero and no bias: off, and sampling is exactly as without controls.
+    // Setting the controls starts a new completion (counts from zero, a new completion generation), so device-side copies keyed
+    // on the generation always hold the controls in force.
+    void setControls(float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias);
+    // Starts a completion: zeroes the counts and takes a new completion generation.
+    void beginCompletion();
+    void applyControls(float *logits) const;   // the transform above, in place ([vocabSize])
+    bool controlsActive() const { return presence_ != 0.f || frequency_ != 0.f || !bias_.empty(); }
+    float presencePenalty() const { return presence_; }
+    float frequencyPenalty() const { return frequency_; }
+    const std::vector<std::pair<int32_t, float>> &logitBias() const { return bias_; }
+    const std::vector<uint32_t> &counts() const { return counts_; }   // per token of this completion (empty while controls are off)
+    // Unique in the process across all samplers: a new sampler and every beginCompletion take a fresh one, so device-side count
+    // rows keyed on it are zeroed for every completion, including a fresh sampler per choice.
+    uint64_t completionGeneration() const { return completion_; }
     float nextCoin() { return rng_.nextF32(); }
     // A fresh 64-bit seed drawn from this sampler's generator (advances it): the base seed of a request for several
     // completions that names no seed, so that repeated requests differ.
@@ -97,12 +122,18 @@ public:
     uint32_t vocabSize() const { return vocabSize_; }
 
 private:
+    int32_t draw(float *logits);            // greedy / temperature / top-p draw
     uint32_t vocabSize_;
     float temperature_, topp_;
     Rng rng_;
     uint64_t seed_ = 0;
     uint32_t seedGeneration_ = 0;
     std::vector<std::pair<float, int32_t>> candidates_;
+    float presence_ = 0.f, frequency_ = 0.f;
+    std::vector<std::pair<int32_t, float>> bias_;
+    std::vector<float> biasDense_;
+    std::vector<uint32_t> counts_;
+    uint64_t completion_;
 };
 
 enum ChatTemplateType : int32_t { TEMPLATE_UNKNOWN = 0, TEMPLATE_LLAMA2 = 1, TEMPLATE_LLAMA3 = 2, TEMPLATE_DEEP_SEEK3 = 3, TEMPLATE_CHATML = 4 };

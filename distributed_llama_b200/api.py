@@ -43,10 +43,12 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     the context up to its last row. Rows up to P-1 are never written; row P is written by the forward
     of `token` (once on the batched path, once per choice, with the same values, on the sequential path). The single-sequence
     generator continues its stream afterwards. on_token(i, tok) is called for every generated token and returns True when
-    choice i is finished (end of sequence or stop string). `backend` provides next_token(token, pos, sampler),
-    forget_device_seed(), save_sampler() / restore_sampler(saved), and for the batched path batched_choices(n),
-    seed_choices(seeds), choices_first(token, P, n, T, topp) and choices_step(tokens, P, C, j, active, T, topp)
-    (InferenceSession and apps.runtime.RootInference). Returns each choice's tokens."""
+    choice i is finished (end of sequence or stop string). The sampler's controls (presence / frequency penalty, logit bias)
+    apply to every choice, each with its own token counts, which start at zero. `backend` provides
+    next_token(token, pos, sampler), forget_device_seed(), save_sampler() / restore_sampler(saved), and for the batched path
+    batched_choices(n), seed_choices(seeds), choice_controls(sampler, n), choices_first(token, P, n, T, topp) and
+    choices_step(tokens, P, C, j, active, T, topp) (InferenceSession and apps.runtime.RootInference). Returns each choice's
+    tokens."""
     H = host()
     if not 1 <= n <= MAX_CHOICES:
         raise ValueError(f"n must be between 1 and {MAX_CHOICES}")
@@ -57,6 +59,7 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     out: List[List[int]] = [[] for _ in range(n)]
     if limit <= 0:
         return out
+    sampler.begin_completion()
 
     def single(smp, choices):
         # today's single-sequence path from P; rows past P belong to this sequence until the next one overwrites them
@@ -83,11 +86,14 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
         try:
             for i in range(n):
                 backend.forget_device_seed()
-                single(H.Sampler(sampler.vocab_size, T, topp, seeds[i]), [i])
+                smp = H.Sampler(sampler.vocab_size, T, topp, seeds[i])   # a fresh sampler: its own counts, from zero
+                smp.set_controls(sampler.presence_penalty, sampler.frequency_penalty, sampler.logit_bias)
+                single(smp, [i])
         finally:
             backend.restore_sampler(saved)
         return out
     backend.seed_choices(seeds)
+    backend.choice_controls(sampler, n)
     last = backend.choices_first(token, P, n, T, topp)
     active = [True] * n
     j = 0
@@ -107,7 +113,11 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
 class InferenceSession:
     def __init__(self, model_path: str, tokenizer_path: Optional[str] = None, max_seq_len: int = 0,
                  temperature: float = 0.0, topp: float = 0.9, seed: int = 12345, device: Optional[str] = None,
-                 max_batch: int = 8, use_pdl: bool = True, comm=None, moe_mode: str = "auto"):
+                 max_batch: int = 8, use_pdl: bool = True, comm=None, moe_mode: str = "auto", presence_penalty: float = 0.0,
+                 frequency_penalty: float = 0.0, logit_bias: Optional[dict] = None):
+        """presence_penalty, frequency_penalty and logit_bias ({token id: value}) are the sampling controls of every
+        completion (host Sampler.set_controls; they may be changed later through self.sampler.set_controls, which restarts the
+        counts of the current completion)."""
         from .models.loader import load_device_weights
         from .runtime.engine import Engine
 
@@ -125,10 +135,12 @@ class InferenceSession:
         self.tokenizer = H.Tokenizer(tokenizer_path) if tokenizer_path else None
         vocab = self.tokenizer.vocab_size if self.tokenizer else self.header.vocab_size
         self.sampler = H.Sampler(vocab, temperature, topp, seed)
+        self.sampler.set_controls(presence_penalty, frequency_penalty, sorted((int(k), float(v)) for k, v in (logit_bias or {}).items()))
         if self.tokenizer and self.tokenizer.vocab_size < self.header.vocab_size:
             self.engine.set_vocab_limit(self.tokenizer.vocab_size)
         self.pos = 0
         self._dev_seeded = None
+        self._dev_controls = None   # completion generation whose controls the device holds (None: off)
         self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory()
         self._pin_out = torch.zeros(1, dtype=torch.int32).pin_memory()
 
@@ -153,7 +165,7 @@ class InferenceSession:
         if pos is not None:
             self.pos = pos
         smp = self.sampler if sampler is None else sampler
-        if smp.temperature == 0.0:
+        if smp.temperature == 0.0 and not smp.controls_active:
             self._pin_in[0] = token
             self._pin_in[1] = self.pos
             eng = self.engine
@@ -169,9 +181,10 @@ class InferenceSession:
         if self.device.type == "cuda" and not getattr(eng, "_parts", False):
             # temperature / top-p on the device (csrc/cuda/sampler.cu): only the sampled token crosses PCIe
             gen = (smp.seed, smp.seed_generation)
-            if self._dev_seeded != gen:
+            if smp.temperature != 0.0 and self._dev_seeded != gen:
                 eng.seed_sampler(smp.seed)
                 self._dev_seeded = gen
+            self._sync_controls(smp)
             eng.step_sampled(token, self.pos, smp.temperature, smp.topp)
             self._pin_out.copy_(eng.tokens[:1], non_blocking=True)
             torch.cuda.current_stream().synchronize()
@@ -181,9 +194,23 @@ class InferenceSession:
         lg = self.forward_logits(token)
         return int(smp.sample(lg.float().cpu().numpy()))
 
+    def _sync_controls(self, smp):
+        """Hands the sampler's controls to the device at the start of each of its completions (count row 0 zeroed)."""
+        key = smp.completion_generation if smp.controls_active else None
+        if self._dev_controls != key:
+            self.engine.set_sampling_controls(smp.presence_penalty, smp.frequency_penalty, smp.logit_bias, 1)
+            self._dev_controls = key
+
     # ---- several completions of one prompt ----
     def forget_device_seed(self):
         self._dev_seeded = None
+
+    def choice_controls(self, sampler, n: int):
+        """The sampler's controls for the batched choices, count rows 1..n zeroed."""
+        if sampler.controls_active or self._dev_controls is not None:
+            self.engine.set_sampling_controls(sampler.presence_penalty, sampler.frequency_penalty, sampler.logit_bias,
+                                              ((1 << n) - 1) << 1)
+            self._dev_controls = -1 if sampler.controls_active else None   # row 0's counts are not this sampler's
 
     def save_sampler(self):
         key = self._dev_seeded
@@ -236,6 +263,7 @@ class InferenceSession:
         self.prefill(toks[:-1])
         tok = toks[-1]
         self.tokenizer.reset_decoder()
+        self.sampler.begin_completion()
         out = []
         while self.pos < min(steps, self.header.seq_len):
             tok = self.next_token(tok)

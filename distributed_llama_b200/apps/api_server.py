@@ -9,6 +9,7 @@ on non-stream responses.
 from __future__ import annotations
 
 import json
+import re
 import socket
 import sys
 import time
@@ -121,6 +122,37 @@ def parse_n(body: dict) -> int:
     return n
 
 
+MAX_PENALTY = 2.0           # |presence_penalty|, |frequency_penalty|
+MAX_LOGIT_BIAS = 100.0       # |logit_bias value|
+MAX_LOGIT_BIAS_ENTRIES = 100  # one tensor-parallel control packet carries them all (both runtimes)
+
+
+def _number(v, lo: float, hi: float, what: str) -> float:
+    if isinstance(v, bool) or not isinstance(v, (int, float)) or not lo <= v <= hi:
+        raise ValueError(f"'{what}' must be a number from {lo:g} to {hi:g}")
+    return float(v)
+
+
+def parse_controls(body: dict, vocab: int, presence: float, frequency: float):
+    """The request's sampling controls: (presence_penalty, frequency_penalty, logit_bias as (id, value) pairs sorted by id).
+    Absent penalties take the server's defaults. Penalties are numbers in [-2, 2]; logit_bias is an object of at most 100
+    entries whose keys are decimal token ids in [0, vocab) without leading zeros and whose values are numbers in [-100, 100].
+    Anything else is refused."""
+    if "presence_penalty" in body:
+        presence = _number(body["presence_penalty"], -MAX_PENALTY, MAX_PENALTY, "presence_penalty")
+    if "frequency_penalty" in body:
+        frequency = _number(body["frequency_penalty"], -MAX_PENALTY, MAX_PENALTY, "frequency_penalty")
+    bias = body.get("logit_bias", {})
+    if not isinstance(bias, dict) or len(bias) > MAX_LOGIT_BIAS_ENTRIES:
+        raise ValueError(f"'logit_bias' must be an object of at most {MAX_LOGIT_BIAS_ENTRIES} entries")
+    pairs = []
+    for k, v in bias.items():
+        if not re.fullmatch(r"0|[1-9][0-9]{0,9}", k) or int(k) >= vocab:
+            raise ValueError(f"'logit_bias' keys must be token ids from 0 to {vocab - 1}")
+        pairs.append((int(k), _number(v, -MAX_LOGIT_BIAS, MAX_LOGIT_BIAS, "logit_bias")))
+    return presence, frequency, sorted(pairs)
+
+
 def chunk_json(delta: Optional[str], stop: bool, index: int = 0) -> str:
     choice = {"index": index, "finish_reason": "stop" if stop else ""}
     if not stop:
@@ -148,6 +180,10 @@ class ApiServer:
         tok, inf, h, smp = ctx.tokenizer, ctx.inference, ctx.header, ctx.sampler
         body = req.json or {}
         n = parse_n(body)
+        # server defaults: --presence-penalty / --frequency-penalty (argument objects that predate them mean 0)
+        presence, frequency, bias = parse_controls(body, smp.vocab_size, getattr(ctx.args, "presence_penalty", 0.0),
+                                                   getattr(ctx.args, "frequency_penalty", 0.0))
+        smp.set_controls(presence, frequency, bias)
         messages = [(m["role"], m["content"]) for m in body["messages"]]
         stream = bool(body.get("stream", False))
         max_tokens = int(body.get("max_tokens", -1))
@@ -252,7 +288,8 @@ def serve(ctx: AppContext, max_requests: int = 0) -> None:
 
 USAGE = """Usage: dllama-api {--model <path>} {--tokenizer <path>} [--host <addr>] [--port <p>]
         [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>] [--gpus <n>] [--workers <ip:port> ...]
-        [--temperature <temp>] [--topp <t>] [--seed <s>] [--chat-template {llama2|llama3|deepSeek3|chatml}]
+        [--temperature <temp>] [--topp <t>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]
+        [--chat-template {llama2|llama3|deepSeek3|chatml}]
 """
 
 

@@ -28,6 +28,8 @@ class AppArgs:
     steps: int = 0
     temperature: float = 0.8
     topp: float = 0.9
+    presence_penalty: float = 0.0    # sampling controls (host Sampler.set_controls), each in [-2, 2]
+    frequency_penalty: float = 0.0
     seed: int = field(default_factory=lambda: int(time.time()))
     chat_template: Optional[str] = None
     max_seq_len: int = 0
@@ -91,6 +93,11 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
             a.temperature = float(value)
         elif name == "--topp":
             a.topp = float(value)
+        elif name in ("--presence-penalty", "--frequency-penalty"):
+            v = float(value)
+            if not -2.0 <= v <= 2.0:
+                raise ValueError(f"{name} must be from -2 to 2")
+            setattr(a, "presence_penalty" if name == "--presence-penalty" else "frequency_penalty", v)
         elif name == "--seed":
             a.seed = int(value)
         elif name == "--chat-template":
@@ -119,7 +126,8 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
 
 USAGE = """Usage: dllama {inference|chat|perplexity|worker} {--model <path>} {--tokenizer <path>}
         [--prompt <text>] [--steps <n>] [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>]
-        [--temperature <temp>] [--topp <t>] [--seed <s>] [--chat-template {llama2|llama3|deepSeek3|chatml}]
+        [--temperature <temp>] [--topp <t>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]
+        [--chat-template {llama2|llama3|deepSeek3|chatml}]
         [--gpus <n>]                      run tensor-parallel on n local GPUs (spawns one process per GPU)
         [--workers <ip:port> ...] [--nthreads <n>] [--net-turbo {0|1}] [--gpu-index <i>] [--gpu-segments <a:b>]
                                           accepted for compatibility with the reference CLI

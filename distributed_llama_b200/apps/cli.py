@@ -57,6 +57,7 @@ def inference(ctx: AppContext) -> None:
     pred_ms = 0.0
     max_pos = min(h.seq_len, a.steps)
     greedy = ctx.sampler.temperature == 0.0
+    ctx.sampler.begin_completion()
     n_pred = 0
     sync_prev = ctx.sess.engine.sync_ns() if inf.comm is not None else 0
     sync_total_us = 0
@@ -158,6 +159,7 @@ def chat(ctx: AppContext) -> None:
         token = tokens[n] if n < len(tokens) else tokens[-1]
         tok.reset_decoder()
         det.reset()
+        ctx.sampler.begin_completion()
         print("\n🤖 Assistant")
         if public:
             print(public.decode("utf-8", errors="replace"), end="")

@@ -22,6 +22,7 @@ from .args import AppArgs
 
 OP_STOP, OP_PREFILL, OP_STEP_LOGITS, OP_STEP_GREEDY, OP_DECODE_N, OP_STEP_SAMPLE, OP_SEED = 0, 1, 2, 3, 4, 5, 6
 OP_CHOICES_SEED, OP_CHOICES_FIRST, OP_CHOICES_STEP = 7, 8, 9
+OP_CONTROLS = 10   # [presence bits, frequency bits, count-row mask, (id, bias bits) ...]: Engine.set_sampling_controls
 
 
 def _split_seed(seed: int) -> List[int]:
@@ -167,15 +168,28 @@ class RootInference:
         self.eng.check_abort()
         return int(self._pin_out[0])
 
+    def set_controls(self, sampler, row_mask: int) -> None:
+        bias = sampler.logit_bias
+        words = _f32_bits(sampler.presence_penalty, sampler.frequency_penalty) + [row_mask]
+        for t, v in bias:
+            words += [t] + _f32_bits(v)
+        self._send(OP_CONTROLS, 0, words)
+        self.eng.set_sampling_controls(sampler.presence_penalty, sampler.frequency_penalty, bias, row_mask)
+
     def next_token(self, token: int, pos: int, sampler) -> int:
         """One generated token with the sampler's settings: greedy and temperature/top-p both run on the device; the host sampler
-        is only used with the library-collective (multi-node) mode or DL_HOST_SAMPLER=1."""
-        if sampler.temperature == 0.0:
+        is only used with the library-collective (multi-node) mode or DL_HOST_SAMPLER=1. Greedy with sampling controls runs
+        on the device sampler (arg-max of the controlled logits), not on the fused arg-max."""
+        if sampler.temperature == 0.0 and not sampler.controls_active:
             return self.forward_greedy(token, pos)
         if self.device_sampling:
-            if getattr(self, "_seeded", None) != (sampler.seed, sampler.seed_generation):
+            if sampler.temperature != 0.0 and getattr(self, "_seeded", None) != (sampler.seed, sampler.seed_generation):
                 self.seed(sampler.seed)
                 self._seeded = (sampler.seed, sampler.seed_generation)
+            key = sampler.completion_generation if sampler.controls_active else None
+            if getattr(self, "_controls", None) != key:   # a new completion: count row 0 starts from zero
+                self.set_controls(sampler, 1)
+                self._controls = key
             return self.forward_sampled(token, pos, sampler.temperature, sampler.topp)
         return int(sampler.sample(self.forward_logits(token, pos).float().cpu().numpy()))
 
@@ -195,6 +209,11 @@ class RootInference:
 
     def batched_choices(self, n: int) -> bool:
         return self.device_sampling and self.eng.supports_choices(n)
+
+    def choice_controls(self, sampler, n: int) -> None:
+        if sampler.controls_active or getattr(self, "_controls", None) is not None:
+            self.set_controls(sampler, ((1 << n) - 1) << 1)
+            self._controls = -1 if sampler.controls_active else None   # row 0's counts are not this sampler's
 
     def seed_choices(self, seeds: Sequence[int]) -> None:
         self._send(OP_CHOICES_SEED, 0, [w for s in seeds for w in _split_seed(s)])
@@ -264,6 +283,11 @@ def worker_loop(sess: InferenceSession, comm, chan=None) -> None:
             temperature, topp = _bits_f32(toks[3], toks[4])
             tokens = toks[5:]
             eng.choices_step(tokens, pos, C, j, _active_list(mask, len(tokens)), temperature, topp)
+        elif op == OP_CONTROLS:
+            presence, frequency = _bits_f32(toks[0], toks[1])
+            pairs = toks[3:]
+            bias = [(pairs[i], _bits_f32(pairs[i + 1])[0]) for i in range(0, len(pairs), 2)]
+            eng.set_sampling_controls(presence, frequency, bias, toks[2])
         elif op == OP_STEP_SAMPLE:
             import struct
             temperature, topp = struct.unpack("<ff", struct.pack("<ii", toks[1], toks[2]))
@@ -293,7 +317,8 @@ def run_inference_app(args: AppArgs, handler: Callable[[AppContext], None]) -> N
     if header.weight_type == H.F_Q40 and args.buffer_float_type != "q80":
         raise RuntimeError("This version supports only Q40 weights with Q80 sync type")
     sess = InferenceSession(args.model, args.tokenizer, max_seq_len=args.max_seq_len, temperature=args.temperature,
-                            topp=args.topp, seed=args.seed, comm=comm, moe_mode=getattr(args, "moe_mode", "auto") or "auto")
+                            topp=args.topp, seed=args.seed, comm=comm, moe_mode=getattr(args, "moe_mode", "auto") or "auto",
+                            presence_penalty=args.presence_penalty, frequency_penalty=args.frequency_penalty)
     chan = open_control_channel(comm)
     if rank != 0:
         worker_loop(sess, comm, chan)

@@ -120,6 +120,10 @@ def lib() -> C.CDLL:
     L.dl_sample_logits.restype = i32
     L.dl_sample_rows.argtypes = [vp, u32, vp, u32, f32, f32, vp, vp, u32, u32, vp]
     L.dl_sample_rows.restype = i32
+    L.dl_sample_rows_controlled.argtypes = [vp, u32, vp, u32, f32, f32, vp, vp, u32, u32, vp, vp, u32, f32, f32, vp]
+    L.dl_sample_rows_controlled.restype = i32
+    L.dl_engine_set_sampling_controls.argtypes = [vp, f32, f32, C.POINTER(C.c_int32), C.POINTER(f32), i32, u32, vp]
+    L.dl_engine_set_sampling_controls.restype = i32
     L.dl_choice_attn.argtypes = [vp, u32, vp, vp, vp, vp, f32, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
     L.dl_choice_attn.restype = i32
     L.dl_choice_attn_only.argtypes = [vp, u32, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
@@ -164,6 +168,7 @@ _ERRORS = {
     -32: "mixture-of-experts down-projection shape not covered by the TMA GEMV (per-rank expert ffDim must be a multiple of 128: use moe_mode=ep)",
     -33: "arg-max under tensor parallelism needs the fused logits kernel",
     -36: "mixture-of-experts prefill shape not covered (dim, ffDim multiples of 256, chunk <= 256 tokens)",
+    -53: "logit_bias token id outside the sampled vocabulary",
 }
 
 

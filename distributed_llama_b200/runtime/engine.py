@@ -165,6 +165,19 @@ class Engine:
         self.forward_batch([token], pos, logits_mode=1)
         cl.check(self._lib.dl_engine_sample(self._h, float(temperature), float(topp), cl.stream_ptr()), "engine_sample")
 
+    def set_sampling_controls(self, presence: float, frequency: float, bias: Sequence, row_mask: int) -> None:
+        """Presence / frequency penalties and logit bias ((id, value) pairs) of the following device draws; zeroes the count
+        rows in row_mask (bit 0: single sequence, bit 1 + i: choice i). All zero and no bias: off. Every rank makes the same
+        call. With controls on, step_sampled and the choices steps accept temperature 0 (arg-max of the controlled logits)."""
+        n = len(bias)
+        ids = (C.c_int32 * max(n, 1))(*[int(t) for t, _ in bias])
+        vals = (C.c_float * max(n, 1))(*[float(v) for _, v in bias])
+        cl.check(self._lib.dl_engine_set_sampling_controls(self._h, float(presence), float(frequency), ids, vals, n, int(row_mask),
+                                                            cl.stream_ptr()),
+                 "engine_set_sampling_controls")
+        if presence or frequency or n:
+            self._sampler_ready = True
+
     # -- choices: several completions of one prompt, one row per choice (csrc/cuda/choices.cu) --
     def supports_choices(self, n: int) -> bool:
         """True if n choices can run as one batched step: dense layers, kernel-fused collectives, n <= max_batch."""

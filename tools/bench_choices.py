@@ -1,6 +1,6 @@
 """Throughput of n completions of one prompt: the batched choices step against n sequential single-sequence completions.
 
-    python tools/bench_choices.py [--model llama-3.1-8b] [--tokens 64] [--repeats 3]
+    python tools/bench_choices.py [--model llama-3.1-8b] [--tokens 64] [--repeats 3] [--controls]
 
 On the synthetic q40 model of bench.py, one GPU, temperature 0.8 / top-p 0.9. For each prompt length and n it prefills the
 prompt, then times the generation of `--tokens` tokens per choice (every choice runs to the limit: no stop token is checked)
@@ -8,7 +8,8 @@ with a host clock around work that ends in a device synchronise (every step read
 warm-up run of the same shape. It prints one JSON line per measurement: aggregate generated tokens/s of the batched path and of
 the sequential path (each choice in turn through the persistent single-token kernel), and the device time (CUDA events over
 200 launches) of choiceAttnKernel alone at P = 2048 for B = 1 and 8 with the model's attention shape. The GPU name and
-power limit are read in the same run.
+power limit are read in the same run. With --controls every measurement is also taken with the sampling controls on
+(presence and frequency penalty 0.5, 100 logit_bias entries), alternating with the controls off (keys *_controls_tok_s).
 """
 import argparse
 import json
@@ -52,6 +53,9 @@ def time_choices(sess, backend, prompt, n, tokens):
     return sum(len(o) for o in out) / dt
 
 
+CONTROLS = (0.5, 0.5, [(t, 1.0 if t % 2 else -1.0) for t in range(1000, 1100)])
+
+
 def time_attention(eng, B, P, launches=200):
     import torch
     from distributed_llama_b200.ops import cuda_lib as cl
@@ -91,6 +95,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--prompt-lens", default="64,2048")
     ap.add_argument("--ns", default="1,2,4,8")
+    ap.add_argument("--controls", action="store_true", help="also time every measurement with sampling controls on")
     args = ap.parse_args()
     import torch
     from bench import ensure_model
@@ -103,13 +108,21 @@ def main():
         prompt = [(7 * i + 3) % 1000 + 1 for i in range(plen)]
         for n in map(int, args.ns.split(",")):
             row = {"gpu": gpu, "prompt_len": plen, "n": n, "tokens_per_choice": args.tokens}
+            variants = [("", (0.0, 0.0, []))] + ([("_controls", CONTROLS)] if args.controls else [])
             for name, backend in (("batched", sess), ("sequential", Sequential(sess))):
                 if n == 1 and name == "sequential":
                     continue
-                time_choices(sess, backend, prompt, n, args.tokens)   # warm-up
-                rates = sorted(time_choices(sess, backend, prompt, n, args.tokens) for _ in range(args.repeats))
-                row[f"{name}_tok_s"] = round(rates[len(rates) // 2], 1)
-                row[f"{name}_tok_s_min_max"] = [round(rates[0], 1), round(rates[-1], 1)]
+                rates = {suffix: [] for suffix, _ in variants}
+                for rep in range(args.repeats + 1):          # the first round is the warm-up
+                    for suffix, ctl in variants:
+                        sess.sampler.set_controls(*ctl)
+                        r = time_choices(sess, backend, prompt, n, args.tokens)
+                        if rep:
+                            rates[suffix].append(r)
+                for suffix, rs in rates.items():
+                    rs.sort()
+                    row[f"{name}{suffix}_tok_s"] = round(rs[len(rs) // 2], 1)
+                    row[f"{name}{suffix}_tok_s_min_max"] = [round(rs[0], 1), round(rs[-1], 1)]
             print(json.dumps(row), flush=True)
     for B in (1, 8):
         us = time_attention(sess.engine, B, 2048)
