@@ -8,6 +8,11 @@
 
 #include <algorithm>
 #include <cctype>
+#include <condition_variable>
+#include <deque>
+#include <memory>
+#include <mutex>
+#include <thread>
 #include <cstdio>
 #include <cstring>
 #include <ctime>
@@ -133,6 +138,14 @@ uint32_t NaiveCache::resolveDeltaPrompt(std::vector<ChatItem> &messages) {
     }
     clear();
     return 0;
+}
+
+size_t NaiveCache::coveredPrefix(const std::vector<ChatItem> &messages) const {
+    const size_t n = items_.size();
+    if (messages.size() <= n) return 0;
+    for (size_t i = 0; i < n; i++)
+        if (items_[i].msg.role != messages[i].role || items_[i].msg.message != messages[i].message) return 0;
+    return n;
 }
 
 std::string chunkJson(const std::string *delta, bool stop, uint32_t index) {
@@ -352,6 +365,273 @@ void ApiServer::models(HttpRequest &req) const {
     req.writeJson("{\"object\": \"list\", \"data\": [{\"id\": " + jsonEscape(cfg_.modelName) + ", \"object\": \"model\", \"created\": 0, \"owned_by\": \"user\"}]}");
 }
 
+// ---- concurrent requests (--parallel): the rules of distributed_llama_b200.api.SlotScheduler --------------------------------
+
+namespace {
+std::string completionJson(uint32_t nPrompt, const std::vector<std::vector<int32_t>> &out, const std::vector<std::string> &buffers) {
+    uint32_t nCompletion = 0;
+    std::string choices;
+    for (uint32_t i = 0; i < buffers.size(); i++) {
+        nCompletion += (uint32_t)out[i].size();
+        choices += std::string(i ? ", " : "") + "{\"index\": " + std::to_string(i) + ", \"message\": {\"role\": \"assistant\", \"content\": " +
+                   jsonEscape(buffers[i]) + "}, \"finish_reason\": \"stop\"}";
+    }
+    return "{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
+           ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
+           ", \"prompt_tokens\": " + std::to_string(nPrompt) + ", \"total_tokens\": " + std::to_string(nPrompt + nCompletion) +
+           "}, \"choices\": [" + choices + "]}";
+}
+
+// One validated chat completion and, once admitted, its slots and progress.
+struct SlotJob {
+    HttpRequest req;
+    std::vector<ChatItem> messages;
+    bool stream = false, hasSeed = false;
+    int maxTokens = -1;
+    uint32_t n = 1;
+    float temperature = 0.f, topp = 0.9f, presence = 0.f, frequency = 0.f;
+    std::vector<std::pair<int32_t, float>> bias;
+    uint64_t seed = 0;
+    // admitted
+    std::vector<uint32_t> slots;
+    uint32_t P = 0, nPrompt = 0, limit = 0, live = 0;
+    std::vector<std::vector<int32_t>> out;
+    std::vector<EosDetector> dets;
+    std::vector<std::string> pending, buffers;
+};
+
+struct SlotRow {
+    std::shared_ptr<SlotJob> job;
+    int32_t token = 0, pos = 0;
+    std::vector<uint32_t> choices;   // completions this row serves (all n for a greedy request)
+    std::vector<bool> done;
+    uint32_t nDone = 0;
+};
+}  // namespace
+
+void ApiServer::serveParallel(int srv) {
+    const uint32_t N = cfg_.parallel, L = backend_.slotLen();
+    std::vector<NaiveCache> caches(N);
+    std::mutex mu;
+    std::condition_variable cv;
+    std::deque<std::shared_ptr<SlotJob>> queue;
+    int open = 0;           // connections accepted and not yet finished
+    bool accepting = true;
+    const auto closeConn = [&](int fd) {
+        ::close(fd);
+        std::lock_guard<std::mutex> lk(mu);
+        open--;
+        cv.notify_all();
+    };
+    // Reads and validates one connection; chat completions go to the engine thread, which closes them when they end.
+    const auto handle = [&](int fd) {
+        try {
+            HttpRequest req = HttpRequest::read(fd);
+            std::printf("🔷 %s %s\n", req.method.c_str(), req.path.c_str());
+            std::fflush(stdout);
+            if (req.method == "POST" && req.path == "/v1/chat/completions") {
+                if (!req.hasJson || !req.json.isObject()) throw std::runtime_error("request body must be a JSON object");
+                const JsonValue &body = req.json;
+                auto job = std::make_shared<SlotJob>();
+                if (const JsonValue *v = body.find("n")) {
+                    if (v->kind != JsonValue::Number || v->num != (double)(int64_t)v->num || v->num < 1 || v->num > kMaxChoices)
+                        throw std::runtime_error("'n' must be an integer from 1 to 8");
+                    job->n = (uint32_t)v->num;
+                }
+                if (job->n > N) throw std::runtime_error("'n' must not exceed --parallel");
+                job->presence = cfg_.presencePenalty;
+                job->frequency = cfg_.frequencyPenalty;
+                parseControls(body, sampler_.vocabSize(), job->presence, job->frequency, job->bias);
+                for (const JsonValue &m : body.at("messages").arr) job->messages.push_back({m.at("role").str, m.at("content").str});
+                job->stream = body.boolOr("stream", false);
+                job->temperature = (float)body.numberOr("temperature", cfg_.temperature);
+                if (job->temperature < 0.f) throw std::runtime_error("'temperature' must not be negative");
+                job->topp = (float)body.numberOr("top_p", cfg_.topp);
+                if (const JsonValue *sd = body.find("seed")) if (sd->kind == JsonValue::Number) { job->seed = (uint64_t)sd->num; job->hasSeed = true; }
+                job->maxTokens = (int)body.numberOr("max_tokens", -1);
+                job->req = std::move(req);
+                std::lock_guard<std::mutex> lk(mu);
+                queue.push_back(job);
+                cv.notify_all();
+                return;
+            }
+            if (req.method == "OPTIONS") req.writeCors();
+            else if (req.method == "GET" && req.path == "/v1/models") models(req);
+            else req.writeNotFound();
+        } catch (const std::exception &e) {
+            std::printf("Socket error: %s\n", e.what());
+            std::fflush(stdout);
+        }
+        closeConn(fd);
+    };
+    std::thread acceptor([&] {
+        int one = 1, served = 0;
+        while (cfg_.maxRequests == 0 || served < cfg_.maxRequests) {
+            const int fd = ::accept(srv, nullptr, nullptr);
+            if (fd < 0) continue;
+            ::setsockopt(fd, IPPROTO_TCP, TCP_NODELAY, &one, sizeof(one));
+            { std::lock_guard<std::mutex> lk(mu); open++; }
+            std::thread(handle, fd).detach();
+            served++;
+        }
+        std::lock_guard<std::mutex> lk(mu);
+        accepting = false;
+        cv.notify_all();
+    });
+
+    std::vector<std::shared_ptr<SlotJob>> owner(N);
+    std::vector<SlotRow> rows(N);
+    const auto release = [&](const std::shared_ptr<SlotJob> &job) {
+        for (uint32_t s : job->slots) if (owner[s] == job) { owner[s].reset(); rows[s] = SlotRow(); }
+    };
+    const auto fail = [&](const std::shared_ptr<SlotJob> &job, const std::exception &e) {
+        for (uint32_t s : job->slots) caches[s].clear();   // their rows may not match what their caches say
+        std::printf("Socket error: %s\n", e.what());
+        std::fflush(stdout);
+        closeConn(job->req.fd);
+    };
+    const auto finish = [&](const std::shared_ptr<SlotJob> &job) {
+        SlotJob &j = *job;
+        NaiveCache &cache = caches[j.slots[0]];
+        if (j.n == 1) {
+            const uint32_t end = j.P + (uint32_t)j.out[0].size();
+            if (end == L) cache.clear();
+            else cache.push(end, {"assistant", j.buffers[0]});
+        }
+        for (size_t k = 1; k < j.slots.size(); k++) caches[j.slots[k]].copyFrom(cache);   // they hold a copy of the prompt rows
+        if (j.stream) {
+            for (uint32_t i = 0; i < j.n; i++) j.req.writeStreamChunk("data: " + chunkJson(nullptr, true, i) + "\r\n\r\n");
+            j.req.writeStreamChunk("data: [DONE]");
+            j.req.writeStreamEnd();
+        } else {
+            j.req.writeJson(completionJson(j.nPrompt, j.out, j.buffers));
+        }
+        std::printf("🔶 slot %u%s\n", j.slots[0], j.n > 1 ? (" (" + std::to_string(j.n) + " choices)").c_str() : "");
+        std::fflush(stdout);
+        closeConn(j.req.fd);
+    };
+    // Admission: the free slot whose cache covers most of the messages (lowest index on ties), then the lowest other free slots.
+    const auto admit = [&](const std::shared_ptr<SlotJob> &job, const std::vector<uint32_t> &free, uint32_t need) {
+        SlotJob &j = *job;
+        uint32_t first = free[0];
+        size_t best = caches[first].coveredPrefix(j.messages);
+        for (uint32_t s : free) { const size_t c = caches[s].coveredPrefix(j.messages); if (c > best) { best = c; first = s; } }
+        j.slots = {first};
+        for (uint32_t s : free) if (s != first && j.slots.size() < need) j.slots.push_back(s);
+        NaiveCache &cache = caches[first];
+        std::vector<ChatItem> delta = j.messages;
+        const uint32_t start = cache.resolveDeltaPrompt(delta);
+        const GeneratedChat g = gen_.generate(delta, true);
+        const std::vector<int32_t> tokens = tok_.encode(g.content, start == 0, true);
+        j.nPrompt = (uint32_t)tokens.size();
+        j.P = std::min(start + j.nPrompt - 1, L);
+        j.buffers.assign(j.n, g.publicPrompt);
+        j.pending.assign(j.n, std::string());
+        j.dets.assign(j.n, EosDetector(tok_.data().eosIds, stops_, maxLen(stops_), maxLen(stops_)));
+        j.out.assign(j.n, {});
+        if (j.stream) {
+            j.req.writeStreamStart();
+            if (!g.publicPrompt.empty())
+                for (uint32_t i = 0; i < j.n; i++) j.req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false, i) + "\r\n\r\n");
+        }
+        for (const ChatItem &m : delta) cache.push(j.P, m);
+        const uint32_t nPref = j.P - start;
+        if (nPref) backend_.slotPrefill(first, std::vector<int32_t>(tokens.begin(), tokens.begin() + nPref), start);
+        const int32_t token = nPref < tokens.size() ? tokens[nPref] : tokens.back();
+        for (size_t k = 1; k < j.slots.size(); k++) backend_.slotCopy(first, j.slots[k], j.P);
+        const uint64_t seed = j.hasSeed ? j.seed : (j.temperature != 0.f ? sampler_.nextSeed() : 0);
+        for (size_t k = 0; k < j.slots.size(); k++)
+            backend_.slotSampling(j.slots[k], j.n == 1 ? seed : choiceSeed(seed, (uint32_t)k), j.temperature, j.topp, j.presence, j.frequency, j.bias);
+        j.limit = L - j.P;
+        if (j.maxTokens > 0) j.limit = std::min<uint32_t>(j.limit, (uint32_t)j.maxTokens);
+        if (j.limit == 0) { finish(job); return; }
+        j.live = (uint32_t)j.slots.size();
+        for (size_t k = 0; k < j.slots.size(); k++) {
+            SlotRow &r = rows[j.slots[k]];
+            owner[j.slots[k]] = job;
+            r.job = job; r.token = token; r.pos = (int32_t)j.P; r.nDone = 0;
+            r.choices.clear();
+            if (need == 1) for (uint32_t i = 0; i < j.n; i++) r.choices.push_back(i);
+            else r.choices.push_back((uint32_t)k);
+            r.done.assign(r.choices.size(), false);
+        }
+    };
+    const auto onToken = [&](SlotJob &j, uint32_t i, int32_t t) {
+        const std::string piece = tok_.decodeWith(j.pending[i], t);
+        const EosDetectorResult kind = j.dets[i].append(t, piece);
+        if (kind == NOT_EOS || kind == EOS) {
+            const std::string delta = j.dets[i].getDelta();
+            if (!delta.empty()) {
+                if (j.stream) j.req.writeStreamChunk("data: " + chunkJson(&delta, false, i) + "\r\n\r\n");
+                j.buffers[i] += delta;
+            }
+            j.dets[i].reset();
+        }
+        return kind == EOS;
+    };
+
+    std::deque<std::shared_ptr<SlotJob>> waiting;
+    while (true) {
+        bool busy = false;
+        for (const SlotRow &r : rows) busy = busy || r.job != nullptr;
+        {
+            std::unique_lock<std::mutex> lk(mu);
+            if (!busy && waiting.empty()) cv.wait(lk, [&] { return !queue.empty() || (!accepting && open == 0); });
+            while (!queue.empty()) { waiting.push_back(queue.front()); queue.pop_front(); }
+            if (!busy && waiting.empty() && !accepting && open == 0) break;
+        }
+        while (!waiting.empty()) {
+            std::vector<uint32_t> free;
+            for (uint32_t s = 0; s < N; s++) if (!owner[s]) free.push_back(s);
+            const std::shared_ptr<SlotJob> job = waiting.front();
+            const uint32_t need = job->temperature == 0.f ? 1 : job->n;
+            if (free.size() < need) break;
+            waiting.pop_front();
+            try {
+                admit(job, free, need);
+            } catch (const std::exception &e) {
+                release(job);
+                fail(job, e);
+            }
+        }
+        std::vector<int32_t> tokens(N, 0), pos(N, 0);
+        uint32_t active = 0;
+        for (uint32_t s = 0; s < N; s++)
+            if (rows[s].job) { tokens[s] = rows[s].token; pos[s] = rows[s].pos; active |= 1u << s; }
+        if (!active) continue;
+        const std::vector<int32_t> drawn = backend_.slotsStep(tokens, pos, active);
+        for (uint32_t s = 0; s < N; s++) {
+            SlotRow &r = rows[s];
+            if (!r.job) continue;
+            const std::shared_ptr<SlotJob> job = r.job;
+            SlotJob &j = *job;
+            r.token = drawn[s];
+            r.pos++;
+            try {
+                for (size_t c = 0; c < r.choices.size(); c++) {
+                    if (r.done[c]) continue;
+                    const uint32_t i = r.choices[c];
+                    j.out[i].push_back(drawn[s]);
+                    if (onToken(j, i, drawn[s]) || j.out[i].size() >= j.limit) { r.done[c] = true; r.nDone++; }
+                }
+            } catch (const std::exception &e) {
+                release(job);
+                fail(job, e);
+                continue;
+            }
+            if (r.nDone == r.choices.size()) {
+                rows[s] = SlotRow();
+                if (--j.live == 0) {
+                    release(job);
+                    try { finish(job); } catch (const std::exception &e) { fail(job, e); }
+                }
+            }
+        }
+    }
+    acceptor.join();
+    ::close(srv);
+}
+
 void ApiServer::serve() {
     const int srv = ::socket(AF_INET, SOCK_STREAM, 0);
     if (srv < 0) throw std::runtime_error("Cannot create socket");
@@ -367,6 +647,11 @@ void ApiServer::serve() {
     }
     if (cfg_.host == "0.0.0.0" || cfg_.host == "127.0.0.1") std::printf("Server URL: http://localhost:%d/v1/\n", cfg_.port);
     std::fflush(stdout);
+    if (cfg_.parallel > 1) {
+        if (backend_.slots() != cfg_.parallel) { ::close(srv); throw std::runtime_error("the backend has no KV-cache slots for --parallel"); }
+        serveParallel(srv);
+        return;
+    }
     int served = 0;
     while (cfg_.maxRequests == 0 || served < cfg_.maxRequests) {
         const int fd = ::accept(srv, nullptr, nullptr);

@@ -6,6 +6,7 @@
 #include <cstdint>
 #include <functional>
 #include <map>
+#include <stdexcept>
 #include <string>
 #include <vector>
 
@@ -34,6 +35,18 @@ struct InferenceBackend {
     // the sequential path re-seeds the single-sequence generator per choice; these keep its stream across the request
     virtual uint64_t saveSampler() { return 0; }
     virtual void restoreSampler(uint64_t /*saved*/) {}
+    // KV-cache slots (--parallel): independent sequences decoded together, one batched step per token. slots() == 0: unsupported.
+    virtual uint32_t slots() const { return 0; }
+    virtual uint32_t slotLen() const { return 0; }
+    virtual void slotPrefill(uint32_t /*slot*/, const std::vector<int32_t> & /*tokens*/, uint32_t /*pos*/) { throw std::runtime_error("slots unsupported"); }
+    virtual void slotCopy(uint32_t /*src*/, uint32_t /*dst*/, uint32_t /*P*/) { throw std::runtime_error("slots unsupported"); }
+    // seeds slot `slot`'s generator, zeroes its counts and sets its temperature (0: arg-max), top-p, penalties and logit bias
+    virtual void slotSampling(uint32_t /*slot*/, uint64_t /*seed*/, float /*temperature*/, float /*topp*/, float /*presence*/, float /*frequency*/,
+                              const std::vector<std::pair<int32_t, float>> & /*bias*/) { throw std::runtime_error("slots unsupported"); }
+    // row b feeds tokens[b] at pos[b] of slot b (active rows: bit b of activeMask); returns each active row's draw
+    virtual std::vector<int32_t> slotsStep(const std::vector<int32_t> & /*tokens*/, const std::vector<int32_t> & /*pos*/, uint32_t /*activeMask*/) {
+        throw std::runtime_error("slots unsupported");
+    }
 };
 
 constexpr uint32_t kMaxChoices = 8;   // the engine's widest batch: one row per choice
@@ -73,6 +86,9 @@ public:
     size_t size() const { return items_.size(); }
     // Returns the position generation restarts from and trims `messages` to the part that still has to be evaluated.
     uint32_t resolveDeltaPrompt(std::vector<ChatItem> &messages);
+    // How many cached messages resolveDeltaPrompt would re-use for `messages` (0: none).
+    size_t coveredPrefix(const std::vector<ChatItem> &messages) const;
+    void copyFrom(const NaiveCache &o) { items_ = o.items_; }
 private:
     struct Item { uint32_t endPos; ChatItem msg; };
     std::vector<Item> items_;
@@ -90,6 +106,7 @@ struct ApiConfig {
     float presencePenalty = 0.f, frequencyPenalty = 0.f;   // defaults of the request fields
     uint64_t seed = 0;
     int maxRequests = 0;   // 0 = serve forever
+    uint32_t parallel = 1; // > 1: that many requests decoded together in KV-cache slots (serveParallel)
 };
 
 class ApiServer {
@@ -97,8 +114,9 @@ public:
     ApiServer(InferenceBackend &backend, Tokenizer &tokenizer, const ApiConfig &cfg);
     void complete(HttpRequest &req);
     void models(HttpRequest &req) const;
-    void serve();          // accept loop
+    void serve();          // accept loop (parallel > 1: serveParallel)
 private:
+    void serveParallel(int srv);   // one engine thread, a reader thread per connection; same rules as api.SlotScheduler
     InferenceBackend &backend_;
     Tokenizer &tok_;
     ApiConfig cfg_;

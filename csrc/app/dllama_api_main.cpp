@@ -2,6 +2,7 @@
 // GPU — api_server.cpp (HTTP, JSON, NaiveCache, templates, stop detection) over NativeEngine. Multi-GPU serving: ./dllama-api --gpus N.
 #include <chrono>
 #include <cstdio>
+#include <cstdlib>
 #include <ctime>
 #include <stdexcept>
 #include <string>
@@ -39,12 +40,44 @@ struct EngineBackend : InferenceBackend {
     }
     uint64_t saveSampler() override { return e.nRanks() > 1 ? tp.samplerState() : 0; }
     void restoreSampler(uint64_t saved) override { if (e.nRanks() > 1) tp.restoreSampler(saved); }
+    // KV-cache slots (--parallel > 1): one GPU only, so the calls go straight to the engine
+    uint32_t slotCount = 0;
+    uint32_t slots() const override { return slotCount; }
+    uint32_t slotLen() const override { return e.slotLen(); }
+    void slotPrefill(uint32_t slot, const std::vector<int32_t> &tokens, uint32_t pos) override { e.slotPrefill(slot, tokens, pos); }
+    void slotCopy(uint32_t src, uint32_t dst, uint32_t P) override { e.slotCopy(src, dst, P); }
+    void slotSampling(uint32_t slot, uint64_t seed, float temperature, float topp, float presence, float frequency,
+                      const std::vector<std::pair<int32_t, float>> &bias) override {
+        e.slotSampling(slot, seed, temperature, topp, presence, frequency, bias);
+    }
+    std::vector<int32_t> slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask) override {
+        return e.slotsStep(tokens, pos, activeMask);
+    }
 };
+
+// A --parallel value this configuration cannot serve: reported in one line, not retried.
+struct ParallelRefused : std::runtime_error {
+    using std::runtime_error::runtime_error;
+};
+
+// Why --parallel `parallel` cannot run here (empty: it can); the rules of distributed_llama_b200.api.parallel_refusal.
+std::string parallelRefusal(uint32_t parallel, uint32_t nRanks, uint32_t nExperts) {
+    if (parallel < 1 || parallel > kMaxChoices) return "--parallel must be from 1 to 8";
+    if (parallel == 1) return "";
+    if (nRanks > 1) return "--parallel > 1 runs on one GPU only (workers cannot mirror slot steps yet)";
+    if (nExperts > 0) return "--parallel > 1 does not support mixture-of-experts models (the batched step has no MoE path)";
+    const char *c = std::getenv("DL_COLLECTIVES");
+    if (c && std::string(c) == "nccl") return "--parallel > 1 does not support DL_COLLECTIVES=nccl";
+    if (std::getenv("DL_HOST_SAMPLER")) return "--parallel > 1 samples on the device: unset DL_HOST_SAMPLER";
+    return "";
+}
 
 const char *kUsage =
     "Usage: dllama-api-native --model <path> --tokenizer <path> [--host <addr>] [--port <p>] [--max-seq-len <n>]\n"
     "        [--temperature <t>] [--topp <p>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]\n"
     "        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--gpu-index <i>]\n"
+    "        [--parallel <n>]  decode up to n (1..8) chat requests together, each in its own KV-cache slot of floor(context / n)\n"
+    "                       tokens; one GPU and dense models only\n"
     "        [--gpus <n>]   tensor parallel over n GPUs: a supervisor forks one process per GPU (rank 0 serves HTTP) and restarts\n"
     "                       the whole job 3 s after any rank fails\n";
 
@@ -59,6 +92,12 @@ int serveOnce(const std::string &model, const std::string &tokenizer, uint32_t m
                     engine.multicast() ? "the NVSwitch multicast mapping (multimem.st)" : "NVLink peer memory");
     std::printf("💿 Weights loaded\n");
     EngineBackend backend(engine, job);
+    const std::string why = parallelRefusal(cfg.parallel, job.nRanks, engine.header().nExperts);
+    if (!why.empty()) throw ParallelRefused(why);
+    if (cfg.parallel > 1) {
+        engine.setSlots(cfg.parallel);
+        backend.slotCount = cfg.parallel;
+    }
     ApiServer server(backend, tok, cfg);
     server.serve();
     return 0;
@@ -72,12 +111,12 @@ int main(int argc, char **argv) {
     cfg.seed = (uint64_t)std::time(nullptr);
     uint32_t maxSeqLen = 0;
     int gpu = 0;
-    uint32_t gpus = 1;
+    uint32_t gpus = 1, workers = 0;
     try {
         for (int i = 1; i < argc;) {
             const std::string name = argv[i];
             if (name == "--help" || name == "-h" || name == "--usage") { std::fprintf(stderr, "%s", kUsage); return 0; }
-            if (name == "--workers") { i++; while (i < argc && argv[i][0] != '-') i++; continue; }
+            if (name == "--workers") { i++; while (i < argc && argv[i][0] != '-') { i++; workers++; } continue; }
             if (i + 1 >= argc) throw std::runtime_error("Missing value for " + name);
             const std::string v = argv[i + 1];
             if (name == "--model") model = v;
@@ -94,6 +133,7 @@ int main(int argc, char **argv) {
             else if (name == "--gpu-index") gpu = std::max(0, std::stoi(v));
             else if (name == "--gpus") gpus = (uint32_t)std::max(1, std::stoi(v));
             else if (name == "--max-requests") cfg.maxRequests = std::stoi(v);
+            else if (name == "--parallel") cfg.parallel = (uint32_t)std::max(0, std::stoi(v));
             else if (name == "--buffer-float-type" || name == "--nthreads" || name == "--net-turbo" || name == "--gpu-segments") {}
             else throw std::runtime_error("Unknown option: " + name);
             i += 2;
@@ -104,6 +144,10 @@ int main(int argc, char **argv) {
         std::printf("🚨 Critical error: %s\n", e.what());
         return 1;
     }
+    {
+        const std::string why = parallelRefusal(cfg.parallel, gpus + workers, 0);
+        if (!why.empty()) { std::fprintf(stderr, "%s\n", why.c_str()); return 1; }
+    }
     const size_t slash = model.find_last_of("/\\");
     cfg.modelName = slash == std::string::npos ? model : model.substr(slash + 1);
     // the reference retries its whole inference app every 3 s on errors (dllama-api.cpp:616-628)
@@ -112,6 +156,9 @@ int main(int argc, char **argv) {
             try {
                 TpJob job;
                 return serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job);
+            } catch (const ParallelRefused &e) {
+                std::fprintf(stderr, "%s\n", e.what());
+                return 1;
             } catch (const std::exception &e) {
                 std::printf("🚨 Inference error: %s\n🔄 Retrying in 3 seconds...\n", e.what());
                 std::fflush(stdout);

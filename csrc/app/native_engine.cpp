@@ -470,6 +470,44 @@ std::vector<int32_t> NativeEngine::choicesStep(const std::vector<int32_t> &token
     return out;
 }
 
+void NativeEngine::setSlots(uint32_t n) {
+    engCheck(dl_engine_set_slots(impl_->engine, n), "dl_engine_set_slots");
+    slots_ = n;
+}
+
+uint32_t NativeEngine::slotLen() const { return dl_engine_slot_len(impl_->engine); }
+
+void NativeEngine::slotPrefill(uint32_t slot, const std::vector<int32_t> &tokens, uint32_t pos) {
+    if (pos + tokens.size() > slotLen()) throw std::runtime_error("position beyond the slot length");
+    for (size_t i = 0; i < tokens.size();) {
+        const uint32_t n = (uint32_t)std::min<size_t>(tokens.size() - i, maxPrefill_);
+        setInputs(tokens.data() + i, n, pos + (uint32_t)i, true);
+        engCheck(dl_engine_slot_prefill(impl_->engine, slot, n, pos + (uint32_t)i, impl_->stream), "dl_engine_slot_prefill");
+        i += n;
+    }
+}
+
+void NativeEngine::slotCopy(uint32_t src, uint32_t dst, uint32_t P) {
+    engCheck(dl_engine_slot_copy(impl_->engine, src, dst, P, impl_->stream), "dl_engine_slot_copy");
+}
+
+void NativeEngine::slotSampling(uint32_t slot, uint64_t seed, float temperature, float topp, float presence, float frequency,
+                                const std::vector<std::pair<int32_t, float>> &bias) {
+    std::vector<int32_t> ids;
+    std::vector<float> vals;
+    for (const auto &b : bias) { ids.push_back(b.first); vals.push_back(b.second); }
+    engCheck(dl_engine_slot_sampling(impl_->engine, slot, seed, temperature, topp, presence, frequency, ids.data(), vals.data(), (int)ids.size(),
+                                     impl_->stream), "dl_engine_slot_sampling");
+}
+
+std::vector<int32_t> NativeEngine::slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask) {
+    if (tokens.size() != slots_ || pos.size() != slots_) throw std::runtime_error("slotsStep: one token and position per slot");
+    std::vector<int32_t> out(slots_, -1);
+    const uint32_t inactive = ~activeMask & ((1u << slots_) - 1u);
+    engCheck(dl_engine_slots_step(impl_->engine, tokens.data(), pos.data(), inactive, out.data(), impl_->stream), "dl_engine_slots_step");
+    return out;
+}
+
 uint64_t NativeEngine::syncNs() const { return nRanks_ > 1 ? (uint64_t)dl_engine_sync_ns(impl_->engine) : 0; }
 
 void NativeEngine::linkBytes(uint32_t nTokens, uint64_t &sent, uint64_t &received) const {

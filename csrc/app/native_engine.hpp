@@ -62,6 +62,15 @@ public:
     std::vector<int32_t> choicesFirst(int32_t token, uint32_t P, uint32_t n, float temperature, float topp);
     std::vector<int32_t> choicesStep(const std::vector<int32_t> &tokens, uint32_t P, uint32_t C, uint32_t j, uint32_t activeMask, float temperature,
                                      float topp);
+    // KV-cache slots (csrc/cuda/slots.cu): n <= 8 independent sequences, each in its own floor(seqLen / n) rows of the cache, decoded
+    // together by slotsStep. Single GPU, dense q40 models. Row b of a step is slot b (activeMask bit b); inactive rows return -1.
+    void setSlots(uint32_t n);
+    uint32_t slotLen() const;
+    void slotPrefill(uint32_t slot, const std::vector<int32_t> &tokens, uint32_t pos);
+    void slotCopy(uint32_t src, uint32_t dst, uint32_t P);
+    void slotSampling(uint32_t slot, uint64_t seed, float temperature, float topp, float presence, float frequency,
+                      const std::vector<std::pair<int32_t, float>> &bias);
+    std::vector<int32_t> slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask);
     // n greedy steps back to back on the device without host round trips; returns the generated tokens.
     std::vector<int32_t> decodeGreedy(int32_t firstToken, uint32_t pos, uint32_t nSteps);
     void synchronize();
@@ -83,6 +92,7 @@ private:
 
     ModelHeader h_;
     std::vector<TensorEntry> dir_;
+    uint32_t slots_ = 1;
     uint32_t seqLen_ = 0, maxBatch_ = 8, maxPrefill_ = 192, nSplits_ = 1, qkvDim_ = 0;
     uint32_t rank_ = 0, nRanks_ = 1, kvRank_ = 0, kvSlices_ = 1;          // tensor-parallel placement of this process
     uint32_t headsL_ = 0, kvHeadsL_ = 0, ffL_ = 0, vocabL_ = 0;          // per-rank slice sizes

@@ -63,7 +63,7 @@ __global__ void __launch_bounds__(128) ropeKvKernel(RopeKvArgs a) {
     } else if (!inactive && cacheRow < a.seqLen) {
         const uint32_t kvh = isK ? head - a.nHeads : head - a.nHeads - a.nKvHeads;
         __nv_bfloat16 *cache = isK ? a.kCache : a.vCache;
-        __nv_bfloat162 *dst = reinterpret_cast<__nv_bfloat162 *>(cache + ((size_t)kvh * a.seqLen + cacheRow) * hd);
+        __nv_bfloat162 *dst = reinterpret_cast<__nv_bfloat162 *>(cache + t * a.slotStride + ((size_t)kvh * a.seqLen + cacheRow) * hd);
         dst[j] = __floats2bfloat162_rn(v.x, v.y);
     }
 }

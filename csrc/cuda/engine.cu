@@ -54,6 +54,12 @@ struct Engine {
     float *ctlBias = nullptr;
     bool ctlActive = false, ctlBiasActive = false;
     float ctlPresence = 0.f, ctlFrequency = 0.f;
+    // KV-cache slots (dl_engine_set_slots): slots > 1 splits every layer's cache into `slots` blocks of slotLen rows
+    uint32_t slots = 1, slotLen = 0;
+    float *slotParams = nullptr;       // [kChoiceRngSlots][4] per-slot {temperature, top-p, presence, frequency}
+    float *slotBias = nullptr;         // [kChoiceRngSlots][vocabFull] per-slot logit bias
+    int32_t *slotStage = nullptr;      // pinned [3][kChoiceRngSlots]: tokens, positions in; drawn tokens out
+    cudaEvent_t slotStaged = nullptr;  // the uploads of the staged tokens / positions are done: the buffer may be rewritten
     bool prefillFusedAr = false; // TP prefill: GEMM + all-reduce in one kernel (DL_PREFILL_FUSED_AR=1) instead of GEMM, then all-reduce kernel
     bool tcAttn = true;          // prefill attention on the tensor cores (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
     bool fusedAttn = true, fusedArgmax = true, useTma = true;   // debugging switches (DL_NO_FUSED_ATTN / DL_NO_FUSED_ARGMAX / DL_NO_TMA)
@@ -186,15 +192,21 @@ static int engineDecodeMega(Engine &e, bool greedyAdvance, cudaStream_t stream) 
 // Geometry of a choices step (see choices.cu): nb rows at rotary position P + 1 + j, row b stored at P + 1 + b * C + j.
 struct ChoiceStep { uint32_t P, C, j, inactiveMask; };
 
+// A slots step (see slots.cu): row b is KV-cache slot b at position pos[b].
+struct SlotStep { uint32_t inactiveMask; };
+
+static uint64_t slotElems(const Engine &e) { return (uint64_t)e.cfg.nKvHeads * e.slotLen * e.cfg.headDim; }
+
 // logitsMode: 0 = none (prefill chunk), 1 = logits of the last token in the batch into logits[0], 2 = all tokens.
-// ch: a choices step instead of a batch of consecutive tokens (logitsMode 2, dense layers only).
-static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, cudaStream_t stream, const ChoiceStep *ch = nullptr) {
+// ch: a choices step instead of a batch of consecutive tokens (logitsMode 2, dense layers only); sl: a slots step (same limits).
+static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, cudaStream_t stream, const ChoiceStep *ch = nullptr,
+                         const SlotStep *sl = nullptr) {
     const EngineConfig &c = e.cfg;
     const bool pdl = c.usePdl != 0;
     const uint32_t qDim = c.nHeads * c.headDim, kvDim = c.nKvHeads * c.headDim, qkvDim = qDim + 2 * kvDim;
     if (nb < 1 || (uint32_t)nb > c.maxBatch || (nb & (nb - 1))) return -10;
     e.lastDecodeMega = false;
-    if (ch && (c.nExperts > 0 || logitsMode != 2 || greedyAdvance)) return -14;
+    if ((ch || sl) && (c.nExperts > 0 || logitsMode != 2 || greedyAdvance)) return -14;
     if (nb == 1 && logitsMode == 1 && e.useMega) {
         const int r = engineDecodeMega(e, greedyAdvance, stream);
         if (r != 1) { e.lastDecodeMega = r == 0; return r; }
@@ -215,7 +227,20 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
         a.qs = (const uint32_t *)L.qkvQs; a.scales = (const __half *)L.qkvSc; a.d = qkvDim; a.n = c.dim;
         a.in = e.g.x; a.inStride = c.dim; a.normW = L.norm0; a.eps = c.eps; a.out = e.g.qkv; a.outStride = qkvDim; a.trace = nextTrace();
         DL_TRY(gemvSel(e, PRO_RMSNORM_, EPI_STORE_, nb, a, c.numSms, stream, pdl));
-        if (ch) {
+        if (sl) {
+            // 2+3. qk-norm + rope + K/V append at row pos[b] of slot b, then attention of each row over its own slot
+            RopeKvArgs r{};
+            r.qkv = e.g.qkv; r.qkvStride = qkvDim; r.pos = e.g.pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
+            r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = e.slotLen;
+            r.kCache = (__nv_bfloat16 *)L.kCache; r.vCache = (__nv_bfloat16 *)L.vCache; r.slotStride = slotElems(e); r.inactiveMask = sl->inactiveMask;
+            DL_TRY(launchRopeKv(r, nb, stream, pdl));
+            SlotAttnArgs t{};
+            t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache; t.slotStride = r.slotStride;
+            t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.L = e.slotLen; t.nSplits = c.nSplits;
+            t.B = (uint32_t)nb; t.inactiveMask = sl->inactiveMask;
+            t.partial = e.g.attnPartial; t.counters = e.g.attnCounters; t.out = e.g.z; t.outStride = qDim;
+            DL_TRY(launchSlotAttn(t, stream, pdl));
+        } else if (ch) {
             // 2+3. qk-norm + rope + K/V append at the choices' own rows, then attention over the shared prompt + own rows
             RopeKvArgs r{};
             r.qkv = e.g.qkv; r.qkvStride = qkvDim; r.pos = e.g.pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
@@ -315,13 +340,17 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
 }
 
 // Prompt chunk of T <= maxPrefill tokens on the tensor-core path. Logits (optional) are produced for the last token.
-static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cudaStream_t stream) {
+// slot >= 0: the chunk goes into KV-cache slot `slot` (a cache of its own of slotLen rows).
+static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cudaStream_t stream, int slot = -1) {
     const EngineConfig &c = e.cfg;
     const GlobalPtrs &g = e.g;
     const bool pdl = c.usePdl != 0;   // every kernel of this chain waits (griddepcontrol.wait) before touching its predecessor's data
     const uint32_t qDim = c.nHeads * c.headDim, kvDim = c.nKvHeads * c.headDim, qkvDim = qDim + 2 * kvDim;
     if (T < 1 || T > g.maxPrefill || T > 256) return -11;
     if (c.wType != 0) return -35;   // tensor-core path: q40 matrices
+    const uint32_t seqLen = slot >= 0 ? e.slotLen : c.seqLen;
+    const uint64_t cacheOff = slot >= 0 ? (uint64_t)slot * slotElems(e) : 0;
+    if (slot >= 0 && ((uint32_t)slot >= e.slots || p0 + T > seqLen)) return -60;
     const bool tp = e.comm.nRanks > 1;
     ArArgs arP{};
     if (tp) {
@@ -338,15 +367,15 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
         DL_TRY(gemmQ40Tc(GEPI_STORE_F32_, L.qkvQs, L.qkvSc, qkvDim, c.dim, g.pxn, c.dim, T, g.pqkv, qkvDim, c.numSms, stream, pdl));
         RopeKvArgs r{};
         r.qkv = g.pqkv; r.qkvStride = qkvDim; r.pos = g.pPos; r.rope = g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
-        r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = c.seqLen;
-        r.kCache = (__nv_bfloat16 *)L.kCache; r.vCache = (__nv_bfloat16 *)L.vCache;
+        r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = seqLen;
+        r.kCache = (__nv_bfloat16 *)L.kCache + cacheOff; r.vCache = (__nv_bfloat16 *)L.vCache + cacheOff;
         DL_TRY(launchRopeKv(r, (int)T, stream, pdl));
         int attnRc = 1;
         if (e.tcAttn) {
             // tensor-core attention over the whole chunk: the tokens of a chunk sit at consecutive positions p0 .. p0 + T - 1
             AttnPrefillArgs ap{};
             ap.qkv = g.pqkv; ap.qkvStride = qkvDim; ap.T = T; ap.p0 = p0; ap.nHeads = c.nHeads; ap.nKvHeads = c.nKvHeads;
-            ap.headDim = c.headDim; ap.seqLen = c.seqLen; ap.kCache = r.kCache; ap.vCache = r.vCache;
+            ap.headDim = c.headDim; ap.seqLen = seqLen; ap.kCache = r.kCache; ap.vCache = r.vCache;
             ap.out = (__nv_bfloat16 *)g.pzb; ap.outStride = qDim;
             attnRc = launchAttnPrefillTc(ap, stream, pdl);
             if (attnRc < 0) return attnRc;
@@ -354,7 +383,7 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
         if (attnRc == 1) {
             AttnArgs t{};
             t.qkv = g.pqkv; t.qkvStride = qkvDim; t.pos = g.pPos; t.kCache = r.kCache; t.vCache = r.vCache;
-            t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.seqLen = c.seqLen; t.nSplits = 1;
+            t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.seqLen = seqLen; t.nSplits = 1;
             t.partial = g.pAttnPartial; t.counters = g.pAttnCounters; t.out = nullptr; t.outStride = qDim; t.outBf16 = (__nv_bfloat16 *)g.pzb;
             DL_TRY(launchAttnDecode(t, (int)T, stream, pdl));
         }
@@ -433,6 +462,10 @@ DL_EXPORT void dl_engine_destroy(void *h) {
     if (e->abortHost) cudaFreeHost(e->abortHost);
     if (e->ctlCounts) cudaFree(e->ctlCounts);
     if (e->ctlBias) cudaFree(e->ctlBias);
+    if (e->slotParams) cudaFree(e->slotParams);
+    if (e->slotBias) cudaFree(e->slotBias);
+    if (e->slotStage) cudaFreeHost(e->slotStage);
+    if (e->slotStaged) cudaEventDestroy(e->slotStaged);
     delete e;
 }
 
@@ -539,6 +572,17 @@ static int ensureSampler(Engine *e) {
     return 0;
 }
 
+// Count rows [1 + kChoiceRngSlots][vocabFull] of the sampling controls (row 0: single sequence, row 1 + b: choice or slot b).
+static int ensureCounts(Engine *e, cudaStream_t stream) {
+    const uint32_t full = e->cfg.vocab * (e->comm.nRanks > 1 ? e->comm.nRanks : 1);
+    const size_t bytes = (size_t)(1 + kChoiceRngSlots) * full * sizeof(uint32_t);
+    if (!e->ctlCounts) {
+        DL_CUDA_CHECK(cudaMalloc(&e->ctlCounts, bytes));
+        DL_CUDA_CHECK(cudaMemsetAsync(e->ctlCounts, 0, bytes, stream));
+    }
+    return 0;
+}
+
 DL_EXPORT int dl_engine_sampler_seed(void *h, unsigned long long seed) {
     Engine *e = (Engine *)h;
     DL_TRY(ensureSampler(e));
@@ -571,10 +615,7 @@ DL_EXPORT int dl_engine_set_sampling_controls(void *h, float presence, float fre
     e->ctlActive = false;   // set again only once every buffer below is in place
     if (presence == 0.f && frequency == 0.f && nBias == 0) return 0;
     DL_TRY(ensureSampler(e));
-    if (!e->ctlCounts) {
-        DL_CUDA_CHECK(cudaMalloc(&e->ctlCounts, (size_t)rows * full * sizeof(uint32_t)));
-        DL_CUDA_CHECK(cudaMemsetAsync(e->ctlCounts, 0, (size_t)rows * full * sizeof(uint32_t), stream));
-    }
+    DL_TRY(ensureCounts(e, stream));
     if (!e->ctlBias) DL_CUDA_CHECK(cudaMalloc(&e->ctlBias, (size_t)full * sizeof(float)));
     std::vector<float> bias;
     if (nBias > 0) {
@@ -796,5 +837,138 @@ DL_EXPORT int dl_engine_decode_graph(void *h, int nSteps, cudaStream_t stream) {
     Engine *e = (Engine *)h;
     if (!e->decodeGraph) return -20;
     for (int i = 0; i < nSteps; i++) DL_CUDA_CHECK(cudaGraphLaunch(e->decodeGraph, stream));
+    return 0;
+}
+
+// ---- KV-cache slots: up to 8 independent sequences decoded together (slots.cu) ----------------------------------------------------
+
+// Splits every layer's K/V cache into n equal slots of floor(seqLen / n) rows (no extra memory) and allocates the per-slot sampling
+// state. Single GPU, dense (non-MoE) q40 layers only. n = 1 leaves the engine exactly as it was.
+DL_EXPORT int dl_engine_set_slots(void *h, uint32_t n) {
+    Engine *e = (Engine *)h;
+    const dl::EngineConfig &c = e->cfg;
+    if (n < 1 || n > kChoiceRngSlots) return -61;
+    if (n > 1 && (e->comm.nRanks > 1 || c.nExperts > 0 || c.wType != 0)) return -62;
+    uint32_t nb = 1;
+    while (nb < n) nb *= 2;
+    if (nb > c.maxBatch) return -63;
+    e->slots = n;
+    e->slotLen = c.seqLen / n;
+    if (n == 1) return 0;
+    DL_TRY(ensureSampler(e));
+    DL_TRY(ensureCounts(e, 0));
+    const uint32_t full = c.vocab;
+    if (!e->slotParams) {
+        DL_CUDA_CHECK(cudaMalloc(&e->slotParams, kChoiceRngSlots * 4 * sizeof(float)));
+        DL_CUDA_CHECK(cudaMemset(e->slotParams, 0, kChoiceRngSlots * 4 * sizeof(float)));
+        DL_CUDA_CHECK(cudaMalloc(&e->slotBias, (size_t)kChoiceRngSlots * full * sizeof(float)));
+        DL_CUDA_CHECK(cudaMemset(e->slotBias, 0, (size_t)kChoiceRngSlots * full * sizeof(float)));
+        DL_CUDA_CHECK(cudaHostAlloc((void **)&e->slotStage, 3 * kChoiceRngSlots * sizeof(int32_t), cudaHostAllocDefault));
+        DL_CUDA_CHECK(cudaEventCreateWithFlags(&e->slotStaged, cudaEventDisableTiming));
+    }
+    DL_CUDA_CHECK(cudaDeviceSynchronize());
+    return 0;
+}
+
+DL_EXPORT uint32_t dl_engine_slot_len(void *h) {
+    Engine *e = (Engine *)h;
+    return e->slots > 1 ? e->slotLen : e->cfg.seqLen;
+}
+
+// Prompt chunk of T tokens (staged in pTokens / pPos at positions p0 .. p0 + T - 1 < slot length) into slot `slot`: the prefill
+// kernels of dl_engine_prefill with the slot's cache and length. No logits.
+DL_EXPORT int dl_engine_slot_prefill(void *h, uint32_t slot, uint32_t T, uint32_t p0, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    if (e->slots < 2) return -64;
+    return dl::enginePrefill(*e, T, p0, 0, stream, (int)slot);
+}
+
+// Copies rows [0, P) of slot src into slot dst, every layer and KV head (several completions of one prompt).
+DL_EXPORT int dl_engine_slot_copy(void *h, uint32_t src, uint32_t dst, uint32_t P, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    const dl::EngineConfig &c = e->cfg;
+    if (e->slots < 2 || src >= e->slots || dst >= e->slots || P > e->slotLen) return -64;
+    if (src == dst || P == 0) return 0;
+    const size_t rowBytes = (size_t)c.headDim * sizeof(__nv_bfloat16), pitch = (size_t)e->slotLen * rowBytes;
+    const size_t slotBytes = (size_t)c.nKvHeads * pitch;
+    for (const dl::LayerPtrs &L : e->layers)
+        for (void *cache : {L.kCache, L.vCache})
+            DL_CUDA_CHECK(cudaMemcpy2DAsync((uint8_t *)cache + dst * slotBytes, pitch, (const uint8_t *)cache + src * slotBytes, pitch,
+                                            (size_t)P * rowBytes, c.nKvHeads, cudaMemcpyDeviceToDevice, stream));
+    return 0;
+}
+
+// The sampling settings of the sequence admitted to slot `slot`: seeds its generator (rngState[kChoiceRngSlots + slot]), zeroes its
+// count row (1 + slot) and sets its temperature (0: arg-max), top-p, penalties and logit bias (nBias (id, value) pairs, ids below the
+// sampled vocabulary). The uploads are complete when the call returns.
+DL_EXPORT int dl_engine_slot_sampling(void *h, uint32_t slot, unsigned long long seed, float temperature, float topp, float presence,
+                                      float frequency, const int32_t *ids, const float *vals, int nBias, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    if (e->slots < 2 || slot >= e->slots) return -64;
+    const uint32_t full = e->cfg.vocab;
+    const uint32_t n = (e->vocabLimit && e->vocabLimit < full) ? e->vocabLimit : full;
+    if (!(temperature >= 0.f) || nBias < 0) return -52;
+    for (int i = 0; i < nBias; i++) if (ids[i] < 0 || (uint32_t)ids[i] >= n) return -53;
+    if (seed == 0) seed = 0x9E3779B97F4A7C15ull;   // xorshift state must not be zero
+    std::vector<float> bias(full, 0.f);
+    for (int i = 0; i < nBias; i++) bias[ids[i]] = vals[i];
+    const float params[4] = {temperature, topp, presence, frequency};
+    DL_CUDA_CHECK(cudaMemcpyAsync(e->rngState + kChoiceRngSlots + slot, &seed, sizeof(seed), cudaMemcpyHostToDevice, stream));
+    DL_CUDA_CHECK(cudaMemcpyAsync(e->slotParams + 4 * slot, params, sizeof(params), cudaMemcpyHostToDevice, stream));
+    DL_CUDA_CHECK(cudaMemcpyAsync(e->slotBias + (size_t)slot * full, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
+    DL_CUDA_CHECK(cudaMemsetAsync(e->ctlCounts + (size_t)(1 + slot) * full, 0, (size_t)full * sizeof(uint32_t), stream));
+    DL_CUDA_CHECK(cudaStreamSynchronize(stream));   // host temporaries
+    return 0;
+}
+
+// Rows of a slots step: the power of two >= slots, so a row's arithmetic does not depend on how many slots are busy.
+static int slotRows(const Engine *e) {
+    int nb = 1;
+    while ((uint32_t)nb < e->slots) nb *= 2;
+    return nb;
+}
+
+// Forward of one slots step: row b feeds tokens[b] at position pos[b] (host arrays of `slots` entries) and writes K/V row pos[b]
+// of slot b. Rows set in inactiveMask (and the padding rows up to the power of two) write nothing. Logits of every row land in
+// logits[0..nb).
+DL_EXPORT int dl_engine_slots_forward(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    if (e->slots < 2) return -64;
+    const int nb = slotRows(e);
+    uint32_t mask = inactiveMask;
+    for (int b = (int)e->slots; b < nb; b++) mask |= 1u << b;
+    if ((mask & ((1u << nb) - 1u)) == ((1u << nb) - 1u)) return -65;   // nothing to run
+    int32_t *tok = e->slotStage, *ps = e->slotStage + kChoiceRngSlots;
+    DL_CUDA_CHECK(cudaEventSynchronize(e->slotStaged));   // the previous call's uploads have read the staging buffer
+    for (int b = 0; b < nb; b++) {
+        const bool on = !((mask >> b) & 1u);
+        if (on && (pos[b] < 0 || (uint32_t)pos[b] >= e->slotLen)) return -66;
+        tok[b] = on ? tokens[b] : 0;
+        ps[b] = on ? pos[b] : 0;
+    }
+    DL_CUDA_CHECK(cudaMemcpyAsync(e->g.tokens, tok, nb * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+    DL_CUDA_CHECK(cudaMemcpyAsync(e->g.pos, ps, nb * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+    DL_CUDA_CHECK(cudaEventRecord(e->slotStaged, stream));
+    const dl::SlotStep sl{mask};
+    return dl::engineForward(*e, nb, 2, false, stream, nullptr, &sl);
+}
+
+// dl_engine_slots_forward, then every active row draws its next token with its slot's settings (dl_engine_slot_sampling) into
+// out[b]; inactive rows leave out[b] as it was. One device-to-host copy for all rows; returns once the tokens are on the host.
+DL_EXPORT int dl_engine_slots_step(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    DL_TRY(dl_engine_slots_forward(h, tokens, pos, inactiveMask, stream));
+    const dl::EngineConfig &c = e->cfg;
+    const int nb = slotRows(e);
+    uint32_t mask = inactiveMask;
+    for (int b = (int)e->slots; b < nb; b++) mask |= 1u << b;
+    const uint32_t n = (e->vocabLimit && e->vocabLimit < c.vocab) ? e->vocabLimit : c.vocab;
+    const dl::SampleControls ctl{e->slotBias, e->ctlCounts + c.vocab, c.vocab, 0.f, 0.f, c.vocab};
+    DL_TRY(dl::launchSampleRows(e->g.logits, c.vocab, e->probScratch, n, 0.f, 0.f, e->rngState + kChoiceRngSlots, e->g.tokens, (uint32_t)nb, mask,
+                                nullptr, nullptr, 1, stream, &ctl, e->slotParams));
+    int32_t *drawn = e->slotStage + 2 * kChoiceRngSlots;
+    DL_CUDA_CHECK(cudaMemcpyAsync(drawn, e->g.tokens, nb * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+    DL_CUDA_CHECK(cudaStreamSynchronize(stream));
+    for (uint32_t b = 0; b < e->slots; b++) if (!((mask >> b) & 1u)) out[b] = drawn[b];
     return 0;
 }

@@ -99,6 +99,15 @@ int dl_engine_sampler_seed_rows(void *h, const unsigned long long *seeds, int n)
 unsigned long long dl_engine_sampler_state(void *h);   // single-sequence generator state (seed with it to continue the stream)
 int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, float temperature, float topp, int firstStep, cudaStream_t stream);
 int dl_engine_choices_forward(void *h, int nb, uint32_t P, uint32_t C, uint32_t j, uint32_t inactiveMask, cudaStream_t stream);
+// KV-cache slots (csrc/cuda/slots.cu): n <= 8 independent sequences, slot s = rows [0, floor(seqLen / n)) of its own cache block
+int dl_engine_set_slots(void *h, uint32_t n);
+uint32_t dl_engine_slot_len(void *h);
+int dl_engine_slot_prefill(void *h, uint32_t slot, uint32_t T, uint32_t p0, cudaStream_t stream);   // T tokens staged in pTokens/pPos
+int dl_engine_slot_copy(void *h, uint32_t src, uint32_t dst, uint32_t P, cudaStream_t stream);
+int dl_engine_slot_sampling(void *h, uint32_t slot, unsigned long long seed, float temperature, float topp, float presence, float frequency,
+                            const int32_t *ids, const float *vals, int nBias, cudaStream_t stream);
+int dl_engine_slots_forward(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, cudaStream_t stream);
+int dl_engine_slots_step(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, cudaStream_t stream);
 int dl_engine_set_trace(void *h, uint64_t *buf, uint32_t capLaunches);
 int dl_engine_set_trace_all(void *h, int allCtas);
 uint32_t dl_engine_num_sms(void *h);

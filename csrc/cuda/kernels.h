@@ -84,6 +84,9 @@ struct RopeKvArgs {
     // Choice steps (several sequences at one rotary position): token t stores its K/V row at pos[t] + t * rowStride, and tokens
     // whose bit is set in inactiveMask store nothing. Both 0 for a plain batch of consecutive tokens.
     uint32_t rowStride, inactiveMask;
+    // Slots steps (slots.cu): token t stores its K/V row pos[t] at element offset t * slotStride (slot t, seqLen = the slot's
+    // length L). 0 for every other caller.
+    uint64_t slotStride;
 };
 int launchRopeKv(const RopeKvArgs &a, int nb, cudaStream_t stream, bool pdl);
 
@@ -104,6 +107,24 @@ struct ChoiceAttnArgs {
     uint32_t outStride;
 };
 int launchChoiceAttn(const ChoiceAttnArgs &a, cudaStream_t stream, bool pdl);
+
+// Attention of B independent sequences, row b in KV-cache slot b (slots.cu): slot b is the [nKvHeads][L][headDim] block at element
+// offset b * slotStride of the cache; query row b (position pos[b], already normalised and rotated by ropeKvKernel) attends to rows
+// [0, pos[b]] of its slot. A CTA owns (KV head, split, row) and serves the nHeads / nKvHeads q-heads of that KV head.
+struct SlotAttnArgs {
+    const float *qkv;
+    uint32_t qkvStride;
+    const int *pos;          // [B]
+    const __nv_bfloat16 *kCache, *vCache;
+    uint64_t slotStride;     // elements between slots: nKvHeads * L * headDim
+    uint32_t nHeads, nKvHeads, headDim, L, nSplits;
+    uint32_t B, inactiveMask;   // rows whose bit is set do nothing; their output is not meaningful
+    float *partial;          // >= B * nHeads * nSplits * (headDim + 2) floats
+    unsigned int *counters;  // [B][nKvHeads], zero-initialised, self-resetting
+    float *out;              // [B][outStride], head h at columns h * headDim
+    uint32_t outStride;
+};
+int launchSlotAttn(const SlotAttnArgs &a, cudaStream_t stream, bool pdl);
 
 struct AttnArgs {
     const float *qkv;
@@ -187,6 +208,7 @@ struct SampleControls {
     uint32_t *counts;         // [rows][countsStride] or null
     uint32_t countsStride;
     float presence, frequency;
+    uint32_t biasStride;      // row b's bias at bias + b * biasStride (0: one bias for every row)
 };
 int launchSample(const float *logits, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng, int *tokenOut, int *pos,
                  int *history, uint32_t historyCap, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
@@ -195,9 +217,11 @@ int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t 
                        unsigned int *flagMc, unsigned int *const *flagUcDev, unsigned int *blockCounter, cudaStream_t stream, uint32_t rows = 1);
 // B draws, one CTA per row: row b reads logits + b * logitsStride (0: every row draws from the same logits), uses rng[b] and writes
 // tokenOut[b]. Rows whose bit is set in inactiveMask draw nothing and keep their generator state. No position advance.
+// rowParams (device [B][4], may be null): row b's {temperature, top-p, presence, frequency} in place of the scalar arguments and the
+// controls' penalties; a row with temperature 0 draws the arg-max (lowest index among ties).
 int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
                      int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                     cudaStream_t stream, const SampleControls *controls = nullptr);
+                     cudaStream_t stream, const SampleControls *controls = nullptr, const float *rowParams = nullptr);
 
 // Persistent decode kernel (mega_decode.cu)
 struct MegaLayer {

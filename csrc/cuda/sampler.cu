@@ -40,6 +40,7 @@ struct SampleArgs {
     // batched draws (grid B, one CTA per row): row b reads logits + b * logitsStride, probs + b * probsStride, rng[b], tokenOut[b]
     uint32_t logitsStride, probsStride, inactiveMask;
     SampleControls ctl;        // bias / penalties (kernels.h); row b counts at ctl.counts + b * ctl.countsStride
+    const float *rowParams;    // [B][4] per-row {temperature, top-p, presence, frequency}, or null (launchSampleRows)
 };
 
 // The controls' transform of one logit (kernels.h); explicit roundings because the library is built with --use_fast_math.
@@ -241,6 +242,11 @@ __global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
     a.rng += row;
     a.tokenOut += row;
     if (a.ctl.counts) a.ctl.counts += (size_t)row * a.ctl.countsStride;
+    if (a.ctl.bias) a.ctl.bias += (size_t)row * a.ctl.biasStride;
+    if (a.rowParams) {
+        const float *rp = a.rowParams + 4 * (size_t)row;
+        a.temperature = rp[0]; a.topp = rp[1]; a.ctl.presence = rp[2]; a.ctl.frequency = rp[3];
+    }
     if (a.gatherFlag && a.nRanks > 1) {
         if (threadIdx.x == 0) {
             const unsigned int want = (*a.gatherEpoch + 1u) * a.nRanks;
@@ -254,7 +260,7 @@ __global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
     // With controls the max pass stores the transformed logits in probs, and the later passes read them from there: counts and
     // bias are read once per logit.
     const bool ctl = a.ctl.bias || a.ctl.counts;
-    const bool greedy = a.temperature == 0.f;   // reached with controls only (the launchers refuse it otherwise)
+    const bool greedy = a.temperature == 0.f;   // reached with controls or per-row parameters only (the launchers refuse it otherwise)
     const float *src = ctl ? a.probs : a.logits;
     // softmax statistics (IEEE division / shared exp / integer normaliser: the host sampler computes the very same numbers)
     float m = -INFINITY;
@@ -343,12 +349,12 @@ int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t 
 
 int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
                      int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                     cudaStream_t stream, const SampleControls *controls) {
-    if (n < 2 || !(temperature > 0.f || (temperature == 0.f && controls)) || B < 1 || B > 32) return -1;
+                     cudaStream_t stream, const SampleControls *controls, const float *rowParams) {
+    if (n < 2 || !(temperature > 0.f || (temperature == 0.f && (controls || rowParams))) || B < 1 || B > 32) return -1;
     SampleArgs a{};
     a.logits = logits; a.probs = probs; a.n = n; a.temperature = temperature; a.topp = topp; a.rng = rng; a.tokenOut = tokenOut;
     a.gatherFlag = gatherFlag; a.gatherEpoch = gatherEpoch; a.nRanks = nRanks;
-    a.logitsStride = logitsStride; a.probsStride = n; a.inactiveMask = inactiveMask;
+    a.logitsStride = logitsStride; a.probsStride = n; a.inactiveMask = inactiveMask; a.rowParams = rowParams;
     if (controls) a.ctl = *controls;
     sampleKernel<<<B, kSampThreads, 0, stream>>>(a);
     DL_CUDA_CHECK(cudaGetLastError());
@@ -383,4 +389,14 @@ DL_EXPORT int dl_sample_rows_controlled(const float *logits, uint32_t logitsStri
     const dl::SampleControls ctl{bias, counts, countsStride, presence, frequency};
     return dl::launchSampleRows(logits, logitsStride, probsScratch, n, temperature, topp, rngState, tokenOut, B, inactiveMask, nullptr, nullptr, 1,
                                 stream, &ctl);
+}
+
+// dl_sample_rows_controlled with per-row settings: rowParams (device f32 [B][4]) holds row b's {temperature, top-p, presence,
+// frequency}; row b's bias (may be null) is bias + b * biasStride. A row with temperature 0 draws the arg-max.
+DL_EXPORT int dl_sample_rows_per_row(const float *logits, uint32_t logitsStride, float *probsScratch, uint32_t n, const float *rowParams,
+                                     unsigned long long *rngState, int *tokenOut, uint32_t B, uint32_t inactiveMask, const float *bias,
+                                     uint32_t biasStride, uint32_t *counts, uint32_t countsStride, cudaStream_t stream) {
+    dl::SampleControls ctl{bias, counts, countsStride, 0.f, 0.f, biasStride};
+    return dl::launchSampleRows(logits, logitsStride, probsScratch, n, 0.f, 0.f, rngState, tokenOut, B, inactiveMask, nullptr, nullptr, 1, stream,
+                                (bias || counts) ? &ctl : nullptr, rowParams);
 }

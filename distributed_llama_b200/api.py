@@ -10,6 +10,8 @@ src/app.cpp:232-304).
 from __future__ import annotations
 
 import os
+import queue
+import threading
 import time
 from dataclasses import dataclass
 from typing import Callable, List, Optional, Sequence
@@ -110,20 +112,207 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     return out
 
 
+class ParallelRefused(ValueError):
+    """A --parallel value this configuration cannot serve (see parallel_refusal)."""
+
+
+def parallel_refusal(parallel: int, n_ranks: int = 1, n_experts: int = 0) -> Optional[str]:
+    """Why `parallel` concurrent sequences (KV-cache slots) cannot run in this configuration, or None if they can."""
+    if not 1 <= parallel <= MAX_CHOICES:
+        return f"--parallel must be from 1 to {MAX_CHOICES}"
+    if parallel == 1:
+        return None
+    if n_ranks > 1:
+        return "--parallel > 1 runs on one GPU only (workers cannot mirror slot steps yet)"
+    if n_experts > 0:
+        return "--parallel > 1 does not support mixture-of-experts models (the batched step has no MoE path)"
+    if os.environ.get("DL_COLLECTIVES") == "nccl":
+        return "--parallel > 1 does not support DL_COLLECTIVES=nccl"
+    if os.environ.get("DL_HOST_SAMPLER") is not None:
+        return "--parallel > 1 samples on the device: unset DL_HOST_SAMPLER"
+    return None
+
+
+class SlotRequest:
+    """One request of a SlotScheduler. The server fills in the fields and overrides the hooks; the scheduler calls them on its
+    engine thread.
+
+    n: completions; temperature / topp / presence / frequency / bias: the sampling settings; seed: the request's seed or None;
+    max_tokens (<= 0: no limit but the slot's context)."""
+    n = 1
+    temperature, topp, presence, frequency = 0.0, 0.9, 0.0, 0.0
+    bias: Sequence = ()
+    seed: Optional[int] = None
+    max_tokens = -1
+
+    def cached_prefix(self, slot: int) -> int:
+        """How many of the request's messages slot `slot`'s prompt cache covers (slot choice; ties go to the lowest index)."""
+        return 0
+
+    def prepare(self, slot: int):
+        """Resolves the prompt against slot `slot`'s cache: (tokens to prefill, their start position, last prompt token, P)
+        with P = the last prompt token's position."""
+        raise NotImplementedError
+
+    def on_token(self, i: int, token: int) -> bool:
+        """Token of completion i; True when completion i is finished (end of sequence or stop string)."""
+        raise NotImplementedError
+
+    def finish(self, out: List[List[int]], slots: List[int], P: int) -> None:
+        """Every completion is done: out[i] holds completion i's tokens."""
+
+    def fail(self, error: Exception, slots: List[int]) -> None:
+        """The request ended early: refused (slots == []), or a client write, the prefill or the step failed. Its slots are
+        already free; what they hold may no longer match what their prompt caches say."""
+
+
+class SlotScheduler:
+    """Serves SlotRequests on the KV-cache slots of a backend: one engine thread owns the GPU and decodes every busy slot in one
+    batched step per token.
+
+    Between steps it admits waiting requests first-in, first-out into free slots: a request takes n slots (one when greedy:
+    every greedy completion is the same), the free slot whose prompt cache covers most of its messages first. It prefills the
+    request's delta prompt into that slot (the running rows wait for this prefill), copies the prompt rows into its other slots
+    and seeds each slot: completion i with choice_seed(seed, i) when n > 1, the seed itself when n = 1; a request without a seed
+    takes seed_source() in admission order. The prompt's last token then enters the next batched step. A completion stops at
+    end of sequence or after min(max_tokens, slot_len - P) tokens. If on_token raises (a client went away), the request ends
+    and frees its slots; the other requests continue.
+
+    `backend` provides slots, slot_len, slot_prefill(slot, tokens, pos), slot_copy(src, dst, P),
+    slot_sampling(slot, seed, temperature, topp, presence, frequency, bias) and slots_step(tokens, pos, active)
+    (InferenceSession(parallel=N))."""
+
+    def __init__(self, backend, seed_source: Callable[[], int]):
+        self.backend = backend
+        self.seed_source = seed_source
+        self.queue: "queue.Queue" = queue.Queue()
+        self.owner: List[Optional[object]] = [None] * backend.slots
+        self._stop = threading.Event()
+
+    def submit(self, req: SlotRequest) -> None:
+        """Queues the request; one that needs more slots than there are is refused at once (fail with no slots)."""
+        if req.temperature != 0.0 and req.n > self.backend.slots:
+            req.fail(ValueError(f"n = {req.n} needs more than the {self.backend.slots} slots"), [])
+            return
+        self.queue.put(req)
+
+    def stop(self) -> None:
+        self._stop.set()
+        self.queue.put(None)
+
+    def _admit(self, req: SlotRequest, free: List[int], rows: List[dict]) -> None:
+        be = self.backend
+        rows_needed = 1 if req.temperature == 0.0 else req.n
+        first = max(free, key=lambda s: (req.cached_prefix(s), -s))
+        slots = [first] + [s for s in free if s != first][:rows_needed - 1]
+        try:
+            self._start(req, slots, rows, rows_needed)
+        except Exception as e:   # e.g. the client went away while its prompt was prepared
+            req.fail(e, slots)
+
+    def _start(self, req: SlotRequest, slots: List[int], rows: List[dict], rows_needed: int) -> None:
+        be, first = self.backend, slots[0]
+        prefill, start, token, P = req.prepare(first)
+        if prefill:
+            be.slot_prefill(first, prefill, start)
+        for s in slots[1:]:
+            be.slot_copy(first, s, P)
+        seed = req.seed if req.seed is not None else (self.seed_source() if req.temperature != 0.0 else 0)
+        seeds = [seed] if req.n == 1 else [host().choice_seed(seed, i) for i in range(len(slots))]
+        for s, sd in zip(slots, seeds):
+            be.slot_sampling(s, sd, req.temperature, req.topp, req.presence, req.frequency, req.bias)
+        limit = be.slot_len - P
+        if req.max_tokens > 0:
+            limit = min(limit, req.max_tokens)
+        job = {"req": req, "slots": slots, "P": P, "out": [[] for _ in range(req.n)], "limit": limit, "live": len(slots)}
+        if limit <= 0:
+            req.finish(job["out"], slots, P)
+            return
+        for k, s in enumerate(slots):
+            self.owner[s] = job
+            # completion k of the request; a greedy request's only row serves all n completions
+            rows[s] = {"job": job, "k": k, "token": token, "pos": P,
+                       "choices": list(range(req.n)) if rows_needed == 1 else [k], "done": set()}
+
+    def _release(self, job, rows) -> None:
+        for s in job["slots"]:
+            if self.owner[s] is job:
+                self.owner[s] = None
+                rows[s] = None
+
+    def run(self) -> None:
+        """The engine loop; returns after stop()."""
+        be = self.backend
+        N = be.slots
+        rows: List[Optional[dict]] = [None] * N
+        waiting: List[SlotRequest] = []
+        while not self._stop.is_set():
+            busy = any(r is not None for r in rows)
+            try:
+                while True:
+                    item = self.queue.get(block=not busy and not waiting, timeout=None)
+                    if item is None:
+                        return
+                    waiting.append(item)
+            except queue.Empty:
+                pass
+            while waiting:
+                free = [s for s in range(N) if self.owner[s] is None]
+                need = 1 if waiting[0].temperature == 0.0 else waiting[0].n
+                if len(free) < need:
+                    break
+                self._admit(waiting.pop(0), free, rows)
+            active = [r is not None for r in rows]
+            if not any(active):
+                continue
+            drawn = be.slots_step([r["token"] if r else 0 for r in rows], [r["pos"] if r else 0 for r in rows], active)
+            for s in range(N):
+                r = rows[s]
+                if r is None:
+                    continue
+                job, req = r["job"], r["job"]["req"]
+                tok = drawn[s]
+                r["token"], r["pos"] = tok, r["pos"] + 1
+                try:
+                    for i in r["choices"]:
+                        if i in r["done"]:
+                            continue
+                        job["out"][i].append(tok)
+                        if req.on_token(i, tok) or len(job["out"][i]) >= job["limit"]:
+                            r["done"].add(i)
+                except Exception as e:
+                    self._release(job, rows)
+                    req.fail(e, job["slots"])
+                    continue
+                if len(r["done"]) == len(r["choices"]):
+                    rows[s] = None
+                    job["live"] -= 1
+                    if job["live"] == 0:
+                        self._release(job, rows)
+                        try:
+                            req.finish(job["out"], job["slots"], job["P"])
+                        except Exception as e:
+                            req.fail(e, job["slots"])
+
+
 class InferenceSession:
     def __init__(self, model_path: str, tokenizer_path: Optional[str] = None, max_seq_len: int = 0,
                  temperature: float = 0.0, topp: float = 0.9, seed: int = 12345, device: Optional[str] = None,
                  max_batch: int = 8, use_pdl: bool = True, comm=None, moe_mode: str = "auto", presence_penalty: float = 0.0,
-                 frequency_penalty: float = 0.0, logit_bias: Optional[dict] = None):
+                 frequency_penalty: float = 0.0, logit_bias: Optional[dict] = None, parallel: int = 1):
         """presence_penalty, frequency_penalty and logit_bias ({token id: value}) are the sampling controls of every
         completion (host Sampler.set_controls; they may be changed later through self.sampler.set_controls, which restarts the
-        counts of the current completion)."""
+        counts of the current completion). parallel > 1 splits the KV cache into that many slots for SlotScheduler
+        (slot_prefill, slot_copy, slot_sampling, slots_step); the single-sequence calls then must not be used."""
         from .models.loader import load_device_weights
         from .runtime.engine import Engine
 
         self.model_file = ModelFile(model_path, max_seq_len)
         self.header = self.model_file.header
         self.comm = comm
+        why = parallel_refusal(parallel, comm.world_size if comm is not None else 1, self.header.n_experts)
+        if why:
+            raise ParallelRefused(why)
         rank = comm.rank if comm is not None else 0
         n_ranks = comm.world_size if comm is not None else 1
         if device is None:
@@ -143,6 +332,23 @@ class InferenceSession:
         self._dev_controls = None   # completion generation whose controls the device holds (None: off)
         self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory()
         self._pin_out = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self.slots = parallel
+        if parallel > 1:
+            self.engine.set_slots(parallel)
+        self.slot_len = self.engine.slot_len
+
+    # ---- KV-cache slots (SlotScheduler) ----
+    def slot_prefill(self, slot: int, tokens: Sequence[int], pos: int) -> None:
+        self.engine.slot_prefill(slot, tokens, pos)
+
+    def slot_copy(self, src: int, dst: int, P: int) -> None:
+        self.engine.slot_copy(src, dst, P)
+
+    def slot_sampling(self, slot: int, seed: int, temperature: float, topp: float, presence: float, frequency: float, bias) -> None:
+        self.engine.slot_sampling(slot, seed, temperature, topp, presence, frequency, bias)
+
+    def slots_step(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]) -> List[int]:
+        return self.engine.slots_step(tokens, pos, active)
 
     # ---- token level ----
     def reset(self):

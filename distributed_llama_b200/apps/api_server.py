@@ -12,11 +12,12 @@ import json
 import re
 import socket
 import sys
+import threading
 import time
 from typing import Dict, List, Optional, Tuple
 
 from .. import host
-from ..api import MAX_CHOICES, run_choices
+from ..api import MAX_CHOICES, ParallelRefused, SlotRequest, SlotScheduler, parallel_refusal, run_choices
 from .args import AppArgs, parse_args
 from .cli import make_chat_tools
 from .runtime import AppContext, run_inference_app
@@ -250,9 +251,159 @@ class ApiServer:
                             for i, b in enumerate(buffers)]}))
         print("🔶" if n == 1 else f"({n} choices)🔶")
 
+    def slot_request(self, req: HttpRequest, caches: List[NaiveCache], n_slots: int) -> SlotRequest:
+        """A validated chat completion for SlotScheduler (--parallel > 1): the same fields, limits and responses as complete(),
+        with the prompt cache of the slot the scheduler picks. Raises ValueError / KeyError on a malformed body."""
+        ctx, H = self.ctx, self.H
+        tok, smp = ctx.tokenizer, ctx.sampler
+        body = req.json or {}
+        n = parse_n(body)
+        if n > n_slots:
+            raise ValueError(f"'n' must not exceed --parallel ({n_slots})")
+        presence, frequency, bias = parse_controls(body, smp.vocab_size, getattr(ctx.args, "presence_penalty", 0.0),
+                                                   getattr(ctx.args, "frequency_penalty", 0.0))
+        messages = [(m["role"], m["content"]) for m in body["messages"]]
+        stream = bool(body.get("stream", False))
+        temperature = float(body.get("temperature", ctx.args.temperature))
+        if temperature < 0:
+            raise ValueError("'temperature' must not be negative")
+        detector_args, gen = self.detector_args, self.gen
+
+        class Chat(SlotRequest):
+            def cached_prefix(self, slot):
+                items = caches[slot].items
+                ok = len(messages) > len(items) and all(items[i][1] == messages[i] for i in range(len(items)))
+                return len(items) if ok else 0
+
+            def prepare(self, slot):
+                cache = caches[slot]
+                delta, start = cache.resolve_delta_prompt(list(messages))
+                content, public = gen.generate(delta, True)
+                tokens = tok.encode(content, start == 0, True)
+                self.n_prompt = len(tokens)
+                P = min(start + len(tokens) - 1, slot_len)
+                p = public.decode("utf-8", errors="replace")
+                self.buffers = [p] * n
+                if stream:
+                    req.write_stream_start()
+                    if p:
+                        for i in range(n):
+                            req.write_stream_chunk("data: " + chunk_json(p, False, i) + "\r\n\r\n")
+                for m in delta:
+                    cache.push(P, m)
+                self.slot_cache = cache
+                n_pref = P - start
+                return tokens[:n_pref], start, (tokens[n_pref] if n_pref < len(tokens) else tokens[-1]), P
+
+            def on_token(self, i, t):
+                piece = self.decoders[i].decode(tok, t)
+                kind = self.dets[i].append(t, piece)
+                if kind in (H.NOT_EOS, H.EOS):
+                    delta = self.dets[i].get_delta()
+                    if delta:
+                        d = delta.decode("utf-8", errors="replace")
+                        if stream:
+                            req.write_stream_chunk("data: " + chunk_json(d, False, i) + "\r\n\r\n")
+                        self.buffers[i] += d
+                    self.dets[i].reset()
+                return kind == H.EOS
+
+            def finish(self, out, slots, P):
+                if n == 1:
+                    end = P + len(out[0])
+                    if end == slot_len:
+                        self.slot_cache.clear()
+                    else:
+                        self.slot_cache.push(end, ("assistant", self.buffers[0]))
+                for s in slots[1:]:   # they hold a copy of the prompt rows
+                    caches[s].items = list(caches[slots[0]].items)
+                if stream:
+                    for i in range(n):
+                        req.write_stream_chunk("data: " + chunk_json(None, True, i) + "\r\n\r\n")
+                    req.write_stream_chunk("data: [DONE]")
+                    req.write_stream_end()
+                else:
+                    n_completion = sum(len(o) for o in out)
+                    req.write_json(json.dumps({
+                        "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
+                        "usage": {"completion_tokens": n_completion, "prompt_tokens": self.n_prompt,
+                                  "total_tokens": self.n_prompt + n_completion},
+                        "choices": [{"index": i, "message": {"role": "assistant", "content": b}, "finish_reason": "stop"}
+                                    for i, b in enumerate(self.buffers)]}))
+                print(f"🔶 slot {slots[0]}" + (f" ({n} choices)" if n > 1 else ""), flush=True)
+                self.done()
+
+            def fail(self, error, slots):
+                for s in slots:   # their rows may not match what their caches say (e.g. a prefill that never ran)
+                    caches[s].clear()
+                print(f"Socket error: {error}", flush=True)
+                self.done()
+
+        slot_len = self.slot_len
+        r = Chat()
+        r.n, r.temperature, r.topp = n, temperature, float(body.get("top_p", ctx.args.topp))
+        r.presence, r.frequency, r.bias = presence, frequency, bias
+        r.seed = int(body["seed"]) if "seed" in body else None
+        r.max_tokens = int(body.get("max_tokens", -1))
+        r.dets = [H.EosDetector(*detector_args) for _ in range(n)]
+        r.decoders = [H.TokenDecoder() for _ in range(n)]
+        r.done = lambda: None
+        return r
+
     def models(self, req: HttpRequest):
         name = self.ctx.args.model.replace("\\", "/").split("/")[-1]
         req.write_json(json.dumps({"object": "list", "data": [{"id": name, "object": "model", "created": 0, "owned_by": "user"}]}))
+
+
+def serve_parallel(ctx: AppContext, srv: socket.socket, api: ApiServer, n_slots: int, max_requests: int = 0) -> None:
+    """--parallel > 1: every connection is read and validated on its own thread; chat completions go to a SlotScheduler whose
+    engine thread (this one) decodes up to n_slots requests together. A malformed body closes its connection without a response."""
+    backend = ctx.sess if ctx.sess is not None else ctx.inference
+    api.slot_len = backend.slot_len
+    caches = [NaiveCache() for _ in range(n_slots)]
+    sched = SlotScheduler(backend, ctx.sampler.next_seed)
+    pending = threading.Semaphore(0)   # one release per finished connection
+
+    def handle(conn):
+        keep = False
+        try:
+            req = HttpRequest.read(conn)
+            print(f"🔷 {req.method} {req.path}", flush=True)
+            if req.method == "OPTIONS":
+                req.write_cors()
+            elif req.method == "POST" and req.path == "/v1/chat/completions":
+                r = api.slot_request(req, caches, n_slots)
+
+                def done():
+                    conn.close()
+                    pending.release()
+                r.done = done
+                keep = True
+                sched.submit(r)
+            elif req.method == "GET" and req.path == "/v1/models":
+                api.models(req)
+            else:
+                req.write_not_found()
+        except (ConnectionError, BrokenPipeError, ValueError, KeyError, TypeError, json.JSONDecodeError) as e:
+            print(f"Socket error: {e}", flush=True)
+        finally:
+            if not keep:
+                conn.close()
+                pending.release()
+
+    def accept():
+        served = 0
+        while max_requests == 0 or served < max_requests:
+            conn, _ = srv.accept()
+            threading.Thread(target=handle, args=(conn,), daemon=True).start()
+            served += 1
+        for _ in range(served):
+            pending.acquire()
+        sched.stop()
+
+    threading.Thread(target=accept, daemon=True).start()
+    sched.run()
+    srv.close()
 
 
 def serve(ctx: AppContext, max_requests: int = 0) -> None:
@@ -264,6 +415,10 @@ def serve(ctx: AppContext, max_requests: int = 0) -> None:
     api = ApiServer(ctx)
     if a.host in ("0.0.0.0", "127.0.0.1"):
         print(f"Server URL: http://localhost:{a.port}/v1/", flush=True)
+    n_slots = getattr(a, "parallel", 1)
+    if n_slots > 1:
+        serve_parallel(ctx, srv, api, n_slots, max_requests)
+        return
     served = 0
     while max_requests == 0 or served < max_requests:
         conn, _ = srv.accept()
@@ -289,7 +444,9 @@ def serve(ctx: AppContext, max_requests: int = 0) -> None:
 USAGE = """Usage: dllama-api {--model <path>} {--tokenizer <path>} [--host <addr>] [--port <p>]
         [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>] [--gpus <n>] [--workers <ip:port> ...]
         [--temperature <temp>] [--topp <t>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]
-        [--chat-template {llama2|llama3|deepSeek3|chatml}]
+        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--parallel <n>]
+        --parallel <n>: decode up to n (1..8) chat requests together, each in its own KV-cache slot of
+                        floor(context / n) tokens; single GPU and dense models only
 """
 
 
@@ -300,6 +457,10 @@ def main(argv=None) -> int:
     if args.help:
         sys.stderr.write(USAGE)
         return 0
+    why = parallel_refusal(args.parallel, max(args.gpus, 1, int(os.environ.get("WORLD_SIZE", "1"))) + len(args.workers))
+    if why:
+        sys.stderr.write(why + "\n")
+        return 1
     if args.gpus > 1 and os.environ.get("DLLAMA_SPAWNED") != "1" and int(os.environ.get("WORLD_SIZE", "1")) == 1:
         # Supervisor of a tensor-parallel serving job: a rank that loses a peer (control-channel heartbeat, device-side wait timeout)
         # exits non-zero and torchrun tears the job down; the whole job is then started again after 3 s — the reference's root retry
@@ -324,6 +485,9 @@ def main(argv=None) -> int:
         try:
             run_inference_app(args, serve)
             return 0
+        except ParallelRefused as e:   # found once the model header is read (mixture of experts)
+            sys.stderr.write(f"{e}\n")
+            return 1
         except (ConnectionError, RuntimeError) as e:
             print(f"🚨 Inference error: {e}")
             if int(os.environ.get("WORLD_SIZE", "1")) > 1:

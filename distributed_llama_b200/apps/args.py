@@ -40,6 +40,7 @@ class AppArgs:
     # GPU build extras
     gpus: int = 0            # spawn this many local ranks (0 = use the current torch.distributed world / single GPU)
     moe_mode: str = "auto"   # tp | ep | auto
+    parallel: int = 1        # dllama-api: chat requests decoded together, one KV-cache slot each (1..8)
 
 
 FLOAT_TYPES = ("f32", "f16", "q40", "q80")
@@ -118,6 +119,8 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
             a.gpus = int(value)
         elif name == "--moe-mode":
             a.moe_mode = value
+        elif name == "--parallel" and not require_mode:   # dllama-api only; its range is checked by api.parallel_refusal
+            a.parallel = int(value)
         else:
             raise ValueError(f"Unknown option: {name}")
         i += 2

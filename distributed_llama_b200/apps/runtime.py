@@ -318,7 +318,8 @@ def run_inference_app(args: AppArgs, handler: Callable[[AppContext], None]) -> N
         raise RuntimeError("This version supports only Q40 weights with Q80 sync type")
     sess = InferenceSession(args.model, args.tokenizer, max_seq_len=args.max_seq_len, temperature=args.temperature,
                             topp=args.topp, seed=args.seed, comm=comm, moe_mode=getattr(args, "moe_mode", "auto") or "auto",
-                            presence_penalty=args.presence_penalty, frequency_penalty=args.frequency_penalty)
+                            presence_penalty=args.presence_penalty, frequency_penalty=args.frequency_penalty,
+                            parallel=getattr(args, "parallel", 1))
     chan = open_control_channel(comm)
     if rank != 0:
         worker_loop(sess, comm, chan)

@@ -136,6 +136,25 @@ def lib() -> C.CDLL:
     L.dl_engine_sample_rows.restype = i32
     L.dl_engine_choices_forward.argtypes = [vp, i32, u32, u32, u32, u32, vp]
     L.dl_engine_choices_forward.restype = i32
+    L.dl_sample_rows_per_row.argtypes = [vp, u32, vp, u32, vp, vp, vp, u32, u32, vp, u32, vp, u32, vp]
+    L.dl_sample_rows_per_row.restype = i32
+    L.dl_slot_attn.argtypes = [vp, u32, vp, vp, vp, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
+    L.dl_slot_attn.restype = i32
+    ip = C.POINTER(C.c_int32)
+    L.dl_engine_set_slots.argtypes = [vp, u32]
+    L.dl_engine_set_slots.restype = i32
+    L.dl_engine_slot_len.argtypes = [vp]
+    L.dl_engine_slot_len.restype = u32
+    L.dl_engine_slot_prefill.argtypes = [vp, u32, u32, u32, vp]
+    L.dl_engine_slot_prefill.restype = i32
+    L.dl_engine_slot_copy.argtypes = [vp, u32, u32, u32, vp]
+    L.dl_engine_slot_copy.restype = i32
+    L.dl_engine_slot_sampling.argtypes = [vp, u32, C.c_uint64, f32, f32, f32, f32, ip, C.POINTER(f32), i32, vp]
+    L.dl_engine_slot_sampling.restype = i32
+    L.dl_engine_slots_forward.argtypes = [vp, ip, ip, u32, vp]
+    L.dl_engine_slots_forward.restype = i32
+    L.dl_engine_slots_step.argtypes = [vp, ip, ip, u32, ip, vp]
+    L.dl_engine_slots_step.restype = i32
     L.dl_engine_sync_ns.argtypes = [vp]
     L.dl_engine_sync_ns.restype = C.c_uint64
     L.dl_engine_mega_active.argtypes = [vp]

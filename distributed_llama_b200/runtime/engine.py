@@ -133,6 +133,7 @@ class Engine:
             self.enable_mega(True)     # persistent decode kernel by default; the engine falls back per call if a shape is unsupported
         self.tc_min_tokens = 9          # shorter chunks stay on the GEMV path
         self._graph_ready = False
+        self.slots, self.slot_len = 1, self.seq_len
         self._stage_tok = torch.zeros(max_batch, dtype=torch.int32).pin_memory()
         self._stage_pos = torch.zeros(max_batch, dtype=torch.int32).pin_memory()
 
@@ -239,6 +240,62 @@ class Engine:
         out = self.tokens[:len(tokens)].tolist()
         self.check_abort()
         return out
+
+    # -- KV-cache slots: up to 8 independent sequences decoded together (csrc/cuda/slots.cu) --
+    def set_slots(self, n: int) -> None:
+        """Splits every layer's KV cache into n slots of floor(seq_len / n) rows. Single GPU, dense q40 layers only; n = 1 is
+        the ordinary single-sequence engine."""
+        cl.check(self._lib.dl_engine_set_slots(self._h, int(n)), "engine_set_slots")
+        self.slots = int(n)
+        self.slot_len = int(self._lib.dl_engine_slot_len(self._h))
+
+    def slot_prefill(self, slot: int, tokens: Sequence[int], start_pos: int) -> None:
+        """Feeds tokens at positions start_pos.. into slot `slot` (tensor-core prefill kernels with the slot's cache). No logits."""
+        tokens = list(tokens)
+        if start_pos + len(tokens) > self.slot_len:
+            raise ValueError("position beyond the slot length")
+        i = 0
+        while i < len(tokens):
+            n = min(len(tokens) - i, self.max_prefill)
+            self.p_tokens[:n].copy_(torch.tensor(tokens[i:i + n], dtype=torch.int32))
+            self.p_pos[:n].copy_(torch.arange(start_pos + i, start_pos + i + n, dtype=torch.int32))
+            cl.check(self._lib.dl_engine_slot_prefill(self._h, int(slot), n, start_pos + i, cl.stream_ptr()), "engine_slot_prefill")
+            i += n
+
+    def slot_copy(self, src: int, dst: int, P: int) -> None:
+        """Copies rows [0, P) of slot src into slot dst (every layer and KV head)."""
+        cl.check(self._lib.dl_engine_slot_copy(self._h, int(src), int(dst), int(P), cl.stream_ptr()), "engine_slot_copy")
+
+    def slot_sampling(self, slot: int, seed: int, temperature: float, topp: float, presence: float = 0.0, frequency: float = 0.0,
+                      bias: Sequence = ()) -> None:
+        """Seeds slot `slot`'s generator, zeroes its token counts and sets its temperature (0: arg-max), top-p, penalties and
+        logit bias ((id, value) pairs)."""
+        n = len(bias)
+        ids = (C.c_int32 * max(n, 1))(*[int(t) for t, _ in bias])
+        vals = (C.c_float * max(n, 1))(*[float(v) for _, v in bias])
+        cl.check(self._lib.dl_engine_slot_sampling(self._h, int(slot), int(seed) & 0xFFFFFFFFFFFFFFFF, float(temperature), float(topp),
+                                                    float(presence), float(frequency), ids, vals, n, cl.stream_ptr()),
+                 "engine_slot_sampling")
+
+    def _slot_args(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]):
+        n = self.slots
+        mask = sum(1 << b for b in range(n) if not active[b])
+        return (C.c_int32 * n)(*[int(t) for t in tokens]), (C.c_int32 * n)(*[int(p) for p in pos]), mask
+
+    def slots_forward(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]) -> torch.Tensor:
+        """Row b feeds tokens[b] at position pos[b] of slot b (active rows only). Returns the logits rows [slots][vocab]."""
+        t, p, mask = self._slot_args(tokens, pos, active)
+        cl.check(self._lib.dl_engine_slots_forward(self._h, t, p, mask, cl.stream_ptr()), "engine_slots_forward")
+        return self.logits[:self.slots]
+
+    def slots_step(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]) -> List[int]:
+        """slots_forward, then every active row draws its next token with its slot's settings. Returns the draws (inactive
+        rows: -1)."""
+        t, p, mask = self._slot_args(tokens, pos, active)
+        out = (C.c_int32 * self.slots)(*([-1] * self.slots))
+        cl.check(self._lib.dl_engine_slots_step(self._h, t, p, mask, out, cl.stream_ptr()), "engine_slots_step")
+        self.check_abort()
+        return list(out)
 
     def sampler_state(self) -> int:
         """State of the single-sequence device generator (0 before the first seeding); seed_sampler(state) continues its stream."""
