@@ -55,14 +55,14 @@ public:
     // rowMask (bit 0: stepSampled, bit 1 + i: choice i). All zero: off. With controls on, stepSampled and the choices steps accept
     // temperature 0 (arg-max of the controlled logits). Every rank must make the same call.
     void setSamplingControls(float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias, uint32_t rowMask);
-    // Several completions of one prompt (csrc/cuda/choices.cu), dense models, n <= 8: generators of the batched sampler (separate
+    // Several completions of one prompt (csrc/cuda/attn_decode.cu), dense models, n <= 8: generators of the batched sampler (separate
     // from the single-sequence one), first draws from the logits of `token` at P, one batched step (see InferenceBackend).
     bool supportsChoices(uint32_t n) const { return n >= 1 && n <= maxBatch_ && h_.nExperts == 0; }
     void seedChoiceSamplers(const std::vector<uint64_t> &seeds);
     std::vector<int32_t> choicesFirst(int32_t token, uint32_t P, uint32_t n, float temperature, float topp);
     std::vector<int32_t> choicesStep(const std::vector<int32_t> &tokens, uint32_t P, uint32_t C, uint32_t j, uint32_t activeMask, float temperature,
                                      float topp);
-    // KV-cache slots (csrc/cuda/slots.cu): n <= 8 independent sequences, each in its own floor(seqLen / n) rows of the cache, decoded
+    // KV-cache slots (csrc/cuda/attn_decode.cu): n <= 8 independent sequences, each in its own floor(seqLen / n) rows of the cache, decoded
     // together by slotsStep. Single GPU, dense q40 models. Row b of a step is slot b (activeMask bit b); inactive rows return -1.
     void setSlots(uint32_t n);
     uint32_t slotLen() const;

@@ -189,13 +189,24 @@ static int engineDecodeMega(Engine &e, bool greedyAdvance, cudaStream_t stream) 
     return launchMegaDecode(m, (int)(e.megaCtas ? e.megaCtas : c.numSms), stream);
 }
 
-// Geometry of a choices step (see choices.cu): nb rows at rotary position P + 1 + j, row b stored at P + 1 + b * C + j.
+// Geometry of a choices step (see attn_decode.cu): nb rows at rotary position P + 1 + j, row b stored at P + 1 + b * C + j.
 struct ChoiceStep { uint32_t P, C, j, inactiveMask; };
 
-// A slots step (see slots.cu): row b is KV-cache slot b at position pos[b].
+// A slots step (see attn_decode.cu): row b is KV-cache slot b at position pos[b].
 struct SlotStep { uint32_t inactiveMask; };
 
 static uint64_t slotElems(const Engine &e) { return (uint64_t)e.cfg.nKvHeads * e.slotLen * e.cfg.headDim; }
+
+// QK-norm + RoPE + K/V write of layer L over the q|k|v rows `qkv` at positions `pos`, into the cache that starts cacheOff elements
+// into the layer's K/V and holds seqLen rows per KV head. rowStride, slotStride and inactiveMask are left 0 for the caller to set.
+static RopeKvArgs layerRopeKv(const Engine &e, const LayerPtrs &L, float *qkv, const int *pos, uint64_t cacheOff, uint32_t seqLen) {
+    const EngineConfig &c = e.cfg;
+    RopeKvArgs r{};
+    r.qkv = qkv; r.qkvStride = (c.nHeads + 2 * c.nKvHeads) * c.headDim; r.pos = pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
+    r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = seqLen;
+    r.kCache = (__nv_bfloat16 *)L.kCache + cacheOff; r.vCache = (__nv_bfloat16 *)L.vCache + cacheOff;
+    return r;
+}
 
 // logitsMode: 0 = none (prefill chunk), 1 = logits of the last token in the batch into logits[0], 2 = all tokens.
 // ch: a choices step instead of a batch of consecutive tokens (logitsMode 2, dense layers only); sl: a slots step (same limits).
@@ -229,10 +240,8 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
         DL_TRY(gemvSel(e, PRO_RMSNORM_, EPI_STORE_, nb, a, c.numSms, stream, pdl));
         if (sl) {
             // 2+3. qk-norm + rope + K/V append at row pos[b] of slot b, then attention of each row over its own slot
-            RopeKvArgs r{};
-            r.qkv = e.g.qkv; r.qkvStride = qkvDim; r.pos = e.g.pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
-            r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = e.slotLen;
-            r.kCache = (__nv_bfloat16 *)L.kCache; r.vCache = (__nv_bfloat16 *)L.vCache; r.slotStride = slotElems(e); r.inactiveMask = sl->inactiveMask;
+            RopeKvArgs r = layerRopeKv(e, L, e.g.qkv, e.g.pos, 0, e.slotLen);
+            r.slotStride = slotElems(e); r.inactiveMask = sl->inactiveMask;
             DL_TRY(launchRopeKv(r, nb, stream, pdl));
             SlotAttnArgs t{};
             t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache; t.slotStride = r.slotStride;
@@ -242,10 +251,8 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
             DL_TRY(launchSlotAttn(t, stream, pdl));
         } else if (ch) {
             // 2+3. qk-norm + rope + K/V append at the choices' own rows, then attention over the shared prompt + own rows
-            RopeKvArgs r{};
-            r.qkv = e.g.qkv; r.qkvStride = qkvDim; r.pos = e.g.pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
-            r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = c.seqLen;
-            r.kCache = (__nv_bfloat16 *)L.kCache; r.vCache = (__nv_bfloat16 *)L.vCache; r.rowStride = ch->C; r.inactiveMask = ch->inactiveMask;
+            RopeKvArgs r = layerRopeKv(e, L, e.g.qkv, e.g.pos, 0, c.seqLen);
+            r.rowStride = ch->C; r.inactiveMask = ch->inactiveMask;
             DL_TRY(launchRopeKv(r, nb, stream, pdl));
             ChoiceAttnArgs t{};
             t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.kCache = r.kCache; t.vCache = r.vCache;
@@ -263,10 +270,7 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
             DL_TRY(launchAttnFused(f, stream, pdl));
         } else {
             // 2. qk-norm + rope + kv write
-            RopeKvArgs r{};
-            r.qkv = e.g.qkv; r.qkvStride = qkvDim; r.pos = e.g.pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
-            r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = c.seqLen;
-            r.kCache = (__nv_bfloat16 *)L.kCache; r.vCache = (__nv_bfloat16 *)L.vCache;
+            const RopeKvArgs r = layerRopeKv(e, L, e.g.qkv, e.g.pos, 0, c.seqLen);
             DL_TRY(launchRopeKv(r, nb, stream, pdl));
             // 3. attention
             AttnArgs t{};
@@ -365,10 +369,7 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
         const LayerPtrs &L = e.layers[l];
         DL_TRY(launchRmsNormBf16(g.px, c.dim, L.norm0, g.pxn, c.dim, c.dim, c.eps, T, stream, pdl));
         DL_TRY(gemmQ40Tc(GEPI_STORE_F32_, L.qkvQs, L.qkvSc, qkvDim, c.dim, g.pxn, c.dim, T, g.pqkv, qkvDim, c.numSms, stream, pdl));
-        RopeKvArgs r{};
-        r.qkv = g.pqkv; r.qkvStride = qkvDim; r.pos = g.pPos; r.rope = g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
-        r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = seqLen;
-        r.kCache = (__nv_bfloat16 *)L.kCache + cacheOff; r.vCache = (__nv_bfloat16 *)L.vCache + cacheOff;
+        const RopeKvArgs r = layerRopeKv(e, L, g.pqkv, g.pPos, cacheOff, seqLen);
         DL_TRY(launchRopeKv(r, (int)T, stream, pdl));
         int attnRc = 1;
         if (e.tcAttn) {
@@ -756,10 +757,7 @@ DL_EXPORT int dl_engine_forward_part(void *h, int nb, uint32_t layer, int part, 
         a.qs = (const uint32_t *)L.qkvQs; a.scales = (const __half *)L.qkvSc; a.d = qkvDim; a.n = c.dim;
         a.in = e.g.x; a.inStride = c.dim; a.normW = L.norm0; a.eps = c.eps; a.out = e.g.qkv; a.outStride = qkvDim;
         DL_TRY(dl::gemvSel(e, dl::PRO_RMSNORM_, dl::EPI_STORE_, nb, a, c.numSms, stream, false));
-        dl::RopeKvArgs r{};
-        r.qkv = e.g.qkv; r.qkvStride = qkvDim; r.pos = e.g.pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
-        r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = c.seqLen;
-        r.kCache = (__nv_bfloat16 *)L.kCache; r.vCache = (__nv_bfloat16 *)L.vCache;
+        const dl::RopeKvArgs r = dl::layerRopeKv(e, L, e.g.qkv, e.g.pos, 0, c.seqLen);
         DL_TRY(dl::launchRopeKv(r, nb, stream, false));
         dl::AttnArgs t{};
         t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache;
@@ -840,7 +838,7 @@ DL_EXPORT int dl_engine_decode_graph(void *h, int nSteps, cudaStream_t stream) {
     return 0;
 }
 
-// ---- KV-cache slots: up to 8 independent sequences decoded together (slots.cu) ----------------------------------------------------
+// ---- KV-cache slots: up to 8 independent sequences decoded together (attn_decode.cu) -------------------------------------------------
 
 // Splits every layer's K/V cache into n equal slots of floor(seqLen / n) rows (no extra memory) and allocates the per-slot sampling
 // state. Single GPU, dense (non-MoE) q40 layers only. n = 1 leaves the engine exactly as it was.

@@ -94,12 +94,12 @@ int dl_engine_sample(void *h, float temperature, float topp, cudaStream_t stream
 // bit 1 + b: choice b). All zero: off.
 int dl_engine_set_sampling_controls(void *h, float presence, float frequency, const int32_t *ids, const float *vals, int nBias, uint32_t rowMask,
                                     cudaStream_t stream);
-// choices (several completions of one prompt, csrc/cuda/choices.cu): generators 0..n-1, batched draws, one choices forward
+// choices (several completions of one prompt, csrc/cuda/attn_decode.cu): generators 0..n-1, batched draws, one choices forward
 int dl_engine_sampler_seed_rows(void *h, const unsigned long long *seeds, int n);   // separate from the single-sequence generator
 unsigned long long dl_engine_sampler_state(void *h);   // single-sequence generator state (seed with it to continue the stream)
 int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, float temperature, float topp, int firstStep, cudaStream_t stream);
 int dl_engine_choices_forward(void *h, int nb, uint32_t P, uint32_t C, uint32_t j, uint32_t inactiveMask, cudaStream_t stream);
-// KV-cache slots (csrc/cuda/slots.cu): n <= 8 independent sequences, slot s = rows [0, floor(seqLen / n)) of its own cache block
+// KV-cache slots (csrc/cuda/attn_decode.cu): n <= 8 independent sequences, slot s = rows [0, floor(seqLen / n)) of its own cache block
 int dl_engine_set_slots(void *h, uint32_t n);
 uint32_t dl_engine_slot_len(void *h);
 int dl_engine_slot_prefill(void *h, uint32_t slot, uint32_t T, uint32_t p0, cudaStream_t stream);   // T tokens staged in pTokens/pPos

@@ -84,13 +84,13 @@ struct RopeKvArgs {
     // Choice steps (several sequences at one rotary position): token t stores its K/V row at pos[t] + t * rowStride, and tokens
     // whose bit is set in inactiveMask store nothing. Both 0 for a plain batch of consecutive tokens.
     uint32_t rowStride, inactiveMask;
-    // Slots steps (slots.cu): token t stores its K/V row pos[t] at element offset t * slotStride (slot t, seqLen = the slot's
+    // Slots steps (attn_decode.cu): token t stores its K/V row pos[t] at element offset t * slotStride (slot t, seqLen = the slot's
     // length L). 0 for every other caller.
     uint64_t slotStride;
 };
 int launchRopeKv(const RopeKvArgs &a, int nb, cudaStream_t stream, bool pdl);
 
-// Attention of B choices that share the prompt rows [0, P] of the cache (choices.cu). Query row b (choice b, rotary position
+// Attention of B choices that share the prompt rows [0, P] of the cache (attn_decode.cu). Query row b (choice b, rotary position
 // P + 1 + j, already normalised and rotated by ropeKvKernel) attends to [0, P] and to its own rows [P + 1 + b * C, P + 1 + b * C + j].
 // A CTA owns (KV head, prefix split) and serves all B * nHeads / nKvHeads query rows of that head, so each prefix row is read
 // once per step. The last split also runs the per-choice suffixes; the last CTA to finish merges the splits.
@@ -108,7 +108,7 @@ struct ChoiceAttnArgs {
 };
 int launchChoiceAttn(const ChoiceAttnArgs &a, cudaStream_t stream, bool pdl);
 
-// Attention of B independent sequences, row b in KV-cache slot b (slots.cu): slot b is the [nKvHeads][L][headDim] block at element
+// Attention of B independent sequences, row b in KV-cache slot b (attn_decode.cu): slot b is the [nKvHeads][L][headDim] block at element
 // offset b * slotStride of the cache; query row b (position pos[b], already normalised and rotated by ropeKvKernel) attends to rows
 // [0, pos[b]] of its slot. A CTA owns (KV head, split, row) and serves the nHeads / nKvHeads q-heads of that KV head.
 struct SlotAttnArgs {

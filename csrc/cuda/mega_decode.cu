@@ -520,7 +520,7 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
 }
 
 // Attention phase: work items (head, split) are dealt round-robin to the CTAs (AttnItem); the 16 consumer warps of a CTA share
-// the positions of one item. Same math as attnFusedKernel (decode_ops.cu). The cached K/V rows of an item arrive through the ring,
+// the positions of one item. Same math as attnFusedKernel (attn_decode.cu). The cached K/V rows of an item arrive through the ring,
 // kKvChunk rows per fill (the producer issues them between this layer's QKV and WO fills), warp w takes rows 4w..4w+3 of each.
 // The q|k|v words are polled by warp 0 alone, and q is handed to the other warps through shared memory: this phase follows the
 // QKV epilogue without a grid barrier, so the poll covers the other CTAs' arrival skew.

@@ -179,7 +179,7 @@ class Engine:
         if presence or frequency or n:
             self._sampler_ready = True
 
-    # -- choices: several completions of one prompt, one row per choice (csrc/cuda/choices.cu) --
+    # -- choices: several completions of one prompt, one row per choice (csrc/cuda/attn_decode.cu) --
     def supports_choices(self, n: int) -> bool:
         """True if n choices can run as one batched step: dense layers, kernel-fused collectives, n <= max_batch."""
         return 1 <= n <= min(8, self.max_batch) and self.w.header.n_experts == 0 and not self._parts
@@ -241,7 +241,7 @@ class Engine:
         self.check_abort()
         return out
 
-    # -- KV-cache slots: up to 8 independent sequences decoded together (csrc/cuda/slots.cu) --
+    # -- KV-cache slots: up to 8 independent sequences decoded together (csrc/cuda/attn_decode.cu) --
     def set_slots(self, n: int) -> None:
         """Splits every layer's KV cache into n slots of floor(seq_len / n) rows. Single GPU, dense q40 layers only; n = 1 is
         the ordinary single-sequence engine."""

@@ -1,4 +1,4 @@
-"""Several completions of one prompt ("choices", csrc/cuda/choices.cu and the engine's choices step).
+"""Several completions of one prompt ("choices", csrc/cuda/attn_decode.cu and the engine's choices step).
 
 * choiceAttnKernel (+ ropeKvKernel with a row stride) against a float64 reference over the same bf16 cache. The inputs give
   scores with a standard deviation of about 4, and "needle" keys parallel to choice 0's first q-head sit on the first and last

@@ -1,4 +1,4 @@
-"""Decode attention (csrc/cuda/decode_ops.cu) against a float64 reference, beyond the first KV split.
+"""Decode attention (csrc/cuda/attn_decode.cu) against a float64 reference, beyond the first KV split.
 
 Kernels under test, through their stand-alone entry points:
 * attnFusedKernel: QK-norm + RoPE + KV append + split-KV attention of one token; ceil(nPos / 64) splits, capped at nSplits.

@@ -1,4 +1,4 @@
-"""Independent sequences in KV-cache slots (csrc/cuda/slots.cu, the engine's slots step, per-row sampling).
+"""Independent sequences in KV-cache slots (csrc/cuda/attn_decode.cu, the engine's slots step, per-row sampling).
 
 * slotAttnKernel against a float64 reference over the same bf16 cache, rows at different positions in different slots. "Needle"
   keys parallel to a row's first q-head sit on both sides of its split boundaries, and in the neighbouring slots at rows the
