@@ -725,6 +725,21 @@ DL_EXPORT int dl_engine_set_trace_all(void *h, int allCtas) {
 
 DL_EXPORT int dl_engine_mega_active(void *h) { return ((Engine *)h)->lastDecodeMega ? 1 : 0; }
 
+// Copies the persistent kernel's phase vectors, 8 zeroed tail words included, into caller-provided device memory: x (dim + 8
+// LL words), q|k|v (qkvDim + 8 LL words), z (qDim + 8 LL words) and the SwiGLU output (ffDim plain f32 in a buffer of ffDim + 8
+// words). Changes no engine state. -1 before the first dl_engine_enable_mega.
+DL_EXPORT int dl_engine_mega_copy_vectors(void *h, void *x, void *qkv, void *z, void *hF, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    if (!e->megaX) return -1;
+    const dl::EngineConfig &c = e->cfg;
+    const size_t qDim = (size_t)c.nHeads * c.headDim, qkvDim = qDim + 2 * (size_t)c.nKvHeads * c.headDim;
+    void *dst[4] = {x, qkv, z, hF};
+    const uint2 *src[4] = {e->megaX, e->megaQkv, e->megaZ, e->megaH};
+    const size_t n[4] = {c.dim, qkvDim, qDim, c.ffDim};
+    for (int i = 0; i < 4; i++) DL_CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], (n[i] + 8) * sizeof(uint2), cudaMemcpyDeviceToDevice, stream));
+    return 0;
+}
+
 DL_EXPORT uint32_t dl_engine_num_sms(void *h) { return ((Engine *)h)->cfg.numSms; }
 
 DL_EXPORT int dl_engine_forward(void *h, int nb, int logitsMode, int greedyAdvance, cudaStream_t stream) {

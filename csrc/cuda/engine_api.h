@@ -87,6 +87,8 @@ int dl_engine_enable_mega(void *h, int enable);
 int dl_engine_set_vocab_limit(void *h, uint32_t limit);   // greedy arg-max never returns ids >= limit (tokenizer vocabulary size)
 int dl_engine_aborted(void *h);
 int dl_engine_mega_active(void *h);   // 1 if the last single-token forward ran on the persistent kernel (0: fell back to the multi-kernel path)
+// Copies the persistent kernel's x, q|k|v, z (LL words) and SwiGLU (f32) vectors with their 8 tail words into device memory (tests).
+int dl_engine_mega_copy_vectors(void *h, void *x, void *qkv, void *z, void *hF, cudaStream_t stream);
 unsigned long long dl_engine_sync_ns(void *h);
 int dl_engine_sampler_seed(void *h, unsigned long long seed);
 int dl_engine_sample(void *h, float temperature, float topp, cudaStream_t stream);   // after a forward with logitsMode 1

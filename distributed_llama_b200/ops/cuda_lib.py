@@ -159,6 +159,8 @@ def lib() -> C.CDLL:
     L.dl_engine_sync_ns.restype = C.c_uint64
     L.dl_engine_mega_active.argtypes = [vp]
     L.dl_engine_mega_active.restype = i32
+    L.dl_engine_mega_copy_vectors.argtypes = [vp, vp, vp, vp, vp, vp]
+    L.dl_engine_mega_copy_vectors.restype = i32
     L.dl_engine_aborted.argtypes = [vp]
     L.dl_engine_aborted.restype = i32
     L.dl_engine_set_trace_all.argtypes = [vp, i32]

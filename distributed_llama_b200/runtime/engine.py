@@ -323,6 +323,22 @@ class Engine:
         the co-residency check rules it out)."""
         return bool(self._lib.dl_engine_mega_active(self._h))
 
+    def mega_vectors(self) -> dict:
+        """The persistent kernel's phase vectors after its last launch, copied on the current stream: "x" (final residual),
+        "qkv" (q|k|v before QK-norm and RoPE) and "z" (attention output) as (f32 payload, int64 epoch) pairs of LL words, and
+        "h" (the last layer's SwiGLU output) as plain f32. Every vector carries its 8 tail words (zero unless overwritten)."""
+        h = self.w.header
+        n = {"x": h.dim, "qkv": self.qkv_dim, "z": self.w.n_heads * h.head_dim, "h": self.w.ff_dim}
+        buf = {k: torch.empty((v + 8) * 2, dtype=torch.int32, device=self.device) for k, v in n.items()}
+        cl.check(self._lib.dl_engine_mega_copy_vectors(self._h, *(buf[k].data_ptr() for k in ("x", "qkv", "z", "h")), cl.stream_ptr()),
+                 "engine_mega_copy_vectors")
+        out = {}
+        for k in ("x", "qkv", "z"):
+            words = buf[k].view(-1, 2)
+            out[k] = (words[:, 0].view(torch.float32), words[:, 1].to(torch.int64) & 0xFFFFFFFF)
+        out["h"] = buf["h"].view(torch.float32)
+        return out
+
     def check_abort(self):
         """Raises if a device-side wait loop ran out of its spin budget (a peer rank died or a CTA never became resident): the
         kernels drain instead of hanging and flag the step as invalid (csrc/cuda/mega_decode.cu: SpinGuard)."""
