@@ -76,14 +76,16 @@ const char *kUsage =
     "Usage: dllama-api-native --model <path> --tokenizer <path> [--host <addr>] [--port <p>] [--max-seq-len <n>]\n"
     "        [--temperature <t>] [--topp <p>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]\n"
     "        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--gpu-index <i>]\n"
+    "        [--kv-cache-float-type {bf16|q80}]  KV-cache storage (default bf16; q80 = int8 blocks of 32 + f16 scale)\n"
     "        [--parallel <n>]  decode up to n (1..8) chat requests together, each in its own KV-cache slot of floor(context / n)\n"
     "                       tokens; one GPU and dense models only\n"
     "        [--gpus <n>]   tensor parallel over n GPUs: a supervisor forks one process per GPU (rank 0 serves HTTP) and restarts\n"
     "                       the whole job 3 s after any rank fails\n";
 
 // One attempt of rank 0 of a job (or the only process on one GPU): engine + tokenizer + HTTP server until --max-requests is reached.
-int serveOnce(const std::string &model, const std::string &tokenizer, uint32_t maxSeqLen, int gpu, const ApiConfig &cfg, TpJob &job) {
-    NativeEngine engine(model, maxSeqLen, gpu, 0, job.nRanks, job.tag, [&job] { job.barrier(); });
+int serveOnce(const std::string &model, const std::string &tokenizer, uint32_t maxSeqLen, int gpu, const ApiConfig &cfg, TpJob &job,
+              uint32_t kvType) {
+    NativeEngine engine(model, maxSeqLen, gpu, 0, job.nRanks, job.tag, [&job] { job.barrier(); }, kvType);
     Tokenizer tok(tokenizer);
     if (job.nRanks > 1) job.barrier();   // every rank has its weights
     std::printf("%s%s", tok.describe().c_str(), describeModelHeader(engine.header()).c_str());
@@ -109,7 +111,7 @@ int main(int argc, char **argv) {
     std::string model, tokenizer;
     ApiConfig cfg;
     cfg.seed = (uint64_t)std::time(nullptr);
-    uint32_t maxSeqLen = 0;
+    uint32_t maxSeqLen = 0, kvType = 0;
     int gpu = 0;
     uint32_t gpus = 1, workers = 0;
     try {
@@ -124,6 +126,7 @@ int main(int argc, char **argv) {
             else if (name == "--host") cfg.host = v;
             else if (name == "--port") cfg.port = std::stoi(v);
             else if (name == "--max-seq-len") maxSeqLen = (uint32_t)std::stoul(v);
+            else if (name == "--kv-cache-float-type") kvType = parseKvCacheFloatType(v);
             else if (name == "--temperature") cfg.temperature = std::stof(v);
             else if (name == "--topp") cfg.topp = std::stof(v);
             else if (name == "--presence-penalty") cfg.presencePenalty = parsePenalty(name, v);
@@ -155,7 +158,7 @@ int main(int argc, char **argv) {
         while (true) {
             try {
                 TpJob job;
-                return serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job);
+                return serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType);
             } catch (const ParallelRefused &e) {
                 std::fprintf(stderr, "%s\n", e.what());
                 return 1;
@@ -186,7 +189,7 @@ int main(int argc, char **argv) {
                 int rc = 1;
                 if (r == 0) {
                     try {
-                        rc = serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job);
+                        rc = serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType);
                         job.sendExit();
                     } catch (const std::exception &e) {
                         job.fail(e.what());
@@ -194,7 +197,7 @@ int main(int argc, char **argv) {
                     }
                 } else {
                     std::fclose(stdin);
-                    rc = tpWorkerMain(model, tokenizer, maxSeqLen, gpu, job);
+                    rc = tpWorkerMain(model, tokenizer, maxSeqLen, gpu, job, kvType);
                 }
                 std::fflush(stdout);
                 _exit(rc);

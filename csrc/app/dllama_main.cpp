@@ -42,6 +42,7 @@ struct Args {
     std::string mode, model, tokenizer, prompt, chatTemplate, bufferFloatType = "q80";
     bool hasPrompt = false, help = false;
     uint32_t steps = 0, maxSeqLen = 0;
+    uint32_t kvType = 0;    // --kv-cache-float-type: 0 = bf16, 1 = q80
     float temperature = 0.8f, topp = 0.9f;
     float presencePenalty = 0.f, frequencyPenalty = 0.f;
     uint64_t seed = (uint64_t)std::time(nullptr);
@@ -52,7 +53,7 @@ struct Args {
 const char *kUsage =
     "Usage: dllama-native {inference|perplexity|chat} --model <path> --tokenizer <path>\n"
     "        [--prompt <text>] [--steps <n>] [--temperature <t>] [--topp <p>] [--presence-penalty <p>] [--frequency-penalty <f>]\n"
-    "        [--seed <s>] [--max-seq-len <n>]\n"
+    "        [--seed <s>] [--max-seq-len <n>] [--kv-cache-float-type {bf16|q80}]\n"
     "        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--buffer-float-type q80] [--gpu-index <i>]\n"
     "        [--gpus <n>]   tensor parallel over GPUs gpu-index .. gpu-index + n - 1 of this machine (one process per GPU)\n"
     "        (accepted for drop-in compatibility and ignored: --nthreads --net-turbo --gpu-segments --workers --host --port)\n";
@@ -81,6 +82,7 @@ Args parse(int argc, char **argv) {
         else if (name == "--frequency-penalty") a.frequencyPenalty = parsePenalty(name, value);
         else if (name == "--seed") a.seed = std::stoull(value);
         else if (name == "--max-seq-len") a.maxSeqLen = (uint32_t)std::stoul(value);
+        else if (name == "--kv-cache-float-type") a.kvType = parseKvCacheFloatType(value);
         else if (name == "--chat-template") a.chatTemplate = value;
         else if (name == "--buffer-float-type") a.bufferFloatType = value;
         else if (name == "--gpu-index") a.gpuIndex = std::max(0, std::stoi(value));
@@ -105,7 +107,7 @@ struct App {
     Sampler sampler;
     TpEngine tp;
     App(const Args &a, TpJob &j)
-        : args(a), job(j), engine(a.model, a.maxSeqLen, a.gpuIndex + (int)j.rank, j.rank, j.nRanks, j.tag, [&j] { j.barrier(); }),
+        : args(a), job(j), engine(a.model, a.maxSeqLen, a.gpuIndex + (int)j.rank, j.rank, j.nRanks, j.tag, [&j] { j.barrier(); }, a.kvType),
           tokenizer(a.tokenizer),
           sampler(std::min<uint32_t>(tokenizer.vocabSize(), engine.header().vocabSize), a.temperature, a.topp, a.seed), tp{engine, j} {
         // sampling ranges over the tokenizer's vocabulary (reference src/app.cpp:243-246); padded embedding rows never win
@@ -281,7 +283,7 @@ int main(int argc, char **argv) {
                     prctl(PR_SET_PDEATHSIG, SIGKILL);
                     job.rank = r; job.reapChildren = false; job.parentPid = rootPid;
                     std::fclose(stdin);
-                    _exit(tpWorkerMain(a.model, a.tokenizer, a.maxSeqLen, a.gpuIndex, job));
+                    _exit(tpWorkerMain(a.model, a.tokenizer, a.maxSeqLen, a.gpuIndex, job, a.kvType));
                 }
                 children.push_back(pid);
             }
@@ -304,7 +306,7 @@ int main(int argc, char **argv) {
             std::printf("Tokenizer vocab size (%u) does not match the model vocab size (%u)\n", app.tokenizer.vocabSize(), h.vocabSize);
         std::printf("%s", app.tokenizer.describe().c_str());
         std::printf("%s", describeModelHeader(h).c_str());
-        std::printf("📀 RequiredMemory: %llu MB\n", (unsigned long long)(requiredDeviceBytes(h, job.nRanks, 2) / (1024 * 1024)));
+        std::printf("📀 RequiredMemory: %llu MB\n", (unsigned long long)((requiredDeviceBytes(h, job.nRanks, 0) + kvCacheBytes(h, job.nRanks, a.kvType)) / (1024 * 1024)));
         if (job.nRanks > 1)
             std::printf("🔗 %u GPUs (one process each), all-reduce inside the kernels over %s\n", job.nRanks,
                         app.engine.multicast() ? "the NVSwitch multicast mapping (multimem.st)" : "NVLink peer memory");

@@ -60,6 +60,7 @@ struct NativeEngine::Impl {
         Q40Dev qkv, wo, w13, w2;
         float *norm0 = nullptr, *norm1 = nullptr, *qNorm = nullptr, *kNorm = nullptr, *moeGate = nullptr;
         void *kCache = nullptr, *vCache = nullptr;
+        void *kScale = nullptr, *vScale = nullptr;   // q80 cache (kvType 1)
     };
     std::vector<Layer> layers;
     // activations / state
@@ -84,7 +85,7 @@ void *NativeEngine::dev(size_t bytes) {
 }
 
 NativeEngine::NativeEngine(const std::string &modelPath, uint32_t maxSeqLen, int device, uint32_t rank, uint32_t nRanks,
-                           const std::string &commTag, std::function<void()> hostBarrier) {
+                           const std::string &commTag, std::function<void()> hostBarrier, uint32_t kvType) {
     rank_ = rank; nRanks_ = std::max(1u, nRanks);
     h_ = loadModelHeader(modelPath, maxSeqLen);
     if (h_.weightType != F_Q40)
@@ -92,6 +93,8 @@ NativeEngine::NativeEngine(const std::string &modelPath, uint32_t maxSeqLen, int
     if (h_.headDim != 64 && h_.headDim != 128) throw std::runtime_error("unsupported head dimension");
     dir_ = buildTensorDirectory(h_, true);
     seqLen_ = h_.seqLen;
+    if (kvType > 1) throw std::runtime_error("unknown KV-cache float type");
+    kvType_ = kvType;
     impl_ = new Impl();
     try {
         cudaCheck(cudaSetDevice(device), "cudaSetDevice");
@@ -156,6 +159,7 @@ NativeEngine::NativeEngine(const std::string &modelPath, uint32_t maxSeqLen, int
         cfg.nSplits = nSplits_; cfg.rank = rank_; cfg.nRanks = N; cfg.numSms = (uint32_t)sms; cfg.eps = h_.normEpsilon; cfg.usePdl = 1;
         cfg.moeFirstExpert = 0; cfg.moeNumLocal = h_.nExperts; cfg.wType = 0;
         cfg.hiddenAct = h_.hiddenAct == ACT_GELU ? 1u : 0u;
+        cfg.kvType = kvType_;
         I.engine = dl_engine_create(&cfg);
         if (!I.engine) throw std::runtime_error("dl_engine_create failed");
         for (uint32_t l = 0; l < h_.nLayers; l++) {
@@ -164,7 +168,7 @@ NativeEngine::NativeEngine(const std::string &modelPath, uint32_t maxSeqLen, int
             lp.qkvQs = L.qkv.qs; lp.qkvSc = L.qkv.scales; lp.woQs = L.wo.qs; lp.woSc = L.wo.scales;
             lp.w13Qs = L.w13.qs; lp.w13Sc = L.w13.scales; lp.w2Qs = L.w2.qs; lp.w2Sc = L.w2.scales;
             lp.norm0 = L.norm0; lp.norm1 = L.norm1; lp.qNorm = L.qNorm; lp.kNorm = L.kNorm; lp.moeGate = L.moeGate;
-            lp.kCache = L.kCache; lp.vCache = L.vCache;
+            lp.kCache = L.kCache; lp.vCache = L.vCache; lp.kScale = L.kScale; lp.vScale = L.vScale;
             engCheck(dl_engine_set_layer(I.engine, l, &lp), "dl_engine_set_layer");
         }
         engCheck(dl_engine_set_globals(I.engine, &g), "dl_engine_set_globals");
@@ -314,8 +318,13 @@ void NativeEngine::uploadWeights(const uint8_t *file) {
             L.kNorm = f32Tensor(I.entry("block_norm_k", l), neox ? &perm : nullptr);
         }
         if (h_.nExperts > 0) L.moeGate = f32Tensor(I.entry("block_moe_gate", l));
-        L.kCache = dev((size_t)kvHeadsL_ * seqLen_ * hd * 2);
-        L.vCache = dev((size_t)kvHeadsL_ * seqLen_ * hd * 2);
+        const size_t kvValues = (size_t)kvHeadsL_ * seqLen_ * hd;
+        L.kCache = dev(kvValues * (kvType_ ? 1 : 2));
+        L.vCache = dev(kvValues * (kvType_ ? 1 : 2));
+        if (kvType_) {   // q80 scale planes, 16 bytes of tail padding for the persistent kernel's aligned bulk copies
+            L.kScale = dev(kvValues / 16 + 16);
+            L.vScale = dev(kvValues / 16 + 16);
+        }
     }
     cudaCheck(cudaStreamSynchronize(st), "weight upload");
     cudaFree(staging);

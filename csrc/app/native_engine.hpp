@@ -8,12 +8,27 @@
 #pragma once
 #include <cstdint>
 #include <functional>
+#include <stdexcept>
 #include <string>
 #include <vector>
 
 #include "../host/model_format.hpp"
 
 namespace dl {
+
+// --kv-cache-float-type {bf16|q80} -> EngineConfig::kvType; throws std::runtime_error on anything else.
+inline uint32_t parseKvCacheFloatType(const std::string &v) {
+    if (v == "bf16") return 0;
+    if (v == "q80") return 1;
+    throw std::runtime_error("Invalid KV-cache float type: " + v + " (expected bf16 or q80)");
+}
+
+// Device bytes of one rank's K and V caches: bf16 = 2 bytes a value, q80 = 1 byte a value + a 2-byte scale per 32.
+inline uint64_t kvCacheBytes(const ModelHeader &h, uint32_t nRanks, uint32_t kvType) {
+    const uint64_t kvHeads = h.nKvHeads >= nRanks ? h.nKvHeads / nRanks : 1;
+    const uint64_t values = 2ull * h.nLayers * h.seqLen * kvHeads * h.headDim;
+    return kvType == 0 ? 2 * values : values + values / 16;
+}
 
 class NativeEngine {
 public:
@@ -24,14 +39,16 @@ public:
     // multicast, bootstrapped over unix sockets named after `commTag`) and the kernels do their all-reduces over it. `hostBarrier`
     // must synchronise all ranks of the job (it is called between the two bootstrap steps). Every rank then issues the same
     // sequence of prefill / step calls (reference: root + `dllama worker` processes, src/dllama.cpp:260-285).
+    // kvType: KV-cache storage, 0 = bf16, 1 = q80 (EngineConfig::kvType; parseKvCacheFloatType).
     NativeEngine(const std::string &modelPath, uint32_t maxSeqLen, int device, uint32_t rank = 0, uint32_t nRanks = 1,
-                 const std::string &commTag = std::string(), std::function<void()> hostBarrier = std::function<void()>());
+                 const std::string &commTag = std::string(), std::function<void()> hostBarrier = std::function<void()>(), uint32_t kvType = 0);
     ~NativeEngine();
     NativeEngine(const NativeEngine &) = delete;
     NativeEngine &operator=(const NativeEngine &) = delete;
 
     const ModelHeader &header() const { return h_; }
     uint32_t seqLen() const { return seqLen_; }
+    uint32_t kvType() const { return kvType_; }
     uint64_t bytesUploaded() const { return bytesUploaded_; }
     uint32_t rank() const { return rank_; }
     uint32_t nRanks() const { return nRanks_; }
@@ -94,6 +111,7 @@ private:
     std::vector<TensorEntry> dir_;
     uint32_t slots_ = 1;
     uint32_t seqLen_ = 0, maxBatch_ = 8, maxPrefill_ = 192, nSplits_ = 1, qkvDim_ = 0;
+    uint32_t kvType_ = 0;                                                  // KV-cache storage: 0 = bf16, 1 = q80
     uint32_t rank_ = 0, nRanks_ = 1, kvRank_ = 0, kvSlices_ = 1;          // tensor-parallel placement of this process
     uint32_t headsL_ = 0, kvHeadsL_ = 0, ffL_ = 0, vocabL_ = 0;          // per-rank slice sizes
     bool mega_ = false, graphReady_ = false, multicast_ = false;

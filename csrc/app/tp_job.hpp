@@ -223,9 +223,10 @@ inline std::vector<uint64_t> tpChoiceSeeds(const int32_t *w, uint32_t n) {
 }
 
 // ranks >= 1: mirror the root's engine calls until TP_OP_EXIT (reference: runWorkerApp, src/app.cpp:306-365). Returns the exit code.
-inline int tpWorkerMain(const std::string &model, const std::string &tokenizer, uint32_t maxSeqLen, int gpuIndex, TpJob &job) {
+inline int tpWorkerMain(const std::string &model, const std::string &tokenizer, uint32_t maxSeqLen, int gpuIndex, TpJob &job,
+                        uint32_t kvType = 0) {
     try {
-        NativeEngine engine(model, maxSeqLen, gpuIndex + (int)job.rank, job.rank, job.nRanks, job.tag, [&job] { job.barrier(); });
+        NativeEngine engine(model, maxSeqLen, gpuIndex + (int)job.rank, job.rank, job.nRanks, job.tag, [&job] { job.barrier(); }, kvType);
         {
             Tokenizer tok(tokenizer);      // only for the vocabulary limit of the greedy arg-max (must match the root)
             engine.setVocabLimit(tok.vocabSize());

@@ -1,6 +1,7 @@
-// Decode attention: a few query tokens against the bf16 head-major KV cache ([nKvHeads][seqLen][headDim]), flash-decoding style
+// Decode attention: a few query tokens against the head-major KV cache ([nKvHeads][seqLen][headDim]), flash-decoding style
 // (online softmax over KV splits, merged in split order by the last CTA to finish). Reference op: OP_MULTIHEAD_ATT
-// (nn-cpu-ops.cpp:753-788).
+// (nn-cpu-ops.cpp:753-788). Every kernel is instantiated for both cache storages (template parameter Q8, see kernels.h): bf16 rows,
+// or q80 rows dequantised on load; the q.k and p.v math is f32 either way.
 //
 // Four kernels, built from the shared pieces of the anonymous namespace below:
 // * attnDecodeKernel: one CTA per (q-head, split, token), K/V rows streamed through registers. The GEMV-path batch and the
@@ -25,10 +26,19 @@
 // element offset s * slotStride, slotStride = nKvHeads * L * headDim. Row b of the step is slot b; its token sits at position pos[b]
 // and its K/V row pos[b] was written by ropeKvKernel (RopeKvArgs::slotStride) before slotAttnKernel runs. Row b attends to rows
 // [0, pos[b]] of its own slot and nothing else.
+#include <type_traits>
+
 #include "kernels.h"
 
 namespace dl {
 namespace {
+
+// The value plane of a cache (bf16, or int8 for Q8) advanced by `elems` elements.
+template <bool Q8, typename P>
+__device__ __forceinline__ P *kvPlane(P *plane, size_t elems) {
+    using B = typename std::conditional<std::is_const<P>::value, const uint8_t, uint8_t>::type;
+    return reinterpret_cast<B *>(plane) + elems * (Q8 ? 1 : 2);
+}
 
 // Split `split` when the number of splits follows from the length: ceil(nPos / 64) of them, at most nSplits, so short contexts run
 // as one CTA per group with no merge pass. A row's splits depend on its own length only.
@@ -45,35 +55,22 @@ __device__ __forceinline__ SplitRange effectiveSplit(uint32_t nPos, uint32_t nSp
 }
 
 // Online softmax of one query head over cache rows [begin, end), K/V streamed through registers: each warp takes UN = 4 rows at a
-// time, the 4 warps round robin, and lane i holds dims [i * DPL, (i + 1) * DPL). kBase / vBase point at the lane's dims of row 0.
-template <int HD>
-__device__ __forceinline__ void scanRows(const __nv_bfloat16 *kBase, const __nv_bfloat16 *vBase, const float (&q)[HD / 32],
+// time, the 4 warps round robin, and lane i holds dims [i * DPL, (i + 1) * DPL). kHead / vHead (and kSc / vSc, Q8) point at the
+// KV head's row 0.
+template <int HD, bool Q8>
+__device__ __forceinline__ void scanRows(const void *kHead, const void *vHead, const __half *kSc, const __half *vSc, const float (&q)[HD / 32],
                                          uint32_t begin, uint32_t end, float &m, float &l, float (&acc)[HD / 32]) {
     constexpr int DPL = HD / 32, UN = 4;
     const int warp = threadIdx.x >> 5;
+    const uint32_t d0 = (threadIdx.x & 31) * DPL;
     for (uint32_t s0 = begin + warp * UN; s0 < end; s0 += 4 * UN) {
         float kf[UN][DPL], vf[UN][DPL];
 #pragma unroll
         for (int u = 0; u < UN; u++) {
             const uint32_t s = s0 + u;
             if (s < end) {
-                if constexpr (DPL == 4) {
-                    const uint2 kr = *reinterpret_cast<const uint2 *>(kBase + (size_t)s * HD);
-                    const uint2 vr = *reinterpret_cast<const uint2 *>(vBase + (size_t)s * HD);
-                    const float2 k0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&kr.x));
-                    const float2 k1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&kr.y));
-                    const float2 v0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&vr.x));
-                    const float2 v1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&vr.y));
-                    kf[u][0] = k0.x; kf[u][1] = k0.y; kf[u][2] = k1.x; kf[u][3] = k1.y;
-                    vf[u][0] = v0.x; vf[u][1] = v0.y; vf[u][2] = v1.x; vf[u][3] = v1.y;
-                } else {
-                    const uint32_t kr = *reinterpret_cast<const uint32_t *>(kBase + (size_t)s * HD);
-                    const uint32_t vr = *reinterpret_cast<const uint32_t *>(vBase + (size_t)s * HD);
-                    const float2 k0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&kr));
-                    const float2 v0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&vr));
-                    kf[u][0] = k0.x; kf[u][1] = k0.y;
-                    vf[u][0] = v0.x; vf[u][1] = v0.y;
-                }
+                loadKv<DPL, Q8>(kHead, kSc, (size_t)s * HD + d0, kf[u]);
+                loadKv<DPL, Q8>(vHead, vSc, (size_t)s * HD + d0, vf[u]);
             } else {
 #pragma unroll
                 for (int i = 0; i < DPL; i++) { kf[u][i] = 0.f; vf[u][i] = 0.f; }
@@ -182,50 +179,73 @@ __device__ __forceinline__ void finishSplit(float *partial, unsigned int *counte
 constexpr int kTile = 32;   // K/V rows per shared-memory tile
 
 // Dynamic shared memory of a tile kernel with R query rows: q [R][HD] (pre-scaled by 1/sqrt(HD)), the online-softmax state acc
-// [R][HD], m [R] and l [R], then one K and one V tile of kTile rows.
-template <int HD>
+// [R][HD], m [R] and l [R], then one K and one V tile of kTile rows. A bf16 cache is staged as bf16; a q80 one is widened to f32 on
+// the way in (q * d needs more mantissa than bf16 has).
+template <int HD, bool Q8>
 struct TileSmem {
-    static constexpr int kRowPad = HD + 2;   // bf16 per staged row: the odd word stride keeps lane-per-row K reads conflict-free
+    using T = typename std::conditional<Q8, float, __nv_bfloat16>::type;
+    // elements per staged row: the odd word stride keeps lane-per-row K reads conflict-free
+    static constexpr int kRowPad = Q8 ? HD + 1 : HD + 2;
     float *q, *acc, *m, *l;
-    __nv_bfloat16 *k, *v;
+    T *k, *v;
     __device__ TileSmem(unsigned char *smem, uint32_t R)
         : q(reinterpret_cast<float *>(smem)), acc(q + (size_t)R * HD), m(acc + (size_t)R * HD), l(m + R),
-          k(reinterpret_cast<__nv_bfloat16 *>(l + R)), v(k + kTile * kRowPad) {}
+          k(reinterpret_cast<T *>(l + R)), v(k + kTile * kRowPad) {}
     static size_t bytes(uint32_t R) {
-        return (size_t)R * HD * 4 /* q */ + (size_t)R * HD * 4 /* acc */ + (size_t)R * 8 /* m, l */ + 2ull * kTile * kRowPad * 2;
+        return (size_t)R * HD * 4 /* q */ + (size_t)R * HD * 4 /* acc */ + (size_t)R * 8 /* m, l */ + 2ull * kTile * kRowPad * sizeof(T);
     }
 };
 
-// Query rows [r0, r1) attend to cache rows [row0, row0 + n) of one KV head (kHead / vHead point at its row 0). The rows are staged
-// kTile at a time; inside a tile lane i scores row i, and the query rows go to the warps round robin.
-template <int HD>
-__device__ __forceinline__ void attendTiles(const TileSmem<HD> &sm, const __nv_bfloat16 *kHead, const __nv_bfloat16 *vHead, uint32_t row0,
-                                            uint32_t n, uint32_t r0, uint32_t r1) {
-    constexpr int DPL = HD / 32, RP = TileSmem<HD>::kRowPad;
+// Query rows [r0, r1) attend to cache rows [row0, row0 + n) of one KV head (kHead / vHead, and kSc / vSc for Q8, point at its row 0).
+// The rows are staged kTile at a time; inside a tile lane i scores row i, and the query rows go to the warps round robin.
+template <int HD, bool Q8>
+__device__ __forceinline__ void attendTiles(const TileSmem<HD, Q8> &sm, const void *kHead, const void *vHead, const __half *kSc,
+                                            const __half *vSc, uint32_t row0, uint32_t n, uint32_t r0, uint32_t r1) {
+    constexpr int DPL = HD / 32, RP = TileSmem<HD, Q8>::kRowPad;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (uint32_t t0 = 0; t0 < n; t0 += kTile) {
         const uint32_t len = min((uint32_t)kTile, n - t0);
         __syncthreads();   // the previous tile (and the caller's initialisation) is complete
-        for (uint32_t i = threadIdx.x; i < kTile * (HD / 2); i += blockDim.x) {
-            const uint32_t rr = i / (HD / 2), c = i % (HD / 2);
-            __nv_bfloat162 kv = __floats2bfloat162_rn(0.f, 0.f), vv = kv;
-            if (rr < len) {
-                const size_t off = (size_t)(row0 + t0 + rr) * HD + 2 * c;
-                kv = *reinterpret_cast<const __nv_bfloat162 *>(kHead + off);
-                vv = *reinterpret_cast<const __nv_bfloat162 *>(vHead + off);
+        if constexpr (Q8) {
+            for (uint32_t i = threadIdx.x; i < kTile * (HD / 4); i += blockDim.x) {
+                const uint32_t rr = i / (HD / 4), c = i % (HD / 4);
+                float kf[4] = {0.f, 0.f, 0.f, 0.f}, vf[4] = {0.f, 0.f, 0.f, 0.f};
+                if (rr < len) {
+                    const size_t off = (size_t)(row0 + t0 + rr) * HD + 4 * c;
+                    loadKv<4, true>(kHead, kSc, off, kf);
+                    loadKv<4, true>(vHead, vSc, off, vf);
+                }
+#pragma unroll
+                for (int x = 0; x < 4; x++) { sm.k[rr * RP + 4 * c + x] = kf[x]; sm.v[rr * RP + 4 * c + x] = vf[x]; }
             }
-            reinterpret_cast<__nv_bfloat162 *>(sm.k + rr * RP)[c] = kv;
-            reinterpret_cast<__nv_bfloat162 *>(sm.v + rr * RP)[c] = vv;
+        } else {
+            for (uint32_t i = threadIdx.x; i < kTile * (HD / 2); i += blockDim.x) {
+                const uint32_t rr = i / (HD / 2), c = i % (HD / 2);
+                __nv_bfloat162 kv = __floats2bfloat162_rn(0.f, 0.f), vv = kv;
+                if (rr < len) {
+                    const size_t off = (size_t)(row0 + t0 + rr) * HD + 2 * c;
+                    kv = *reinterpret_cast<const __nv_bfloat162 *>(reinterpret_cast<const __nv_bfloat16 *>(kHead) + off);
+                    vv = *reinterpret_cast<const __nv_bfloat162 *>(reinterpret_cast<const __nv_bfloat16 *>(vHead) + off);
+                }
+                reinterpret_cast<__nv_bfloat162 *>(sm.k + rr * RP)[c] = kv;
+                reinterpret_cast<__nv_bfloat162 *>(sm.v + rr * RP)[c] = vv;
+            }
         }
         __syncthreads();
         for (uint32_t r = r0 + warp; r < r1; r += 4) {
             const float *q = sm.q + (size_t)r * HD;
-            const __nv_bfloat162 *kr = reinterpret_cast<const __nv_bfloat162 *>(sm.k + lane * RP);
             float s = 0.f;
+            if constexpr (Q8) {
+                const float *kr = sm.k + lane * RP;
 #pragma unroll 8
-            for (int c = 0; c < HD / 2; c++) {
-                const float2 k2 = __bfloat1622float2(kr[c]);
-                s += q[2 * c] * k2.x + q[2 * c + 1] * k2.y;
+                for (int c = 0; c < HD / 2; c++) s += q[2 * c] * kr[2 * c] + q[2 * c + 1] * kr[2 * c + 1];
+            } else {
+                const __nv_bfloat162 *kr = reinterpret_cast<const __nv_bfloat162 *>(sm.k + lane * RP);
+#pragma unroll 8
+                for (int c = 0; c < HD / 2; c++) {
+                    const float2 k2 = __bfloat1622float2(kr[c]);
+                    s += q[2 * c] * k2.x + q[2 * c + 1] * k2.y;
+                }
             }
             const bool valid = (uint32_t)lane < len;
             const float mOld = sm.m[r];
@@ -238,12 +258,18 @@ __device__ __forceinline__ void attendTiles(const TileSmem<HD> &sm, const __nv_b
             for (int i = 0; i < DPL; i++) acc[i] = sm.acc[(size_t)r * HD + lane * DPL + i] * corr;
             for (uint32_t u = 0; u < len; u++) {
                 const float pu = __shfl_sync(0xffffffffu, pr, u);
-                const __nv_bfloat16 *vr = sm.v + u * RP + lane * DPL;
+                if constexpr (Q8) {
+                    const float *vr = sm.v + u * RP + lane * DPL;
 #pragma unroll
-                for (int i = 0; i < DPL; i += 2) {
-                    const float2 v2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(vr + i));
-                    acc[i] += pu * v2.x;
-                    acc[i + 1] += pu * v2.y;
+                    for (int i = 0; i < DPL; i++) acc[i] += pu * vr[i];
+                } else {
+                    const __nv_bfloat16 *vr = sm.v + u * RP + lane * DPL;
+#pragma unroll
+                    for (int i = 0; i < DPL; i += 2) {
+                        const float2 v2 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(vr + i));
+                        acc[i] += pu * v2.x;
+                        acc[i + 1] += pu * v2.y;
+                    }
                 }
             }
 #pragma unroll
@@ -271,7 +297,7 @@ int launchTiles(dim3 grid, size_t smem, cudaStream_t stream, bool pdl, const Arg
 
 // ---- GEMV-path batch: grid (nHeads, nSplits, nb), block 128 (4 warps). HD in {64, 128} --------------------------------------------
 // Every one of the nSplits splits runs, those past nPos empty, so the merge sums the same splits whatever the length.
-template <int HD>
+template <int HD, bool Q8>
 __global__ void __launch_bounds__(128) attnDecodeKernel(AttnArgs a) {
     constexpr int DPL = HD / 32;   // dims per lane
     pdlLaunchDependents();
@@ -294,13 +320,13 @@ __global__ void __launch_bounds__(128) attnDecodeKernel(AttnArgs a) {
 #pragma unroll
         for (int i = 0; i < DPL; i++) q[i] = qrow[i] * scale;
     }
-    const __nv_bfloat16 *kBase = a.kCache + (size_t)kvh * a.seqLen * HD + lane * DPL;
-    const __nv_bfloat16 *vBase = a.vCache + (size_t)kvh * a.seqLen * HD + lane * DPL;
+    const size_t headOff = (size_t)kvh * a.seqLen * HD;
+    const __half *kSc = Q8 ? a.kScale + headOff / 32 : nullptr, *vSc = Q8 ? a.vScale + headOff / 32 : nullptr;
 
     float m = -INFINITY, l = 0.f, acc[DPL];
 #pragma unroll
     for (int i = 0; i < DPL; i++) acc[i] = 0.f;
-    scanRows<HD>(kBase, vBase, q, begin, end, m, l, acc);
+    scanRows<HD, Q8>(kvPlane<Q8>(a.kCache, headOff), kvPlane<Q8>(a.vCache, headOff), kSc, vSc, q, begin, end, m, l, acc);
     float num, L;
     const float M = combineWarps<HD, false>(m, l, acc, num, L);
     finishSplit<HD>(a.partial, a.counters, (size_t)t * a.nHeads + h, a.nSplits, 1, split, a.nSplits, [&](uint32_t) { return num; },
@@ -316,7 +342,7 @@ __global__ void __launch_bounds__(128) attnDecodeKernel(AttnArgs a) {
 // (effectiveSplit), so short contexts run as one CTA per head with no merge pass at all.
 // The current token's K/V never round-trips through the cache: the split that covers position `pos` rotates k
 // in registers; the first q-head of every KV group also appends k/v to the cache for later steps.
-template <int HD>
+template <int HD, bool Q8>
 __global__ void __launch_bounds__(128) attnFusedKernel(AttnFusedArgs a) {
     constexpr int DPL = HD / 32;
     static_assert(DPL == 2 || DPL == 4, "head dim must be 64 or 128");
@@ -369,8 +395,9 @@ __global__ void __launch_bounds__(128) attnFusedKernel(AttnFusedArgs a) {
 #pragma unroll
     for (int i = 0; i < DPL; i++) acc[i] = 0.f;
 
-    __nv_bfloat16 *kHead = a.kCache + (size_t)kvh * a.seqLen * HD;
-    __nv_bfloat16 *vHead = a.vCache + (size_t)kvh * a.seqLen * HD;
+    const size_t headOff = (size_t)kvh * a.seqLen * HD;
+    void *kHead = kvPlane<Q8>(a.kCache, headOff), *vHead = kvPlane<Q8>(a.vCache, headOff);
+    __half *kSc = Q8 ? a.kScale + headOff / 32 : nullptr, *vSc = Q8 ? a.vScale + headOff / 32 : nullptr;
     if (ownsNew && warp == 0) {
         float kn[DPL], vn[DPL];
 #pragma unroll
@@ -379,22 +406,10 @@ __global__ void __launch_bounds__(128) attnFusedKernel(AttnFusedArgs a) {
             vn[i] = a.qkv[qDim + kvDim + (size_t)kvh * HD + lane * DPL + i];
         }
         normRope(kn, a.kNorm);
-        // the cache holds bf16: use the rounded values here too so this step matches what later steps will read
-        __nv_bfloat162 kb[DPL / 2], vb[DPL / 2];
-#pragma unroll
-        for (int k = 0; k < DPL / 2; k++) {
-            kb[k] = __floats2bfloat162_rn(kn[2 * k], kn[2 * k + 1]);
-            vb[k] = __floats2bfloat162_rn(vn[2 * k], vn[2 * k + 1]);
-            const float2 kf = __bfloat1622float2(kb[k]), vf = __bfloat1622float2(vb[k]);
-            kn[2 * k] = kf.x; kn[2 * k + 1] = kf.y;
-            vn[2 * k] = vf.x; vn[2 * k + 1] = vf.y;
-        }
-        if (h % kvMul == 0) {
-            __nv_bfloat162 *kd = reinterpret_cast<__nv_bfloat162 *>(kHead + (size_t)p * HD + lane * DPL);
-            __nv_bfloat162 *vd = reinterpret_cast<__nv_bfloat162 *>(vHead + (size_t)p * HD + lane * DPL);
-#pragma unroll
-            for (int k = 0; k < DPL / 2; k++) { kd[k] = kb[k]; vd[k] = vb[k]; }
-        }
+        // use the values as the cache stores them here too, so this step matches what later steps will read
+        const size_t e = (size_t)p * HD + lane * DPL;
+        roundStoreKv<DPL, Q8>(kn, kHead, kSc, e, h % kvMul == 0);
+        roundStoreKv<DPL, Q8>(vn, vHead, vSc, e, h % kvMul == 0);
         float d = 0.f;
 #pragma unroll
         for (int i = 0; i < DPL; i++) d += q[i] * kn[i];
@@ -404,7 +419,7 @@ __global__ void __launch_bounds__(128) attnFusedKernel(AttnFusedArgs a) {
         for (int i = 0; i < DPL; i++) acc[i] = vn[i];
     }
 
-    scanRows<HD>(kHead + lane * DPL, vHead + lane * DPL, q, sp.begin, cachedEnd, m, l, acc);
+    scanRows<HD, Q8>(kHead, vHead, kSc, vSc, q, sp.begin, cachedEnd, m, l, acc);
     float num, L;
     const float M = combineWarps<HD, true>(m, l, acc, num, L);
     float *outRow = a.out + (size_t)h * HD;
@@ -447,13 +462,13 @@ __global__ void __launch_bounds__(128) attnFusedKernel(AttnFusedArgs a) {
 // ---- choices step: grid (nKvHeads, nSplits), block 128 (4 warps) ------------------------------------------------------------------
 // CTA (kvh, split) runs every query row of the KV head over its prefix chunk: R = B * kvMul rows, row r = b * kvMul + g is q-head
 // kvh * kvMul + g of choice b. The last effective split also attends each active choice to its own rows.
-template <int HD>
+template <int HD, bool Q8>
 __global__ void __launch_bounds__(128) choiceAttnKernel(ChoiceAttnArgs a) {
     pdlLaunchDependents();
     pdlWait();
     extern __shared__ __align__(16) unsigned char smem[];
     const uint32_t kvMul = a.nHeads / a.nKvHeads, R = a.B * kvMul;
-    const TileSmem<HD> sm(smem, R);
+    const TileSmem<HD, Q8> sm(smem, R);
     const uint32_t kvh = blockIdx.x, split = blockIdx.y;
     const SplitRange sp = effectiveSplit(a.P + 1, a.nSplits, split);
     if (split >= sp.eff) return;
@@ -466,13 +481,14 @@ __global__ void __launch_bounds__(128) choiceAttnKernel(ChoiceAttnArgs a) {
     }
     for (uint32_t r = threadIdx.x; r < R; r += blockDim.x) { sm.m[r] = -INFINITY; sm.l[r] = 0.f; }
 
-    const __nv_bfloat16 *kHead = a.kCache + (size_t)kvh * a.seqLen * HD;
-    const __nv_bfloat16 *vHead = a.vCache + (size_t)kvh * a.seqLen * HD;
-    attendTiles(sm, kHead, vHead, sp.begin, sp.end - sp.begin, 0, R);
+    const size_t headOff = (size_t)kvh * a.seqLen * HD;
+    const void *kHead = kvPlane<Q8>(a.kCache, headOff), *vHead = kvPlane<Q8>(a.vCache, headOff);
+    const __half *kSc = Q8 ? a.kScale + headOff / 32 : nullptr, *vSc = Q8 ? a.vScale + headOff / 32 : nullptr;
+    attendTiles(sm, kHead, vHead, kSc, vSc, sp.begin, sp.end - sp.begin, 0, R);
     if (split == sp.eff - 1) {
         for (uint32_t b = 0; b < a.B; b++) {
             if ((a.inactiveMask >> b) & 1u) continue;
-            attendTiles(sm, kHead, vHead, a.P + 1 + b * a.C, a.j + 1, b * kvMul, (b + 1) * kvMul);
+            attendTiles(sm, kHead, vHead, kSc, vSc, a.P + 1 + b * a.C, a.j + 1, b * kvMul, (b + 1) * kvMul);
         }
     }
     __syncthreads();
@@ -491,7 +507,7 @@ __global__ void __launch_bounds__(128) choiceAttnKernel(ChoiceAttnArgs a) {
 
 // ---- slots step: grid (nKvHeads, nSplits, B), block 128 (4 warps) -----------------------------------------------------------------
 // CTA (kvh, split, b) runs the kvMul q-heads of the KV head over its chunk of row b's slot (one q-head per warp, round robin).
-template <int HD>
+template <int HD, bool Q8>
 __global__ void __launch_bounds__(128) slotAttnKernel(SlotAttnArgs a) {
     pdlLaunchDependents();
     pdlWait();
@@ -499,7 +515,7 @@ __global__ void __launch_bounds__(128) slotAttnKernel(SlotAttnArgs a) {
     if (b < 32 && ((a.inactiveMask >> b) & 1u)) return;
     extern __shared__ __align__(16) unsigned char smem[];
     const uint32_t R = a.nHeads / a.nKvHeads;   // q-heads of this KV head
-    const TileSmem<HD> sm(smem, R);
+    const TileSmem<HD, Q8> sm(smem, R);
     int p = a.pos[b];
     if (p < 0) p = 0;
     if ((uint32_t)p >= a.L) p = (int)a.L - 1;
@@ -512,7 +528,8 @@ __global__ void __launch_bounds__(128) slotAttnKernel(SlotAttnArgs a) {
     for (uint32_t r = threadIdx.x; r < R; r += blockDim.x) { sm.m[r] = -INFINITY; sm.l[r] = 0.f; }
 
     const size_t headOff = (size_t)b * a.slotStride + (size_t)kvh * a.L * HD;
-    attendTiles(sm, a.kCache + headOff, a.vCache + headOff, sp.begin, sp.end - sp.begin, 0, R);
+    attendTiles(sm, kvPlane<Q8>(a.kCache, headOff), kvPlane<Q8>(a.vCache, headOff), Q8 ? a.kScale + headOff / 32 : nullptr,
+                Q8 ? a.vScale + headOff / 32 : nullptr, sp.begin, sp.end - sp.begin, 0, R);
     __syncthreads();
 
     float *outRow = a.out + (size_t)b * a.outStride + (size_t)kvh * R * HD;
@@ -527,16 +544,20 @@ __global__ void __launch_bounds__(128) slotAttnKernel(SlotAttnArgs a) {
 
 int launchAttnDecode(const AttnArgs &a, int nb, cudaStream_t stream, bool pdl) {
     const dim3 grid(a.nHeads, a.nSplits, nb);
-    if (a.headDim == 128) DL_CUDA_CHECK(launchPdl(attnDecodeKernel<128>, grid, dim3(128), 0, stream, pdl, a));
-    else if (a.headDim == 64) DL_CUDA_CHECK(launchPdl(attnDecodeKernel<64>, grid, dim3(128), 0, stream, pdl, a));
+    if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
+    const bool q8 = a.kScale != nullptr;
+    if (a.headDim == 128) DL_CUDA_CHECK(launchPdl(q8 ? attnDecodeKernel<128, true> : attnDecodeKernel<128, false>, grid, dim3(128), 0, stream, pdl, a));
+    else if (a.headDim == 64) DL_CUDA_CHECK(launchPdl(q8 ? attnDecodeKernel<64, true> : attnDecodeKernel<64, false>, grid, dim3(128), 0, stream, pdl, a));
     else return -1;
     return 0;
 }
 
 int launchAttnFused(const AttnFusedArgs &a, cudaStream_t stream, bool pdl) {
     const dim3 grid(a.nHeads, a.nSplits);
-    if (a.headDim == 128) DL_CUDA_CHECK(launchPdl(attnFusedKernel<128>, grid, dim3(128), 0, stream, pdl, a));
-    else if (a.headDim == 64) DL_CUDA_CHECK(launchPdl(attnFusedKernel<64>, grid, dim3(128), 0, stream, pdl, a));
+    if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
+    const bool q8 = a.kScale != nullptr;
+    if (a.headDim == 128) DL_CUDA_CHECK(launchPdl(q8 ? attnFusedKernel<128, true> : attnFusedKernel<128, false>, grid, dim3(128), 0, stream, pdl, a));
+    else if (a.headDim == 64) DL_CUDA_CHECK(launchPdl(q8 ? attnFusedKernel<64, true> : attnFusedKernel<64, false>, grid, dim3(128), 0, stream, pdl, a));
     else return -1;
     return 0;
 }
@@ -553,19 +574,31 @@ static bool choiceRowsFit(uint32_t B, uint32_t P, uint32_t C, uint32_t j, uint32
 int launchChoiceAttn(const ChoiceAttnArgs &a, cudaStream_t stream, bool pdl) {
     if (a.nKvHeads == 0 || a.nHeads % a.nKvHeads || a.nSplits < 1) return -1;
     if (!choiceRowsFit(a.B, a.P, a.C, a.j, a.inactiveMask, a.seqLen)) return -1;
+    if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
     const uint32_t R = a.B * (a.nHeads / a.nKvHeads);
     const dim3 grid(a.nKvHeads, a.nSplits);
-    if (a.headDim == 128) return launchTiles<choiceAttnKernel<128>>(grid, TileSmem<128>::bytes(R), stream, pdl, a);
-    if (a.headDim == 64) return launchTiles<choiceAttnKernel<64>>(grid, TileSmem<64>::bytes(R), stream, pdl, a);
+    if (a.kScale) {
+        if (a.headDim == 128) return launchTiles<choiceAttnKernel<128, true>>(grid, TileSmem<128, true>::bytes(R), stream, pdl, a);
+        if (a.headDim == 64) return launchTiles<choiceAttnKernel<64, true>>(grid, TileSmem<64, true>::bytes(R), stream, pdl, a);
+        return -1;
+    }
+    if (a.headDim == 128) return launchTiles<choiceAttnKernel<128, false>>(grid, TileSmem<128, false>::bytes(R), stream, pdl, a);
+    if (a.headDim == 64) return launchTiles<choiceAttnKernel<64, false>>(grid, TileSmem<64, false>::bytes(R), stream, pdl, a);
     return -1;
 }
 
 int launchSlotAttn(const SlotAttnArgs &a, cudaStream_t stream, bool pdl) {
     if (a.nKvHeads == 0 || a.nHeads % a.nKvHeads || a.nSplits < 1 || a.L < 1 || a.B < 1 || a.B > 32) return -1;
+    if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
     const uint32_t R = a.nHeads / a.nKvHeads;
     const dim3 grid(a.nKvHeads, a.nSplits, a.B);
-    if (a.headDim == 128) return launchTiles<slotAttnKernel<128>>(grid, TileSmem<128>::bytes(R), stream, pdl, a);
-    if (a.headDim == 64) return launchTiles<slotAttnKernel<64>>(grid, TileSmem<64>::bytes(R), stream, pdl, a);
+    if (a.kScale) {
+        if (a.headDim == 128) return launchTiles<slotAttnKernel<128, true>>(grid, TileSmem<128, true>::bytes(R), stream, pdl, a);
+        if (a.headDim == 64) return launchTiles<slotAttnKernel<64, true>>(grid, TileSmem<64, true>::bytes(R), stream, pdl, a);
+        return -1;
+    }
+    if (a.headDim == 128) return launchTiles<slotAttnKernel<128, false>>(grid, TileSmem<128, false>::bytes(R), stream, pdl, a);
+    if (a.headDim == 64) return launchTiles<slotAttnKernel<64, false>>(grid, TileSmem<64, false>::bytes(R), stream, pdl, a);
     return -1;
 }
 
@@ -579,7 +612,7 @@ DL_EXPORT int dl_attn_decode(const float *qkv, uint32_t qkvStride, const int *po
                              float *out, uint32_t outStride, void *outBf16, int nb, cudaStream_t stream) {
     dl::AttnArgs a{};
     a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos;
-    a.kCache = (const __nv_bfloat16 *)kCache; a.vCache = (const __nv_bfloat16 *)vCache;
+    a.kCache = kCache; a.vCache = vCache;
     a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
     a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride; a.outBf16 = (__nv_bfloat16 *)outBf16;
     return dl::launchAttnDecode(a, nb, stream, false);
@@ -590,7 +623,7 @@ DL_EXPORT int dl_attn_fused(const float *qkv, const int *pos, const float *rope,
                             uint32_t nSplits, float *partial, unsigned int *counters, float *out, cudaStream_t stream) {
     dl::AttnFusedArgs a{};
     a.qkv = qkv; a.pos = pos; a.rope = rope; a.qNorm = qNorm; a.kNorm = kNorm; a.eps = eps;
-    a.kCache = (__nv_bfloat16 *)kCache; a.vCache = (__nv_bfloat16 *)vCache;
+    a.kCache = kCache; a.vCache = vCache;
     a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
     a.partial = partial; a.counters = counters; a.out = out;
     return dl::launchAttnFused(a, stream, false);
@@ -605,7 +638,7 @@ DL_EXPORT int dl_choice_attn(float *qkv, uint32_t qkvStride, const int *pos, con
     dl::RopeKvArgs r{};
     r.qkv = qkv; r.qkvStride = qkvStride; r.pos = pos; r.rope = rope; r.qNorm = qNorm; r.kNorm = kNorm; r.eps = eps;
     r.nHeads = nHeads; r.nKvHeads = nKvHeads; r.headDim = headDim; r.seqLen = seqLen;
-    r.kCache = (__nv_bfloat16 *)kCache; r.vCache = (__nv_bfloat16 *)vCache; r.rowStride = C; r.inactiveMask = inactiveMask;
+    r.kCache = kCache; r.vCache = vCache; r.rowStride = C; r.inactiveMask = inactiveMask;
     dl::ChoiceAttnArgs a{};
     a.qkv = qkv; a.qkvStride = qkvStride; a.kCache = r.kCache; a.vCache = r.vCache;
     a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
@@ -621,7 +654,7 @@ DL_EXPORT int dl_choice_attn_only(const float *qkv, uint32_t qkvStride, const vo
                                   uint32_t headDim, uint32_t seqLen, uint32_t nSplits, uint32_t B, uint32_t P, uint32_t C, uint32_t j,
                                   uint32_t inactiveMask, float *partial, unsigned int *counters, float *out, uint32_t outStride, cudaStream_t stream) {
     dl::ChoiceAttnArgs a{};
-    a.qkv = qkv; a.qkvStride = qkvStride; a.kCache = (const __nv_bfloat16 *)kCache; a.vCache = (const __nv_bfloat16 *)vCache;
+    a.qkv = qkv; a.qkvStride = qkvStride; a.kCache = kCache; a.vCache = vCache;
     a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
     a.B = B; a.P = P; a.C = C; a.j = j; a.inactiveMask = inactiveMask; a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride;
     return dl::launchChoiceAttn(a, stream, false);
@@ -633,7 +666,53 @@ DL_EXPORT int dl_slot_attn(const float *qkv, uint32_t qkvStride, const int *pos,
                            uint32_t nKvHeads, uint32_t headDim, uint32_t L, uint32_t nSplits, uint32_t B, uint32_t inactiveMask, float *partial,
                            unsigned int *counters, float *out, uint32_t outStride, cudaStream_t stream) {
     dl::SlotAttnArgs a{};
-    a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos; a.kCache = (const __nv_bfloat16 *)kCache; a.vCache = (const __nv_bfloat16 *)vCache;
+    a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos; a.kCache = kCache; a.vCache = vCache;
+    a.slotStride = (uint64_t)nKvHeads * L * headDim; a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.L = L;
+    a.nSplits = nSplits; a.B = B; a.inactiveMask = inactiveMask; a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride;
+    return dl::launchSlotAttn(a, stream, false);
+}
+
+// q80 variants of the entry points above: kCache / vCache are the int8 value planes, kScale / vScale the f16 scale planes
+// [nKvHeads][seqLen][headDim / 32] (for slots: every slot's, at element offset slot * slotStride / 32).
+DL_EXPORT int dl_attn_decode_q80(const float *qkv, uint32_t qkvStride, const int *pos, const void *kCache, const void *vCache, const void *kScale,
+                                 const void *vScale, uint32_t nHeads, uint32_t nKvHeads, uint32_t headDim, uint32_t seqLen, uint32_t nSplits,
+                                 float *partial, unsigned int *counters, float *out, uint32_t outStride, void *outBf16, int nb, cudaStream_t stream) {
+    dl::AttnArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos;
+    a.kCache = kCache; a.vCache = vCache; a.kScale = (const __half *)kScale; a.vScale = (const __half *)vScale;
+    a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
+    a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride; a.outBf16 = (__nv_bfloat16 *)outBf16;
+    return dl::launchAttnDecode(a, nb, stream, false);
+}
+
+DL_EXPORT int dl_attn_fused_q80(const float *qkv, const int *pos, const float *rope, const float *qNorm, const float *kNorm, float eps,
+                                void *kCache, void *vCache, void *kScale, void *vScale, uint32_t nHeads, uint32_t nKvHeads, uint32_t headDim,
+                                uint32_t seqLen, uint32_t nSplits, float *partial, unsigned int *counters, float *out, cudaStream_t stream) {
+    dl::AttnFusedArgs a{};
+    a.qkv = qkv; a.pos = pos; a.rope = rope; a.qNorm = qNorm; a.kNorm = kNorm; a.eps = eps;
+    a.kCache = kCache; a.vCache = vCache; a.kScale = (__half *)kScale; a.vScale = (__half *)vScale;
+    a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
+    a.partial = partial; a.counters = counters; a.out = out;
+    return dl::launchAttnFused(a, stream, false);
+}
+
+DL_EXPORT int dl_choice_attn_only_q80(const float *qkv, uint32_t qkvStride, const void *kCache, const void *vCache, const void *kScale,
+                                      const void *vScale, uint32_t nHeads, uint32_t nKvHeads, uint32_t headDim, uint32_t seqLen, uint32_t nSplits,
+                                      uint32_t B, uint32_t P, uint32_t C, uint32_t j, uint32_t inactiveMask, float *partial, unsigned int *counters,
+                                      float *out, uint32_t outStride, cudaStream_t stream) {
+    dl::ChoiceAttnArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.kCache = kCache; a.vCache = vCache; a.kScale = (const __half *)kScale; a.vScale = (const __half *)vScale;
+    a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen; a.nSplits = nSplits;
+    a.B = B; a.P = P; a.C = C; a.j = j; a.inactiveMask = inactiveMask; a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride;
+    return dl::launchChoiceAttn(a, stream, false);
+}
+
+DL_EXPORT int dl_slot_attn_q80(const float *qkv, uint32_t qkvStride, const int *pos, const void *kCache, const void *vCache, const void *kScale,
+                               const void *vScale, uint32_t nHeads, uint32_t nKvHeads, uint32_t headDim, uint32_t L, uint32_t nSplits, uint32_t B,
+                               uint32_t inactiveMask, float *partial, unsigned int *counters, float *out, uint32_t outStride, cudaStream_t stream) {
+    dl::SlotAttnArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos; a.kCache = kCache; a.vCache = vCache;
+    a.kScale = (const __half *)kScale; a.vScale = (const __half *)vScale;
     a.slotStride = (uint64_t)nKvHeads * L * headDim; a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.L = L;
     a.nSplits = nSplits; a.B = B; a.inactiveMask = inactiveMask; a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride;
     return dl::launchSlotAttn(a, stream, false);

@@ -8,6 +8,8 @@
 //   pass 1: S tiles -> per-row running maximum m and normaliser l
 //   pass 2: S tiles again -> P = exp2(S - m) as bf16 registers (the A operand of the next wgmma) -> O += P.V
 // Warp roles: 0 = TMA producer; warps 4..7 and 8..11 = two consumer warpgroups, each owning 64 query rows of the tile (wgmma M = 64).
+// A q80 cache (the Q8 variant) has no TMA path: warps 0..3 read the int8 rows and their scales, widen them to bf16 and store them in
+// the same swizzled layout the TMA would have produced; everything after the full barrier is the same kernel.
 // Each 128-position KV tile is processed as two halves of 64 positions (S half = 32 registers a thread).
 //
 // Replaces (reference): OP_MULTIHEAD_ATT over a prompt chunk, multiheadAtt_F32 + softmax_F32 per (head, batch row)
@@ -55,9 +57,32 @@ struct AttnPrefillKArgs {
     __nv_bfloat16 *out;         // [T][outStride]: token-major, head h at columns h * HD
     uint32_t outStride;
     float scaleLog2;            // log2(e) / sqrt(headDim), folded into q
+    const int8_t *kQ8, *vQ8;    // q80 cache (Q8 kernels): value planes and scale planes [nKvHeads][seqLen][HD / 32]
+    const __half *kScale, *vScale;
 };
 
+// Q8: one 128-position K or V tile of a q80 cache, widened to bf16 by the 128 threads of warps 0..3 into the SWIZZLE_128B layout
+// ([NA][128 rows][128 B], 16-byte chunk c of row r at ((c ^ (r & 7)) << 4)). Rows at or past `rowEnd` (not yet written) are zero.
 template <int HD>
+__device__ __forceinline__ void apWidenTile(uint8_t *dst, const int8_t *q, const __half *sc, uint32_t kvRow0, uint32_t pos0, uint32_t rowEnd) {
+    constexpr uint32_t CPR = HD / 8;   // 16-byte bf16 chunks per row
+    for (uint32_t u = threadIdx.x; u < 128 * CPR; u += 128) {
+        const uint32_t r = u / CPR, cc = u % CPR;
+        uint4 packed = make_uint4(0u, 0u, 0u, 0u);
+        if (pos0 + r < rowEnd) {
+            const size_t e = (size_t)(kvRow0 + pos0 + r) * HD + cc * 8;
+            const float d = __half2float(sc[e / 32]);
+            const uint2 w = *reinterpret_cast<const uint2 *>(q + e);
+            packed = make_uint4(apPack(q8ToFloat(w.x, 0) * d, q8ToFloat(w.x, 1) * d), apPack(q8ToFloat(w.x, 2) * d, q8ToFloat(w.x, 3) * d),
+                                apPack(q8ToFloat(w.y, 0) * d, q8ToFloat(w.y, 1) * d), apPack(q8ToFloat(w.y, 2) * d, q8ToFloat(w.y, 3) * d));
+        }
+        *reinterpret_cast<uint4 *>(dst + (cc >> 3) * kApAtomBytes + r * 128 + (((cc & 7) ^ (r & 7)) << 4)) = packed;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
+    __syncwarp();
+}
+
+template <int HD, bool Q8>
 __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __grid_constant__ CUtensorMap tmapK,
                                                                      const __grid_constant__ CUtensorMap tmapV, AttnPrefillKArgs a) {
     constexpr uint32_t NA = HD / 64;                    // 64-wide atom columns along headDim
@@ -82,16 +107,35 @@ __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __gri
 
     pdlLaunchDependents();
     if (tid == 0) {
+        const uint32_t fills = Q8 ? 4 : 1;   // Q8: the lane 0 of each of warps 0..3 arrives once its rows are stored
         for (int i = 0; i < 2; i++) {
-            apBarInit(&kFull[i], 1); apBarInit(&kEmpty[i], kApConsumerWarps);
-            apBarInit(&vFull[i], 1); apBarInit(&vEmpty[i], kApConsumerWarps);
+            apBarInit(&kFull[i], fills); apBarInit(&kEmpty[i], kApConsumerWarps);
+            apBarInit(&vFull[i], fills); apBarInit(&vEmpty[i], kApConsumerWarps);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
     pdlWait();   // q rows and the new K/V rows come from the rope kernel before this one
 
-    if (warp == 0) {
+    if (Q8 && warp < 4) {
+        // ================================ q80 producer: warps 0..3 ================================
+        const uint32_t rowEnd = a.p0 + a.T;   // rows [0, p0 + T) of the head are in the cache
+        uint32_t itK = 0;
+        for (uint32_t pass = 0; pass < 2; pass++) {
+            for (uint32_t j = 0; j < nKv; j++, itK++) {
+                const uint32_t st = itK & 1, ph = (itK >> 1) & 1;
+                apBarWait(&kEmpty[st], ph ^ 1);
+                apWidenTile<HD>(Ks + st * kTileBytes, a.kQ8, a.kScale, kvRow0, j * 128, rowEnd);
+                if (lane == 0) apBarArrive(&kFull[st]);
+                if (pass == 1) {
+                    const uint32_t vs = j & 1, vph = (j >> 1) & 1;
+                    apBarWait(&vEmpty[vs], vph ^ 1);
+                    apWidenTile<HD>(Vs + vs * kTileBytes, a.vQ8, a.vScale, kvRow0, j * 128, rowEnd);
+                    if (lane == 0) apBarArrive(&vFull[vs]);
+                }
+            }
+        }
+    } else if (!Q8 && warp == 0) {
         // ================================ TMA producer ================================
         if (lane == 0) {
             uint32_t itK = 0;
@@ -284,15 +328,15 @@ bool apCacheMap(CUtensorMap *map, const void *cache, uint32_t hd, uint64_t rows)
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int HD>
+template <int HD, bool Q8>
 int apLaunch(const CUtensorMap &mk, const CUtensorMap &mv, const AttnPrefillKArgs &k, uint32_t grid, cudaStream_t stream, bool pdl) {
     constexpr size_t smemBytes = (size_t)(HD / 64) * kApAtomBytes * 5 + 256 + 1024;
     static bool configured = false;
     if (!configured) {
-        DL_CUDA_CHECK(cudaFuncSetAttribute(attnPrefillTcKernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
+        DL_CUDA_CHECK(cudaFuncSetAttribute(attnPrefillTcKernel<HD, Q8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
         configured = true;
     }
-    DL_CUDA_CHECK(launchPdl(attnPrefillTcKernel<HD>, dim3(grid), dim3(kApThreads), smemBytes, stream, pdl, mk, mv, k));
+    DL_CUDA_CHECK(launchPdl(attnPrefillTcKernel<HD, Q8>, dim3(grid), dim3(kApThreads), smemBytes, stream, pdl, mk, mv, k));
     DL_CUDA_CHECK(cudaGetLastError());
     return 0;
 }
@@ -311,11 +355,17 @@ int launchAttnPrefillTc(const AttnPrefillArgs &a, cudaStream_t stream, bool pdl)
     k.kvMul = kvMul; k.tq = 128 / kvMul; k.nQTiles = (a.T + k.tq - 1) / k.tq;
     k.out = a.out; k.outStride = a.outStride;
     k.scaleLog2 = 1.4426950408889634f / sqrtf((float)a.headDim);
+    const uint32_t grid = a.nKvHeads * k.nQTiles;
+    if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
+    if (a.kScale) {   // q80: widened by the kernel itself, no tensor maps
+        CUtensorMap none{};
+        k.kQ8 = (const int8_t *)a.kCache; k.vQ8 = (const int8_t *)a.vCache; k.kScale = a.kScale; k.vScale = a.vScale;
+        return a.headDim == 128 ? apLaunch<128, true>(none, none, k, grid, stream, pdl) : apLaunch<64, true>(none, none, k, grid, stream, pdl);
+    }
     CUtensorMap mk, mv;
     const uint64_t rows = (uint64_t)a.nKvHeads * a.seqLen;
     if (!apCacheMap(&mk, a.kCache, a.headDim, rows) || !apCacheMap(&mv, a.vCache, a.headDim, rows)) return -2;
-    const uint32_t grid = a.nKvHeads * k.nQTiles;
-    return a.headDim == 128 ? apLaunch<128>(mk, mv, k, grid, stream, pdl) : apLaunch<64>(mk, mv, k, grid, stream, pdl);
+    return a.headDim == 128 ? apLaunch<128, false>(mk, mv, k, grid, stream, pdl) : apLaunch<64, false>(mk, mv, k, grid, stream, pdl);
 }
 
 }  // namespace dl
@@ -326,6 +376,17 @@ DL_EXPORT int dl_attn_prefill_tc(const float *qkv, uint32_t qkvStride, uint32_t 
                                  cudaStream_t stream) {
     dl::AttnPrefillArgs a{};
     a.qkv = qkv; a.qkvStride = qkvStride; a.T = T; a.p0 = p0; a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen;
-    a.kCache = (const __nv_bfloat16 *)kCache; a.vCache = (const __nv_bfloat16 *)vCache; a.out = (__nv_bfloat16 *)out; a.outStride = outStride;
+    a.kCache = kCache; a.vCache = vCache; a.out = (__nv_bfloat16 *)out; a.outStride = outStride;
+    return dl::launchAttnPrefillTc(a, stream);
+}
+
+// The same over a q80 cache: int8 value planes kCache / vCache, f16 scale planes kScale / vScale [nKvHeads][seqLen][headDim / 32].
+DL_EXPORT int dl_attn_prefill_tc_q80(const float *qkv, uint32_t qkvStride, uint32_t T, uint32_t p0, uint32_t nHeads, uint32_t nKvHeads,
+                                     uint32_t headDim, uint32_t seqLen, const void *kCache, const void *vCache, const void *kScale,
+                                     const void *vScale, void *out, uint32_t outStride, cudaStream_t stream) {
+    dl::AttnPrefillArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.T = T; a.p0 = p0; a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen;
+    a.kCache = kCache; a.vCache = vCache; a.kScale = (const __half *)kScale; a.vScale = (const __half *)vScale;
+    a.out = (__nv_bfloat16 *)out; a.outStride = outStride;
     return dl::launchAttnPrefillTc(a, stream);
 }

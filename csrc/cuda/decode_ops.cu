@@ -23,7 +23,9 @@ __global__ void __launch_bounds__(256) embeddingKernel(const EmbTable table, con
 }
 
 // ---- QK-norm + RoPE + KV write -------------------------------------------------------------------------
-// grid (nHeads + 2*nKvHeads, nb), block headDim/2: thread j rotates pair (2j, 2j+1)
+// grid (nHeads + 2*nKvHeads, nb), block headDim/2: thread j rotates pair (2j, 2j+1). Q8: the cache is q80 (a 32-value block is
+// the pairs of 16 neighbouring threads).
+template <bool Q8>
 __global__ void __launch_bounds__(128) ropeKvKernel(RopeKvArgs a) {
     pdlLaunchDependents();
     pdlWait();
@@ -58,11 +60,16 @@ __global__ void __launch_bounds__(128) ropeKvKernel(RopeKvArgs a) {
     const bool inactive = t < 32 && ((a.inactiveMask >> t) & 1u);
     if (isQ) {
         reinterpret_cast<float2 *>(row)[j] = v;
-    } else if (!inactive && cacheRow < a.seqLen) {
+    } else if (!inactive && cacheRow < a.seqLen) {   // (uniform over the block: every thread of the row's warps gets here)
         const uint32_t kvh = isK ? head - a.nHeads : head - a.nHeads - a.nKvHeads;
-        __nv_bfloat16 *cache = isK ? a.kCache : a.vCache;
-        __nv_bfloat162 *dst = reinterpret_cast<__nv_bfloat162 *>(cache + t * a.slotStride + ((size_t)kvh * a.seqLen + cacheRow) * hd);
-        dst[j] = __floats2bfloat162_rn(v.x, v.y);
+        const size_t e = t * a.slotStride + ((size_t)kvh * a.seqLen + cacheRow) * hd + 2 * j;
+        if constexpr (Q8) {
+            float f[2] = {v.x, v.y};
+            roundStoreKv<2, true>(f, isK ? a.kCache : a.vCache, isK ? a.kScale : a.vScale, e, true);
+        } else {
+            __nv_bfloat16 *cache = reinterpret_cast<__nv_bfloat16 *>(isK ? a.kCache : a.vCache);
+            *reinterpret_cast<__nv_bfloat162 *>(cache + e) = __floats2bfloat162_rn(v.x, v.y);
+        }
     }
 }
 
@@ -204,7 +211,10 @@ int launchEmbedding(const EmbTable &table, const int *tokens, float *x, uint32_t
 
 int launchRopeKv(const RopeKvArgs &a, int nb, cudaStream_t stream, bool pdl) {
     if (a.headDim != 64 && a.headDim != 128 && a.headDim != 256) return -1;
-    DL_CUDA_CHECK(launchPdl(ropeKvKernel, dim3(a.nHeads + 2 * a.nKvHeads, nb), dim3(a.headDim / 2), 0, stream, pdl, a));
+    if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
+    const dim3 grid(a.nHeads + 2 * a.nKvHeads, nb), block(a.headDim / 2);
+    if (a.kScale) DL_CUDA_CHECK(launchPdl(ropeKvKernel<true>, grid, block, 0, stream, pdl, a));
+    else DL_CUDA_CHECK(launchPdl(ropeKvKernel<false>, grid, block, 0, stream, pdl, a));
     return 0;
 }
 
@@ -230,7 +240,18 @@ DL_EXPORT int dl_rope_kv(float *qkv, uint32_t qkvStride, const int *pos, const f
     dl::RopeKvArgs a{};
     a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos; a.rope = rope; a.qNorm = qNorm; a.kNorm = kNorm; a.eps = eps;
     a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen;
-    a.kCache = (__nv_bfloat16 *)kCache; a.vCache = (__nv_bfloat16 *)vCache;
+    a.kCache = kCache; a.vCache = vCache;
+    return dl::launchRopeKv(a, nb, stream, false);
+}
+
+// dl_rope_kv into a q80 cache: int8 value planes kCache / vCache and f16 scale planes kScale / vScale [nKvHeads][seqLen][headDim / 32].
+DL_EXPORT int dl_rope_kv_q80(float *qkv, uint32_t qkvStride, const int *pos, const float *rope, const float *qNorm, const float *kNorm,
+                             float eps, uint32_t nHeads, uint32_t nKvHeads, uint32_t headDim, uint32_t seqLen, void *kCache, void *vCache,
+                             void *kScale, void *vScale, int nb, cudaStream_t stream) {
+    dl::RopeKvArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos; a.rope = rope; a.qNorm = qNorm; a.kNorm = kNorm; a.eps = eps;
+    a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen;
+    a.kCache = kCache; a.vCache = vCache; a.kScale = (__half *)kScale; a.vScale = (__half *)vScale;
     return dl::launchRopeKv(a, nb, stream, false);
 }
 

@@ -31,6 +31,7 @@ struct Engine {
     uint32_t traceCap = 0;
     bool traceAllCtas = false;   // persistent kernel: every CTA records its phase stamps (skew analysis, tools/trace_mega.py --all)
     MegaLayer *megaLayers = nullptr;   // device copy of the per-layer pointer table for the persistent decode kernel
+    MegaKvScales *megaKvScales = nullptr;   // q80 caches: device copy of the per-layer scale planes (null: bf16)
     unsigned int *megaCounter = nullptr;
     uint2 *megaX2 = nullptr;
     uint32_t megaFlags = 0;            // DL_MEGA_FLAGS (bit 0: barrier-free LL hand-off)
@@ -182,6 +183,7 @@ static int engineDecodeMega(Engine &e, bool greedyAdvance, cudaStream_t stream) 
     m.argVal = e.g.argVal; m.argIdx = e.g.argIdx; m.argCounter = e.g.argCounter; m.gridCounter = e.megaCounter;
     m.rowOffsetGlobal = c.rank * c.vocab; m.greedyAdvance = greedyAdvance ? 1u : 0u; m.vocabLimit = e.vocabLimit;
     m.trace = e.trace;
+    m.kvScales = e.megaKvScales;
     m.traceCtas = e.traceAllCtas ? c.numSms : 1u;
     m.traceStride = e.traceAllCtas ? (uint32_t)(((size_t)e.traceCap * 4) / c.numSms) : 0u;
     m.traceProdSlot = (e.trace && m.traceStride >= megaTraceRowSlots(c.nLayers)) ? megaTraceProdSlot(c.nLayers) : 0u;
@@ -197,6 +199,13 @@ struct SlotStep { uint32_t inactiveMask; };
 
 static uint64_t slotElems(const Engine &e) { return (uint64_t)e.cfg.nKvHeads * e.slotLen * e.cfg.headDim; }
 
+// The layer's K/V caches from element cacheOff on, in the engine's storage (bf16, or q80 value and scale planes).
+struct KvPtrs { void *k, *v; __half *ks, *vs; };
+static KvPtrs layerKv(const Engine &e, const LayerPtrs &L, uint64_t cacheOff) {
+    if (e.cfg.kvType == 0) return {(__nv_bfloat16 *)L.kCache + cacheOff, (__nv_bfloat16 *)L.vCache + cacheOff, nullptr, nullptr};
+    return {(int8_t *)L.kCache + cacheOff, (int8_t *)L.vCache + cacheOff, (__half *)L.kScale + cacheOff / 32, (__half *)L.vScale + cacheOff / 32};
+}
+
 // QK-norm + RoPE + K/V write of layer L over the q|k|v rows `qkv` at positions `pos`, into the cache that starts cacheOff elements
 // into the layer's K/V and holds seqLen rows per KV head. rowStride, slotStride and inactiveMask are left 0 for the caller to set.
 static RopeKvArgs layerRopeKv(const Engine &e, const LayerPtrs &L, float *qkv, const int *pos, uint64_t cacheOff, uint32_t seqLen) {
@@ -204,7 +213,8 @@ static RopeKvArgs layerRopeKv(const Engine &e, const LayerPtrs &L, float *qkv, c
     RopeKvArgs r{};
     r.qkv = qkv; r.qkvStride = (c.nHeads + 2 * c.nKvHeads) * c.headDim; r.pos = pos; r.rope = e.g.rope; r.qNorm = L.qNorm; r.kNorm = L.kNorm;
     r.eps = c.eps; r.nHeads = c.nHeads; r.nKvHeads = c.nKvHeads; r.headDim = c.headDim; r.seqLen = seqLen;
-    r.kCache = (__nv_bfloat16 *)L.kCache + cacheOff; r.vCache = (__nv_bfloat16 *)L.vCache + cacheOff;
+    const KvPtrs kv = layerKv(e, L, cacheOff);
+    r.kCache = kv.k; r.vCache = kv.v; r.kScale = kv.ks; r.vScale = kv.vs;
     return r;
 }
 
@@ -244,7 +254,7 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
             r.slotStride = slotElems(e); r.inactiveMask = sl->inactiveMask;
             DL_TRY(launchRopeKv(r, nb, stream, pdl));
             SlotAttnArgs t{};
-            t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache; t.slotStride = r.slotStride;
+            t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache; t.kScale = r.kScale; t.vScale = r.vScale; t.slotStride = r.slotStride;
             t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.L = e.slotLen; t.nSplits = c.nSplits;
             t.B = (uint32_t)nb; t.inactiveMask = sl->inactiveMask;
             t.partial = e.g.attnPartial; t.counters = e.g.attnCounters; t.out = e.g.z; t.outStride = qDim;
@@ -255,7 +265,7 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
             r.rowStride = ch->C; r.inactiveMask = ch->inactiveMask;
             DL_TRY(launchRopeKv(r, nb, stream, pdl));
             ChoiceAttnArgs t{};
-            t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.kCache = r.kCache; t.vCache = r.vCache;
+            t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.kCache = r.kCache; t.vCache = r.vCache; t.kScale = r.kScale; t.vScale = r.vScale;
             t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.seqLen = c.seqLen; t.nSplits = c.nSplits;
             t.B = (uint32_t)nb; t.P = ch->P; t.C = ch->C; t.j = ch->j; t.inactiveMask = ch->inactiveMask;
             t.partial = e.g.attnPartial; t.counters = e.g.attnCounters; t.out = e.g.z; t.outStride = qDim;
@@ -264,7 +274,8 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
             // 2+3. qk-norm + rope + kv append + attention in one launch
             AttnFusedArgs f{};
             f.qkv = e.g.qkv; f.pos = e.g.pos; f.rope = e.g.rope; f.qNorm = L.qNorm; f.kNorm = L.kNorm; f.eps = c.eps;
-            f.kCache = (__nv_bfloat16 *)L.kCache; f.vCache = (__nv_bfloat16 *)L.vCache;
+            const KvPtrs kv = layerKv(e, L, 0);
+            f.kCache = kv.k; f.vCache = kv.v; f.kScale = kv.ks; f.vScale = kv.vs;
             f.nHeads = c.nHeads; f.nKvHeads = c.nKvHeads; f.headDim = c.headDim; f.seqLen = c.seqLen; f.nSplits = c.nSplits;
             f.partial = e.g.attnPartial; f.counters = e.g.attnCounters; f.out = e.g.z; f.trace = nextTrace();
             DL_TRY(launchAttnFused(f, stream, pdl));
@@ -274,7 +285,7 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
             DL_TRY(launchRopeKv(r, nb, stream, pdl));
             // 3. attention
             AttnArgs t{};
-            t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache;
+            t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache; t.kScale = r.kScale; t.vScale = r.vScale;
             t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.seqLen = c.seqLen; t.nSplits = c.nSplits;
             t.partial = e.g.attnPartial; t.counters = e.g.attnCounters; t.out = e.g.z; t.outStride = qDim;
             DL_TRY(launchAttnDecode(t, nb, stream, pdl));
@@ -376,14 +387,14 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
             // tensor-core attention over the whole chunk: the tokens of a chunk sit at consecutive positions p0 .. p0 + T - 1
             AttnPrefillArgs ap{};
             ap.qkv = g.pqkv; ap.qkvStride = qkvDim; ap.T = T; ap.p0 = p0; ap.nHeads = c.nHeads; ap.nKvHeads = c.nKvHeads;
-            ap.headDim = c.headDim; ap.seqLen = seqLen; ap.kCache = r.kCache; ap.vCache = r.vCache;
+            ap.headDim = c.headDim; ap.seqLen = seqLen; ap.kCache = r.kCache; ap.vCache = r.vCache; ap.kScale = r.kScale; ap.vScale = r.vScale;
             ap.out = (__nv_bfloat16 *)g.pzb; ap.outStride = qDim;
             attnRc = launchAttnPrefillTc(ap, stream, pdl);
             if (attnRc < 0) return attnRc;
         }
         if (attnRc == 1) {
             AttnArgs t{};
-            t.qkv = g.pqkv; t.qkvStride = qkvDim; t.pos = g.pPos; t.kCache = r.kCache; t.vCache = r.vCache;
+            t.qkv = g.pqkv; t.qkvStride = qkvDim; t.pos = g.pPos; t.kCache = r.kCache; t.vCache = r.vCache; t.kScale = r.kScale; t.vScale = r.vScale;
             t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.seqLen = seqLen; t.nSplits = 1;
             t.partial = g.pAttnPartial; t.counters = g.pAttnCounters; t.out = nullptr; t.outStride = qDim; t.outBf16 = (__nv_bfloat16 *)g.pzb;
             DL_TRY(launchAttnDecode(t, (int)T, stream, pdl));
@@ -434,6 +445,7 @@ using dl::Engine;
 constexpr uint32_t kChoiceRngSlots = 8;
 
 DL_EXPORT void *dl_engine_create(const dl::EngineConfig *cfg) {
+    if (cfg->kvType > 1 || (cfg->kvType == 1 && cfg->headDim % 32)) return nullptr;   // unknown KV-cache storage
     Engine *e = new Engine();
     e->cfg = *cfg;
     dl::gHiddenAct = cfg->hiddenAct;
@@ -458,6 +470,7 @@ DL_EXPORT void dl_engine_destroy(void *h) {
     if (e->decodeGraph) cudaGraphExecDestroy(e->decodeGraph);
     if (e->captureStream) cudaStreamDestroy(e->captureStream);
     if (e->megaLayers) cudaFree(e->megaLayers);
+    if (e->megaKvScales) cudaFree(e->megaKvScales);
     if (e->megaCounter) cudaFree(e->megaCounter);
     for (void *q : {(void *)e->megaX, (void *)e->megaX2, (void *)e->megaQkv, (void *)e->megaZ, (void *)e->megaH, (void *)e->megaSeq}) if (q) cudaFree(q);
     if (e->abortHost) cudaFreeHost(e->abortHost);
@@ -493,10 +506,16 @@ DL_EXPORT int dl_engine_enable_mega(void *h, int enable) {
             m.qkvQs = (const uint8_t *)L.qkvQs; m.qkvSc = (const uint8_t *)L.qkvSc; m.woQs = (const uint8_t *)L.woQs; m.woSc = (const uint8_t *)L.woSc;
             m.w13Qs = (const uint8_t *)L.w13Qs; m.w13Sc = (const uint8_t *)L.w13Sc; m.w2Qs = (const uint8_t *)L.w2Qs; m.w2Sc = (const uint8_t *)L.w2Sc;
             m.norm0 = L.norm0; m.norm1 = L.norm1; m.qNorm = L.qNorm; m.kNorm = L.kNorm;
-            m.kCache = (__nv_bfloat16 *)L.kCache; m.vCache = (__nv_bfloat16 *)L.vCache;
+            m.kCache = L.kCache; m.vCache = L.vCache;
         }
         DL_CUDA_CHECK(cudaMalloc(&e->megaLayers, tab.size() * sizeof(dl::MegaLayer)));
         DL_CUDA_CHECK(cudaMemcpy(e->megaLayers, tab.data(), tab.size() * sizeof(dl::MegaLayer), cudaMemcpyHostToDevice));
+        if (e->cfg.kvType != 0) {
+            std::vector<dl::MegaKvScales> sc(e->layers.size());
+            for (size_t l = 0; l < sc.size(); l++) sc[l] = {(__half *)e->layers[l].kScale, (__half *)e->layers[l].vScale};
+            DL_CUDA_CHECK(cudaMalloc(&e->megaKvScales, sc.size() * sizeof(dl::MegaKvScales)));
+            DL_CUDA_CHECK(cudaMemcpy(e->megaKvScales, sc.data(), sc.size() * sizeof(dl::MegaKvScales), cudaMemcpyHostToDevice));
+        }
         DL_CUDA_CHECK(cudaMalloc(&e->megaCounter, 256));
         DL_CUDA_CHECK(cudaMemset(e->megaCounter, 0, 256));
         const dl::EngineConfig &c = e->cfg;
@@ -775,7 +794,7 @@ DL_EXPORT int dl_engine_forward_part(void *h, int nb, uint32_t layer, int part, 
         const dl::RopeKvArgs r = dl::layerRopeKv(e, L, e.g.qkv, e.g.pos, 0, c.seqLen);
         DL_TRY(dl::launchRopeKv(r, nb, stream, false));
         dl::AttnArgs t{};
-        t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache;
+        t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache; t.kScale = r.kScale; t.vScale = r.vScale;
         t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.seqLen = c.seqLen; t.nSplits = c.nSplits;
         t.partial = e.g.attnPartial; t.counters = e.g.attnCounters; t.out = e.g.z; t.outStride = qDim;
         DL_TRY(dl::launchAttnDecode(t, nb, stream, false));
@@ -902,12 +921,16 @@ DL_EXPORT int dl_engine_slot_copy(void *h, uint32_t src, uint32_t dst, uint32_t 
     const dl::EngineConfig &c = e->cfg;
     if (e->slots < 2 || src >= e->slots || dst >= e->slots || P > e->slotLen) return -64;
     if (src == dst || P == 0) return 0;
-    const size_t rowBytes = (size_t)c.headDim * sizeof(__nv_bfloat16), pitch = (size_t)e->slotLen * rowBytes;
-    const size_t slotBytes = (size_t)c.nKvHeads * pitch;
+    // bf16: one plane per cache; q80: the int8 values (headDim bytes a row) and the scales (headDim / 16 bytes a row)
+    const bool q8 = c.kvType != 0;
+    const size_t rowBytes[2] = {(size_t)c.headDim * (q8 ? 1 : sizeof(__nv_bfloat16)), (size_t)c.headDim / 16};
     for (const dl::LayerPtrs &L : e->layers)
-        for (void *cache : {L.kCache, L.vCache})
-            DL_CUDA_CHECK(cudaMemcpy2DAsync((uint8_t *)cache + dst * slotBytes, pitch, (const uint8_t *)cache + src * slotBytes, pitch,
-                                            (size_t)P * rowBytes, c.nKvHeads, cudaMemcpyDeviceToDevice, stream));
+        for (int plane = 0; plane < (q8 ? 2 : 1); plane++) {
+            const size_t pitch = (size_t)e->slotLen * rowBytes[plane], slotBytes = (size_t)c.nKvHeads * pitch;
+            for (void *cache : {plane ? L.kScale : L.kCache, plane ? L.vScale : L.vCache})
+                DL_CUDA_CHECK(cudaMemcpy2DAsync((uint8_t *)cache + dst * slotBytes, pitch, (const uint8_t *)cache + src * slotBytes, pitch,
+                                                (size_t)P * rowBytes[plane], c.nKvHeads, cudaMemcpyDeviceToDevice, stream));
+        }
     return 0;
 }
 

@@ -20,6 +20,7 @@ struct EngineConfig {   // mirrored by ctypes in distributed_llama_b200/ops/cuda
     uint32_t moeFirstExpert, moeNumLocal;   // experts held by this rank (expert parallelism); TP mode: 0, nExperts
     uint32_t wType;          // matrix storage: 0 = q40 device layout, 1 = dense f32, 2 = dense f16 (gemv_dense.cu)
     uint32_t hiddenAct;      // gate activation: 0 = SiLU, 1 = GELU (tanh form) — the `.m` header's hidden_act
+    uint32_t kvType;         // KV-cache storage: 0 = bf16, 1 = q80 (int8 values + f16 scale per 32, LayerPtrs::kScale / vScale)
 };
 
 struct LayerPtrs {
@@ -29,7 +30,8 @@ struct LayerPtrs {
     const void *w2Qs, *w2Sc;     // [dim][ff];                          MoE: [nExperts][dim][ff]
     const float *norm0, *norm1, *qNorm, *kNorm;
     const float *moeGate;        // [nExperts][dim] f32
-    void *kCache, *vCache;       // bf16 [nKvHeads][seqLen][hd]
+    void *kCache, *vCache;       // bf16 [nKvHeads][seqLen][hd]; kvType 1: int8 [nKvHeads][seqLen][hd]
+    void *kScale, *vScale;       // kvType 1: f16 [nKvHeads][seqLen][hd / 32] + 16 bytes of tail padding; unused for bf16
 };
 
 struct GlobalPtrs {

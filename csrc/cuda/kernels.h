@@ -70,6 +70,95 @@ inline int gemvQ40Auto(int pro, int epi, int nb, const GemvArgs &a, int numSms, 
 // f32 / f16 weight files (gemv_dense.cu): wtype 1 = f32, 2 = f16; a.qs is the row-major [d][n] matrix
 int gemvDense(int wtype, int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t stream, bool pdl);
 
+// ---- KV-cache storage --------------------------------------------------------------------------------------------------------------
+// Every cache below is head-major [nKvHeads][seqLen][headDim]. Its rows are bf16 (kScale / vScale null), or q80 (EngineConfig::kvType
+// 1): int8 values in the value plane (kCache / vCache) and one f16 scale per 32 values in a separate scale plane
+// [nKvHeads][seqLen][headDim / 32], so value rows stay 16-byte aligned for bulk copies. A row is rounded once, where it is written,
+// with the GEMV q80 prologue's arithmetic: d = amax / 127, q = rint(x / d), scale f16(d); readers see q * f16(d).
+// Element offsets apply to both planes: value element e has its scale at e / 32.
+
+// Rounds the DPL consecutive values a lane holds of one row (a 32-value block spans 32 / DPL neighbouring lanes) to q80 in place:
+// v becomes q * f16(d). All 32 lanes of the warp take part.
+template <int DPL>
+__device__ __forceinline__ void q80RoundLane(float (&v)[DPL], int8_t (&q)[DPL], __half &d16) {
+    float amax = 0.f;
+#pragma unroll
+    for (int i = 0; i < DPL; i++) amax = fmaxf(amax, fabsf(v[i]));
+#pragma unroll
+    for (int o = 1; o < 32 / DPL; o <<= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    const float d = amax / 127.f;
+    const float id = d != 0.f ? 1.f / d : 0.f;
+    d16 = __float2half_rn(d);
+    const float dq = __half2float(d16);
+#pragma unroll
+    for (int i = 0; i < DPL; i++) {
+        const int qi = __float2int_rn(v[i] * id);
+        q[i] = (int8_t)qi;
+        v[i] = (float)qi * dq;
+    }
+}
+
+// int8 value i (0..3) of the packed word w as f32, exactly. An int-to-float conversion (I2F) runs at a fraction of the FP32 rate
+// on sm_90, and the decode kernels convert every cached value once per q-head: instead the biased byte (x + 128) goes into the
+// low mantissa byte of 2^23 (one PRMT) and one FADD removes 2^23 + 128.
+__device__ __forceinline__ float q8ToFloat(uint32_t w, int i) {
+    return __uint_as_float(__byte_perm(w ^ 0x80808080u, 0x4B000000u, 0x7650u | (uint32_t)i)) - 8388736.f;
+}
+
+// The DPL values of one cache row at element offset e (DPL in {2, 4}, e a multiple of DPL) as f32.
+template <int DPL, bool Q8>
+__device__ __forceinline__ void loadKv(const void *plane, const __half *scale, size_t e, float (&o)[DPL]) {
+    if constexpr (Q8) {
+        const float d = __half2float(scale[e / 32]);
+        const int8_t *p = reinterpret_cast<const int8_t *>(plane) + e;
+        const uint32_t w = DPL == 4 ? *reinterpret_cast<const uint32_t *>(p) : (uint32_t)*reinterpret_cast<const uint16_t *>(p);
+#pragma unroll
+        for (int i = 0; i < DPL; i++) o[i] = q8ToFloat(w, i) * d;
+    } else {
+        const __nv_bfloat16 *p = reinterpret_cast<const __nv_bfloat16 *>(plane) + e;
+        if constexpr (DPL == 4) {
+            const uint2 r = *reinterpret_cast<const uint2 *>(p);
+            const float2 a0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&r.x));
+            const float2 a1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&r.y));
+            o[0] = a0.x; o[1] = a0.y; o[2] = a1.x; o[3] = a1.y;
+        } else {
+            const uint32_t r = *reinterpret_cast<const uint32_t *>(p);
+            const float2 a0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162 *>(&r));
+            o[0] = a0.x; o[1] = a0.y;
+        }
+    }
+}
+
+// Rounds the DPL values a lane holds of a new row to the cache's storage in place (all 32 lanes take part) and, if `store`, writes
+// them at element offset e. For bf16 every lane rounds its own values; for q80 the lane that holds the start of a block writes its scale.
+template <int DPL, bool Q8>
+__device__ __forceinline__ void roundStoreKv(float (&v)[DPL], void *plane, __half *scale, size_t e, bool store) {
+    if constexpr (Q8) {
+        int8_t q[DPL];
+        __half d16;
+        q80RoundLane<DPL>(v, q, d16);
+        if (store) {
+            int8_t *p = reinterpret_cast<int8_t *>(plane) + e;
+            if constexpr (DPL == 4) *reinterpret_cast<char4 *>(p) = make_char4(q[0], q[1], q[2], q[3]);
+            else *reinterpret_cast<char2 *>(p) = make_char2(q[0], q[1]);
+            if (e % 32 == 0) scale[e / 32] = d16;
+        }
+    } else {
+        __nv_bfloat162 b[DPL / 2];
+#pragma unroll
+        for (int k = 0; k < DPL / 2; k++) {
+            b[k] = __floats2bfloat162_rn(v[2 * k], v[2 * k + 1]);
+            const float2 f = __bfloat1622float2(b[k]);
+            v[2 * k] = f.x; v[2 * k + 1] = f.y;
+        }
+        if (store) {
+            __nv_bfloat162 *p = reinterpret_cast<__nv_bfloat162 *>(reinterpret_cast<__nv_bfloat16 *>(plane) + e);
+#pragma unroll
+            for (int k = 0; k < DPL / 2; k++) p[k] = b[k];
+        }
+    }
+}
+
 struct RopeKvArgs {
     float *qkv;
     uint32_t qkvStride;
@@ -79,8 +168,8 @@ struct RopeKvArgs {
     const float *kNorm;
     float eps;
     uint32_t nHeads, nKvHeads, headDim, seqLen;
-    __nv_bfloat16 *kCache;
-    __nv_bfloat16 *vCache;
+    void *kCache, *vCache;       // bf16, or the int8 value planes of a q80 cache
+    __half *kScale, *vScale;     // q80 scale planes; null: bf16 cache
     // Choice steps (several sequences at one rotary position): token t stores its K/V row at pos[t] + t * rowStride, and tokens
     // whose bit is set in inactiveMask store nothing. Both 0 for a plain batch of consecutive tokens.
     uint32_t rowStride, inactiveMask;
@@ -97,7 +186,8 @@ int launchRopeKv(const RopeKvArgs &a, int nb, cudaStream_t stream, bool pdl);
 struct ChoiceAttnArgs {
     const float *qkv;
     uint32_t qkvStride;
-    const __nv_bfloat16 *kCache, *vCache;
+    const void *kCache, *vCache;
+    const __half *kScale, *vScale;   // q80 scale planes; null: bf16 cache
     uint32_t nHeads, nKvHeads, headDim, seqLen, nSplits;
     uint32_t B, P, C, j;
     uint32_t inactiveMask;   // rows whose bit is set skip their suffix; their output is not meaningful
@@ -115,7 +205,8 @@ struct SlotAttnArgs {
     const float *qkv;
     uint32_t qkvStride;
     const int *pos;          // [B]
-    const __nv_bfloat16 *kCache, *vCache;
+    const void *kCache, *vCache;
+    const __half *kScale, *vScale;   // q80 scale planes; null: bf16 cache
     uint64_t slotStride;     // elements between slots: nKvHeads * L * headDim
     uint32_t nHeads, nKvHeads, headDim, L, nSplits;
     uint32_t B, inactiveMask;   // rows whose bit is set do nothing; their output is not meaningful
@@ -130,7 +221,8 @@ struct AttnArgs {
     const float *qkv;
     uint32_t qkvStride;
     const int *pos;
-    const __nv_bfloat16 *kCache, *vCache;
+    const void *kCache, *vCache;
+    const __half *kScale, *vScale;   // q80 scale planes; null: bf16 cache
     uint32_t nHeads, nKvHeads, headDim, seqLen, nSplits;
     float *partial;
     unsigned int *counters;
@@ -146,7 +238,8 @@ struct AttnPrefillArgs {
     uint32_t qkvStride;
     uint32_t T, p0;
     uint32_t nHeads, nKvHeads, headDim, seqLen;
-    const __nv_bfloat16 *kCache, *vCache;   // [nKvHeads][seqLen][headDim]
+    const void *kCache, *vCache;            // [nKvHeads][seqLen][headDim]
+    const __half *kScale, *vScale;          // q80 scale planes; null: bf16 cache
     __nv_bfloat16 *out;          // [T][outStride], head h at columns h * headDim
     uint32_t outStride;
 };
@@ -159,7 +252,8 @@ struct AttnFusedArgs {
     const float *rope;       // [seqLen][hd/2][2]
     const float *qNorm, *kNorm;
     float eps;
-    __nv_bfloat16 *kCache, *vCache;
+    void *kCache, *vCache;
+    __half *kScale, *vScale;   // q80 scale planes; null: bf16 cache
     uint32_t nHeads, nKvHeads, headDim, seqLen, nSplits;
     float *partial;
     unsigned int *counters;
@@ -227,7 +321,11 @@ int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, u
 struct MegaLayer {
     const uint8_t *qkvQs, *qkvSc, *woQs, *woSc, *w13Qs, *w13Sc, *w2Qs, *w2Sc;
     const float *norm0, *norm1, *qNorm, *kNorm;
-    __nv_bfloat16 *kCache, *vCache;
+    void *kCache, *vCache;     // bf16, or the int8 value planes of a q80 cache (MegaArgs::kvScales)
+};
+
+struct MegaKvScales {          // q80 caches: the scale planes of one layer
+    __half *k, *v;
 };
 
 struct MegaPhase {   // host-computed geometry of one GEMV phase (QKV, WO, W1|W3, W2, logits)
@@ -269,6 +367,7 @@ struct MegaArgs {
     uint32_t traceCtas, traceStride;   // CTAs 0..traceCtas-1 record their phase stamps at trace[cta * traceStride + slot]
     uint32_t traceProdSlot;      // != 0: first producer slot of a CTA's trace row (megaTraceProdSlot; all-CTA tracing only)
     ArArgs ar;
+    const MegaKvScales *kvScales;   // [nLayers] in global memory: the caches are q80; null: bf16
 };
 
 // Trace row of one CTA of the persistent kernel: 18 * nLayers + 5 consumer phase stamps, then (from this slot on, 8-aligned) two

@@ -189,6 +189,14 @@ struct FillCursor {
 // the K/V fills of this CTA from the same rule as the consumers, so both must come from here.
 constexpr uint32_t kKvChunk = kConsumerWarps * 4;   // cached K/V rows per ring fill: warp w takes rows 4w..4w+3
 constexpr uint32_t kKvInflight = 2;                  // producer pacing of the K/V fills (the weight fills: MegaArgs::maxInflight)
+
+// A q80 K/V fill (MegaArgs::kvScales set): the int8 K rows at stage offset 0, the V rows kKvChunk * HD bytes further, then the K and the V scale rows
+// (HD / 16 bytes a row) in two regions of kvScRegion(HD) bytes. A bulk copy moves multiples of 16 bytes from 16-byte aligned
+// addresses, so a fill copies the aligned span around its scale rows (the cache's scale planes carry 16 bytes of tail padding) and
+// the consumers skip the leading kvScSkip bytes.
+__host__ __device__ constexpr uint32_t kvScRegion(uint32_t hd) { return kKvChunk * hd / 16 + 16; }
+__device__ __forceinline__ uint32_t kvScSkip(const void *firstRow) { return (uint32_t)(reinterpret_cast<uintptr_t>(firstRow) & 15u); }
+
 // Effective split count: grows with the position (read on the device, so a replayed graph follows it), capped at nSplits.
 __device__ __forceinline__ uint32_t attnSplits(const MegaArgs &m, uint32_t nPos) {
     uint32_t eff = (nPos + 255) / 256;
@@ -524,7 +532,7 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
 // kKvChunk rows per fill (the producer issues them between this layer's QKV and WO fills), warp w takes rows 4w..4w+3 of each.
 // The q|k|v words are polled by warp 0 alone, and q is handed to the other warps through shared memory: this phase follows the
 // QKV epilogue without a grid barrier, so the poll covers the other CTAs' arrival skew.
-template <int HD>
+template <int HD, bool Q8>
 __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaLayer &L, int p, int tid, uint32_t inEpoch, uint32_t outEpoch,
                              RingPos &ring) {
     constexpr int DPL = HD / 32;
@@ -561,8 +569,13 @@ __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaL
         const AttnItem it(m, item, nPos, eff);
         const uint32_t h = it.h, split = it.split, kvh = it.kvh, cachedEnd = it.cachedEnd;
         const bool ownsNew = it.ownsNew;
-        __nv_bfloat16 *kHead = L.kCache + (size_t)kvh * m.seqLen * HD;
-        __nv_bfloat16 *vHead = L.vCache + (size_t)kvh * m.seqLen * HD;
+        // (the bf16 path keeps its own pointer arithmetic: same code as before the q80 variant)
+        using KvT = typename std::conditional<Q8, int8_t, __nv_bfloat16>::type;
+        KvT *kHead = reinterpret_cast<KvT *>(L.kCache) + (size_t)kvh * m.seqLen * HD;
+        KvT *vHead = reinterpret_cast<KvT *>(L.vCache) + (size_t)kvh * m.seqLen * HD;
+        const MegaKvScales *lsc = Q8 ? m.kvScales + (&L - m.layers) : nullptr;
+        __half *kSc = Q8 ? lsc->k + (size_t)kvh * m.seqLen * (HD / 32) : nullptr;
+        __half *vSc = Q8 ? lsc->v + (size_t)kvh * m.seqLen * (HD / 32) : nullptr;
         constexpr int UN = 4;
         static_assert(kConsumerWarps * UN == kKvChunk, "one ring fill of K/V rows = one batch of the 16 warps");
         using RawT = typename std::conditional<DPL == 4, uint2, uint32_t>::type;   // DPL bf16 values of one cache row
@@ -624,20 +637,26 @@ __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaL
         for (int i = 0; i < DPL; i++) acc[i] = 0.f;
         if (newRow) {
             normRope(kn, L.kNorm);
-            __nv_bfloat162 kb[DPL / 2], vb[DPL / 2];
+            if constexpr (Q8) {
+                const size_t e = (size_t)p * HD + lane * DPL;
+                roundStoreKv<DPL, true>(kn, kHead, kSc, e, h % kvMul == 0);
+                roundStoreKv<DPL, true>(vn, vHead, vSc, e, h % kvMul == 0);
+            } else {
+                __nv_bfloat162 kb[DPL / 2], vb[DPL / 2];
 #pragma unroll
-            for (int k = 0; k < DPL / 2; k++) {
-                kb[k] = __floats2bfloat162_rn(kn[2 * k], kn[2 * k + 1]);
-                vb[k] = __floats2bfloat162_rn(vn[2 * k], vn[2 * k + 1]);
-                const float2 kf = __bfloat1622float2(kb[k]), vf = __bfloat1622float2(vb[k]);
-                kn[2 * k] = kf.x; kn[2 * k + 1] = kf.y;
-                vn[2 * k] = vf.x; vn[2 * k + 1] = vf.y;
-            }
-            if (h % kvMul == 0) {
-                __nv_bfloat162 *kd = reinterpret_cast<__nv_bfloat162 *>(kHead + (size_t)p * HD + lane * DPL);
-                __nv_bfloat162 *vd = reinterpret_cast<__nv_bfloat162 *>(vHead + (size_t)p * HD + lane * DPL);
+                for (int k = 0; k < DPL / 2; k++) {
+                    kb[k] = __floats2bfloat162_rn(kn[2 * k], kn[2 * k + 1]);
+                    vb[k] = __floats2bfloat162_rn(vn[2 * k], vn[2 * k + 1]);
+                    const float2 kf = __bfloat1622float2(kb[k]), vf = __bfloat1622float2(vb[k]);
+                    kn[2 * k] = kf.x; kn[2 * k + 1] = kf.y;
+                    vn[2 * k] = vf.x; vn[2 * k + 1] = vf.y;
+                }
+                if (h % kvMul == 0) {
+                    __nv_bfloat162 *kd = reinterpret_cast<__nv_bfloat162 *>(kHead + (size_t)p * HD + lane * DPL);
+                    __nv_bfloat162 *vd = reinterpret_cast<__nv_bfloat162 *>(vHead + (size_t)p * HD + lane * DPL);
 #pragma unroll
-                for (int k = 0; k < DPL / 2; k++) { kd[k] = kb[k]; vd[k] = vb[k]; }
+                    for (int k = 0; k < DPL / 2; k++) { kd[k] = kb[k]; vd[k] = vb[k]; }
+                }
             }
             float dsum = 0.f;
 #pragma unroll
@@ -650,19 +669,38 @@ __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaL
         // one ring fill per kKvChunk cached rows: K rows at the start of the stage, V rows kKvChunk rows further
         for (uint32_t c0 = it.begin; c0 < cachedEnd; c0 += kKvChunk) {
             const uint32_t st = ring.st;
-            const __nv_bfloat16 *sK = reinterpret_cast<const __nv_bfloat16 *>(sm.ring + st * m.stageBytes) + warp * UN * HD + lane * DPL;
+            const uint8_t *stage = sm.ring + st * m.stageBytes;
+            const __nv_bfloat16 *sK = reinterpret_cast<const __nv_bfloat16 *>(stage) + warp * UN * HD + lane * DPL;
             const __nv_bfloat16 *sV = sK + kKvChunk * HD;
             const uint32_t cur = c0 + warp * UN;
             mbarWait(&sm.fullBar[st], ring.par);
             float kf[UN][DPL], vf[UN][DPL];
+            if constexpr (Q8) {
+                // the rows and their scales as the producer placed them (see kvScRegion)
+                const int8_t *sK8 = reinterpret_cast<const int8_t *>(stage);
+                const __half *sKs = reinterpret_cast<const __half *>(stage + 2 * kKvChunk * HD + kvScSkip(kSc + (size_t)c0 * (HD / 32)));
+                const __half *sVs = reinterpret_cast<const __half *>(stage + 2 * kKvChunk * HD + kvScRegion(HD) + kvScSkip(vSc + (size_t)c0 * (HD / 32)));
+                const size_t e0 = (size_t)warp * UN * HD + lane * DPL;
 #pragma unroll
-            for (int u = 0; u < UN; u++) {
-                if (cur + u < cachedEnd) {
-                    unpack(*reinterpret_cast<const RawT *>(sK + u * HD), kf[u]);
-                    unpack(*reinterpret_cast<const RawT *>(sV + u * HD), vf[u]);
-                } else {
+                for (int u = 0; u < UN; u++) {
+                    if (cur + u < cachedEnd) {
+                        loadKv<DPL, true>(sK8, sKs, e0 + u * HD, kf[u]);
+                        loadKv<DPL, true>(sK8 + kKvChunk * HD, sVs, e0 + u * HD, vf[u]);
+                    } else {
 #pragma unroll
-                    for (int i = 0; i < DPL; i++) { kf[u][i] = 0.f; vf[u][i] = 0.f; }
+                        for (int i = 0; i < DPL; i++) { kf[u][i] = 0.f; vf[u][i] = 0.f; }
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int u = 0; u < UN; u++) {
+                    if (cur + u < cachedEnd) {
+                        unpack(*reinterpret_cast<const RawT *>(sK + u * HD), kf[u]);
+                        unpack(*reinterpret_cast<const RawT *>(sV + u * HD), vf[u]);
+                    } else {
+#pragma unroll
+                        for (int i = 0; i < DPL; i++) { kf[u][i] = 0.f; vf[u][i] = 0.f; }
+                    }
                 }
             }
             __syncwarp();
@@ -740,7 +778,7 @@ __device__ void megaAttention(const MegaArgs &m, const MegaSmem &sm, const MegaL
     }
 }
 
-template <int HD>
+template <int HD, bool Q8>
 __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_constant__ MegaArgs m) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -837,14 +875,32 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
                 const MegaLayer &L = m.layers[l];
                 for (uint32_t item = blockIdx.x; item < m.nHeads * eff; item += gridDim.x) {
                     const AttnItem it(m, item, nPos, eff);
-                    const __nv_bfloat16 *kHead = L.kCache + (size_t)it.kvh * m.seqLen * HD;
-                    const __nv_bfloat16 *vHead = L.vCache + (size_t)it.kvh * m.seqLen * HD;
+                    using KvT = typename std::conditional<Q8, int8_t, __nv_bfloat16>::type;
+                    const KvT *kHead = reinterpret_cast<const KvT *>(L.kCache) + (size_t)it.kvh * m.seqLen * HD;
+                    const KvT *vHead = reinterpret_cast<const KvT *>(L.vCache) + (size_t)it.kvh * m.seqLen * HD;
                     for (uint32_t c0 = it.begin; c0 < it.cachedEnd; c0 += kKvChunk) {
-                        const uint32_t bytes = min(kKvChunk, it.cachedEnd - c0) * HD * 2;
-                        fill(4 * l + MP_QKV, kvInflight, 2 * bytes, [&](uint8_t *dst, uint64_t *bar) {
-                            tmaBulkLoad(dst, kHead + (size_t)c0 * HD, bytes, bar, kvPolicy);
-                            tmaBulkLoad(dst + kKvChunk * HD * 2, vHead + (size_t)c0 * HD, bytes, bar, kvPolicy);
-                        });
+                        if constexpr (Q8) {
+                            const uint32_t n = min(kKvChunk, it.cachedEnd - c0);
+                            const size_t headOff = (size_t)it.kvh * m.seqLen * HD;
+                            // int8 rows, then the 16-byte aligned span around their scale rows
+                            const uint32_t bytes = n * HD;
+                            const uint8_t *ks = reinterpret_cast<const uint8_t *>(m.kvScales[l].k + (headOff + (size_t)c0 * HD) / 32);
+                            const uint8_t *vs = reinterpret_cast<const uint8_t *>(m.kvScales[l].v + (headOff + (size_t)c0 * HD) / 32);
+                            const uint32_t kSkip = kvScSkip(ks), vSkip = kvScSkip(vs);
+                            const uint32_t kSb = (kSkip + n * (HD / 16) + 15) & ~15u, vSb = (vSkip + n * (HD / 16) + 15) & ~15u;
+                            fill(4 * l + MP_QKV, kvInflight, 2 * bytes + kSb + vSb, [&](uint8_t *dst, uint64_t *bar) {
+                                tmaBulkLoad(dst, kHead + (size_t)c0 * HD, bytes, bar, kvPolicy);
+                                tmaBulkLoad(dst + kKvChunk * HD, vHead + (size_t)c0 * HD, bytes, bar, kvPolicy);
+                                tmaBulkLoad(dst + 2 * kKvChunk * HD, ks - kSkip, kSb, bar, kvPolicy);
+                                tmaBulkLoad(dst + 2 * kKvChunk * HD + kvScRegion(HD), vs - vSkip, vSb, bar, kvPolicy);
+                            });
+                        } else {
+                            const uint32_t bytes = min(kKvChunk, it.cachedEnd - c0) * HD * 2;
+                            fill(4 * l + MP_QKV, kvInflight, 2 * bytes, [&](uint8_t *dst, uint64_t *bar) {
+                                tmaBulkLoad(dst, kHead + (size_t)c0 * HD, bytes, bar, kvPolicy);
+                                tmaBulkLoad(dst + kKvChunk * HD * 2, vHead + (size_t)c0 * HD, bytes, bar, kvPolicy);
+                            });
+                        }
                     }
                 }
             };
@@ -909,7 +965,7 @@ __global__ void __launch_bounds__(kTmaThreads, 1) megaDecodeKernel(const __grid_
         stamp();
         // no barrier: attention polls the q|k|v words it needs, CTAs without an attention item go on to the next barrier
         stamp();
-        megaAttention<HD>(m, sm, L, p, tid, e0 + 1, e0 + 2, ring);
+        megaAttention<HD, Q8>(m, sm, L, p, tid, e0 + 1, e0 + 2, ring);
         stamp();
         llBarrier();
         stamp();
@@ -966,6 +1022,7 @@ int launchMegaDecode(MegaArgs m, int numSms, cudaStream_t stream) {
     uint32_t stageBytes = 36 * 1024;
     if (maxRowBytes * 4 > stageBytes) stageBytes = (maxRowBytes * 4 + 127) / 128 * 128;
     if (2 * kKvChunk * m.headDim * 2 > stageBytes) return 1;   // a K/V fill: kKvChunk bf16 rows of K and of V
+    if (m.kvScales && 2 * kKvChunk * m.headDim + 2 * kvScRegion(m.headDim) > stageBytes) return 1;   // q80: int8 rows + scale spans
     if (fixedBytes + 2 * (size_t)stageBytes > budget) return 1;
     uint32_t stages = (uint32_t)((budget - fixedBytes) / stageBytes);
     if (stages > (uint32_t)kMaxStages) stages = kMaxStages;
@@ -992,12 +1049,14 @@ int launchMegaDecode(MegaArgs m, int numSms, cudaStream_t stream) {
     const size_t smemBytes = fixedBytes + (size_t)stages * stageBytes;
     // The kernel spins on grid barriers: every CTA must be resident at the same time. A cooperative launch makes the driver
     // verify that (and fail the launch instead of letting the barrier hang); the attribute cache is per device.
-    const int v = m.headDim == 128 ? 1 : 0;
+    const int v = (m.headDim == 128 ? 1 : 0) + (m.kvScales ? 2 : 0);
     int dev = 0;
     DL_CUDA_CHECK(cudaGetDevice(&dev));
-    static size_t configured[16][2] = {};
-    static int maxCoResident[16][2] = {};
-    const void *fn = v ? (const void *)megaDecodeKernel<128> : (const void *)megaDecodeKernel<64>;
+    static size_t configured[16][4] = {};
+    static int maxCoResident[16][4] = {};
+    void (*const kernels[4])(MegaArgs) = {megaDecodeKernel<64, false>, megaDecodeKernel<128, false>, megaDecodeKernel<64, true>,
+                                          megaDecodeKernel<128, true>};
+    const void *fn = (const void *)kernels[v];
     const int d = dev & 15;
     if (smemBytes > configured[d][v]) {
         DL_CUDA_CHECK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
@@ -1019,8 +1078,7 @@ int launchMegaDecode(MegaArgs m, int numSms, cudaStream_t stream) {
     attr[0].val.cooperative = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    if (v) DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, megaDecodeKernel<128>, m));
-    else DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, megaDecodeKernel<64>, m));
+    DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernels[v], m));
     return 0;
 }
 

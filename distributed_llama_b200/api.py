@@ -299,11 +299,13 @@ class InferenceSession:
     def __init__(self, model_path: str, tokenizer_path: Optional[str] = None, max_seq_len: int = 0,
                  temperature: float = 0.0, topp: float = 0.9, seed: int = 12345, device: Optional[str] = None,
                  max_batch: int = 8, use_pdl: bool = True, comm=None, moe_mode: str = "auto", presence_penalty: float = 0.0,
-                 frequency_penalty: float = 0.0, logit_bias: Optional[dict] = None, parallel: int = 1):
+                 frequency_penalty: float = 0.0, logit_bias: Optional[dict] = None, parallel: int = 1,
+                 kv_cache_float_type: str = "bf16"):
         """presence_penalty, frequency_penalty and logit_bias ({token id: value}) are the sampling controls of every
         completion (host Sampler.set_controls; they may be changed later through self.sampler.set_controls, which restarts the
         counts of the current completion). parallel > 1 splits the KV cache into that many slots for SlotScheduler
-        (slot_prefill, slot_copy, slot_sampling, slots_step); the single-sequence calls then must not be used."""
+        (slot_prefill, slot_copy, slot_sampling, slots_step); the single-sequence calls then must not be used.
+        kv_cache_float_type: "bf16" or "q80" (runtime.engine.Engine)."""
         from .models.loader import load_device_weights
         from .runtime.engine import Engine
 
@@ -319,7 +321,7 @@ class InferenceSession:
             device = f"cuda:{torch.cuda.current_device()}"
         self.device = torch.device(device)
         self.weights = load_device_weights(self.model_file, rank, n_ranks, self.device, moe_mode=moe_mode, comm=comm)
-        self.engine = Engine(self.weights, max_batch=max_batch, use_pdl=use_pdl, comm=comm)
+        self.engine = Engine(self.weights, max_batch=max_batch, use_pdl=use_pdl, comm=comm, kv_cache_float_type=kv_cache_float_type)
         H = host()
         self.tokenizer = H.Tokenizer(tokenizer_path) if tokenizer_path else None
         vocab = self.tokenizer.vocab_size if self.tokenizer else self.header.vocab_size

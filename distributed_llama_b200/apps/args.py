@@ -41,9 +41,11 @@ class AppArgs:
     gpus: int = 0            # spawn this many local ranks (0 = use the current torch.distributed world / single GPU)
     moe_mode: str = "auto"   # tp | ep | auto
     parallel: int = 1        # dllama-api: chat requests decoded together, one KV-cache slot each (1..8)
+    kv_cache_float_type: str = "bf16"   # KV-cache storage: bf16 | q80 (int8 blocks of 32 with an f16 scale)
 
 
 FLOAT_TYPES = ("f32", "f16", "q40", "q80")
+KV_CACHE_FLOAT_TYPES = ("bf16", "q80")
 TEMPLATES = ("llama2", "llama3", "deepSeek3", "chatml")
 
 
@@ -119,6 +121,10 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
             a.gpus = int(value)
         elif name == "--moe-mode":
             a.moe_mode = value
+        elif name == "--kv-cache-float-type":
+            if value not in KV_CACHE_FLOAT_TYPES:
+                raise ValueError(f"Invalid KV-cache float type: {value} (expected bf16 or q80)")
+            a.kv_cache_float_type = value
         elif name == "--parallel" and not require_mode:   # dllama-api only; its range is checked by api.parallel_refusal
             a.parallel = int(value)
         else:
@@ -131,6 +137,7 @@ USAGE = """Usage: dllama {inference|chat|perplexity|worker} {--model <path>} {--
         [--prompt <text>] [--steps <n>] [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>]
         [--temperature <temp>] [--topp <t>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]
         [--chat-template {llama2|llama3|deepSeek3|chatml}]
+        [--kv-cache-float-type {bf16|q80}] KV-cache storage (default bf16; q80 = int8 blocks of 32 + f16 scale)
         [--gpus <n>]                      run tensor-parallel on n local GPUs (spawns one process per GPU)
         [--workers <ip:port> ...] [--nthreads <n>] [--net-turbo {0|1}] [--gpu-index <i>] [--gpu-segments <a:b>]
                                           accepted for compatibility with the reference CLI

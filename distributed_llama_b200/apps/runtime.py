@@ -294,6 +294,13 @@ def worker_loop(sess: InferenceSession, comm, chan=None) -> None:
             eng.step_sampled(toks[0], pos, temperature, topp)
 
 
+def kv_cache_bytes(header, n_ranks: int, kv_type: str) -> int:
+    """Device bytes of one rank's K and V caches: bf16 = 2 bytes a value, q80 = 1 byte a value + a 2-byte scale per 32."""
+    kv_heads = header.n_kv_heads // n_ranks if header.n_kv_heads >= n_ranks else 1
+    values = 2 * header.n_layers * header.seq_len * kv_heads * header.head_dim
+    return values * 2 if kv_type == "bf16" else values + values // 16
+
+
 @dataclass
 class AppContext:
     args: AppArgs
@@ -319,7 +326,7 @@ def run_inference_app(args: AppArgs, handler: Callable[[AppContext], None]) -> N
     sess = InferenceSession(args.model, args.tokenizer, max_seq_len=args.max_seq_len, temperature=args.temperature,
                             topp=args.topp, seed=args.seed, comm=comm, moe_mode=getattr(args, "moe_mode", "auto") or "auto",
                             presence_penalty=args.presence_penalty, frequency_penalty=args.frequency_penalty,
-                            parallel=getattr(args, "parallel", 1))
+                            parallel=getattr(args, "parallel", 1), kv_cache_float_type=args.kv_cache_float_type)
     chan = open_control_channel(comm)
     if rank != 0:
         worker_loop(sess, comm, chan)
@@ -330,7 +337,7 @@ def run_inference_app(args: AppArgs, handler: Callable[[AppContext], None]) -> N
             print(f"Tokenizer vocab size ({tok.vocab_size}) does not match the model vocab size ({header.vocab_size})")
         print(tok.describe(), end="")
         print(header.describe(), end="")
-        req = H.required_device_bytes(header, n_nodes, 2)
+        req = H.required_device_bytes(header, n_nodes, 0) + kv_cache_bytes(header, n_nodes, args.kv_cache_float_type)
         print(f"📀 RequiredMemory: {req // (1024 * 1024)} MB")
         name = torch.cuda.get_device_name(sess.device)
         print(f"🧠 GPU: {name} x{n_nodes} (sm_90a kernels; tensor parallel over NVLink peer memory)")

@@ -4,7 +4,8 @@ Implements the math of the graph the reference builds in src/llm.cpp:247-603 (em
 [rmsnorm, q/k/v, (qk-norm), rope, causal GQA attention, wo, residual] + [rmsnorm, SwiGLU FFN | MoE, residual]
 -> final norm -> logits), on dequantised weights. `act_quant="q80"` additionally rounds activations to the
 q80 grid wherever the reference casts to its q80 buffers (before every q40 matmul), so the CUDA kernels —
-which do the same — can be compared tightly.
+which do the same — can be compared tightly. `kv_quant="q80"` rounds every K/V row to the q80 grid as it is stored in the
+cache (the engine's `--kv-cache-float-type q80`); every attention, the token's own row included, reads the rounded values.
 """
 from __future__ import annotations
 
@@ -33,10 +34,14 @@ def q80_round(x: torch.Tensor) -> torch.Tensor:
 
 
 class OracleModel:
-    def __init__(self, model_file: ModelFile, act_quant: str = "none", device: str = "cpu", dtype=torch.float32):
+    def __init__(self, model_file: ModelFile, act_quant: str = "none", device: str = "cpu", dtype=torch.float32,
+                 kv_quant: str = "none"):
+        if kv_quant not in ("none", "q80"):
+            raise ValueError(f"unknown kv_quant {kv_quant!r}")
         self.mf = model_file
         self.h = h = model_file.header
         self.act_quant = act_quant
+        self.kv_quant = kv_quant
         self.device = device
         self.dtype = dtype
         t = lambda name, l=0, e=0: torch.from_numpy(model_file.tensor_f32(model_file.entry(name, l, e))).to(device=device, dtype=dtype)
@@ -110,6 +115,8 @@ class OracleModel:
                 k = self._rms(k, L["k_norm"], eps)
             q = self._rope(q, pos)
             k = self._rope(k, pos)
+            if self.kv_quant == "q80":
+                k, v = q80_round(k).to(self.dtype), q80_round(v).to(self.dtype)
             self.k_cache[l][start_pos:start_pos + T] = k
             self.v_cache[l][start_pos:start_pos + T] = v
             K = self.k_cache[l][: start_pos + T]

@@ -18,12 +18,13 @@ u32, u64, i32, f32, vp = C.c_uint32, C.c_uint64, C.c_int, C.c_float, C.c_void_p
 class EngineConfig(C.Structure):
     _fields_ = [(n, u32) for n in ("dim", "nLayers", "nHeads", "nKvHeads", "headDim", "ffDim", "vocab", "seqLen",
                                    "nExperts", "nActiveExperts", "maxBatch", "nSplits", "rank", "nRanks", "numSms")] + \
-               [("eps", f32), ("usePdl", u32), ("moeFirstExpert", u32), ("moeNumLocal", u32), ("wType", u32), ("hiddenAct", u32)]
+               [("eps", f32), ("usePdl", u32), ("moeFirstExpert", u32), ("moeNumLocal", u32), ("wType", u32), ("hiddenAct", u32),
+                                             ("kvType", u32)]
 
 
 class LayerPtrs(C.Structure):
     _fields_ = [(n, vp) for n in ("qkvQs", "qkvSc", "woQs", "woSc", "w13Qs", "w13Sc", "w2Qs", "w2Sc",
-                                  "norm0", "norm1", "qNorm", "kNorm", "moeGate", "kCache", "vCache")]
+                                  "norm0", "norm1", "qNorm", "kNorm", "moeGate", "kCache", "vCache", "kScale", "vScale")]
 
 
 class GlobalPtrs(C.Structure):
@@ -64,6 +65,18 @@ def lib() -> C.CDLL:
     L.dl_attn_prefill_tc.restype = i32
     L.dl_rope_kv.argtypes = [vp, u32, vp, vp, vp, vp, f32, u32, u32, u32, u32, vp, vp, i32, vp]
     L.dl_rope_kv.restype = i32
+    L.dl_rope_kv_q80.argtypes = [vp, u32, vp, vp, vp, vp, f32, u32, u32, u32, u32, vp, vp, vp, vp, i32, vp]
+    L.dl_rope_kv_q80.restype = i32
+    L.dl_attn_decode_q80.argtypes = [vp, u32, vp, vp, vp, vp, vp, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp, i32, vp]
+    L.dl_attn_decode_q80.restype = i32
+    L.dl_attn_fused_q80.argtypes = [vp, vp, vp, vp, vp, f32, vp, vp, vp, vp, u32, u32, u32, u32, u32, vp, vp, vp, vp]
+    L.dl_attn_fused_q80.restype = i32
+    L.dl_choice_attn_only_q80.argtypes = [vp, u32, vp, vp, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
+    L.dl_choice_attn_only_q80.restype = i32
+    L.dl_slot_attn_q80.argtypes = [vp, u32, vp, vp, vp, vp, vp, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
+    L.dl_slot_attn_q80.restype = i32
+    L.dl_attn_prefill_tc_q80.argtypes = [vp, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, vp, vp, u32, vp]
+    L.dl_attn_prefill_tc_q80.restype = i32
     L.dl_attn_decode.argtypes = [vp, u32, vp, vp, vp, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp, i32, vp]
     L.dl_attn_decode.restype = i32
     L.dl_attn_fused.argtypes = [vp, vp, vp, vp, vp, f32, vp, vp, u32, u32, u32, u32, u32, vp, vp, vp, vp]
@@ -202,6 +215,9 @@ def stream_ptr() -> int:
     import torch
     return torch.cuda.current_stream().cuda_stream
 
+
+# KV-cache storage (EngineConfig.kvType): name of --kv-cache-float-type -> code
+KV_CACHE_TYPES = {"bf16": 0, "q80": 1}
 
 PRO_RMSNORM, PRO_PLAIN = 0, 1
 EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU = 0, 1, 2

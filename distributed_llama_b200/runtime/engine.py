@@ -24,7 +24,11 @@ def _p(t: Optional[torch.Tensor]):
 
 class Engine:
     def __init__(self, weights: DeviceWeights, max_batch: int = 8, n_splits: int = 0, use_pdl: bool = True,
-                 seq_len: Optional[int] = None, comm=None, max_prefill: int = 192, collectives: str = "auto"):
+                 seq_len: Optional[int] = None, comm=None, max_prefill: int = 192, collectives: str = "auto",
+                 kv_cache_float_type: str = "bf16"):
+        if kv_cache_float_type not in cl.KV_CACHE_TYPES:
+            raise ValueError(f"unknown KV-cache float type {kv_cache_float_type!r} (expected one of: {', '.join(cl.KV_CACHE_TYPES)})")
+        self.kv_cache_float_type = kv_cache_float_type
         self.w = w = weights
         h = w.header
         dev = w.embedding.device
@@ -65,8 +69,18 @@ class Engine:
         self.attn_partial = torch.zeros(max_batch * w.n_heads * n_splits * (hd + 2), **f32)
         self.attn_counters = torch.zeros(max_batch * w.n_heads, dtype=torch.int32, device=dev)
         self.history = torch.zeros(self.seq_len + 1, dtype=torch.int32, device=dev)
-        self.k_cache = [torch.zeros(w.n_kv_heads, self.seq_len, hd, dtype=torch.bfloat16, device=dev) for _ in range(h.n_layers)]
-        self.v_cache = [torch.zeros(w.n_kv_heads, self.seq_len, hd, dtype=torch.bfloat16, device=dev) for _ in range(h.n_layers)]
+        if kv_cache_float_type == "q80":
+            # int8 values [nKvHeads][seqLen][hd] and f16 scales [nKvHeads][seqLen][hd / 32] (+ 8 halves of tail padding: the
+            # persistent kernel copies the 16-byte aligned span around a chunk's scale rows)
+            kv_shape, kv_dtype = (w.n_kv_heads, self.seq_len, hd), torch.int8
+            sc_elems = w.n_kv_heads * self.seq_len * (hd // 32)
+            self.k_scale = [torch.zeros(sc_elems + 8, dtype=torch.float16, device=dev) for _ in range(h.n_layers)]
+            self.v_scale = [torch.zeros(sc_elems + 8, dtype=torch.float16, device=dev) for _ in range(h.n_layers)]
+        else:
+            kv_shape, kv_dtype = (w.n_kv_heads, self.seq_len, hd), torch.bfloat16
+            self.k_scale = self.v_scale = [None] * h.n_layers
+        self.k_cache = [torch.zeros(*kv_shape, dtype=kv_dtype, device=dev) for _ in range(h.n_layers)]
+        self.v_cache = [torch.zeros(*kv_shape, dtype=kv_dtype, device=dev) for _ in range(h.n_layers)]
         self.expert_idx = torch.zeros(max_batch * max(1, h.n_active_experts), dtype=torch.int32, device=dev)
         self.expert_weight = torch.zeros(max_batch * max(1, h.n_active_experts), **f32)
         self.max_prefill = mp = min(max_prefill, 256)
@@ -90,14 +104,16 @@ class Engine:
                               nRanks=w.n_ranks, numSms=self.num_sms, eps=h.norm_epsilon, usePdl=1 if use_pdl else 0,
                               moeFirstExpert=w.first_expert, moeNumLocal=w.n_local_experts,
                               wType=getattr(w, "weight_kind", 0),
-                              hiddenAct=1 if int(h.hidden_act) == 0 else 0)   # header: ACT_GELU = 0, ACT_SILU = 1
+                              hiddenAct=1 if int(h.hidden_act) == 0 else 0,   # header: ACT_GELU = 0, ACT_SILU = 1
+                              kvType=cl.KV_CACHE_TYPES[kv_cache_float_type])
         self._lib = cl.lib()
         self._h = self._lib.dl_engine_create(C.byref(cfg))
         for l, L in enumerate(w.layers):
             lp = cl.LayerPtrs(qkvQs=_p(L.qkv.qs), qkvSc=_p(L.qkv.scales), woQs=_p(L.wo.qs), woSc=_p(L.wo.scales),
                               w13Qs=_p(L.w13.qs), w13Sc=_p(L.w13.scales), w2Qs=_p(L.w2.qs), w2Sc=_p(L.w2.scales),
                               norm0=_p(L.norm0), norm1=_p(L.norm1), qNorm=_p(L.q_norm), kNorm=_p(L.k_norm),
-                              moeGate=_p(L.moe_gate), kCache=_p(self.k_cache[l]), vCache=_p(self.v_cache[l]))
+                              moeGate=_p(L.moe_gate), kCache=_p(self.k_cache[l]), vCache=_p(self.v_cache[l]),
+                              kScale=_p(self.k_scale[l]), vScale=_p(self.v_scale[l]))
             cl.check(self._lib.dl_engine_set_layer(self._h, l, C.byref(lp)), "engine_set_layer")
         emb_peers = (C.c_void_p * 8)(*([C.c_void_p(p) for p in (w.embedding_ptrs or [])] + [None] * (8 - len(w.embedding_ptrs or []))))
         gp = cl.GlobalPtrs(embedding=_p(w.embedding), embeddingPeers=emb_peers, embRowsPerRank=w.embedding_rows or 0, finalNorm=_p(w.final_norm), wclsQs=_p(w.wcls.qs),

@@ -1,8 +1,9 @@
 """Phase timeline of the persistent decode kernel (one %globaltimer stamp at every phase start on CTA 0).
 
-    python tools/trace_mega.py [model] [--all] [--pos=N] [--save=FILE]
+    python tools/trace_mega.py [model] [--all] [--pos=N] [--kv=bf16|q80] [--save=FILE]
 
 --pos=N traces the step at position N (default 63, the position after the 64-token prompt; the context is sized to fit it).
+--kv=q80 runs with the q80 KV cache (--kv-cache-float-type), default bf16.
 """
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -15,6 +16,7 @@ args = [a for a in sys.argv[1:] if not a.startswith("--")]
 ALL = "--all" in sys.argv          # every CTA records its stamps: barrier skew analysis
 SAVE = next((a.split("=", 1)[1] for a in sys.argv[1:] if a.startswith("--save=")), None)   # --all: also write the stamps (us) as .npy
 POS = int(next((a.split("=", 1)[1] for a in sys.argv[1:] if a.startswith("--pos=")), 63))
+KV = next((a.split("=", 1)[1] for a in sys.argv[1:] if a.startswith("--kv=")), "bf16")
 model = args[0] if args else "llama-3.1-8b"
 comm = None
 rank = int(os.environ.get("RANK", "0"))
@@ -28,7 +30,7 @@ if int(os.environ.get("WORLD_SIZE", "1")) > 1:
         ensure_model(model)
     dist.barrier()
 m, t = ensure_model(model)
-sess = InferenceSession(m, t, max_seq_len=max(2048, POS + 64), comm=comm)
+sess = InferenceSession(m, t, max_seq_len=max(2048, POS + 64), comm=comm, kv_cache_float_type=KV)
 eng = sess.engine
 eng.enable_trace(4096, all_ctas=ALL)
 eng.enable_mega()
