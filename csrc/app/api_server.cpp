@@ -13,7 +13,9 @@
 #include <memory>
 #include <mutex>
 #include <thread>
+#include <cmath>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <ctime>
 #include <stdexcept>
@@ -148,19 +150,173 @@ size_t NaiveCache::coveredPrefix(const std::vector<ChatItem> &messages) const {
     return n;
 }
 
-std::string chunkJson(const std::string *delta, bool stop, uint32_t index) {
+namespace {
+std::string joinEntries(const std::vector<std::string> &entries) {
+    std::string s = "{\"content\": [";
+    for (size_t i = 0; i < entries.size(); i++) s += (i ? ", " : "") + entries[i];
+    return s + "]}";
+}
+}  // namespace
+
+std::string chunkJson(const std::string *delta, bool stop, uint32_t index, const std::vector<std::string> *logprobs) {
     std::string s = "{\"id\": \"cmpl-c0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
                     ", \"model\": \"Distributed Model\", \"choices\": [{\"index\": " + std::to_string(index) + ", \"finish_reason\": " +
                     (stop ? "\"stop\"" : "\"\"");
     if (!stop) s += ", \"delta\": {\"role\": \"assistant\", \"content\": " + jsonEscape(delta ? *delta : std::string()) + "}";
+    if (!stop && logprobs) s += ", \"logprobs\": " + joinEntries(*logprobs);
     s += "}]}";
     return s;
 }
 
+// ---- log-probabilities --------------------------------------------------------------------------------------------------------
+
+TokenLogprobs decodeLogprobs(const int32_t *w) {
+    const auto f = [](int32_t bits) { float v; std::memcpy(&v, &bits, 4); return v; };
+    TokenLogprobs e;
+    e.token = w[0];
+    e.logprob = f(w[1]);
+    for (int j = 0; j < w[2]; j++) e.top.push_back({w[4 + 2 * j], f(w[5 + 2 * j])});
+    return e;
+}
+
+int parseLogprobs(const JsonValue &body) {
+    const JsonValue *on = body.find("logprobs"), *k = body.find("top_logprobs");
+    if (on && on->kind != JsonValue::Bool) throw std::runtime_error("'logprobs' must be a boolean");
+    const bool enabled = on && on->b;
+    if (k && !enabled) throw std::runtime_error("'top_logprobs' needs 'logprobs': true");
+    if (k && !(k->kind == JsonValue::Number && k->integral && k->num >= 0 && k->num <= kMaxTopLogprobs))
+        throw std::runtime_error("'top_logprobs' must be an integer from 0 to 20");
+    return enabled ? (k ? (int)k->num : 0) : -1;
+}
+
+namespace {
+// repr() of a Python float: the shortest digits that read back as v, positional for exponents -4 .. 15, else d.ddde±XX
+std::string pyFloat(double v) {
+    if (std::isnan(v)) return "NaN";
+    if (std::isinf(v)) return v < 0 ? "-Infinity" : "Infinity";
+    if (v == 0) return std::signbit(v) ? "-0.0" : "0.0";
+    char buf[64];
+    for (int p = 1; p <= 17; p++) {
+        std::snprintf(buf, sizeof(buf), "%.*e", p - 1, v);
+        if (std::strtod(buf, nullptr) == v) break;
+    }
+    std::string s(buf), sign;
+    if (s[0] == '-') { sign = "-"; s = s.substr(1); }
+    const size_t ePos = s.find('e');
+    const int e = std::atoi(s.c_str() + ePos + 1);
+    std::string digits;
+    for (size_t i = 0; i < ePos; i++) if (s[i] != '.') digits += s[i];
+    while (digits.size() > 1 && digits.back() == '0') digits.pop_back();
+    if (e >= -4 && e < 16) {
+        if (e < 0) return sign + "0." + std::string((size_t)(-e - 1), '0') + digits;
+        if (digits.size() <= (size_t)e + 1) return sign + digits + std::string((size_t)e + 1 - digits.size(), '0') + ".0";
+        return sign + digits.substr(0, (size_t)e + 1) + "." + digits.substr((size_t)e + 1);
+    }
+    std::snprintf(buf, sizeof(buf), "e%c%02d", e < 0 ? '-' : '+', std::abs(e));
+    return sign + digits.substr(0, 1) + (digits.size() > 1 ? "." + digits.substr(1) : "") + buf;
+}
+
+// bytes decoded as UTF-8 with replacement (one U+FFFD per maximal invalid subpart, as Python's errors="replace"), then escaped as
+// json.dumps does by default: every character outside ' '..'~' as \uXXXX (surrogate pairs above U+FFFF)
+std::string jsonEscapeUtf8Ascii(const std::string &bytes) {
+    std::string out = "\"";
+    const auto put = [&](uint32_t cp) {
+        char buf[16];
+        if (cp == '"') out += "\\\"";
+        else if (cp == '\\') out += "\\\\";
+        else if (cp == '\n') out += "\\n";
+        else if (cp == '\r') out += "\\r";
+        else if (cp == '\t') out += "\\t";
+        else if (cp == '\b') out += "\\b";
+        else if (cp == '\f') out += "\\f";
+        else if (cp >= 0x20 && cp < 0x7f) out += (char)cp;
+        else if (cp < 0x10000) { std::snprintf(buf, sizeof(buf), "\\u%04x", cp); out += buf; }
+        else {
+            const uint32_t c = cp - 0x10000;
+            std::snprintf(buf, sizeof(buf), "\\u%04x\\u%04x", 0xd800 + (c >> 10), 0xdc00 + (c & 0x3ff));
+            out += buf;
+        }
+    };
+    const size_t n = bytes.size();
+    for (size_t i = 0; i < n;) {
+        const unsigned char c = (unsigned char)bytes[i];
+        int need;
+        uint32_t cp;
+        if (c < 0x80) { put(c); i++; continue; }
+        else if (c >= 0xc2 && c <= 0xdf) { need = 1; cp = c & 0x1f; }
+        else if (c >= 0xe0 && c <= 0xef) { need = 2; cp = c & 0x0f; }
+        else if (c >= 0xf0 && c <= 0xf4) { need = 3; cp = c & 0x07; }
+        else { put(0xfffd); i++; continue; }
+        size_t j = i + 1;
+        int got = 0;
+        for (; got < need && j < n; got++, j++) {
+            const unsigned char d = (unsigned char)bytes[j];
+            unsigned char lo = 0x80, hi = 0xbf;
+            if (got == 0) {
+                if (c == 0xe0) lo = 0xa0;
+                else if (c == 0xed) hi = 0x9f;
+                else if (c == 0xf0) lo = 0x90;
+                else if (c == 0xf4) hi = 0x8f;
+            }
+            if (d < lo || d > hi) break;
+            cp = (cp << 6) | (d & 0x3f);
+        }
+        if (got == need) put(cp);
+        else put(0xfffd);
+        i = j;
+    }
+    return out + "\"";
+}
+
+std::string tokenJson(const Tokenizer &tok, int32_t id, float logprob) {
+    const std::string &b = tok.data().vocab.at((size_t)id);
+    std::string bytes;
+    for (size_t i = 0; i < b.size(); i++) bytes += (i ? ", " : "") + std::to_string((unsigned)(unsigned char)b[i]);
+    return "{\"token\": " + jsonEscapeUtf8Ascii(b) + ", \"logprob\": " + pyFloat((double)logprob) + ", \"bytes\": [" + bytes + "]";
+}
+}  // namespace
+
+std::string logprobEntryJson(const Tokenizer &tok, const TokenLogprobs &e) {
+    std::string s = tokenJson(tok, e.token, e.logprob) + ", \"top_logprobs\": [";
+    for (size_t i = 0; i < e.top.size(); i++) s += (i ? ", " : "") + tokenJson(tok, e.top[i].first, e.top[i].second) + "}";
+    return s + "]}";
+}
+
+namespace {
+// Entries of the tokens of n choices: all of them for the final JSON, those not yet sent for the stream. The token that ends a
+// choice by end of sequence gets none (the Python server's LogprobsLog).
+struct LogprobsLog {
+    std::vector<std::string> next;
+    std::vector<std::vector<std::string>> all, pending;
+    explicit LogprobsLog(uint32_t n = 0) : next(n), all(n), pending(n) {}
+    void consumed(uint32_t i, bool eos) {
+        if (!eos) { all[i].push_back(next[i]); pending[i].push_back(next[i]); }
+        next[i].clear();
+    }
+    std::vector<std::string> take(uint32_t i) { std::vector<std::string> out; out.swap(pending[i]); return out; }
+};
+
+// choice i's stop chunk, after one delta chunk with empty content for entries still unsent
+void writeStreamFinish(const HttpRequest &req, uint32_t i, LogprobsLog *lps) {
+    if (lps && !lps->pending[i].empty()) {
+        const std::string empty;
+        const std::vector<std::string> e = lps->take(i);
+        req.writeStreamChunk("data: " + chunkJson(&empty, false, i, &e) + "\r\n\r\n");
+    }
+    req.writeStreamChunk("data: " + chunkJson(nullptr, true, i) + "\r\n\r\n");
+}
+
+std::string choiceJson(uint32_t i, const std::string &content, const LogprobsLog *lps) {
+    return "{\"index\": " + std::to_string(i) + ", \"message\": {\"role\": \"assistant\", \"content\": " + jsonEscape(content) +
+           "}, \"finish_reason\": \"stop\"" + (lps ? ", \"logprobs\": " + joinEntries(lps->all[i]) : std::string()) + "}";
+}
+}  // namespace
+
 // ---- several completions of one prompt ------------------------------------------------------------------------------------
 
 std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t token, uint32_t P, uint32_t n, int maxTokens, uint32_t seqLen,
-                                             Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken) {
+                                             Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken,
+                                             const std::function<void(uint32_t, const TokenLogprobs &)> &onLogprobs) {
     if (n < 1 || n > kMaxChoices) throw std::runtime_error("n must be between 1 and 8");
     std::vector<std::vector<int32_t>> out(n);
     const uint32_t C = P + 1 < seqLen ? (seqLen - 1 - P) / n : 0;
@@ -176,9 +332,11 @@ std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t 
         uint32_t nDone = 0;
         while (out[first].size() < limit) {
             tok = backend.next(tok, pos++, smp);
+            const TokenLogprobs entry = onLogprobs ? backend.lastLogprobs().at(0) : TokenLogprobs();
             for (uint32_t i = first; i <= last; i++) {
                 if (done[i]) continue;
                 out[i].push_back(tok);
+                if (onLogprobs) onLogprobs(i, entry);
                 if (onToken(i, tok)) { done[i] = true; nDone++; }
             }
             if (nDone == last - first + 1) break;
@@ -206,9 +364,11 @@ std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t 
     std::vector<int32_t> last = backend.choicesFirst(token, P, n, T, topp);
     uint32_t active = (1u << n) - 1u;
     for (uint32_t j = 0;; j++) {
+        const std::vector<TokenLogprobs> entries = onLogprobs ? backend.lastLogprobs() : std::vector<TokenLogprobs>();
         for (uint32_t i = 0; i < n; i++) {
             if (!((active >> i) & 1u)) continue;
             out[i].push_back(last[i]);
+            if (onLogprobs) onLogprobs(i, entries.at(i));
             if (onToken(i, last[i]) || out[i].size() >= limit) active &= ~(1u << i);
         }
         if (!active) break;
@@ -295,6 +455,8 @@ void ApiServer::complete(HttpRequest &req) {
     float presence = cfg_.presencePenalty, frequency = cfg_.frequencyPenalty;
     std::vector<std::pair<int32_t, float>> bias;
     parseControls(body, sampler_.vocabSize(), presence, frequency, bias);
+    const int lpK = parseLogprobs(body);
+    backend_.setLogprobs(lpK);   // refuses where they cannot run (tensor parallelism)
     sampler_.setControls(presence, frequency, bias);
     bool seeded = false;
     if (const JsonValue *s = body.find("seed")) if (s->kind == JsonValue::Number) { sampler_.setSeed((uint64_t)s->num); seeded = true; }
@@ -312,10 +474,15 @@ void ApiServer::complete(HttpRequest &req) {
 
     std::vector<EosDetector> dets(n, EosDetector(tok_.data().eosIds, stops_, maxLen(stops_), maxLen(stops_)));
     std::vector<std::string> pending(n), buffers(n, g.publicPrompt);
+    LogprobsLog log(n);
+    LogprobsLog *lps = lpK >= 0 ? &log : nullptr;
     if (stream) {
         req.writeStreamStart();
         if (!g.publicPrompt.empty())
-            for (uint32_t i = 0; i < n; i++) req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false, i) + "\r\n\r\n");
+            for (uint32_t i = 0; i < n; i++) {
+                const std::vector<std::string> e;
+                req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false, i, lps ? &e : nullptr) + "\r\n\r\n");
+            }
     }
     const uint32_t nPref = promptEnd - startPos;
     backend_.prefill(std::vector<int32_t>(tokens.begin(), tokens.begin() + nPref), startPos);
@@ -324,24 +491,31 @@ void ApiServer::complete(HttpRequest &req) {
         const std::string piece = tok_.decodeWith(pending[i], t);
         if (n == 1 && !piece.empty()) { std::printf("%s", piece.c_str()); std::fflush(stdout); }
         const EosDetectorResult kind = dets[i].append(t, piece);
+        if (lps) lps->consumed(i, kind == EOS);
         if (kind == NOT_EOS || kind == EOS) {
             const std::string delta = dets[i].getDelta();
             if (!delta.empty()) {
-                if (stream) req.writeStreamChunk("data: " + chunkJson(&delta, false, i) + "\r\n\r\n");
+                if (stream) {
+                    const std::vector<std::string> e = lps ? lps->take(i) : std::vector<std::string>();
+                    req.writeStreamChunk("data: " + chunkJson(&delta, false, i, lps ? &e : nullptr) + "\r\n\r\n");
+                }
                 buffers[i] += delta;
             }
             dets[i].reset();
         }
         return kind == EOS;
     };
-    const std::vector<std::vector<int32_t>> out = runChoices(backend_, token, promptEnd, n, maxTokens, seqLen, sampler_, baseSeed, onToken);
+    std::function<void(uint32_t, const TokenLogprobs &)> onLogprobs;
+    if (lps) onLogprobs = [&](uint32_t i, const TokenLogprobs &e) { log.next[i] = logprobEntryJson(tok_, e); };
+    const std::vector<std::vector<int32_t>> out = runChoices(backend_, token, promptEnd, n, maxTokens, seqLen, sampler_, baseSeed, onToken,
+                                                             onLogprobs);
     if (n == 1) {
         const uint32_t end = promptEnd + (uint32_t)out[0].size();
         if (end == seqLen) cache_.clear();
         else cache_.push(end, {"assistant", buffers[0]});
     }
     if (stream) {
-        for (uint32_t i = 0; i < n; i++) req.writeStreamChunk("data: " + chunkJson(nullptr, true, i) + "\r\n\r\n");
+        for (uint32_t i = 0; i < n; i++) writeStreamFinish(req, i, lps);
         req.writeStreamChunk("data: [DONE]");
         req.writeStreamEnd();
     } else {
@@ -349,8 +523,7 @@ void ApiServer::complete(HttpRequest &req) {
         std::string choices;
         for (uint32_t i = 0; i < n; i++) {
             nCompletion += (uint32_t)out[i].size();
-            choices += std::string(i ? ", " : "") + "{\"index\": " + std::to_string(i) + ", \"message\": {\"role\": \"assistant\", \"content\": " +
-                       jsonEscape(buffers[i]) + "}, \"finish_reason\": \"stop\"}";
+            choices += std::string(i ? ", " : "") + choiceJson(i, buffers[i], lps);
         }
         req.writeJson("{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
                       ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
@@ -368,13 +541,13 @@ void ApiServer::models(HttpRequest &req) const {
 // ---- concurrent requests (--parallel): the rules of distributed_llama_b200.api.SlotScheduler --------------------------------
 
 namespace {
-std::string completionJson(uint32_t nPrompt, const std::vector<std::vector<int32_t>> &out, const std::vector<std::string> &buffers) {
+std::string completionJson(uint32_t nPrompt, const std::vector<std::vector<int32_t>> &out, const std::vector<std::string> &buffers,
+                           const LogprobsLog *lps) {
     uint32_t nCompletion = 0;
     std::string choices;
     for (uint32_t i = 0; i < buffers.size(); i++) {
         nCompletion += (uint32_t)out[i].size();
-        choices += std::string(i ? ", " : "") + "{\"index\": " + std::to_string(i) + ", \"message\": {\"role\": \"assistant\", \"content\": " +
-                   jsonEscape(buffers[i]) + "}, \"finish_reason\": \"stop\"}";
+        choices += std::string(i ? ", " : "") + choiceJson(i, buffers[i], lps);
     }
     return "{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
            ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
@@ -392,12 +565,15 @@ struct SlotJob {
     float temperature = 0.f, topp = 0.9f, presence = 0.f, frequency = 0.f;
     std::vector<std::pair<int32_t, float>> bias;
     uint64_t seed = 0;
+    int logprobs = -1;   // top_logprobs k, -1: none
     // admitted
     std::vector<uint32_t> slots;
     uint32_t P = 0, nPrompt = 0, limit = 0, live = 0;
     std::vector<std::vector<int32_t>> out;
     std::vector<EosDetector> dets;
     std::vector<std::string> pending, buffers;
+    LogprobsLog lps;
+    LogprobsLog *lp() { return logprobs >= 0 ? &lps : nullptr; }
 };
 
 struct SlotRow {
@@ -442,6 +618,7 @@ void ApiServer::serveParallel(int srv) {
                 job->presence = cfg_.presencePenalty;
                 job->frequency = cfg_.frequencyPenalty;
                 parseControls(body, sampler_.vocabSize(), job->presence, job->frequency, job->bias);
+                job->logprobs = parseLogprobs(body);   // --parallel > 1 runs on one GPU
                 for (const JsonValue &m : body.at("messages").arr) job->messages.push_back({m.at("role").str, m.at("content").str});
                 job->stream = body.boolOr("stream", false);
                 job->temperature = (float)body.numberOr("temperature", cfg_.temperature);
@@ -500,11 +677,11 @@ void ApiServer::serveParallel(int srv) {
         }
         for (size_t k = 1; k < j.slots.size(); k++) caches[j.slots[k]].copyFrom(cache);   // they hold a copy of the prompt rows
         if (j.stream) {
-            for (uint32_t i = 0; i < j.n; i++) j.req.writeStreamChunk("data: " + chunkJson(nullptr, true, i) + "\r\n\r\n");
+            for (uint32_t i = 0; i < j.n; i++) writeStreamFinish(j.req, i, j.lp());
             j.req.writeStreamChunk("data: [DONE]");
             j.req.writeStreamEnd();
         } else {
-            j.req.writeJson(completionJson(j.nPrompt, j.out, j.buffers));
+            j.req.writeJson(completionJson(j.nPrompt, j.out, j.buffers, j.lp()));
         }
         std::printf("🔶 slot %u%s\n", j.slots[0], j.n > 1 ? (" (" + std::to_string(j.n) + " choices)").c_str() : "");
         std::fflush(stdout);
@@ -529,10 +706,14 @@ void ApiServer::serveParallel(int srv) {
         j.pending.assign(j.n, std::string());
         j.dets.assign(j.n, EosDetector(tok_.data().eosIds, stops_, maxLen(stops_), maxLen(stops_)));
         j.out.assign(j.n, {});
+        j.lps = LogprobsLog(j.n);
         if (j.stream) {
             j.req.writeStreamStart();
             if (!g.publicPrompt.empty())
-                for (uint32_t i = 0; i < j.n; i++) j.req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false, i) + "\r\n\r\n");
+                for (uint32_t i = 0; i < j.n; i++) {
+                    const std::vector<std::string> e;
+                    j.req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false, i, j.lp() ? &e : nullptr) + "\r\n\r\n");
+                }
         }
         for (const ChatItem &m : delta) cache.push(j.P, m);
         const uint32_t nPref = j.P - start;
@@ -541,7 +722,10 @@ void ApiServer::serveParallel(int srv) {
         for (size_t k = 1; k < j.slots.size(); k++) backend_.slotCopy(first, j.slots[k], j.P);
         const uint64_t seed = j.hasSeed ? j.seed : (j.temperature != 0.f ? sampler_.nextSeed() : 0);
         for (size_t k = 0; k < j.slots.size(); k++)
+        {
             backend_.slotSampling(j.slots[k], j.n == 1 ? seed : choiceSeed(seed, (uint32_t)k), j.temperature, j.topp, j.presence, j.frequency, j.bias);
+            if (j.logprobs >= 0) backend_.slotLogprobs(j.slots[k], j.logprobs);
+        }
         j.limit = L - j.P;
         if (j.maxTokens > 0) j.limit = std::min<uint32_t>(j.limit, (uint32_t)j.maxTokens);
         if (j.limit == 0) { finish(job); return; }
@@ -559,10 +743,15 @@ void ApiServer::serveParallel(int srv) {
     const auto onToken = [&](SlotJob &j, uint32_t i, int32_t t) {
         const std::string piece = tok_.decodeWith(j.pending[i], t);
         const EosDetectorResult kind = j.dets[i].append(t, piece);
+        LogprobsLog *lps = j.lp();
+        if (lps) lps->consumed(i, kind == EOS);
         if (kind == NOT_EOS || kind == EOS) {
             const std::string delta = j.dets[i].getDelta();
             if (!delta.empty()) {
-                if (j.stream) j.req.writeStreamChunk("data: " + chunkJson(&delta, false, i) + "\r\n\r\n");
+                if (j.stream) {
+                    const std::vector<std::string> e = lps ? lps->take(i) : std::vector<std::string>();
+                    j.req.writeStreamChunk("data: " + chunkJson(&delta, false, i, lps ? &e : nullptr) + "\r\n\r\n");
+                }
                 j.buffers[i] += delta;
             }
             j.dets[i].reset();
@@ -599,7 +788,10 @@ void ApiServer::serveParallel(int srv) {
         for (uint32_t s = 0; s < N; s++)
             if (rows[s].job) { tokens[s] = rows[s].token; pos[s] = rows[s].pos; active |= 1u << s; }
         if (!active) continue;
-        const std::vector<int32_t> drawn = backend_.slotsStep(tokens, pos, active);
+        bool wantLp = false;
+        for (uint32_t s = 0; s < N; s++) wantLp = wantLp || (rows[s].job && rows[s].job->logprobs >= 0);
+        std::vector<TokenLogprobs> entries;
+        const std::vector<int32_t> drawn = wantLp ? backend_.slotsStepLogprobs(tokens, pos, active, entries) : backend_.slotsStep(tokens, pos, active);
         for (uint32_t s = 0; s < N; s++) {
             SlotRow &r = rows[s];
             if (!r.job) continue;
@@ -612,6 +804,7 @@ void ApiServer::serveParallel(int srv) {
                     if (r.done[c]) continue;
                     const uint32_t i = r.choices[c];
                     j.out[i].push_back(drawn[s]);
+                    if (j.logprobs >= 0) j.lps.next[i] = logprobEntryJson(tok_, entries.at(s));
                     if (onToken(j, i, drawn[s]) || j.out[i].size() >= j.limit) { r.done[c] = true; r.nDone++; }
                 }
             } catch (const std::exception &e) {

@@ -15,6 +15,15 @@
 
 namespace dl {
 
+constexpr int kMaxTopLogprobs = 20;   // the largest `top_logprobs` (csrc/cuda/logprobs.cu)
+
+// The log-probabilities of one drawn token: its logprob and the k most likely (id, logprob) in the order (logprob desc, id asc).
+struct TokenLogprobs {
+    int32_t token = -1;
+    float logprob = 0.f;
+    std::vector<std::pair<int32_t, float>> top;
+};
+
 struct InferenceBackend {
     virtual ~InferenceBackend() {}
     virtual uint32_t seqLen() const = 0;
@@ -47,7 +56,20 @@ struct InferenceBackend {
     virtual std::vector<int32_t> slotsStep(const std::vector<int32_t> & /*tokens*/, const std::vector<int32_t> & /*pos*/, uint32_t /*activeMask*/) {
         throw std::runtime_error("slots unsupported");
     }
+    // Log-probabilities of the following next / choicesFirst / choicesStep draws with k (0..20) top entries, -1: none (throws where
+    // they cannot run, e.g. under tensor parallelism). lastLogprobs(): one entry per row of the last such call.
+    virtual void setLogprobs(int k) { if (k >= 0) throw std::runtime_error("logprobs are not supported by this backend"); }
+    virtual std::vector<TokenLogprobs> lastLogprobs() { return {}; }
+    // slot `slot`'s draws with k top entries (-1: none; every slotSampling resets it), and slotsStep that also returns them
+    virtual void slotLogprobs(uint32_t /*slot*/, int k) { if (k >= 0) throw std::runtime_error("logprobs are not supported by this backend"); }
+    virtual std::vector<int32_t> slotsStepLogprobs(const std::vector<int32_t> & /*tokens*/, const std::vector<int32_t> & /*pos*/,
+                                                   uint32_t /*activeMask*/, std::vector<TokenLogprobs> & /*rows*/) {
+        throw std::runtime_error("logprobs are not supported by this backend");
+    }
 };
+
+// One row's result block of the log-probability kernel (kApiLogprobsWords int32 words, csrc/cuda/engine_api.h) decoded.
+TokenLogprobs decodeLogprobs(const int32_t *words);
 
 constexpr uint32_t kMaxChoices = 8;   // the engine's widest batch: one row per choice
 
@@ -57,8 +79,10 @@ constexpr uint32_t kMaxChoices = 8;   // the engine's widest batch: one row per 
 // single-sequence loop of the CLIs instead: it stops after min(maxTokens, seqLen - P) tokens, so it may fill the context up to
 // its last row. onToken(i, token) returns true when choice i is finished. The sampler's controls apply to every choice, each with
 // its own counts from zero. Same rules as distributed_llama_b200.api.run_choices.
+// onLogprobs (optional, with backend.setLogprobs(k) made): called with each token's entry right before onToken(i, token).
 std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t token, uint32_t P, uint32_t n, int maxTokens, uint32_t seqLen,
-                                             Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken);
+                                             Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken,
+                                             const std::function<void(uint32_t, const TokenLogprobs &)> &onLogprobs = nullptr);
 
 struct HttpRequest {
     int fd = -1;
@@ -94,7 +118,14 @@ private:
     std::vector<Item> items_;
 };
 
-std::string chunkJson(const std::string *delta, bool stop, uint32_t index = 0);   // one streamed `chat.completion` chunk
+// one streamed `chat.completion` chunk; `logprobs` (entries as JSON text, may be empty) adds "logprobs": {"content": [...]}
+std::string chunkJson(const std::string *delta, bool stop, uint32_t index = 0, const std::vector<std::string> *logprobs = nullptr);
+
+// The request's log-probabilities: -1 without them, else the number of top entries; the rules of
+// distributed_llama_b200.apps.api_server.parse_logprobs (throws on anything else).
+int parseLogprobs(const JsonValue &body);
+// One token's response entry {"token", "logprob", "bytes", "top_logprobs"}, formatted as the Python server's json.dumps does.
+std::string logprobEntryJson(const Tokenizer &tok, const TokenLogprobs &e);
 
 // A --presence-penalty / --frequency-penalty value: a number in [-kMaxPenalty, kMaxPenalty] (throws otherwise).
 float parsePenalty(const std::string &flag, const std::string &value);

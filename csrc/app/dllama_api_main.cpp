@@ -11,6 +11,7 @@
 #include "api_server.hpp"
 #include <sys/prctl.h>
 
+#include "../cuda/engine_api.h"
 #include "native_engine.hpp"
 #include "tp_job.hpp"
 
@@ -52,6 +53,27 @@ struct EngineBackend : InferenceBackend {
     }
     std::vector<int32_t> slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask) override {
         return e.slotsStep(tokens, pos, activeMask);
+    }
+    // log-probabilities: one GPU only (the vocabulary is sliced over the ranks of a --gpus N job)
+    void setLogprobs(int k) override {
+        if (k >= 0 && e.nRanks() > 1) throw std::runtime_error("logprobs are not supported under tensor parallelism yet");
+        e.setLogprobs(k);
+    }
+    std::vector<TokenLogprobs> lastLogprobs() override {
+        const std::vector<int32_t> &w = e.logprobsBlocks();
+        std::vector<TokenLogprobs> out;
+        for (size_t r = 0; r + kApiLogprobsWords <= w.size(); r += kApiLogprobsWords) out.push_back(decodeLogprobs(w.data() + r));
+        return out;
+    }
+    void slotLogprobs(uint32_t slot, int k) override { e.slotLogprobs(slot, k); }
+    std::vector<int32_t> slotsStepLogprobs(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask,
+                                           std::vector<TokenLogprobs> &rows) override {
+        std::vector<int32_t> blocks;
+        std::vector<int32_t> out = e.slotsStepLogprobs(tokens, pos, activeMask, blocks);
+        rows.assign(out.size(), TokenLogprobs());
+        for (size_t s = 0; s < out.size(); s++)
+            if (blocks[s * kApiLogprobsWords + 2] >= 0) rows[s] = decodeLogprobs(blocks.data() + s * kApiLogprobsWords);
+        return out;
     }
 };
 

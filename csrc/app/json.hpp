@@ -15,6 +15,7 @@ struct JsonValue {
     enum Kind { Null, Bool, Number, String, Array, Object } kind = Null;
     bool b = false;
     double num = 0;
+    bool integral = false;   // Number written without a fraction or exponent (`1`, not `1.0`)
     std::string str;
     std::vector<JsonValue> arr;
     std::vector<std::pair<std::string, JsonValue>> obj;   // insertion order kept
@@ -165,6 +166,7 @@ private:
             v.num = std::strtod(start, &end);
             if (end == start) fail("unexpected character");
             v.kind = JsonValue::Number;
+            v.integral = std::string(start, (size_t)(end - start)).find_first_of(".eE") == std::string::npos;
             p_ += (size_t)(end - start);
         }
         return v;

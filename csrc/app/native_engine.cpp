@@ -406,6 +406,7 @@ int32_t NativeEngine::stepGreedy(int32_t token, uint32_t pos) {
         setInputs(&token, 1, pos, false);
     }
     engCheck(dl_engine_decode_graph(I.engine, 1, I.stream), "dl_engine_decode_graph");
+    if (lpK_ >= 0) logprobsAfterDraw(1, 1u, 0, 0);
     int32_t next = 0;   // the arg-max kernel leaves the sampled token in tokens[0] (and advances pos[0]) on the device
     cudaCheck(cudaMemcpyAsync(&next, I.tokens, 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(token)");
     cudaCheck(cudaStreamSynchronize(I.stream), "stepGreedy");
@@ -421,6 +422,7 @@ int32_t NativeEngine::stepSampled(int32_t token, uint32_t pos, float temperature
     setInputs(&token, 1, pos, false);
     forward(1, 1, false);
     engCheck(dl_engine_sample(I.engine, temperature, topp, I.stream), "dl_engine_sample");
+    if (lpK_ >= 0) logprobsAfterDraw(1, 1u, 0, kLogprobsControlled);
     int32_t next = 0;   // the sampler leaves the drawn token in tokens[0]
     cudaCheck(cudaMemcpyAsync(&next, I.tokens, 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(token)");
     cudaCheck(cudaStreamSynchronize(I.stream), "stepSampled");
@@ -453,6 +455,7 @@ std::vector<int32_t> NativeEngine::choicesFirst(int32_t token, uint32_t P, uint3
     forward(1, 1, false);
     const uint32_t nb = choiceBatch(n), mask = ((1u << nb) - 1u) & ~((1u << n) - 1u);
     engCheck(dl_engine_sample_rows(I.engine, (int)nb, mask, temperature, topp, 1, I.stream), "dl_engine_sample_rows");
+    if (lpK_ >= 0) logprobsAfterDraw(n, (1u << n) - 1u, 1, kLogprobsControlled | kLogprobsSharedRow);
     std::vector<int32_t> out(n);
     cudaCheck(cudaMemcpyAsync(out.data(), I.tokens, n * 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(tokens)");
     cudaCheck(cudaStreamSynchronize(I.stream), "choicesFirst");
@@ -472,6 +475,7 @@ std::vector<int32_t> NativeEngine::choicesStep(const std::vector<int32_t> &token
     cudaCheck(cudaMemcpyAsync(I.pos, p.data(), nb * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(pos)");
     engCheck(dl_engine_choices_forward(I.engine, (int)nb, P, C, j, mask, I.stream), "dl_engine_choices_forward");
     engCheck(dl_engine_sample_rows(I.engine, (int)nb, mask, temperature, topp, 0, I.stream), "dl_engine_sample_rows");
+    if (lpK_ >= 0) logprobsAfterDraw(n, activeMask & ((1u << n) - 1u), 1, kLogprobsControlled);
     std::vector<int32_t> out(n);
     cudaCheck(cudaMemcpyAsync(out.data(), I.tokens, n * 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(tokens)");
     cudaCheck(cudaStreamSynchronize(I.stream), "choicesStep");
@@ -514,6 +518,54 @@ std::vector<int32_t> NativeEngine::slotsStep(const std::vector<int32_t> &tokens,
     std::vector<int32_t> out(slots_, -1);
     const uint32_t inactive = ~activeMask & ((1u << slots_) - 1u);
     engCheck(dl_engine_slots_step(impl_->engine, tokens.data(), pos.data(), inactive, out.data(), impl_->stream), "dl_engine_slots_step");
+    return out;
+}
+
+static constexpr size_t kLogprobsRows = 8;   // the widest draw: one row per choice or slot
+
+void NativeEngine::logprobsAfterDraw(uint32_t rows, uint32_t rowMask, int firstRow, int flags) {
+    if (nRanks_ > 1) throw std::runtime_error("logprobs are not supported under tensor parallelism yet");
+    Impl &I = *impl_;
+    if (!lpDev_) lpDev_ = (int32_t *)dev(kLogprobsRows * kApiLogprobsWords * sizeof(int32_t));
+    const std::vector<int32_t> k(rows, lpK_);
+    engCheck(dl_engine_logprobs(I.engine, (int)rows, rowMask, k.data(), firstRow, flags, lpDev_, I.stream), "dl_engine_logprobs");
+    lpHost_.assign((size_t)rows * kApiLogprobsWords, 0);
+    cudaCheck(cudaMemcpyAsync(lpHost_.data(), lpDev_, lpHost_.size() * 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(logprobs)");
+}
+
+void NativeEngine::logprobsHostDraw(int32_t token, uint32_t n, const std::vector<float> &bias, const std::vector<uint32_t> &counts, float presence,
+                                    float frequency) {
+    if (nRanks_ > 1) throw std::runtime_error("logprobs are not supported under tensor parallelism yet");
+    Impl &I = *impl_;
+    if (!lpDev_) lpDev_ = (int32_t *)dev(kLogprobsRows * kApiLogprobsWords * sizeof(int32_t));
+    // scratch: chosen id, then the bias and counts rows of the host sampler (uploaded only when it has controls)
+    const size_t V = h_.vocabSize;
+    if (!lpScratch_) lpScratch_ = (uint8_t *)dev(16 + 8 * V);
+    int32_t *chosen = (int32_t *)lpScratch_;
+    float *biasDev = bias.empty() ? nullptr : (float *)(lpScratch_ + 16);
+    uint32_t *countsDev = counts.empty() ? nullptr : (uint32_t *)(lpScratch_ + 16 + 4 * V);
+    cudaCheck(cudaMemcpyAsync(chosen, &token, 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(logprobs)");
+    if (biasDev) cudaCheck(cudaMemcpyAsync(biasDev, bias.data(), std::min(bias.size(), V) * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(bias)");
+    if (countsDev) cudaCheck(cudaMemcpyAsync(countsDev, counts.data(), std::min(counts.size(), V) * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(counts)");
+    const int k = lpK_;
+    engCheck(dl_logprobs_rows(I.logits, 0, std::min<uint32_t>(n, h_.vocabSize), 1, 1u, &k, chosen, biasDev, 0, countsDev, 0, presence, frequency,
+                              nullptr, lpDev_, I.stream), "dl_logprobs_rows");
+    lpHost_.assign(kApiLogprobsWords, 0);
+    cudaCheck(cudaMemcpyAsync(lpHost_.data(), lpDev_, lpHost_.size() * 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(logprobs)");
+    cudaCheck(cudaStreamSynchronize(I.stream), "logprobs");   // the host vectors are read by the copies above
+}
+
+void NativeEngine::slotLogprobs(uint32_t slot, int k) { engCheck(dl_engine_slot_logprobs(impl_->engine, slot, k), "dl_engine_slot_logprobs"); }
+
+std::vector<int32_t> NativeEngine::slotsStepLogprobs(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask,
+                                                     std::vector<int32_t> &blocks) {
+    if (tokens.size() != slots_ || pos.size() != slots_) throw std::runtime_error("slotsStep: one token and position per slot");
+    std::vector<int32_t> out(slots_, -1);
+    blocks.assign((size_t)slots_ * kApiLogprobsWords, 0);
+    for (uint32_t b = 0; b < slots_; b++) blocks[(size_t)b * kApiLogprobsWords + 2] = -1;   // rows the step leaves alone keep k = -1
+    const uint32_t inactive = ~activeMask & ((1u << slots_) - 1u);
+    engCheck(dl_engine_slots_step_logprobs(impl_->engine, tokens.data(), pos.data(), inactive, out.data(), blocks.data(), impl_->stream),
+             "dl_engine_slots_step_logprobs");
     return out;
 }
 

@@ -88,6 +88,19 @@ public:
     void slotSampling(uint32_t slot, uint64_t seed, float temperature, float topp, float presence, float frequency,
                       const std::vector<std::pair<int32_t, float>> &bias);
     std::vector<int32_t> slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask);
+    // Log-probabilities (csrc/cuda/logprobs.cu, one GPU): setLogprobs(k) makes the following stepGreedy / stepSampled / choicesFirst /
+    // choicesStep also compute them for their draws (k top entries, -1: off); logprobsBlocks() holds the result blocks of the last
+    // such call, kApiLogprobsWords int32 words per row (engine_api.h). logprobsHostDraw computes them for a token a host Sampler drew
+    // from the logits of the last step() (its bias and its counts after the draw are uploaded). slotsStepLogprobs is slotsStep that
+    // also fills `blocks` ([slots][kApiLogprobsWords]) for the active slots whose logprobs are on (slotLogprobs).
+    void setLogprobs(int k) { lpK_ = k; }
+    int logprobs() const { return lpK_; }
+    const std::vector<int32_t> &logprobsBlocks() const { return lpHost_; }
+    void logprobsHostDraw(int32_t token, uint32_t n, const std::vector<float> &bias, const std::vector<uint32_t> &counts, float presence,
+                          float frequency);
+    void slotLogprobs(uint32_t slot, int k);
+    std::vector<int32_t> slotsStepLogprobs(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask,
+                                           std::vector<int32_t> &blocks);
     // n greedy steps back to back on the device without host round trips; returns the generated tokens.
     std::vector<int32_t> decodeGreedy(int32_t firstToken, uint32_t pos, uint32_t nSteps);
     void synchronize();
@@ -106,6 +119,12 @@ private:
     void uploadWeights(const uint8_t *file);
     void setInputs(const int32_t *tokens, uint32_t n, uint32_t pos, bool prefillBuffers);
     void forward(uint32_t n, int logitsMode, bool greedyAdvance);
+    void logprobsAfterDraw(uint32_t rows, uint32_t rowMask, int firstRow, int flags);   // enqueue + copy the blocks, before the sync
+
+    int lpK_ = -1;
+    int32_t *lpDev_ = nullptr;
+    uint8_t *lpScratch_ = nullptr;
+    std::vector<int32_t> lpHost_;
 
     ModelHeader h_;
     std::vector<TensorEntry> dir_;

@@ -137,7 +137,17 @@ struct TpEngine {
         if (engine.nRanks() > 1) return stepSampled(token, pos, sampler);
         const float *logits = engine.step(token, pos);
         hostLogits.assign(logits, logits + sampler.vocabSize());
-        return sampler.sample(hostLogits.data());
+        const int32_t t = sampler.sample(hostLogits.data());
+        if (engine.logprobs() >= 0) {   // the device kernel on the device logits, with this sampler's controls
+            std::vector<float> bias;
+            if (sampler.controlsActive() && !sampler.logitBias().empty()) {
+                bias.assign(sampler.vocabSize(), 0.f);
+                for (const auto &b : sampler.logitBias()) bias[(size_t)b.first] = b.second;
+            }
+            engine.logprobsHostDraw(t, sampler.vocabSize(), bias, sampler.controlsActive() ? sampler.counts() : std::vector<uint32_t>(),
+                                    sampler.presencePenalty(), sampler.frequencyPenalty());
+        }
+        return t;
     }
     // temperature / top-p on the device (the logits stay sharded); `sampler` only supplies the parameters and the seed
     int32_t stepSampled(int32_t token, uint32_t pos, Sampler &sampler) {

@@ -18,6 +18,7 @@ namespace dl {
 uint32_t gHiddenAct = 0;
 
 static_assert(kApiMaxRanks == kMaxRanks, "engine_api.h and kernels.h disagree on the rank limit");
+static_assert(kApiLogprobsWords == kLogprobsWords && kApiLogprobsMaxTop == kLogprobsMaxTop, "engine_api.h and kernels.h disagree on logprobs");
 
 struct Engine {
     EngineConfig cfg{};
@@ -61,6 +62,8 @@ struct Engine {
     float *slotBias = nullptr;         // [kChoiceRngSlots][vocabFull] per-slot logit bias
     int32_t *slotStage = nullptr;      // pinned [3][kChoiceRngSlots]: tokens, positions in; drawn tokens out
     cudaEvent_t slotStaged = nullptr;  // the uploads of the staged tokens / positions are done: the buffer may be rewritten
+    int slotLogprobs[8] = {-1, -1, -1, -1, -1, -1, -1, -1};   // per-slot top_logprobs k (-1: no logprobs), one per slot
+    int32_t *slotLpDev = nullptr, *slotLpHost = nullptr;   // [kChoiceRngSlots][kLogprobsWords] results of a slots step (device, pinned)
     bool prefillFusedAr = false; // TP prefill: GEMM + all-reduce in one kernel (DL_PREFILL_FUSED_AR=1) instead of GEMM, then all-reduce kernel
     bool tcAttn = true;          // prefill attention on the tensor cores (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
     bool fusedAttn = true, fusedArgmax = true, useTma = true;   // debugging switches (DL_NO_FUSED_ATTN / DL_NO_FUSED_ARGMAX / DL_NO_TMA)
@@ -443,6 +446,7 @@ using dl::Engine;
 
 // rngState: [0] = single-sequence generator, [kChoiceRngSlots + b] = generator of choice b
 constexpr uint32_t kChoiceRngSlots = 8;
+static_assert(sizeof(Engine::slotLogprobs) == kChoiceRngSlots * sizeof(int), "one logprobs setting per slot");
 
 DL_EXPORT void *dl_engine_create(const dl::EngineConfig *cfg) {
     if (cfg->kvType > 1 || (cfg->kvType == 1 && cfg->headDim % 32)) return nullptr;   // unknown KV-cache storage
@@ -480,6 +484,8 @@ DL_EXPORT void dl_engine_destroy(void *h) {
     if (e->slotBias) cudaFree(e->slotBias);
     if (e->slotStage) cudaFreeHost(e->slotStage);
     if (e->slotStaged) cudaEventDestroy(e->slotStaged);
+    if (e->slotLpDev) cudaFree(e->slotLpDev);
+    if (e->slotLpHost) cudaFreeHost(e->slotLpHost);
     delete e;
 }
 
@@ -726,6 +732,23 @@ DL_EXPORT int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, floa
                                 flagLocal, e->gatherEpoch, nR, stream, ctl);
 }
 
+// Log-probabilities of the tokens the last step drew (logprobs.cu), enqueued on `stream` behind the draw: row b of the last
+// forward's logits (every row reads logits[0] with kLogprobsSharedRow: the choices' first draw) and the token in tokens[b], for
+// the rows set in rowMask (b < rows), with k[b] (host, 0..20) top entries. kLogprobsControlled: the logits are transformed by the
+// sampling controls the draw used, with count row firstRow + b (0: single sequence, 1 + b: choice b). out: device int32
+// [rows][kLogprobsWords]. Single GPU only. flags: dl::kLogprobsControlled, dl::kLogprobsSharedRow (engine_api.h).
+
+DL_EXPORT int dl_engine_logprobs(void *h, int rows, uint32_t rowMask, const int32_t *k, int firstRow, int flags, int32_t *out, cudaStream_t stream) {
+    Engine *e = (Engine *)h;
+    const dl::EngineConfig &c = e->cfg;
+    if (e->comm.nRanks > 1) return -70;
+    if (rows < 1 || (uint32_t)rows > c.maxBatch || firstRow < 0 || (uint32_t)(firstRow + rows) > 1 + kChoiceRngSlots) return -10;
+    dl::SampleControls ctlArgs;
+    const dl::SampleControls *ctl = (flags & dl::kLogprobsControlled) ? activeControls(e, (uint32_t)firstRow, ctlArgs) : nullptr;
+    return dl::launchLogprobsRows(e->g.logits, (flags & dl::kLogprobsSharedRow) ? 0u : c.vocab, dl::localVocabLimit(*e), (uint32_t)rows, rowMask, k,
+                                  e->g.tokens, out, stream, ctl);
+}
+
 DL_EXPORT int dl_engine_set_comm(void *h, const dl::CommPtrs *p) {
     ((Engine *)h)->comm = *p;
     return 0;
@@ -954,6 +977,7 @@ DL_EXPORT int dl_engine_slot_sampling(void *h, uint32_t slot, unsigned long long
     DL_CUDA_CHECK(cudaMemcpyAsync(e->slotBias + (size_t)slot * full, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
     DL_CUDA_CHECK(cudaMemsetAsync(e->ctlCounts + (size_t)(1 + slot) * full, 0, (size_t)full * sizeof(uint32_t), stream));
     DL_CUDA_CHECK(cudaStreamSynchronize(stream));   // host temporaries
+    e->slotLogprobs[slot] = -1;   // a new sequence starts without logprobs (dl_engine_slot_logprobs)
     return 0;
 }
 
@@ -989,9 +1013,22 @@ DL_EXPORT int dl_engine_slots_forward(void *h, const int32_t *tokens, const int3
     return dl::engineForward(*e, nb, 2, false, stream, nullptr, &sl);
 }
 
+// Log-probabilities of slot `slot`'s draws in dl_engine_slots_step_logprobs: k (0..20) top entries, -1: none (the default).
+DL_EXPORT int dl_engine_slot_logprobs(void *h, uint32_t slot, int k) {
+    Engine *e = (Engine *)h;
+    if (e->slots < 2 || slot >= e->slots) return -64;
+    if (k < -1 || k > dl::kLogprobsMaxTop) return -67;
+    e->slotLogprobs[slot] = k;
+    return 0;
+}
+
 // dl_engine_slots_forward, then every active row draws its next token with its slot's settings (dl_engine_slot_sampling) into
 // out[b]; inactive rows leave out[b] as it was. One device-to-host copy for all rows; returns once the tokens are on the host.
-DL_EXPORT int dl_engine_slots_step(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, cudaStream_t stream) {
+// lpOut (host int32 [slots][kLogprobsWords], may be null): an active row whose slot has logprobs on (dl_engine_slot_logprobs) also
+// gets the log-probabilities of its draw there (kernels.h: launchLogprobsRows), computed behind the draw and copied out with the
+// tokens; other rows of lpOut are left as they were, and without such a row nothing more runs.
+DL_EXPORT int dl_engine_slots_step_logprobs(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, int32_t *lpOut,
+                                            cudaStream_t stream) {
     Engine *e = (Engine *)h;
     DL_TRY(dl_engine_slots_forward(h, tokens, pos, inactiveMask, stream));
     const dl::EngineConfig &c = e->cfg;
@@ -1002,9 +1039,27 @@ DL_EXPORT int dl_engine_slots_step(void *h, const int32_t *tokens, const int32_t
     const dl::SampleControls ctl{e->slotBias, e->ctlCounts + c.vocab, c.vocab, 0.f, 0.f, c.vocab};
     DL_TRY(dl::launchSampleRows(e->g.logits, c.vocab, e->probScratch, n, 0.f, 0.f, e->rngState + kChoiceRngSlots, e->g.tokens, (uint32_t)nb, mask,
                                 nullptr, nullptr, 1, stream, &ctl, e->slotParams));
+    uint32_t lpMask = 0;
+    int lpK[kChoiceRngSlots] = {};
+    for (uint32_t b = 0; lpOut && b < e->slots; b++)
+        if (!((mask >> b) & 1u) && e->slotLogprobs[b] >= 0) { lpMask |= 1u << b; lpK[b] = e->slotLogprobs[b]; }
+    if (lpMask) {
+        if (!e->slotLpDev) {
+            DL_CUDA_CHECK(cudaMalloc(&e->slotLpDev, kChoiceRngSlots * dl::kLogprobsWords * sizeof(int32_t)));
+            DL_CUDA_CHECK(cudaHostAlloc((void **)&e->slotLpHost, kChoiceRngSlots * dl::kLogprobsWords * sizeof(int32_t), cudaHostAllocDefault));
+        }
+        DL_TRY(dl::launchLogprobsRows(e->g.logits, c.vocab, n, (uint32_t)nb, lpMask, lpK, e->g.tokens, e->slotLpDev, stream, &ctl, e->slotParams));
+        DL_CUDA_CHECK(cudaMemcpyAsync(e->slotLpHost, e->slotLpDev, (size_t)nb * dl::kLogprobsWords * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+    }
     int32_t *drawn = e->slotStage + 2 * kChoiceRngSlots;
     DL_CUDA_CHECK(cudaMemcpyAsync(drawn, e->g.tokens, nb * sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
     DL_CUDA_CHECK(cudaStreamSynchronize(stream));
     for (uint32_t b = 0; b < e->slots; b++) if (!((mask >> b) & 1u)) out[b] = drawn[b];
+    for (uint32_t b = 0; b < e->slots; b++)
+        if ((lpMask >> b) & 1u) std::memcpy(lpOut + b * dl::kLogprobsWords, e->slotLpHost + b * dl::kLogprobsWords, dl::kLogprobsWords * sizeof(int32_t));
     return 0;
+}
+
+DL_EXPORT int dl_engine_slots_step(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, cudaStream_t stream) {
+    return dl_engine_slots_step_logprobs(h, tokens, pos, inactiveMask, out, nullptr, stream);
 }

@@ -7,6 +7,9 @@
 namespace dl {
 
 constexpr int kApiMaxRanks = 8;
+constexpr int kApiLogprobsWords = 44;   // int32 words of one row's log-probabilities (dl_engine_logprobs)
+constexpr int kApiLogprobsMaxTop = 20;
+constexpr int kLogprobsControlled = 1, kLogprobsSharedRow = 2;   // dl_engine_logprobs flags
 
 struct EngineConfig {   // mirrored by ctypes in distributed_llama_b200/ops/cuda_lib.py
     uint32_t dim, nLayers, nHeads, nKvHeads, headDim, ffDim, vocab, seqLen;   // per-rank (sliced) head/ff/vocab counts
@@ -112,6 +115,17 @@ int dl_engine_slot_sampling(void *h, uint32_t slot, unsigned long long seed, flo
                             const int32_t *ids, const float *vals, int nBias, cudaStream_t stream);
 int dl_engine_slots_forward(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, cudaStream_t stream);
 int dl_engine_slots_step(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, cudaStream_t stream);
+// per-token log-probabilities (csrc/cuda/logprobs.cu): results are int32 blocks of kLogprobsWords words per row,
+// {chosen id, its logprob (f32 bits), k, 0, k x (id, logprob bits)} in the order (logprob desc, id asc); flags: bit 0 = the
+// sampling controls of the last draw apply, bit 1 = every row reads logits row 0 (the choices' first draw)
+int dl_engine_logprobs(void *h, int rows, uint32_t rowMask, const int32_t *k, int firstRow, int flags, int32_t *out, cudaStream_t stream);
+int dl_engine_slot_logprobs(void *h, uint32_t slot, int k);
+// the kernel on explicit device buffers (csrc/cuda/logprobs.cu: counts are those after the draws of chosen[b])
+int dl_logprobs_rows(const float *logits, uint32_t logitsStride, uint32_t n, uint32_t B, uint32_t rowMask, const int *k, const int *chosen,
+                     const float *bias, uint32_t biasStride, uint32_t *counts, uint32_t countsStride, float presence, float frequency,
+                     const float *rowParams, int32_t *out, cudaStream_t stream);   // k = -1: off (every dl_engine_slot_sampling resets it)
+int dl_engine_slots_step_logprobs(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, int32_t *lpOut,
+                                  cudaStream_t stream);
 int dl_engine_set_trace(void *h, uint64_t *buf, uint32_t capLaunches);
 int dl_engine_set_trace_all(void *h, int allCtas);
 uint32_t dl_engine_num_sms(void *h);

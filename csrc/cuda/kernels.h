@@ -304,6 +304,17 @@ struct SampleControls {
     float presence, frequency;
     uint32_t biasStride;      // row b's bias at bias + b * biasStride (0: one bias for every row)
 };
+// The controls' transform of logit i; explicit roundings because the library is built with --use_fast_math. `drawn`: an id whose
+// count holds one draw to leave out (the log-probabilities read a row's counts after its draw incremented them), -1: none.
+__device__ __forceinline__ float controlled(const SampleControls &c, float x, uint32_t i, int drawn = -1) {
+    if (c.bias) x = __fadd_rn(x, c.bias[i]);
+    if (c.counts) {
+        uint32_t k = c.counts[i];
+        if ((int)i == drawn && k > 0) k--;
+        if (k > 0) x = __fsub_rn(__fsub_rn(x, __fmul_rn((float)k, c.frequency)), c.presence);
+    }
+    return x;
+}
 int launchSample(const float *logits, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng, int *tokenOut, int *pos,
                  int *history, uint32_t historyCap, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
                  cudaStream_t stream, const SampleControls *controls = nullptr);
@@ -316,6 +327,17 @@ int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t 
 int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
                      int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
                      cudaStream_t stream, const SampleControls *controls = nullptr, const float *rowParams = nullptr);
+
+// Per-token log-probabilities (logprobs.cu): logprob(i) = x[i] - logsumexp(x[0..n)) of the row that drew token chosen[b], where x
+// is the logits row after the controls (the values the sampler draws from, before temperature). One CTA per row b < B whose bit
+// is set in rowMask; other rows read nothing. Row b reads logits + b * logitsStride (0: every row reads one row), its controls as
+// launchSampleRows does (rowParams: per-row penalties at [b][2..3]) with its counts read after the draw, and writes kLogprobsWords
+// int32 words at out + b * kLogprobsWords: {chosen id, its logprob (f32 bits), k, 0, then k (id, logprob bits) pairs}: the k[b]
+// largest logprobs in the order (value desc, id asc). The chosen token's logprob is bitwise its value in that list.
+constexpr int kLogprobsMaxTop = 20;
+constexpr int kLogprobsWords = 4 + 2 * kLogprobsMaxTop;
+int launchLogprobsRows(const float *logits, uint32_t logitsStride, uint32_t n, uint32_t B, uint32_t rowMask, const int *k, const int *chosen,
+                       int32_t *out, cudaStream_t stream, const SampleControls *controls = nullptr, const float *rowParams = nullptr);
 
 // Persistent decode kernel (mega_decode.cu)
 struct MegaLayer {

@@ -43,16 +43,6 @@ struct SampleArgs {
     const float *rowParams;    // [B][4] per-row {temperature, top-p, presence, frequency}, or null (launchSampleRows)
 };
 
-// The controls' transform of one logit (kernels.h); explicit roundings because the library is built with --use_fast_math.
-__device__ __forceinline__ float controlled(const SampleControls &c, float x, uint32_t i) {
-    if (c.bias) x = __fadd_rn(x, c.bias[i]);
-    if (c.counts) {
-        const uint32_t k = c.counts[i];
-        if (k > 0) x = __fsub_rn(__fsub_rn(x, __fmul_rn((float)k, c.frequency)), c.presence);
-    }
-    return x;
-}
-
 __device__ float blockMax(float v, float *red) {
     v = warpMax(v);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;

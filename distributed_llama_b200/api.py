@@ -32,10 +32,21 @@ class GenerationStats:
 
 
 MAX_CHOICES = 8   # the engine's widest batch: one row per choice
+MAX_TOP_LOGPROBS = 20   # the largest `top_logprobs` (csrc/cuda/logprobs.cu)
+
+
+def check_logprobs(k: int, n_ranks: int = 1) -> None:
+    """Raises ValueError unless log-probabilities with k top entries can run here: 0 <= k <= 20, one GPU (under tensor
+    parallelism the vocabulary is sliced over the ranks)."""
+    if isinstance(k, bool) or not isinstance(k, int) or not 0 <= k <= MAX_TOP_LOGPROBS:
+        raise ValueError(f"top_logprobs must be an integer from 0 to {MAX_TOP_LOGPROBS}")
+    if n_ranks > 1:
+        raise ValueError("logprobs are not supported under tensor parallelism yet")
 
 
 def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: int, sampler, base_seed: int,
-                on_token: Callable[[int, int], bool]) -> List[List[int]]:
+                on_token: Callable[[int, int], bool], logprobs: Optional[int] = None,
+                on_logprobs: Optional[Callable[[int, tuple], None]] = None) -> List[List[int]]:
     """Generates n completions of one prompt whose last token `token` sits at position P, everything before it prefilled.
 
     Choice i draws with an xorshift* generator seeded with choice_seed(base_seed, i); its j-th token has rotary position
@@ -50,10 +61,16 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     next_token(token, pos, sampler), forget_device_seed(), save_sampler() / restore_sampler(saved), and for the batched path
     batched_choices(n), seed_choices(seeds), choice_controls(sampler, n), choices_first(token, P, n, T, topp) and
     choices_step(tokens, P, C, j, active, T, topp) (InferenceSession and apps.runtime.RootInference). Returns each choice's
-    tokens."""
+    tokens.
+
+    logprobs = k (0..20): on_logprobs(i, entry) is called right before on_token(i, tok) with the entry of that token,
+    (tok, logprob, [(id, logprob), ...] k most likely); the backend's next_token, choices_first and choices_step then take a
+    `logprobs=k` keyword and last_logprobs() returns the entries of their last call, one per row. The tokens are the same as
+    without it."""
     H = host()
     if not 1 <= n <= MAX_CHOICES:
         raise ValueError(f"n must be between 1 and {MAX_CHOICES}")
+    lp = {} if logprobs is None else {"logprobs": logprobs}
     C = (seq_len - 1 - P) // n
     limit = seq_len - P if n == 1 else C
     if max_tokens > 0:
@@ -67,11 +84,14 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
         # today's single-sequence path from P; rows past P belong to this sequence until the next one overwrites them
         tok, pos, done = token, P, set()
         while len(out[choices[0]]) < limit:
-            tok = backend.next_token(tok, pos, smp)
+            tok = backend.next_token(tok, pos, smp, **lp)
+            entry = backend.last_logprobs()[0] if lp else None
             pos += 1
             for i in choices:
                 if i not in done:
                     out[i].append(tok)
+                    if lp:
+                        on_logprobs(i, entry)
                     if on_token(i, tok):
                         done.add(i)
             if len(done) == len(choices):
@@ -96,18 +116,21 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
         return out
     backend.seed_choices(seeds)
     backend.choice_controls(sampler, n)
-    last = backend.choices_first(token, P, n, T, topp)
+    last = backend.choices_first(token, P, n, T, topp, **lp)
     active = [True] * n
     j = 0
     while True:
+        entries = backend.last_logprobs() if lp else None
         for i in range(n):
             if active[i]:
                 out[i].append(last[i])
+                if lp:
+                    on_logprobs(i, entries[i])
                 if on_token(i, last[i]) or len(out[i]) >= limit:
                     active[i] = False
         if not any(active):
             break
-        last = backend.choices_step(last, P, C, j, active, T, topp)
+        last = backend.choices_step(last, P, C, j, active, T, topp, **lp)
         j += 1
     return out
 
@@ -138,12 +161,18 @@ class SlotRequest:
     engine thread.
 
     n: completions; temperature / topp / presence / frequency / bias: the sampling settings; seed: the request's seed or None;
-    max_tokens (<= 0: no limit but the slot's context)."""
+    max_tokens (<= 0: no limit but the slot's context); logprobs: k (0..20) top entries of the log-probabilities of every
+    token, passed to on_logprobs, or None."""
     n = 1
     temperature, topp, presence, frequency = 0.0, 0.9, 0.0, 0.0
     bias: Sequence = ()
     seed: Optional[int] = None
     max_tokens = -1
+    logprobs: Optional[int] = None
+
+    def on_logprobs(self, i: int, entry: tuple) -> None:
+        """With logprobs set: the entry (token, logprob, [(id, logprob), ...]) of completion i's next token, right before
+        on_token is called with that token."""
 
     def cached_prefix(self, slot: int) -> int:
         """How many of the request's messages slot `slot`'s prompt cache covers (slot choice; ties go to the lowest index)."""
@@ -180,7 +209,8 @@ class SlotScheduler:
 
     `backend` provides slots, slot_len, slot_prefill(slot, tokens, pos), slot_copy(src, dst, P),
     slot_sampling(slot, seed, temperature, topp, presence, frequency, bias) and slots_step(tokens, pos, active)
-    (InferenceSession(parallel=N))."""
+    (InferenceSession(parallel=N)); for requests with logprobs also slot_logprobs(slot, k) and slots_step_logprobs(tokens, pos,
+    active) -> (draws, per-slot entries), used only while such a request holds a slot."""
 
     def __init__(self, backend, seed_source: Callable[[], int]):
         self.backend = backend
@@ -221,6 +251,8 @@ class SlotScheduler:
         seeds = [seed] if req.n == 1 else [host().choice_seed(seed, i) for i in range(len(slots))]
         for s, sd in zip(slots, seeds):
             be.slot_sampling(s, sd, req.temperature, req.topp, req.presence, req.frequency, req.bias)
+            if req.logprobs is not None:
+                be.slot_logprobs(s, req.logprobs)
         limit = be.slot_len - P
         if req.max_tokens > 0:
             limit = min(limit, req.max_tokens)
@@ -265,7 +297,12 @@ class SlotScheduler:
             active = [r is not None for r in rows]
             if not any(active):
                 continue
-            drawn = be.slots_step([r["token"] if r else 0 for r in rows], [r["pos"] if r else 0 for r in rows], active)
+            args = ([r["token"] if r else 0 for r in rows], [r["pos"] if r else 0 for r in rows], active)
+            entries = None
+            if any(r is not None and r["job"]["req"].logprobs is not None for r in rows):
+                drawn, entries = be.slots_step_logprobs(*args)
+            else:
+                drawn = be.slots_step(*args)
             for s in range(N):
                 r = rows[s]
                 if r is None:
@@ -278,6 +315,8 @@ class SlotScheduler:
                         if i in r["done"]:
                             continue
                         job["out"][i].append(tok)
+                        if entries is not None and req.logprobs is not None:
+                            req.on_logprobs(i, entries[s])
                         if req.on_token(i, tok) or len(job["out"][i]) >= job["limit"]:
                             r["done"].add(i)
                 except Exception as e:
@@ -352,6 +391,12 @@ class InferenceSession:
     def slots_step(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]) -> List[int]:
         return self.engine.slots_step(tokens, pos, active)
 
+    def slot_logprobs(self, slot: int, k: Optional[int]) -> None:
+        self.engine.slot_logprobs(slot, k)
+
+    def slots_step_logprobs(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]):
+        return self.engine.slots_step_logprobs(tokens, pos, active)
+
     # ---- token level ----
     def reset(self):
         self.pos = 0
@@ -367,12 +412,16 @@ class InferenceSession:
         self.pos += 1
         return lg
 
-    def next_token(self, token: int, pos: Optional[int] = None, sampler=None) -> int:
+    def next_token(self, token: int, pos: Optional[int] = None, sampler=None, logprobs: Optional[int] = None) -> int:
         """One decode step with host-visible result: H2D (token,pos) from pinned memory, forward + sampling, D2H. `pos` and
-        `sampler` default to the session's own; run_choices passes its own, as it does to apps.runtime.RootInference."""
+        `sampler` default to the session's own; run_choices passes its own, as it does to apps.runtime.RootInference.
+        logprobs = k (0..20): also computes the log-probabilities of the drawn token and the k most likely ones on the device,
+        from the same logits the draw saw (last_logprobs()); the token is the same as without it."""
         if pos is not None:
             self.pos = pos
         smp = self.sampler if sampler is None else sampler
+        if logprobs is not None:
+            check_logprobs(logprobs, self.comm.world_size if self.comm is not None else 1)
         if smp.temperature == 0.0 and not smp.controls_active:
             self._pin_in[0] = token
             self._pin_in[1] = self.pos
@@ -380,10 +429,14 @@ class InferenceSession:
             eng.tokens[:1].copy_(self._pin_in[:1], non_blocking=True)
             eng.pos[:1].copy_(self._pin_in[1:2], non_blocking=True)
             eng.run_decode_step()
+            if logprobs is not None:
+                eng.logprobs([logprobs])
             self._pin_out.copy_(eng.tokens[:1], non_blocking=True)
             torch.cuda.current_stream().synchronize()
             eng.check_abort()
             self.pos += 1
+            if logprobs is not None:
+                self._last_logprobs = eng.read_logprobs()
             return int(self._pin_out[0])
         eng = self.engine
         if self.device.type == "cuda" and not getattr(eng, "_parts", False):
@@ -394,13 +447,27 @@ class InferenceSession:
                 self._dev_seeded = gen
             self._sync_controls(smp)
             eng.step_sampled(token, self.pos, smp.temperature, smp.topp)
+            if logprobs is not None:
+                eng.logprobs([logprobs], controlled=True)
             self._pin_out.copy_(eng.tokens[:1], non_blocking=True)
             torch.cuda.current_stream().synchronize()
             eng.check_abort()
             self.pos += 1
+            if logprobs is not None:
+                self._last_logprobs = eng.read_logprobs()
             return int(self._pin_out[0])
         lg = self.forward_logits(token)
-        return int(smp.sample(lg.float().cpu().numpy()))
+        t = int(smp.sample(lg.float().cpu().numpy()))
+        if logprobs is not None:
+            self._last_logprobs = [eng.logprobs_host_draw(t, logprobs, smp)]
+        return t
+
+    def last_logprobs(self) -> list:
+        """Per row of the last step that was asked for logprobs (next_token: one row; choices_first / choices_step: one per
+        choice, None for inactive ones): (token id, logprob, [(id, logprob), ...] the k most likely in order of logprob desc,
+        id asc). logprob(i) = x[i] - logsumexp(x) over the tokenizer's vocabulary, x the logits after logit_bias and the
+        penalties (before temperature and top-p)."""
+        return self._last_logprobs
 
     def _sync_controls(self, smp):
         """Hands the sampler's controls to the device at the start of each of its completions (count row 0 zeroed)."""
@@ -436,12 +503,18 @@ class InferenceSession:
     def seed_choices(self, seeds: Sequence[int]):
         self.engine.seed_choice_samplers(seeds)
 
-    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float) -> List[int]:
-        return self.engine.choices_first(token, P, n, temperature, topp)
+    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float, logprobs: Optional[int] = None) -> List[int]:
+        out = self.engine.choices_first(token, P, n, temperature, topp, logprobs=logprobs)
+        if logprobs is not None:
+            self._last_logprobs = self.engine.read_logprobs()
+        return out
 
     def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
-                     topp: float) -> List[int]:
-        return self.engine.choices_step(tokens, P, C, j, active, temperature, topp)
+                     topp: float, logprobs: Optional[int] = None) -> List[int]:
+        out = self.engine.choices_step(tokens, P, C, j, active, temperature, topp, logprobs=logprobs)
+        if logprobs is not None:
+            self._last_logprobs = self.engine.read_logprobs()
+        return out
 
     def generate_choices(self, prompt: str, n: int, max_tokens: int, seed: Optional[int] = None) -> List[str]:
         """n completions of `prompt`, each at most max_tokens tokens (and at most its share of the remaining context, see

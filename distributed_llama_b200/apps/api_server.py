@@ -17,7 +17,8 @@ import time
 from typing import Dict, List, Optional, Tuple
 
 from .. import host
-from ..api import MAX_CHOICES, ParallelRefused, SlotRequest, SlotScheduler, parallel_refusal, run_choices
+from ..api import (MAX_CHOICES, MAX_TOP_LOGPROBS, ParallelRefused, SlotRequest, SlotScheduler, check_logprobs, parallel_refusal,
+                   run_choices)
 from .args import AppArgs, parse_args
 from .cli import make_chat_tools
 from .runtime import AppContext, run_inference_app
@@ -154,12 +155,84 @@ def parse_controls(body: dict, vocab: int, presence: float, frequency: float):
     return presence, frequency, sorted(pairs)
 
 
-def chunk_json(delta: Optional[str], stop: bool, index: int = 0) -> str:
+def parse_logprobs(body: dict, n_ranks: int = 1) -> Optional[int]:
+    """The request's log-probabilities: None without them, else the number of top entries. `logprobs` is a boolean (absent:
+    false); `top_logprobs`, an integer from 0 to 20 (absent: 0), is allowed only with `logprobs: true`. Anything else is refused,
+    as is `logprobs: true` under tensor parallelism."""
+    on = body.get("logprobs", False)
+    if not isinstance(on, bool):
+        raise ValueError("'logprobs' must be a boolean")
+    k = body.get("top_logprobs", 0)
+    if "top_logprobs" in body and not on:
+        raise ValueError("'top_logprobs' needs 'logprobs': true")
+    if isinstance(k, bool) or not isinstance(k, int) or not 0 <= k <= MAX_TOP_LOGPROBS:
+        raise ValueError(f"'top_logprobs' must be an integer from 0 to {MAX_TOP_LOGPROBS}")
+    if not on:
+        return None
+    check_logprobs(k, n_ranks)
+    return k
+
+
+def logprob_entry(tokenizer, entry) -> dict:
+    """The response form of one token's log-probabilities (api.run_choices on_logprobs entry): `bytes` are the token's piece,
+    `token` those bytes decoded as UTF-8 with replacement."""
+    def one(t: int, lp: float) -> dict:
+        b = tokenizer.piece(t)
+        return {"token": b.decode("utf-8", errors="replace"), "logprob": lp, "bytes": list(b)}
+    t, lp, top = entry
+    e = one(t, lp)
+    e["top_logprobs"] = [one(i, v) for i, v in top]
+    return e
+
+
+class LogprobsLog:
+    """Entries of the tokens of n choices: all of them for the final JSON, and those not yet sent for the stream. The token that
+    ends a choice by end of sequence gets none."""
+
+    def __init__(self, tokenizer, n: int):
+        self.tokenizer = tokenizer
+        self.next: List[Optional[dict]] = [None] * n
+        self.all: List[List[dict]] = [[] for _ in range(n)]
+        self.pending: List[List[dict]] = [[] for _ in range(n)]
+
+    def on_logprobs(self, i: int, entry) -> None:
+        self.next[i] = logprob_entry(self.tokenizer, entry)
+
+    def consumed(self, i: int, eos: bool) -> None:
+        """Choice i's token (the last one given to on_logprobs) went through on_token; eos: it ended the choice."""
+        if not eos:
+            self.all[i].append(self.next[i])
+            self.pending[i].append(self.next[i])
+        self.next[i] = None
+
+    def take(self, i: int) -> List[dict]:
+        out, self.pending[i] = self.pending[i], []
+        return out
+
+
+def chunk_json(delta: Optional[str], stop: bool, index: int = 0, logprobs: Optional[List[dict]] = None) -> str:
+    """One stream chunk; `logprobs` (a list, possibly empty) adds the entries of the tokens consumed since the last chunk."""
     choice = {"index": index, "finish_reason": "stop" if stop else ""}
     if not stop:
         choice["delta"] = {"role": "assistant", "content": delta}
+        if logprobs is not None:
+            choice["logprobs"] = {"content": logprobs}
     return json.dumps({"id": "cmpl-c0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
                        "choices": [choice]})
+
+
+def write_stream_finish(req: "HttpRequest", i: int, lps: Optional[LogprobsLog]) -> None:
+    """Choice i's stop chunk, after one delta chunk with empty content for log-probability entries still unsent."""
+    if lps and lps.pending[i]:
+        req.write_stream_chunk("data: " + chunk_json("", False, i, lps.take(i)) + "\r\n\r\n")
+    req.write_stream_chunk("data: " + chunk_json(None, True, i) + "\r\n\r\n")
+
+
+def choice_json(i: int, content: str, lps: Optional[LogprobsLog]) -> dict:
+    c = {"index": i, "message": {"role": "assistant", "content": content}, "finish_reason": "stop"}
+    if lps:
+        c["logprobs"] = {"content": lps.all[i]}
+    return c
 
 
 class ApiServer:
@@ -184,6 +257,7 @@ class ApiServer:
         # server defaults: --presence-penalty / --frequency-penalty (argument objects that predate them mean 0)
         presence, frequency, bias = parse_controls(body, smp.vocab_size, getattr(ctx.args, "presence_penalty", 0.0),
                                                    getattr(ctx.args, "frequency_penalty", 0.0))
+        lp_k = parse_logprobs(body, getattr(getattr(inf, "comm", None), "world_size", 1))
         smp.set_controls(presence, frequency, bias)
         messages = [(m["role"], m["content"]) for m in body["messages"]]
         stream = bool(body.get("stream", False))
@@ -206,11 +280,12 @@ class ApiServer:
         decoders = [H.TokenDecoder() for _ in range(n)]
         p = public.decode("utf-8", errors="replace")
         buffers = [p] * n
+        lps = LogprobsLog(tok, n) if lp_k is not None else None
         if stream:
             req.write_stream_start()
             if p:
                 for i in range(n):
-                    req.write_stream_chunk("data: " + chunk_json(p, False, i) + "\r\n\r\n")
+                    req.write_stream_chunk("data: " + chunk_json(p, False, i, lps.take(i) if lps else None) + "\r\n\r\n")
         n_pref = prompt_end - start_pos
         inf.prefill(tokens[:n_pref], start_pos)
         token = tokens[n_pref] if n_pref < len(tokens) else tokens[-1]
@@ -220,17 +295,20 @@ class ApiServer:
             if n == 1 and piece:
                 print(piece.decode("utf-8", errors="replace"), end="", flush=True)
             kind = dets[i].append(t, piece)
+            if lps:
+                lps.consumed(i, kind == H.EOS)
             if kind in (H.NOT_EOS, H.EOS):
                 delta = dets[i].get_delta()
                 if delta:
                     d = delta.decode("utf-8", errors="replace")
                     if stream:
-                        req.write_stream_chunk("data: " + chunk_json(d, False, i) + "\r\n\r\n")
+                        req.write_stream_chunk("data: " + chunk_json(d, False, i, lps.take(i) if lps else None) + "\r\n\r\n")
                     buffers[i] += d
                 dets[i].reset()
             return kind == H.EOS
 
-        out = run_choices(inf, token, prompt_end, n, max_tokens, h.seq_len, smp, base_seed, on_token)
+        out = run_choices(inf, token, prompt_end, n, max_tokens, h.seq_len, smp, base_seed, on_token,
+                          **({"logprobs": lp_k, "on_logprobs": lps.on_logprobs} if lps else {}))
         if n == 1:
             end = prompt_end + len(out[0])
             if end == h.seq_len:
@@ -239,7 +317,7 @@ class ApiServer:
                 self.cache.push(end, ("assistant", buffers[0]))
         if stream:
             for i in range(n):
-                req.write_stream_chunk("data: " + chunk_json(None, True, i) + "\r\n\r\n")
+                write_stream_finish(req, i, lps)
             req.write_stream_chunk("data: [DONE]")
             req.write_stream_end()
         else:
@@ -247,8 +325,7 @@ class ApiServer:
             req.write_json(json.dumps({
                 "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
                 "usage": {"completion_tokens": n_completion, "prompt_tokens": n_prompt, "total_tokens": n_prompt + n_completion},
-                "choices": [{"index": i, "message": {"role": "assistant", "content": b}, "finish_reason": "stop"}
-                            for i, b in enumerate(buffers)]}))
+                "choices": [choice_json(i, b, lps) for i, b in enumerate(buffers)]}))
         print("🔶" if n == 1 else f"({n} choices)🔶")
 
     def slot_request(self, req: HttpRequest, caches: List[NaiveCache], n_slots: int) -> SlotRequest:
@@ -267,6 +344,7 @@ class ApiServer:
         temperature = float(body.get("temperature", ctx.args.temperature))
         if temperature < 0:
             raise ValueError("'temperature' must not be negative")
+        lp_k = parse_logprobs(body)   # --parallel > 1 runs on one GPU
         detector_args, gen = self.detector_args, self.gen
 
         class Chat(SlotRequest):
@@ -284,26 +362,33 @@ class ApiServer:
                 P = min(start + len(tokens) - 1, slot_len)
                 p = public.decode("utf-8", errors="replace")
                 self.buffers = [p] * n
+                lps = self.lps
                 if stream:
                     req.write_stream_start()
                     if p:
                         for i in range(n):
-                            req.write_stream_chunk("data: " + chunk_json(p, False, i) + "\r\n\r\n")
+                            req.write_stream_chunk("data: " + chunk_json(p, False, i, lps.take(i) if lps else None) + "\r\n\r\n")
                 for m in delta:
                     cache.push(P, m)
                 self.slot_cache = cache
                 n_pref = P - start
                 return tokens[:n_pref], start, (tokens[n_pref] if n_pref < len(tokens) else tokens[-1]), P
 
+            def on_logprobs(self, i, entry):
+                self.lps.on_logprobs(i, entry)
+
             def on_token(self, i, t):
                 piece = self.decoders[i].decode(tok, t)
                 kind = self.dets[i].append(t, piece)
+                lps = self.lps
+                if lps:
+                    lps.consumed(i, kind == H.EOS)
                 if kind in (H.NOT_EOS, H.EOS):
                     delta = self.dets[i].get_delta()
                     if delta:
                         d = delta.decode("utf-8", errors="replace")
                         if stream:
-                            req.write_stream_chunk("data: " + chunk_json(d, False, i) + "\r\n\r\n")
+                            req.write_stream_chunk("data: " + chunk_json(d, False, i, lps.take(i) if lps else None) + "\r\n\r\n")
                         self.buffers[i] += d
                     self.dets[i].reset()
                 return kind == H.EOS
@@ -319,7 +404,7 @@ class ApiServer:
                     caches[s].items = list(caches[slots[0]].items)
                 if stream:
                     for i in range(n):
-                        req.write_stream_chunk("data: " + chunk_json(None, True, i) + "\r\n\r\n")
+                        write_stream_finish(req, i, self.lps)
                     req.write_stream_chunk("data: [DONE]")
                     req.write_stream_end()
                 else:
@@ -328,8 +413,7 @@ class ApiServer:
                         "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
                         "usage": {"completion_tokens": n_completion, "prompt_tokens": self.n_prompt,
                                   "total_tokens": self.n_prompt + n_completion},
-                        "choices": [{"index": i, "message": {"role": "assistant", "content": b}, "finish_reason": "stop"}
-                                    for i, b in enumerate(self.buffers)]}))
+                        "choices": [choice_json(i, b, self.lps) for i, b in enumerate(self.buffers)]}))
                 print(f"🔶 slot {slots[0]}" + (f" ({n} choices)" if n > 1 else ""), flush=True)
                 self.done()
 
@@ -345,6 +429,8 @@ class ApiServer:
         r.presence, r.frequency, r.bias = presence, frequency, bias
         r.seed = int(body["seed"]) if "seed" in body else None
         r.max_tokens = int(body.get("max_tokens", -1))
+        r.logprobs = lp_k
+        r.lps = LogprobsLog(tok, n) if lp_k is not None else None
         r.dets = [H.EosDetector(*detector_args) for _ in range(n)]
         r.decoders = [H.TokenDecoder() for _ in range(n)]
         r.done = lambda: None

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from .. import host
-from ..api import InferenceSession
+from ..api import InferenceSession, check_logprobs
 from .args import AppArgs
 
 OP_STOP, OP_PREFILL, OP_STEP_LOGITS, OP_STEP_GREEDY, OP_DECODE_N, OP_STEP_SAMPLE, OP_SEED = 0, 1, 2, 3, 4, 5, 6
@@ -49,6 +49,10 @@ def _f32_bits(*xs: float) -> List[int]:
 def _bits_f32(*xs: int) -> List[float]:
     import struct
     return list(struct.unpack(f"<{len(xs)}f", struct.pack(f"<{len(xs)}i", *xs)))
+
+
+def _lp_kw(logprobs: Optional[int]) -> dict:
+    return {} if logprobs is None else {"logprobs": logprobs}
 
 
 def world():
@@ -133,7 +137,7 @@ class RootInference:
         self._send(OP_STEP_LOGITS, pos, [token])
         return self.eng.step(token, pos)
 
-    def forward_greedy(self, token: int, pos: int) -> int:
+    def forward_greedy(self, token: int, pos: int, logprobs: Optional[int] = None) -> int:
         self._send(OP_STEP_GREEDY, pos, [token])
         if self._pin_in is None:          # session on the CPU (protocol tests)
             self.eng._set_inputs([token], pos)
@@ -144,9 +148,14 @@ class RootInference:
         self.eng.tokens[:1].copy_(self._pin_in[:1], non_blocking=True)
         self.eng.pos[:1].copy_(self._pin_in[1:2], non_blocking=True)
         self.eng.run_decode_step()
+        lp = logprobs
+        if lp is not None:
+            self.eng.logprobs([lp])
         self._pin_out.copy_(self.eng.tokens[:1], non_blocking=True)
         torch.cuda.current_stream().synchronize()
         self.eng.check_abort()
+        if lp is not None:
+            self._last_logprobs = self.eng.read_logprobs()
         return int(self._pin_out[0])
 
     # ---- sampling on the device: the logits never leave the GPUs (csrc/cuda/sampler.cu) ----
@@ -158,14 +167,19 @@ class RootInference:
         self._send(OP_SEED, 0, _split_seed(seed))
         self.eng.seed_sampler(seed)
 
-    def forward_sampled(self, token: int, pos: int, temperature: float, topp: float) -> int:
+    def forward_sampled(self, token: int, pos: int, temperature: float, topp: float, logprobs: Optional[int] = None) -> int:
         import struct
         t_bits, p_bits = struct.unpack("<ii", struct.pack("<ff", temperature, topp))
         self._send(OP_STEP_SAMPLE, pos, [token, t_bits, p_bits])
         self.eng.step_sampled(token, pos, temperature, topp)
+        lp = logprobs
+        if lp is not None:
+            self.eng.logprobs([lp], controlled=True)
         self._pin_out.copy_(self.eng.tokens[:1], non_blocking=True)
         torch.cuda.current_stream().synchronize()
         self.eng.check_abort()
+        if lp is not None:
+            self._last_logprobs = self.eng.read_logprobs()
         return int(self._pin_out[0])
 
     def set_controls(self, sampler, row_mask: int) -> None:
@@ -176,12 +190,15 @@ class RootInference:
         self._send(OP_CONTROLS, 0, words)
         self.eng.set_sampling_controls(sampler.presence_penalty, sampler.frequency_penalty, bias, row_mask)
 
-    def next_token(self, token: int, pos: int, sampler) -> int:
+    def next_token(self, token: int, pos: int, sampler, logprobs: Optional[int] = None) -> int:
         """One generated token with the sampler's settings: greedy and temperature/top-p both run on the device; the host sampler
         is only used with the library-collective (multi-node) mode or DL_HOST_SAMPLER=1. Greedy with sampling controls runs
-        on the device sampler (arg-max of the controlled logits), not on the fused arg-max."""
+        on the device sampler (arg-max of the controlled logits), not on the fused arg-max. logprobs = k: also the
+        log-probabilities of the draw on the device (last_logprobs(); one GPU only), enqueued behind it."""
+        if logprobs is not None:
+            check_logprobs(logprobs, self.comm.world_size if self.comm is not None else 1)
         if sampler.temperature == 0.0 and not sampler.controls_active:
-            return self.forward_greedy(token, pos)
+            return self.forward_greedy(token, pos, logprobs)
         if self.device_sampling:
             if sampler.temperature != 0.0 and getattr(self, "_seeded", None) != (sampler.seed, sampler.seed_generation):
                 self.seed(sampler.seed)
@@ -190,8 +207,15 @@ class RootInference:
             if getattr(self, "_controls", None) != key:   # a new completion: count row 0 starts from zero
                 self.set_controls(sampler, 1)
                 self._controls = key
-            return self.forward_sampled(token, pos, sampler.temperature, sampler.topp)
-        return int(sampler.sample(self.forward_logits(token, pos).float().cpu().numpy()))
+            return self.forward_sampled(token, pos, sampler.temperature, sampler.topp, logprobs)
+        t = int(sampler.sample(self.forward_logits(token, pos).float().cpu().numpy()))
+        if logprobs is not None:
+            self._last_logprobs = [self.eng.logprobs_host_draw(t, logprobs, sampler)]
+        return t
+
+    def last_logprobs(self) -> list:
+        """The log-probability entries of the last next_token / choices call asked for them (InferenceSession.last_logprobs)."""
+        return self._last_logprobs
 
     # ---- several completions of one prompt (api.run_choices); workers mirror every batched step ----
     def forget_device_seed(self):
@@ -219,14 +243,20 @@ class RootInference:
         self._send(OP_CHOICES_SEED, 0, [w for s in seeds for w in _split_seed(s)])
         self.eng.seed_choice_samplers(seeds)
 
-    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float) -> List[int]:
+    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float, logprobs: Optional[int] = None) -> List[int]:
         self._send(OP_CHOICES_FIRST, P, [token, n] + _f32_bits(temperature, topp))
-        return self.eng.choices_first(token, P, n, temperature, topp)
+        out = self.eng.choices_first(token, P, n, temperature, topp, **_lp_kw(logprobs))
+        if logprobs is not None:
+            self._last_logprobs = self.eng.read_logprobs()
+        return out
 
     def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
-                     topp: float) -> List[int]:
+                     topp: float, logprobs: Optional[int] = None) -> List[int]:
         self._send(OP_CHOICES_STEP, P, [C, j, _active_mask(active)] + _f32_bits(temperature, topp) + list(tokens))
-        return self.eng.choices_step(tokens, P, C, j, active, temperature, topp)
+        out = self.eng.choices_step(tokens, P, C, j, active, temperature, topp, **_lp_kw(logprobs))
+        if logprobs is not None:
+            self._last_logprobs = self.eng.read_logprobs()
+        return out
 
     def decode_greedy(self, token: int, pos: int, n_steps: int) -> List[int]:
         """n greedy steps with the token fed back on the device (no host round trip per step): one control packet for all."""

@@ -168,6 +168,14 @@ def lib() -> C.CDLL:
     L.dl_engine_slots_forward.restype = i32
     L.dl_engine_slots_step.argtypes = [vp, ip, ip, u32, ip, vp]
     L.dl_engine_slots_step.restype = i32
+    L.dl_engine_slot_logprobs.argtypes = [vp, u32, i32]
+    L.dl_engine_slot_logprobs.restype = i32
+    L.dl_engine_slots_step_logprobs.argtypes = [vp, ip, ip, u32, ip, ip, vp]
+    L.dl_engine_slots_step_logprobs.restype = i32
+    L.dl_engine_logprobs.argtypes = [vp, i32, u32, ip, i32, i32, vp, vp]
+    L.dl_engine_logprobs.restype = i32
+    L.dl_logprobs_rows.argtypes = [vp, u32, u32, u32, u32, ip, vp, vp, u32, vp, u32, f32, f32, vp, vp, vp]
+    L.dl_logprobs_rows.restype = i32
     L.dl_engine_sync_ns.argtypes = [vp]
     L.dl_engine_sync_ns.restype = C.c_uint64
     L.dl_engine_mega_active.argtypes = [vp]
@@ -218,6 +226,19 @@ def stream_ptr() -> int:
 
 # KV-cache storage (EngineConfig.kvType): name of --kv-cache-float-type -> code
 KV_CACHE_TYPES = {"bf16": 0, "q80": 1}
+
+# Log-probabilities (csrc/cuda/logprobs.cu): int32 words of one row's result block, the largest top_logprobs, dl_engine_logprobs flags
+LOGPROBS_WORDS, LOGPROBS_MAX_TOP = 44, 20
+LP_CONTROLLED, LP_SHARED_ROW = 1, 2
+
+
+def decode_logprobs(words) -> tuple:
+    """One row's result block (LOGPROBS_WORDS int32 values) -> (chosen id, its logprob, [(id, logprob), ...] top entries)."""
+    import struct
+    w = [int(x) for x in words]
+    f = lambda bits: struct.unpack("<f", struct.pack("<i", bits))[0]
+    k = w[2]
+    return w[0], f(w[1]), [(w[4 + 2 * j], f(w[5 + 2 * j])) for j in range(k)]
 
 PRO_RMSNORM, PRO_PLAIN = 0, 1
 EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU = 0, 1, 2

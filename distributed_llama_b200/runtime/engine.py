@@ -22,6 +22,28 @@ def _p(t: Optional[torch.Tensor]):
     return t.data_ptr() if t is not None else None
 
 
+def logprobs_rows(logits: torch.Tensor, chosen: torch.Tensor, k: Sequence[int], row_mask: Optional[int] = None,
+                  bias: Optional[torch.Tensor] = None, counts: Optional[torch.Tensor] = None, presence: float = 0.0,
+                  frequency: float = 0.0, row_params: Optional[torch.Tensor] = None, shared_row: bool = False) -> torch.Tensor:
+    """The log-probability kernel (csrc/cuda/logprobs.cu) on explicit device buffers: B = len(k) rows of `logits` ([B][n] f32,
+    or one row read by every row with shared_row), chosen ([B] int32: each row's draw; counts are those after it), k[b] top
+    entries, rows outside row_mask (default: all) untouched. Optional controls: bias ([n], or [B][n]: one per row) f32, counts
+    [B][n] int32, and the penalties, per row through row_params ([B][4] f32, columns 2 and 3). Returns the device result blocks
+    [B][LOGPROBS_WORDS] int32 (ops.cuda_lib.decode_logprobs reads one)."""
+    B = len(k)
+    n = logits.shape[-1]
+    mask = ((1 << B) - 1) if row_mask is None else int(row_mask)
+    out = torch.zeros(B, cl.LOGPROBS_WORDS, dtype=torch.int32, device=logits.device)
+    ks = (C.c_int32 * B)(*[int(x) for x in k])
+    stride = 0 if shared_row or logits.dim() == 1 else logits.stride(0)
+    bias_stride = bias.stride(0) if bias is not None and bias.dim() == 2 else 0
+    counts_stride = counts.stride(0) if counts is not None and counts.dim() == 2 else 0
+    cl.check(cl.lib().dl_logprobs_rows(logits.data_ptr(), stride, n, B, mask, ks, chosen.data_ptr(), _p(bias), bias_stride, _p(counts),
+                                       counts_stride, float(presence), float(frequency), _p(row_params), out.data_ptr(), cl.stream_ptr()),
+             "logprobs_rows")
+    return out
+
+
 class Engine:
     def __init__(self, weights: DeviceWeights, max_batch: int = 8, n_splits: int = 0, use_pdl: bool = True,
                  seq_len: Optional[int] = None, comm=None, max_prefill: int = 192, collectives: str = "auto",
@@ -238,21 +260,26 @@ class Engine:
         self.pos[:nb].fill_(P + 1 + j)
         cl.check(self._lib.dl_engine_choices_forward(self._h, nb, P, C, j, mask, cl.stream_ptr()), "engine_choices_forward")
 
-    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float) -> List[int]:
-        """Forward of the prompt's last token at P, then choice i draws its first token from that row with generator i."""
+    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float, logprobs: Optional[int] = None) -> List[int]:
+        """Forward of the prompt's last token at P, then choice i draws its first token from that row with generator i.
+        logprobs = k: also the log-probabilities of every draw (read_logprobs())."""
         self.forward_batch([token], P, logits_mode=1)
         self.sample_choices_first(n, temperature, topp)
+        if logprobs is not None:
+            self.logprobs([logprobs] * n, (1 << n) - 1, first_row=1, controlled=True, shared_row=True)
         out = self.tokens[:n].tolist()
         self.check_abort()
         return out
 
     def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
-                     topp: float) -> List[int]:
+                     topp: float, logprobs: Optional[int] = None) -> List[int]:
         """choices_forward, then every active row draws its next token with its own generator. Returns the draws (inactive
-        rows: whatever tokens[] held)."""
+        rows: whatever tokens[] held). logprobs = k: also the log-probabilities of the active rows' draws (read_logprobs())."""
         self.choices_forward(tokens, P, C, j, active)
         nb, mask = self._choice_batch(len(tokens), active)
         cl.check(self._lib.dl_engine_sample_rows(self._h, nb, mask, float(temperature), float(topp), 0, cl.stream_ptr()), "engine_sample_rows")
+        if logprobs is not None:
+            self.logprobs([logprobs] * len(tokens), sum(1 << b for b in range(len(tokens)) if active[b]), first_row=1, controlled=True)
         out = self.tokens[:len(tokens)].tolist()
         self.check_abort()
         return out
@@ -312,6 +339,65 @@ class Engine:
         cl.check(self._lib.dl_engine_slots_step(self._h, t, p, mask, out, cl.stream_ptr()), "engine_slots_step")
         self.check_abort()
         return list(out)
+
+    def slot_logprobs(self, slot: int, k: Optional[int]) -> None:
+        """Log-probabilities of slot `slot`'s draws with k top entries (None: off, as after every slot_sampling)."""
+        cl.check(self._lib.dl_engine_slot_logprobs(self._h, int(slot), -1 if k is None else int(k)), "engine_slot_logprobs")
+
+    def slots_step_logprobs(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]):
+        """slots_step that also returns, per slot, the log-probabilities of its draw (see logprobs) for the active slots whose
+        logprobs are on (slot_logprobs), None for the others."""
+        t, p, mask = self._slot_args(tokens, pos, active)
+        out = (C.c_int32 * self.slots)(*([-1] * self.slots))
+        lp = (C.c_int32 * (self.slots * cl.LOGPROBS_WORDS))()
+        for b in range(self.slots):
+            lp[b * cl.LOGPROBS_WORDS + 2] = -1   # rows the step leaves alone keep k = -1
+        cl.check(self._lib.dl_engine_slots_step_logprobs(self._h, t, p, mask, out, lp, cl.stream_ptr()), "engine_slots_step_logprobs")
+        self.check_abort()
+        W = cl.LOGPROBS_WORDS
+        rows = [None if lp[b * W + 2] < 0 else cl.decode_logprobs(lp[b * W:(b + 1) * W]) for b in range(self.slots)]
+        return list(out), rows
+
+    # -- per-token log-probabilities of the last draw (csrc/cuda/logprobs.cu) --
+    def logprobs(self, k: Sequence[int], row_mask: int = 1, first_row: int = 0, controlled: bool = False, shared_row: bool = False) -> None:
+        """Enqueues, behind the last draw on the current stream, the log-probabilities of the tokens in tokens[b] for the rows b set
+        in row_mask: logprob(i) = x[i] - logsumexp(x) over the sampled vocabulary of logits row b (row 0 for every row with
+        shared_row), x the logits after the sampling controls the draw used when `controlled` (count row first_row + b), and the
+        k[b] largest entries. The result block is copied to pinned memory on the same stream: read it with read_logprobs() after
+        the stream has been synchronised (the token copy that follows does that)."""
+        rows = len(k)
+        if not hasattr(self, "lp_out"):
+            self.lp_out = torch.zeros(self.max_batch, cl.LOGPROBS_WORDS, dtype=torch.int32, device=self.device)
+            self._lp_host = torch.zeros(self.max_batch, cl.LOGPROBS_WORDS, dtype=torch.int32).pin_memory()
+        ks = (C.c_int32 * rows)(*[int(x) for x in k])
+        flags = (cl.LP_CONTROLLED if controlled else 0) | (cl.LP_SHARED_ROW if shared_row else 0)
+        cl.check(self._lib.dl_engine_logprobs(self._h, rows, int(row_mask), ks, int(first_row), flags, self.lp_out.data_ptr(), cl.stream_ptr()),
+                 "engine_logprobs")
+        self._lp_host[:rows].copy_(self.lp_out[:rows], non_blocking=True)
+        self._lp_mask, self._lp_rows = int(row_mask), rows
+
+    def read_logprobs(self) -> list:
+        """The rows of the last logprobs() call, once its stream is synchronised: (chosen id, logprob, [(id, logprob), ...]) per row
+        of its mask, None for the other rows."""
+        h = self._lp_host.numpy()
+        return [cl.decode_logprobs(h[b]) if (self._lp_mask >> b) & 1 else None for b in range(self._lp_rows)]
+
+    def logprobs_host_draw(self, chosen: int, k: int, sampler) -> tuple:
+        """Log-probabilities of a token the host sampler drew from logits[0] of the last forward (single GPU): the same kernel on
+        the device logits, with the sampler's controls and its counts after the draw uploaded. Returns the decoded row."""
+        dev = self.device
+        bias = counts = None
+        if sampler.controls_active:
+            n = sampler.vocab_size
+            bias = torch.zeros(n, dtype=torch.float32)
+            for t, v in sampler.logit_bias:
+                bias[t] = v
+            bias = bias.to(dev)
+            counts = torch.as_tensor(np.asarray(sampler.counts, dtype=np.uint32).view(np.int32)).reshape(1, -1).to(dev)
+        n = min(sampler.vocab_size, self.w.vocab)
+        out = logprobs_rows(self.logits[0:1, :n], torch.tensor([chosen], dtype=torch.int32, device=dev), [k], bias=bias, counts=counts,
+                            presence=sampler.presence_penalty, frequency=sampler.frequency_penalty)
+        return cl.decode_logprobs(out[0].cpu().tolist())
 
     def sampler_state(self) -> int:
         """State of the single-sequence device generator (0 before the first seeding); seed_sampler(state) continues its stream."""
