@@ -416,6 +416,146 @@ void parseControls(const JsonValue &body, uint32_t vocab, float &presence, float
     if (byId.size() > kMaxLogitBiasEntries) throw std::runtime_error("'logit_bias' has more than 100 entries");
     bias.assign(byId.begin(), byId.end());
 }
+
+// A validated chat completion request: the rules of distributed_llama_b200.apps.api_server.parse_chat, except that a number field
+// that is not a number counts as absent.
+struct ChatRequest {
+    std::vector<ChatItem> messages;
+    bool stream = false, hasSeed = false;
+    uint32_t n = 1;
+    int maxTokens = -1;
+    int logprobs = -1;   // top_logprobs k, -1: none
+    float temperature = 0.f, topp = 0.9f, presence = 0.f, frequency = 0.f;
+    std::vector<std::pair<int32_t, float>> bias;
+    uint64_t seed = 0;
+};
+
+// maxN: the largest `n` (the slot count under --parallel)
+ChatRequest parseChat(const JsonValue &body, const ApiConfig &cfg, uint32_t vocab, uint32_t maxN) {
+    if (!body.isObject()) throw std::runtime_error("request body must be a JSON object");
+    ChatRequest c;
+    if (const JsonValue *v = body.find("n")) {
+        if (v->kind != JsonValue::Number || v->num != (double)(int64_t)v->num || v->num < 1 || v->num > kMaxChoices)
+            throw std::runtime_error("'n' must be an integer from 1 to 8");
+        c.n = (uint32_t)v->num;
+    }
+    if (c.n > maxN) throw std::runtime_error("'n' must not exceed --parallel");
+    c.presence = cfg.presencePenalty;
+    c.frequency = cfg.frequencyPenalty;
+    parseControls(body, vocab, c.presence, c.frequency, c.bias);
+    c.logprobs = parseLogprobs(body);
+    for (const JsonValue &m : body.at("messages").arr) c.messages.push_back({m.at("role").str, m.at("content").str});
+    c.stream = body.boolOr("stream", false);
+    c.temperature = (float)body.numberOr("temperature", cfg.temperature);
+    if (c.temperature < 0.f) throw std::runtime_error("'temperature' must not be negative");
+    c.topp = (float)body.numberOr("top_p", cfg.topp);
+    if (const JsonValue *sd = body.find("seed")) if (sd->kind == JsonValue::Number) { c.seed = (uint64_t)sd->num; c.hasSeed = true; }
+    c.maxTokens = (int)body.numberOr("max_tokens", -1);
+    return c;
+}
+
+std::string completionJson(uint32_t nPrompt, const std::vector<std::vector<int32_t>> &out, const std::vector<std::string> &buffers,
+                           const LogprobsLog *lps) {
+    uint32_t nCompletion = 0;
+    std::string choices;
+    for (uint32_t i = 0; i < buffers.size(); i++) {
+        nCompletion += (uint32_t)out[i].size();
+        choices += std::string(i ? ", " : "") + choiceJson(i, buffers[i], lps);
+    }
+    return "{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
+           ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
+           ", \"prompt_tokens\": " + std::to_string(nPrompt) + ", \"total_tokens\": " + std::to_string(nPrompt + nCompletion) +
+           "}, \"choices\": [" + choices + "]}";
+}
+
+// The response to one chat request: its n choices' decoders, stop detectors, texts and log-probability entries, written as stream
+// chunks or as one cmpl-j0 JSON body (the Python server's ChatResponse). echo: print the tokens' pieces to stdout.
+class ChatResponse {
+public:
+    ChatResponse(const HttpRequest &req, const ChatRequest &chat, const Tokenizer &tok, const std::vector<std::string> &stops, bool echo = false)
+        : req_(req), tok_(tok), n_(chat.n), stream_(chat.stream), echo_(echo), hasLog_(chat.logprobs >= 0), log_(chat.n),
+          dets_(chat.n, EosDetector(tok.data().eosIds, stops, maxLen(stops), maxLen(stops))), pending_(chat.n), buffers_(chat.n) {}
+    const std::string &text(uint32_t i) const { return buffers_[i]; }
+    // every choice's text starts with the prompt's public part; a stream sends its head and that part
+    void start(const std::string &publicPrompt) {
+        buffers_.assign(n_, publicPrompt);
+        if (!stream_) return;
+        req_.writeStreamStart();
+        if (!publicPrompt.empty())
+            for (uint32_t i = 0; i < n_; i++) chunk(i, publicPrompt);
+    }
+    void onLogprobs(uint32_t i, const TokenLogprobs &e) { log_.next[i] = logprobEntryJson(tok_, e); }
+    // choice i's next token; true when it ended the choice (end of sequence or stop string)
+    bool onToken(uint32_t i, int32_t t) {
+        const std::string piece = tok_.decodeWith(pending_[i], t);
+        if (echo_ && !piece.empty()) { std::printf("%s", piece.c_str()); std::fflush(stdout); }
+        const EosDetectorResult kind = dets_[i].append(t, piece);
+        if (hasLog_) log_.consumed(i, kind == EOS);
+        if (kind == NOT_EOS || kind == EOS) {
+            const std::string delta = dets_[i].getDelta();
+            if (!delta.empty()) {
+                if (stream_) chunk(i, delta);
+                buffers_[i] += delta;
+            }
+            dets_[i].reset();
+        }
+        return kind == EOS;
+    }
+    // every choice is done (out[i]: choice i's tokens): the stop chunks and [DONE], or the JSON body
+    void finish(const std::vector<std::vector<int32_t>> &out, uint32_t nPrompt) {
+        if (!stream_) { req_.writeJson(completionJson(nPrompt, out, buffers_, lps())); return; }
+        for (uint32_t i = 0; i < n_; i++) writeStreamFinish(req_, i, lps());
+        req_.writeStreamChunk("data: [DONE]");
+        req_.writeStreamEnd();
+    }
+private:
+    LogprobsLog *lps() { return hasLog_ ? &log_ : nullptr; }
+    void chunk(uint32_t i, const std::string &text) {
+        const std::vector<std::string> e = hasLog_ ? log_.take(i) : std::vector<std::string>();
+        req_.writeStreamChunk("data: " + chunkJson(&text, false, i, hasLog_ ? &e : nullptr) + "\r\n\r\n");
+    }
+    const HttpRequest &req_;
+    const Tokenizer &tok_;
+    uint32_t n_;
+    bool stream_, echo_, hasLog_;
+    LogprobsLog log_;
+    std::vector<EosDetector> dets_;
+    std::vector<std::string> pending_, buffers_;
+};
+
+// A prompt resolved against a NaiveCache: the tokens to prefill from `start`, the last prompt token at P, the prompt's token count
+// and its public part.
+struct Prompt {
+    std::vector<int32_t> prefill;
+    uint32_t start = 0, P = 0, nPrompt = 0;
+    int32_t token = 0;
+    std::string publicPrompt;
+};
+
+// Resolves `messages` against `cache` and records the messages still to be evaluated in it. echo: print the prompt to stdout.
+Prompt preparePrompt(const ChatTemplateGenerator &gen, const Tokenizer &tok, NaiveCache &cache, std::vector<ChatItem> messages, uint32_t ctxLen,
+                     bool echo = false) {
+    Prompt p;
+    p.start = cache.resolveDeltaPrompt(messages);
+    const GeneratedChat g = gen.generate(messages, true);
+    if (echo) std::printf("🔹%s🔸", g.content.c_str());
+    const std::vector<int32_t> tokens = tok.encode(g.content, p.start == 0, true);
+    p.nPrompt = (uint32_t)tokens.size();
+    p.P = std::min(p.start + p.nPrompt - 1, ctxLen);
+    for (const ChatItem &m : messages) cache.push(p.P, m);
+    const uint32_t nPref = p.P - p.start;
+    p.prefill.assign(tokens.begin(), tokens.begin() + nPref);
+    p.token = nPref < tokens.size() ? tokens[nPref] : tokens.back();
+    p.publicPrompt = g.publicPrompt;
+    return p;
+}
+
+// After a single completion of the prompt ending at P the cache keeps its answer too, unless it filled the context.
+void rememberAnswer(NaiveCache &cache, uint32_t P, size_t nOut, const std::string &text, uint32_t ctxLen) {
+    const uint32_t end = P + (uint32_t)nOut;
+    if (end == ctxLen) cache.clear();
+    else cache.push(end, {"assistant", text});
+}
 }  // namespace
 
 float parsePenalty(const std::string &flag, const std::string &value) {
@@ -438,100 +578,27 @@ ApiServer::ApiServer(InferenceBackend &backend, Tokenizer &tokenizer, const ApiC
 // keeps its answer too; after several it keeps only the prompt messages, so a follow-up that quotes any one choice re-uses the
 // prompt.
 void ApiServer::complete(HttpRequest &req) {
-    if (!req.hasJson || !req.json.isObject()) throw std::runtime_error("request body must be a JSON object");
-    const JsonValue &body = req.json;
-    std::vector<ChatItem> messages;
-    for (const JsonValue &m : body.at("messages").arr) messages.push_back({m.at("role").str, m.at("content").str});
-    const bool stream = body.boolOr("stream", false);
-    const int maxTokens = (int)body.numberOr("max_tokens", -1);
-    sampler_.setTemperature((float)body.numberOr("temperature", cfg_.temperature));
-    sampler_.setTopp((float)body.numberOr("top_p", cfg_.topp));
-    uint32_t n = 1;
-    if (const JsonValue *v = body.find("n")) {
-        if (v->kind != JsonValue::Number || v->num != (double)(int64_t)v->num || v->num < 1 || v->num > kMaxChoices)
-            throw std::runtime_error("'n' must be an integer from 1 to 8");
-        n = (uint32_t)v->num;
-    }
-    float presence = cfg_.presencePenalty, frequency = cfg_.frequencyPenalty;
-    std::vector<std::pair<int32_t, float>> bias;
-    parseControls(body, sampler_.vocabSize(), presence, frequency, bias);
-    const int lpK = parseLogprobs(body);
-    backend_.setLogprobs(lpK);   // refuses where they cannot run (tensor parallelism)
-    sampler_.setControls(presence, frequency, bias);
-    bool seeded = false;
-    if (const JsonValue *s = body.find("seed")) if (s->kind == JsonValue::Number) { sampler_.setSeed((uint64_t)s->num); seeded = true; }
+    const ChatRequest chat = parseChat(req.json, cfg_, sampler_.vocabSize(), kMaxChoices);
+    backend_.setLogprobs(chat.logprobs);   // refuses where they cannot run (tensor parallelism)
+    sampler_.setControls(chat.presence, chat.frequency, chat.bias);
+    sampler_.setTemperature(chat.temperature);
+    sampler_.setTopp(chat.topp);
+    if (chat.hasSeed) sampler_.setSeed(chat.seed);
     // several completions: choice i uses choiceSeed(base, i); without a seed the base is drawn from the advancing generator
-    const uint64_t baseSeed = seeded ? sampler_.seed() : (n > 1 ? sampler_.nextSeed() : 0);
-
+    const uint64_t baseSeed = chat.hasSeed ? sampler_.seed() : (chat.n > 1 ? sampler_.nextSeed() : 0);
     const uint32_t seqLen = backend_.seqLen();
-    const uint32_t startPos = cache_.resolveDeltaPrompt(messages);
-    const GeneratedChat g = gen_.generate(messages, true);
-    std::printf("🔹%s🔸", g.content.c_str());
-    const std::vector<int32_t> tokens = tok_.encode(g.content, startPos == 0, true);
-    const uint32_t nPrompt = (uint32_t)tokens.size();
-    const uint32_t promptEnd = std::min(startPos + nPrompt - 1, seqLen);
-    for (const ChatItem &m : messages) cache_.push(promptEnd, m);
-
-    std::vector<EosDetector> dets(n, EosDetector(tok_.data().eosIds, stops_, maxLen(stops_), maxLen(stops_)));
-    std::vector<std::string> pending(n), buffers(n, g.publicPrompt);
-    LogprobsLog log(n);
-    LogprobsLog *lps = lpK >= 0 ? &log : nullptr;
-    if (stream) {
-        req.writeStreamStart();
-        if (!g.publicPrompt.empty())
-            for (uint32_t i = 0; i < n; i++) {
-                const std::vector<std::string> e;
-                req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false, i, lps ? &e : nullptr) + "\r\n\r\n");
-            }
-    }
-    const uint32_t nPref = promptEnd - startPos;
-    backend_.prefill(std::vector<int32_t>(tokens.begin(), tokens.begin() + nPref), startPos);
-    const int32_t token = nPref < tokens.size() ? tokens[nPref] : tokens.back();
-    const auto onToken = [&](uint32_t i, int32_t t) {
-        const std::string piece = tok_.decodeWith(pending[i], t);
-        if (n == 1 && !piece.empty()) { std::printf("%s", piece.c_str()); std::fflush(stdout); }
-        const EosDetectorResult kind = dets[i].append(t, piece);
-        if (lps) lps->consumed(i, kind == EOS);
-        if (kind == NOT_EOS || kind == EOS) {
-            const std::string delta = dets[i].getDelta();
-            if (!delta.empty()) {
-                if (stream) {
-                    const std::vector<std::string> e = lps ? lps->take(i) : std::vector<std::string>();
-                    req.writeStreamChunk("data: " + chunkJson(&delta, false, i, lps ? &e : nullptr) + "\r\n\r\n");
-                }
-                buffers[i] += delta;
-            }
-            dets[i].reset();
-        }
-        return kind == EOS;
-    };
+    const Prompt p = preparePrompt(gen_, tok_, cache_, chat.messages, seqLen, true);
+    ChatResponse resp(req, chat, tok_, stops_, chat.n == 1);
+    resp.start(p.publicPrompt);
+    backend_.prefill(p.prefill, p.start);
     std::function<void(uint32_t, const TokenLogprobs &)> onLogprobs;
-    if (lps) onLogprobs = [&](uint32_t i, const TokenLogprobs &e) { log.next[i] = logprobEntryJson(tok_, e); };
-    const std::vector<std::vector<int32_t>> out = runChoices(backend_, token, promptEnd, n, maxTokens, seqLen, sampler_, baseSeed, onToken,
-                                                             onLogprobs);
-    if (n == 1) {
-        const uint32_t end = promptEnd + (uint32_t)out[0].size();
-        if (end == seqLen) cache_.clear();
-        else cache_.push(end, {"assistant", buffers[0]});
-    }
-    if (stream) {
-        for (uint32_t i = 0; i < n; i++) writeStreamFinish(req, i, lps);
-        req.writeStreamChunk("data: [DONE]");
-        req.writeStreamEnd();
-    } else {
-        uint32_t nCompletion = 0;
-        std::string choices;
-        for (uint32_t i = 0; i < n; i++) {
-            nCompletion += (uint32_t)out[i].size();
-            choices += std::string(i ? ", " : "") + choiceJson(i, buffers[i], lps);
-        }
-        req.writeJson("{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
-                      ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
-                      ", \"prompt_tokens\": " + std::to_string(nPrompt) + ", \"total_tokens\": " + std::to_string(nPrompt + nCompletion) +
-                      "}, \"choices\": [" + choices + "]}");
-    }
-    if (n == 1) std::printf("🔶\n");
-    else std::printf("(%u choices)🔶\n", n);
+    if (chat.logprobs >= 0) onLogprobs = [&](uint32_t i, const TokenLogprobs &e) { resp.onLogprobs(i, e); };
+    const std::vector<std::vector<int32_t>> out = runChoices(backend_, p.token, p.P, chat.n, chat.maxTokens, seqLen, sampler_, baseSeed,
+                                                             [&](uint32_t i, int32_t t) { return resp.onToken(i, t); }, onLogprobs);
+    if (chat.n == 1) rememberAnswer(cache_, p.P, out[0].size(), resp.text(0), seqLen);
+    resp.finish(out, p.nPrompt);
+    if (chat.n == 1) std::printf("🔶\n");
+    else std::printf("(%u choices)🔶\n", chat.n);
 }
 
 void ApiServer::models(HttpRequest &req) const {
@@ -541,39 +608,16 @@ void ApiServer::models(HttpRequest &req) const {
 // ---- concurrent requests (--parallel): the rules of distributed_llama_b200.api.SlotScheduler --------------------------------
 
 namespace {
-std::string completionJson(uint32_t nPrompt, const std::vector<std::vector<int32_t>> &out, const std::vector<std::string> &buffers,
-                           const LogprobsLog *lps) {
-    uint32_t nCompletion = 0;
-    std::string choices;
-    for (uint32_t i = 0; i < buffers.size(); i++) {
-        nCompletion += (uint32_t)out[i].size();
-        choices += std::string(i ? ", " : "") + choiceJson(i, buffers[i], lps);
-    }
-    return "{\"id\": \"cmpl-j0\", \"object\": \"chat.completion\", \"created\": " + std::to_string((long long)std::time(nullptr)) +
-           ", \"model\": \"Distributed Model\", \"usage\": {\"completion_tokens\": " + std::to_string(nCompletion) +
-           ", \"prompt_tokens\": " + std::to_string(nPrompt) + ", \"total_tokens\": " + std::to_string(nPrompt + nCompletion) +
-           "}, \"choices\": [" + choices + "]}";
-}
-
 // One validated chat completion and, once admitted, its slots and progress.
 struct SlotJob {
     HttpRequest req;
-    std::vector<ChatItem> messages;
-    bool stream = false, hasSeed = false;
-    int maxTokens = -1;
-    uint32_t n = 1;
-    float temperature = 0.f, topp = 0.9f, presence = 0.f, frequency = 0.f;
-    std::vector<std::pair<int32_t, float>> bias;
-    uint64_t seed = 0;
-    int logprobs = -1;   // top_logprobs k, -1: none
-    // admitted
+    ChatRequest chat;
+    ChatResponse resp;
     std::vector<uint32_t> slots;
     uint32_t P = 0, nPrompt = 0, limit = 0, live = 0;
     std::vector<std::vector<int32_t>> out;
-    std::vector<EosDetector> dets;
-    std::vector<std::string> pending, buffers;
-    LogprobsLog lps;
-    LogprobsLog *lp() { return logprobs >= 0 ? &lps : nullptr; }
+    SlotJob(HttpRequest r, ChatRequest c, const Tokenizer &tok, const std::vector<std::string> &stops)
+        : req(std::move(r)), chat(std::move(c)), resp(req, chat, tok, stops) {}
 };
 
 struct SlotRow {
@@ -606,27 +650,8 @@ void ApiServer::serveParallel(int srv) {
             std::printf("🔷 %s %s\n", req.method.c_str(), req.path.c_str());
             std::fflush(stdout);
             if (req.method == "POST" && req.path == "/v1/chat/completions") {
-                if (!req.hasJson || !req.json.isObject()) throw std::runtime_error("request body must be a JSON object");
-                const JsonValue &body = req.json;
-                auto job = std::make_shared<SlotJob>();
-                if (const JsonValue *v = body.find("n")) {
-                    if (v->kind != JsonValue::Number || v->num != (double)(int64_t)v->num || v->num < 1 || v->num > kMaxChoices)
-                        throw std::runtime_error("'n' must be an integer from 1 to 8");
-                    job->n = (uint32_t)v->num;
-                }
-                if (job->n > N) throw std::runtime_error("'n' must not exceed --parallel");
-                job->presence = cfg_.presencePenalty;
-                job->frequency = cfg_.frequencyPenalty;
-                parseControls(body, sampler_.vocabSize(), job->presence, job->frequency, job->bias);
-                job->logprobs = parseLogprobs(body);   // --parallel > 1 runs on one GPU
-                for (const JsonValue &m : body.at("messages").arr) job->messages.push_back({m.at("role").str, m.at("content").str});
-                job->stream = body.boolOr("stream", false);
-                job->temperature = (float)body.numberOr("temperature", cfg_.temperature);
-                if (job->temperature < 0.f) throw std::runtime_error("'temperature' must not be negative");
-                job->topp = (float)body.numberOr("top_p", cfg_.topp);
-                if (const JsonValue *sd = body.find("seed")) if (sd->kind == JsonValue::Number) { job->seed = (uint64_t)sd->num; job->hasSeed = true; }
-                job->maxTokens = (int)body.numberOr("max_tokens", -1);
-                job->req = std::move(req);
+                ChatRequest chat = parseChat(req.json, cfg_, sampler_.vocabSize(), N);   // --parallel > 1 runs on one GPU
+                auto job = std::make_shared<SlotJob>(std::move(req), std::move(chat), tok_, stops_);
                 std::lock_guard<std::mutex> lk(mu);
                 queue.push_back(job);
                 cv.notify_all();
@@ -670,93 +695,48 @@ void ApiServer::serveParallel(int srv) {
     const auto finish = [&](const std::shared_ptr<SlotJob> &job) {
         SlotJob &j = *job;
         NaiveCache &cache = caches[j.slots[0]];
-        if (j.n == 1) {
-            const uint32_t end = j.P + (uint32_t)j.out[0].size();
-            if (end == L) cache.clear();
-            else cache.push(end, {"assistant", j.buffers[0]});
-        }
+        if (j.chat.n == 1) rememberAnswer(cache, j.P, j.out[0].size(), j.resp.text(0), L);
         for (size_t k = 1; k < j.slots.size(); k++) caches[j.slots[k]].copyFrom(cache);   // they hold a copy of the prompt rows
-        if (j.stream) {
-            for (uint32_t i = 0; i < j.n; i++) writeStreamFinish(j.req, i, j.lp());
-            j.req.writeStreamChunk("data: [DONE]");
-            j.req.writeStreamEnd();
-        } else {
-            j.req.writeJson(completionJson(j.nPrompt, j.out, j.buffers, j.lp()));
-        }
-        std::printf("🔶 slot %u%s\n", j.slots[0], j.n > 1 ? (" (" + std::to_string(j.n) + " choices)").c_str() : "");
+        j.resp.finish(j.out, j.nPrompt);
+        std::printf("🔶 slot %u%s\n", j.slots[0], j.chat.n > 1 ? (" (" + std::to_string(j.chat.n) + " choices)").c_str() : "");
         std::fflush(stdout);
         closeConn(j.req.fd);
     };
     // Admission: the free slot whose cache covers most of the messages (lowest index on ties), then the lowest other free slots.
     const auto admit = [&](const std::shared_ptr<SlotJob> &job, const std::vector<uint32_t> &free, uint32_t need) {
         SlotJob &j = *job;
+        const ChatRequest &c = j.chat;
         uint32_t first = free[0];
-        size_t best = caches[first].coveredPrefix(j.messages);
-        for (uint32_t s : free) { const size_t c = caches[s].coveredPrefix(j.messages); if (c > best) { best = c; first = s; } }
+        size_t best = caches[first].coveredPrefix(c.messages);
+        for (uint32_t s : free) { const size_t n = caches[s].coveredPrefix(c.messages); if (n > best) { best = n; first = s; } }
         j.slots = {first};
         for (uint32_t s : free) if (s != first && j.slots.size() < need) j.slots.push_back(s);
-        NaiveCache &cache = caches[first];
-        std::vector<ChatItem> delta = j.messages;
-        const uint32_t start = cache.resolveDeltaPrompt(delta);
-        const GeneratedChat g = gen_.generate(delta, true);
-        const std::vector<int32_t> tokens = tok_.encode(g.content, start == 0, true);
-        j.nPrompt = (uint32_t)tokens.size();
-        j.P = std::min(start + j.nPrompt - 1, L);
-        j.buffers.assign(j.n, g.publicPrompt);
-        j.pending.assign(j.n, std::string());
-        j.dets.assign(j.n, EosDetector(tok_.data().eosIds, stops_, maxLen(stops_), maxLen(stops_)));
-        j.out.assign(j.n, {});
-        j.lps = LogprobsLog(j.n);
-        if (j.stream) {
-            j.req.writeStreamStart();
-            if (!g.publicPrompt.empty())
-                for (uint32_t i = 0; i < j.n; i++) {
-                    const std::vector<std::string> e;
-                    j.req.writeStreamChunk("data: " + chunkJson(&g.publicPrompt, false, i, j.lp() ? &e : nullptr) + "\r\n\r\n");
-                }
-        }
-        for (const ChatItem &m : delta) cache.push(j.P, m);
-        const uint32_t nPref = j.P - start;
-        if (nPref) backend_.slotPrefill(first, std::vector<int32_t>(tokens.begin(), tokens.begin() + nPref), start);
-        const int32_t token = nPref < tokens.size() ? tokens[nPref] : tokens.back();
+        const Prompt p = preparePrompt(gen_, tok_, caches[first], c.messages, L);
+        j.P = p.P;
+        j.nPrompt = p.nPrompt;
+        j.out.assign(c.n, {});
+        j.resp.start(p.publicPrompt);
+        if (!p.prefill.empty()) backend_.slotPrefill(first, p.prefill, p.start);
         for (size_t k = 1; k < j.slots.size(); k++) backend_.slotCopy(first, j.slots[k], j.P);
-        const uint64_t seed = j.hasSeed ? j.seed : (j.temperature != 0.f ? sampler_.nextSeed() : 0);
+        const uint64_t seed = c.hasSeed ? c.seed : (c.temperature != 0.f ? sampler_.nextSeed() : 0);
         for (size_t k = 0; k < j.slots.size(); k++)
         {
-            backend_.slotSampling(j.slots[k], j.n == 1 ? seed : choiceSeed(seed, (uint32_t)k), j.temperature, j.topp, j.presence, j.frequency, j.bias);
-            if (j.logprobs >= 0) backend_.slotLogprobs(j.slots[k], j.logprobs);
+            backend_.slotSampling(j.slots[k], c.n == 1 ? seed : choiceSeed(seed, (uint32_t)k), c.temperature, c.topp, c.presence, c.frequency, c.bias);
+            if (c.logprobs >= 0) backend_.slotLogprobs(j.slots[k], c.logprobs);
         }
         j.limit = L - j.P;
-        if (j.maxTokens > 0) j.limit = std::min<uint32_t>(j.limit, (uint32_t)j.maxTokens);
+        if (c.maxTokens > 0) j.limit = std::min<uint32_t>(j.limit, (uint32_t)c.maxTokens);
         if (j.limit == 0) { finish(job); return; }
         j.live = (uint32_t)j.slots.size();
         for (size_t k = 0; k < j.slots.size(); k++) {
             SlotRow &r = rows[j.slots[k]];
             owner[j.slots[k]] = job;
-            r.job = job; r.token = token; r.pos = (int32_t)j.P; r.nDone = 0;
+            r.job = job; r.token = p.token; r.pos = (int32_t)j.P; r.nDone = 0;
             r.choices.clear();
-            if (need == 1) for (uint32_t i = 0; i < j.n; i++) r.choices.push_back(i);
+            if (need == 1) for (uint32_t i = 0; i < c.n; i++) r.choices.push_back(i);
             else r.choices.push_back((uint32_t)k);
             r.done.assign(r.choices.size(), false);
         }
-    };
-    const auto onToken = [&](SlotJob &j, uint32_t i, int32_t t) {
-        const std::string piece = tok_.decodeWith(j.pending[i], t);
-        const EosDetectorResult kind = j.dets[i].append(t, piece);
-        LogprobsLog *lps = j.lp();
-        if (lps) lps->consumed(i, kind == EOS);
-        if (kind == NOT_EOS || kind == EOS) {
-            const std::string delta = j.dets[i].getDelta();
-            if (!delta.empty()) {
-                if (j.stream) {
-                    const std::vector<std::string> e = lps ? lps->take(i) : std::vector<std::string>();
-                    j.req.writeStreamChunk("data: " + chunkJson(&delta, false, i, lps ? &e : nullptr) + "\r\n\r\n");
-                }
-                j.buffers[i] += delta;
-            }
-            j.dets[i].reset();
-        }
-        return kind == EOS;
     };
 
     std::deque<std::shared_ptr<SlotJob>> waiting;
@@ -773,7 +753,7 @@ void ApiServer::serveParallel(int srv) {
             std::vector<uint32_t> free;
             for (uint32_t s = 0; s < N; s++) if (!owner[s]) free.push_back(s);
             const std::shared_ptr<SlotJob> job = waiting.front();
-            const uint32_t need = job->temperature == 0.f ? 1 : job->n;
+            const uint32_t need = job->chat.temperature == 0.f ? 1 : job->chat.n;
             if (free.size() < need) break;
             waiting.pop_front();
             try {
@@ -789,7 +769,7 @@ void ApiServer::serveParallel(int srv) {
             if (rows[s].job) { tokens[s] = rows[s].token; pos[s] = rows[s].pos; active |= 1u << s; }
         if (!active) continue;
         bool wantLp = false;
-        for (uint32_t s = 0; s < N; s++) wantLp = wantLp || (rows[s].job && rows[s].job->logprobs >= 0);
+        for (uint32_t s = 0; s < N; s++) wantLp = wantLp || (rows[s].job && rows[s].job->chat.logprobs >= 0);
         std::vector<TokenLogprobs> entries;
         const std::vector<int32_t> drawn = wantLp ? backend_.slotsStepLogprobs(tokens, pos, active, entries) : backend_.slotsStep(tokens, pos, active);
         for (uint32_t s = 0; s < N; s++) {
@@ -804,8 +784,8 @@ void ApiServer::serveParallel(int srv) {
                     if (r.done[c]) continue;
                     const uint32_t i = r.choices[c];
                     j.out[i].push_back(drawn[s]);
-                    if (j.logprobs >= 0) j.lps.next[i] = logprobEntryJson(tok_, entries.at(s));
-                    if (onToken(j, i, drawn[s]) || j.out[i].size() >= j.limit) { r.done[c] = true; r.nDone++; }
+                    if (j.chat.logprobs >= 0) j.resp.onLogprobs(i, entries.at(s));
+                    if (j.resp.onToken(i, drawn[s]) || j.out[i].size() >= j.limit) { r.done[c] = true; r.nDone++; }
                 }
             } catch (const std::exception &e) {
                 release(job);

@@ -14,6 +14,7 @@ import socket
 import sys
 import threading
 import time
+from types import SimpleNamespace
 from typing import Dict, List, Optional, Tuple
 
 from .. import host
@@ -173,6 +174,43 @@ def parse_logprobs(body: dict, n_ranks: int = 1) -> Optional[int]:
     return k
 
 
+def _number_field(body: dict, key: str, default):
+    v = body.get(key, default)
+    if isinstance(v, bool) or not isinstance(v, (int, float)):
+        raise ValueError(f"'{key}' must be a number")
+    return v
+
+
+def parse_chat(body, defaults, vocab: int, max_n: int, n_ranks: int) -> SimpleNamespace:
+    """A chat completion request: messages as (role, content) pairs, n, stream, max_tokens, temperature, topp, seed (None
+    without one), presence, frequency, bias (parse_controls) and logprobs (parse_logprobs). `defaults` holds the server's
+    --temperature, --topp and penalties; n may not exceed max_n (the slot count under --parallel); n_ranks > 1 (tensor
+    parallelism) refuses logprobs. A body that is not an object, `messages` that are not a list of {role, content} objects
+    with string values, a number field that is not a number, a negative temperature or a malformed control raise ValueError;
+    a body without `messages` raises KeyError."""
+    if not isinstance(body, dict):
+        raise ValueError("request body must be a JSON object")
+    n = parse_n(body)
+    if n > max_n:
+        raise ValueError(f"'n' must not exceed --parallel ({max_n})")
+    # server defaults: --presence-penalty / --frequency-penalty (argument objects that predate them mean 0)
+    presence, frequency, bias = parse_controls(body, vocab, getattr(defaults, "presence_penalty", 0.0),
+                                               getattr(defaults, "frequency_penalty", 0.0))
+    logprobs = parse_logprobs(body, n_ranks)
+    messages = body["messages"]
+    if not isinstance(messages, list) or not all(isinstance(m, dict) and isinstance(m.get("role"), str) and
+                                                 isinstance(m.get("content"), str) for m in messages):
+        raise ValueError("'messages' must be a list of {role, content} objects")
+    temperature = float(_number_field(body, "temperature", defaults.temperature))
+    if temperature < 0:
+        raise ValueError("'temperature' must not be negative")
+    return SimpleNamespace(messages=[(m["role"], m["content"]) for m in messages], n=n, stream=bool(body.get("stream", False)),
+                           max_tokens=int(_number_field(body, "max_tokens", -1)), temperature=temperature,
+                           topp=float(_number_field(body, "top_p", defaults.topp)),
+                           seed=int(_number_field(body, "seed", 0)) if "seed" in body else None,
+                           presence=presence, frequency=frequency, bias=bias, logprobs=logprobs)
+
+
 def logprob_entry(tokenizer, entry) -> dict:
     """The response form of one token's log-probabilities (api.run_choices on_logprobs entry): `bytes` are the token's piece,
     `token` those bytes decoded as UTF-8 with replacement."""
@@ -235,6 +273,76 @@ def choice_json(i: int, content: str, lps: Optional[LogprobsLog]) -> dict:
     return c
 
 
+class ChatResponse:
+    """The response to one chat request: its n choices' decoders, stop detectors, texts and log-probability entries, written as
+    stream chunks or as one `cmpl-j0` JSON body. echo: print the tokens' pieces to stdout."""
+
+    def __init__(self, api: "ApiServer", req: HttpRequest, chat: SimpleNamespace, echo: bool = False):
+        H, n = api.H, chat.n
+        self.req, self.stream, self.n, self.tok, self.H, self.echo = req, chat.stream, n, api.ctx.tokenizer, H, echo
+        self.dets = [H.EosDetector(*api.detector_args) for _ in range(n)]
+        self.decoders = [H.TokenDecoder() for _ in range(n)]
+        self.lps = LogprobsLog(self.tok, n) if chat.logprobs is not None else None
+        self.buffers = [""] * n
+
+    def _chunk(self, i: int, text: str) -> None:
+        self.req.write_stream_chunk("data: " + chunk_json(text, False, i, self.lps.take(i) if self.lps else None) + "\r\n\r\n")
+
+    def start(self, public: str) -> None:
+        """Every choice's text starts with the prompt's public part; a stream sends its head and that part."""
+        self.buffers = [public] * self.n
+        if self.stream:
+            self.req.write_stream_start()
+            if public:
+                for i in range(self.n):
+                    self._chunk(i, public)
+
+    def on_logprobs(self, i: int, entry) -> None:
+        self.lps.on_logprobs(i, entry)
+
+    def on_token(self, i: int, t: int) -> bool:
+        """Choice i's next token; True when it ended the choice (end of sequence or stop string)."""
+        H = self.H
+        piece = self.decoders[i].decode(self.tok, t)
+        if self.echo and piece:
+            print(piece.decode("utf-8", errors="replace"), end="", flush=True)
+        kind = self.dets[i].append(t, piece)
+        if self.lps:
+            self.lps.consumed(i, kind == H.EOS)
+        if kind in (H.NOT_EOS, H.EOS):
+            delta = self.dets[i].get_delta()
+            if delta:
+                d = delta.decode("utf-8", errors="replace")
+                if self.stream:
+                    self._chunk(i, d)
+                self.buffers[i] += d
+            self.dets[i].reset()
+        return kind == H.EOS
+
+    def finish(self, out: List[List[int]], n_prompt: int) -> None:
+        """Every choice is done (out[i]: choice i's tokens): the stop chunks and [DONE], or the JSON body."""
+        if self.stream:
+            for i in range(self.n):
+                write_stream_finish(self.req, i, self.lps)
+            self.req.write_stream_chunk("data: [DONE]")
+            self.req.write_stream_end()
+        else:
+            n_completion = sum(len(o) for o in out)
+            self.req.write_json(json.dumps({
+                "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
+                "usage": {"completion_tokens": n_completion, "prompt_tokens": n_prompt, "total_tokens": n_prompt + n_completion},
+                "choices": [choice_json(i, b, self.lps) for i, b in enumerate(self.buffers)]}))
+
+
+def remember_answer(cache: NaiveCache, P: int, out0: List[int], text: str, ctx_len: int) -> None:
+    """After a single completion of the prompt ending at P the cache keeps its answer too, unless it filled the context."""
+    end = P + len(out0)
+    if end == ctx_len:
+        cache.clear()
+    else:
+        cache.push(end, ("assistant", text))
+
+
 class ApiServer:
     def __init__(self, ctx: AppContext):
         self.ctx = ctx
@@ -246,106 +354,53 @@ class ApiServer:
         pad = max((len(x) for x in stops), default=0)
         self.detector_args = (eos_ids, stops, pad, pad)
 
+    def prepare_prompt(self, cache: NaiveCache, messages: List[Tuple[str, str]], ctx_len: int, echo: bool = False):
+        """Resolves `messages` against `cache` and records the messages still to be evaluated in it: (tokens to prefill, their
+        start position, the last prompt token, P = its position, the prompt's token count, the public prompt). echo: print
+        the prompt to stdout."""
+        delta, start = cache.resolve_delta_prompt(list(messages))
+        content, public = self.gen.generate(delta, True)
+        if echo:
+            print(f"🔹{content.decode('utf-8', errors='replace')}🔸", end="")
+        tokens = self.ctx.tokenizer.encode(content, start == 0, True)
+        P = min(start + len(tokens) - 1, ctx_len)
+        for m in delta:
+            cache.push(P, m)
+        n_pref = P - start
+        return (tokens[:n_pref], start, tokens[n_pref] if n_pref < len(tokens) else tokens[-1], P, len(tokens),
+                public.decode("utf-8", errors="replace"))
+
     def complete(self, req: HttpRequest):
         """n completions of one prompt (api.run_choices; n = 1 without `n`): the prompt is prefilled once. After one completion
         the cache keeps its answer too; after several it keeps only the prompt messages, so a follow-up that quotes any one
-        choice reuses the prompt."""
-        ctx, H = self.ctx, self.H
-        tok, inf, h, smp = ctx.tokenizer, ctx.inference, ctx.header, ctx.sampler
-        body = req.json or {}
-        n = parse_n(body)
-        # server defaults: --presence-penalty / --frequency-penalty (argument objects that predate them mean 0)
-        presence, frequency, bias = parse_controls(body, smp.vocab_size, getattr(ctx.args, "presence_penalty", 0.0),
-                                                   getattr(ctx.args, "frequency_penalty", 0.0))
-        lp_k = parse_logprobs(body, getattr(getattr(inf, "comm", None), "world_size", 1))
-        smp.set_controls(presence, frequency, bias)
-        messages = [(m["role"], m["content"]) for m in body["messages"]]
-        stream = bool(body.get("stream", False))
-        max_tokens = int(body.get("max_tokens", -1))
-        smp.set_temperature(float(body.get("temperature", ctx.args.temperature)))
-        smp.set_topp(float(body.get("top_p", ctx.args.topp)))
-        if "seed" in body:
-            smp.set_seed(int(body["seed"]))
+        choice reuses the prompt. The request's sampling settings stay with the server's sampler."""
+        ctx = self.ctx
+        inf, smp, seq_len = ctx.inference, ctx.sampler, ctx.header.seq_len
+        chat = parse_chat(req.json, ctx.args, smp.vocab_size, MAX_CHOICES, getattr(getattr(inf, "comm", None), "world_size", 1))
+        smp.set_controls(chat.presence, chat.frequency, chat.bias)
+        smp.set_temperature(chat.temperature)
+        smp.set_topp(chat.topp)
+        if chat.seed is not None:
+            smp.set_seed(chat.seed)
         # several completions: choice i uses choice_seed(base, i); without a seed the base is drawn from the advancing generator
-        base_seed = smp.seed if "seed" in body else (smp.next_seed() if n > 1 else 0)
-        delta_prompt, start_pos = self.cache.resolve_delta_prompt(list(messages))
-        content, public = self.gen.generate(delta_prompt, True)
-        print(f"🔹{content.decode('utf-8', errors='replace')}🔸", end="")
-        tokens = tok.encode(content, start_pos == 0, True)
-        n_prompt = len(tokens)
-        prompt_end = min(start_pos + n_prompt - 1, h.seq_len)
-        for m in delta_prompt:
-            self.cache.push(prompt_end, m)
-        dets = [H.EosDetector(*self.detector_args) for _ in range(n)]
-        decoders = [H.TokenDecoder() for _ in range(n)]
-        p = public.decode("utf-8", errors="replace")
-        buffers = [p] * n
-        lps = LogprobsLog(tok, n) if lp_k is not None else None
-        if stream:
-            req.write_stream_start()
-            if p:
-                for i in range(n):
-                    req.write_stream_chunk("data: " + chunk_json(p, False, i, lps.take(i) if lps else None) + "\r\n\r\n")
-        n_pref = prompt_end - start_pos
-        inf.prefill(tokens[:n_pref], start_pos)
-        token = tokens[n_pref] if n_pref < len(tokens) else tokens[-1]
-
-        def on_token(i: int, t: int) -> bool:
-            piece = decoders[i].decode(tok, t)
-            if n == 1 and piece:
-                print(piece.decode("utf-8", errors="replace"), end="", flush=True)
-            kind = dets[i].append(t, piece)
-            if lps:
-                lps.consumed(i, kind == H.EOS)
-            if kind in (H.NOT_EOS, H.EOS):
-                delta = dets[i].get_delta()
-                if delta:
-                    d = delta.decode("utf-8", errors="replace")
-                    if stream:
-                        req.write_stream_chunk("data: " + chunk_json(d, False, i, lps.take(i) if lps else None) + "\r\n\r\n")
-                    buffers[i] += d
-                dets[i].reset()
-            return kind == H.EOS
-
-        out = run_choices(inf, token, prompt_end, n, max_tokens, h.seq_len, smp, base_seed, on_token,
-                          **({"logprobs": lp_k, "on_logprobs": lps.on_logprobs} if lps else {}))
-        if n == 1:
-            end = prompt_end + len(out[0])
-            if end == h.seq_len:
-                self.cache.clear()
-            else:
-                self.cache.push(end, ("assistant", buffers[0]))
-        if stream:
-            for i in range(n):
-                write_stream_finish(req, i, lps)
-            req.write_stream_chunk("data: [DONE]")
-            req.write_stream_end()
-        else:
-            n_completion = sum(len(o) for o in out)
-            req.write_json(json.dumps({
-                "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
-                "usage": {"completion_tokens": n_completion, "prompt_tokens": n_prompt, "total_tokens": n_prompt + n_completion},
-                "choices": [choice_json(i, b, lps) for i, b in enumerate(buffers)]}))
-        print("🔶" if n == 1 else f"({n} choices)🔶")
+        base_seed = smp.seed if chat.seed is not None else (smp.next_seed() if chat.n > 1 else 0)
+        prefill, start, token, P, n_prompt, public = self.prepare_prompt(self.cache, chat.messages, seq_len, echo=True)
+        resp = ChatResponse(self, req, chat, echo=chat.n == 1)
+        resp.start(public)
+        inf.prefill(prefill, start)
+        out = run_choices(inf, token, P, chat.n, chat.max_tokens, seq_len, smp, base_seed, resp.on_token,
+                          **({"logprobs": chat.logprobs, "on_logprobs": resp.on_logprobs} if resp.lps else {}))
+        if chat.n == 1:
+            remember_answer(self.cache, P, out[0], resp.buffers[0], seq_len)
+        resp.finish(out, n_prompt)
+        print("🔶" if chat.n == 1 else f"({chat.n} choices)🔶")
 
     def slot_request(self, req: HttpRequest, caches: List[NaiveCache], n_slots: int) -> SlotRequest:
         """A validated chat completion for SlotScheduler (--parallel > 1): the same fields, limits and responses as complete(),
         with the prompt cache of the slot the scheduler picks. Raises ValueError / KeyError on a malformed body."""
-        ctx, H = self.ctx, self.H
-        tok, smp = ctx.tokenizer, ctx.sampler
-        body = req.json or {}
-        n = parse_n(body)
-        if n > n_slots:
-            raise ValueError(f"'n' must not exceed --parallel ({n_slots})")
-        presence, frequency, bias = parse_controls(body, smp.vocab_size, getattr(ctx.args, "presence_penalty", 0.0),
-                                                   getattr(ctx.args, "frequency_penalty", 0.0))
-        messages = [(m["role"], m["content"]) for m in body["messages"]]
-        stream = bool(body.get("stream", False))
-        temperature = float(body.get("temperature", ctx.args.temperature))
-        if temperature < 0:
-            raise ValueError("'temperature' must not be negative")
-        lp_k = parse_logprobs(body)   # --parallel > 1 runs on one GPU
-        detector_args, gen = self.detector_args, self.gen
+        chat = parse_chat(req.json, self.ctx.args, self.ctx.sampler.vocab_size, n_slots, 1)   # --parallel > 1 runs on one GPU
+        resp = ChatResponse(self, req, chat)
+        api, slot_len, messages = self, self.slot_len, chat.messages
 
         class Chat(SlotRequest):
             def cached_prefix(self, slot):
@@ -354,67 +409,19 @@ class ApiServer:
                 return len(items) if ok else 0
 
             def prepare(self, slot):
-                cache = caches[slot]
-                delta, start = cache.resolve_delta_prompt(list(messages))
-                content, public = gen.generate(delta, True)
-                tokens = tok.encode(content, start == 0, True)
-                self.n_prompt = len(tokens)
-                P = min(start + len(tokens) - 1, slot_len)
-                p = public.decode("utf-8", errors="replace")
-                self.buffers = [p] * n
-                lps = self.lps
-                if stream:
-                    req.write_stream_start()
-                    if p:
-                        for i in range(n):
-                            req.write_stream_chunk("data: " + chunk_json(p, False, i, lps.take(i) if lps else None) + "\r\n\r\n")
-                for m in delta:
-                    cache.push(P, m)
-                self.slot_cache = cache
-                n_pref = P - start
-                return tokens[:n_pref], start, (tokens[n_pref] if n_pref < len(tokens) else tokens[-1]), P
+                prefill, start, token, P, self.n_prompt, public = api.prepare_prompt(caches[slot], messages, slot_len)
+                resp.start(public)
+                return prefill, start, token, P
 
-            def on_logprobs(self, i, entry):
-                self.lps.on_logprobs(i, entry)
-
-            def on_token(self, i, t):
-                piece = self.decoders[i].decode(tok, t)
-                kind = self.dets[i].append(t, piece)
-                lps = self.lps
-                if lps:
-                    lps.consumed(i, kind == H.EOS)
-                if kind in (H.NOT_EOS, H.EOS):
-                    delta = self.dets[i].get_delta()
-                    if delta:
-                        d = delta.decode("utf-8", errors="replace")
-                        if stream:
-                            req.write_stream_chunk("data: " + chunk_json(d, False, i, lps.take(i) if lps else None) + "\r\n\r\n")
-                        self.buffers[i] += d
-                    self.dets[i].reset()
-                return kind == H.EOS
+            on_logprobs, on_token = resp.on_logprobs, resp.on_token
 
             def finish(self, out, slots, P):
-                if n == 1:
-                    end = P + len(out[0])
-                    if end == slot_len:
-                        self.slot_cache.clear()
-                    else:
-                        self.slot_cache.push(end, ("assistant", self.buffers[0]))
+                if chat.n == 1:
+                    remember_answer(caches[slots[0]], P, out[0], resp.buffers[0], slot_len)
                 for s in slots[1:]:   # they hold a copy of the prompt rows
                     caches[s].items = list(caches[slots[0]].items)
-                if stream:
-                    for i in range(n):
-                        write_stream_finish(req, i, self.lps)
-                    req.write_stream_chunk("data: [DONE]")
-                    req.write_stream_end()
-                else:
-                    n_completion = sum(len(o) for o in out)
-                    req.write_json(json.dumps({
-                        "id": "cmpl-j0", "object": "chat.completion", "created": int(time.time()), "model": "Distributed Model",
-                        "usage": {"completion_tokens": n_completion, "prompt_tokens": self.n_prompt,
-                                  "total_tokens": self.n_prompt + n_completion},
-                        "choices": [choice_json(i, b, self.lps) for i, b in enumerate(self.buffers)]}))
-                print(f"🔶 slot {slots[0]}" + (f" ({n} choices)" if n > 1 else ""), flush=True)
+                resp.finish(out, self.n_prompt)
+                print(f"🔶 slot {slots[0]}" + (f" ({chat.n} choices)" if chat.n > 1 else ""), flush=True)
                 self.done()
 
             def fail(self, error, slots):
@@ -423,16 +430,8 @@ class ApiServer:
                 print(f"Socket error: {error}", flush=True)
                 self.done()
 
-        slot_len = self.slot_len
         r = Chat()
-        r.n, r.temperature, r.topp = n, temperature, float(body.get("top_p", ctx.args.topp))
-        r.presence, r.frequency, r.bias = presence, frequency, bias
-        r.seed = int(body["seed"]) if "seed" in body else None
-        r.max_tokens = int(body.get("max_tokens", -1))
-        r.logprobs = lp_k
-        r.lps = LogprobsLog(tok, n) if lp_k is not None else None
-        r.dets = [H.EosDetector(*detector_args) for _ in range(n)]
-        r.decoders = [H.TokenDecoder() for _ in range(n)]
+        vars(r).update(vars(chat))   # the SlotRequest fields: n, temperature, topp, seed, max_tokens, logprobs and the controls
         r.done = lambda: None
         return r
 

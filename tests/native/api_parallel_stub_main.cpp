@@ -1,8 +1,10 @@
 // CPU-only harness for the --parallel server of csrc/app/api_server.cpp: the real HTTP / JSON / template / stop-detector / per-slot
 // NaiveCache / scheduling code over a fake slot backend. A row's next token is a fixed function of (token, position, and its
 // slot's seed when sampling), never of the slot index or the other rows; EOS comes after `eos-after` tokens of a completion. Every
-// step sleeps `delay-ms`, so that requests overlap in time. The Python twin is SlotStub in tests/test_api_parallel.py.
-// Prints "POS <slot> <start> <n>" for every prefill and "COPY <src> <dst> <P>" for every prompt copy.
+// step sleeps `delay-ms`, so that requests overlap in time. A row's log-probability entry is a fixed float32 function of (drawn
+// token, position, k). The Python twin is SlotStub in tests/test_api_parallel.py.
+// Prints "POS <slot> <start> <n>" for every prefill, "COPY <src> <dst> <P>" for every prompt copy and "SEED <slot> <seed>" for
+// every slotSampling.
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -19,6 +21,7 @@ struct SlotStub : InferenceBackend {
     std::vector<uint64_t> seed;
     std::vector<float> temp;
     std::vector<uint32_t> produced;
+    std::vector<int> k;   // top_logprobs of each slot's draws, -1: none
     uint32_t seqLen() const override { return n * len; }
     uint32_t vocabSize() const override { return vocab; }
     void prefill(const std::vector<int32_t> &, uint32_t) override { throw std::runtime_error("single-sequence call in --parallel mode"); }
@@ -30,9 +33,25 @@ struct SlotStub : InferenceBackend {
     }
     void slotCopy(uint32_t src, uint32_t dst, uint32_t P) override { std::printf("COPY %u %u %u\n", src, dst, P); }
     void slotSampling(uint32_t slot, uint64_t s, float temperature, float, float, float, const std::vector<std::pair<int32_t, float>> &) override {
+        std::printf("SEED %u %llu\n", slot, (unsigned long long)s);
         seed[slot] = s;
         temp[slot] = temperature;
         produced[slot] = 0;
+        k[slot] = -1;
+    }
+    void slotLogprobs(uint32_t slot, int kk) override { k[slot] = kk; }
+    std::vector<int32_t> slotsStepLogprobs(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask,
+                                           std::vector<TokenLogprobs> &rows) override {
+        const std::vector<int32_t> out = slotsStep(tokens, pos, activeMask);
+        rows.assign(n, TokenLogprobs());
+        for (uint32_t b = 0; b < n; b++) {
+            if (!((activeMask >> b) & 1u) || k[b] < 0) continue;
+            TokenLogprobs &e = rows[b];
+            e.token = out[b];
+            e.logprob = -(float)(pos[b] % 7) * 0.37f;
+            for (int j = 0; j < k[b]; j++) e.top.push_back({(int32_t)((out[b] + 31 * j) % regular), -(float)j * 0.2517f - 0.001f});
+        }
+        return out;
     }
     std::vector<int32_t> slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask) override {
         std::this_thread::sleep_for(std::chrono::milliseconds(delayMs));
@@ -63,6 +82,7 @@ int main(int argc, char **argv) {
     b.seed.assign(b.n, 0);
     b.temp.assign(b.n, 0.f);
     b.produced.assign(b.n, 0);
+    b.k.assign(b.n, -1);
     ApiConfig cfg;
     cfg.host = "127.0.0.1";
     cfg.port = std::atoi(argv[2]);

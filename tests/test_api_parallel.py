@@ -9,6 +9,7 @@ import threading
 import time
 from types import SimpleNamespace
 
+import numpy as np
 import pytest
 
 from distributed_llama_b200 import host
@@ -16,23 +17,40 @@ from distributed_llama_b200 import host
 
 class SlotStub:
     """N KV-cache slots: a row's next token depends on (token, position, its slot's seed when sampling), never on the slot index
-    or on the other rows. Every call is logged."""
+    or on the other rows; its log-probability entry is a fixed float32 function of (drawn token, position, k). Every call is
+    logged, and `log` keeps the prefills, copies and seeds as the native stub prints them."""
 
     def __init__(self, slots, slot_len, regular, eos, eos_after=10, delay=0.02):
         self.slots, self.slot_len, self.regular, self.eos, self.eos_after, self.delay = slots, slot_len, regular, eos, eos_after, delay
-        self.seed, self.temp, self.produced = [0] * slots, [0.0] * slots, [0] * slots
-        self.prefills, self.copies, self.sampling = [], [], []
+        self.seed, self.temp, self.produced, self.k = [0] * slots, [0.0] * slots, [0] * slots, [None] * slots
+        self.prefills, self.copies, self.sampling, self.log = [], [], [], []
         self.max_active = 0
 
     def slot_prefill(self, slot, tokens, pos):
         self.prefills.append((slot, pos, len(tokens)))
+        self.log.append(f"POS {slot} {pos} {len(tokens)}")
 
     def slot_copy(self, src, dst, P):
         self.copies.append((src, dst, P))
+        self.log.append(f"COPY {src} {dst} {P}")
 
     def slot_sampling(self, slot, seed, temperature, topp, presence, frequency, bias):
         self.sampling.append(slot)
-        self.seed[slot], self.temp[slot], self.produced[slot] = seed, temperature, 0
+        self.log.append(f"SEED {slot} {seed}")
+        self.seed[slot], self.temp[slot], self.produced[slot], self.k[slot] = seed, temperature, 0, None
+
+    def slot_logprobs(self, slot, k):
+        self.k[slot] = k
+
+    def slots_step_logprobs(self, tokens, pos, active):
+        drawn = self.slots_step(tokens, pos, active)
+        entries = []
+        for b, t in enumerate(drawn):
+            k = self.k[b] if active[b] else None
+            entries.append(None if k is None else
+                           (t, float(-np.float32(pos[b] % 7) * np.float32(0.37)),
+                            [((t + 31 * j) % self.regular, float(-np.float32(j) * np.float32(0.2517) - np.float32(0.001))) for j in range(k)]))
+        return drawn, entries
 
     def slots_step(self, tokens, pos, active):
         time.sleep(self.delay)
