@@ -354,6 +354,7 @@ std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t 
         for (uint32_t i = 0; i < n; i++) {
             Sampler smp(sampler.vocabSize(), T, topp, seeds[i]);   // a fresh sampler: its own counts, from zero
             smp.setControls(sampler.presencePenalty(), sampler.frequencyPenalty(), sampler.logitBias());
+            smp.setFilters(sampler.topK(), sampler.minP());
             single(smp, i, i);
         }
         backend.restoreSampler(saved);
@@ -417,6 +418,22 @@ void parseControls(const JsonValue &body, uint32_t vocab, float &presence, float
     bias.assign(byId.begin(), byId.end());
 }
 
+}  // namespace
+
+void parseFilters(const JsonValue &body, uint32_t &topK, float &minP) {
+    if (const JsonValue *v = body.find("top_k")) {
+        if (!(v->kind == JsonValue::Number && v->integral && v->num >= 0 && v->num <= (double)kMaxTopK))
+            throw std::runtime_error("'top_k' must be an integer from 0 to 2147483647");
+        topK = (uint32_t)v->num;
+    }
+    if (const JsonValue *v = body.find("min_p")) {
+        if (!(v->kind == JsonValue::Number && v->num >= 0 && v->num <= 1)) throw std::runtime_error("'min_p' must be a number from 0 to 1");
+        minP = (float)v->num;
+    }
+}
+
+namespace {
+
 // A validated chat completion request: the rules of distributed_llama_b200.apps.api_server.parse_chat, except that a number field
 // that is not a number counts as absent.
 struct ChatRequest {
@@ -427,6 +444,8 @@ struct ChatRequest {
     int logprobs = -1;   // top_logprobs k, -1: none
     float temperature = 0.f, topp = 0.9f, presence = 0.f, frequency = 0.f;
     std::vector<std::pair<int32_t, float>> bias;
+    uint32_t topK = 0;   // sampling filters (parseFilters)
+    float minP = 0.f;
     uint64_t seed = 0;
 };
 
@@ -443,6 +462,9 @@ ChatRequest parseChat(const JsonValue &body, const ApiConfig &cfg, uint32_t voca
     c.presence = cfg.presencePenalty;
     c.frequency = cfg.frequencyPenalty;
     parseControls(body, vocab, c.presence, c.frequency, c.bias);
+    c.topK = cfg.topK;
+    c.minP = cfg.minP;
+    parseFilters(body, c.topK, c.minP);
     c.logprobs = parseLogprobs(body);
     for (const JsonValue &m : body.at("messages").arr) c.messages.push_back({m.at("role").str, m.at("content").str});
     c.stream = body.boolOr("stream", false);
@@ -564,6 +586,19 @@ float parsePenalty(const std::string &flag, const std::string &value) {
     return v;
 }
 
+uint32_t parseTopK(const std::string &flag, const std::string &value) {
+    bool ok = !value.empty() && value.size() <= 10;
+    for (char c : value) ok = ok && c >= '0' && c <= '9';
+    if (!ok || std::stoull(value) > kMaxTopK) throw std::runtime_error(flag + " must be an integer from 0 to 2147483647");
+    return (uint32_t)std::stoull(value);
+}
+
+float parseMinP(const std::string &flag, const std::string &value) {
+    const float v = std::stof(value);
+    if (!(v >= 0.f && v <= 1.f)) throw std::runtime_error(flag + " must be from 0 to 1");
+    return v;
+}
+
 ApiServer::ApiServer(InferenceBackend &backend, Tokenizer &tokenizer, const ApiConfig &cfg)
     : backend_(backend), tok_(tokenizer), cfg_(cfg), sampler_(std::min<uint32_t>(backend.vocabSize(), tokenizer.vocabSize()), cfg.temperature, cfg.topp, cfg.seed),
       stops_(stopPieces(tokenizer)),
@@ -581,6 +616,7 @@ void ApiServer::complete(HttpRequest &req) {
     const ChatRequest chat = parseChat(req.json, cfg_, sampler_.vocabSize(), kMaxChoices);
     backend_.setLogprobs(chat.logprobs);   // refuses where they cannot run (tensor parallelism)
     sampler_.setControls(chat.presence, chat.frequency, chat.bias);
+    sampler_.setFilters(chat.topK, chat.minP);
     sampler_.setTemperature(chat.temperature);
     sampler_.setTopp(chat.topp);
     if (chat.hasSeed) sampler_.setSeed(chat.seed);
@@ -722,6 +758,7 @@ void ApiServer::serveParallel(int srv) {
         for (size_t k = 0; k < j.slots.size(); k++)
         {
             backend_.slotSampling(j.slots[k], c.n == 1 ? seed : choiceSeed(seed, (uint32_t)k), c.temperature, c.topp, c.presence, c.frequency, c.bias);
+            if (c.topK || c.minP > 0.f) backend_.slotFilters(j.slots[k], c.topK, c.minP);
             if (c.logprobs >= 0) backend_.slotLogprobs(j.slots[k], c.logprobs);
         }
         j.limit = L - j.P;

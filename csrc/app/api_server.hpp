@@ -52,6 +52,8 @@ struct InferenceBackend {
     // seeds slot `slot`'s generator, zeroes its counts and sets its temperature (0: arg-max), top-p, penalties and logit bias
     virtual void slotSampling(uint32_t /*slot*/, uint64_t /*seed*/, float /*temperature*/, float /*topp*/, float /*presence*/, float /*frequency*/,
                               const std::vector<std::pair<int32_t, float>> & /*bias*/) { throw std::runtime_error("slots unsupported"); }
+    // slot `slot`'s top_k / min_p (Sampler::setFilters), called after slotSampling (which switches them off) only when one is on
+    virtual void slotFilters(uint32_t /*slot*/, uint32_t /*topK*/, float /*minP*/) { throw std::runtime_error("sampling filters unsupported"); }
     // row b feeds tokens[b] at pos[b] of slot b (active rows: bit b of activeMask); returns each active row's draw
     virtual std::vector<int32_t> slotsStep(const std::vector<int32_t> & /*tokens*/, const std::vector<int32_t> & /*pos*/, uint32_t /*activeMask*/) {
         throw std::runtime_error("slots unsupported");
@@ -78,7 +80,7 @@ constexpr uint32_t kMaxChoices = 8;   // the engine's widest batch: one row per 
 // C = (seqLen - 1 - P) / n, and it stops after min(maxTokens, C) tokens (maxTokens <= 0: C). A single completion (n = 1) is the
 // single-sequence loop of the CLIs instead: it stops after min(maxTokens, seqLen - P) tokens, so it may fill the context up to
 // its last row. onToken(i, token) returns true when choice i is finished. The sampler's controls apply to every choice, each with
-// its own counts from zero. Same rules as distributed_llama_b200.api.run_choices.
+// its own counts from zero, and so do its filters (top_k / min_p; choiceControls hands them to the batched path). Same rules as distributed_llama_b200.api.run_choices.
 // onLogprobs (optional, with backend.setLogprobs(k) made): called with each token's entry right before onToken(i, token).
 std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t token, uint32_t P, uint32_t n, int maxTokens, uint32_t seqLen,
                                              Sampler &sampler, uint64_t baseSeed, const std::function<bool(uint32_t, int32_t)> &onToken,
@@ -129,12 +131,21 @@ std::string logprobEntryJson(const Tokenizer &tok, const TokenLogprobs &e);
 
 // A --presence-penalty / --frequency-penalty value: a number in [-kMaxPenalty, kMaxPenalty] (throws otherwise).
 float parsePenalty(const std::string &flag, const std::string &value);
+// The request's sampling filters: `top_k` an integer from 0 to kMaxTopK, `min_p` a number from 0 to 1; absent fields keep the
+// values passed in (the server's defaults). The rules of distributed_llama_b200.apps.api_server.parse_filters (throws otherwise).
+constexpr uint32_t kMaxTopK = 2147483647u;
+void parseFilters(const JsonValue &body, uint32_t &topK, float &minP);
+// --top-k / --min-p values, in the ranges above (throws otherwise).
+uint32_t parseTopK(const std::string &flag, const std::string &value);
+float parseMinP(const std::string &flag, const std::string &value);
 
 struct ApiConfig {
     std::string host = "0.0.0.0", modelName = "model", chatTemplate;
     int port = 9990;
     float temperature = 0.8f, topp = 0.9f;
     float presencePenalty = 0.f, frequencyPenalty = 0.f;   // defaults of the request fields
+    uint32_t topK = 0;
+    float minP = 0.f;
     uint64_t seed = 0;
     int maxRequests = 0;   // 0 = serve forever
     uint32_t parallel = 1; // > 1: that many requests decoded together in KV-cache slots (serveParallel)

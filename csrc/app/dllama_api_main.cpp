@@ -51,6 +51,7 @@ struct EngineBackend : InferenceBackend {
                       const std::vector<std::pair<int32_t, float>> &bias) override {
         e.slotSampling(slot, seed, temperature, topp, presence, frequency, bias);
     }
+    void slotFilters(uint32_t slot, uint32_t topK, float minP) override { e.slotFilters(slot, topK, minP); }
     std::vector<int32_t> slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask) override {
         return e.slotsStep(tokens, pos, activeMask);
     }
@@ -97,6 +98,7 @@ std::string parallelRefusal(uint32_t parallel, uint32_t nRanks, uint32_t nExpert
 const char *kUsage =
     "Usage: dllama-api-native --model <path> --tokenizer <path> [--host <addr>] [--port <p>] [--max-seq-len <n>]\n"
     "        [--temperature <t>] [--topp <p>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]\n"
+    "        [--top-k <k>] [--min-p <p>]  sampling filters of sampled draws (default 0 = off; requests may override them)\n"
     "        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--gpu-index <i>]\n"
     "        [--kv-cache-float-type {bf16|q80}]  KV-cache storage (default bf16; q80 = int8 blocks of 32 + f16 scale)\n"
     "        [--parallel <n>]  decode up to n (1..8) chat requests together, each in its own KV-cache slot of floor(context / n)\n"
@@ -153,6 +155,8 @@ int main(int argc, char **argv) {
             else if (name == "--topp") cfg.topp = std::stof(v);
             else if (name == "--presence-penalty") cfg.presencePenalty = parsePenalty(name, v);
             else if (name == "--frequency-penalty") cfg.frequencyPenalty = parsePenalty(name, v);
+            else if (name == "--top-k") cfg.topK = parseTopK(name, v);
+            else if (name == "--min-p") cfg.minP = parseMinP(name, v);
             else if (name == "--seed") cfg.seed = std::stoull(v);
             else if (name == "--chat-template") cfg.chatTemplate = v;
             else if (name == "--gpu-index") gpu = std::max(0, std::stoi(v));

@@ -45,6 +45,8 @@ struct Args {
     uint32_t kvType = 0;    // --kv-cache-float-type: 0 = bf16, 1 = q80
     float temperature = 0.8f, topp = 0.9f;
     float presencePenalty = 0.f, frequencyPenalty = 0.f;
+    uint32_t topK = 0;      // sampling filters (Sampler::setFilters), 0 = off
+    float minP = 0.f;
     uint64_t seed = (uint64_t)std::time(nullptr);
     int gpuIndex = 0;
     uint32_t gpus = 1;
@@ -53,6 +55,7 @@ struct Args {
 const char *kUsage =
     "Usage: dllama-native {inference|perplexity|chat} --model <path> --tokenizer <path>\n"
     "        [--prompt <text>] [--steps <n>] [--temperature <t>] [--topp <p>] [--presence-penalty <p>] [--frequency-penalty <f>]\n"
+    "        [--top-k <k>] [--min-p <p>]   sampling filters of sampled draws (default 0 = off)\n"
     "        [--seed <s>] [--max-seq-len <n>] [--kv-cache-float-type {bf16|q80}]\n"
     "        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--buffer-float-type q80] [--gpu-index <i>]\n"
     "        [--gpus <n>]   tensor parallel over GPUs gpu-index .. gpu-index + n - 1 of this machine (one process per GPU)\n"
@@ -80,6 +83,8 @@ Args parse(int argc, char **argv) {
         else if (name == "--topp") a.topp = std::stof(value);
         else if (name == "--presence-penalty") a.presencePenalty = parsePenalty(name, value);
         else if (name == "--frequency-penalty") a.frequencyPenalty = parsePenalty(name, value);
+        else if (name == "--top-k") a.topK = parseTopK(name, value);
+        else if (name == "--min-p") a.minP = parseMinP(name, value);
         else if (name == "--seed") a.seed = std::stoull(value);
         else if (name == "--max-seq-len") a.maxSeqLen = (uint32_t)std::stoul(value);
         else if (name == "--kv-cache-float-type") a.kvType = parseKvCacheFloatType(value);
@@ -113,6 +118,7 @@ struct App {
         // sampling ranges over the tokenizer's vocabulary (reference src/app.cpp:243-246); padded embedding rows never win
         engine.setVocabLimit(tokenizer.vocabSize());
         sampler.setControls(a.presencePenalty, a.frequencyPenalty, {});
+        sampler.setFilters(a.topK, a.minP);
     }
 
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos) { tp.prefill(tokens, pos); }

@@ -441,6 +441,10 @@ void NativeEngine::setSamplingControls(float presence, float frequency, const st
              "dl_engine_set_sampling_controls");
 }
 
+void NativeEngine::setSamplingFilters(uint32_t topK, float minP) {
+    engCheck(dl_engine_set_sampling_filters(impl_->engine, topK, minP), "dl_engine_set_sampling_filters");
+}
+
 void NativeEngine::seedChoiceSamplers(const std::vector<uint64_t> &seeds) {
     std::vector<unsigned long long> s(seeds.begin(), seeds.end());
     engCheck(dl_engine_sampler_seed_rows(impl_->engine, s.data(), (int)s.size()), "dl_engine_sampler_seed_rows");
@@ -511,6 +515,10 @@ void NativeEngine::slotSampling(uint32_t slot, uint64_t seed, float temperature,
     for (const auto &b : bias) { ids.push_back(b.first); vals.push_back(b.second); }
     engCheck(dl_engine_slot_sampling(impl_->engine, slot, seed, temperature, topp, presence, frequency, ids.data(), vals.data(), (int)ids.size(),
                                      impl_->stream), "dl_engine_slot_sampling");
+}
+
+void NativeEngine::slotFilters(uint32_t slot, uint32_t topK, float minP) {
+    engCheck(dl_engine_slot_filters(impl_->engine, slot, topK, minP), "dl_engine_slot_filters");
 }
 
 std::vector<int32_t> NativeEngine::slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask) {

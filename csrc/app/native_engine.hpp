@@ -72,6 +72,9 @@ public:
     // rowMask (bit 0: stepSampled, bit 1 + i: choice i). All zero: off. With controls on, stepSampled and the choices steps accept
     // temperature 0 (arg-max of the controlled logits). Every rank must make the same call.
     void setSamplingControls(float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias, uint32_t rowMask);
+    // top_k / min_p (dl::Sampler::setFilters) of the following sampled device draws of stepSampled and the choices; 0 / 0: off.
+    // They persist until changed. Every rank must make the same call.
+    void setSamplingFilters(uint32_t topK, float minP);
     // Several completions of one prompt (csrc/cuda/attn_decode.cu), dense models, n <= 8: generators of the batched sampler (separate
     // from the single-sequence one), first draws from the logits of `token` at P, one batched step (see InferenceBackend).
     bool supportsChoices(uint32_t n) const { return n >= 1 && n <= maxBatch_ && h_.nExperts == 0; }
@@ -87,6 +90,7 @@ public:
     void slotCopy(uint32_t src, uint32_t dst, uint32_t P);
     void slotSampling(uint32_t slot, uint64_t seed, float temperature, float topp, float presence, float frequency,
                       const std::vector<std::pair<int32_t, float>> &bias);
+    void slotFilters(uint32_t slot, uint32_t topK, float minP);   // off again after every slotSampling
     std::vector<int32_t> slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t activeMask);
     // Log-probabilities (csrc/cuda/logprobs.cu, one GPU): setLogprobs(k) makes the following stepGreedy / stepSampled / choicesFirst /
     // choicesStep also compute them for their draws (k top entries, -1: off); logprobsBlocks() holds the result blocks of the last

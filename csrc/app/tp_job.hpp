@@ -26,7 +26,8 @@ namespace dl {
 
 enum : uint32_t { TP_OP_PREFILL = 1, TP_OP_STEP_GREEDY = 2, TP_OP_STEP_SAMPLED = 3, TP_OP_EXIT = 4, TP_OP_SEED = 5,
                   TP_OP_CHOICES_SEED = 6, TP_OP_CHOICES_FIRST = 7, TP_OP_CHOICES_STEP = 8,
-                  TP_OP_CONTROLS = 9 };   // penalties in (temperature, topp), count-row mask in pos, tokens = (id, bias bits) pairs
+                  TP_OP_CONTROLS = 9,     // penalties in (temperature, topp), count-row mask in pos, tokens = (id, bias bits) pairs
+                  TP_OP_FILTERS = 10 };   // sampling filters: top_k in pos, min_p in temperature
 constexpr uint32_t kTpMaxRanks = 8, kTpCtrlTokens = 256;
 
 struct TpControl {
@@ -118,6 +119,8 @@ struct TpEngine {
     uint64_t savedGen = ~0ull, savedSeed = 0;
     std::vector<float> hostLogits = {};     // the host sampler's copy of the logits (one GPU)
     uint64_t controlsGen = 0;               // completion generation whose controls the devices hold for stepSampled (0: off)
+    uint32_t filtersTopK = 0;               // the sampling filters every rank holds
+    float filtersMinP = 0.f;
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos) {
         for (size_t i = 0; i < tokens.size(); i += 192) {   // one control packet per tensor-core chunk
             const uint32_t n = (uint32_t)std::min<size_t>(192, tokens.size() - i);
@@ -156,6 +159,7 @@ struct TpEngine {
             setControls(sampler, 1u);
             controlsGen = gen;
         }
+        setFilters(sampler);
         if (sampler.temperature() != 0.f && (sampler.seedGeneration() != seedGen || sampler.seed() != seedOf)) {
             seedGen = sampler.seedGeneration();
             seedOf = sampler.seed();
@@ -176,8 +180,18 @@ struct TpEngine {
         job.issue(TP_OP_CONTROLS, w.data(), (uint32_t)w.size(), rowMask, sampler.presencePenalty(), sampler.frequencyPenalty());
         engine.setSamplingControls(sampler.presencePenalty(), sampler.frequencyPenalty(), sampler.logitBias(), rowMask);
     }
-    // the batched choices' controls (count rows 1..n zeroed)
+    // The sampler's top_k / min_p on every rank before the first draw that uses them: each rank draws from the gathered logits
+    // with its own generator, so all ranks must hold the same filters.
+    void setFilters(const Sampler &sampler) {
+        if (sampler.topK() == filtersTopK && sampler.minP() == filtersMinP) return;
+        job.issue(TP_OP_FILTERS, nullptr, 0, sampler.topK(), sampler.minP());
+        engine.setSamplingFilters(sampler.topK(), sampler.minP());
+        filtersTopK = sampler.topK();
+        filtersMinP = sampler.minP();
+    }
+    // the batched choices' controls (count rows 1..n zeroed) and filters
     void choiceControls(const Sampler &sampler, uint32_t n) {
+        setFilters(sampler);
         if (!sampler.controlsActive() && controlsGen == 0) return;
         setControls(sampler, ((1u << n) - 1u) << 1);
         controlsGen = sampler.controlsActive() ? ~0ull : 0;   // row 0's counts are not this sampler's
@@ -253,6 +267,7 @@ inline int tpWorkerMain(const std::string &model, const std::string &tokenizer, 
             else if (c.op == TP_OP_STEP_SAMPLED) engine.stepSampled(c.tokens[0], c.pos, c.temperature, c.topp);
             else if (c.op == TP_OP_SEED) engine.seedSampler(c.seed);
             else if (c.op == TP_OP_CONTROLS) engine.setSamplingControls(c.temperature, c.topp, tpControlBias(c.tokens, c.n), c.pos);
+            else if (c.op == TP_OP_FILTERS) engine.setSamplingFilters(c.pos, c.temperature);
             else if (c.op == TP_OP_CHOICES_SEED) engine.seedChoiceSamplers(tpChoiceSeeds(c.tokens, c.n));
             else if (c.op == TP_OP_CHOICES_FIRST) engine.choicesFirst(c.tokens[0], c.pos, (uint32_t)c.tokens[1], c.temperature, c.topp);
             else if (c.op == TP_OP_CHOICES_STEP)

@@ -56,10 +56,13 @@ struct Engine {
     float *ctlBias = nullptr;
     bool ctlActive = false, ctlBiasActive = false;
     float ctlPresence = 0.f, ctlFrequency = 0.f;
+    dl::SampleFilters filters{};       // top_k / min_p of the single sequence and the choices (dl_engine_set_sampling_filters)
     // KV-cache slots (dl_engine_set_slots): slots > 1 splits every layer's cache into `slots` blocks of slotLen rows
     uint32_t slots = 1, slotLen = 0;
     float *slotParams = nullptr;       // [kChoiceRngSlots][4] per-slot {temperature, top-p, presence, frequency}
     float *slotBias = nullptr;         // [kChoiceRngSlots][vocabFull] per-slot logit bias
+    dl::SampleFilters *slotFiltersDev = nullptr;   // [kChoiceRngSlots] per-slot top_k / min_p (dl_engine_slot_filters)
+    dl::SampleFilters slotFilters[8] = {};         // host copy: the step reads the device array only while one is on
     int32_t *slotStage = nullptr;      // pinned [3][kChoiceRngSlots]: tokens, positions in; drawn tokens out
     cudaEvent_t slotStaged = nullptr;  // the uploads of the staged tokens / positions are done: the buffer may be rewritten
     int slotLogprobs[8] = {-1, -1, -1, -1, -1, -1, -1, -1};   // per-slot top_logprobs k (-1: no logprobs), one per slot
@@ -482,6 +485,7 @@ DL_EXPORT void dl_engine_destroy(void *h) {
     if (e->ctlBias) cudaFree(e->ctlBias);
     if (e->slotParams) cudaFree(e->slotParams);
     if (e->slotBias) cudaFree(e->slotBias);
+    if (e->slotFiltersDev) cudaFree(e->slotFiltersDev);
     if (e->slotStage) cudaFreeHost(e->slotStage);
     if (e->slotStaged) cudaEventDestroy(e->slotStaged);
     if (e->slotLpDev) cudaFree(e->slotLpDev);
@@ -667,6 +671,19 @@ static const dl::SampleControls *activeControls(const Engine *e, uint32_t firstR
     return &ctl;
 }
 
+static bool filtersOn(const dl::SampleFilters &f) { return f.topK > 0 || f.minP > 0.f; }
+
+// The sampling filters (kernels.h: SampleFilters) of the following sampled draws of the single sequence (dl_engine_sample) and of
+// the choices (dl_engine_sample_rows): topK 0 and minP 0 switch them off. They persist until changed. Temperature-0 draws ignore
+// them. Under tensor parallelism every rank makes the same call.
+DL_EXPORT int dl_engine_set_sampling_filters(void *h, uint32_t topK, float minP) {
+    Engine *e = (Engine *)h;
+    const dl::SampleFilters f{topK, minP};
+    if (!dl::sampleFiltersValid(f)) return -54;
+    e->filters = f;
+    return 0;
+}
+
 // Samples the next token from the logits of the last forward (logitsMode 1) on the device: tokens[0] <- sample, pos[0]++, history.
 // Tensor parallel: the vocabulary slices are first gathered into every rank's arena (peer / multicast stores, no NCCL); every rank
 // then draws the same token from its own copy of the generator. With sampling controls active, temperature 0 draws the arg-max of
@@ -680,9 +697,10 @@ DL_EXPORT int dl_engine_sample(void *h, float temperature, float topp, cudaStrea
     const uint32_t n = (e->vocabLimit && e->vocabLimit < full) ? e->vocabLimit : full;
     dl::SampleControls ctlArgs;
     const dl::SampleControls *ctl = activeControls(e, 0, ctlArgs);
+    const dl::SampleFilters *filt = filtersOn(e->filters) ? &e->filters : nullptr;
     if (nR == 1)
         return dl::launchSample(e->g.logits, e->probScratch, n, temperature, topp, e->rngState, e->g.tokens, e->g.pos, e->g.history, c.seqLen,
-                                nullptr, nullptr, 1, stream, ctl);
+                                nullptr, nullptr, 1, stream, ctl, filt);
     uint8_t *mine = (uint8_t *)e->comm.arena[e->comm.rank];
     float *gatherLocal = (float *)(mine + e->comm.gatherOff);
     unsigned int *flagLocal = (unsigned int *)(mine + e->comm.flagsOff);
@@ -690,7 +708,7 @@ DL_EXPORT int dl_engine_sample(void *h, float temperature, float topp, cudaStrea
     unsigned int *flagMc = e->comm.mcArena ? (unsigned int *)((uint8_t *)e->comm.mcArena + e->comm.flagsOff) : nullptr;
     DL_TRY(dl::launchLogitsGather(e->g.logits, c.vocab, c.rank, nR, gatherMc, e->gatherUcDev, flagMc, e->flagUcDev, e->gatherBlockCounter, stream));
     return dl::launchSample(gatherLocal, e->probScratch, n, temperature, topp, e->rngState, e->g.tokens, e->g.pos, e->g.history, c.seqLen, flagLocal,
-                            e->gatherEpoch, nR, stream, ctl);
+                            e->gatherEpoch, nR, stream, ctl, filt);
 }
 
 // Seeds the n <= 8 generators of the batched sampler. They are separate from the single-sequence generator of dl_engine_sample,
@@ -719,9 +737,10 @@ DL_EXPORT int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, floa
     const uint32_t rows = firstStep ? 1u : (uint32_t)nb;
     dl::SampleControls ctlArgs;
     const dl::SampleControls *ctl = activeControls(e, 1, ctlArgs);
+    const dl::SampleFilters *filt = filtersOn(e->filters) ? &e->filters : nullptr;
     if (nR == 1)
         return dl::launchSampleRows(e->g.logits, firstStep ? 0u : c.vocab, e->probScratch, n, temperature, topp, e->rngState + kChoiceRngSlots, e->g.tokens, nb,
-                                    inactiveMask, nullptr, nullptr, 1, stream, ctl);
+                                    inactiveMask, nullptr, nullptr, 1, stream, ctl, nullptr, filt);
     uint8_t *mine = (uint8_t *)e->comm.arena[e->comm.rank];
     float *gatherLocal = (float *)(mine + e->comm.gatherOff);
     unsigned int *flagLocal = (unsigned int *)(mine + e->comm.flagsOff);
@@ -729,7 +748,7 @@ DL_EXPORT int dl_engine_sample_rows(void *h, int nb, uint32_t inactiveMask, floa
     unsigned int *flagMc = e->comm.mcArena ? (unsigned int *)((uint8_t *)e->comm.mcArena + e->comm.flagsOff) : nullptr;
     DL_TRY(dl::launchLogitsGather(e->g.logits, c.vocab, c.rank, nR, gatherMc, e->gatherUcDev, flagMc, e->flagUcDev, e->gatherBlockCounter, stream, rows));
     return dl::launchSampleRows(gatherLocal, firstStep ? 0u : full, e->probScratch, n, temperature, topp, e->rngState + kChoiceRngSlots, e->g.tokens, nb, inactiveMask,
-                                flagLocal, e->gatherEpoch, nR, stream, ctl);
+                                flagLocal, e->gatherEpoch, nR, stream, ctl, nullptr, filt);
 }
 
 // Log-probabilities of the tokens the last step drew (logprobs.cu), enqueued on `stream` behind the draw: row b of the last
@@ -918,6 +937,8 @@ DL_EXPORT int dl_engine_set_slots(void *h, uint32_t n) {
         DL_CUDA_CHECK(cudaMemset(e->slotParams, 0, kChoiceRngSlots * 4 * sizeof(float)));
         DL_CUDA_CHECK(cudaMalloc(&e->slotBias, (size_t)kChoiceRngSlots * full * sizeof(float)));
         DL_CUDA_CHECK(cudaMemset(e->slotBias, 0, (size_t)kChoiceRngSlots * full * sizeof(float)));
+        DL_CUDA_CHECK(cudaMalloc(&e->slotFiltersDev, kChoiceRngSlots * sizeof(dl::SampleFilters)));
+        DL_CUDA_CHECK(cudaMemset(e->slotFiltersDev, 0, kChoiceRngSlots * sizeof(dl::SampleFilters)));
         DL_CUDA_CHECK(cudaHostAlloc((void **)&e->slotStage, 3 * kChoiceRngSlots * sizeof(int32_t), cudaHostAllocDefault));
         DL_CUDA_CHECK(cudaEventCreateWithFlags(&e->slotStaged, cudaEventDisableTiming));
     }
@@ -976,8 +997,24 @@ DL_EXPORT int dl_engine_slot_sampling(void *h, uint32_t slot, unsigned long long
     DL_CUDA_CHECK(cudaMemcpyAsync(e->slotParams + 4 * slot, params, sizeof(params), cudaMemcpyHostToDevice, stream));
     DL_CUDA_CHECK(cudaMemcpyAsync(e->slotBias + (size_t)slot * full, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice, stream));
     DL_CUDA_CHECK(cudaMemsetAsync(e->ctlCounts + (size_t)(1 + slot) * full, 0, (size_t)full * sizeof(uint32_t), stream));
+    if (filtersOn(e->slotFilters[slot])) {   // a new sequence starts without filters (dl_engine_slot_filters)
+        e->slotFilters[slot] = dl::SampleFilters{};
+        DL_CUDA_CHECK(cudaMemsetAsync(e->slotFiltersDev + slot, 0, sizeof(dl::SampleFilters), stream));
+    }
     DL_CUDA_CHECK(cudaStreamSynchronize(stream));   // host temporaries
     e->slotLogprobs[slot] = -1;   // a new sequence starts without logprobs (dl_engine_slot_logprobs)
+    return 0;
+}
+
+// top_k / min_p (kernels.h: SampleFilters) of slot `slot`'s sampled draws, for the sequence admitted by the last
+// dl_engine_slot_sampling (which switches them off). The upload is complete when the call returns.
+DL_EXPORT int dl_engine_slot_filters(void *h, uint32_t slot, uint32_t topK, float minP) {
+    Engine *e = (Engine *)h;
+    if (e->slots < 2 || slot >= e->slots) return -64;
+    const dl::SampleFilters f{topK, minP};
+    if (!dl::sampleFiltersValid(f)) return -54;
+    DL_CUDA_CHECK(cudaMemcpy(e->slotFiltersDev + slot, &f, sizeof(f), cudaMemcpyHostToDevice));
+    e->slotFilters[slot] = f;
     return 0;
 }
 
@@ -1037,8 +1074,10 @@ DL_EXPORT int dl_engine_slots_step_logprobs(void *h, const int32_t *tokens, cons
     for (int b = (int)e->slots; b < nb; b++) mask |= 1u << b;
     const uint32_t n = (e->vocabLimit && e->vocabLimit < c.vocab) ? e->vocabLimit : c.vocab;
     const dl::SampleControls ctl{e->slotBias, e->ctlCounts + c.vocab, c.vocab, 0.f, 0.f, c.vocab};
+    bool anyFilters = false;
+    for (uint32_t b = 0; b < e->slots; b++) anyFilters = anyFilters || (!((mask >> b) & 1u) && filtersOn(e->slotFilters[b]));
     DL_TRY(dl::launchSampleRows(e->g.logits, c.vocab, e->probScratch, n, 0.f, 0.f, e->rngState + kChoiceRngSlots, e->g.tokens, (uint32_t)nb, mask,
-                                nullptr, nullptr, 1, stream, &ctl, e->slotParams));
+                                nullptr, nullptr, 1, stream, &ctl, e->slotParams, nullptr, anyFilters ? e->slotFiltersDev : nullptr));
     uint32_t lpMask = 0;
     int lpK[kChoiceRngSlots] = {};
     for (uint32_t b = 0; lpOut && b < e->slots; b++)

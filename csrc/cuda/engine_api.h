@@ -101,6 +101,9 @@ int dl_engine_sample(void *h, float temperature, float topp, cudaStream_t stream
 // bit 1 + b: choice b). All zero: off.
 int dl_engine_set_sampling_controls(void *h, float presence, float frequency, const int32_t *ids, const float *vals, int nBias, uint32_t rowMask,
                                     cudaStream_t stream);
+// top_k / min_p of the following sampled draws of the single sequence and the choices (kernels.h: SampleFilters); 0 / 0: off.
+// minP in [0, 1]. They persist until changed.
+int dl_engine_set_sampling_filters(void *h, uint32_t topK, float minP);
 // choices (several completions of one prompt, csrc/cuda/attn_decode.cu): generators 0..n-1, batched draws, one choices forward
 int dl_engine_sampler_seed_rows(void *h, const unsigned long long *seeds, int n);   // separate from the single-sequence generator
 unsigned long long dl_engine_sampler_state(void *h);   // single-sequence generator state (seed with it to continue the stream)
@@ -113,6 +116,7 @@ int dl_engine_slot_prefill(void *h, uint32_t slot, uint32_t T, uint32_t p0, cuda
 int dl_engine_slot_copy(void *h, uint32_t src, uint32_t dst, uint32_t P, cudaStream_t stream);
 int dl_engine_slot_sampling(void *h, uint32_t slot, unsigned long long seed, float temperature, float topp, float presence, float frequency,
                             const int32_t *ids, const float *vals, int nBias, cudaStream_t stream);
+int dl_engine_slot_filters(void *h, uint32_t slot, uint32_t topK, float minP);   // off after every dl_engine_slot_sampling
 int dl_engine_slots_forward(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, cudaStream_t stream);
 int dl_engine_slots_step(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, cudaStream_t stream);
 // per-token log-probabilities (csrc/cuda/logprobs.cu): results are int32 blocks of kLogprobsWords words per row,

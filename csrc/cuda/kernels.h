@@ -315,18 +315,30 @@ __device__ __forceinline__ float controlled(const SampleControls &c, float x, ui
     }
     return x;
 }
+// Optional sampling filters of a temperature > 0 draw. With e[i] = exp(x[i] / T - max(x / T)) (the sampler's unnormalised
+// probabilities), the candidate set S keeps the ids that pass both active filters: top_k keeps the topK first ids in the order
+// (e desc, id asc), min_p keeps e[i] >= f32(minP * max e). Ids outside S get e = 0 before the normaliser; a nucleus draw then
+// drops below (1 - top-p) / (|S| - 1), and |S| == 1 returns that id. topK 0 (or >= n) and minP 0 are off: the draw is exactly
+// the unfiltered one. minP must lie in [0, 1]. Temperature 0 ignores the filters (the arg-max is always in S).
+struct SampleFilters {
+    uint32_t topK;
+    float minP;
+};
+bool sampleFiltersValid(const SampleFilters &f);   // minP in [0, 1]
 int launchSample(const float *logits, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng, int *tokenOut, int *pos,
                  int *history, uint32_t historyCap, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                 cudaStream_t stream, const SampleControls *controls = nullptr);
+                 cudaStream_t stream, const SampleControls *controls = nullptr, const SampleFilters *filters = nullptr);
 int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t nRanks, float *gatherMc, float *const *gatherUcDev,
                        unsigned int *flagMc, unsigned int *const *flagUcDev, unsigned int *blockCounter, cudaStream_t stream, uint32_t rows = 1);
 // B draws, one CTA per row: row b reads logits + b * logitsStride (0: every row draws from the same logits), uses rng[b] and writes
 // tokenOut[b]. Rows whose bit is set in inactiveMask draw nothing and keep their generator state. No position advance.
 // rowParams (device [B][4], may be null): row b's {temperature, top-p, presence, frequency} in place of the scalar arguments and the
 // controls' penalties; a row with temperature 0 draws the arg-max (lowest index among ties).
+// filters (host, may be null): the filters of every row. rowFilters (device [B], may be null): row b's filters in their place.
 int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
                      int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                     cudaStream_t stream, const SampleControls *controls = nullptr, const float *rowParams = nullptr);
+                     cudaStream_t stream, const SampleControls *controls = nullptr, const float *rowParams = nullptr,
+                     const SampleFilters *filters = nullptr, const SampleFilters *rowFilters = nullptr);
 
 // Per-token log-probabilities (logprobs.cu): logprob(i) = x[i] - logsumexp(x[0..n)) of the row that drew token chosen[b], where x
 // is the logits row after the controls (the values the sampler draws from, before temperature). One CTA per row b < B whose bit

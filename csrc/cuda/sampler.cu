@@ -9,6 +9,8 @@
 // prefix arithmetic is 2^-40 fixed point in 64-bit integers, so histogram atomics are order independent: the sampler is bit
 // reproducible run to run and across ranks — under tensor parallelism every rank samples the same token from the gathered
 // logits with its own copy of the generator state, and no token broadcast is needed.
+// The filters top_k / min_p (kernels.h: SampleFilters) zero every id outside the candidate set before the normaliser; top_k finds
+// its threshold by the same radix descent over counts instead of mass (topKFilter).
 //
 // Tensor parallelism (K4, reference: gather of vocab slices to the root, src/llm.cpp:587-599): logitsGatherKernel pushes this
 // rank's vocabulary slice into every rank's gather buffer (one multimem.st per 16 bytes through the NVSwitch multicast mapping, or
@@ -41,6 +43,9 @@ struct SampleArgs {
     uint32_t logitsStride, probsStride, inactiveMask;
     SampleControls ctl;        // bias / penalties (kernels.h); row b counts at ctl.counts + b * ctl.countsStride
     const float *rowParams;    // [B][4] per-row {temperature, top-p, presence, frequency}, or null (launchSampleRows)
+    uint32_t topK;             // filters (kernels.h: SampleFilters); 0 / 0.f: off
+    float minP;
+    const SampleFilters *rowFilters;   // [B] per-row filters in place of topK / minP, or null
 };
 
 __device__ float blockMax(float v, float *red) {
@@ -166,18 +171,95 @@ __device__ Found radixFind(const SampleArgs &a, float inv, float cutoff, unsigne
     return Found{sInt[2], base + need * fStar};
 }
 
+// top_k filter over the unnormalised probabilities in a.probs (a.topK < number of nonzero-or-kept ids): finds the K-th key in
+// the order (key desc, index asc) by a radix descent over counts (4 levels x 8 bits, a 256-bin u32 histogram per level; the keys
+// are non-negative floats, so their bit patterns order like their values), then keeps every key above it and the lowest-index ties
+// up to K in all. Zeroes every other id; returns this thread's fixed-point sum over its contiguous index chunk of the kept ones.
+__device__ unsigned long long topKFilter(const SampleArgs &a, unsigned long long *histMem, unsigned long long *scratch, int *sInt) {
+    const uint32_t n = a.n, K = a.topK;
+    unsigned int *hist = reinterpret_cast<unsigned int *>(histMem);
+    const int lane = threadIdx.x & 31;
+    uint32_t prefix = 0;   // decided high bits of the K-th key
+    uint32_t above = 0;    // ids whose key is above the current prefix range
+    for (int level = 0; level < 4; level++) {
+        const int shift = 24 - 8 * level;
+        for (int b = threadIdx.x; b < 256; b += kSampThreads) hist[b] = 0;
+        __syncthreads();
+        // every thread runs the same trip count, so whole warps aggregate equal bins before the shared atomic
+        for (uint32_t base = 0; base < n; base += kSampThreads) {
+            const uint32_t i = base + threadIdx.x;
+            uint32_t bin = 256u;
+            if (i < n) {
+                const uint32_t key = __float_as_uint(a.probs[i]);
+                if (level == 0 || (key >> (shift + 8)) == prefix) bin = (key >> shift) & 255u;
+            }
+            const unsigned peers = __match_any_sync(0xffffffffu, bin);
+            if (bin < 256u && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], (unsigned)__popc(peers));
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint32_t run = above;
+            int chosen = 0;
+            for (int b = 255; b >= 0; b--) {
+                if (run + hist[b] >= K) { chosen = b; break; }
+                run += hist[b];
+            }
+            sInt[0] = chosen;
+            sInt[1] = (int)run;
+        }
+        __syncthreads();
+        prefix = (prefix << 8) | (uint32_t)sInt[0];
+        above = (uint32_t)sInt[1];
+        __syncthreads();
+    }
+    // keep the K - above lowest indices among the keys equal to the K-th key (per-thread contiguous chunks keep the index order)
+    const uint32_t chunk = (n + kSampThreads - 1) / kSampThreads;
+    const uint32_t lo = threadIdx.x * chunk, hi = min(lo + chunk, n);
+    unsigned long long ties = 0;
+    for (uint32_t i = lo; i < hi; i++) ties += (__float_as_uint(a.probs[i]) == prefix) ? 1ull : 0ull;
+    unsigned long long seen = blockExclusiveScan(ties, scratch + 8, nullptr);
+    const unsigned long long need = K - above;
+    unsigned long long sFix = 0;
+    for (uint32_t i = lo; i < hi; i++) {
+        const float e = a.probs[i];
+        const uint32_t key = __float_as_uint(e);
+        if (key > prefix || (key == prefix && seen++ < need)) sFix += toFix(e);
+        else a.probs[i] = 0.f;
+    }
+    return sFix;
+}
+
 // Temperature / top-p draw from src (logits, or the transformed logits under controls) whose maximum after division by T is m.
+// Filtered: the row's top_k / min_p (kernels.h: SampleFilters) are active; the unfiltered instance is the draw without them.
+template <bool Filtered>
 __device__ int drawSampled(const SampleArgs &a, const float *src, float m, unsigned long long *hist, unsigned long long *scratch, int *sInt,
                            float *sCoin) {
     const uint32_t n = a.n;
     // per-thread sums over contiguous chunks (index order), combined by a fixed tree
     const uint32_t chunk = (n + kSampThreads - 1) / kSampThreads;
     const uint32_t lo = threadIdx.x * chunk, hi = min(lo + chunk, n);
-    unsigned long long sFix = 0;
+    // min_p threshold: max e = expNeg(max(x / T) - m) = expNeg(m - m) (1 for a finite maximum, 0 otherwise)
+    const bool useMinP = Filtered && a.minP > 0.f;
+    const float eMax = Filtered ? expNeg(__fsub_rn(m, m)) : 0.f;
+    const float thr = useMinP ? __fmul_rn(a.minP, eMax) : 0.f;
+    unsigned long long sFix = 0, kept = 0;
     for (uint32_t i = lo; i < hi; i++) {
-        const float e = expNeg(__fsub_rn(__fdiv_rn(src[i], a.temperature), m));
+        float e = expNeg(__fsub_rn(__fdiv_rn(src[i], a.temperature), m));
+        if (useMinP) {
+            if (e < thr) e = 0.f;
+            else kept++;
+        }
         a.probs[i] = e;
         sFix += toFix(e);
+    }
+    unsigned long long nS = n;   // |S|: ids in the candidate set
+    if (Filtered) {
+        if (useMinP) (void)blockExclusiveScan(kept, scratch + 8, &nS);
+        if (a.topK && a.topK < nS) {
+            __syncthreads();
+            sFix = topKFilter(a, hist, scratch, sInt);
+            nS = a.topK;
+        }
     }
     unsigned long long sTotal = 0;
     (void)blockExclusiveScan(sFix, scratch + 8, &sTotal);
@@ -189,8 +271,16 @@ __device__ int drawSampled(const SampleArgs &a, const float *src, float m, unsig
         const uint32_t u = (uint32_t)((st * 0x2545F4914F6CDD1Dull) >> 32);
         *sCoin = (float)(u >> 8) * 5.9604644775390625e-8f;   // / 2^24, exact
         sInt[2] = (int)n - 1;
+        if (Filtered) sInt[3] = (int)n - 1;
     }
     __syncthreads();
+    if (Filtered && nS == 1) {   // one candidate: the id holding max e (the coin is drawn all the same)
+        for (uint32_t i = threadIdx.x; i < n; i += kSampThreads) {
+            if (a.probs[i] == eMax) { atomicMin(&sInt[3], (int)i); break; }
+        }
+        __syncthreads();
+        return sInt[3];
+    }
     const float coin = *sCoin;
     if (a.topp <= 0.f || a.topp >= 1.f) {
         // multinomial walk in index order
@@ -209,7 +299,7 @@ __device__ int drawSampled(const SampleArgs &a, const float *src, float m, unsig
         __syncthreads();
         return sInt[2];
     }
-    const float cutoff = __fdiv_rn(1.0f - a.topp, (float)(n - 1));
+    const float cutoff = __fdiv_rn(1.0f - a.topp, (float)((Filtered ? (uint32_t)nS : n) - 1));
     const Found cut = radixFind(a, inv, cutoff, toFix(a.topp), hist, scratch, sInt);
     // r = coin * cumulative (the reference multiplies the float prefix sum)
     const float cumulative = __fdiv_rn((float)cut.prefix, kFix);
@@ -237,6 +327,7 @@ __global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
         const float *rp = a.rowParams + 4 * (size_t)row;
         a.temperature = rp[0]; a.topp = rp[1]; a.ctl.presence = rp[2]; a.ctl.frequency = rp[3];
     }
+    if (a.rowFilters) { a.topK = a.rowFilters[row].topK; a.minP = a.rowFilters[row].minP; }
     if (a.gatherFlag && a.nRanks > 1) {
         if (threadIdx.x == 0) {
             const unsigned int want = (*a.gatherEpoch + 1u) * a.nRanks;
@@ -269,8 +360,10 @@ __global__ void __launch_bounds__(kSampThreads, 1) sampleKernel(SampleArgs a) {
         }
         __syncthreads();
         token = sInt[3];
+    } else if ((a.topK && a.topK < n) || a.minP > 0.f) {
+        token = drawSampled<true>(a, src, m, hist, scratch, sInt, &sCoin);
     } else {
-        token = drawSampled(a, src, m, hist, scratch, sInt, &sCoin);
+        token = drawSampled<false>(a, src, m, hist, scratch, sInt, &sCoin);
     }
     if (threadIdx.x == 0) {
         a.tokenOut[0] = token;
@@ -316,14 +409,18 @@ __global__ void __launch_bounds__(256) logitsGatherKernel(const float *local, ui
 
 }  // namespace
 
+bool sampleFiltersValid(const SampleFilters &f) { return f.minP >= 0.f && f.minP <= 1.f; }
+
 int launchSample(const float *logits, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng, int *tokenOut, int *pos,
                  int *history, uint32_t historyCap, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                 cudaStream_t stream, const SampleControls *controls) {
+                 cudaStream_t stream, const SampleControls *controls, const SampleFilters *filters) {
     if (n < 2 || !(temperature > 0.f || (temperature == 0.f && controls))) return -1;
+    if (filters && !sampleFiltersValid(*filters)) return -2;
     SampleArgs a{};
     a.logits = logits; a.probs = probs; a.n = n; a.temperature = temperature; a.topp = topp; a.rng = rng; a.tokenOut = tokenOut; a.pos = pos;
     a.history = history; a.historyCap = historyCap; a.gatherFlag = gatherFlag; a.gatherEpoch = gatherEpoch; a.nRanks = nRanks;
     if (controls) a.ctl = *controls;
+    if (filters) { a.topK = filters->topK; a.minP = filters->minP; }
     sampleKernel<<<1, kSampThreads, 0, stream>>>(a);
     DL_CUDA_CHECK(cudaGetLastError());
     return 0;
@@ -339,13 +436,17 @@ int launchLogitsGather(const float *local, uint32_t v0, uint32_t rank, uint32_t 
 
 int launchSampleRows(const float *logits, uint32_t logitsStride, float *probs, uint32_t n, float temperature, float topp, unsigned long long *rng,
                      int *tokenOut, uint32_t B, uint32_t inactiveMask, const unsigned int *gatherFlag, unsigned int *gatherEpoch, uint32_t nRanks,
-                     cudaStream_t stream, const SampleControls *controls, const float *rowParams) {
+                     cudaStream_t stream, const SampleControls *controls, const float *rowParams, const SampleFilters *filters,
+                     const SampleFilters *rowFilters) {
     if (n < 2 || !(temperature > 0.f || (temperature == 0.f && (controls || rowParams))) || B < 1 || B > 32) return -1;
+    if (filters && !sampleFiltersValid(*filters)) return -2;
     SampleArgs a{};
     a.logits = logits; a.probs = probs; a.n = n; a.temperature = temperature; a.topp = topp; a.rng = rng; a.tokenOut = tokenOut;
     a.gatherFlag = gatherFlag; a.gatherEpoch = gatherEpoch; a.nRanks = nRanks;
     a.logitsStride = logitsStride; a.probsStride = n; a.inactiveMask = inactiveMask; a.rowParams = rowParams;
     if (controls) a.ctl = *controls;
+    if (filters) { a.topK = filters->topK; a.minP = filters->minP; }
+    a.rowFilters = rowFilters;
     sampleKernel<<<B, kSampThreads, 0, stream>>>(a);
     DL_CUDA_CHECK(cudaGetLastError());
     if (gatherFlag && nRanks > 1 && B > 1) {
@@ -389,4 +490,21 @@ DL_EXPORT int dl_sample_rows_per_row(const float *logits, uint32_t logitsStride,
     dl::SampleControls ctl{bias, counts, countsStride, 0.f, 0.f, biasStride};
     return dl::launchSampleRows(logits, logitsStride, probsScratch, n, 0.f, 0.f, rngState, tokenOut, B, inactiveMask, nullptr, nullptr, 1, stream,
                                 (bias || counts) ? &ctl : nullptr, rowParams);
+}
+
+// dl_sample_logits with the filters (kernels.h: SampleFilters) topK / minP.
+DL_EXPORT int dl_sample_logits_filtered(const float *logits, float *probsScratch, uint32_t n, float temperature, float topp, uint32_t topK,
+                                        float minP, unsigned long long *rngState, int *tokenOut, cudaStream_t stream) {
+    const dl::SampleFilters f{topK, minP};
+    return dl::launchSample(logits, probsScratch, n, temperature, topp, rngState, tokenOut, nullptr, nullptr, 0, nullptr, nullptr, 1, stream,
+                            nullptr, &f);
+}
+
+// dl_sample_rows_per_row with per-row filters: rowFilters (device [B] {u32 topK, f32 minP}, may be null) holds row b's filters.
+DL_EXPORT int dl_sample_rows_filtered(const float *logits, uint32_t logitsStride, float *probsScratch, uint32_t n, const float *rowParams,
+                                      const void *rowFilters, unsigned long long *rngState, int *tokenOut, uint32_t B, uint32_t inactiveMask,
+                                      const float *bias, uint32_t biasStride, uint32_t *counts, uint32_t countsStride, cudaStream_t stream) {
+    dl::SampleControls ctl{bias, counts, countsStride, 0.f, 0.f, biasStride};
+    return dl::launchSampleRows(logits, logitsStride, probsScratch, n, 0.f, 0.f, rngState, tokenOut, B, inactiveMask, nullptr, nullptr, 1, stream,
+                                (bias || counts) ? &ctl : nullptr, rowParams, nullptr, (const dl::SampleFilters *)rowFilters);
 }

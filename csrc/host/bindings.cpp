@@ -196,6 +196,10 @@ PYBIND11_MODULE(_host, m) {
         .def("set_controls", [](Sampler &s, float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias) {
             s.setControls(presence, frequency, bias);
         }, py::arg("presence_penalty"), py::arg("frequency_penalty"), py::arg("logit_bias") = std::vector<std::pair<int32_t, float>>{})
+        .def("set_filters", &Sampler::setFilters, py::arg("top_k"), py::arg("min_p"))
+        .def_property_readonly("top_k", &Sampler::topK)
+        .def_property_readonly("min_p", &Sampler::minP)
+        .def_property_readonly("filters_active", &Sampler::filtersActive)
         .def("begin_completion", &Sampler::beginCompletion)
         .def("apply_controls", [](const Sampler &s, F32Array logits) {
             if ((uint32_t)logits.size() < s.vocabSize()) throw std::invalid_argument("Sampler: logits shorter than vocab size");

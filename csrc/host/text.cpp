@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cstring>
 #include <fstream>
+#include <functional>
 #include <stdexcept>
 
 namespace dl {
@@ -296,6 +297,44 @@ void Sampler::setControls(float presence, float frequency, const std::vector<std
     completion_ = nextCompletionGeneration();
 }
 
+void Sampler::setFilters(uint32_t topK, float minP) {
+    if (!(minP >= 0.f && minP <= 1.f)) throw std::invalid_argument("min_p must lie in [0, 1]");
+    topK_ = topK;
+    minP_ = minP;
+}
+
+// Without FMA, like applyControls: the min_p threshold is one rounded multiply, as the device's __fmul_rn.
+uint32_t Sampler::applyFilters(float *e) {
+    const uint32_t n = vocabSize_;
+    uint32_t kept = n;
+    if (minP_ > 0.f) {
+        float eMax = 0.f;
+        for (uint32_t i = 0; i < n; i++) eMax = std::max(eMax, e[i]);
+        const float thr = minP_ * eMax;
+        kept = 0;
+        for (uint32_t i = 0; i < n; i++) {
+            if (e[i] < thr) e[i] = 0.f;
+            else kept++;
+        }
+    }
+    if (topK_ > 0 && topK_ < kept) {
+        // the K-th value of the order (e desc, id asc); every id above it stays, and the lowest ids among its ties up to K in all
+        keys_.assign(e, e + n);
+        std::nth_element(keys_.begin(), keys_.begin() + (topK_ - 1), keys_.end(), std::greater<float>());
+        const float kth = keys_[topK_ - 1];
+        uint32_t above = 0;
+        for (uint32_t i = 0; i < n; i++) above += e[i] > kth ? 1u : 0u;
+        uint32_t ties = topK_ - above;
+        for (uint32_t i = 0; i < n; i++) {
+            if (e[i] > kth) continue;
+            if (e[i] == kth && ties > 0) { ties--; continue; }
+            e[i] = 0.f;
+        }
+        kept = topK_;
+    }
+    return kept;
+}
+
 void Sampler::beginCompletion() {
     std::fill(counts_.begin(), counts_.end(), 0u);
     completion_ = nextCompletionGeneration();
@@ -336,9 +375,21 @@ int32_t Sampler::draw(float *logits) {
     for (int i = 0; i < n; i++) { logits[i] /= temperature_; mx = std::max(mx, logits[i]); }
     uint64_t sumFix = 0;
     for (int i = 0; i < n; i++) { logits[i] = expNeg(logits[i] - mx); sumFix += (uint64_t)(logits[i] * 1099511627776.0f); }
+    int nS = n;   // |S|: the candidates left by the filters
+    int single = -1;
+    if (filtersActive()) {
+        nS = (int)applyFilters(logits);
+        sumFix = 0;
+        for (int i = 0; i < n; i++) sumFix += (uint64_t)(logits[i] * 1099511627776.0f);
+        if (nS == 1) {   // the one candidate: the lowest id holding the largest value
+            single = 0;
+            for (int i = 1; i < n; i++) if (logits[i] > logits[single]) single = i;
+        }
+    }
     const float inv = 1.0f / ((float)sumFix / 1099511627776.0f);
     for (int i = 0; i < n; i++) logits[i] *= inv;
     const float coin = rng_.nextF32();
+    if (single >= 0) return single;
     // Prefix sums run in 2^-40 fixed point (64-bit integers): exact and order independent, so the device sampler
     // (csrc/cuda/sampler.cu), which adds the same terms in parallel, reaches the same decisions. The reference accumulates the same
     // sums in float (src/tokenizer.cpp:405-467); the two differ only when the coin falls within float rounding of a boundary.
@@ -350,7 +401,7 @@ int32_t Sampler::draw(float *logits) {
         return n - 1;
     }
     // nucleus: tokens below (1-p)/(n-1) can never be inside the top-p set, drop them before sorting
-    const float cutoff = (1.0f - topp_) / (float)(n - 1);
+    const float cutoff = (1.0f - topp_) / (float)(nS - 1);
     candidates_.clear();
     for (int i = 0; i < n; i++) if (logits[i] >= cutoff) candidates_.push_back({logits[i], i});
     std::sort(candidates_.begin(), candidates_.end(), [](const std::pair<float, int32_t> &a, const std::pair<float, int32_t> &b) {

@@ -97,6 +97,15 @@ public:
     // Setting the controls starts a new completion (counts from zero, a new completion generation), so device-side copies keyed
     // on the generation always hold the controls in force.
     void setControls(float presence, float frequency, const std::vector<std::pair<int32_t, float>> &bias);
+    // Sampling filters of the following temperature > 0 draws (top_k, min_p); they persist until changed. With e[i] =
+    // exp(x[i] / T - max(x / T)) from the shared exp, the candidate set S keeps the ids that pass both active filters: top_k the
+    // topK first ids in the order (e desc, id asc), min_p those with e[i] >= f32(minP * max e). Ids outside S get e = 0 before
+    // the fixed-point normaliser, the nucleus pre-filter divides by |S| - 1, and |S| == 1 returns that id (the coin is drawn
+    // all the same). topK 0 (or >= vocabSize) and minP 0 are off. The device sampler computes the same set.
+    void setFilters(uint32_t topK, float minP);   // minP in [0, 1]
+    uint32_t topK() const { return topK_; }
+    float minP() const { return minP_; }
+    bool filtersActive() const { return (topK_ > 0 && topK_ < vocabSize_) || minP_ > 0.f; }
     // Starts a completion: zeroes the counts and takes a new completion generation.
     void beginCompletion();
     void applyControls(float *logits) const;   // the transform above, in place ([vocabSize])
@@ -123,7 +132,11 @@ public:
 
 private:
     int32_t draw(float *logits);            // greedy / temperature / top-p draw
+    uint32_t applyFilters(float *e);        // zeroes e outside S, returns |S|
     uint32_t vocabSize_;
+    uint32_t topK_ = 0;
+    float minP_ = 0.f;
+    std::vector<float> keys_;
     float temperature_, topp_;
     Rng rng_;
     uint64_t seed_ = 0;

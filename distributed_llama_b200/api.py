@@ -57,7 +57,8 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     of `token` (once on the batched path, once per choice, with the same values, on the sequential path). The single-sequence
     generator continues its stream afterwards. on_token(i, tok) is called for every generated token and returns True when
     choice i is finished (end of sequence or stop string). The sampler's controls (presence / frequency penalty, logit bias)
-    apply to every choice, each with its own token counts, which start at zero. `backend` provides
+    apply to every choice, each with its own token counts, which start at zero, and so do its filters (top_k, min_p; the
+    backend's choice_controls hands them to the batched path). `backend` provides
     next_token(token, pos, sampler), forget_device_seed(), save_sampler() / restore_sampler(saved), and for the batched path
     batched_choices(n), seed_choices(seeds), choice_controls(sampler, n), choices_first(token, P, n, T, topp) and
     choices_step(tokens, P, C, j, active, T, topp) (InferenceSession and apps.runtime.RootInference). Returns each choice's
@@ -110,6 +111,7 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
                 backend.forget_device_seed()
                 smp = H.Sampler(sampler.vocab_size, T, topp, seeds[i])   # a fresh sampler: its own counts, from zero
                 smp.set_controls(sampler.presence_penalty, sampler.frequency_penalty, sampler.logit_bias)
+                smp.set_filters(sampler.top_k, sampler.min_p)
                 single(smp, [i])
         finally:
             backend.restore_sampler(saved)
@@ -160,12 +162,13 @@ class SlotRequest:
     """One request of a SlotScheduler. The server fills in the fields and overrides the hooks; the scheduler calls them on its
     engine thread.
 
-    n: completions; temperature / topp / presence / frequency / bias: the sampling settings; seed: the request's seed or None;
-    max_tokens (<= 0: no limit but the slot's context); logprobs: k (0..20) top entries of the log-probabilities of every
-    token, passed to on_logprobs, or None."""
+    n: completions; temperature / topp / presence / frequency / bias / top_k / min_p: the sampling settings; seed: the
+    request's seed or None; max_tokens (<= 0: no limit but the slot's context); logprobs: k (0..20) top entries of the
+    log-probabilities of every token, passed to on_logprobs, or None."""
     n = 1
     temperature, topp, presence, frequency = 0.0, 0.9, 0.0, 0.0
     bias: Sequence = ()
+    top_k, min_p = 0, 0.0
     seed: Optional[int] = None
     max_tokens = -1
     logprobs: Optional[int] = None
@@ -208,8 +211,8 @@ class SlotScheduler:
     and frees its slots; the other requests continue.
 
     `backend` provides slots, slot_len, slot_prefill(slot, tokens, pos), slot_copy(src, dst, P),
-    slot_sampling(slot, seed, temperature, topp, presence, frequency, bias) and slots_step(tokens, pos, active)
-    (InferenceSession(parallel=N)); for requests with logprobs also slot_logprobs(slot, k) and slots_step_logprobs(tokens, pos,
+    slot_sampling(slot, seed, temperature, topp, presence, frequency, bias, top_k=.., min_p=..) (the filters are passed only
+    when one is on) and slots_step(tokens, pos, active) (InferenceSession(parallel=N)); for requests with logprobs also slot_logprobs(slot, k) and slots_step_logprobs(tokens, pos,
     active) -> (draws, per-slot entries), used only while such a request holds a slot."""
 
     def __init__(self, backend, seed_source: Callable[[], int]):
@@ -250,7 +253,8 @@ class SlotScheduler:
         seed = req.seed if req.seed is not None else (self.seed_source() if req.temperature != 0.0 else 0)
         seeds = [seed] if req.n == 1 else [host().choice_seed(seed, i) for i in range(len(slots))]
         for s, sd in zip(slots, seeds):
-            be.slot_sampling(s, sd, req.temperature, req.topp, req.presence, req.frequency, req.bias)
+            filters = {"top_k": req.top_k, "min_p": req.min_p} if (req.top_k or req.min_p) else {}
+            be.slot_sampling(s, sd, req.temperature, req.topp, req.presence, req.frequency, req.bias, **filters)
             if req.logprobs is not None:
                 be.slot_logprobs(s, req.logprobs)
         limit = be.slot_len - P
@@ -339,10 +343,11 @@ class InferenceSession:
                  temperature: float = 0.0, topp: float = 0.9, seed: int = 12345, device: Optional[str] = None,
                  max_batch: int = 8, use_pdl: bool = True, comm=None, moe_mode: str = "auto", presence_penalty: float = 0.0,
                  frequency_penalty: float = 0.0, logit_bias: Optional[dict] = None, parallel: int = 1,
-                 kv_cache_float_type: str = "bf16"):
+                 kv_cache_float_type: str = "bf16", top_k: int = 0, min_p: float = 0.0):
         """presence_penalty, frequency_penalty and logit_bias ({token id: value}) are the sampling controls of every
         completion (host Sampler.set_controls; they may be changed later through self.sampler.set_controls, which restarts the
-        counts of the current completion). parallel > 1 splits the KV cache into that many slots for SlotScheduler
+        counts of the current completion). top_k and min_p are the sampling filters of every sampled draw (host
+        Sampler.set_filters, 0: off; self.sampler.set_filters changes them). parallel > 1 splits the KV cache into that many slots for SlotScheduler
         (slot_prefill, slot_copy, slot_sampling, slots_step); the single-sequence calls then must not be used.
         kv_cache_float_type: "bf16" or "q80" (runtime.engine.Engine)."""
         from .models.loader import load_device_weights
@@ -366,11 +371,13 @@ class InferenceSession:
         vocab = self.tokenizer.vocab_size if self.tokenizer else self.header.vocab_size
         self.sampler = H.Sampler(vocab, temperature, topp, seed)
         self.sampler.set_controls(presence_penalty, frequency_penalty, sorted((int(k), float(v)) for k, v in (logit_bias or {}).items()))
+        self.sampler.set_filters(top_k, min_p)
         if self.tokenizer and self.tokenizer.vocab_size < self.header.vocab_size:
             self.engine.set_vocab_limit(self.tokenizer.vocab_size)
         self.pos = 0
         self._dev_seeded = None
         self._dev_controls = None   # completion generation whose controls the device holds (None: off)
+        self._dev_filters = (0, 0.0)   # (top_k, min_p) the device holds
         self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory()
         self._pin_out = torch.zeros(1, dtype=torch.int32).pin_memory()
         self.slots = parallel
@@ -385,8 +392,9 @@ class InferenceSession:
     def slot_copy(self, src: int, dst: int, P: int) -> None:
         self.engine.slot_copy(src, dst, P)
 
-    def slot_sampling(self, slot: int, seed: int, temperature: float, topp: float, presence: float, frequency: float, bias) -> None:
-        self.engine.slot_sampling(slot, seed, temperature, topp, presence, frequency, bias)
+    def slot_sampling(self, slot: int, seed: int, temperature: float, topp: float, presence: float, frequency: float, bias, *,
+                      top_k: int = 0, min_p: float = 0.0) -> None:
+        self.engine.slot_sampling(slot, seed, temperature, topp, presence, frequency, bias, top_k=top_k, min_p=min_p)
 
     def slots_step(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]) -> List[int]:
         return self.engine.slots_step(tokens, pos, active)
@@ -446,6 +454,7 @@ class InferenceSession:
                 eng.seed_sampler(smp.seed)
                 self._dev_seeded = gen
             self._sync_controls(smp)
+            self._sync_filters(smp)
             eng.step_sampled(token, self.pos, smp.temperature, smp.topp)
             if logprobs is not None:
                 eng.logprobs([logprobs], controlled=True)
@@ -476,12 +485,20 @@ class InferenceSession:
             self.engine.set_sampling_controls(smp.presence_penalty, smp.frequency_penalty, smp.logit_bias, 1)
             self._dev_controls = key
 
+    def _sync_filters(self, smp):
+        """Hands the sampler's top_k / min_p to the device when they differ from what it holds."""
+        key = (smp.top_k, smp.min_p)
+        if self._dev_filters != key:
+            self.engine.set_sampling_filters(*key)
+            self._dev_filters = key
+
     # ---- several completions of one prompt ----
     def forget_device_seed(self):
         self._dev_seeded = None
 
     def choice_controls(self, sampler, n: int):
-        """The sampler's controls for the batched choices, count rows 1..n zeroed."""
+        """The sampler's controls and filters for the batched choices, count rows 1..n zeroed."""
+        self._sync_filters(sampler)
         if sampler.controls_active or self._dev_controls is not None:
             self.engine.set_sampling_controls(sampler.presence_penalty, sampler.frequency_penalty, sampler.logit_bias,
                                               ((1 << n) - 1) << 1)

@@ -156,6 +156,23 @@ def parse_controls(body: dict, vocab: int, presence: float, frequency: float):
     return presence, frequency, sorted(pairs)
 
 
+MAX_TOP_K = 2**31 - 1
+
+
+def parse_filters(body: dict, top_k: int, min_p: float):
+    """The request's sampling filters: (top_k, min_p). Absent fields take the server's defaults. top_k is an integer from 0 to
+    2^31 - 1 (0: off; k >= the vocabulary keeps every token), min_p a number from 0 to 1 (0: off). Booleans, non-integer top_k
+    and values out of range are refused."""
+    if "top_k" in body:
+        k = body["top_k"]
+        if isinstance(k, bool) or not isinstance(k, int) or not 0 <= k <= MAX_TOP_K:
+            raise ValueError(f"'top_k' must be an integer from 0 to {MAX_TOP_K}")
+        top_k = k
+    if "min_p" in body:
+        min_p = _number(body["min_p"], 0.0, 1.0, "min_p")
+    return int(top_k), float(min_p)
+
+
 def parse_logprobs(body: dict, n_ranks: int = 1) -> Optional[int]:
     """The request's log-probabilities: None without them, else the number of top entries. `logprobs` is a boolean (absent:
     false); `top_logprobs`, an integer from 0 to 20 (absent: 0), is allowed only with `logprobs: true`. Anything else is refused,
@@ -183,9 +200,9 @@ def _number_field(body: dict, key: str, default):
 
 def parse_chat(body, defaults, vocab: int, max_n: int, n_ranks: int) -> SimpleNamespace:
     """A chat completion request: messages as (role, content) pairs, n, stream, max_tokens, temperature, topp, seed (None
-    without one), presence, frequency, bias (parse_controls) and logprobs (parse_logprobs). `defaults` holds the server's
-    --temperature, --topp and penalties; n may not exceed max_n (the slot count under --parallel); n_ranks > 1 (tensor
-    parallelism) refuses logprobs. A body that is not an object, `messages` that are not a list of {role, content} objects
+    without one), presence, frequency, bias (parse_controls), top_k, min_p (parse_filters) and logprobs (parse_logprobs).
+    `defaults` holds the server's --temperature, --topp, penalties and filters; n may not exceed max_n (the slot count under
+    --parallel); n_ranks > 1 (tensor parallelism) refuses logprobs. A body that is not an object, `messages` that are not a list of {role, content} objects
     with string values, a number field that is not a number, a negative temperature or a malformed control raise ValueError;
     a body without `messages` raises KeyError."""
     if not isinstance(body, dict):
@@ -196,6 +213,7 @@ def parse_chat(body, defaults, vocab: int, max_n: int, n_ranks: int) -> SimpleNa
     # server defaults: --presence-penalty / --frequency-penalty (argument objects that predate them mean 0)
     presence, frequency, bias = parse_controls(body, vocab, getattr(defaults, "presence_penalty", 0.0),
                                                getattr(defaults, "frequency_penalty", 0.0))
+    top_k, min_p = parse_filters(body, getattr(defaults, "top_k", 0), getattr(defaults, "min_p", 0.0))
     logprobs = parse_logprobs(body, n_ranks)
     messages = body["messages"]
     if not isinstance(messages, list) or not all(isinstance(m, dict) and isinstance(m.get("role"), str) and
@@ -208,7 +226,7 @@ def parse_chat(body, defaults, vocab: int, max_n: int, n_ranks: int) -> SimpleNa
                            max_tokens=int(_number_field(body, "max_tokens", -1)), temperature=temperature,
                            topp=float(_number_field(body, "top_p", defaults.topp)),
                            seed=int(_number_field(body, "seed", 0)) if "seed" in body else None,
-                           presence=presence, frequency=frequency, bias=bias, logprobs=logprobs)
+                           presence=presence, frequency=frequency, bias=bias, logprobs=logprobs, top_k=top_k, min_p=min_p)
 
 
 def logprob_entry(tokenizer, entry) -> dict:
@@ -378,6 +396,7 @@ class ApiServer:
         inf, smp, seq_len = ctx.inference, ctx.sampler, ctx.header.seq_len
         chat = parse_chat(req.json, ctx.args, smp.vocab_size, MAX_CHOICES, getattr(getattr(inf, "comm", None), "world_size", 1))
         smp.set_controls(chat.presence, chat.frequency, chat.bias)
+        smp.set_filters(chat.top_k, chat.min_p)
         smp.set_temperature(chat.temperature)
         smp.set_topp(chat.topp)
         if chat.seed is not None:
@@ -431,7 +450,7 @@ class ApiServer:
                 self.done()
 
         r = Chat()
-        vars(r).update(vars(chat))   # the SlotRequest fields: n, temperature, topp, seed, max_tokens, logprobs and the controls
+        vars(r).update(vars(chat))   # the SlotRequest fields: n, temperature, topp, seed, max_tokens, logprobs, the controls and filters
         r.done = lambda: None
         return r
 
@@ -529,7 +548,7 @@ def serve(ctx: AppContext, max_requests: int = 0) -> None:
 USAGE = """Usage: dllama-api {--model <path>} {--tokenizer <path>} [--host <addr>] [--port <p>]
         [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>] [--gpus <n>] [--workers <ip:port> ...]
         [--temperature <temp>] [--topp <t>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]
-        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--parallel <n>]
+        [--top-k <k>] [--min-p <p>] [--chat-template {llama2|llama3|deepSeek3|chatml}] [--parallel <n>]
         --parallel <n>: decode up to n (1..8) chat requests together, each in its own KV-cache slot of
                         floor(context / n) tokens; single GPU and dense models only
 """

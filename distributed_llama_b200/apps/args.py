@@ -30,6 +30,8 @@ class AppArgs:
     topp: float = 0.9
     presence_penalty: float = 0.0    # sampling controls (host Sampler.set_controls), each in [-2, 2]
     frequency_penalty: float = 0.0
+    top_k: int = 0                   # sampling filters (host Sampler.set_filters): 0 = off; top_k in [0, 2^31 - 1]
+    min_p: float = 0.0               # in [0, 1]
     seed: int = field(default_factory=lambda: int(time.time()))
     chat_template: Optional[str] = None
     max_seq_len: int = 0
@@ -46,6 +48,7 @@ class AppArgs:
 
 FLOAT_TYPES = ("f32", "f16", "q40", "q80")
 KV_CACHE_FLOAT_TYPES = ("bf16", "q80")
+MAX_TOP_K = 2**31 - 1
 TEMPLATES = ("llama2", "llama3", "deepSeek3", "chatml")
 
 
@@ -101,6 +104,16 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
             if not -2.0 <= v <= 2.0:
                 raise ValueError(f"{name} must be from -2 to 2")
             setattr(a, "presence_penalty" if name == "--presence-penalty" else "frequency_penalty", v)
+        elif name == "--top-k":
+            v = int(value)
+            if not 0 <= v <= MAX_TOP_K:
+                raise ValueError(f"--top-k must be an integer from 0 to {MAX_TOP_K}")
+            a.top_k = v
+        elif name == "--min-p":
+            v = float(value)
+            if not 0.0 <= v <= 1.0:
+                raise ValueError("--min-p must be from 0 to 1")
+            a.min_p = v
         elif name == "--seed":
             a.seed = int(value)
         elif name == "--chat-template":
@@ -136,6 +149,7 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
 USAGE = """Usage: dllama {inference|chat|perplexity|worker} {--model <path>} {--tokenizer <path>}
         [--prompt <text>] [--steps <n>] [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>]
         [--temperature <temp>] [--topp <t>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]
+        [--top-k <k>] [--min-p <p>]        sampling filters of sampled draws (default 0 = off)
         [--chat-template {llama2|llama3|deepSeek3|chatml}]
         [--kv-cache-float-type {bf16|q80}] KV-cache storage (default bf16; q80 = int8 blocks of 32 + f16 scale)
         [--gpus <n>]                      run tensor-parallel on n local GPUs (spawns one process per GPU)

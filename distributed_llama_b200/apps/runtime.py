@@ -23,6 +23,7 @@ from .args import AppArgs
 OP_STOP, OP_PREFILL, OP_STEP_LOGITS, OP_STEP_GREEDY, OP_DECODE_N, OP_STEP_SAMPLE, OP_SEED = 0, 1, 2, 3, 4, 5, 6
 OP_CHOICES_SEED, OP_CHOICES_FIRST, OP_CHOICES_STEP = 7, 8, 9
 OP_CONTROLS = 10   # [presence bits, frequency bits, count-row mask, (id, bias bits) ...]: Engine.set_sampling_controls
+OP_FILTERS = 11    # [top_k, min_p bits]: Engine.set_sampling_filters
 
 
 def _split_seed(seed: int) -> List[int]:
@@ -190,6 +191,15 @@ class RootInference:
         self._send(OP_CONTROLS, 0, words)
         self.eng.set_sampling_controls(sampler.presence_penalty, sampler.frequency_penalty, bias, row_mask)
 
+    def set_filters(self, sampler) -> None:
+        """The sampler's top_k / min_p on every rank, before the first draw that uses them (each rank draws from the gathered
+        logits with its own generator, so all ranks must hold the same filters)."""
+        key = (sampler.top_k, sampler.min_p)
+        if getattr(self, "_filters", (0, 0.0)) != key:
+            self._send(OP_FILTERS, 0, [key[0]] + _f32_bits(key[1]))
+            self.eng.set_sampling_filters(*key)
+            self._filters = key
+
     def next_token(self, token: int, pos: int, sampler, logprobs: Optional[int] = None) -> int:
         """One generated token with the sampler's settings: greedy and temperature/top-p both run on the device; the host sampler
         is only used with the library-collective (multi-node) mode or DL_HOST_SAMPLER=1. Greedy with sampling controls runs
@@ -207,6 +217,7 @@ class RootInference:
             if getattr(self, "_controls", None) != key:   # a new completion: count row 0 starts from zero
                 self.set_controls(sampler, 1)
                 self._controls = key
+            self.set_filters(sampler)
             return self.forward_sampled(token, pos, sampler.temperature, sampler.topp, logprobs)
         t = int(sampler.sample(self.forward_logits(token, pos).float().cpu().numpy()))
         if logprobs is not None:
@@ -235,6 +246,7 @@ class RootInference:
         return self.device_sampling and self.eng.supports_choices(n)
 
     def choice_controls(self, sampler, n: int) -> None:
+        self.set_filters(sampler)
         if sampler.controls_active or getattr(self, "_controls", None) is not None:
             self.set_controls(sampler, ((1 << n) - 1) << 1)
             self._controls = -1 if sampler.controls_active else None   # row 0's counts are not this sampler's
@@ -318,6 +330,8 @@ def worker_loop(sess: InferenceSession, comm, chan=None) -> None:
             pairs = toks[3:]
             bias = [(pairs[i], _bits_f32(pairs[i + 1])[0]) for i in range(0, len(pairs), 2)]
             eng.set_sampling_controls(presence, frequency, bias, toks[2])
+        elif op == OP_FILTERS:
+            eng.set_sampling_filters(toks[0], _bits_f32(toks[1])[0])
         elif op == OP_STEP_SAMPLE:
             import struct
             temperature, topp = struct.unpack("<ff", struct.pack("<ii", toks[1], toks[2]))
@@ -356,7 +370,8 @@ def run_inference_app(args: AppArgs, handler: Callable[[AppContext], None]) -> N
     sess = InferenceSession(args.model, args.tokenizer, max_seq_len=args.max_seq_len, temperature=args.temperature,
                             topp=args.topp, seed=args.seed, comm=comm, moe_mode=getattr(args, "moe_mode", "auto") or "auto",
                             presence_penalty=args.presence_penalty, frequency_penalty=args.frequency_penalty,
-                            parallel=getattr(args, "parallel", 1), kv_cache_float_type=args.kv_cache_float_type)
+                            parallel=getattr(args, "parallel", 1), kv_cache_float_type=args.kv_cache_float_type,
+                            top_k=getattr(args, "top_k", 0), min_p=getattr(args, "min_p", 0.0))
     chan = open_control_channel(comm)
     if rank != 0:
         worker_loop(sess, comm, chan)

@@ -137,6 +137,12 @@ def lib() -> C.CDLL:
     L.dl_sample_rows_controlled.restype = i32
     L.dl_engine_set_sampling_controls.argtypes = [vp, f32, f32, C.POINTER(C.c_int32), C.POINTER(f32), i32, u32, vp]
     L.dl_engine_set_sampling_controls.restype = i32
+    L.dl_engine_set_sampling_filters.argtypes = [vp, u32, f32]
+    L.dl_engine_set_sampling_filters.restype = i32
+    L.dl_sample_logits_filtered.argtypes = [vp, vp, u32, f32, f32, u32, f32, vp, vp, vp]
+    L.dl_sample_logits_filtered.restype = i32
+    L.dl_sample_rows_filtered.argtypes = [vp, u32, vp, u32, vp, vp, vp, vp, u32, u32, vp, u32, vp, u32, vp]
+    L.dl_sample_rows_filtered.restype = i32
     L.dl_choice_attn.argtypes = [vp, u32, vp, vp, vp, vp, f32, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
     L.dl_choice_attn.restype = i32
     L.dl_choice_attn_only.argtypes = [vp, u32, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
@@ -164,6 +170,8 @@ def lib() -> C.CDLL:
     L.dl_engine_slot_copy.restype = i32
     L.dl_engine_slot_sampling.argtypes = [vp, u32, C.c_uint64, f32, f32, f32, f32, ip, C.POINTER(f32), i32, vp]
     L.dl_engine_slot_sampling.restype = i32
+    L.dl_engine_slot_filters.argtypes = [vp, u32, u32, f32]
+    L.dl_engine_slot_filters.restype = i32
     L.dl_engine_slots_forward.argtypes = [vp, ip, ip, u32, vp]
     L.dl_engine_slots_forward.restype = i32
     L.dl_engine_slots_step.argtypes = [vp, ip, ip, u32, ip, vp]

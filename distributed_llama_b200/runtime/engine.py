@@ -217,6 +217,11 @@ class Engine:
         if presence or frequency or n:
             self._sampler_ready = True
 
+    def set_sampling_filters(self, top_k: int, min_p: float) -> None:
+        """top_k / min_p of the following sampled device draws of the single sequence and the choices (host Sampler.set_filters
+        defines them); 0 / 0.0: off. They persist until changed; temperature-0 draws ignore them. Every rank makes the same call."""
+        cl.check(self._lib.dl_engine_set_sampling_filters(self._h, int(top_k), float(min_p)), "engine_set_sampling_filters")
+
     # -- choices: several completions of one prompt, one row per choice (csrc/cuda/attn_decode.cu) --
     def supports_choices(self, n: int) -> bool:
         """True if n choices can run as one batched step: dense layers, kernel-fused collectives, n <= max_batch."""
@@ -310,15 +315,17 @@ class Engine:
         cl.check(self._lib.dl_engine_slot_copy(self._h, int(src), int(dst), int(P), cl.stream_ptr()), "engine_slot_copy")
 
     def slot_sampling(self, slot: int, seed: int, temperature: float, topp: float, presence: float = 0.0, frequency: float = 0.0,
-                      bias: Sequence = ()) -> None:
-        """Seeds slot `slot`'s generator, zeroes its token counts and sets its temperature (0: arg-max), top-p, penalties and
-        logit bias ((id, value) pairs)."""
+                      bias: Sequence = (), *, top_k: int = 0, min_p: float = 0.0) -> None:
+        """Seeds slot `slot`'s generator, zeroes its token counts and sets its temperature (0: arg-max), top-p, penalties,
+        logit bias ((id, value) pairs) and sampling filters (top_k / min_p, 0: off)."""
         n = len(bias)
         ids = (C.c_int32 * max(n, 1))(*[int(t) for t, _ in bias])
         vals = (C.c_float * max(n, 1))(*[float(v) for _, v in bias])
         cl.check(self._lib.dl_engine_slot_sampling(self._h, int(slot), int(seed) & 0xFFFFFFFFFFFFFFFF, float(temperature), float(topp),
                                                     float(presence), float(frequency), ids, vals, n, cl.stream_ptr()),
                  "engine_slot_sampling")
+        if top_k or min_p:
+            cl.check(self._lib.dl_engine_slot_filters(self._h, int(slot), int(top_k), float(min_p)), "engine_slot_filters")
 
     def _slot_args(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]):
         n = self.slots
