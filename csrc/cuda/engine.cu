@@ -116,6 +116,7 @@ struct MoeDecodeArgs {
     float *out;                           // [dim] the weighted expert sum is added here
     const float *norm, *gate;             // ffn rms-norm weight [dim], router gate [nExperts][dim] f32
     const void *w13Qs, *w13Sc, *w2Qs, *w2Sc;   // [nLocal][2*ff][dim] gate/up interleaved, [nLocal][dim][ff]
+    int wType;                            // 0 = q40 device layout; 1 = f32, 2 = f16 dense rows (the *Sc pointers are unused)
     uint32_t dim, ff, nExperts, k, firstLocal, nLocal;
     float eps;
     float *routerLogits;                  // [nExperts]
@@ -130,7 +131,8 @@ struct MoeDecodeArgs {
     ArArgs ar;                            // nRanks > 1: all-reduce in the W2 epilogue
 };
 
-// router -> k x (W1|W3 -> silu*up) -> k x W2; the weighted expert sum is *added* to `out`.
+// router -> k x (W1|W3 -> silu*up) -> k x W2; the weighted expert sum is *added* to `out`. q40 experts run on the TMA GEMV,
+// f32 / f16 experts on the expert-routed mode of the dense GEMV (gemv_dense.cu).
 static int moeDecodeFfn(const MoeDecodeArgs &m, cudaStream_t stream, bool pdl) {
     RouterArgs ro{};
     ro.x = m.x; ro.normW = m.norm; ro.gate = m.gate; ro.eps = m.eps; ro.dim = m.dim; ro.nExperts = m.nExperts;
@@ -143,7 +145,8 @@ static int moeDecodeFfn(const MoeDecodeArgs &m, cudaStream_t stream, bool pdl) {
     a.moeCtasPerSlot = perSlot; a.kActive = m.k; a.expertIdx = m.expertIdx; a.outSlotStride = m.ff;
     a.expertQsStride = (uint64_t)2 * m.ff * (m.dim / 8); a.expertScaleStride = (uint64_t)2 * m.ff * (m.dim / 32);
     a.moeFirstExpert = m.firstLocal; a.moeNumLocal = m.nLocal;
-    { const int r = gemvQ40Tma(PRO_RMSNORM_, EPI_SWIGLU_, 1, a, (int)m.numSms, stream, pdl); if (r != 0) return r == 1 ? -31 : r; }
+    if (m.wType != 0) DL_TRY(gemvDense(m.wType, PRO_RMSNORM_, EPI_SWIGLU_, 1, a, (int)m.numSms, stream, pdl));
+    else { const int r = gemvQ40Tma(PRO_RMSNORM_, EPI_SWIGLU_, 1, a, (int)m.numSms, stream, pdl); if (r != 0) return r == 1 ? -31 : r; }
     a = GemvArgs{};
     a.qs = (const uint32_t *)m.w2Qs; a.scales = (const __half *)m.w2Sc; a.d = m.dim; a.n = m.ff;
     a.in = m.h; a.inStride = m.ff; a.inSlotStride = m.ff; a.out = m.out; a.outStride = m.dim; a.trace = m.trace2;
@@ -151,7 +154,8 @@ static int moeDecodeFfn(const MoeDecodeArgs &m, cudaStream_t stream, bool pdl) {
     a.expertQsStride = (uint64_t)m.dim * (m.ff / 8); a.expertScaleStride = (uint64_t)m.dim * (m.ff / 32);
     a.moeFirstExpert = m.firstLocal; a.moeNumLocal = m.nLocal; a.moeScratch = m.moeScratch; a.moeCounters = m.moeCounters;
     a.ar = m.ar;
-    { const int r = gemvQ40Tma(PRO_PLAIN_, EPI_MOE_DOWN_, 1, a, (int)m.numSms, stream, pdl); if (r != 0) return r == 1 ? -32 : r; }
+    if (m.wType != 0) DL_TRY(gemvDense(m.wType, PRO_PLAIN_, EPI_MOE_DOWN_, 1, a, (int)m.numSms, stream, pdl));
+    else { const int r = gemvQ40Tma(PRO_PLAIN_, EPI_MOE_DOWN_, 1, a, (int)m.numSms, stream, pdl); if (r != 0) return r == 1 ? -32 : r; }
     return 0;
 }
 
@@ -160,10 +164,9 @@ static int moeDecodeFfn(const MoeDecodeArgs &m, cudaStream_t stream, bool pdl) {
 static int runMoe(Engine &e, const LayerPtrs &L, float *out, bool fusedAr, uint64_t *trace13, uint64_t *trace2, cudaStream_t stream,
                   bool pdl) {
     const EngineConfig &c = e.cfg;
-    if (c.wType != 0) return -34;   // expert-indexed kernels exist for q40 matrices only
     MoeDecodeArgs m{};
     m.x = e.g.x; m.out = out; m.norm = L.norm1; m.gate = L.moeGate;
-    m.w13Qs = L.w13Qs; m.w13Sc = L.w13Sc; m.w2Qs = L.w2Qs; m.w2Sc = L.w2Sc;
+    m.w13Qs = L.w13Qs; m.w13Sc = L.w13Sc; m.w2Qs = L.w2Qs; m.w2Sc = L.w2Sc; m.wType = (int)c.wType;
     m.dim = c.dim; m.ff = c.ffDim; m.nExperts = c.nExperts; m.k = c.nActiveExperts; m.firstLocal = c.moeFirstExpert; m.nLocal = c.moeNumLocal;
     m.eps = c.eps; m.routerLogits = e.g.routerLogits; m.routerCounter = e.g.routerCounter; m.expertIdx = e.g.expertIdx;
     m.expertWeight = e.g.expertWeight; m.h = e.g.h; m.moeScratch = e.g.moeScratch; m.moeCounters = e.g.moeCounters; m.numSms = c.numSms;
@@ -879,6 +882,23 @@ DL_EXPORT int dl_moe_decode_ffn(const float *x, float *out, const float *norm, c
                                 uint32_t numSms, uint32_t hiddenAct, cudaStream_t stream) {
     dl::MoeDecodeArgs m{};
     m.x = x; m.out = out; m.norm = norm; m.gate = gate; m.w13Qs = w13Qs; m.w13Sc = w13Sc; m.w2Qs = w2Qs; m.w2Sc = w2Sc;
+    m.dim = dim; m.ff = ff; m.nExperts = nExperts; m.k = k; m.firstLocal = firstLocal; m.nLocal = nLocal; m.eps = eps;
+    m.routerLogits = routerLogits; m.routerCounter = routerCounter; m.expertIdx = expertIdx; m.expertWeight = expertWeight;
+    m.h = hOut; m.moeScratch = moeScratch; m.moeCounters = moeCounters; m.numSms = numSms;
+    const dl::HiddenActScope act(hiddenAct);
+    return dl::moeDecodeFfn(m, stream, false);
+}
+
+// dl_moe_decode_ffn for dense experts (tests/test_gpu_moe_dense.py): wtype 1 = f32, 2 = f16; w13 is [nLocal][2 * ff][dim] with
+// gate and up rows interleaved, w2 is [nLocal][dim][ff].
+DL_EXPORT int dl_moe_decode_ffn_dense(int wtype, const float *x, float *out, const float *norm, const float *gate, const void *w13,
+                                      const void *w2, uint32_t dim, uint32_t ff, uint32_t nExperts, uint32_t k, uint32_t firstLocal,
+                                      uint32_t nLocal, float eps, float *routerLogits, unsigned int *routerCounter, int *expertIdx,
+                                      float *expertWeight, float *hOut, float *moeScratch, unsigned int *moeCounters, uint32_t numSms,
+                                      uint32_t hiddenAct, cudaStream_t stream) {
+    if (wtype != 1 && wtype != 2) return -4;
+    dl::MoeDecodeArgs m{};
+    m.x = x; m.out = out; m.norm = norm; m.gate = gate; m.w13Qs = w13; m.w2Qs = w2; m.wType = wtype;
     m.dim = dim; m.ff = ff; m.nExperts = nExperts; m.k = k; m.firstLocal = firstLocal; m.nLocal = nLocal; m.eps = eps;
     m.routerLogits = routerLogits; m.routerCounter = routerCounter; m.expertIdx = expertIdx; m.expertWeight = expertWeight;
     m.h = hOut; m.moeScratch = moeScratch; m.moeCounters = moeCounters; m.numSms = numSms;

@@ -157,10 +157,144 @@ __global__ void __launch_bounds__(kDenseThreads, 1) gemvDenseKernel(GemvArgs a) 
     }
 }
 
-template <typename WT, int PRO, int EPI, int NB>
-int launchDense(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
-    auto kernel = gemvDenseKernel<WT, PRO, EPI, NB>;
-    static size_t configured = 0;   // per instantiation
+// Expert-routed mode (mixture of experts, one token): the dense counterpart of the q40 TMA kernel's moeCtasPerSlot launches.
+// The grid is kActive x moeCtasPerSlot; CTA b serves routing slot b / moeCtasPerSlot on the pair-aligned row tile
+// b % moeCtasPerSlot of expert expertIdx[slot], so every slot uses the same tiling and the tiles line up for the combine.
+//   PRO_RMSNORM_ + EPI_SWIGLU_ (W1|W3): rmsnorm(x) -> silu(gate) * up of slot s into out + s * outSlotStride.
+//   PRO_PLAIN_ + EPI_MOE_DOWN_ (W2):    reads in + s * inSlotStride, leaves expertWeight[s] * product in moeScratch[s]; the
+//                                       last CTA of a row tile (self-resetting moeCounters) adds sum_s moeScratch[s], summed in
+//                                       slot order, to `out`: the result does not depend on which CTA finishes last.
+// Under expert parallelism experts outside [moeFirstExpert, +moeNumLocal) stream nothing: their CTAs write zero products and
+// still arrive at the combine counter. RPW rows per warp are streamed together with kMoeLoads / RPW 16-byte loads each, so
+// short expert rows (a Qwen3-30B-A3B W2 row is 768 f16 values, 96 loads of a warp) still keep a lane's load slots full.
+constexpr int kMoeLoads = 16;
+
+template <typename WT, int PRO, int EPI, int RPW>
+__global__ void __launch_bounds__(kDenseThreads, 1) gemvDenseMoeKernel(GemvArgs a) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    constexpr int E = Chunk<WT>::kElems;
+    constexpr int U = kMoeLoads / RPW;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+
+    const uint32_t tileIdx = blockIdx.x % a.moeCtasPerSlot, slot = blockIdx.x / a.moeCtasPerSlot;
+    const uint32_t nPairs = a.d / 2;
+    const uint32_t pairBegin = (uint32_t)(((uint64_t)tileIdx * nPairs) / a.moeCtasPerSlot);
+    const uint32_t pairEnd = (uint32_t)(((uint64_t)(tileIdx + 1) * nPairs) / a.moeCtasPerSlot);
+    const uint32_t rowBase = pairBegin * 2;
+    const uint32_t tileRows = (pairEnd - pairBegin) * 2;
+
+    float *xs = reinterpret_cast<float *>(smem);                 // [n] (normalised) activations of this slot
+    float *rowOut = xs + a.n;                                    // [maxTileRows]
+    float *red = rowOut + a.maxTileRows;                         // [16]
+
+    pdlLaunchDependents();
+    pdlWait();   // the expert choice comes from the router, W2's input from the W1|W3 launch
+    const uint32_t e = (uint32_t)a.expertIdx[slot] - a.moeFirstExpert;
+    const bool active = e < a.moeNumLocal;
+
+    if (active) {
+        // ---- prologue: (rmsnorm) activations -> shared memory ----
+        const uint32_t nVec = a.n / 4;
+        const float4 *x4 = reinterpret_cast<const float4 *>(a.in + (size_t)slot * a.inSlotStride);
+        float inv = 1.f;
+        if (PRO == PRO_RMSNORM_) {
+            float ss = 0.f;
+            for (uint32_t i = tid; i < nVec; i += kDenseThreads) {
+                const float4 v = x4[i];
+                ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+            }
+            ss = blockSumDense(ss, red);
+            inv = rsqrtf(ss / (float)a.n + a.eps);
+        }
+        float4 *dst = reinterpret_cast<float4 *>(xs);
+        for (uint32_t i = tid; i < nVec; i += kDenseThreads) {
+            float4 v = x4[i];
+            if (PRO == PRO_RMSNORM_) {
+                const float4 w = reinterpret_cast<const float4 *>(a.normW)[i];
+                v.x = w.x * (v.x * inv); v.y = w.y * (v.y * inv); v.z = w.z * (v.z * inv); v.w = w.w * (v.w * inv);
+            }
+            dst[i] = v;
+        }
+        __syncthreads();
+
+        // ---- main loop: RPW adjacent rows per warp, U x 16 B in flight per lane and row ----
+        const uint32_t nChunks = a.n / E;
+        const WT *wBase = reinterpret_cast<const WT *>(a.qs) + (size_t)e * a.d * a.n;
+        for (uint32_t r0 = warp * RPW; r0 < tileRows; r0 += kDenseWarps * RPW) {
+            float acc[RPW];
+#pragma unroll
+            for (int j = 0; j < RPW; j++) acc[j] = 0.f;
+            for (uint32_t c0 = lane; c0 < nChunks; c0 += 32 * U) {
+                uint4 q[RPW][U];
+#pragma unroll
+                for (int j = 0; j < RPW; j++) {
+                    const uint4 *row = reinterpret_cast<const uint4 *>(wBase + (size_t)(rowBase + r0 + j) * a.n);
+#pragma unroll
+                    for (int u = 0; u < U; u++) {
+                        const uint32_t c = c0 + u * 32;
+                        q[j][u] = (r0 + j < tileRows && c < nChunks) ? ldgStream16(row + c) : make_uint4(0, 0, 0, 0);
+                    }
+                }
+#pragma unroll
+                for (int j = 0; j < RPW; j++) {
+#pragma unroll
+                    for (int u = 0; u < U; u++) {
+                        const uint32_t c = c0 + u * 32;
+                        if (c < nChunks) {
+                            float w[E];
+                            Chunk<WT>::unpack(q[j][u], w);
+                            const float4 *xv = reinterpret_cast<const float4 *>(xs + (size_t)c * E);
+#pragma unroll
+                            for (int k = 0; k < E / 4; k++) {
+                                const float4 x = xv[k];
+                                acc[j] = fmaf(w[4 * k], x.x, acc[j]);
+                                acc[j] = fmaf(w[4 * k + 1], x.y, acc[j]);
+                                acc[j] = fmaf(w[4 * k + 2], x.z, acc[j]);
+                                acc[j] = fmaf(w[4 * k + 3], x.w, acc[j]);
+                            }
+                        }
+                    }
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < RPW; j++) {
+                const float v = warpSum(acc[j]);
+                if (lane == 0 && r0 + j < tileRows) rowOut[r0 + j] = v;
+            }
+        }
+    }
+    __syncthreads();
+
+    // ---- epilogue ----
+    if (EPI == EPI_SWIGLU_) {
+        float *outBase = a.out + (size_t)slot * a.outSlotStride;
+        for (uint32_t p = tid; p < tileRows / 2; p += kDenseThreads)
+            outBase[pairBegin + p] = active ? gateAct(rowOut[2 * p], a.act) * rowOut[2 * p + 1] : 0.f;
+    } else {
+        __shared__ bool sLastSlot;
+        const float wgt = active ? a.expertWeight[slot] : 0.f;
+        for (uint32_t i = tid; i < tileRows; i += kDenseThreads)
+            a.moeScratch[(size_t)slot * a.d + rowBase + i] = active ? rowOut[i] * wgt : 0.f;
+        __threadfence();
+        __syncthreads();
+        if (tid == 0) {
+            const unsigned int prev = atomicAdd(&a.moeCounters[tileIdx], 1u);
+            sLastSlot = prev == a.kActive - 1;
+            if (sLastSlot) a.moeCounters[tileIdx] = 0;
+        }
+        __syncthreads();
+        if (!sLastSlot) return;
+        __threadfence();
+        for (uint32_t i = tid; i < tileRows; i += kDenseThreads) {
+            float v = 0.f;
+            for (uint32_t j = 0; j < a.kActive; j++) v += __ldcg(a.moeScratch + (size_t)j * a.d + rowBase + i);
+            a.out[rowBase + i] += v;
+        }
+    }
+}
+
+template <typename Kernel>
+int launchDenseKernel(Kernel kernel, size_t &configured, const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
     if (smemBytes > configured) {
         DL_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
         configured = smemBytes;
@@ -177,6 +311,34 @@ int launchDense(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stre
     cfg.numAttrs = 1;
     DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, a));
     return 0;
+}
+
+template <typename WT, int PRO, int EPI, int RPW>
+int launchDenseMoe(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
+    static size_t configured = 0;   // per instantiation
+    return launchDenseKernel(gemvDenseMoeKernel<WT, PRO, EPI, RPW>, configured, a, grid, smemBytes, stream, pdl);
+}
+
+template <typename WT>
+int dispatchDenseMoe(int pro, int epi, int rpw, const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
+#define DL_MOE_CASE(P, E, R) \
+    if (pro == P && epi == E && rpw == R) return launchDenseMoe<WT, P, E, R>(a, grid, smemBytes, stream, pdl);
+#define DL_MOE_RPW(P, E) DL_MOE_CASE(P, E, 1) DL_MOE_CASE(P, E, 2)
+    DL_MOE_RPW(PRO_RMSNORM_, EPI_SWIGLU_)
+    DL_MOE_RPW(PRO_PLAIN_, EPI_MOE_DOWN_)
+    if constexpr (sizeof(WT) == 2) {   // four f32 rows of 4 loads each would spill: f32 stops at two rows per warp
+        DL_MOE_CASE(PRO_RMSNORM_, EPI_SWIGLU_, 4)
+        DL_MOE_CASE(PRO_PLAIN_, EPI_MOE_DOWN_, 4)
+    }
+#undef DL_MOE_RPW
+#undef DL_MOE_CASE
+    return -3;
+}
+
+template <typename WT, int PRO, int EPI, int NB>
+int launchDense(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
+    static size_t configured = 0;   // per instantiation
+    return launchDenseKernel(gemvDenseKernel<WT, PRO, EPI, NB>, configured, a, grid, smemBytes, stream, pdl);
 }
 
 template <typename WT>
@@ -199,11 +361,28 @@ size_t gemvDenseSmemBytes(uint32_t n, uint32_t maxTileRows, int nb) {
     return (size_t)nb * n * 4 + (size_t)maxTileRows * nb * 4 + 16 * 4 + 16;
 }
 
-// wtype: 1 = f32, 2 = f16. `a.qs` points at the row-major [d][n] matrix, `a.scales` is unused.
+// wtype: 1 = f32, 2 = f16. `a.qs` points at the row-major [d][n] matrix, `a.scales` is unused. Expert-routed launches
+// (moeCtasPerSlot > 0, nb == 1) read `a.qs` as [moeNumLocal][d][n].
 int gemvDense(int wtype, int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t stream, bool pdl) {
     if (a.d % 2 || a.n % 8) return -1;
     a.act = gHiddenAct;
-    if (a.expertIdx || a.moeCtasPerSlot || a.ar.nRanks > 1) return -40;   // MoE routing / in-kernel all-reduce: q40 kernels only
+    if (a.ar.nRanks > 1) return -40;   // in-kernel all-reduce: q40 kernels only
+    if (a.moeCtasPerSlot) {
+        if (nb != 1 || !a.expertIdx || a.kActive == 0) return -41;
+        const uint32_t nPairs = a.d / 2;
+        const uint32_t tiles = a.moeCtasPerSlot < nPairs ? a.moeCtasPerSlot : nPairs;
+        a.moeCtasPerSlot = tiles;
+        a.maxTileRows = 2 * ((nPairs + tiles - 1) / tiles);
+        const size_t smemBytes = gemvDenseSmemBytes(a.n, a.maxTileRows, 1);
+        if (smemBytes > 227 * 1024) return -2;
+        const uint32_t nChunks = a.n / (wtype == 1 ? 4 : 8);
+        const int rpw = (wtype == 2 && nChunks <= 32 * (kMoeLoads / 4)) ? 4 : nChunks <= 32 * (kMoeLoads / 2) ? 2 : 1;
+        const int grid = (int)(tiles * a.kActive);
+        if (wtype == 1) return dispatchDenseMoe<float>(pro, epi, rpw, a, grid, smemBytes, stream, pdl);
+        if (wtype == 2) return dispatchDenseMoe<__half>(pro, epi, rpw, a, grid, smemBytes, stream, pdl);
+        return -4;
+    }
+    if (a.expertIdx) return -41;
     const uint32_t nPairs = a.d / 2;
     const int grid = (int)(nPairs < (uint32_t)numSms ? nPairs : (uint32_t)numSms);
     a.maxTileRows = 2 * ((nPairs + grid - 1) / grid);

@@ -275,8 +275,10 @@ void buildRopeTable(const ModelHeader &h, uint32_t seqLen, float *out) {
 uint64_t requiredDeviceBytes(const ModelHeader &h, uint32_t nRanks, uint32_t kvBytesPerElem) {
     uint64_t total = 0;
     for (const TensorEntry &t : buildTensorDirectory(h, false)) {
-        if (t.part == PART_ROOT || t.part == PART_REPLICATE) total += t.nBytes;
-        else total += t.nBytes / nRanks;
+        // device size: q40 keeps its blocks, f16 / f32 stay as they are, q80 matrices are dequantised to f32 (models/loader.py)
+        const uint64_t bytes = t.type == F_Q80 ? t.d * t.n * 4 : t.nBytes;
+        if (t.part == PART_ROOT || t.part == PART_REPLICATE) total += bytes;
+        else total += bytes / nRanks;
     }
     const uint64_t kvHeads = h.nKvHeads >= nRanks ? h.nKvHeads / nRanks : 1;
     total += (uint64_t)2 * h.nLayers * h.seqLen * kvHeads * h.headDim * kvBytesPerElem;

@@ -105,17 +105,20 @@ class _Uploader:
         return torch.from_numpy(np.ascontiguousarray(x)).to(self.device)
 
 
-def _load_dense(mf: ModelFile, up: "_Uploader", rank, n_ranks, kv_rank, kv_ranks, nh, nkv, ff0, v0, neox, device) -> "DeviceWeights":
+def _load_dense(mf: ModelFile, up: "_Uploader", rank, n_ranks, kv_rank, kv_ranks, nh, nkv, ff0, v0, neox, device,
+                first_exp=0, n_local=1, ep=False) -> "DeviceWeights":
     """f32 / f16 / q80 weight files: matrices stay dense on the device (f16 files as f16, everything else as f32 — q80 blocks
     are dequantised exactly) and run through csrc/cuda/gemv_dense.cu with f32 activations. This is the reference's
-    F32_F32_F32 matmul path (`--buffer-float-type f32`, src/nn/nn-cpu-ops.cpp:1138-1160); same partition rules."""
+    F32_F32_F32 matmul path (`--buffer-float-type f32`, src/nn/nn-cpu-ops.cpp:1138-1160); same partition rules.
+    Mixture-of-experts files keep experts [first_exp, +n_local) as w13 [n_local][2 * ff0][dim] (gate / up rows interleaved)
+    and w2 [n_local][dim][ff0]: every expert's ff slice under "tp", whole experts under "ep" (`ep`)."""
     h = mf.header
     H = host()
     hd, dim = h.head_dim, h.dim
     dt = torch.float16 if h.weight_type == quants.F_16 else torch.float32
 
-    def sliced(name, layer, r, n):
-        x = mf.slice_f32(mf.entry(name, layer, 0), r, n)
+    def sliced(name, layer, r, n, expert=0):
+        x = mf.slice_f32(mf.entry(name, layer, expert), r, n)
         up.bytes += x.nbytes
         return torch.from_numpy(np.ascontiguousarray(x))
 
@@ -132,21 +135,35 @@ def _load_dense(mf: ModelFile, up: "_Uploader", rank, n_ranks, kv_rank, kv_ranks
                       embedding=up.f32(mf.entry("embedding")), final_norm=up.f32(mf.entry("final_norm")),
                       wcls=dev(sliced("final_matmul_logits", 0, rank, n_ranks), v0, dim),
                       rope=torch.from_numpy(np.asarray(H.build_rope_table(h, h.seq_len))).to(device))
+    if h.n_experts > 0:
+        W.first_expert, W.n_local_experts, W.moe_mode = first_exp, n_local, ("ep" if ep else "tp")
+    er, en = (0, 1) if ep else (rank, n_ranks)    # expert tensors: whole matrices under EP
     perm_dev = torch.from_numpy(_interleave_perm(hd)).to(device) if neox else None
     for l in range(h.n_layers):
         q = heads_interleaved(sliced("block_matmul_q", l, rank, n_ranks), nh)
         k = heads_interleaved(sliced("block_matmul_k", l, kv_rank, kv_ranks), nkv)
         v = sliced("block_matmul_v", l, kv_rank, kv_ranks)
-        w1, w3 = sliced("block_matmul_w1", l, rank, n_ranks), sliced("block_matmul_w3", l, rank, n_ranks)
+        if h.n_experts > 0:
+            w13 = DeviceDense(torch.empty(n_local * 2 * ff0, dim, dtype=dt, device=device), 2 * ff0, dim)
+            w2 = DeviceDense(torch.empty(n_local * dim, ff0, dtype=dt, device=device), dim, ff0)
+            for le in range(n_local):
+                e = first_exp + le
+                w1, w3 = sliced("block_matmul_w1", l, er, en, e), sliced("block_matmul_w3", l, er, en, e)
+                w13.data[le * 2 * ff0:(le + 1) * 2 * ff0].copy_(torch.stack([w1, w3], 1).reshape(2 * ff0, dim).to(dt))
+                w2.data[le * dim:(le + 1) * dim].copy_(sliced("block_matmul_w2", l, er, en, e).to(dt))
+        else:
+            w1, w3 = sliced("block_matmul_w1", l, rank, n_ranks), sliced("block_matmul_w3", l, rank, n_ranks)
+            w13 = dev(torch.stack([w1, w3], 1).reshape(2 * ff0, dim), 2 * ff0, dim)
+            w2 = dev(sliced("block_matmul_w2", l, rank, n_ranks), dim, ff0)
         L = LayerWeights(qkv=dev(torch.cat([q, k, v], 0), (nh + 2 * nkv) * hd, dim),
-                         wo=dev(sliced("block_matmul_wo", l, rank, n_ranks), dim, nh * hd),
-                         w13=dev(torch.stack([w1, w3], 1).reshape(2 * ff0, dim), 2 * ff0, dim),
-                         w2=dev(sliced("block_matmul_w2", l, rank, n_ranks), dim, ff0),
+                         wo=dev(sliced("block_matmul_wo", l, rank, n_ranks), dim, nh * hd), w13=w13, w2=w2,
                          norm0=up.f32(mf.entry("block_norm_0", l)), norm1=up.f32(mf.entry("block_norm_1", l)))
         if h.qk_norm:
             qn, kn = up.f32(mf.entry("block_norm_q", l)), up.f32(mf.entry("block_norm_k", l))
             L.q_norm = qn[perm_dev].contiguous() if neox else qn
             L.k_norm = kn[perm_dev].contiguous() if neox else kn
+        if h.n_experts > 0:
+            L.moe_gate = up.f32(mf.entry("block_moe_gate", l))
         W.layers.append(L)
     if torch.device(device).type == "cuda":
         torch.cuda.synchronize(device)
@@ -194,8 +211,6 @@ def load_device_weights(mf: ModelFile, rank: int = 0, n_ranks: int = 1, device="
     combine is the same in-kernel all-reduce); "auto" picks ep when the TP slice would be narrower than 128 columns."""
     h = mf.header
     dense = h.weight_type != quants.F_Q40
-    if dense and h.n_experts > 0:
-        raise NotImplementedError("mixture-of-experts models need q40 weights (the expert-routed kernels are q40 only)")
     H = host()
     if moe_mode == "auto":
         moe_mode = "ep" if (h.n_experts > 0 and n_ranks > 1 and (h.ff_dim // n_ranks) % 128 != 0 and h.n_experts % n_ranks == 0) else "tp"
@@ -221,8 +236,10 @@ def load_device_weights(mf: ModelFile, rank: int = 0, n_ranks: int = 1, device="
     neox = h.rope_type == ROPE_FALCON
     up = _Uploader(mf, device)
     dim = h.dim
+    n_exp = max(h.n_experts, 1)
+    first_exp, n_local = (rank * (h.n_experts // n_ranks), h.n_experts // n_ranks) if ep else (0, n_exp)
     if dense:
-        return _load_dense(mf, up, rank, n_ranks, kv_rank, kv_ranks, nh, nkv, ff0, v0, neox, device)
+        return _load_dense(mf, up, rank, n_ranks, kv_rank, kv_ranks, nh, nkv, ff0, v0, neox, device, first_exp, n_local, ep)
 
     def row_sliced(name, layer, expert, dst: DeviceQ40, rows_local, dst_stride=1, dst_off=0, head_dim=0, slice_rank=None):
         e = mf.entry(name, layer, expert)
@@ -247,8 +264,6 @@ def load_device_weights(mf: ModelFile, rank: int = 0, n_ranks: int = 1, device="
         W.embedding_ptrs, W.embedding_rows = shard[1], shard[2]
     row_sliced("final_matmul_logits", 0, 0, W.wcls, v0)
     perm = torch.from_numpy(_interleave_perm(hd)).to(device) if neox else None
-    n_exp = max(h.n_experts, 1)
-    first_exp, n_local = (rank * (h.n_experts // n_ranks), h.n_experts // n_ranks) if ep else (0, n_exp)
     W.first_expert, W.n_local_experts, W.moe_mode = first_exp, (n_local if h.n_experts > 0 else 0), ("ep" if ep else "tp")
     esr = 0 if ep else None      # expert tensors: whole matrices under EP
     for l in range(h.n_layers):
@@ -280,11 +295,12 @@ def load_device_weights(mf: ModelFile, rank: int = 0, n_ranks: int = 1, device="
 
 
 def synthetic_device_weights(cfg, rank: int = 0, n_ranks: int = 1, device="cuda", moe_mode: str = "auto", seed: int = 1234,
-                             max_seq_len: int = 0) -> DeviceWeights:
+                             max_seq_len: int = 0, weight_type: str = "q40") -> DeviceWeights:
     """Random-init weights of architecture `cfg`, created directly in the device layout of this rank (no `.m` file, no upload):
     used to benchmark the large configurations (Qwen3-14B, Qwen3-30B-A3B, Llama-3.3-70B) whose 11-40 GB files would take minutes
     to write on a fresh box. Shapes, partitioning (row / column slices, KV-head replication, expert placement) and value
-    statistics follow load_device_weights / write_synthetic_model; the values themselves are not those of a file with that seed."""
+    statistics follow load_device_weights / write_synthetic_model; the values themselves are not those of a file with that seed.
+    weight_type "f16" / "f32" builds the dense layout of an f16 / f32 file instead of q40 (normal values of the same std)."""
     import io
     from ..formats.model_file import write_model_header
     from .config import ARCH_QWEN3, ARCH_QWEN3_MOE
@@ -314,6 +330,12 @@ def synthetic_device_weights(cfg, rank: int = 0, n_ranks: int = 1, device="cuda"
         w.scales.copy_(((std / 4.61) * (0.7 + 0.6 * torch.rand(w.scales.shape, device=device, generator=g))).half())
         return w
 
+    def matrix(d, n, std, lead=1):
+        if weight_type == "q40":
+            return q40(d, n, std, lead)
+        dt = {"f16": torch.float16, "f32": torch.float32}[weight_type]
+        return DeviceDense(torch.randn(lead * d, n, device=device, generator=g, dtype=dt).mul_(std), d, n)
+
     def norm(n):
         return (1.0 + 0.1 * torch.randn(n, device=device, generator=g)).float()
 
@@ -321,7 +343,7 @@ def synthetic_device_weights(cfg, rank: int = 0, n_ranks: int = 1, device="cuda"
     ge.manual_seed(seed)      # the embedding is replicated: same values on every rank
     emb = torch.randn(h.vocab_size, dim, device=device, generator=ge)
     W = DeviceWeights(header=h, rank=rank, n_ranks=n_ranks, n_heads=nh, n_kv_heads=nkv, ff_dim=ff0, vocab=v0, embedding=emb,
-                      final_norm=norm(dim), wcls=q40(v0, dim, dim ** -0.5),
+                      final_norm=norm(dim), wcls=matrix(v0, dim, dim ** -0.5),
                       rope=torch.from_numpy(np.asarray(H.build_rope_table(h, h.seq_len))).to(device))
     n_exp = max(h.n_experts, 1)
     first_exp, n_local = (rank * (h.n_experts // n_ranks), h.n_experts // n_ranks) if ep else (0, n_exp)
@@ -329,8 +351,8 @@ def synthetic_device_weights(cfg, rank: int = 0, n_ranks: int = 1, device="cuda"
     gn = torch.Generator(device=device)
     gn.manual_seed(seed + 1)   # replicated tensors (norms, router gates)
     for _ in range(h.n_layers):
-        L = LayerWeights(qkv=q40(q0 + 2 * kv0, dim, dim ** -0.5), wo=q40(dim, q0, 0.5 * (h.n_heads * hd) ** -0.5),
-                         w13=q40(2 * ff0, dim, dim ** -0.5, lead=n_local), w2=q40(dim, ff0, 0.5 * h.ff_dim ** -0.5, lead=n_local),
+        L = LayerWeights(qkv=matrix(q0 + 2 * kv0, dim, dim ** -0.5), wo=matrix(dim, q0, 0.5 * (h.n_heads * hd) ** -0.5),
+                         w13=matrix(2 * ff0, dim, dim ** -0.5, lead=n_local), w2=matrix(dim, ff0, 0.5 * h.ff_dim ** -0.5, lead=n_local),
                          norm0=(1.0 + 0.1 * torch.randn(dim, device=device, generator=gn)), norm1=(1.0 + 0.1 * torch.randn(dim, device=device, generator=gn)))
         if h.qk_norm:
             L.q_norm = 1.0 + 0.1 * torch.randn(hd, device=device, generator=gn)
@@ -340,4 +362,5 @@ def synthetic_device_weights(cfg, rank: int = 0, n_ranks: int = 1, device="cuda"
         W.layers.append(L)
     torch.cuda.synchronize(device)
     W.bytes_uploaded = 0
+    W.weight_kind = {"q40": 0, "f32": 1, "f16": 2}[weight_type]
     return W

@@ -89,6 +89,8 @@ def lib() -> C.CDLL:
     L.dl_moe_prefill_ffn.restype = i32
     L.dl_moe_decode_ffn.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, u32, u32, u32, u32, u32, u32, f32, vp, vp, vp, vp, vp, vp, vp, u32, u32, vp]
     L.dl_moe_decode_ffn.restype = i32
+    L.dl_moe_decode_ffn_dense.argtypes = [i32, vp, vp, vp, vp, vp, vp, u32, u32, u32, u32, u32, u32, f32, vp, vp, vp, vp, vp, vp, vp, u32, u32, vp]
+    L.dl_moe_decode_ffn_dense.restype = i32
     L.dl_engine_create.argtypes = [C.POINTER(EngineConfig)]
     L.dl_engine_create.restype = vp
     L.dl_engine_destroy.argtypes = [vp]
@@ -218,6 +220,8 @@ _ERRORS = {
     -32: "mixture-of-experts down-projection shape not covered by the TMA GEMV (per-rank expert ffDim must be a multiple of 128: use moe_mode=ep)",
     -33: "arg-max under tensor parallelism needs the fused logits kernel",
     -36: "mixture-of-experts prefill shape not covered (dim, ffDim multiples of 256, chunk <= 256 tokens)",
+    -40: "the dense-weight GEMV has no in-kernel all-reduce (dense weight files use library collectives under tensor parallelism)",
+    -41: "expert-routed dense-weight GEMV needs one token, the routing slots' expert indices and k >= 1",
     -53: "logit_bias token id outside the sampled vocabulary",
 }
 
