@@ -1,5 +1,8 @@
 // Prompt-chunk (prefill) attention on the Hopper tensor cores: S = Q.K^T and O = P.V are wgmma.mma_async instructions with the
 // accumulators in registers; K and V tiles stream from the bf16 head-major KV cache through TMA tensor maps.
+// The maps are 3-D, {headDim, p0 + T, nKvHeads}, so TMA fills the rows of a tile at or past p0 + T with zeros: the kernel reads only
+// rows [0, p0 + T) of its own head, never a later (not yet written, or a previous request's) row or the next head's rows. Those rows
+// are masked to P = 0, but 0 * NaN is NaN on the tensor core as anywhere else.
 //
 // Work item (one CTA) = one KV head x one query tile. The `kvMul` query heads that share the KV head (GQA) are packed on the
 // MMA M dimension: a tile holds tq = 128 / kvMul consecutive prompt tokens x kvMul heads = up to 128 query rows, so every K / V
@@ -38,9 +41,9 @@ __device__ __forceinline__ void apBarWait(uint64_t *b, uint32_t parity) {
         "r"(parity)
         : "memory");
 }
-__device__ __forceinline__ void apTmaLoad2d(void *dst, const CUtensorMap *map, uint32_t c0, uint32_t c1, uint64_t *bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(apAddr(dst)),
-                 "l"(reinterpret_cast<uint64_t>(map)), "r"(apAddr(bar)), "r"(c0), "r"(c1)
+__device__ __forceinline__ void apTmaLoad3d(void *dst, const CUtensorMap *map, uint32_t c0, uint32_t c1, uint32_t c2, uint64_t *bar) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(apAddr(dst)),
+                 "l"(reinterpret_cast<uint64_t>(map)), "r"(apAddr(bar)), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
 }
 __device__ __forceinline__ uint32_t apPack(float lo, float hi) {
@@ -137,6 +140,7 @@ __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __gri
         }
     } else if (!Q8 && warp == 0) {
         // ================================ TMA producer ================================
+        // expect_tx counts the whole box: TMA delivers the zero-filled rows past p0 + T like the loaded ones
         if (lane == 0) {
             uint32_t itK = 0;
             for (uint32_t pass = 0; pass < 2; pass++) {
@@ -144,12 +148,12 @@ __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __gri
                     const uint32_t st = itK & 1, ph = (itK >> 1) & 1;
                     apBarWait(&kEmpty[st], ph ^ 1);
                     apBarExpectTx(&kFull[st], kTileBytes);
-                    for (uint32_t c = 0; c < NA; c++) apTmaLoad2d(Ks + st * kTileBytes + c * kApAtomBytes, &tmapK, c * 64, kvRow0 + j * 128, &kFull[st]);
+                    for (uint32_t c = 0; c < NA; c++) apTmaLoad3d(Ks + st * kTileBytes + c * kApAtomBytes, &tmapK, c * 64, j * 128, kvh, &kFull[st]);
                     if (pass == 1) {
                         const uint32_t vs = j & 1, vph = (j >> 1) & 1;
                         apBarWait(&vEmpty[vs], vph ^ 1);
                         apBarExpectTx(&vFull[vs], kTileBytes);
-                        for (uint32_t c = 0; c < NA; c++) apTmaLoad2d(Vs + vs * kTileBytes + c * kApAtomBytes, &tmapV, c * 64, kvRow0 + j * 128, &vFull[vs]);
+                        for (uint32_t c = 0; c < NA; c++) apTmaLoad3d(Vs + vs * kTileBytes + c * kApAtomBytes, &tmapV, c * 64, j * 128, kvh, &vFull[vs]);
                     }
                 }
             }
@@ -317,14 +321,15 @@ ApEncodeFn apEncode() {
     return fn;
 }
 
-bool apCacheMap(CUtensorMap *map, const void *cache, uint32_t hd, uint64_t rows) {
+// Rows [0, rows) of every head of a [nKvHeads][seqLen][hd] bf16 cache; a box is 64 columns x 128 rows of one head.
+bool apCacheMap(CUtensorMap *map, const void *cache, uint32_t hd, uint32_t rows, uint32_t nKvHeads, uint32_t seqLen) {
     ApEncodeFn enc = apEncode();
     if (!enc) return false;
-    const cuuint64_t dims[2] = {hd, rows};
-    const cuuint64_t strides[1] = {(cuuint64_t)hd * 2};
-    const cuuint32_t box[2] = {64, 128};
-    const cuuint32_t estr[2] = {1, 1};
-    return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(cache), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    const cuuint64_t dims[3] = {hd, rows, nKvHeads};
+    const cuuint64_t strides[2] = {(cuuint64_t)hd * 2, (cuuint64_t)hd * 2 * seqLen};
+    const cuuint32_t box[3] = {64, 128, 1};
+    const cuuint32_t estr[3] = {1, 1, 1};
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(cache), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -363,8 +368,9 @@ int launchAttnPrefillTc(const AttnPrefillArgs &a, cudaStream_t stream, bool pdl)
         return a.headDim == 128 ? apLaunch<128, true>(none, none, k, grid, stream, pdl) : apLaunch<64, true>(none, none, k, grid, stream, pdl);
     }
     CUtensorMap mk, mv;
-    const uint64_t rows = (uint64_t)a.nKvHeads * a.seqLen;
-    if (!apCacheMap(&mk, a.kCache, a.headDim, rows) || !apCacheMap(&mv, a.vCache, a.headDim, rows)) return -2;
+    const uint32_t rows = a.p0 + a.T;   // rows of each head this chunk may read; TMA zero-fills the rest of the last tile
+    if (!apCacheMap(&mk, a.kCache, a.headDim, rows, a.nKvHeads, a.seqLen) || !apCacheMap(&mv, a.vCache, a.headDim, rows, a.nKvHeads, a.seqLen))
+        return -2;
     return a.headDim == 128 ? apLaunch<128, false>(mk, mv, k, grid, stream, pdl) : apLaunch<64, false>(mk, mv, k, grid, stream, pdl);
 }
 

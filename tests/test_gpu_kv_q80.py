@@ -4,8 +4,8 @@
   f32, so where x / d lies within a hair of a rounding boundary either neighbour is accepted (the bracket of test_gpu_moe.py).
 * Every decode-attention kernel over q80 caches against float64 attention over the dequantised cache, bound 2e-4 * max|V|, with
   the needle keys of test_gpu_slots.py at split boundaries and in the neighbouring slots.
-* Prefill attention on the tensor cores over q80 caches against float64 (the tiles are widened to bf16: the bound of
-  test_gpu_attn_prefill.py).
+* Prefill attention over q80 caches, on the tensor cores and on the per-token fallback: test_gpu_attn_prefill.py, where the cache
+  type is a parameter of every case (the reference widens the tiles to bf16 as the kernel does).
 * The engine on q80 against OracleModel(kv_quant="q80") for every tiny family; the slots and choices steps; the persistent kernel
   against the multi-kernel path at Llama-3.1-8B layer shapes; slots batch invariance; both command-line stacks.
 """
@@ -290,47 +290,6 @@ def test_choice_attention_q80_matches_float64(B, P, j, hd, kv_mul):
             assert err <= bound, (b, h, err, bound)
 
 
-# ---- prefill attention -----------------------------------------------------------------------------------------------------------
-
-@pytest.mark.parametrize("n_heads,n_kv,hd", [(32, 8, 128), (8, 8, 128), (32, 8, 64), (6, 2, 64)])
-@pytest.mark.parametrize("T,p0", [(1, 7), (63, 100), (64, 0), (192, 300), (256, 5)])
-def test_attn_prefill_tc_q80_matches_float64(n_heads, n_kv, hd, T, p0):
-    from distributed_llama_b200.ops import cuda_lib as cl
-    lib = cl.lib()
-    g = torch.Generator().manual_seed(T + p0 + hd + n_heads)
-    seq = p0 + T + 40
-    q_dim = n_heads * hd
-    stride = q_dim + 2 * n_kv * hd
-    kv_mul = n_heads // n_kv
-    qkv = torch.randn(T, stride, generator=g)
-    k = torch.randn(n_kv, seq, hd, generator=g) * 0.6
-    v = torch.randn(n_kv, seq, hd, generator=g)
-    kq, ks, K = _planes(k)
-    vq, vs, V = _planes(v)
-    n_sc = n_kv * seq * hd // 32
-    for sc in (ks, vs):                                            # rows not yet written (and the tail padding) are never read
-        sc[n_sc:] = float("inf")
-        sc[:n_sc].view(n_kv, seq, hd // 32)[:, p0 + T:] = float("inf")
-    out = torch.zeros(T, q_dim, dtype=torch.bfloat16, device="cuda")
-    qd = qkv.cuda().contiguous()
-    assert lib.dl_attn_prefill_tc_q80(qd.data_ptr(), stride, T, p0, n_heads, n_kv, hd, seq, kq.data_ptr(), vq.data_ptr(), ks.data_ptr(),
-                                      vs.data_ptr(), out.data_ptr(), q_dim, cl.stream_ptr()) == 0
-    torch.cuda.synchronize()
-    got = out.cpu().double()
-    assert torch.isfinite(got).all()
-    scale = 1.0 / math.sqrt(hd)
-    err, ref_max = 0.0, 0.0
-    for t in range(T):
-        n = p0 + t + 1
-        for h in range(n_heads):
-            kvh = h // kv_mul
-            want = _attn_ref(qkv[t, h * hd:(h + 1) * hd], K[kvh], V[kvh], n, scale)
-            err = max(err, (got[t, h * hd:(h + 1) * hd] - want).abs().max().item())
-            ref_max = max(ref_max, want.abs().max().item())
-    bound = 0.03 * ref_max + 2e-3
-    assert err < bound, f"error {err:.3e} over the bound {bound:.3e} by {err - bound:.3e}"
-
-
 # ---- engine ----------------------------------------------------------------------------------------------------------------------
 
 def _engine(path, **kw):
@@ -357,7 +316,7 @@ def test_unknown_kv_cache_type_is_refused(tmp_models):
 @pytest.mark.parametrize("name", ["tiny-llama", "tiny-llama31", "tiny-qwen3", "tiny-qwen3-moe"])
 def test_engine_q80_matches_oracle(tmp_models, name):
     """Token by token, and a batched prefill then decode, on q80 caches against the oracle that rounds its stored K/V rows the same
-    way: test_engine_matches_oracle's sequence, paths and tolerance (the tensor-core prefill has its float64 test above)."""
+    way: test_engine_matches_oracle's sequence, paths and tolerance (the tensor-core prefill has its float64 test in test_gpu_attn_prefill.py)."""
     path = tmp_models[name][0]
     toks = [3, 17, 250, 9, 44, 101, 7, 300, 12, 5, 77]
     ref = _oracle(path).forward(toks, 0)
