@@ -64,7 +64,7 @@ struct NativeEngine::Impl {
     };
     std::vector<Layer> layers;
     // activations / state
-    int32_t *tokens = nullptr, *pos = nullptr, *history = nullptr, *pTokens = nullptr, *pPos = nullptr;
+    int32_t *tokens = nullptr, *pos = nullptr, *history = nullptr;
     float *logits = nullptr;
     std::vector<float> hostLogits;
     std::map<std::tuple<std::string, uint32_t, uint32_t>, const TensorEntry *> index;
@@ -128,30 +128,17 @@ NativeEngine::NativeEngine(const std::string &modelPath, uint32_t maxSeqLen, int
         Mapping file(modelPath);
         uploadWeights(file.data);
 
-        // ---- activation buffers (sizes as in distributed_llama_b200/runtime/engine.py) ----
+        // ---- the buffers this class reads or writes (the engine allocates its scratch itself) ----
         Impl &I = *impl_;
-        const uint32_t mb = maxBatch_, mp = maxPrefill_, kAct = std::max(1u, h_.nActiveExperts);
+        const uint32_t mb = maxBatch_;
         I.tokens = (int32_t *)dev(mb * 4); I.pos = (int32_t *)dev(mb * 4);
-        float *x = (float *)dev((size_t)mb * dim * 4), *qkv = (float *)dev((size_t)mb * qkvDim_ * 4), *z = (float *)dev((size_t)mb * qDim * 4);
-        float *hbuf = (float *)dev((size_t)std::max(mb, kAct) * ff * 4);
         I.logits = (float *)dev((size_t)mb * vocabL_ * 4);
         I.hostLogits.resize(vocab);
         I.history = (int32_t *)dev((size_t)(seqLen_ + 1) * 4);
-        I.pTokens = (int32_t *)dev(mp * 4); I.pPos = (int32_t *)dev(mp * 4);
         GlobalPtrs g{};
         g.embedding = I.embedding; g.finalNorm = I.finalNorm; g.wclsQs = I.wcls.qs; g.wclsSc = I.wcls.scales; g.rope = I.rope;
-        g.vocabFull = vocab; g.tokens = I.tokens; g.pos = I.pos; g.x = x; g.qkv = qkv; g.z = z; g.h = hbuf; g.logits = I.logits;
-        g.attnPartial = (float *)dev((size_t)mb * headsL_ * nSplits_ * (hd + 2) * 4);
-        g.attnCounters = (unsigned int *)dev((size_t)mb * headsL_ * 4);
+        g.vocabFull = vocab; g.tokens = I.tokens; g.pos = I.pos; g.x = (float *)dev((size_t)mb * dim * 4); g.logits = I.logits;
         g.history = I.history;
-        g.expertIdx = (int *)dev((size_t)mb * kAct * 4); g.expertWeight = (float *)dev((size_t)mb * kAct * 4);
-        g.routerLogits = (float *)dev((size_t)mb * std::max(1u, h_.nExperts) * 4); g.routerCounter = (unsigned int *)dev(mb * 4);
-        g.moeScratch = (float *)dev((size_t)kAct * dim * 4); g.moeCounters = (unsigned int *)dev(256 * 4);
-        g.maxPrefill = mp; g.pTokens = I.pTokens; g.pPos = I.pPos;
-        g.px = (float *)dev((size_t)mp * dim * 4); g.pqkv = (float *)dev((size_t)mp * std::max(qkvDim_, dim) * 4);   // also the [T][dim] partial product of the tensor-parallel WO / W2 GEMMs
-        g.pxn = dev((size_t)mp * dim * 2); g.pzb = dev((size_t)mp * qDim * 2); g.phb = dev((size_t)mp * ff * 2);
-        g.pAttnPartial = (float *)dev((size_t)mp * headsL_ * (hd + 2) * 4); g.pAttnCounters = (unsigned int *)dev((size_t)mp * headsL_ * 4);
-        g.argVal = (float *)dev(256 * 4); g.argIdx = (int *)dev(256 * 4); g.argCounter = (unsigned int *)dev(16);
 
         EngineConfig cfg{};
         cfg.dim = dim; cfg.nLayers = h_.nLayers; cfg.nHeads = headsL_; cfg.nKvHeads = kvHeadsL_; cfg.headDim = hd; cfg.ffDim = ff;
@@ -160,6 +147,7 @@ NativeEngine::NativeEngine(const std::string &modelPath, uint32_t maxSeqLen, int
         cfg.moeFirstExpert = 0; cfg.moeNumLocal = h_.nExperts; cfg.wType = 0;
         cfg.hiddenAct = h_.hiddenAct == ACT_GELU ? 1u : 0u;
         cfg.kvType = kvType_;
+        cfg.maxPrefill = 192;
         I.engine = dl_engine_create(&cfg);
         if (!I.engine) throw std::runtime_error("dl_engine_create failed");
         for (uint32_t l = 0; l < h_.nLayers; l++) {
@@ -173,28 +161,20 @@ NativeEngine::NativeEngine(const std::string &modelPath, uint32_t maxSeqLen, int
         }
         engCheck(dl_engine_set_globals(I.engine, &g), "dl_engine_set_globals");
         if (N > 1) {
-            // symmetric peer-memory arena, same layout as distributed_llama_b200/parallel/comm.py:arena_layout
-            auto align = [](uint64_t x) { return (x + 255) / 256 * 256; };
-            const uint32_t maxCtas = 256;
-            CommPtrs cp{};
-            uint64_t off = 0;
-            cp.slotsOff = off; off = align(off + 2ull * N * mb * dim * 8);            // LL words of the decode all-reduce
-            cp.flagsOff = off; off = align(off + 2ull * N * maxCtas * 4);             // logits-gather arrival counters
-            cp.candValOff = off; off = align(off + 8 * 8);                            // cross-rank arg-max candidates
-            cp.gatherOff = off; off = align(off + (uint64_t)mb * vocab * 4);          // gathered logits (device sampler)
-            cp.prefillSlotsOff = off; off = align(off + 2ull * N * mp * dim * 8);     // LL words of the prefill all-reduce
-            I.vmm = dl_vmm_create(rank_, N, off, commTag.c_str(), 1);
+            // symmetric peer-memory arena, laid out by the engine
+            const uint64_t bytes = dl_engine_arena_bytes(I.engine);
+            I.vmm = dl_vmm_create(rank_, N, bytes, commTag.c_str(), 1);
             if (!I.vmm) throw std::runtime_error("cannot create the peer-memory arena (CUDA VMM with POSIX file-descriptor handles is required)");
             if (hostBarrier) hostBarrier();      // every rank has bound its bootstrap socket
             engCheck(dl_vmm_connect(I.vmm), "dl_vmm_connect");
-            cudaCheck(cudaMemsetAsync(dl_vmm_ptr(I.vmm, rank_), 0, off, I.stream), "cudaMemset(arena)");
+            cudaCheck(cudaMemsetAsync(dl_vmm_ptr(I.vmm, rank_), 0, bytes, I.stream), "cudaMemset(arena)");
             cudaCheck(cudaStreamSynchronize(I.stream), "cudaMemset(arena)");
             engCheck(dl_vmm_barrier(I.vmm, 3), "dl_vmm_barrier");   // nobody pushes into an arena that is still being cleared
-            cp.nRanks = N; cp.rank = rank_; cp.maxCtas = maxCtas; cp.slotStride = mb * dim;
+            CommPtrs cp{};
+            cp.nRanks = N; cp.rank = rank_;
             for (uint32_t r = 0; r < N; r++) cp.arena[r] = dl_vmm_ptr(I.vmm, r);
             cp.mcArena = dl_vmm_mc_ptr(I.vmm);
             multicast_ = cp.mcArena != nullptr;
-            cp.prefillSlotStride = mp * dim;
             engCheck(dl_engine_set_comm(I.engine, &cp), "dl_engine_set_comm");
         }
         if (!moe) {
@@ -330,13 +310,13 @@ void NativeEngine::uploadWeights(const uint8_t *file) {
     cudaFree(staging);
 }
 
-void NativeEngine::setInputs(const int32_t *tokens, uint32_t n, uint32_t pos, bool prefillBuffers) {
+void NativeEngine::setInputs(const int32_t *tokens, uint32_t n, uint32_t pos) {
     std::vector<int32_t> p(n);
     for (uint32_t i = 0; i < n; i++) p[i] = (int32_t)(pos + i);
     Impl &I = *impl_;
     // pageable sources: the copies are staged before the call returns, so the vectors may die right away
-    cudaCheck(cudaMemcpyAsync(prefillBuffers ? I.pTokens : I.tokens, tokens, n * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(tokens)");
-    cudaCheck(cudaMemcpyAsync(prefillBuffers ? I.pPos : I.pos, p.data(), n * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(pos)");
+    cudaCheck(cudaMemcpyAsync(I.tokens, tokens, n * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(tokens)");
+    cudaCheck(cudaMemcpyAsync(I.pos, p.data(), n * 4, cudaMemcpyHostToDevice, I.stream), "cudaMemcpy(pos)");
 }
 
 void NativeEngine::forward(uint32_t n, int logitsMode, bool greedyAdvance) {
@@ -345,29 +325,13 @@ void NativeEngine::forward(uint32_t n, int logitsMode, bool greedyAdvance) {
 
 void NativeEngine::prefill(const std::vector<int32_t> &tokens, uint32_t pos) {
     if (pos + tokens.size() > seqLen_) throw std::runtime_error("position beyond the context length");
-    const bool tc = h_.nExperts == 0 || (h_.dim % 256 == 0 && ffL_ % 256 == 0);   // MoE: grouped tensor-core GEMMs need 256-wide K
-    size_t i = 0;
-    while (i < tokens.size()) {
-        const size_t rem = tokens.size() - i;
-        uint32_t n;
-        if (tc && rem >= 9) {
-            n = (uint32_t)std::min<size_t>(rem, maxPrefill_);
-            setInputs(tokens.data() + i, n, pos + (uint32_t)i, true);
-            engCheck(dl_engine_prefill(impl_->engine, n, pos + (uint32_t)i, 0, impl_->stream), "dl_engine_prefill");
-        } else {
-            n = 1;
-            while (n * 2 <= std::min<size_t>(rem, maxBatch_)) n *= 2;
-            setInputs(tokens.data() + i, n, pos + (uint32_t)i, false);
-            forward(n, 0, false);
-        }
-        i += n;
-    }
+    engCheck(dl_engine_prefill(impl_->engine, tokens.data(), (uint32_t)tokens.size(), pos, -1, 0, impl_->stream), "dl_engine_prefill");
 }
 
 const float *NativeEngine::step(int32_t token, uint32_t pos) {
     if (nRanks_ > 1) throw std::runtime_error("host-side logits are not gathered under tensor parallelism: use stepGreedy / stepSampled");
     if (pos >= seqLen_) throw std::runtime_error("position beyond the context length");
-    setInputs(&token, 1, pos, false);
+    setInputs(&token, 1, pos);
     forward(1, 1, false);
     Impl &I = *impl_;
     cudaCheck(cudaMemcpyAsync(I.hostLogits.data(), I.logits, (size_t)h_.vocabSize * 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(logits)");
@@ -378,15 +342,7 @@ const float *NativeEngine::step(int32_t token, uint32_t pos) {
 std::vector<int32_t> NativeEngine::decodeGreedy(int32_t firstToken, uint32_t pos, uint32_t nSteps) {
     if (pos + nSteps > seqLen_) throw std::runtime_error("decode would run past the context length");
     Impl &I = *impl_;
-    setInputs(&firstToken, 1, pos, false);
-    if (!graphReady_) {
-        // warm-up run configures kernel attributes outside of capture; inputs are restored afterwards
-        forward(1, 1, false);
-        cudaCheck(cudaStreamSynchronize(I.stream), "warm-up");
-        engCheck(dl_engine_capture_decode(I.engine), "dl_engine_capture_decode");
-        graphReady_ = true;
-        setInputs(&firstToken, 1, pos, false);
-    }
+    setInputs(&firstToken, 1, pos);
     engCheck(dl_engine_decode_graph(I.engine, (int)nSteps, I.stream), "dl_engine_decode_graph");
     std::vector<int32_t> out(nSteps);
     cudaCheck(cudaMemcpyAsync(out.data(), I.history + pos + 1, (size_t)nSteps * 4, cudaMemcpyDeviceToHost, I.stream), "cudaMemcpy(history)");
@@ -397,14 +353,7 @@ std::vector<int32_t> NativeEngine::decodeGreedy(int32_t firstToken, uint32_t pos
 int32_t NativeEngine::stepGreedy(int32_t token, uint32_t pos) {
     if (pos >= seqLen_) throw std::runtime_error("position beyond the context length");
     Impl &I = *impl_;
-    setInputs(&token, 1, pos, false);
-    if (!graphReady_) {
-        forward(1, 1, false);
-        cudaCheck(cudaStreamSynchronize(I.stream), "warm-up");
-        engCheck(dl_engine_capture_decode(I.engine), "dl_engine_capture_decode");
-        graphReady_ = true;
-        setInputs(&token, 1, pos, false);
-    }
+    setInputs(&token, 1, pos);
     engCheck(dl_engine_decode_graph(I.engine, 1, I.stream), "dl_engine_decode_graph");
     if (lpK_ >= 0) logprobsAfterDraw(1, 1u, 0, 0);
     int32_t next = 0;   // the arg-max kernel leaves the sampled token in tokens[0] (and advances pos[0]) on the device
@@ -419,7 +368,7 @@ void NativeEngine::seedSampler(uint64_t seed) { engCheck(dl_engine_sampler_seed(
 int32_t NativeEngine::stepSampled(int32_t token, uint32_t pos, float temperature, float topp) {
     if (pos >= seqLen_) throw std::runtime_error("position beyond the context length");
     Impl &I = *impl_;
-    setInputs(&token, 1, pos, false);
+    setInputs(&token, 1, pos);
     forward(1, 1, false);
     engCheck(dl_engine_sample(I.engine, temperature, topp, I.stream), "dl_engine_sample");
     if (lpK_ >= 0) logprobsAfterDraw(1, 1u, 0, kLogprobsControlled);
@@ -455,7 +404,7 @@ static uint32_t choiceBatch(uint32_t n) { uint32_t nb = 1; while (nb < n) nb *= 
 std::vector<int32_t> NativeEngine::choicesFirst(int32_t token, uint32_t P, uint32_t n, float temperature, float topp) {
     if (!supportsChoices(n) || P >= seqLen_) throw std::runtime_error("choices: unsupported batch or position");
     Impl &I = *impl_;
-    setInputs(&token, 1, P, false);
+    setInputs(&token, 1, P);
     forward(1, 1, false);
     const uint32_t nb = choiceBatch(n), mask = ((1u << nb) - 1u) & ~((1u << n) - 1u);
     engCheck(dl_engine_sample_rows(I.engine, (int)nb, mask, temperature, topp, 1, I.stream), "dl_engine_sample_rows");
@@ -496,12 +445,7 @@ uint32_t NativeEngine::slotLen() const { return dl_engine_slot_len(impl_->engine
 
 void NativeEngine::slotPrefill(uint32_t slot, const std::vector<int32_t> &tokens, uint32_t pos) {
     if (pos + tokens.size() > slotLen()) throw std::runtime_error("position beyond the slot length");
-    for (size_t i = 0; i < tokens.size();) {
-        const uint32_t n = (uint32_t)std::min<size_t>(tokens.size() - i, maxPrefill_);
-        setInputs(tokens.data() + i, n, pos + (uint32_t)i, true);
-        engCheck(dl_engine_slot_prefill(impl_->engine, slot, n, pos + (uint32_t)i, impl_->stream), "dl_engine_slot_prefill");
-        i += n;
-    }
+    engCheck(dl_engine_prefill(impl_->engine, tokens.data(), (uint32_t)tokens.size(), pos, (int)slot, 0, impl_->stream), "dl_engine_prefill");
 }
 
 void NativeEngine::slotCopy(uint32_t src, uint32_t dst, uint32_t P) {
@@ -592,7 +536,6 @@ void NativeEngine::synchronize() { cudaCheck(cudaStreamSynchronize(impl_->stream
 void NativeEngine::setVocabLimit(uint32_t limit) {
     if (limit >= h_.vocabSize) limit = 0;
     engCheck(dl_engine_set_vocab_limit(impl_->engine, limit), "dl_engine_set_vocab_limit");
-    graphReady_ = false;   // the limit is a launch parameter of the captured step
 }
 
 }  // namespace dl

@@ -55,8 +55,8 @@ public:
     bool multicast() const { return multicast_; }
     bool persistentKernel() const { return mega_; }
 
-    // Feeds prompt tokens at positions [pos, pos + n): chunks of up to 192 tokens on the tensor-core path (dense models),
-    // power-of-two batches of up to 8 on the GEMV path otherwise. No logits are produced.
+    // Feeds prompt tokens at positions [pos, pos + n), chunked by the engine (dl_engine_prefill): up to 192 tokens a chunk on
+    // the tensor-core path, power-of-two batches of up to 8 on the GEMV path. No logits are produced.
     void prefill(const std::vector<int32_t> &tokens, uint32_t pos);
     // One token; returns the logits row (host memory owned by the engine, valid until the next call). Single GPU only: under tensor
     // parallelism the logits stay sharded on the devices (use stepGreedy / stepSampled).
@@ -121,7 +121,7 @@ private:
     void *dev(size_t bytes);            // zero-initialised device allocation owned by the engine
     void release();
     void uploadWeights(const uint8_t *file);
-    void setInputs(const int32_t *tokens, uint32_t n, uint32_t pos, bool prefillBuffers);
+    void setInputs(const int32_t *tokens, uint32_t n, uint32_t pos);
     void forward(uint32_t n, int logitsMode, bool greedyAdvance);
     void logprobsAfterDraw(uint32_t rows, uint32_t rowMask, int firstRow, int flags);   // enqueue + copy the blocks, before the sync
 
@@ -133,11 +133,11 @@ private:
     ModelHeader h_;
     std::vector<TensorEntry> dir_;
     uint32_t slots_ = 1;
-    uint32_t seqLen_ = 0, maxBatch_ = 8, maxPrefill_ = 192, nSplits_ = 1, qkvDim_ = 0;
+    uint32_t seqLen_ = 0, maxBatch_ = 8, nSplits_ = 1, qkvDim_ = 0;
     uint32_t kvType_ = 0;                                                  // KV-cache storage: 0 = bf16, 1 = q80
     uint32_t rank_ = 0, nRanks_ = 1, kvRank_ = 0, kvSlices_ = 1;          // tensor-parallel placement of this process
     uint32_t headsL_ = 0, kvHeadsL_ = 0, ffL_ = 0, vocabL_ = 0;          // per-rank slice sizes
-    bool mega_ = false, graphReady_ = false, multicast_ = false;
+    bool mega_ = false, multicast_ = false;
     uint64_t bytesUploaded_ = 0;
     Impl *impl_ = nullptr;
 };

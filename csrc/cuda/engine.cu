@@ -1,4 +1,4 @@
-// Per-rank inference engine: owns the kernel schedule of one forward pass and the CUDA graph of the decode step.
+// Per-rank inference engine: owns the kernel schedule of one forward pass, its scratch, arena layout, prompt chunking and decode graph.
 //
 // Role in the reference: NnExecutor + NnCpuDevice/NnVulkanDevice + the `start/att/ff/end` segments emitted by
 // buildLlmNet (src/nn/nn-executor.cpp:45-207, src/llm.cpp:247-603) — ~26 barrier-separated ops per layer driven
@@ -6,8 +6,10 @@
 // programmatic dependent launch, and the single-token step is captured once into a CUDA graph whose inputs
 // (token id, position) live in device memory so the graph replays without host round trips:
 // the sampling kernel writes the next token and advances the position on the device.
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include <vector>
 
 #include "engine_api.h"
@@ -20,11 +22,43 @@ uint32_t gHiddenAct = 0;
 static_assert(kApiMaxRanks == kMaxRanks, "engine_api.h and kernels.h disagree on the rank limit");
 static_assert(kApiLogprobsWords == kLogprobsWords && kApiLogprobsMaxTop == kLogprobsMaxTop, "engine_api.h and kernels.h disagree on logprobs");
 
+// The client's GlobalPtrs and the scratch buffers the engine allocates for itself (allocScratch).
+struct Buffers : GlobalPtrs {
+    float *qkv, *z, *h;          // [maxBatch][qkvDim | qDim | ff] (h: at least nActiveExperts rows)
+    float *attnPartial;          // [maxBatch][nHeads][nSplits][hd+2]
+    unsigned int *attnCounters;  // [maxBatch][nHeads]
+    // MoE scratch
+    int *expertIdx;              // [maxBatch][nActive]
+    float *expertWeight;         // [maxBatch][nActive]
+    float *routerLogits;         // [maxBatch][nExperts]
+    unsigned int *routerCounter; // [maxBatch]
+    float *moeScratch;           // [nActive][dim]
+    unsigned int *moeCounters;   // [256]
+    // prefill (tensor-core GEMM path) buffers, maxPrefill tokens
+    int *pTokens, *pPos;         // [maxPrefill]
+    float *px, *pqkv;            // [maxPrefill][dim | max(qkvDim, dim)] f32
+    void *pxn, *pzb, *phb;       // bf16 [maxPrefill][dim | qDim | ff]
+    float *pAttnPartial;         // [maxPrefill][nHeads][hd+2]
+    unsigned int *pAttnCounters; // [maxPrefill][nHeads]
+    // fused arg-max scratch
+    float *argVal;               // [256 >= numSms]
+    int *argIdx;                 // [256]
+    unsigned int *argCounter;    // [4]
+};
+
+// The client's CommPtrs and the arena layout the engine derives from its configuration (arenaLayout).
+struct Comm : CommPtrs {
+    uint32_t maxCtas, slotStride, prefillSlotStride;
+    uint64_t slotsOff, flagsOff, candValOff, gatherOff, prefillSlotsOff;
+};
+
 struct Engine {
     EngineConfig cfg{};
-    CommPtrs comm{};
+    Comm comm{};
     std::vector<LayerPtrs> layers;
-    GlobalPtrs g{};
+    Buffers g{};
+    uint8_t *scratch = nullptr;    // the allocation behind the Buffers scratch pointers
+    uint32_t prefillMinTc = 9;     // shortest prompt chunk on the tensor cores (0: never)
     cudaGraphExec_t decodeGraph = nullptr;
     cudaStream_t captureStream = nullptr;
     int lastError = 0;
@@ -87,7 +121,7 @@ static EmbTable embTable(const Engine &e) {
 }
 
 static void fillAr(const Engine &e, ArArgs &ar, uint32_t parity) {
-    const CommPtrs &c = e.comm;
+    const Comm &c = e.comm;
     ar.nRanks = c.nRanks; ar.rank = c.rank; ar.parity = parity; ar.maxCtas = c.maxCtas; ar.slotStride = c.slotStride; ar.dim = e.cfg.dim;
     ar.slotsMc = c.mcArena ? (uint64_t *)((uint8_t *)c.mcArena + c.slotsOff) : nullptr;
     for (uint32_t r = 0; r < c.nRanks && r < (uint32_t)kMaxRanks; r++) {
@@ -367,10 +401,10 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
 // slot >= 0: the chunk goes into KV-cache slot `slot` (a cache of its own of slotLen rows).
 static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cudaStream_t stream, int slot = -1) {
     const EngineConfig &c = e.cfg;
-    const GlobalPtrs &g = e.g;
+    const Buffers &g = e.g;
     const bool pdl = c.usePdl != 0;   // every kernel of this chain waits (griddepcontrol.wait) before touching its predecessor's data
     const uint32_t qDim = c.nHeads * c.headDim, kvDim = c.nKvHeads * c.headDim, qkvDim = qDim + 2 * kvDim;
-    if (T < 1 || T > g.maxPrefill || T > 256) return -11;
+    if (T < 1 || T > c.maxPrefill) return -11;
     if (c.wType != 0) return -35;   // tensor-core path: q40 matrices
     const uint32_t seqLen = slot >= 0 ? e.slotLen : c.seqLen;
     const uint64_t cacheOff = slot >= 0 ? (uint64_t)slot * slotElems(e) : 0;
@@ -446,6 +480,56 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
     return 0;
 }
 
+// Every buffer that only the engine's kernels touch, carved from one zero-filled allocation with the decode step's buffers first
+// (one cudaMalloc each decoded 0.5% slower on an H100): the attention, router, MoE, arg-max and prefill counters reset themselves
+// and rely on starting at zero.
+static bool allocScratch(Engine &e) {
+    const EngineConfig &c = e.cfg;
+    const size_t mb = c.maxBatch, mp = c.maxPrefill, hd = c.headDim, f = sizeof(float);
+    const size_t qDim = c.nHeads * hd, qkvDim = qDim + 2 * c.nKvHeads * hd, kAct = std::max(1u, c.nActiveExperts);
+    Buffers &g = e.g;
+    size_t off = 0;
+    auto carve = [&](auto &p, size_t bytes) {
+        p = (std::remove_reference_t<decltype(p)>)((uintptr_t)e.scratch + off);
+        off += (bytes + 255) / 256 * 256;
+    };
+    auto carveAll = [&] {
+        off = 0;
+        carve(g.qkv, mb * qkvDim * f); carve(g.z, mb * qDim * f); carve(g.h, std::max(mb, kAct) * c.ffDim * f);
+        carve(g.attnPartial, mb * c.nHeads * c.nSplits * (hd + 2) * f); carve(g.attnCounters, mb * c.nHeads * 4);
+        carve(g.argVal, 256 * f); carve(g.argIdx, 256 * 4); carve(g.argCounter, 16);
+        carve(g.expertIdx, mb * kAct * 4); carve(g.expertWeight, mb * kAct * f);
+        carve(g.routerLogits, mb * std::max(1u, c.nExperts) * f); carve(g.routerCounter, mb * 4);
+        carve(g.moeScratch, kAct * c.dim * f); carve(g.moeCounters, 256 * 4);
+        carve(g.pTokens, mp * 4); carve(g.pPos, mp * 4);
+        carve(g.px, mp * c.dim * f); carve(g.pqkv, mp * std::max<size_t>(qkvDim, c.dim) * f);   // also the [T][dim] partial of the TP WO / W2 GEMMs
+        carve(g.pxn, mp * c.dim * 2); carve(g.pzb, mp * qDim * 2); carve(g.phb, mp * c.ffDim * 2);
+        carve(g.pAttnPartial, mp * c.nHeads * (hd + 2) * f); carve(g.pAttnCounters, mp * c.nHeads * 4);
+    };
+    carveAll();   // sizes
+    if (cudaMalloc(&e.scratch, off) != cudaSuccess) return false;
+    carveAll();   // pointers
+    return cudaMemset(e.scratch, 0, off) == cudaSuccess && cudaDeviceSynchronize() == cudaSuccess;   // zero before any client stream runs
+}
+
+// Offsets of the symmetric peer-memory arena, every rank alike; returns its size.
+static uint64_t arenaLayout(const EngineConfig &c, uint32_t vocabFull, Comm &m) {
+    auto align = [](uint64_t x) { return (x + 255) / 256 * 256; };
+    const uint64_t N = c.nRanks, mb = c.maxBatch, mp = c.maxPrefill, dim = c.dim;
+    m.maxCtas = 256; m.slotStride = c.maxBatch * c.dim; m.prefillSlotStride = c.maxPrefill * c.dim;
+    uint64_t off = 0;
+    m.slotsOff = off; off = align(off + 2 * N * mb * dim * 8);            // LL words (f32 payload, flag) of the decode all-reduce
+    m.flagsOff = off; off = align(off + 2 * N * m.maxCtas * 4);           // logits-gather arrival counters (sampler.cu)
+    m.candValOff = off; off = align(off + 8 * 8);                         // cross-rank arg-max candidates, one LL word per rank
+    m.gatherOff = off; off = align(off + mb * vocabFull * 4);             // gathered logits (device sampler)
+    m.prefillSlotsOff = off; off = align(off + 2 * N * mp * dim * 8);     // LL words of the prefill all-reduce
+    return off;
+}
+
+static void dropGraph(Engine &e) {
+    if (e.decodeGraph) { cudaGraphExecDestroy(e.decodeGraph); e.decodeGraph = nullptr; }
+}
+
 }  // namespace dl
 
 using dl::Engine;
@@ -456,6 +540,7 @@ static_assert(sizeof(Engine::slotLogprobs) == kChoiceRngSlots * sizeof(int), "on
 
 DL_EXPORT void *dl_engine_create(const dl::EngineConfig *cfg) {
     if (cfg->kvType > 1 || (cfg->kvType == 1 && cfg->headDim % 32)) return nullptr;   // unknown KV-cache storage
+    if (cfg->maxPrefill < 1 || cfg->maxPrefill > 256) return nullptr;
     Engine *e = new Engine();
     e->cfg = *cfg;
     dl::gHiddenAct = cfg->hiddenAct;
@@ -470,6 +555,10 @@ DL_EXPORT void *dl_engine_create(const dl::EngineConfig *cfg) {
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         e->cfg.numSms = (uint32_t)sms;
+    }
+    if (!dl::allocScratch(*e)) {
+        dl_engine_destroy(e);
+        return nullptr;
     }
     return e;
 }
@@ -493,6 +582,7 @@ DL_EXPORT void dl_engine_destroy(void *h) {
     if (e->slotStaged) cudaEventDestroy(e->slotStaged);
     if (e->slotLpDev) cudaFree(e->slotLpDev);
     if (e->slotLpHost) cudaFreeHost(e->slotLpHost);
+    if (e->scratch) cudaFree(e->scratch);
     delete e;
 }
 
@@ -504,7 +594,7 @@ DL_EXPORT int dl_engine_set_layer(void *h, uint32_t layer, const dl::LayerPtrs *
 }
 
 DL_EXPORT int dl_engine_set_globals(void *h, const dl::GlobalPtrs *p) {
-    ((Engine *)h)->g = *p;
+    static_cast<dl::GlobalPtrs &>(((Engine *)h)->g) = *p;
     return 0;
 }
 
@@ -553,12 +643,13 @@ DL_EXPORT int dl_engine_enable_mega(void *h, int enable) {
         if (const char *g = std::getenv("DL_MEGA_INFLIGHT")) e->megaInflight = (uint32_t)std::atoi(g);
     }
     e->useMega = enable != 0;
+    dl::dropGraph(*e);   // the captured step runs the kernels chosen at capture
     return 0;
 }
 
 DL_EXPORT int dl_engine_set_vocab_limit(void *h, uint32_t limit) {
     Engine *e = (Engine *)h;
-    if (e->vocabLimit != limit && e->decodeGraph) { cudaGraphExecDestroy(e->decodeGraph); e->decodeGraph = nullptr; }   // the limit is baked into the captured launch
+    if (e->vocabLimit != limit) dl::dropGraph(*e);   // the limit is baked into the captured launch
     e->vocabLimit = limit;
     return 0;
 }
@@ -771,19 +862,30 @@ DL_EXPORT int dl_engine_logprobs(void *h, int rows, uint32_t rowMask, const int3
                                   e->g.tokens, out, stream, ctl);
 }
 
+DL_EXPORT uint64_t dl_engine_arena_bytes(void *h) {
+    dl::Comm layout{};
+    return dl::arenaLayout(((Engine *)h)->cfg, ((Engine *)h)->g.vocabFull, layout);
+}
+
+// Every rank's arena of dl_engine_arena_bytes bytes, zeroed on every rank before any rank's kernels use it.
 DL_EXPORT int dl_engine_set_comm(void *h, const dl::CommPtrs *p) {
-    ((Engine *)h)->comm = *p;
+    Engine *e = (Engine *)h;
+    if (p->nRanks != e->cfg.nRanks) return -2;
+    static_cast<dl::CommPtrs &>(e->comm) = *p;
+    dl::arenaLayout(e->cfg, e->g.vocabFull, e->comm);
     return 0;
 }
 
 DL_EXPORT int dl_engine_set_trace(void *h, uint64_t *buf, uint32_t capLaunches) {
     ((Engine *)h)->trace = buf;
     ((Engine *)h)->traceCap = capLaunches;
+    dl::dropGraph(*(Engine *)h);   // the trace buffer is a launch parameter of the captured step
     return 0;
 }
 
 DL_EXPORT int dl_engine_set_trace_all(void *h, int allCtas) {
     ((Engine *)h)->traceAllCtas = allCtas != 0;
+    dl::dropGraph(*(Engine *)h);
     return 0;
 }
 
@@ -906,15 +1008,46 @@ DL_EXPORT int dl_moe_decode_ffn_dense(int wtype, const float *x, float *out, con
     return dl::moeDecodeFfn(m, stream, false);
 }
 
-DL_EXPORT int dl_engine_prefill(void *h, uint32_t T, uint32_t p0, int wantLogits, cudaStream_t stream) {
-    return dl::enginePrefill(*(Engine *)h, T, p0, wantLogits, stream);
+// A prompt of n tokens (host memory) at positions p0 .. p0 + n - 1, staged chunk by chunk on `stream`; logits of the last
+// token with wantLogits. A chunk of up to maxPrefill tokens runs on the tensor cores while at least prefillMinTc tokens remain
+// and the shape allows it: q40 matrices; MoE: dim and ff multiples of 256 (grouped GEMMs); tensor parallel: per-rank qDim, ff and
+// dim multiples of 256 (prefill all-reduce). Otherwise the largest power-of-two GEMV batch <= min(remaining, maxBatch) runs.
+// slot >= 0: into KV-cache slot `slot`, every chunk on the tensor cores.
+DL_EXPORT int dl_engine_prefill(void *h, const int32_t *hostTokens, uint32_t n, uint32_t p0, int slot, int wantLogits, cudaStream_t stream) {
+    Engine &e = *(Engine *)h;
+    const dl::EngineConfig &c = e.cfg;
+    if (slot >= 0 && e.slots < 2) return -64;
+    if ((uint64_t)p0 + n > (slot >= 0 ? e.slotLen : c.seqLen)) return -60;
+    const bool tpOk = e.comm.nRanks <= 1 || ((c.nHeads * c.headDim) % 256 == 0 && c.ffDim % 256 == 0 && c.dim % 256 == 0);
+    const bool moeOk = c.nExperts == 0 || (c.dim % 256 == 0 && c.ffDim % 256 == 0);
+    const bool tc = e.prefillMinTc > 0 && c.wType == 0 && tpOk && moeOk;
+    std::vector<int32_t> pos(n);
+    for (uint32_t i = 0; i < n; i++) pos[i] = (int32_t)(p0 + i);
+    for (uint32_t i = 0; i < n;) {
+        const uint32_t rem = n - i;
+        const bool onTc = slot >= 0 || (tc && rem >= e.prefillMinTc);
+        uint32_t T = 1;
+        if (onTc) T = std::min(rem, c.maxPrefill);
+        else while (T * 2 <= std::min(rem, c.maxBatch)) T *= 2;
+        const bool logits = wantLogits && i + T == n;
+        // pageable sources: each copy has read its host bytes when the call returns
+        DL_CUDA_CHECK(cudaMemcpyAsync(onTc ? e.g.pTokens : e.g.tokens, hostTokens + i, T * 4, cudaMemcpyHostToDevice, stream));
+        DL_CUDA_CHECK(cudaMemcpyAsync(onTc ? e.g.pPos : e.g.pos, pos.data() + i, T * 4, cudaMemcpyHostToDevice, stream));
+        if (onTc) DL_TRY(dl::enginePrefill(e, T, p0 + i, logits, stream, slot));
+        else DL_TRY(dl::engineForward(e, (int)T, logits ? 1 : 0, false, stream));
+        i += T;
+    }
+    return 0;
 }
 
-// Captures one greedy decode step (forward of 1 token + argmax + position advance) into a graph.
-DL_EXPORT int dl_engine_capture_decode(void *h) {
-    Engine *e = (Engine *)h;
+DL_EXPORT int dl_engine_set_prefill_min_tc(void *h, uint32_t n) { ((Engine *)h)->prefillMinTc = n; return 0; }
+
+// Captures one greedy decode step (forward of 1 token + argmax + position advance) into a graph, after a warm-up forward on
+// `stream` that sets kernel attributes outside of capture. Without greedyAdvance no kernel writes tokens, pos or history.
+static int captureDecode(Engine *e, cudaStream_t stream) {
+    DL_TRY(dl::engineForward(*e, 1, 1, false, stream));
+    DL_CUDA_CHECK(cudaStreamSynchronize(stream));
     if (!e->captureStream) DL_CUDA_CHECK(cudaStreamCreateWithFlags(&e->captureStream, cudaStreamNonBlocking));
-    if (e->decodeGraph) { cudaGraphExecDestroy(e->decodeGraph); e->decodeGraph = nullptr; }
     DL_CUDA_CHECK(cudaStreamBeginCapture(e->captureStream, cudaStreamCaptureModeThreadLocal));
     const int r = dl::engineForward(*e, 1, 1, true, e->captureStream);
     cudaGraph_t graph = nullptr;
@@ -926,12 +1059,19 @@ DL_EXPORT int dl_engine_capture_decode(void *h) {
     return 0;
 }
 
-// Replays the captured step `nSteps` times back to back on `stream` (no host sync in between).
+// Replays the captured step `nSteps` times back to back on `stream` (no host sync in between), capturing it first if the
+// engine has no graph of its current configuration.
 DL_EXPORT int dl_engine_decode_graph(void *h, int nSteps, cudaStream_t stream) {
     Engine *e = (Engine *)h;
-    if (!e->decodeGraph) return -20;
+    if (!e->decodeGraph) DL_TRY(captureDecode(e, stream));
     for (int i = 0; i < nSteps; i++) DL_CUDA_CHECK(cudaGraphLaunch(e->decodeGraph, stream));
     return 0;
+}
+
+DL_EXPORT int dl_engine_graph_captured(void *h) { return ((Engine *)h)->decodeGraph ? 1 : 0; }
+
+DL_EXPORT void dl_abi_struct_sizes(uint32_t out[4]) {
+    out[0] = sizeof(dl::EngineConfig); out[1] = sizeof(dl::LayerPtrs); out[2] = sizeof(dl::GlobalPtrs); out[3] = sizeof(dl::CommPtrs);
 }
 
 // ---- KV-cache slots: up to 8 independent sequences decoded together (attn_decode.cu) -------------------------------------------------
@@ -969,14 +1109,6 @@ DL_EXPORT int dl_engine_set_slots(void *h, uint32_t n) {
 DL_EXPORT uint32_t dl_engine_slot_len(void *h) {
     Engine *e = (Engine *)h;
     return e->slots > 1 ? e->slotLen : e->cfg.seqLen;
-}
-
-// Prompt chunk of T tokens (staged in pTokens / pPos at positions p0 .. p0 + T - 1 < slot length) into slot `slot`: the prefill
-// kernels of dl_engine_prefill with the slot's cache and length. No logits.
-DL_EXPORT int dl_engine_slot_prefill(void *h, uint32_t slot, uint32_t T, uint32_t p0, cudaStream_t stream) {
-    Engine *e = (Engine *)h;
-    if (e->slots < 2) return -64;
-    return dl::enginePrefill(*e, T, p0, 0, stream, (int)slot);
 }
 
 // Copies rows [0, P) of slot src into slot dst, every layer and KV head (several completions of one prompt).

@@ -24,6 +24,7 @@ struct EngineConfig {   // mirrored by ctypes in distributed_llama_b200/ops/cuda
     uint32_t wType;          // matrix storage: 0 = q40 device layout, 1 = dense f32, 2 = dense f16 (gemv_dense.cu)
     uint32_t hiddenAct;      // gate activation: 0 = SiLU, 1 = GELU (tanh form) — the `.m` header's hidden_act
     uint32_t kvType;         // KV-cache storage: 0 = bf16, 1 = q80 (int8 values + f16 scale per 32, LayerPtrs::kScale / vScale)
+    uint32_t maxPrefill;     // tokens per tensor-core prompt chunk, 1..256
 };
 
 struct LayerPtrs {
@@ -37,7 +38,7 @@ struct LayerPtrs {
     void *kScale, *vScale;       // kvType 1: f16 [nKvHeads][seqLen][hd / 32] + 16 bytes of tail padding; unused for bf16
 };
 
-struct GlobalPtrs {
+struct GlobalPtrs {   // the engine allocates its scratch buffers itself (dl_engine_create)
     const float *embedding;      // [vocabFull][dim] (replicated) or this rank's shard when embRowsPerRank != 0
     const float *embeddingPeers[kApiMaxRanks];   // vocabulary shards of all ranks (peer-mapped), used when embRowsPerRank != 0
     uint32_t embRowsPerRank;     // 0: `embedding` is the whole table
@@ -45,48 +46,27 @@ struct GlobalPtrs {
     const void *wclsQs, *wclsSc; // [vocab][dim]
     const float *rope;           // [seqLen][hd/2][2]
     uint32_t vocabFull;
-    // activations / state
+    // buffers the client reads or writes
     int *tokens, *pos;           // [maxBatch]
-    float *x, *qkv, *z, *h, *logits;   // [maxBatch][dim | qkvDim | qDim | ff | vocab]
-    float *attnPartial;          // [maxBatch][nHeads][nSplits][hd+2]
-    unsigned int *attnCounters;  // [maxBatch][nHeads]
+    float *x;                    // [maxBatch][dim] residual stream (the library-collective path adds its all-reduced partials here)
+    float *logits;               // [maxBatch][vocab]
     int *history;                // [seqLen] generated token per position (device-side log), may be null
-    // MoE scratch
-    int *expertIdx;              // [maxBatch][nActive]
-    float *expertWeight;         // [maxBatch][nActive]
-    float *routerLogits;         // [maxBatch][nExperts]
-    unsigned int *routerCounter; // [maxBatch]
-    float *moeScratch;           // [nActive][dim]
-    unsigned int *moeCounters;   // [256]
-    // prefill (tensor-core GEMM path) buffers, maxPrefill tokens
-    uint32_t maxPrefill;
-    int *pTokens, *pPos;         // [maxPrefill]
-    float *px, *pqkv;            // [maxPrefill][dim | qkvDim] f32
-    void *pxn, *pzb, *phb;       // bf16 [maxPrefill][dim | qDim | ff]
-    float *pAttnPartial;         // [maxPrefill][nHeads][hd+2]
-    unsigned int *pAttnCounters; // [maxPrefill][nHeads]
-    // fused arg-max scratch
-    float *argVal;               // [numSms]
-    int *argIdx;                 // [numSms]
-    unsigned int *argCounter;    // [1]
 };
 
-struct CommPtrs {   // mirrored by ctypes
-    uint32_t nRanks, rank, maxCtas, slotStride;
+struct CommPtrs {   // mirrored by ctypes; the engine lays out the arena itself (dl_engine_arena_bytes)
+    uint32_t nRanks, rank;
     void *arena[kApiMaxRanks];          // every rank's symmetric arena mapped into this process
     void *mcArena;                      // NVLS multicast mapping of the arena (null: none)
-    uint64_t slotsOff, flagsOff, candValOff, gatherOff;   // LL all-reduce slots, logits-gather arrival counters, arg-max candidates, gathered logits
-    uint64_t prefillSlotsOff;        // LL slots for the prefill GEMM all-reduce: [2][nRanks][maxPrefill * dim]
-    uint32_t prefillSlotStride;
 };
 
 }  // namespace dl
 
 extern "C" {
-void *dl_engine_create(const dl::EngineConfig *cfg);
+void *dl_engine_create(const dl::EngineConfig *cfg);   // null on an unsupported configuration or a failed allocation
 void dl_engine_destroy(void *h);
 int dl_engine_set_layer(void *h, uint32_t layer, const dl::LayerPtrs *p);
 int dl_engine_set_globals(void *h, const dl::GlobalPtrs *p);
+uint64_t dl_engine_arena_bytes(void *h);   // size of the symmetric peer-memory arena, after dl_engine_set_globals
 int dl_engine_set_comm(void *h, const dl::CommPtrs *p);
 int dl_engine_enable_mega(void *h, int enable);
 int dl_engine_set_vocab_limit(void *h, uint32_t limit);   // greedy arg-max never returns ids >= limit (tokenizer vocabulary size)
@@ -112,7 +92,6 @@ int dl_engine_choices_forward(void *h, int nb, uint32_t P, uint32_t C, uint32_t 
 // KV-cache slots (csrc/cuda/attn_decode.cu): n <= 8 independent sequences, slot s = rows [0, floor(seqLen / n)) of its own cache block
 int dl_engine_set_slots(void *h, uint32_t n);
 uint32_t dl_engine_slot_len(void *h);
-int dl_engine_slot_prefill(void *h, uint32_t slot, uint32_t T, uint32_t p0, cudaStream_t stream);   // T tokens staged in pTokens/pPos
 int dl_engine_slot_copy(void *h, uint32_t src, uint32_t dst, uint32_t P, cudaStream_t stream);
 int dl_engine_slot_sampling(void *h, uint32_t slot, unsigned long long seed, float temperature, float topp, float presence, float frequency,
                             const int32_t *ids, const float *vals, int nBias, cudaStream_t stream);
@@ -135,9 +114,12 @@ int dl_engine_set_trace_all(void *h, int allCtas);
 uint32_t dl_engine_num_sms(void *h);
 int dl_engine_forward(void *h, int nb, int logitsMode, int greedyAdvance, cudaStream_t stream);
 int dl_engine_forward_part(void *h, int nb, uint32_t layer, int part, float *ybuf, cudaStream_t stream);
-int dl_engine_prefill(void *h, uint32_t T, uint32_t p0, int wantLogits, cudaStream_t stream);   // T tokens staged in pTokens/pPos at positions p0 .. p0 + T - 1
-int dl_engine_capture_decode(void *h);
-int dl_engine_decode_graph(void *h, int nSteps, cudaStream_t stream);
+// n prompt tokens (host memory) at positions p0 .. p0 + n - 1; slot >= 0: into KV-cache slot `slot`
+int dl_engine_prefill(void *h, const int32_t *hostTokens, uint32_t n, uint32_t p0, int slot, int wantLogits, cudaStream_t stream);
+int dl_engine_set_prefill_min_tc(void *h, uint32_t n);   // shortest chunk on the tensor cores (default 9; 0: never)
+int dl_engine_decode_graph(void *h, int nSteps, cudaStream_t stream);   // captures the greedy step on first use
+int dl_engine_graph_captured(void *h);
+void dl_abi_struct_sizes(uint32_t out[4]);   // sizeof EngineConfig, LayerPtrs, GlobalPtrs, CommPtrs
 // symmetric peer-memory arena (csrc/cuda/comm_vmm.cu): create (local, binds the bootstrap socket) -> [job-wide barrier] -> connect
 // (collective: exchanges file descriptors, maps every peer, sets up the NVSwitch multicast mapping)
 void *dl_vmm_create(uint32_t rank, uint32_t nRanks, size_t bytes, const char *tag, int wantMulticast);

@@ -19,7 +19,7 @@ class EngineConfig(C.Structure):
     _fields_ = [(n, u32) for n in ("dim", "nLayers", "nHeads", "nKvHeads", "headDim", "ffDim", "vocab", "seqLen",
                                    "nExperts", "nActiveExperts", "maxBatch", "nSplits", "rank", "nRanks", "numSms")] + \
                [("eps", f32), ("usePdl", u32), ("moeFirstExpert", u32), ("moeNumLocal", u32), ("wType", u32), ("hiddenAct", u32),
-                                             ("kvType", u32)]
+                                             ("kvType", u32), ("maxPrefill", u32)]
 
 
 class LayerPtrs(C.Structure):
@@ -29,18 +29,11 @@ class LayerPtrs(C.Structure):
 
 class GlobalPtrs(C.Structure):
     _fields_ = [("embedding", vp), ("embeddingPeers", vp * 8), ("embRowsPerRank", u32), ("finalNorm", vp), ("wclsQs", vp), ("wclsSc", vp), ("rope", vp), ("vocabFull", u32),
-                ("tokens", vp), ("pos", vp), ("x", vp), ("qkv", vp), ("z", vp), ("h", vp), ("logits", vp),
-                ("attnPartial", vp), ("attnCounters", vp), ("history", vp), ("expertIdx", vp), ("expertWeight", vp),
-                ("routerLogits", vp), ("routerCounter", vp), ("moeScratch", vp), ("moeCounters", vp),
-                ("maxPrefill", u32), ("pTokens", vp), ("pPos", vp), ("px", vp), ("pqkv", vp), ("pxn", vp), ("pzb", vp), ("phb", vp),
-                ("pAttnPartial", vp), ("pAttnCounters", vp),
-                ("argVal", vp), ("argIdx", vp), ("argCounter", vp)]
+                ("tokens", vp), ("pos", vp), ("x", vp), ("logits", vp), ("history", vp)]
 
 
 class CommPtrs(C.Structure):
-    _fields_ = [("nRanks", u32), ("rank", u32), ("maxCtas", u32), ("slotStride", u32), ("arena", vp * 8), ("mcArena", vp),
-                ("slotsOff", u64), ("flagsOff", u64), ("candValOff", u64),
-                ("gatherOff", u64), ("prefillSlotsOff", u64), ("prefillSlotStride", u32)]
+    _fields_ = [("nRanks", u32), ("rank", u32), ("arena", vp * 8), ("mcArena", vp)]
 
 
 def lib() -> C.CDLL:
@@ -49,6 +42,10 @@ def lib() -> C.CDLL:
         return _lib
     path = _build.build_cuda()
     L = C.CDLL(str(path))
+    sizes = (C.c_uint32 * 4)()
+    L.dl_abi_struct_sizes(sizes)
+    if [C.sizeof(s) for s in (EngineConfig, LayerPtrs, GlobalPtrs, CommPtrs)] != list(sizes):
+        raise RuntimeError(f"{path}: sizes {list(sizes)} of EngineConfig, LayerPtrs, GlobalPtrs, CommPtrs differ from their ctypes mirrors")
     L.dl_repack_q40.argtypes = [vp, u64, u64, u32, u32, vp, vp, u32, u32, u32, vp]
     L.dl_repack_q40.restype = i32
     L.dl_dequant_device_q40.argtypes = [vp, vp, u32, u32, vp, vp]
@@ -103,6 +100,8 @@ def lib() -> C.CDLL:
     L.dl_engine_enable_mega.restype = i32
     L.dl_engine_set_vocab_limit.argtypes = [vp, u32]
     L.dl_engine_set_vocab_limit.restype = i32
+    L.dl_engine_arena_bytes.argtypes = [vp]
+    L.dl_engine_arena_bytes.restype = u64
     L.dl_engine_set_comm.argtypes = [vp, C.POINTER(CommPtrs)]
     L.dl_engine_set_comm.restype = i32
     for name, args in (("dl_comm_alloc", [C.c_size_t, C.POINTER(vp)]), ("dl_comm_free", [vp]), ("dl_comm_ipc_handle", [vp, vp]),
@@ -166,8 +165,6 @@ def lib() -> C.CDLL:
     L.dl_engine_set_slots.restype = i32
     L.dl_engine_slot_len.argtypes = [vp]
     L.dl_engine_slot_len.restype = u32
-    L.dl_engine_slot_prefill.argtypes = [vp, u32, u32, u32, vp]
-    L.dl_engine_slot_prefill.restype = i32
     L.dl_engine_slot_copy.argtypes = [vp, u32, u32, u32, vp]
     L.dl_engine_slot_copy.restype = i32
     L.dl_engine_slot_sampling.argtypes = [vp, u32, C.c_uint64, f32, f32, f32, f32, ip, C.POINTER(f32), i32, vp]
@@ -202,12 +199,14 @@ def lib() -> C.CDLL:
     L.dl_engine_forward.restype = i32
     L.dl_engine_forward_part.argtypes = [vp, i32, u32, i32, vp, vp]
     L.dl_engine_forward_part.restype = i32
-    L.dl_engine_prefill.argtypes = [vp, u32, u32, i32, vp]
+    L.dl_engine_prefill.argtypes = [vp, ip, u32, u32, i32, i32, vp]
     L.dl_engine_prefill.restype = i32
-    L.dl_engine_capture_decode.argtypes = [vp]
-    L.dl_engine_capture_decode.restype = i32
+    L.dl_engine_set_prefill_min_tc.argtypes = [vp, u32]
+    L.dl_engine_set_prefill_min_tc.restype = i32
     L.dl_engine_decode_graph.argtypes = [vp, i32, vp]
     L.dl_engine_decode_graph.restype = i32
+    L.dl_engine_graph_captured.argtypes = [vp]
+    L.dl_engine_graph_captured.restype = i32
     _lib = L
     return L
 

@@ -1,6 +1,6 @@
 """Python handle of the native per-rank engine (csrc/cuda/engine.cu).
 
-Owns the device tensors (weights, KV cache, activation buffers), hands their pointers to the C++ engine and exposes
+Owns the device tensors (weights, KV cache, the activation buffers it reads), hands their pointers to the C++ engine and exposes
 the three calls the apps need: `prefill(tokens, pos)`, `step(token, pos)` -> logits, and the device-resident greedy
 decode loop `decode_greedy(n)` that replays the captured CUDA graph.
 Plays the role of the reference's RootLlmInference (src/app.cpp:168-208): setBatchSize/setPosition/setToken/forward.
@@ -80,16 +80,7 @@ class Engine:
         self.tokens = torch.zeros(max_batch, dtype=torch.int32, device=dev)
         self.pos = torch.zeros(max_batch, dtype=torch.int32, device=dev)
         self.x = torch.zeros(max_batch, h.dim, **f32)
-        self.qkv = torch.zeros(max_batch, self.qkv_dim, **f32)
-        self.z = torch.zeros(max_batch, q_dim, **f32)
-        self.h = torch.zeros(max(max_batch, h.n_active_experts, 1), w.ff_dim, **f32)
-        self.router_logits = torch.zeros(max_batch * max(1, h.n_experts), **f32)
-        self.router_counter = torch.zeros(max_batch, dtype=torch.int32, device=dev)
-        self.moe_scratch = torch.zeros(max(1, h.n_active_experts) * h.dim, **f32)
-        self.moe_counters = torch.zeros(256, dtype=torch.int32, device=dev)
         self.logits = torch.zeros(max_batch, w.vocab, **f32)
-        self.attn_partial = torch.zeros(max_batch * w.n_heads * n_splits * (hd + 2), **f32)
-        self.attn_counters = torch.zeros(max_batch * w.n_heads, dtype=torch.int32, device=dev)
         self.history = torch.zeros(self.seq_len + 1, dtype=torch.int32, device=dev)
         if kv_cache_float_type == "q80":
             # int8 values [nKvHeads][seqLen][hd] and f16 scales [nKvHeads][seqLen][hd / 32] (+ 8 halves of tail padding: the
@@ -103,22 +94,6 @@ class Engine:
             self.k_scale = self.v_scale = [None] * h.n_layers
         self.k_cache = [torch.zeros(*kv_shape, dtype=kv_dtype, device=dev) for _ in range(h.n_layers)]
         self.v_cache = [torch.zeros(*kv_shape, dtype=kv_dtype, device=dev) for _ in range(h.n_layers)]
-        self.expert_idx = torch.zeros(max_batch * max(1, h.n_active_experts), dtype=torch.int32, device=dev)
-        self.expert_weight = torch.zeros(max_batch * max(1, h.n_active_experts), **f32)
-        self.max_prefill = mp = min(max_prefill, 256)
-        bf16 = dict(dtype=torch.bfloat16, device=dev)
-        self.p_tokens = torch.zeros(mp, dtype=torch.int32, device=dev)
-        self.p_pos = torch.zeros(mp, dtype=torch.int32, device=dev)
-        self.p_x = torch.zeros(mp, h.dim, **f32)
-        self.p_qkv = torch.zeros(mp, max(self.qkv_dim, h.dim), **f32)   # also the [T][dim] partial of the TP WO / W2 GEMMs
-        self.p_xn = torch.zeros(mp, h.dim, **bf16)
-        self.p_zb = torch.zeros(mp, q_dim, **bf16)
-        self.p_hb = torch.zeros(mp, w.ff_dim, **bf16)
-        self.p_attn_partial = torch.zeros(mp * w.n_heads * (hd + 2), **f32)
-        self.p_attn_counters = torch.zeros(mp * w.n_heads, dtype=torch.int32, device=dev)
-        self.arg_val = torch.zeros(256, **f32)
-        self.arg_idx = torch.zeros(256, dtype=torch.int32, device=dev)
-        self.arg_counter = torch.zeros(4, dtype=torch.int32, device=dev)
 
         cfg = cl.EngineConfig(dim=h.dim, nLayers=h.n_layers, nHeads=w.n_heads, nKvHeads=w.n_kv_heads, headDim=hd,
                               ffDim=w.ff_dim, vocab=w.vocab, seqLen=self.seq_len, nExperts=h.n_experts,
@@ -127,9 +102,11 @@ class Engine:
                               moeFirstExpert=w.first_expert, moeNumLocal=w.n_local_experts,
                               wType=getattr(w, "weight_kind", 0),
                               hiddenAct=1 if int(h.hidden_act) == 0 else 0,   # header: ACT_GELU = 0, ACT_SILU = 1
-                              kvType=cl.KV_CACHE_TYPES[kv_cache_float_type])
+                              kvType=cl.KV_CACHE_TYPES[kv_cache_float_type], maxPrefill=min(max_prefill, 256))
         self._lib = cl.lib()
         self._h = self._lib.dl_engine_create(C.byref(cfg))
+        if not self._h:
+            raise RuntimeError("dl_engine_create failed: unsupported configuration or out of device memory")
         for l, L in enumerate(w.layers):
             lp = cl.LayerPtrs(qkvQs=_p(L.qkv.qs), qkvSc=_p(L.qkv.scales), woQs=_p(L.wo.qs), woSc=_p(L.wo.scales),
                               w13Qs=_p(L.w13.qs), w13Sc=_p(L.w13.scales), w2Qs=_p(L.w2.qs), w2Sc=_p(L.w2.scales),
@@ -140,15 +117,7 @@ class Engine:
         emb_peers = (C.c_void_p * 8)(*([C.c_void_p(p) for p in (w.embedding_ptrs or [])] + [None] * (8 - len(w.embedding_ptrs or []))))
         gp = cl.GlobalPtrs(embedding=_p(w.embedding), embeddingPeers=emb_peers, embRowsPerRank=w.embedding_rows or 0, finalNorm=_p(w.final_norm), wclsQs=_p(w.wcls.qs),
                            wclsSc=_p(w.wcls.scales), rope=_p(w.rope), vocabFull=h.vocab_size, tokens=_p(self.tokens),
-                           pos=_p(self.pos), x=_p(self.x), qkv=_p(self.qkv), z=_p(self.z), h=_p(self.h),
-                           logits=_p(self.logits), attnPartial=_p(self.attn_partial), attnCounters=_p(self.attn_counters),
-                           history=_p(self.history), expertIdx=_p(self.expert_idx), expertWeight=_p(self.expert_weight),
-                           routerLogits=_p(self.router_logits), routerCounter=_p(self.router_counter),
-                           moeScratch=_p(self.moe_scratch), moeCounters=_p(self.moe_counters),
-                           maxPrefill=mp, pTokens=_p(self.p_tokens), pPos=_p(self.p_pos), px=_p(self.p_x), pqkv=_p(self.p_qkv),
-                           pxn=_p(self.p_xn), pzb=_p(self.p_zb), phb=_p(self.p_hb), pAttnPartial=_p(self.p_attn_partial),
-                           pAttnCounters=_p(self.p_attn_counters),
-                           argVal=_p(self.arg_val), argIdx=_p(self.arg_idx), argCounter=_p(self.arg_counter))
+                           pos=_p(self.pos), x=_p(self.x), logits=_p(self.logits), history=_p(self.history))
         cl.check(self._lib.dl_engine_set_globals(self._h, C.byref(gp)), "engine_set_globals")
         self.comm = comm
         tp = comm is not None and comm.world_size > 1
@@ -159,18 +128,15 @@ class Engine:
                    or not getattr(comm, "single_node", True)):
             self.collectives = "nccl"
         if tp and self.collectives == "fused":
-            from ..parallel.comm import arena_layout
-            comm.alloc_arena(arena_layout(comm.world_size, max_batch, h.dim, h.vocab_size, self.max_prefill))
-            cp = comm.comm_ptrs(max_batch * h.dim)
+            comm.alloc_arena(self._lib.dl_engine_arena_bytes(self._h))
+            cp = comm.comm_ptrs()
             cl.check(self._lib.dl_engine_set_comm(self._h, C.byref(cp)), "engine_set_comm")
         self._parts = tp and self.collectives == "nccl"
         self._ybuf = torch.zeros(max_batch, h.dim, **f32)
-        self.use_tc_prefill = not self.dense and not self._parts
+        self._tc_min = 9
         self.mega = False
         if h.n_experts == 0 and not self.dense and not self._parts and os.environ.get("DL_NO_MEGA") is None:
             self.enable_mega(True)     # persistent decode kernel by default; the engine falls back per call if a shape is unsupported
-        self.tc_min_tokens = 9          # shorter chunks stay on the GEMV path
-        self._graph_ready = False
         self.slots, self.slot_len = 1, self.seq_len
         self._stage_tok = torch.zeros(max_batch, dtype=torch.int32).pin_memory()
         self._stage_pos = torch.zeros(max_batch, dtype=torch.int32).pin_memory()
@@ -187,7 +153,6 @@ class Engine:
         """Greedy arg-max on the device never returns ids >= limit (the tokenizer's vocabulary size: embeddings may be padded
         beyond it, reference src/app.cpp:243-246 builds its sampler on the tokenizer size too)."""
         cl.check(self._lib.dl_engine_set_vocab_limit(self._h, int(limit)), "engine_set_vocab_limit")
-        self._graph_ready = False
 
     # -- device-side sampling --
     def seed_sampler(self, seed: int):
@@ -302,13 +267,7 @@ class Engine:
         tokens = list(tokens)
         if start_pos + len(tokens) > self.slot_len:
             raise ValueError("position beyond the slot length")
-        i = 0
-        while i < len(tokens):
-            n = min(len(tokens) - i, self.max_prefill)
-            self.p_tokens[:n].copy_(torch.tensor(tokens[i:i + n], dtype=torch.int32))
-            self.p_pos[:n].copy_(torch.arange(start_pos + i, start_pos + i + n, dtype=torch.int32))
-            cl.check(self._lib.dl_engine_slot_prefill(self._h, int(slot), n, start_pos + i, cl.stream_ptr()), "engine_slot_prefill")
-            i += n
+        self._prefill(tokens, start_pos, int(slot), False)
 
     def slot_copy(self, src: int, dst: int, P: int) -> None:
         """Copies rows [0, P) of slot src into slot dst (every layer and KV head)."""
@@ -455,15 +414,14 @@ class Engine:
             raise RuntimeError("device-side wait timed out: a tensor-parallel peer stopped responding (or the persistent kernel was not co-resident)")
 
     def enable_mega(self, enable: bool = True):
-        """Single-token forwards through the persistent per-token kernel (dense models). Re-captures the decode graph."""
+        """Single-token forwards through the persistent per-token kernel (dense models). The engine re-captures the decode graph."""
         cl.check(self._lib.dl_engine_enable_mega(self._h, 1 if enable else 0), "engine_enable_mega")
         self.mega = enable
-        self._graph_ready = False
 
     # -- tracing --
     def enable_trace(self, cap_launches: int = 1024, all_ctas: bool = False):
         """Device-side timeline: every kernel stamps globaltimer at entry / dependency resolved / prologue done / exit.
-        Must be enabled before the decode graph is captured. `all_ctas`: every CTA of the persistent kernel records its own
+        The engine re-captures the decode graph with it. `all_ctas`: every CTA of the persistent kernel records its own
         phase stamps (row c of `trace_buf.view(num_sms, -1)`), for barrier-skew analysis."""
         if all_ctas:
             cap_launches = max(cap_launches, self.num_sms * 256)
@@ -471,7 +429,6 @@ class Engine:
         cl.check(self._lib.dl_engine_set_trace(self._h, self.trace_buf.data_ptr(), cap_launches), "engine_set_trace")
         cl.check(self._lib.dl_engine_set_trace_all(self._h, 1 if all_ctas else 0), "engine_set_trace_all")
         self.trace_stride = (cap_launches * 4) // self.num_sms if all_ctas else 0
-        self._graph_ready = False
 
     def read_trace(self):
         t = self.trace_buf.cpu().numpy()
@@ -499,36 +456,43 @@ class Engine:
         else:
             cl.check(self._lib.dl_engine_forward(self._h, n, logits_mode, 1 if greedy_advance else 0, cl.stream_ptr()), "engine_forward")
 
+    @property
+    def tc_min_tokens(self) -> int:
+        """Shortest prompt chunk the engine runs on the tensor-core GEMM path (default 9; 0: none). Shorter chunks run as GEMV batches."""
+        return self._tc_min
+
+    @tc_min_tokens.setter
+    def tc_min_tokens(self, n: int) -> None:
+        cl.check(self._lib.dl_engine_set_prefill_min_tc(self._h, int(n)), "engine_set_prefill_min_tc")
+        self._tc_min = int(n)
+
+    use_tc_prefill = property(lambda self: self._tc_min != 0, lambda self, on: setattr(self, "tc_min_tokens", 9 if on else 0))
+
     def prefill(self, tokens: Sequence[int], start_pos: int = 0, want_logits: bool = True) -> Optional[torch.Tensor]:
-        """Feeds a prompt; returns the logits row of its last token (device tensor). Single GPU: chunks of up to 256 tokens
-        on the tensor-core GEMM path. Tensor parallel: chunks of up to max_batch tokens on the GEMV path (fused all-reduce)."""
+        """Feeds a prompt; returns the logits row of its last token (device tensor). The engine chunks it (dl_engine_prefill):
+        up to max_prefill tokens a chunk on the tensor-core GEMM path, power-of-two GEMV batches otherwise. Library-collective
+        tensor parallelism: GEMV batches of up to max_batch tokens with NCCL all-reduces."""
         tokens = list(tokens)
         if start_pos + len(tokens) > self.seq_len:
             raise ValueError("position beyond the context length")
-        hdr = self.w.header
-        tp = self.comm is not None and self.comm.world_size > 1
-        # tensor parallel: the fused GEMM + all-reduce kernel needs 256-wide K slices on every rank
-        tp_ok = (not tp) or ((self.w.n_heads * hdr.head_dim) % 256 == 0 and self.w.ff_dim % 256 == 0 and hdr.dim % 256 == 0)
-        # mixture of experts: the grouped tensor-core GEMMs need 256-wide K on both expert matrices
-        moe_ok = hdr.n_experts == 0 or (hdr.dim % 256 == 0 and self.w.ff_dim % 256 == 0 and os.environ.get("DL_NO_MOE_PREFILL") is None)
-        tc_path = tp_ok and moe_ok and self.use_tc_prefill
+        if not self._parts:
+            self._prefill(tokens, start_pos, -1, want_logits)
+            return self._full_logits(self.logits[0]) if want_logits else None
         i = 0
         while i < len(tokens):
             rem = len(tokens) - i
-            if tc_path and rem >= self.tc_min_tokens:
-                n = min(rem, self.max_prefill)
-                last = i + n == len(tokens)
-                self.p_tokens[:n].copy_(torch.tensor(tokens[i:i + n], dtype=torch.int32))
-                self.p_pos[:n].copy_(torch.arange(start_pos + i, start_pos + i + n, dtype=torch.int32))
-                cl.check(self._lib.dl_engine_prefill(self._h, n, start_pos + i, 1 if (last and want_logits) else 0, cl.stream_ptr()), "engine_prefill")
-            else:
-                n = 1
-                while n * 2 <= min(rem, self.max_batch):
-                    n *= 2
-                last = i + n == len(tokens)
-                self.forward_batch(tokens[i:i + n], start_pos + i, logits_mode=1 if (last and want_logits) else 0)
+            n = 1
+            while n * 2 <= min(rem, self.max_batch):
+                n *= 2
+            last = i + n == len(tokens)
+            self.forward_batch(tokens[i:i + n], start_pos + i, logits_mode=1 if (last and want_logits) else 0)
             i += n
         return self._full_logits(self.logits[0]) if want_logits else None
+
+    def _prefill(self, tokens: List[int], start_pos: int, slot: int, want_logits: bool) -> None:
+        arr = (C.c_int32 * len(tokens))(*tokens)
+        cl.check(self._lib.dl_engine_prefill(self._h, arr, len(tokens), start_pos, slot, 1 if want_logits else 0, cl.stream_ptr()),
+                 "engine_prefill")
 
     def step(self, token: int, pos: int) -> torch.Tensor:
         """Forward of one token; returns the full-vocabulary logits row (gathered over ranks under tensor parallelism)."""
@@ -580,12 +544,6 @@ class Engine:
             self._forward_parts(1, 1, True)
             return
         if use_graph:
-            if not self._graph_ready:
-                saved = (self.tokens.clone(), self.pos.clone())
-                cl.check(self._lib.dl_engine_forward(self._h, 1, 1, 0, cl.stream_ptr()), "engine_forward")
-                torch.cuda.current_stream().synchronize()
-                self.capture_decode()
-                self.tokens.copy_(saved[0]); self.pos.copy_(saved[1])
             cl.check(self._lib.dl_engine_decode_graph(self._h, 1, cl.stream_ptr()), "engine_decode_graph")
         else:
             cl.check(self._lib.dl_engine_forward(self._h, 1, 1, 1, cl.stream_ptr()), "engine_forward")
@@ -600,9 +558,10 @@ class Engine:
             return self.w.header.n_layers * 6 + 2
         return self.w.header.n_layers * 5 + 2   # embedding + 5 fused kernels per layer + logits/arg-max
 
-    def capture_decode(self):
-        cl.check(self._lib.dl_engine_capture_decode(self._h), "engine_capture_decode")
-        self._graph_ready = True
+    @property
+    def graph_captured(self) -> bool:
+        """True while the engine holds a decode graph of its current configuration (captured on the first graph step)."""
+        return bool(self._lib.dl_engine_graph_captured(self._h))
 
     def decode_greedy(self, first_token: int, start_pos: int, n_steps: int, use_graph: bool = True) -> List[int]:
         """Generates n_steps tokens greedily: step i consumes the token at position start_pos+i and emits the next.
@@ -614,11 +573,6 @@ class Engine:
             for _ in range(n_steps):
                 self._forward_parts(1, 1, True)
         elif use_graph:
-            if not self._graph_ready:
-                # warm-up run configures kernel attributes outside of capture
-                cl.check(self._lib.dl_engine_forward(self._h, 1, 1, 0, cl.stream_ptr()), "engine_forward")
-                torch.cuda.current_stream().synchronize()
-                self.capture_decode()
             cl.check(self._lib.dl_engine_decode_graph(self._h, n_steps, cl.stream_ptr()), "engine_decode_graph")
         else:
             for _ in range(n_steps):

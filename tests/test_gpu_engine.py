@@ -58,6 +58,28 @@ def test_graph_decode_equals_eager(tmp_models):
     assert a[:4] == ref[:4]
 
 
+@pytest.mark.parametrize("change", ["mega_off", "trace_on"])
+def test_graph_follows_abi_changes(tmp_models, change):
+    """Switching the persistent kernel off or tracing on through the C ABI, past the Python wrapper, drops the captured decode
+    graph: the next graph step runs the new configuration and decodes what the eager path decodes."""
+    from distributed_llama_b200.ops import cuda_lib as cl
+    prompt, P, n = [3, 17, 250, 9], 3, 8
+    trace = torch.zeros(1024, 4, dtype=torch.int64, device="cuda")
+    toks = {}
+    for use_graph in (True, False):
+        e = _setup(tmp_models, "tiny-llama31")[1]
+        e.prefill(prompt[:-1], 0, want_logits=False)
+        first = e.decode_greedy(prompt[-1], P, n, use_graph=use_graph)
+        assert e.mega_active
+        lib = cl.lib()
+        rc = lib.dl_engine_enable_mega(e._h, 0) if change == "mega_off" else lib.dl_engine_set_trace(e._h, trace.data_ptr(), 1024)
+        assert rc == 0
+        toks[use_graph] = first + e.decode_greedy(first[-1], P + n, n, use_graph=use_graph)   # ends with a device-to-host copy
+        if use_graph:
+            assert not e.mega_active if change == "mega_off" else (trace[:, 0] != 0).any()
+    assert toks[True] == toks[False]
+
+
 @pytest.mark.parametrize("name", ["tiny-llama31", "tiny-qwen3", "tiny-qwen3-moe"])
 def test_tensor_core_prefill_matches_oracle(tmp_models, name):
     """Prompt chunks > 8 tokens run on the tensor-core GEMM path (bf16 activations); later decode steps read its KV cache."""

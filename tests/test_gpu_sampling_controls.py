@@ -198,7 +198,7 @@ def test_zero_controls_keep_the_fused_greedy_path(tmp_models):
     for _ in range(12):
         tok = sess.next_token(tok)
         got.append(tok)
-    assert sess.engine._graph_ready and sess._dev_controls is None
+    assert sess.engine.graph_captured and sess._dev_controls is None
     ref = _session(tmp_models, "tiny-llama31", 0.0)
     ref.prefill(PROMPT[:-1])
     assert got == ref.engine.decode_greedy(PROMPT[-1], len(PROMPT) - 1, 12)

@@ -252,7 +252,7 @@ def test_greedy_with_filters_keeps_the_persistent_kernel(tmp_models):
         tok = s.next_token(tok)
         got.append(tok)
         assert s.engine.mega_active
-    assert s.engine._graph_ready and s._dev_filters == (0, 0.0)   # greedy never hands the filters to the device
+    assert s.engine.graph_captured and s._dev_filters == (0, 0.0)   # greedy never hands the filters to the device
     assert got == _greedy(tmp_models, "tiny-llama31", steps)
 
 

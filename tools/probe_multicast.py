@@ -12,7 +12,7 @@ import torch
 import torch.distributed as dist
 
 from distributed_llama_b200.ops import cuda_lib as cl
-from distributed_llama_b200.parallel.comm import ArenaLayout, Communicator
+from distributed_llama_b200.parallel.comm import Communicator
 
 rank, local = int(os.environ["RANK"]), int(os.environ["LOCAL_RANK"])
 torch.cuda.set_device(local)
@@ -21,7 +21,7 @@ comm = Communicator()
 n = 4096
 W = comm.world_size
 total = (4 + W) * n * 4 + 4096
-comm.alloc_arena(ArenaLayout(0, 0, 0, 0, 0, 0, 0, 0, total))
+comm.alloc_arena(total)
 lib = cl.lib()
 print(f"PROBE rank {rank}: arena kind={comm.arena_kind} mc_ptr={'0x%x' % comm.mc_ptr if comm.mc_ptr else 0} "
       f"uc={[hex(p) for p in comm.arena_ptrs]}", flush=True)
