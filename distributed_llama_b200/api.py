@@ -21,6 +21,8 @@ import torch
 
 from . import host
 from .formats.model_file import ModelFile
+from .parallel.control import (OP_CHOICES_FIRST, OP_CHOICES_SEED, OP_CHOICES_STEP, OP_CONTROLS, OP_DECODE_N, OP_FILTERS, OP_PREFILL,
+                               OP_SEED, OP_STEP_GREEDY, OP_STEP_LOGITS, OP_STEP_SAMPLE, _active_mask, _f32_bits, _split_seed)
 
 
 @dataclass
@@ -61,8 +63,8 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     backend's choice_controls hands them to the batched path). `backend` provides
     next_token(token, pos, sampler), forget_device_seed(), save_sampler() / restore_sampler(saved), and for the batched path
     batched_choices(n), seed_choices(seeds), choice_controls(sampler, n), choices_first(token, P, n, T, topp) and
-    choices_step(tokens, P, C, j, active, T, topp) (InferenceSession and apps.runtime.RootInference). Returns each choice's
-    tokens.
+    choices_step(tokens, P, C, j, active, T, topp) (TokenSteps: InferenceSession and apps.runtime.RootInference). Returns each
+    choice's tokens.
 
     logprobs = k (0..20): on_logprobs(i, entry) is called right before on_token(i, tok) with the entry of that token,
     (tok, logprob, [(id, logprob), ...] k most likely); the backend's next_token, choices_first and choices_step then take a
@@ -135,6 +137,183 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
         last = backend.choices_step(last, P, C, j, active, T, topp, **lp)
         j += 1
     return out
+
+
+def _lp_kw(logprobs: Optional[int]) -> dict:
+    """The engine's `logprobs` keyword, passed only when log-probabilities are asked for."""
+    return {} if logprobs is None else {"logprobs": logprobs}
+
+
+class TokenSteps:
+    """The token steps of one engine, the backend run_choices needs: InferenceSession for the library and
+    apps.runtime.RootInference for the CLIs and API server, which announces every engine call to the workers (_send).
+
+    Greedy draws without sampling controls run on the fused arg-max. Other draws run on the device sampler
+    (csrc/cuda/sampler.cu: the logits never leave the GPUs), unless the engine is not on a GPU, its collectives are the
+    library's (multi-node) or DL_HOST_SAMPLER is set: then the host sampler draws from logits copied back. The device's
+    generator, controls and filters are handed over when the sampler's differ from what the device holds."""
+
+    def __init__(self, engine, device, n_ranks: int):
+        self.engine = engine
+        self.device = torch.device(device)
+        self.n_ranks = n_ranks
+        # the caller synchronises every step, so one pinned staging slot is enough (workers enqueue ahead: pageable staging)
+        on_gpu = self.device.type == "cuda"
+        self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory() if on_gpu else None
+        self._pin_out = torch.zeros(1, dtype=torch.int32).pin_memory() if on_gpu else None
+        self._dev_seeded = None          # (seed, seed generation) of the sampler the device generator follows (None: none)
+        self._dev_controls = None        # completion generation whose controls the device holds (None: off)
+        self._dev_filters = (0, 0.0)     # (top_k, min_p) the device holds
+        self._last_logprobs = None
+
+    def _send(self, op: int, pos: int, words: Sequence[int]) -> None:
+        """Announces an engine call every worker must repeat (parallel.control packets); no workers here."""
+
+    @property
+    def device_sampling(self) -> bool:
+        return self._pin_in is not None and not getattr(self.engine, "_parts", False) and os.environ.get("DL_HOST_SAMPLER") is None
+
+    def prefill(self, tokens: Sequence[int], pos: int) -> None:
+        """Evaluates tokens at positions pos..pos+n-1 without producing logits (prompt minus its last token)."""
+        if tokens:
+            self._send(OP_PREFILL, pos, tokens)
+            self.engine.prefill(tokens, pos, want_logits=False)
+
+    def forward_logits(self, token: int, pos: int) -> torch.Tensor:
+        self._send(OP_STEP_LOGITS, pos, [token])
+        return self.engine.step(token, pos)
+
+    def decode_greedy(self, token: int, pos: int, n_steps: int) -> List[int]:
+        """n greedy steps with the token fed back on the device (no host round trip per step): one control packet for all."""
+        self._send(OP_DECODE_N, pos, [token, n_steps])
+        return self.engine.decode_greedy(token, pos, n_steps)
+
+    def forward_greedy(self, token: int, pos: int, logprobs: Optional[int] = None) -> int:
+        """One step on the fused arg-max: H2D (token, pos) from pinned memory, forward, D2H of the token."""
+        self._send(OP_STEP_GREEDY, pos, [token])
+        eng = self.engine
+        if self._pin_in is None:          # engine on the CPU (protocol tests)
+            eng._set_inputs([token], pos)
+            eng.run_decode_step()
+            return int(eng.tokens[0])
+        self._pin_in[0], self._pin_in[1] = token, pos
+        eng.tokens[:1].copy_(self._pin_in[:1], non_blocking=True)
+        eng.pos[:1].copy_(self._pin_in[1:2], non_blocking=True)
+        eng.run_decode_step()
+        return self._read_token(logprobs, controlled=False)
+
+    def _read_token(self, logprobs: Optional[int], controlled: bool) -> int:
+        """Enqueues the log-probabilities of the draw when asked, then copies the token back and waits for it."""
+        eng = self.engine
+        if logprobs is not None:
+            eng.logprobs([logprobs], controlled=controlled)
+        self._pin_out.copy_(eng.tokens[:1], non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        eng.check_abort()
+        if logprobs is not None:
+            self._last_logprobs = eng.read_logprobs()
+        return int(self._pin_out[0])
+
+    def next_token(self, token: int, pos: int, sampler, logprobs: Optional[int] = None) -> int:
+        """One generated token at `pos` with the sampler's settings. Greedy with sampling controls runs on the device sampler
+        (arg-max of the controlled logits), not on the fused arg-max. logprobs = k (0..20): also the log-probabilities of the
+        drawn token and the k most likely ones, from the same logits the draw saw (last_logprobs()); the token is the same as
+        without it."""
+        if logprobs is not None:
+            check_logprobs(logprobs, self.n_ranks)
+        if sampler.temperature == 0.0 and not sampler.controls_active:
+            return self.forward_greedy(token, pos, logprobs)
+        if not self.device_sampling:
+            t = int(sampler.sample(self.forward_logits(token, pos).float().cpu().numpy()))
+            if logprobs is not None:
+                self._last_logprobs = [self.engine.logprobs_host_draw(t, logprobs, sampler)]
+            return t
+        gen = (sampler.seed, sampler.seed_generation)
+        if sampler.temperature != 0.0 and self._dev_seeded != gen:
+            self.seed(sampler.seed)
+            self._dev_seeded = gen
+        key = sampler.completion_generation if sampler.controls_active else None
+        if self._dev_controls != key:   # a new completion: count row 0 starts from zero
+            self.set_controls(sampler, 1)
+            self._dev_controls = key
+        self.set_filters(sampler)
+        self._send(OP_STEP_SAMPLE, pos, [token] + _f32_bits(sampler.temperature, sampler.topp))
+        self.engine.step_sampled(token, pos, sampler.temperature, sampler.topp)
+        return self._read_token(logprobs, controlled=True)
+
+    def last_logprobs(self) -> list:
+        """Per row of the last step that was asked for logprobs (next_token: one row; choices_first / choices_step: one per
+        choice, None for inactive ones): (token id, logprob, [(id, logprob), ...] the k most likely in order of logprob desc,
+        id asc). logprob(i) = x[i] - logsumexp(x) over the tokenizer's vocabulary, x the logits after logit_bias and the
+        penalties (before temperature and top-p)."""
+        return self._last_logprobs
+
+    # ---- the device sampler's state, the same on every rank ----
+    def seed(self, seed: int) -> None:
+        """Seeds the single-sequence device generator."""
+        self._send(OP_SEED, 0, _split_seed(seed))
+        self.engine.seed_sampler(seed)
+
+    def set_controls(self, sampler, row_mask: int) -> None:
+        """The sampler's penalties and logit bias for the following draws; zeroes the count rows in row_mask."""
+        bias = sampler.logit_bias
+        words = _f32_bits(sampler.presence_penalty, sampler.frequency_penalty) + [row_mask]
+        for t, v in bias:
+            words += [t] + _f32_bits(v)
+        self._send(OP_CONTROLS, 0, words)
+        self.engine.set_sampling_controls(sampler.presence_penalty, sampler.frequency_penalty, bias, row_mask)
+
+    def set_filters(self, sampler) -> None:
+        """The sampler's top_k / min_p, before the first draw that uses them (under tensor parallelism each rank draws from
+        the gathered logits with its own generator, so all ranks must hold the same filters)."""
+        key = (sampler.top_k, sampler.min_p)
+        if self._dev_filters != key:
+            self._send(OP_FILTERS, 0, [key[0]] + _f32_bits(key[1]))
+            self.engine.set_sampling_filters(*key)
+            self._dev_filters = key
+
+    # ---- several completions of one prompt (run_choices) ----
+    def forget_device_seed(self):
+        self._dev_seeded = None
+
+    def save_sampler(self):
+        key = self._dev_seeded
+        return key, (self.engine.sampler_state() if key is not None and self.device_sampling else 0)
+
+    def restore_sampler(self, saved):
+        key, state = saved
+        if key is not None and self.device_sampling:
+            self.seed(state)
+        self._dev_seeded = key
+
+    def batched_choices(self, n: int) -> bool:
+        return self.device_sampling and self.engine.supports_choices(n)
+
+    def choice_controls(self, sampler, n: int) -> None:
+        """The sampler's controls and filters for the batched choices, count rows 1..n zeroed."""
+        self.set_filters(sampler)
+        if sampler.controls_active or self._dev_controls is not None:
+            self.set_controls(sampler, ((1 << n) - 1) << 1)
+            self._dev_controls = -1 if sampler.controls_active else None   # row 0's counts are not this sampler's
+
+    def seed_choices(self, seeds: Sequence[int]) -> None:
+        self._send(OP_CHOICES_SEED, 0, [w for s in seeds for w in _split_seed(s)])
+        self.engine.seed_choice_samplers(seeds)
+
+    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float, logprobs: Optional[int] = None) -> List[int]:
+        self._send(OP_CHOICES_FIRST, P, [token, n] + _f32_bits(temperature, topp))
+        out = self.engine.choices_first(token, P, n, temperature, topp, **_lp_kw(logprobs))
+        if logprobs is not None:
+            self._last_logprobs = self.engine.read_logprobs()
+        return out
+
+    def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
+                     topp: float, logprobs: Optional[int] = None) -> List[int]:
+        self._send(OP_CHOICES_STEP, P, [C, j, _active_mask(active)] + _f32_bits(temperature, topp) + list(tokens))
+        out = self.engine.choices_step(tokens, P, C, j, active, temperature, topp, **_lp_kw(logprobs))
+        if logprobs is not None:
+            self._last_logprobs = self.engine.read_logprobs()
+        return out
 
 
 class ParallelRefused(ValueError):
@@ -338,7 +517,7 @@ class SlotScheduler:
                             req.fail(e, job["slots"])
 
 
-class InferenceSession:
+class InferenceSession(TokenSteps):
     def __init__(self, model_path: str, tokenizer_path: Optional[str] = None, max_seq_len: int = 0,
                  temperature: float = 0.0, topp: float = 0.9, seed: int = 12345, device: Optional[str] = None,
                  max_batch: int = 8, use_pdl: bool = True, comm=None, moe_mode: str = "auto", presence_penalty: float = 0.0,
@@ -363,9 +542,9 @@ class InferenceSession:
         n_ranks = comm.world_size if comm is not None else 1
         if device is None:
             device = f"cuda:{torch.cuda.current_device()}"
-        self.device = torch.device(device)
-        self.weights = load_device_weights(self.model_file, rank, n_ranks, self.device, moe_mode=moe_mode, comm=comm)
-        self.engine = Engine(self.weights, max_batch=max_batch, use_pdl=use_pdl, comm=comm, kv_cache_float_type=kv_cache_float_type)
+        self.weights = load_device_weights(self.model_file, rank, n_ranks, torch.device(device), moe_mode=moe_mode, comm=comm)
+        super().__init__(Engine(self.weights, max_batch=max_batch, use_pdl=use_pdl, comm=comm, kv_cache_float_type=kv_cache_float_type),
+                         device, n_ranks)
         H = host()
         self.tokenizer = H.Tokenizer(tokenizer_path) if tokenizer_path else None
         vocab = self.tokenizer.vocab_size if self.tokenizer else self.header.vocab_size
@@ -375,11 +554,6 @@ class InferenceSession:
         if self.tokenizer and self.tokenizer.vocab_size < self.header.vocab_size:
             self.engine.set_vocab_limit(self.tokenizer.vocab_size)
         self.pos = 0
-        self._dev_seeded = None
-        self._dev_controls = None   # completion generation whose controls the device holds (None: off)
-        self._dev_filters = (0, 0.0)   # (top_k, min_p) the device holds
-        self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory()
-        self._pin_out = torch.zeros(1, dtype=torch.int32).pin_memory()
         self.slots = parallel
         if parallel > 1:
             self.engine.set_slots(parallel)
@@ -405,133 +579,27 @@ class InferenceSession:
     def slots_step_logprobs(self, tokens: Sequence[int], pos: Sequence[int], active: Sequence[bool]):
         return self.engine.slots_step_logprobs(tokens, pos, active)
 
-    # ---- token level ----
+    # ---- token level: the session's position by default, moved past what ran ----
     def reset(self):
         self.pos = 0
 
-    def prefill(self, tokens: Sequence[int]) -> None:
-        """Evaluates tokens at positions pos..pos+n-1 without producing logits (prompt minus its last token)."""
-        if tokens:
-            self.engine.prefill(tokens, self.pos, want_logits=False)
-            self.pos += len(tokens)
+    def prefill(self, tokens: Sequence[int], pos: Optional[int] = None) -> None:
+        pos = self.pos if pos is None else pos
+        super().prefill(tokens, pos)
+        self.pos = pos + len(tokens)
 
-    def forward_logits(self, token: int) -> torch.Tensor:
-        lg = self.engine.step(token, self.pos)
-        self.pos += 1
+    def forward_logits(self, token: int, pos: Optional[int] = None) -> torch.Tensor:
+        pos = self.pos if pos is None else pos
+        lg = super().forward_logits(token, pos)
+        self.pos = pos + 1
         return lg
 
     def next_token(self, token: int, pos: Optional[int] = None, sampler=None, logprobs: Optional[int] = None) -> int:
-        """One decode step with host-visible result: H2D (token,pos) from pinned memory, forward + sampling, D2H. `pos` and
-        `sampler` default to the session's own; run_choices passes its own, as it does to apps.runtime.RootInference.
-        logprobs = k (0..20): also computes the log-probabilities of the drawn token and the k most likely ones on the device,
-        from the same logits the draw saw (last_logprobs()); the token is the same as without it."""
-        if pos is not None:
-            self.pos = pos
-        smp = self.sampler if sampler is None else sampler
-        if logprobs is not None:
-            check_logprobs(logprobs, self.comm.world_size if self.comm is not None else 1)
-        if smp.temperature == 0.0 and not smp.controls_active:
-            self._pin_in[0] = token
-            self._pin_in[1] = self.pos
-            eng = self.engine
-            eng.tokens[:1].copy_(self._pin_in[:1], non_blocking=True)
-            eng.pos[:1].copy_(self._pin_in[1:2], non_blocking=True)
-            eng.run_decode_step()
-            if logprobs is not None:
-                eng.logprobs([logprobs])
-            self._pin_out.copy_(eng.tokens[:1], non_blocking=True)
-            torch.cuda.current_stream().synchronize()
-            eng.check_abort()
-            self.pos += 1
-            if logprobs is not None:
-                self._last_logprobs = eng.read_logprobs()
-            return int(self._pin_out[0])
-        eng = self.engine
-        if self.device.type == "cuda" and not getattr(eng, "_parts", False):
-            # temperature / top-p on the device (csrc/cuda/sampler.cu): only the sampled token crosses PCIe
-            gen = (smp.seed, smp.seed_generation)
-            if smp.temperature != 0.0 and self._dev_seeded != gen:
-                eng.seed_sampler(smp.seed)
-                self._dev_seeded = gen
-            self._sync_controls(smp)
-            self._sync_filters(smp)
-            eng.step_sampled(token, self.pos, smp.temperature, smp.topp)
-            if logprobs is not None:
-                eng.logprobs([logprobs], controlled=True)
-            self._pin_out.copy_(eng.tokens[:1], non_blocking=True)
-            torch.cuda.current_stream().synchronize()
-            eng.check_abort()
-            self.pos += 1
-            if logprobs is not None:
-                self._last_logprobs = eng.read_logprobs()
-            return int(self._pin_out[0])
-        lg = self.forward_logits(token)
-        t = int(smp.sample(lg.float().cpu().numpy()))
-        if logprobs is not None:
-            self._last_logprobs = [eng.logprobs_host_draw(t, logprobs, smp)]
-        return t
-
-    def last_logprobs(self) -> list:
-        """Per row of the last step that was asked for logprobs (next_token: one row; choices_first / choices_step: one per
-        choice, None for inactive ones): (token id, logprob, [(id, logprob), ...] the k most likely in order of logprob desc,
-        id asc). logprob(i) = x[i] - logsumexp(x) over the tokenizer's vocabulary, x the logits after logit_bias and the
-        penalties (before temperature and top-p)."""
-        return self._last_logprobs
-
-    def _sync_controls(self, smp):
-        """Hands the sampler's controls to the device at the start of each of its completions (count row 0 zeroed)."""
-        key = smp.completion_generation if smp.controls_active else None
-        if self._dev_controls != key:
-            self.engine.set_sampling_controls(smp.presence_penalty, smp.frequency_penalty, smp.logit_bias, 1)
-            self._dev_controls = key
-
-    def _sync_filters(self, smp):
-        """Hands the sampler's top_k / min_p to the device when they differ from what it holds."""
-        key = (smp.top_k, smp.min_p)
-        if self._dev_filters != key:
-            self.engine.set_sampling_filters(*key)
-            self._dev_filters = key
-
-    # ---- several completions of one prompt ----
-    def forget_device_seed(self):
-        self._dev_seeded = None
-
-    def choice_controls(self, sampler, n: int):
-        """The sampler's controls and filters for the batched choices, count rows 1..n zeroed."""
-        self._sync_filters(sampler)
-        if sampler.controls_active or self._dev_controls is not None:
-            self.engine.set_sampling_controls(sampler.presence_penalty, sampler.frequency_penalty, sampler.logit_bias,
-                                              ((1 << n) - 1) << 1)
-            self._dev_controls = -1 if sampler.controls_active else None   # row 0's counts are not this sampler's
-
-    def save_sampler(self):
-        key = self._dev_seeded
-        return key, (self.engine.sampler_state() if key is not None else 0)
-
-    def restore_sampler(self, saved):
-        key, state = saved
-        if key is not None:
-            self.engine.seed_sampler(state)
-        self._dev_seeded = key
-
-    def batched_choices(self, n: int) -> bool:
-        return self.device.type == "cuda" and self.engine.supports_choices(n) and os.environ.get("DL_HOST_SAMPLER") is None
-
-    def seed_choices(self, seeds: Sequence[int]):
-        self.engine.seed_choice_samplers(seeds)
-
-    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float, logprobs: Optional[int] = None) -> List[int]:
-        out = self.engine.choices_first(token, P, n, temperature, topp, logprobs=logprobs)
-        if logprobs is not None:
-            self._last_logprobs = self.engine.read_logprobs()
-        return out
-
-    def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
-                     topp: float, logprobs: Optional[int] = None) -> List[int]:
-        out = self.engine.choices_step(tokens, P, C, j, active, temperature, topp, logprobs=logprobs)
-        if logprobs is not None:
-            self._last_logprobs = self.engine.read_logprobs()
-        return out
+        """TokenSteps.next_token with the session's position and sampler by default; run_choices passes its own."""
+        pos = self.pos if pos is None else pos
+        tok = super().next_token(token, pos, self.sampler if sampler is None else sampler, logprobs)
+        self.pos = pos + 1
+        return tok
 
     def generate_choices(self, prompt: str, n: int, max_tokens: int, seed: Optional[int] = None) -> List[str]:
         """n completions of `prompt`, each at most max_tokens tokens (and at most its share of the remaining context, see

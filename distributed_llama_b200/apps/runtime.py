@@ -9,51 +9,18 @@ op 0 is the stop signal. All activation traffic happens inside the kernels over 
 from __future__ import annotations
 
 import os
-import sys
 from dataclasses import dataclass
-from typing import Callable, List, Optional, Sequence
+from typing import Callable, Sequence
 
-import numpy as np
 import torch
 
 from .. import host
-from ..api import InferenceSession, check_logprobs
+from ..api import InferenceSession, TokenSteps
+# the packet format; the op codes and word helpers also stay importable from this module (_f32_bits: encoding only)
+from ..parallel.control import (OP_CHOICES_FIRST, OP_CHOICES_SEED, OP_CHOICES_STEP, OP_CONTROLS, OP_DECODE_N, OP_FILTERS,  # noqa: F401
+                                OP_PREFILL, OP_SEED, OP_STEP_GREEDY, OP_STEP_LOGITS, OP_STEP_SAMPLE, OP_STOP, _active_list,
+                                _bits_f32, _f32_bits, _join_seed)
 from .args import AppArgs
-
-OP_STOP, OP_PREFILL, OP_STEP_LOGITS, OP_STEP_GREEDY, OP_DECODE_N, OP_STEP_SAMPLE, OP_SEED = 0, 1, 2, 3, 4, 5, 6
-OP_CHOICES_SEED, OP_CHOICES_FIRST, OP_CHOICES_STEP = 7, 8, 9
-OP_CONTROLS = 10   # [presence bits, frequency bits, count-row mask, (id, bias bits) ...]: Engine.set_sampling_controls
-OP_FILTERS = 11    # [top_k, min_p bits]: Engine.set_sampling_filters
-
-
-def _split_seed(seed: int) -> List[int]:
-    return [seed & 0x7FFFFFFF, (seed >> 31) & 0x7FFFFFFF, (seed >> 62) & 0x3]
-
-
-def _join_seed(w: Sequence[int]) -> int:
-    return w[0] | (w[1] << 31) | (w[2] << 62)
-
-
-def _active_mask(active: Sequence[bool]) -> int:
-    return sum(1 << i for i, a in enumerate(active) if a)
-
-
-def _active_list(mask: int, n: int) -> List[bool]:
-    return [bool((mask >> i) & 1) for i in range(n)]
-
-
-def _f32_bits(*xs: float) -> List[int]:
-    import struct
-    return list(struct.unpack(f"<{len(xs)}i", struct.pack(f"<{len(xs)}f", *xs)))
-
-
-def _bits_f32(*xs: int) -> List[float]:
-    import struct
-    return list(struct.unpack(f"<{len(xs)}f", struct.pack(f"<{len(xs)}i", *xs)))
-
-
-def _lp_kw(logprobs: Optional[int]) -> dict:
-    return {} if logprobs is None else {"logprobs": logprobs}
 
 
 def world():
@@ -99,181 +66,30 @@ def open_control_channel(comm):
     return chan
 
 
-class RootInference:
-    """Root-side handle (reference RootLlmInference, src/app.cpp:168-208): every call first tells the workers what to run.
-    The packet travels through shared memory (parallel/control.py); the activations never leave the GPUs."""
+class RootInference(TokenSteps):
+    """Root-side handle (reference RootLlmInference, src/app.cpp:168-208): the token steps of api.TokenSteps over the session's
+    engine, every engine call first announced to the workers. The packet travels through shared memory (parallel/control.py),
+    or torch.distributed broadcasts without a channel; the activations never leave the GPUs."""
 
     def __init__(self, sess: InferenceSession, comm, chan=None):
-        self.sess = sess
+        super().__init__(sess.engine, sess.device, comm.world_size if comm is not None else 1)
         self.comm = comm
         self.chan = chan
-        self.eng = sess.engine
-        self.header = sess.header
-        self.eval_ms = 0.0
-        self._ctl = torch.zeros(4, dtype=torch.int64, device=sess.device) if (comm is not None and chan is None) else None
-        on_gpu = torch.device(sess.device).type == "cuda"   # the session's device, not whether the machine has a GPU
-        self._pin_out = torch.zeros(1, dtype=torch.int32).pin_memory() if on_gpu else None
-        self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory() if on_gpu else None
+        self._ctl = torch.zeros(4, dtype=torch.int64, device=self.device) if (comm is not None and chan is None) else None
 
-    def _send(self, op: int, pos: int, tokens: Sequence[int]):
+    def _send(self, op: int, pos: int, words: Sequence[int]) -> None:
         if self.comm is None:
             return
         if self.chan is not None:
-            self.chan.send(op, pos, tokens)
+            self.chan.send(op, pos, words)
             return
         import torch.distributed as dist
-        n = len(tokens)
+        n = len(words)
         self._ctl[0], self._ctl[1], self._ctl[2] = op, pos, n
         dist.broadcast(self._ctl, 0)
         if n:
-            t = torch.tensor(list(tokens), dtype=torch.int64, device=self.sess.device)
+            t = torch.tensor(list(words), dtype=torch.int64, device=self.device)
             dist.broadcast(t, 0)
-
-    def prefill(self, tokens: Sequence[int], pos: int) -> None:
-        if tokens:
-            self._send(OP_PREFILL, pos, tokens)
-            self.eng.prefill(tokens, pos, want_logits=False)
-
-    def forward_logits(self, token: int, pos: int) -> torch.Tensor:
-        self._send(OP_STEP_LOGITS, pos, [token])
-        return self.eng.step(token, pos)
-
-    def forward_greedy(self, token: int, pos: int, logprobs: Optional[int] = None) -> int:
-        self._send(OP_STEP_GREEDY, pos, [token])
-        if self._pin_in is None:          # session on the CPU (protocol tests)
-            self.eng._set_inputs([token], pos)
-            self.eng.run_decode_step()
-            return int(self.eng.tokens[0])
-        # the root synchronises every step, so one pinned staging slot is enough (workers enqueue ahead: pageable staging)
-        self._pin_in[0], self._pin_in[1] = token, pos
-        self.eng.tokens[:1].copy_(self._pin_in[:1], non_blocking=True)
-        self.eng.pos[:1].copy_(self._pin_in[1:2], non_blocking=True)
-        self.eng.run_decode_step()
-        lp = logprobs
-        if lp is not None:
-            self.eng.logprobs([lp])
-        self._pin_out.copy_(self.eng.tokens[:1], non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        self.eng.check_abort()
-        if lp is not None:
-            self._last_logprobs = self.eng.read_logprobs()
-        return int(self._pin_out[0])
-
-    # ---- sampling on the device: the logits never leave the GPUs (csrc/cuda/sampler.cu) ----
-    @property
-    def device_sampling(self) -> bool:
-        return self._pin_in is not None and not getattr(self.eng, "_parts", False) and os.environ.get("DL_HOST_SAMPLER") is None
-
-    def seed(self, seed: int) -> None:
-        self._send(OP_SEED, 0, _split_seed(seed))
-        self.eng.seed_sampler(seed)
-
-    def forward_sampled(self, token: int, pos: int, temperature: float, topp: float, logprobs: Optional[int] = None) -> int:
-        import struct
-        t_bits, p_bits = struct.unpack("<ii", struct.pack("<ff", temperature, topp))
-        self._send(OP_STEP_SAMPLE, pos, [token, t_bits, p_bits])
-        self.eng.step_sampled(token, pos, temperature, topp)
-        lp = logprobs
-        if lp is not None:
-            self.eng.logprobs([lp], controlled=True)
-        self._pin_out.copy_(self.eng.tokens[:1], non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        self.eng.check_abort()
-        if lp is not None:
-            self._last_logprobs = self.eng.read_logprobs()
-        return int(self._pin_out[0])
-
-    def set_controls(self, sampler, row_mask: int) -> None:
-        bias = sampler.logit_bias
-        words = _f32_bits(sampler.presence_penalty, sampler.frequency_penalty) + [row_mask]
-        for t, v in bias:
-            words += [t] + _f32_bits(v)
-        self._send(OP_CONTROLS, 0, words)
-        self.eng.set_sampling_controls(sampler.presence_penalty, sampler.frequency_penalty, bias, row_mask)
-
-    def set_filters(self, sampler) -> None:
-        """The sampler's top_k / min_p on every rank, before the first draw that uses them (each rank draws from the gathered
-        logits with its own generator, so all ranks must hold the same filters)."""
-        key = (sampler.top_k, sampler.min_p)
-        if getattr(self, "_filters", (0, 0.0)) != key:
-            self._send(OP_FILTERS, 0, [key[0]] + _f32_bits(key[1]))
-            self.eng.set_sampling_filters(*key)
-            self._filters = key
-
-    def next_token(self, token: int, pos: int, sampler, logprobs: Optional[int] = None) -> int:
-        """One generated token with the sampler's settings: greedy and temperature/top-p both run on the device; the host sampler
-        is only used with the library-collective (multi-node) mode or DL_HOST_SAMPLER=1. Greedy with sampling controls runs
-        on the device sampler (arg-max of the controlled logits), not on the fused arg-max. logprobs = k: also the
-        log-probabilities of the draw on the device (last_logprobs(); one GPU only), enqueued behind it."""
-        if logprobs is not None:
-            check_logprobs(logprobs, self.comm.world_size if self.comm is not None else 1)
-        if sampler.temperature == 0.0 and not sampler.controls_active:
-            return self.forward_greedy(token, pos, logprobs)
-        if self.device_sampling:
-            if sampler.temperature != 0.0 and getattr(self, "_seeded", None) != (sampler.seed, sampler.seed_generation):
-                self.seed(sampler.seed)
-                self._seeded = (sampler.seed, sampler.seed_generation)
-            key = sampler.completion_generation if sampler.controls_active else None
-            if getattr(self, "_controls", None) != key:   # a new completion: count row 0 starts from zero
-                self.set_controls(sampler, 1)
-                self._controls = key
-            self.set_filters(sampler)
-            return self.forward_sampled(token, pos, sampler.temperature, sampler.topp, logprobs)
-        t = int(sampler.sample(self.forward_logits(token, pos).float().cpu().numpy()))
-        if logprobs is not None:
-            self._last_logprobs = [self.eng.logprobs_host_draw(t, logprobs, sampler)]
-        return t
-
-    def last_logprobs(self) -> list:
-        """The log-probability entries of the last next_token / choices call asked for them (InferenceSession.last_logprobs)."""
-        return self._last_logprobs
-
-    # ---- several completions of one prompt (api.run_choices); workers mirror every batched step ----
-    def forget_device_seed(self):
-        self._seeded = None
-
-    def save_sampler(self):
-        key = getattr(self, "_seeded", None)
-        return key, (self.eng.sampler_state() if key is not None and self.device_sampling else 0)
-
-    def restore_sampler(self, saved):
-        key, state = saved
-        if key is not None and self.device_sampling:
-            self.seed(state)
-        self._seeded = key
-
-    def batched_choices(self, n: int) -> bool:
-        return self.device_sampling and self.eng.supports_choices(n)
-
-    def choice_controls(self, sampler, n: int) -> None:
-        self.set_filters(sampler)
-        if sampler.controls_active or getattr(self, "_controls", None) is not None:
-            self.set_controls(sampler, ((1 << n) - 1) << 1)
-            self._controls = -1 if sampler.controls_active else None   # row 0's counts are not this sampler's
-
-    def seed_choices(self, seeds: Sequence[int]) -> None:
-        self._send(OP_CHOICES_SEED, 0, [w for s in seeds for w in _split_seed(s)])
-        self.eng.seed_choice_samplers(seeds)
-
-    def choices_first(self, token: int, P: int, n: int, temperature: float, topp: float, logprobs: Optional[int] = None) -> List[int]:
-        self._send(OP_CHOICES_FIRST, P, [token, n] + _f32_bits(temperature, topp))
-        out = self.eng.choices_first(token, P, n, temperature, topp, **_lp_kw(logprobs))
-        if logprobs is not None:
-            self._last_logprobs = self.eng.read_logprobs()
-        return out
-
-    def choices_step(self, tokens: Sequence[int], P: int, C: int, j: int, active: Sequence[bool], temperature: float,
-                     topp: float, logprobs: Optional[int] = None) -> List[int]:
-        self._send(OP_CHOICES_STEP, P, [C, j, _active_mask(active)] + _f32_bits(temperature, topp) + list(tokens))
-        out = self.eng.choices_step(tokens, P, C, j, active, temperature, topp, **_lp_kw(logprobs))
-        if logprobs is not None:
-            self._last_logprobs = self.eng.read_logprobs()
-        return out
-
-    def decode_greedy(self, token: int, pos: int, n_steps: int) -> List[int]:
-        """n greedy steps with the token fed back on the device (no host round trip per step): one control packet for all."""
-        self._send(OP_DECODE_N, pos, [token, n_steps])
-        return self.eng.decode_greedy(token, pos, n_steps)
 
     def finish(self):
         try:
@@ -333,8 +149,7 @@ def worker_loop(sess: InferenceSession, comm, chan=None) -> None:
         elif op == OP_FILTERS:
             eng.set_sampling_filters(toks[0], _bits_f32(toks[1])[0])
         elif op == OP_STEP_SAMPLE:
-            import struct
-            temperature, topp = struct.unpack("<ff", struct.pack("<ii", toks[1], toks[2]))
+            temperature, topp = _bits_f32(toks[1], toks[2])
             eng.step_sampled(toks[0], pos, temperature, topp)
 
 

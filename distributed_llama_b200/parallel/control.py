@@ -24,6 +24,37 @@ MAX_TOKENS = 8192
 _HDR_WORDS = 64          # u64 words: [0] seq, [1] op, [2] pos, [3] n, [8..16) ack per rank, [16..24) heartbeat per rank (ns)
 _ACK0, _HB0 = 8, 16
 
+# The packets: op, position and int32 words. The root sends them before every engine call a worker must repeat
+# (api.TokenSteps._send, apps.runtime.RootInference); apps.runtime.worker_loop makes the same call.
+OP_STOP, OP_PREFILL, OP_STEP_LOGITS, OP_STEP_GREEDY, OP_DECODE_N, OP_STEP_SAMPLE, OP_SEED = 0, 1, 2, 3, 4, 5, 6
+OP_CHOICES_SEED, OP_CHOICES_FIRST, OP_CHOICES_STEP = 7, 8, 9
+OP_CONTROLS = 10   # [presence bits, frequency bits, count-row mask, (id, bias bits) ...]: Engine.set_sampling_controls
+OP_FILTERS = 11    # [top_k, min_p bits]: Engine.set_sampling_filters
+
+
+def _split_seed(seed: int) -> List[int]:
+    return [seed & 0x7FFFFFFF, (seed >> 31) & 0x7FFFFFFF, (seed >> 62) & 0x3]
+
+
+def _join_seed(w: Sequence[int]) -> int:
+    return w[0] | (w[1] << 31) | (w[2] << 62)
+
+
+def _active_mask(active: Sequence[bool]) -> int:
+    return sum(1 << i for i, a in enumerate(active) if a)
+
+
+def _active_list(mask: int, n: int) -> List[bool]:
+    return [bool((mask >> i) & 1) for i in range(n)]
+
+
+def _f32_bits(*xs: float) -> List[int]:
+    return list(struct.unpack(f"<{len(xs)}i", struct.pack(f"<{len(xs)}f", *xs)))
+
+
+def _bits_f32(*xs: int) -> List[float]:
+    return list(struct.unpack(f"<{len(xs)}f", struct.pack(f"<{len(xs)}i", *xs)))
+
 
 class PeerLost(RuntimeError):
     """A rank of the job stopped responding (process died or its GPU wedged)."""
