@@ -861,61 +861,54 @@ static size_t tmaGeometry(GemmArgs &a) {
     return 0;
 }
 
-// act: bf16 [T][n] row-major (row stride actStride elements). variant: 0 auto, 1 register-prefetch dequant, 2 TMA-staged raw weights.
-static float *gSplitScratch = nullptr;
-static unsigned int *gSplitCounters = nullptr;
-static size_t gSplitScratchBytes = 0;
+// Dispatch decision of gemmQ40TcV: kernel, shared-memory geometry, split-K and reduce scheme, grid. Pure host code (reads only the
+// DL_GEMM_GEOM / DL_GEMM_CLUSTER / DL_GEMM_SPLITK switches), so dl_gemm_q40_tc_plan can report what a launch with the same
+// arguments runs. rc != 0: the launcher's return code for a shape it does not cover.
+struct GemmPlan {
+    int rc;
+    bool tma;              // TMA-staged variant (else the register-prefetch one)
+    uint32_t stages, rawStages, bStages, splitK, clusterSplit, grid;
+    size_t smemBytes;
+};
 
-int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride, uint32_t T,
-               void *out, uint32_t outStride, int numSms, cudaStream_t stream, bool pdl, int variant, const ArArgs *ar) {
-    if (T == 0 || T > 256 || n % kGmBlockK || d % 2) return -1;
-    EncodeTiledFn enc = encodeTiled();
-    if (!enc) return -2;
-    bool tma = variant == 2 || (variant == 0 && n % 256 == 0);
-    if (tma && n % 256) return -6;
-    GemmArgs a{};
-    a.act = gHiddenAct;
-    a.qs = (const uint32_t *)qs; a.scales = (const __half *)scales; a.d = d; a.n = n; a.T = T;
-    a.out = out; a.outStride = outStride;
-    if (ar) a.ar = *ar;
-    { const char *dbg = getenv("DL_GEMM_DEBUG"); a.debugFlags = dbg ? (uint32_t)atoi(dbg) : 0u; }
+static GemmPlan planGemmQ40Tc(int epi, uint32_t d, uint32_t n, uint32_t T, uint32_t actStride, int numSms, int variant) {
+    GemmPlan p{};
+    p.rc = -1;
+    if (T == 0 || T > 256 || n % kGmBlockK || d % 2) return p;
+    p.rc = -6;
+    p.tma = variant == 2 || (variant == 0 && n % 256 == 0);
+    if (p.tma && n % 256) return p;
+    p.rc = -4;
+    if (actStride % 8) return p;   // the activation tensor map needs a row pitch that is a multiple of 16 bytes
     const size_t stageBytes = kGmATileBytes + kGmBTileBytes;
     const size_t budget = 227 * 1024 - 1024 - 512 - kGmStgBytes;
-    uint32_t stages = 0;
-    size_t tmaSmem = 0;
-    if (tma) {
-        tmaSmem = tmaGeometry(a);
-        if (!tmaSmem) {
-            if (variant == 2) return -9;
-            tma = false;
+    if (p.tma) {
+        GemmArgs g{};
+        p.smemBytes = tmaGeometry(g);
+        if (!p.smemBytes) {
+            p.rc = -9;
+            if (variant == 2) return p;
+            p.tma = false;
         } else {
-            stages = a.stages;
+            p.stages = g.stages; p.rawStages = g.rawStages; p.bStages = g.bStages;
         }
     }
-    if (!tma) {
-        stages = (uint32_t)(budget / stageBytes);
-        if (stages > (uint32_t)kGmMaxStages) stages = kGmMaxStages;
-        if (stages < 2) return -3;
+    if (!p.tma) {
+        p.stages = (uint32_t)(budget / stageBytes);
+        if (p.stages > (uint32_t)kGmMaxStages) p.stages = kGmMaxStages;
+        p.rc = -3;
+        if (p.stages < 2) return p;
+        p.smemBytes = p.stages * stageBytes + 1024 + 512 + kGmStgBytes;
     }
-    a.stages = stages;
-    const size_t smemBytes = tma ? tmaSmem : stages * stageBytes + 1024 + 512 + kGmStgBytes;
-
-    CUtensorMap mapB, mapQ, mapS;
-    if (!encode2d(enc, &mapB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, act, n, T, (uint64_t)actStride * 2, kGmBlockK, kGmTokTile, CU_TENSOR_MAP_SWIZZLE_128B))
-        return -4;
-    if (tma) {
-        if (a.debugFlags & 256u) {
-            if (!encode2d(enc, &mapQ, CU_TENSOR_MAP_DATA_TYPE_UINT8, qs, 128, (uint64_t)d * (n / 2) / 128, 128, 128, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_128B)) return -7;
-            if (!encode2d(enc, &mapS, CU_TENSOR_MAP_DATA_TYPE_UINT8, scales, 16, (uint64_t)d * (n / 16) / 16, 16, 16, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_NONE)) return -8;
-        } else {
-        if (!encode2d(enc, &mapQ, CU_TENSOR_MAP_DATA_TYPE_UINT8, qs, n / 2, d, n / 2, 128, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_128B)) return -7;
-        if (!encode2d(enc, &mapS, CU_TENSOR_MAP_DATA_TYPE_UINT8, scales, n / 16, d, n / 16, 16, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_NONE)) return -8;
-        }
-    }
+    p.rc = -10;
+    if (epi == GEPI_RESIDUAL_AR && !p.tma) return p;
+    p.rc = -5;
+    if (epi < GEPI_STORE_F32 || epi > GEPI_RESIDUAL_AR) return p;
+    p.rc = 0;
     const uint32_t nTilesM = (d + kGmBlockM - 1) / kGmBlockM;
     const uint32_t nTT = (T + kGmTokTile - 1) / kGmTokTile;
-    a.splitK = 1;
-    if (tma && epi != GEPI_RESIDUAL_AR) {
+    p.splitK = 1;
+    if (p.tma && epi != GEPI_RESIDUAL_AR) {
         // small-d matrices (qkv, wo, w2) leave most SMs idle with one CTA per work item: cut K so that ~all SMs get an item
         const uint32_t nkq = n / 256;
         uint32_t sk = (uint32_t)numSms / (nTilesM * nTT);
@@ -930,39 +923,76 @@ int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t
         auto clusterFits = [&](uint32_t k) {
             const uint32_t per = ((min(T, (uint32_t)kGmTokTile) + k - 1) / k + 15u) & ~15u;
             // clusters of 2 or 4 only (a power of two divides the GPC evenly)
-            return (k == 2 || k == 4) && (size_t)(k - 1) * per * kGmBlockM * 4 <= (size_t)a.stages * kGmATileBytes && !(clEnv && clEnv[0] == '0');
+            return (k == 2 || k == 4) && (size_t)(k - 1) * per * kGmBlockM * 4 <= (size_t)p.stages * kGmATileBytes && !(clEnv && clEnv[0] == '0');
         };
         // K < 8192 with fewer than 4 splits does not pay for the reduce
         if (nkq < 32 && sk < 4) sk = 1;
         if (const char *f = getenv("DL_GEMM_SPLITK")) { const uint32_t want = (uint32_t)atoi(f); if (want >= 1 && want < sk) sk = want; }
-        if (sk >= 2) {
-            const size_t need = (size_t)sk * T * d * sizeof(float);
-            if (need > gSplitScratchBytes) {
-                if (gSplitScratch) cudaFree(gSplitScratch);
-                DL_CUDA_CHECK(cudaMalloc(&gSplitScratch, need));
-                gSplitScratchBytes = need;
-            }
-            if (!gSplitCounters) {
-                DL_CUDA_CHECK(cudaMalloc(&gSplitCounters, 4096 * sizeof(unsigned int)));
-                DL_CUDA_CHECK(cudaMemset(gSplitCounters, 0, 4096 * sizeof(unsigned int)));
-            }
-            if (nTilesM * nTT * 8 <= 4096) {
-                a.splitK = sk; a.splitScratch = gSplitScratch; a.splitCounters = gSplitCounters;
-                a.clusterSplit = clusterFits(sk) ? 1u : 0u;
-            }
+        if (sk >= 2 && nTilesM * nTT * 8 <= 4096) {
+            p.splitK = sk;
+            p.clusterSplit = clusterFits(sk) ? 1u : 0u;
         }
     }
-    const uint32_t nItems = nTilesM * nTT * a.splitK;
-    const int grid = (int)(nItems < (uint32_t)numSms ? nItems : (uint32_t)numSms);
-    const CUtensorMap *pq = tma ? &mapQ : nullptr, *ps = tma ? &mapS : nullptr;
+    const uint32_t nItems = nTilesM * nTT * p.splitK;
+    p.grid = nItems < (uint32_t)numSms ? nItems : (uint32_t)numSms;
+    return p;
+}
+
+// act: bf16 [T][n] row-major (row stride actStride elements). variant: 0 auto, 1 register-prefetch dequant, 2 TMA-staged raw weights.
+static float *gSplitScratch = nullptr;
+static unsigned int *gSplitCounters = nullptr;
+static size_t gSplitScratchBytes = 0;
+
+int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride, uint32_t T,
+               void *out, uint32_t outStride, int numSms, cudaStream_t stream, bool pdl, int variant, const ArArgs *ar) {
+    const GemmPlan p = planGemmQ40Tc(epi, d, n, T, actStride, numSms, variant);
+    if (p.rc) return p.rc;
+    if (epi == GEPI_RESIDUAL_AR && !ar) return -10;
+    EncodeTiledFn enc = encodeTiled();
+    if (!enc) return -2;
+    GemmArgs a{};
+    a.act = gHiddenAct;
+    a.qs = (const uint32_t *)qs; a.scales = (const __half *)scales; a.d = d; a.n = n; a.T = T;
+    a.out = out; a.outStride = outStride;
+    if (ar) a.ar = *ar;
+    { const char *dbg = getenv("DL_GEMM_DEBUG"); a.debugFlags = dbg ? (uint32_t)atoi(dbg) : 0u; }
+    a.stages = p.stages; a.rawStages = p.rawStages; a.bStages = p.bStages;
+
+    CUtensorMap mapB, mapQ, mapS;
+    if (!encode2d(enc, &mapB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, act, n, T, (uint64_t)actStride * 2, kGmBlockK, kGmTokTile, CU_TENSOR_MAP_SWIZZLE_128B))
+        return -4;
+    if (p.tma) {
+        if (a.debugFlags & 256u) {
+            if (!encode2d(enc, &mapQ, CU_TENSOR_MAP_DATA_TYPE_UINT8, qs, 128, (uint64_t)d * (n / 2) / 128, 128, 128, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_128B)) return -7;
+            if (!encode2d(enc, &mapS, CU_TENSOR_MAP_DATA_TYPE_UINT8, scales, 16, (uint64_t)d * (n / 16) / 16, 16, 16, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_NONE)) return -8;
+        } else {
+        if (!encode2d(enc, &mapQ, CU_TENSOR_MAP_DATA_TYPE_UINT8, qs, n / 2, d, n / 2, 128, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_128B)) return -7;
+        if (!encode2d(enc, &mapS, CU_TENSOR_MAP_DATA_TYPE_UINT8, scales, n / 16, d, n / 16, 16, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_NONE)) return -8;
+        }
+    }
+    a.splitK = p.splitK;
+    if (p.splitK >= 2) {
+        const size_t need = (size_t)p.splitK * T * d * sizeof(float);
+        if (need > gSplitScratchBytes) {
+            if (gSplitScratch) cudaFree(gSplitScratch);
+            DL_CUDA_CHECK(cudaMalloc(&gSplitScratch, need));
+            gSplitScratchBytes = need;
+        }
+        if (!gSplitCounters) {
+            DL_CUDA_CHECK(cudaMalloc(&gSplitCounters, 4096 * sizeof(unsigned int)));
+            DL_CUDA_CHECK(cudaMemset(gSplitCounters, 0, 4096 * sizeof(unsigned int)));
+        }
+        a.splitScratch = gSplitScratch; a.splitCounters = gSplitCounters;
+        a.clusterSplit = p.clusterSplit;
+    }
+    const int grid = (int)p.grid;
+    const CUtensorMap *pq = p.tma ? &mapQ : nullptr, *ps = p.tma ? &mapS : nullptr;
     switch (epi) {
-        case GEPI_STORE_F32: return launchGemm<GEPI_STORE_F32>(mapB, pq, ps, a, grid, smemBytes, stream, pdl);
-        case GEPI_RESIDUAL: return launchGemm<GEPI_RESIDUAL>(mapB, pq, ps, a, grid, smemBytes, stream, pdl);
-        case GEPI_SWIGLU_BF16: return launchGemm<GEPI_SWIGLU_BF16>(mapB, pq, ps, a, grid, smemBytes, stream, pdl);
-        case GEPI_STORE_BF16: return launchGemm<GEPI_STORE_BF16>(mapB, pq, ps, a, grid, smemBytes, stream, pdl);
-        case GEPI_RESIDUAL_AR:
-            if (!tma || !ar) return -10;
-            return launchGemm<GEPI_RESIDUAL_AR>(mapB, pq, ps, a, grid, smemBytes, stream, pdl);
+        case GEPI_STORE_F32: return launchGemm<GEPI_STORE_F32>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
+        case GEPI_RESIDUAL: return launchGemm<GEPI_RESIDUAL>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
+        case GEPI_SWIGLU_BF16: return launchGemm<GEPI_SWIGLU_BF16>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
+        case GEPI_STORE_BF16: return launchGemm<GEPI_STORE_BF16>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
+        case GEPI_RESIDUAL_AR: return launchGemm<GEPI_RESIDUAL_AR>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
     }
     return -5;
 }
@@ -1048,9 +1078,20 @@ DL_EXPORT int dl_gemm_trace_read(unsigned long long *host) {
     return (int)cudaMemcpyFromSymbol(host, dl::gGemmTrace, sizeof(unsigned long long) * 4096);
 }
 
+// Stand-alone entry point (tests, tools): the gate activation of GEPI_SWIGLU_BF16 is passed explicitly (0 = SiLU, 1 = GELU).
 DL_EXPORT int dl_gemm_q40_tc(int epi, const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride,
-                             uint32_t T, void *out, uint32_t outStride, int numSms, cudaStream_t stream, int pdl, int variant) {
+                             uint32_t T, void *out, uint32_t outStride, int numSms, uint32_t hiddenAct, cudaStream_t stream, int pdl, int variant) {
+    const dl::HiddenActScope a(hiddenAct);
     return dl::gemmQ40TcV(epi, qs, scales, d, n, act, actStride, T, out, outStride, numSms, stream, pdl != 0, variant, nullptr);
+}
+
+// What dl_gemm_q40_tc would run for these arguments (and the current DL_GEMM_* switches), without launching or allocating:
+// out[8] = {rc, kernel (1 register-prefetch, 2 TMA-staged), splitK, cluster reduce (0/1), grid, A stages, raw stages, B stages}.
+DL_EXPORT int dl_gemm_q40_tc_plan(int epi, uint32_t d, uint32_t n, uint32_t T, uint32_t actStride, int numSms, int variant, int *out) {
+    const dl::GemmPlan p = dl::planGemmQ40Tc(epi, d, n, T, actStride, numSms, variant);
+    const int v[8] = {p.rc, p.tma ? 2 : 1, (int)p.splitK, (int)p.clusterSplit, (int)p.grid, (int)p.stages, (int)p.rawStages, (int)p.bStages};
+    for (int i = 0; i < 8; i++) out[i] = p.rc ? (i == 0 ? p.rc : 0) : v[i];
+    return p.rc;
 }
 
 // Grouped mode for the unit tests (tests/test_gpu_moe.py): gemmQ40TcGrouped with caller-provided device arrays grpCount /

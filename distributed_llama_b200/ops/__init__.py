@@ -1,3 +1,3 @@
 from .cuda_lib import lib, check, stream_ptr, PRO_RMSNORM, PRO_PLAIN, EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU
 from .cuda_lib import GEPI_STORE_F32, GEPI_RESIDUAL, GEPI_SWIGLU_BF16, GEPI_STORE_BF16
-from .q40 import DeviceQ40, DeviceDense, repack_q40, gemv_q40, gemv_dense, gemm_q40_tc, rmsnorm_bf16
+from .q40 import DeviceQ40, DeviceDense, repack_q40, gemv_q40, gemv_dense, gemm_q40_tc, gemm_q40_tc_plan, GemmPlan, rmsnorm_bf16

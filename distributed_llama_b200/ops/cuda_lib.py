@@ -54,8 +54,10 @@ def lib() -> C.CDLL:
     L.dl_gemv_q40.restype = i32
     L.dl_gemv_dense.argtypes = [i32, i32, i32, i32, vp, u32, u32, vp, u32, vp, f32, vp, u32, i32, vp, i32]
     L.dl_gemv_dense.restype = i32
-    L.dl_gemm_q40_tc.argtypes = [i32, vp, vp, u32, u32, vp, u32, u32, vp, u32, i32, vp, i32, i32]
+    L.dl_gemm_q40_tc.argtypes = [i32, vp, vp, u32, u32, vp, u32, u32, vp, u32, i32, u32, vp, i32, i32]
     L.dl_gemm_q40_tc.restype = i32
+    L.dl_gemm_q40_tc_plan.argtypes = [i32, u32, u32, u32, u32, i32, i32, C.POINTER(C.c_int)]
+    L.dl_gemm_q40_tc_plan.restype = i32
     L.dl_rmsnorm_bf16.argtypes = [vp, u32, vp, vp, u32, u32, f32, u32, vp]
     L.dl_rmsnorm_bf16.restype = i32
     L.dl_attn_prefill_tc.argtypes = [vp, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]

@@ -1,6 +1,7 @@
 """Device-side q40 matrices: repack from `.m` bytes and the standalone GEMV entry point (tests, microbenchmarks)."""
 from __future__ import annotations
 
+import ctypes
 from dataclasses import dataclass
 from typing import Optional
 
@@ -91,16 +92,41 @@ def gemv_q40(w: DeviceQ40, x: torch.Tensor, *, pro: int, epi: int, out: torch.Te
     return out
 
 
+GEMM_VARIANTS = {"auto": 0, "ldg": 1, "tma": 2}
+
+
 def gemm_q40_tc(w: DeviceQ40, act: torch.Tensor, *, epi: int, out: torch.Tensor, num_sms: int = 0, pdl: bool = False,
-                variant: str = "auto") -> torch.Tensor:
-    """Tensor-core (wgmma) prefill GEMM. act: bf16 [T, n] (T <= 256); out: [T, d] f32 (STORE/RESIDUAL), bf16 [T, d/2] (SWIGLU) or bf16 [T, d]."""
+                variant: str = "auto", act_fn: int = 0) -> torch.Tensor:
+    """Tensor-core (wgmma) prefill GEMM. act: bf16 [T, n] (T <= 256); out: [T, d] f32 (STORE/RESIDUAL), bf16 [T, d/2] (SWIGLU) or bf16 [T, d].
+    act_fn: gate activation of the SwiGLU epilogue (0 = SiLU, 1 = tanh-GELU)."""
     assert act.dtype == torch.bfloat16 and act.is_cuda and act.stride(1) == 1
     if num_sms == 0:
         num_sms = torch.cuda.get_device_properties(act.device).multi_processor_count
     cl.check(cl.lib().dl_gemm_q40_tc(epi, w.qs.data_ptr(), w.scales.data_ptr(), w.d, w.n, act.data_ptr(), act.stride(0), act.shape[0],
-                                     out.data_ptr(), out.stride(0), num_sms, cl.stream_ptr(), 1 if pdl else 0,
-                                     {"auto": 0, "ldg": 1, "tma": 2}[variant]), "gemm_q40_tc")
+                                     out.data_ptr(), out.stride(0), num_sms, act_fn, cl.stream_ptr(), 1 if pdl else 0,
+                                     GEMM_VARIANTS[variant]), "gemm_q40_tc")
     return out
+
+
+@dataclass(frozen=True)
+class GemmPlan:
+    """What gemm_q40_tc runs for a shape (dl_gemm_q40_tc_plan). kernel: 1 register-prefetch ("ldg"), 2 TMA-staged ("tma");
+    split_k > 1 with cluster = 1: partial sums reduced inside a thread-block cluster, cluster = 0: through the global scratch."""
+    rc: int
+    kernel: int
+    split_k: int
+    cluster: int
+    grid: int
+    stages: int
+    raw_stages: int
+    b_stages: int
+
+
+def gemm_q40_tc_plan(epi: int, d: int, n: int, T: int, *, act_stride: Optional[int] = None, num_sms: int, variant: str = "auto") -> GemmPlan:
+    """The dispatch decision of gemm_q40_tc (reads DL_GEMM_CLUSTER / DL_GEMM_SPLITK like the launch); launches nothing."""
+    out = (ctypes.c_int * 8)()
+    cl.lib().dl_gemm_q40_tc_plan(epi, d, n, T, n if act_stride is None else act_stride, num_sms, GEMM_VARIANTS[variant], out)
+    return GemmPlan(*out)
 
 
 def rmsnorm_bf16(x: torch.Tensor, w: Optional[torch.Tensor], eps: float, out: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -38,10 +38,12 @@ FFN), the f16 scale instead of its bf16 rounding (grouped GEMM at K = 2048), gat
 routing weights left unnormalised (router), and no q80 rounding of the kernel's h in decode stage 2 (decode FFN at 2048/768/128/8).
 """
 import math
-import zlib
 
 import pytest
 import torch
+
+from q40_ref import Experts, assert_bracketed, assert_within, bf16_bracket, f64_to_bf16
+from q40_ref import gen as _gen, seed_of as _seed
 
 pytestmark = pytest.mark.gpu
 
@@ -63,14 +65,6 @@ def _cl():
     return cl
 
 
-def _seed(*key):
-    return zlib.crc32(repr(key).encode())
-
-
-def _gen(*key):
-    return torch.Generator(device="cuda").manual_seed(_seed(*key))
-
-
 def _num_sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
 
@@ -80,16 +74,6 @@ def _i32(t):
 
 
 # ---- float64 reference helpers ---------------------------------------------------------------------------------------
-def f64_to_bf16(x):
-    """bf16 rounding of f64 values (via f32, as the kernels round their f32 values)."""
-    return x.float().bfloat16().double()
-
-
-def bf16_bracket(r, e):
-    """bf16 roundings of the interval ends [r - e, r + e]: a value the kernel rounds from inside the interval lies between them."""
-    return f64_to_bf16(r - e), f64_to_bf16(r + e)
-
-
 def q80_ref(v, rel):
     """q80 grid of f64 activations v [..., n] (blocks of 32: d = f16(amax / 127), q = rint(x / d)) and, per element, the most the
     kernel's grid value can differ when its input is within `rel` (relative) of v."""
@@ -124,71 +108,6 @@ def swiglu_ref(gu, e_gu):
 def rms_ref(x, w):
     x = x.double()
     return w.double() * (x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + EPS))
-
-
-def assert_within(got, ref, tol, what):
-    got = got.double()
-    assert torch.isfinite(got).all(), f"{what}: non-finite values"
-    err = (got - ref).abs()
-    ratio = (err / tol.clamp_min(1e-30)).max().item()
-    assert ratio <= 1.0, f"{what}: max err {err.max().item():.3g} = {ratio:.3g} x bound (max|ref| {ref.abs().max().item():.3g})"
-
-
-def assert_bracketed(got, lo, hi, what):
-    got = got.double()
-    assert torch.isfinite(got).all(), f"{what}: non-finite values"
-    bad = (got < lo) | (got > hi)
-    assert not bad.any(), (f"{what}: {int(bad.sum())} of {bad.numel()} values outside the rounding interval "
-                           f"(max distance {torch.maximum(lo - got, got - hi).max().item():.3g})")
-
-
-# ---- random q40 expert stacks ------------------------------------------------------------------------------------------
-class Experts:
-    """E stacked q40 matrices [rows][n] (raw 18-byte blocks + the device layout). Row r of expert e is stack row e * rows + r."""
-
-    def __init__(self, E, rows, n, seed):
-        g = _gen("q40", E, rows, n, seed)
-        nb = E * rows * n // 32
-        sc = (torch.rand(nb, device="cuda", generator=g) + 0.5) / (4.0 * math.sqrt(n))
-        sc = torch.where(torch.rand(nb, device="cuda", generator=g) < 0.5, -sc, sc).half()
-        self.raw = torch.empty(nb, 18, dtype=torch.uint8, device="cuda")
-        self.raw[:, :2] = sc.view(torch.uint8).view(nb, 2)
-        self.raw[:, 2:] = torch.randint(0, 256, (nb, 16), dtype=torch.uint8, device="cuda", generator=g)
-        self.E, self.rows, self.n = E, rows, n
-        self._dev = {}
-
-    def device(self, first=0, count=None):
-        """DeviceQ40 of experts [first, first + count) only (an expert-parallel rank's weights)."""
-        from distributed_llama_b200.ops import DeviceQ40, repack_q40
-        count = self.E - first if count is None else count
-        if (first, count) not in self._dev:
-            r0, nr = first * self.rows, count * self.rows
-            dst = DeviceQ40.empty(nr, self.n)
-            blk = self.n // 32
-            repack_q40(self.raw[r0 * blk:(r0 + nr) * blk].reshape(-1), nr, self.n, dst)
-            self._dev[first, count] = dst
-        return self._dev[first, count]
-
-    def _parts(self, e):
-        blk = self.n // 32
-        raw = self.raw[e * self.rows * blk:(e + 1) * self.rows * blk]
-        sc = raw[:, :2].contiguous().view(torch.float16).view(self.rows, blk)
-        lo = (raw[:, 2:] & 15).double() - 8
-        hi = (raw[:, 2:] >> 4).double() - 8
-        q = torch.cat([lo, hi], dim=1).view(self.rows, self.n)     # per block: low nibbles are elements 0..15
-        return sc, q
-
-    def w_exact(self, e):
-        """Expert e dequantised exactly (the decode GEMV's weights), f64 [rows][n], and |w| + 8 |scale| (its f32 error scale)."""
-        sc, q = self._parts(e)
-        s = sc.double().repeat_interleave(32, dim=1)
-        return s * q, s.abs() * (q.abs() + 8)
-
-    def w_tc(self, e):
-        """Expert e as the tensor-core dequant builds it: rn_bf16(rn_bf16(f16 scale) * (q - 8))."""
-        sc, q = self._parts(e)
-        sb = sc.float().bfloat16().float().repeat_interleave(32, dim=1)
-        return (sb * q.float()).bfloat16().double()
 
 
 _EXPERTS = {}
