@@ -179,6 +179,44 @@ TokenLogprobs decodeLogprobs(const int32_t *w) {
     return e;
 }
 
+namespace {
+// Strict UTF-8 (no overlong forms, surrogates or code points above U+10FFFF): what Python accepts when it decodes a request body.
+bool validUtf8(const std::string &s) {
+    for (size_t i = 0; i < s.size();) {
+        const unsigned char c = (unsigned char)s[i];
+        int need;
+        unsigned char lo = 0x80, hi = 0xbf;
+        if (c < 0x80) { i++; continue; }
+        else if (c >= 0xc2 && c <= 0xdf) need = 1;
+        else if (c >= 0xe0 && c <= 0xef) { need = 2; if (c == 0xe0) lo = 0xa0; else if (c == 0xed) hi = 0x9f; }
+        else if (c >= 0xf0 && c <= 0xf4) { need = 3; if (c == 0xf0) lo = 0x90; else if (c == 0xf4) hi = 0x8f; }
+        else return false;
+        if (i + (size_t)need >= s.size()) return false;
+        for (int k = 1; k <= need; k++) {
+            const unsigned char d = (unsigned char)s[i + (size_t)k];
+            if (d < (k == 1 ? lo : 0x80) || d > (k == 1 ? hi : 0xbf)) return false;
+        }
+        i += (size_t)need + 1;
+    }
+    return true;
+}
+}  // namespace
+
+std::vector<std::string> parseStop(const JsonValue &body) {
+    const JsonValue *v = body.find("stop");
+    std::vector<std::string> out;
+    if (!v || v->kind == JsonValue::Null) return out;
+    const auto take = [&](const JsonValue &s) {
+        if (s.kind != JsonValue::String || s.loneSurrogate || s.str.empty() || s.str.size() > kMaxStopBytes || !validUtf8(s.str))
+            throw std::runtime_error("'stop' strings must be 1 to 256 bytes of UTF-8");
+        out.push_back(s.str);
+    };
+    if (v->kind == JsonValue::String) take(*v);
+    else if (v->kind == JsonValue::Array && v->arr.size() <= kMaxStopStrings) for (const JsonValue &s : v->arr) take(s);
+    else throw std::runtime_error("'stop' must be a string or an array of at most 4 strings");
+    return out;
+}
+
 int parseLogprobs(const JsonValue &body) {
     const JsonValue *on = body.find("logprobs"), *k = body.find("top_logprobs");
     if (on && on->kind != JsonValue::Bool) throw std::runtime_error("'logprobs' must be a boolean");
@@ -447,6 +485,7 @@ struct ChatRequest {
     uint32_t topK = 0;   // sampling filters (parseFilters)
     float minP = 0.f;
     uint64_t seed = 0;
+    std::vector<std::string> stop;   // parseStop
 };
 
 // maxN: the largest `n` (the slot count under --parallel)
@@ -466,6 +505,7 @@ ChatRequest parseChat(const JsonValue &body, const ApiConfig &cfg, uint32_t voca
     c.minP = cfg.minP;
     parseFilters(body, c.topK, c.minP);
     c.logprobs = parseLogprobs(body);
+    c.stop = parseStop(body);
     for (const JsonValue &m : body.at("messages").arr) c.messages.push_back({m.at("role").str, m.at("content").str});
     c.stream = body.boolOr("stream", false);
     c.temperature = (float)body.numberOr("temperature", cfg.temperature);
@@ -491,13 +531,19 @@ std::string completionJson(uint32_t nPrompt, const std::vector<std::vector<int32
 }
 
 // The response to one chat request: its n choices' decoders, stop detectors, texts and log-probability entries, written as stream
-// chunks or as one cmpl-j0 JSON body (the Python server's ChatResponse). echo: print the tokens' pieces to stdout.
+// chunks or as one cmpl-j0 JSON body (the Python server's ChatResponse). With `stop` strings each choice also has a StopMatcher
+// after its detector. echo: print the tokens' pieces to stdout.
 class ChatResponse {
 public:
     ChatResponse(const HttpRequest &req, const ChatRequest &chat, const Tokenizer &tok, const std::vector<std::string> &stops, bool echo = false)
         : req_(req), tok_(tok), n_(chat.n), stream_(chat.stream), echo_(echo), hasLog_(chat.logprobs >= 0), log_(chat.n),
-          dets_(chat.n, EosDetector(tok.data().eosIds, stops, maxLen(stops), maxLen(stops))), pending_(chat.n), buffers_(chat.n) {}
-    const std::string &text(uint32_t i) const { return buffers_[i]; }
+          dets_(chat.n, EosDetector(tok.data().eosIds, stops, maxLen(stops), maxLen(stops))), pending_(chat.n), buffers_(chat.n) {
+        if (!chat.stop.empty()) matchers_.assign(chat.n, StopMatcher(chat.stop));
+    }
+    // choice i's content so far, bytes held back by its matcher included
+    std::string text(uint32_t i) const { return matchers_.empty() ? buffers_[i] : buffers_[i] + matchers_[i].held(); }
+    // choice i ended at a stop string
+    bool stopped(uint32_t i) const { return !matchers_.empty() && matchers_[i].stopped(); }
     // every choice's text starts with the prompt's public part; a stream sends its head and that part
     void start(const std::string &publicPrompt) {
         buffers_.assign(n_, publicPrompt);
@@ -514,19 +560,27 @@ public:
         const EosDetectorResult kind = dets_[i].append(t, piece);
         if (hasLog_) log_.consumed(i, kind == EOS);
         if (kind == NOT_EOS || kind == EOS) {
-            const std::string delta = dets_[i].getDelta();
+            std::string delta = dets_[i].getDelta();
+            if (!matchers_.empty()) delta = matchers_[i].push(delta);
             if (!delta.empty()) {
                 if (stream_) chunk(i, delta);
                 buffers_[i] += delta;
             }
             dets_[i].reset();
         }
-        return kind == EOS;
+        return kind == EOS || stopped(i);
     }
-    // every choice is done (out[i]: choice i's tokens): the stop chunks and [DONE], or the JSON body
+    // every choice is done (out[i]: choice i's tokens): the stop chunks and [DONE], or the JSON body. Bytes a matcher still holds
+    // (a choice that ended another way) join the text, in one delta chunk before the stop chunk of a stream.
     void finish(const std::vector<std::vector<int32_t>> &out, uint32_t nPrompt) {
+        for (uint32_t i = 0; i < n_; i++) {
+            const std::string rest = matchers_.empty() ? std::string() : matchers_[i].flush();
+            buffers_[i] += rest;
+            if (!stream_) continue;
+            if (!rest.empty()) chunk(i, rest);
+            writeStreamFinish(req_, i, lps());
+        }
         if (!stream_) { req_.writeJson(completionJson(nPrompt, out, buffers_, lps())); return; }
-        for (uint32_t i = 0; i < n_; i++) writeStreamFinish(req_, i, lps());
         req_.writeStreamChunk("data: [DONE]");
         req_.writeStreamEnd();
     }
@@ -542,6 +596,7 @@ private:
     bool stream_, echo_, hasLog_;
     LogprobsLog log_;
     std::vector<EosDetector> dets_;
+    std::vector<StopMatcher> matchers_;   // empty without `stop`
     std::vector<std::string> pending_, buffers_;
 };
 
@@ -610,8 +665,8 @@ ApiServer::ApiServer(InferenceBackend &backend, Tokenizer &tokenizer, const ApiC
 }
 
 // n completions of one prompt (runChoices; n = 1 without `n`): the prompt is prefilled once. After one completion the cache
-// keeps its answer too; after several it keeps only the prompt messages, so a follow-up that quotes any one choice re-uses the
-// prompt.
+// keeps its answer too; after several, or after one cut at a stop string (its KV rows hold tokens past the cut), it keeps only the
+// prompt messages, so a follow-up that quotes any one choice re-uses the prompt.
 void ApiServer::complete(HttpRequest &req) {
     const ChatRequest chat = parseChat(req.json, cfg_, sampler_.vocabSize(), kMaxChoices);
     backend_.setLogprobs(chat.logprobs);   // refuses where they cannot run (tensor parallelism)
@@ -631,7 +686,7 @@ void ApiServer::complete(HttpRequest &req) {
     if (chat.logprobs >= 0) onLogprobs = [&](uint32_t i, const TokenLogprobs &e) { resp.onLogprobs(i, e); };
     const std::vector<std::vector<int32_t>> out = runChoices(backend_, p.token, p.P, chat.n, chat.maxTokens, seqLen, sampler_, baseSeed,
                                                              [&](uint32_t i, int32_t t) { return resp.onToken(i, t); }, onLogprobs);
-    if (chat.n == 1) rememberAnswer(cache_, p.P, out[0].size(), resp.text(0), seqLen);
+    if (chat.n == 1 && !resp.stopped(0)) rememberAnswer(cache_, p.P, out[0].size(), resp.text(0), seqLen);
     resp.finish(out, p.nPrompt);
     if (chat.n == 1) std::printf("🔶\n");
     else std::printf("(%u choices)🔶\n", chat.n);
@@ -731,7 +786,7 @@ void ApiServer::serveParallel(int srv) {
     const auto finish = [&](const std::shared_ptr<SlotJob> &job) {
         SlotJob &j = *job;
         NaiveCache &cache = caches[j.slots[0]];
-        if (j.chat.n == 1) rememberAnswer(cache, j.P, j.out[0].size(), j.resp.text(0), L);
+        if (j.chat.n == 1 && !j.resp.stopped(0)) rememberAnswer(cache, j.P, j.out[0].size(), j.resp.text(0), L);
         for (size_t k = 1; k < j.slots.size(); k++) caches[j.slots[k]].copyFrom(cache);   // they hold a copy of the prompt rows
         j.resp.finish(j.out, j.nPrompt);
         std::printf("🔶 slot %u%s\n", j.slots[0], j.chat.n > 1 ? (" (" + std::to_string(j.chat.n) + " choices)").c_str() : "");

@@ -126,6 +126,10 @@ std::string chunkJson(const std::string *delta, bool stop, uint32_t index = 0, c
 // The request's log-probabilities: -1 without them, else the number of top entries; the rules of
 // distributed_llama_b200.apps.api_server.parse_logprobs (throws on anything else).
 int parseLogprobs(const JsonValue &body);
+// The request's `stop` strings (none when absent, null or []): a string or an array of at most kMaxStopStrings strings, each 1 to
+// kMaxStopBytes bytes of UTF-8 after unescaping, without unpaired surrogate escapes. The rules of
+// distributed_llama_b200.apps.api_server.parse_stop (throws on anything else).
+std::vector<std::string> parseStop(const JsonValue &body);
 // One token's response entry {"token", "logprob", "bytes", "top_logprobs"}, formatted as the Python server's json.dumps does.
 std::string logprobEntryJson(const Tokenizer &tok, const TokenLogprobs &e);
 

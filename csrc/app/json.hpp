@@ -16,6 +16,7 @@ struct JsonValue {
     bool b = false;
     double num = 0;
     bool integral = false;   // Number written without a fraction or exponent (`1`, not `1.0`)
+    bool loneSurrogate = false;   // String with a \u escape of an unpaired surrogate (stored as U+FFFD)
     std::string str;
     std::vector<JsonValue> arr;
     std::vector<std::pair<std::string, JsonValue>> obj;   // insertion order kept
@@ -83,7 +84,7 @@ private:
         }
         return v;
     }
-    std::string string() {
+    std::string string(bool *loneSurrogate = nullptr) {
         if (s_[p_] != '"') fail("expected string");
         p_++;
         std::string out;
@@ -109,9 +110,16 @@ private:
                         p_ += 2;
                         const uint32_t lo = hex4();
                         if (lo >= 0xDC00 && lo <= 0xDFFF) cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00);
-                        else { utf8(out, 0xFFFD); cp = lo; }
+                        else {
+                            utf8(out, 0xFFFD);
+                            if (loneSurrogate) *loneSurrogate = true;
+                            cp = lo;
+                        }
                     }
-                    if (cp >= 0xD800 && cp <= 0xDFFF) cp = 0xFFFD;   // unpaired surrogate
+                    if (cp >= 0xD800 && cp <= 0xDFFF) {   // unpaired surrogate
+                        cp = 0xFFFD;
+                        if (loneSurrogate) *loneSurrogate = true;
+                    }
                     utf8(out, cp);
                     break;
                 }
@@ -156,7 +164,7 @@ private:
             }
         } else if (c == '"') {
             v.kind = JsonValue::String;
-            v.str = string();
+            v.str = string(&v.loneSurrogate);
         } else if (eat("true")) { v.kind = JsonValue::Bool; v.b = true; }
         else if (eat("false")) { v.kind = JsonValue::Bool; v.b = false; }
         else if (eat("null")) { v.kind = JsonValue::Null; }

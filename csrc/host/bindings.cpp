@@ -268,4 +268,17 @@ PYBIND11_MODULE(_host, m) {
         .def("is_eos", &EosDetector::isEos)
         .def("get_delta", [](const EosDetector &d) { return asBytes(d.getDelta()); })
         .def("reset", &EosDetector::reset);
+
+    m.attr("MAX_STOP_STRINGS") = kMaxStopStrings;
+    m.attr("MAX_STOP_BYTES") = kMaxStopBytes;
+    py::class_<StopMatcher>(m, "StopMatcher")
+        .def(py::init([](const std::vector<py::bytes> &stops) {
+            std::vector<std::string> s;
+            for (auto &b : stops) s.push_back((std::string)b);
+            return new StopMatcher(std::move(s));
+        }))
+        .def("push", [](StopMatcher &s, py::bytes delta) { return asBytes(s.push((std::string)delta)); })
+        .def("flush", [](StopMatcher &s) { return asBytes(s.flush()); })
+        .def_property_readonly("stopped", &StopMatcher::stopped)
+        .def_property_readonly("held", [](const StopMatcher &s) { return asBytes(s.held()); });
 }

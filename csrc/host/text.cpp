@@ -535,4 +535,43 @@ std::string EosDetector::getDelta() const {
 
 void EosDetector::reset() { buffer_.clear(); }
 
+// ---- stop strings ---------------------------------------------------------------------------------------------------
+
+StopMatcher::StopMatcher(std::vector<std::string> stops) : stops_(std::move(stops)) {
+    for (const std::string &s : stops_)
+        if (s.empty()) throw std::invalid_argument("StopMatcher: empty stop string");
+}
+
+// No occurrence existed before this delta, and every occurrence that ends inside it starts inside the held bytes or the delta
+// (the held bytes are the longest suffix of G that is a proper prefix of a stop string), so searching held + delta is enough.
+std::string StopMatcher::push(const std::string &delta) {
+    if (stopped_) return std::string();
+    std::string text;
+    text.reserve(held_.size() + delta.size());
+    text += held_;
+    text += delta;
+    held_.clear();
+    size_t cut = std::string::npos;
+    for (const std::string &s : stops_) cut = std::min(cut, text.find(s));
+    if (cut != std::string::npos) {
+        stopped_ = true;
+        text.resize(cut);
+        return text;
+    }
+    size_t hold = 0;
+    for (const std::string &s : stops_) {
+        for (size_t l = std::min(text.size(), s.size() - 1); l > hold; l--)
+            if (text[text.size() - l] == s[0] && text.compare(text.size() - l, l, s, 0, l) == 0) { hold = l; break; }
+    }
+    held_.assign(text, text.size() - hold, hold);
+    text.resize(text.size() - hold);
+    return text;
+}
+
+std::string StopMatcher::flush() {
+    std::string out;
+    out.swap(held_);
+    return out;
+}
+
 }  // namespace dl

@@ -186,4 +186,27 @@ private:
     int eosPos_ = -1;
 };
 
+// Limits of a request's `stop` strings (both API servers refuse requests beyond them): they bound the bytes a StopMatcher holds
+// back and its work per token.
+constexpr size_t kMaxStopStrings = 4;
+constexpr size_t kMaxStopBytes = 256;
+
+// A completion's `stop` strings, matched on the bytes of its generated text G (the concatenation of the deltas an EosDetector
+// releases). push() takes the next delta and returns the bytes that can no longer be cut: it holds back the longest suffix of the
+// text not yet returned that is a proper prefix of some stop string. At the first delta that completes an occurrence of any stop
+// string, it returns G up to the start of the earliest-starting occurrence (minus what it returned before) and stopped() turns
+// true; the stop string and everything after it are never returned. flush() returns the held bytes at any other end.
+class StopMatcher {
+public:
+    explicit StopMatcher(std::vector<std::string> stops);   // every string non-empty
+    std::string push(const std::string &delta);
+    std::string flush();
+    bool stopped() const { return stopped_; }
+    const std::string &held() const { return held_; }
+private:
+    std::vector<std::string> stops_;
+    std::string held_;
+    bool stopped_ = false;
+};
+
 }  // namespace dl

@@ -46,6 +46,30 @@ def check_logprobs(k: int, n_ranks: int = 1) -> None:
         raise ValueError("logprobs are not supported under tensor parallelism yet")
 
 
+MAX_STOP_STRINGS = 4   # a request's `stop` strings, each of 1 to MAX_STOP_BYTES bytes (host StopMatcher)
+MAX_STOP_BYTES = 256
+
+
+def check_stop(stop) -> List[bytes]:
+    """Stop strings as the UTF-8 bytes a host StopMatcher matches: None and [] mean none, else a string or a list of at most 4
+    strings of 1 to 256 bytes each. Anything else raises ValueError, as does a string with an unpaired surrogate."""
+    if stop is None:
+        return []
+    items = [stop] if isinstance(stop, str) else stop
+    if not isinstance(items, list) or len(items) > MAX_STOP_STRINGS or not all(isinstance(s, str) for s in items):
+        raise ValueError(f"'stop' must be a string or an array of at most {MAX_STOP_STRINGS} strings")
+    out = []
+    for s in items:
+        try:
+            b = s.encode("utf-8")
+        except UnicodeEncodeError:
+            raise ValueError("'stop' strings must not hold unpaired surrogates") from None
+        if not 1 <= len(b) <= MAX_STOP_BYTES:
+            raise ValueError(f"'stop' strings must be 1 to {MAX_STOP_BYTES} bytes long")
+        out.append(b)
+    return out
+
+
 def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: int, sampler, base_seed: int,
                 on_token: Callable[[int, int], bool], logprobs: Optional[int] = None,
                 on_logprobs: Optional[Callable[[int, tuple], None]] = None) -> List[List[int]]:
@@ -601,25 +625,38 @@ class InferenceSession(TokenSteps):
         self.pos = pos + 1
         return tok
 
-    def generate_choices(self, prompt: str, n: int, max_tokens: int, seed: Optional[int] = None) -> List[str]:
+    def generate_choices(self, prompt: str, n: int, max_tokens: int, seed: Optional[int] = None, stop=None) -> List[str]:
         """n completions of `prompt`, each at most max_tokens tokens (and at most its share of the remaining context, see
         run_choices), with the session's temperature and top-p. Choice i is seeded with choice_seed(seed, i); without a seed
-        the base seed is drawn from the session's sampler, so repeated calls differ. The prompt is prefilled once."""
+        the base seed is drawn from the session's sampler, so repeated calls differ. The prompt is prefilled once.
+        stop: a string or a list of up to 4 strings (check_stop); each choice ends at the token that completes the first
+        occurrence of any of them in its text, which is cut right before that occurrence (host StopMatcher)."""
         assert self.tokenizer is not None
         H = host()
+        stops = check_stop(stop)
         toks = self.tokenizer.encode(prompt, True, True)
         self.prefill(toks[:-1])
         P = self.pos
         decoders = [H.TokenDecoder() for _ in range(n)]
+        matchers = [H.StopMatcher(stops) for _ in range(n)] if stops else None
         pieces: List[List[bytes]] = [[] for _ in range(n)]
 
         def on_token(i: int, tok: int) -> bool:
-            pieces[i].append(decoders[i].decode(self.tokenizer, tok))
+            piece = decoders[i].decode(self.tokenizer, tok)
+            if matchers:
+                pieces[i].append(matchers[i].push(piece))
+                if matchers[i].stopped:
+                    return True
+            else:
+                pieces[i].append(piece)
             return bool(self.tokenizer.is_eos(tok))
 
         base = self.sampler.next_seed() if seed is None else seed
         run_choices(self, toks[-1], P, n, max_tokens, self.engine.seq_len, self.sampler, base, on_token)
         self.pos = P + 1
+        if matchers:
+            for i in range(n):
+                pieces[i].append(matchers[i].flush())
         return [b"".join(p).decode("utf-8", errors="replace") for p in pieces]
 
     # ---- text level ----

@@ -18,8 +18,8 @@ from types import SimpleNamespace
 from typing import Dict, List, Optional, Tuple
 
 from .. import host
-from ..api import (MAX_CHOICES, MAX_TOP_LOGPROBS, ParallelRefused, SlotRequest, SlotScheduler, check_logprobs, parallel_refusal,
-                   run_choices)
+from ..api import (MAX_CHOICES, MAX_TOP_LOGPROBS, ParallelRefused, SlotRequest, SlotScheduler, check_logprobs, check_stop,
+                   parallel_refusal, run_choices)
 from .args import AppArgs, parse_args
 from .cli import make_chat_tools
 from .runtime import AppContext, run_inference_app
@@ -191,6 +191,12 @@ def parse_logprobs(body: dict, n_ranks: int = 1) -> Optional[int]:
     return k
 
 
+def parse_stop(body: dict) -> List[bytes]:
+    """The request's `stop` strings as UTF-8 bytes (api.check_stop): absent, null and [] mean none; a string or an array of at
+    most 4 strings of 1 to 256 bytes each, without unpaired surrogates. Anything else is refused."""
+    return check_stop(body.get("stop"))
+
+
 def _number_field(body: dict, key: str, default):
     v = body.get(key, default)
     if isinstance(v, bool) or not isinstance(v, (int, float)):
@@ -200,7 +206,8 @@ def _number_field(body: dict, key: str, default):
 
 def parse_chat(body, defaults, vocab: int, max_n: int, n_ranks: int) -> SimpleNamespace:
     """A chat completion request: messages as (role, content) pairs, n, stream, max_tokens, temperature, topp, seed (None
-    without one), presence, frequency, bias (parse_controls), top_k, min_p (parse_filters) and logprobs (parse_logprobs).
+    without one), presence, frequency, bias (parse_controls), top_k, min_p (parse_filters), logprobs (parse_logprobs) and stop
+    (parse_stop).
     `defaults` holds the server's --temperature, --topp, penalties and filters; n may not exceed max_n (the slot count under
     --parallel); n_ranks > 1 (tensor parallelism) refuses logprobs. A body that is not an object, `messages` that are not a list of {role, content} objects
     with string values, a number field that is not a number, a negative temperature or a malformed control raise ValueError;
@@ -215,6 +222,7 @@ def parse_chat(body, defaults, vocab: int, max_n: int, n_ranks: int) -> SimpleNa
                                                getattr(defaults, "frequency_penalty", 0.0))
     top_k, min_p = parse_filters(body, getattr(defaults, "top_k", 0), getattr(defaults, "min_p", 0.0))
     logprobs = parse_logprobs(body, n_ranks)
+    stop = parse_stop(body)
     messages = body["messages"]
     if not isinstance(messages, list) or not all(isinstance(m, dict) and isinstance(m.get("role"), str) and
                                                  isinstance(m.get("content"), str) for m in messages):
@@ -226,7 +234,7 @@ def parse_chat(body, defaults, vocab: int, max_n: int, n_ranks: int) -> SimpleNa
                            max_tokens=int(_number_field(body, "max_tokens", -1)), temperature=temperature,
                            topp=float(_number_field(body, "top_p", defaults.topp)),
                            seed=int(_number_field(body, "seed", 0)) if "seed" in body else None,
-                           presence=presence, frequency=frequency, bias=bias, logprobs=logprobs, top_k=top_k, min_p=min_p)
+                           presence=presence, frequency=frequency, bias=bias, logprobs=logprobs, top_k=top_k, min_p=min_p, stop=stop)
 
 
 def logprob_entry(tokenizer, entry) -> dict:
@@ -293,12 +301,14 @@ def choice_json(i: int, content: str, lps: Optional[LogprobsLog]) -> dict:
 
 class ChatResponse:
     """The response to one chat request: its n choices' decoders, stop detectors, texts and log-probability entries, written as
-    stream chunks or as one `cmpl-j0` JSON body. echo: print the tokens' pieces to stdout."""
+    stream chunks or as one `cmpl-j0` JSON body. With `stop` strings each choice also has a host StopMatcher after its detector.
+    echo: print the tokens' pieces to stdout."""
 
     def __init__(self, api: "ApiServer", req: HttpRequest, chat: SimpleNamespace, echo: bool = False):
         H, n = api.H, chat.n
         self.req, self.stream, self.n, self.tok, self.H, self.echo = req, chat.stream, n, api.ctx.tokenizer, H, echo
         self.dets = [H.EosDetector(*api.detector_args) for _ in range(n)]
+        self.matchers = [H.StopMatcher(chat.stop) for _ in range(n)] if chat.stop else None
         self.decoders = [H.TokenDecoder() for _ in range(n)]
         self.lps = LogprobsLog(self.tok, n) if chat.logprobs is not None else None
         self.buffers = [""] * n
@@ -329,19 +339,37 @@ class ChatResponse:
             self.lps.consumed(i, kind == H.EOS)
         if kind in (H.NOT_EOS, H.EOS):
             delta = self.dets[i].get_delta()
+            if self.matchers:
+                delta = self.matchers[i].push(delta)
             if delta:
                 d = delta.decode("utf-8", errors="replace")
                 if self.stream:
                     self._chunk(i, d)
                 self.buffers[i] += d
             self.dets[i].reset()
-        return kind == H.EOS
+        return kind == H.EOS or self.stopped(i)
+
+    def stopped(self, i: int) -> bool:
+        """Choice i ended at a stop string."""
+        return bool(self.matchers) and self.matchers[i].stopped
+
+    def text(self, i: int) -> str:
+        """Choice i's content so far, bytes held back by its matcher included."""
+        if not self.matchers:
+            return self.buffers[i]
+        return self.buffers[i] + self.matchers[i].held.decode("utf-8", errors="replace")
 
     def finish(self, out: List[List[int]], n_prompt: int) -> None:
-        """Every choice is done (out[i]: choice i's tokens): the stop chunks and [DONE], or the JSON body."""
-        if self.stream:
-            for i in range(self.n):
+        """Every choice is done (out[i]: choice i's tokens): the stop chunks and [DONE], or the JSON body. Bytes a matcher still
+        holds (a choice that ended another way) join the text, in one delta chunk before the stop chunk of a stream."""
+        for i in range(self.n):
+            rest = self.matchers[i].flush().decode("utf-8", errors="replace") if self.matchers else ""
+            self.buffers[i] += rest
+            if self.stream:
+                if rest:
+                    self._chunk(i, rest)
                 write_stream_finish(self.req, i, self.lps)
+        if self.stream:
             self.req.write_stream_chunk("data: [DONE]")
             self.req.write_stream_end()
         else:
@@ -390,8 +418,9 @@ class ApiServer:
 
     def complete(self, req: HttpRequest):
         """n completions of one prompt (api.run_choices; n = 1 without `n`): the prompt is prefilled once. After one completion
-        the cache keeps its answer too; after several it keeps only the prompt messages, so a follow-up that quotes any one
-        choice reuses the prompt. The request's sampling settings stay with the server's sampler."""
+        the cache keeps its answer too; after several, or after one cut at a stop string (its KV rows hold tokens past the cut),
+        it keeps only the prompt messages, so a follow-up that quotes any one choice reuses the prompt. The request's sampling
+        settings stay with the server's sampler."""
         ctx = self.ctx
         inf, smp, seq_len = ctx.inference, ctx.sampler, ctx.header.seq_len
         chat = parse_chat(req.json, ctx.args, smp.vocab_size, MAX_CHOICES, getattr(getattr(inf, "comm", None), "world_size", 1))
@@ -409,8 +438,8 @@ class ApiServer:
         inf.prefill(prefill, start)
         out = run_choices(inf, token, P, chat.n, chat.max_tokens, seq_len, smp, base_seed, resp.on_token,
                           **({"logprobs": chat.logprobs, "on_logprobs": resp.on_logprobs} if resp.lps else {}))
-        if chat.n == 1:
-            remember_answer(self.cache, P, out[0], resp.buffers[0], seq_len)
+        if chat.n == 1 and not resp.stopped(0):
+            remember_answer(self.cache, P, out[0], resp.text(0), seq_len)
         resp.finish(out, n_prompt)
         print("🔶" if chat.n == 1 else f"({chat.n} choices)🔶")
 
@@ -435,8 +464,8 @@ class ApiServer:
             on_logprobs, on_token = resp.on_logprobs, resp.on_token
 
             def finish(self, out, slots, P):
-                if chat.n == 1:
-                    remember_answer(caches[slots[0]], P, out[0], resp.buffers[0], slot_len)
+                if chat.n == 1 and not resp.stopped(0):
+                    remember_answer(caches[slots[0]], P, out[0], resp.text(0), slot_len)
                 for s in slots[1:]:   # they hold a copy of the prompt rows
                     caches[s].items = list(caches[slots[0]].items)
                 resp.finish(out, self.n_prompt)
