@@ -255,6 +255,13 @@ DL_EXPORT int dl_rope_kv_q80(float *qkv, uint32_t qkvStride, const int *pos, con
     return dl::launchRopeKv(a, nb, stream, false);
 }
 
+// Greedy token of one logits row (tests/test_gpu_gemv.py): the lowest index among the maxima of logits[0, vocab) into tokenOut[0],
+// pos[0] += 1 and history[pos] = token while pos < historyCap (history may be null).
+DL_EXPORT int dl_argmax_advance(const float *logits, uint32_t vocab, int *tokenOut, int *pos, int *history, uint32_t historyCap,
+                                cudaStream_t stream) {
+    return dl::launchArgmaxAdvance(logits, vocab, tokenOut, pos, history, historyCap, stream, false);
+}
+
 // Router of T tokens (tests/test_gpu_moe.py): logits [T][nExperts], expertIdx / expertWeight [T][k]; counter [T] zeroed, self-resetting.
 DL_EXPORT int dl_moe_router(const float *x, const float *normW, const float *gate, float eps, uint32_t dim, uint32_t nExperts, uint32_t k,
                             float *logits, unsigned int *counter, int *expertIdx, float *expertWeight, int T, cudaStream_t stream) {

@@ -395,14 +395,22 @@ int gemvDense(int wtype, int pro, int epi, int nb, GemvArgs a, int numSms, cudaS
 
 }  // namespace dl
 
-// Standalone entry point (tests / microbenchmarks).
+// Standalone entry points (tests / microbenchmarks). act: gate activation of EPI_SWIGLU (0 = SiLU, 1 = GELU).
 DL_EXPORT int dl_gemv_dense(int wtype, int pro, int epi, int nb, const void *w, uint32_t d, uint32_t n, const float *in,
                             uint32_t inStride, const float *normW, float eps, float *out, uint32_t outStride, int numSms,
-                            cudaStream_t stream, int pdl) {
+                            cudaStream_t stream, int pdl, uint32_t act) {
+    const dl::HiddenActScope scope(act);
     dl::GemvArgs a{};
     a.qs = (const uint32_t *)w;
     a.d = d; a.n = n;
     a.in = in; a.normW = normW; a.eps = eps;
     a.out = out; a.inStride = inStride; a.outStride = outStride;
     return dl::gemvDense(wtype, pro, epi, nb, a, numSms, stream, pdl != 0);
+}
+
+// Shared memory a dense GEMV launch of nb tokens over a [d][n] matrix asks for (launches nothing); above 227 KB it is refused.
+DL_EXPORT uint64_t dl_gemv_dense_smem_bytes(uint32_t d, uint32_t n, int nb, int numSms) {
+    const uint32_t nPairs = d / 2;
+    const uint32_t grid = nPairs < (uint32_t)numSms ? nPairs : (uint32_t)numSms;
+    return dl::gemvDenseSmemBytes(n, 2 * ((nPairs + grid - 1) / grid), nb);
 }

@@ -256,14 +256,11 @@ static int launchGemv(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_
     return 0;
 }
 
-int gemvQ40(int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t stream, bool pdl) {
-    if (a.d % 2 || a.n % 32 || (a.n / 4) % 8) return -1;
+int launchGemvQ40Ldg(int pro, int epi, int nb, GemvArgs a, const GemvQ40Plan &p, cudaStream_t stream, bool pdl) {
     a.act = gHiddenAct;
-    const uint32_t nPairs = a.d / 2;
-    const int grid = (int)(nPairs < (uint32_t)numSms ? nPairs : (uint32_t)numSms);
-    a.maxTileRows = 2 * ((nPairs + grid - 1) / grid);
-    const size_t smemBytes = gemvSmemBytes(a.n, a.maxTileRows, nb);
-    if (smemBytes > 227 * 1024) return -2;
+    a.maxTileRows = p.maxTileRows;
+    const int grid = (int)p.grid;
+    const size_t smemBytes = p.smemBytes;
 #define DL_GEMV_CASE(P, E, N) \
     if (pro == P && epi == E && nb == N) return launchGemv<P, E, N>(a, grid, smemBytes, stream, pdl);
 #define DL_GEMV_NB(P, E) DL_GEMV_CASE(P, E, 1) DL_GEMV_CASE(P, E, 2) DL_GEMV_CASE(P, E, 4) DL_GEMV_CASE(P, E, 8)
@@ -279,17 +276,46 @@ int gemvQ40(int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t strea
 
 }  // namespace dl
 
-// Standalone entry point (tests / microbenchmarks). Engine code calls dl::gemvQ40 directly.
+// Standalone entry points (tests / microbenchmarks). Engine code calls dl::gemvQ40Run directly.
+// impl: 0 = auto, 1 = per-thread loads, 2 = TMA ring (returns 1 when the shape does not fit it). act: gate activation of
+// EPI_SWIGLU (0 = SiLU, 1 = GELU).
 DL_EXPORT int dl_gemv_q40(int pro, int epi, int nb, const void *qs, const void *scales, uint32_t d, uint32_t n,
                           const float *in, uint32_t inStride, const float *normW, float eps, float *out,
-                          uint32_t outStride, int numSms, cudaStream_t stream, int pdl, int impl) {
+                          uint32_t outStride, int numSms, cudaStream_t stream, int pdl, int impl, uint32_t act) {
+    const dl::HiddenActScope scope(act);
     dl::GemvArgs a{};
     a.qs = (const uint32_t *)qs;
     a.scales = (const __half *)scales;
     a.d = d; a.n = n;
     a.in = in; a.normW = normW; a.eps = eps;
     a.out = out; a.inStride = inStride; a.outStride = outStride;
-    if (impl == 1) return dl::gemvQ40(pro, epi, nb, a, numSms, stream, pdl != 0);
-    if (impl == 2) return dl::gemvQ40Tma(pro, epi, nb, a, numSms, stream, pdl != 0);
-    return dl::gemvQ40Auto(pro, epi, nb, a, numSms, stream, pdl != 0);
+    return dl::gemvQ40Run(pro, epi, nb, a, numSms, stream, pdl != 0, impl);
+}
+
+// The plan dl_gemv_q40 follows for a one-rank launch (launches and allocates nothing). out[8]: rc, kernel, grid, maxTileRows,
+// stageRows, nStages, shared-memory bytes, launches the batch is split into.
+DL_EXPORT int dl_gemv_q40_plan(int pro, int epi, int nb, uint32_t d, uint32_t n, int numSms, int impl, int *out) {
+    const dl::GemvQ40Plan p = dl::planGemvQ40(pro, epi, nb, d, n, numSms, impl, true);
+    const int v[8] = {p.rc, p.kernel, (int)p.grid, (int)p.maxTileRows, (int)p.stageRows, (int)p.nStages, (int)p.smemBytes, (int)p.launches};
+    for (int i = 0; i < 8; i++) out[i] = v[i];
+    return p.rc;
+}
+
+// One-rank fused logits + greedy token (RMSNORM prologue, EPI_ARGMAX epilogue of the TMA kernel, one token): logits into out,
+// the lowest-index maximum among global rows rowOffsetGlobal + r < vocabLimit (0: no limit) into tokenOut[0], pos[0] += 1 and
+// history[pos] = token while pos < historyCap. argVal / argIdx hold one entry per CTA (numSms suffice); argCounter starts at 0
+// and is left at 0. Returns 1 when the shape does not fit the TMA kernel.
+DL_EXPORT int dl_gemv_q40_argmax(const void *qs, const void *scales, uint32_t d, uint32_t n, const float *in, const float *normW, float eps,
+                                 float *out, float *argVal, int *argIdx, unsigned int *argCounter, int *tokenOut, int *pos, int *history,
+                                 uint32_t historyCap, uint32_t rowOffsetGlobal, uint32_t vocabLimit, int numSms, cudaStream_t stream) {
+    dl::GemvArgs a{};
+    a.qs = (const uint32_t *)qs;
+    a.scales = (const __half *)scales;
+    a.d = d; a.n = n;
+    a.in = in; a.inStride = n; a.normW = normW; a.eps = eps;
+    a.out = out; a.outStride = d;
+    a.argVal = argVal; a.argIdx = argIdx; a.argCounter = argCounter;
+    a.tokenOut = tokenOut; a.posInOut = pos; a.history = history; a.historyCap = historyCap;
+    a.rowOffsetGlobal = rowOffsetGlobal; a.vocabLimit = vocabLimit;
+    return dl::gemvQ40Tma(dl::PRO_RMSNORM, dl::EPI_ARGMAX_, 1, a, numSms, stream, false);
 }

@@ -170,7 +170,7 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
     const uint32_t stepsPerFullStage = (SR / kRowsPerStep) * nseg;
     const uint32_t rotInc = stepsPerFullStage % kConsumerWarps;
     const uint32_t gInc = kConsumerWarps / nseg, segInc = kConsumerWarps - gInc * nseg;
-    const uint32_t recipNseg = 65536u / nseg + 1u;   // (s * recip) >> 16 == s / nseg for s < 16, nseg <= 16
+    const uint32_t recipNseg = 65536u / nseg + 1u;   // (s * recip) >> 16 == s / nseg for s < 16 while s * nseg < 2^16 (nseg < 4096)
     uint32_t st = 0, par = 0, rot = 0;
     for (uint32_t f = 0; active && f < nFills; f++) {
         const uint32_t r0 = f * SR;
@@ -419,6 +419,85 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
     traceStamp(a.trace, 3);
 }
 
+// TMA-ring plan of one launch; rc 1 when the shape cannot use the TMA path.
+static GemvQ40Plan planTma(int pro, int epi, int nb, uint32_t d, uint32_t n, int numSms, uint32_t moeCtasPerSlot, uint32_t kActive) {
+    GemvQ40Plan p{};
+    p.launches = 1;
+    if (d % 2 || n % 128) { p.rc = 1; return p; }   // bulk copies need 16-byte aligned row starts for the fp16 scale rows
+    const uint32_t nblk = n / 32, nseg = (nblk + 31) / 32;
+    const uint32_t nPairs = d / 2;
+    uint32_t grid = nPairs < (uint32_t)numSms ? nPairs : (uint32_t)numSms;
+    uint32_t tilesPerMatrix = grid;
+    if (moeCtasPerSlot) {
+        if (nb != 1) { p.rc = -4; return p; }
+        tilesPerMatrix = moeCtasPerSlot;
+        grid = moeCtasPerSlot * kActive;
+    }
+    const uint32_t maxTileRows = 2 * ((nPairs + tilesPerMatrix - 1) / tilesPerMatrix);
+    const uint32_t rowBytes = nblk * 18;
+    // a stage should hold >= 16 steps (one per consumer warp) so the per-stage barrier traffic is amortised
+    uint32_t sr = (64 + nseg - 1) / nseg;
+    sr = (sr + 3) / 4 * 4;
+    while (sr > 4 && sr * rowBytes > 36 * 1024) sr -= 4;
+    if (sr * rowBytes > 48 * 1024) { p.rc = 1; return p; }   // rows too wide for a 4-row stage: per-thread-load kernel handles it
+    if (sr > 64) sr = 64;
+    const uint32_t stageBytes = (sr * rowBytes + 127) / 128 * 128;
+    const size_t fixedBytes = (size_t)nb * nblk * (16 + 16 + 4 + 4) + (size_t)(maxTileRows + 2) * nseg * nb * 4 + 32 * 4 +
+                              2 * kMaxStages * 8 + 256;
+    const size_t budget = (nb == 1 ? 112 : 226) * 1024;   // nb == 1: leave room for the next kernel's CTA on the same SM
+    if (fixedBytes + stageBytes > budget) { p.rc = 1; return p; }
+    uint32_t stages = (uint32_t)((budget - fixedBytes) / stageBytes);
+    const uint32_t need = (maxTileRows + sr - 1) / sr;
+    if (stages > need) stages = need;
+    if (stages > kMaxStages) stages = kMaxStages;
+    if (stages < 1) { p.rc = 1; return p; }
+    const bool inst = ((pro == PRO_RMSNORM && (epi == EPI_STORE || epi == EPI_SWIGLU)) || (pro == PRO_PLAIN && (epi == EPI_RESIDUAL || epi == EPI_STORE)))
+                          ? (nb == 1 || nb == 2 || nb == 4 || nb == 8)
+                          : nb == 1 && ((pro == PRO_PLAIN && (epi == EPI_SWIGLU || epi == EPI_MOE_DOWN)) || (pro == PRO_RMSNORM && epi == EPI_ARGMAX));
+    if (!inst) { p.rc = -3; return p; }
+    p.kernel = 2;
+    p.grid = grid;
+    p.maxTileRows = maxTileRows;
+    p.stageRows = sr;
+    p.nStages = stages;
+    p.smemBytes = (uint32_t)(fixedBytes + (size_t)stages * stageBytes);
+    return p;
+}
+
+GemvQ40Plan planGemvQ40(int pro, int epi, int nb, uint32_t d, uint32_t n, int numSms, int impl, bool split, uint32_t moeCtasPerSlot,
+                        uint32_t kActive) {
+    if (impl != 1) {
+        const GemvQ40Plan t = planTma(pro, epi, nb, d, n, numSms, moeCtasPerSlot, kActive);
+        if (t.rc != 1 || impl == 2) return t;
+    }
+    GemvQ40Plan p{};
+    p.launches = 1;
+    if (d % 2 || n % 32 || (n / 4) % 8) { p.rc = -1; return p; }
+    const uint32_t nPairs = d / 2;
+    p.grid = nPairs < (uint32_t)numSms ? nPairs : (uint32_t)numSms;
+    p.maxTileRows = 2 * ((nPairs + p.grid - 1) / p.grid);
+    const size_t smemBytes = gemvSmemBytes(n, p.maxTileRows, nb);
+    if (smemBytes > 227 * 1024) {
+        // no kernel holds nb tokens: the tokens of STORE / RESIDUAL / SWIGLU are independent, so two launches of nb / 2 are exact
+        if (split && nb > 1 && moeCtasPerSlot == 0 && (epi == EPI_STORE || epi == EPI_RESIDUAL || epi == EPI_SWIGLU)) {
+            GemvQ40Plan h = planGemvQ40(pro, epi, nb / 2, d, n, numSms, impl, split);
+            if (h.rc == 0) {
+                h.launches *= 2;
+                return h;
+            }
+        }
+        p.rc = -2;
+        return p;
+    }
+    const bool inst = (pro == PRO_RMSNORM && (epi == EPI_STORE || epi == EPI_SWIGLU)) || (pro == PRO_PLAIN && (epi == EPI_RESIDUAL || epi == EPI_STORE))
+                          ? (nb == 1 || nb == 2 || nb == 4 || nb == 8)
+                          : nb == 1 && pro == PRO_PLAIN && epi == EPI_SWIGLU;
+    if (!inst) { p.rc = -3; return p; }
+    p.kernel = 1;
+    p.smemBytes = (uint32_t)smemBytes;
+    return p;
+}
+
 template <int PRO, int EPI, int NB>
 static int launchTma(const GemvArgs &a, const TmaGemvGeom &geo, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
     auto kernel = gemvQ40TmaKernel<PRO, EPI, NB>;
@@ -441,42 +520,16 @@ static int launchTma(const GemvArgs &a, const TmaGemvGeom &geo, int grid, size_t
     return 0;
 }
 
-// Returns 1 when the shape cannot use the TMA path (caller falls back), <0 on errors, 0 on success.
-int gemvQ40Tma(int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t stream, bool pdl) {
-    if (a.d % 2 || a.n % 128) return 1;   // bulk copies need 16-byte aligned row starts for the fp16 scale rows
+int launchGemvQ40Tma(int pro, int epi, int nb, GemvArgs a, const GemvQ40Plan &p, cudaStream_t stream, bool pdl) {
     a.act = gHiddenAct;
     if (a.vocabLimit == 0) a.vocabLimit = 0xffffffffu;
-    const uint32_t nblk = a.n / 32, nseg = (nblk + 31) / 32;
-    const uint32_t nPairs = a.d / 2;
-    int grid = (int)(nPairs < (uint32_t)numSms ? nPairs : (uint32_t)numSms);
-    uint32_t tilesPerMatrix = (uint32_t)grid;
-    if (a.moeCtasPerSlot) {
-        if (nb != 1) return -4;
-        tilesPerMatrix = a.moeCtasPerSlot;
-        grid = (int)(a.moeCtasPerSlot * a.kActive);
-    }
     TmaGemvGeom geo{};
-    geo.maxTileRows = 2 * ((nPairs + tilesPerMatrix - 1) / tilesPerMatrix);
-    const uint32_t rowBytes = nblk * 18;
-    // a stage should hold >= 16 steps (one per consumer warp) so the per-stage barrier traffic is amortised
-    uint32_t sr = (64 + nseg - 1) / nseg;
-    sr = (sr + 3) / 4 * 4;
-    while (sr > 4 && sr * rowBytes > 36 * 1024) sr -= 4;
-    if (sr * rowBytes > 48 * 1024) return 1;   // rows too wide for a 4-row stage: per-thread-load kernel handles it
-    if (sr > 64) sr = 64;
-    geo.stageRows = sr;
-    geo.stageBytes = (sr * rowBytes + 127) / 128 * 128;
-    const size_t fixedBytes = (size_t)nb * nblk * (16 + 16 + 4 + 4) + (size_t)(geo.maxTileRows + 2) * nseg * nb * 4 + 32 * 4 +
-                              2 * kMaxStages * 8 + 256;
-    const size_t budget = (nb == 1 ? 112 : 226) * 1024;   // nb == 1: leave room for the next kernel's CTA on the same SM
-    if (fixedBytes + geo.stageBytes > budget) return 1;
-    uint32_t stages = (uint32_t)((budget - fixedBytes) / geo.stageBytes);
-    const uint32_t need = (geo.maxTileRows + sr - 1) / sr;
-    if (stages > need) stages = need;
-    if (stages > kMaxStages) stages = kMaxStages;
-    if (stages < 1) return 1;
-    geo.nStages = stages;
-    const size_t smemBytes = fixedBytes + (size_t)stages * geo.stageBytes;
+    geo.maxTileRows = p.maxTileRows;
+    geo.stageRows = p.stageRows;
+    geo.nStages = p.nStages;
+    geo.stageBytes = (p.stageRows * (a.n / 32) * 18 + 127) / 128 * 128;
+    const int grid = (int)p.grid;
+    const size_t smemBytes = p.smemBytes;
 #define DL_TMA_CASE(P, E, N) \
     if (pro == P && epi == E && nb == N) return launchTma<P, E, N>(a, geo, grid, smemBytes, stream, pdl);
 #define DL_TMA_NB(P, E) DL_TMA_CASE(P, E, 1) DL_TMA_CASE(P, E, 2) DL_TMA_CASE(P, E, 4) DL_TMA_CASE(P, E, 8)
@@ -490,6 +543,21 @@ int gemvQ40Tma(int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t st
 #undef DL_TMA_NB
 #undef DL_TMA_CASE
     return -3;
+}
+
+int gemvQ40Run(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl, int impl) {
+    const bool split = a.ar.nRanks <= 1 && a.expertIdx == nullptr;
+    const GemvQ40Plan p = planGemvQ40(pro, epi, nb, a.d, a.n, numSms, impl, split, a.moeCtasPerSlot, a.kActive);
+    if (p.rc != 0) return p.rc;
+    const int sub = nb / (int)p.launches;
+    for (uint32_t i = 0; i < p.launches; i++) {
+        GemvArgs s = a;
+        s.in = a.in + (size_t)i * sub * a.inStride;
+        s.out = a.out + (size_t)i * sub * a.outStride;
+        const int r = p.kernel == 2 ? launchGemvQ40Tma(pro, epi, sub, s, p, stream, pdl) : launchGemvQ40Ldg(pro, epi, sub, s, p, stream, pdl);
+        if (r != 0) return r;
+    }
+    return 0;
 }
 
 }  // namespace dl

@@ -60,15 +60,38 @@ struct GemvArgs {
     uint32_t act;             // gate activation of EPI_SWIGLU (filled in by the launchers from gHiddenAct)
     uint32_t vocabLimit;      // EPI_ARGMAX: rows (global index) >= vocabLimit never win (model vocabulary padded beyond the tokenizer's); 0 = no limit
 };
-int gemvQ40(int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t stream, bool pdl);      // per-thread loads (fallback)
-int gemvQ40Tma(int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t stream, bool pdl);   // TMA ring; returns 1 if shape unsupported
+// What a q40 GEMV launch runs (planGemvQ40, gemv_q40_tma.cu). impl: 0 = TMA ring if the shape fits it, else per-thread loads;
+// 1 = per-thread loads only; 2 = TMA ring only (rc 1: the shape does not fit it).
+// When no kernel fits nb tokens in shared memory and `split` is set, the batch runs as `launches` consecutive launches of
+// nb / launches tokens each; the other fields describe one such launch. rc < 0: the launch is refused.
+struct GemvQ40Plan {
+    int rc, kernel;                 // kernel: 1 = per-thread loads (gemvQ40Kernel), 2 = TMA ring (gemvQ40TmaKernel)
+    uint32_t grid, maxTileRows;
+    uint32_t stageRows, nStages;    // TMA ring geometry (0 for kernel 1)
+    uint32_t smemBytes, launches;
+};
+// moeCtasPerSlot / kActive: mixture-of-experts launches (TMA only, nb == 1): row tiles per routing slot and slots.
+GemvQ40Plan planGemvQ40(int pro, int epi, int nb, uint32_t d, uint32_t n, int numSms, int impl, bool split,
+                        uint32_t moeCtasPerSlot = 0, uint32_t kActive = 0);
+size_t gemvSmemBytes(uint32_t n, uint32_t maxTileRows, int nb);   // per-thread-load kernel
+int launchGemvQ40Ldg(int pro, int epi, int nb, GemvArgs a, const GemvQ40Plan &p, cudaStream_t stream, bool pdl);
+int launchGemvQ40Tma(int pro, int epi, int nb, GemvArgs a, const GemvQ40Plan &p, cudaStream_t stream, bool pdl);
+// Plans and launches. A batch is split only on one rank (ar.nRanks <= 1), outside expert launches and for the STORE, RESIDUAL and
+// SWIGLU epilogues, whose tokens are independent; the in-kernel all-reduce indexes its slots per token.
+int gemvQ40Run(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl, int impl);
+inline int gemvQ40(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl) {       // per-thread loads
+    return gemvQ40Run(pro, epi, nb, a, numSms, stream, pdl, 1);
+}
+inline int gemvQ40Tma(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl) {    // 1: shape unsupported
+    return gemvQ40Run(pro, epi, nb, a, numSms, stream, pdl, 2);
+}
 inline int gemvQ40Auto(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl) {
-    const int r = gemvQ40Tma(pro, epi, nb, a, numSms, stream, pdl);
-    return r == 1 ? gemvQ40(pro, epi, nb, a, numSms, stream, pdl) : r;
+    return gemvQ40Run(pro, epi, nb, a, numSms, stream, pdl, 0);
 }
 
 // f32 / f16 weight files (gemv_dense.cu): wtype 1 = f32, 2 = f16; a.qs is the row-major [d][n] matrix
 int gemvDense(int wtype, int pro, int epi, int nb, GemvArgs a, int numSms, cudaStream_t stream, bool pdl);
+size_t gemvDenseSmemBytes(uint32_t n, uint32_t maxTileRows, int nb);
 
 // ---- KV-cache storage --------------------------------------------------------------------------------------------------------------
 // Every cache below is head-major [nKvHeads][seqLen][headDim]. Its rows are bf16 (kScale / vScale null), or q80 (EngineConfig::kvType

@@ -50,10 +50,18 @@ def lib() -> C.CDLL:
     L.dl_repack_q40.restype = i32
     L.dl_dequant_device_q40.argtypes = [vp, vp, u32, u32, vp, vp]
     L.dl_dequant_device_q40.restype = i32
-    L.dl_gemv_q40.argtypes = [i32, i32, i32, vp, vp, u32, u32, vp, u32, vp, f32, vp, u32, i32, vp, i32, i32]
+    L.dl_gemv_q40.argtypes = [i32, i32, i32, vp, vp, u32, u32, vp, u32, vp, f32, vp, u32, i32, vp, i32, i32, u32]
     L.dl_gemv_q40.restype = i32
-    L.dl_gemv_dense.argtypes = [i32, i32, i32, i32, vp, u32, u32, vp, u32, vp, f32, vp, u32, i32, vp, i32]
+    L.dl_gemv_q40_plan.argtypes = [i32, i32, i32, u32, u32, i32, i32, C.POINTER(C.c_int)]
+    L.dl_gemv_q40_plan.restype = i32
+    L.dl_gemv_q40_argmax.argtypes = [vp, vp, u32, u32, vp, vp, f32, vp, vp, vp, vp, vp, vp, vp, u32, u32, u32, i32, vp]
+    L.dl_gemv_q40_argmax.restype = i32
+    L.dl_argmax_advance.argtypes = [vp, u32, vp, vp, vp, u32, vp]
+    L.dl_argmax_advance.restype = i32
+    L.dl_gemv_dense.argtypes = [i32, i32, i32, i32, vp, u32, u32, vp, u32, vp, f32, vp, u32, i32, vp, i32, u32]
     L.dl_gemv_dense.restype = i32
+    L.dl_gemv_dense_smem_bytes.argtypes = [u32, u32, i32, i32]
+    L.dl_gemv_dense_smem_bytes.restype = u64
     L.dl_gemm_q40_tc.argtypes = [i32, vp, vp, u32, u32, vp, u32, u32, vp, u32, i32, u32, vp, i32, i32]
     L.dl_gemm_q40_tc.restype = i32
     L.dl_gemm_q40_tc_plan.argtypes = [i32, u32, u32, u32, u32, i32, i32, C.POINTER(C.c_int)]
@@ -254,5 +262,5 @@ def decode_logprobs(words) -> tuple:
     return w[0], f(w[1]), [(w[4 + 2 * j], f(w[5 + 2 * j])) for j in range(k)]
 
 PRO_RMSNORM, PRO_PLAIN = 0, 1
-EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU = 0, 1, 2
+EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU, EPI_ARGMAX = 0, 1, 2, 3
 GEPI_STORE_F32, GEPI_RESIDUAL, GEPI_SWIGLU_BF16, GEPI_STORE_BF16 = 0, 1, 2, 3

@@ -57,15 +57,20 @@ class DeviceDense:
 
 
 def gemv_dense(w: DeviceDense, x: torch.Tensor, *, pro: int, epi: int, out: torch.Tensor, norm_w: Optional[torch.Tensor] = None,
-               eps: float = 1e-5, num_sms: int = 0, pdl: bool = False) -> torch.Tensor:
+               eps: float = 1e-5, num_sms: int = 0, pdl: bool = False, act_fn: int = 0) -> torch.Tensor:
     """Dense-weight counterpart of gemv_q40 (f32 activations, no q80 round trip)."""
     nb = x.shape[0]
     if num_sms == 0:
         num_sms = torch.cuda.get_device_properties(x.device).multi_processor_count
     cl.check(cl.lib().dl_gemv_dense(w.wtype, pro, epi, nb, w.data.data_ptr(), w.d, w.n, x.data_ptr(), x.stride(0),
                                     norm_w.data_ptr() if norm_w is not None else None, eps, out.data_ptr(), out.stride(0),
-                                    num_sms, cl.stream_ptr(), 1 if pdl else 0), "gemv_dense")
+                                    num_sms, cl.stream_ptr(), 1 if pdl else 0, act_fn), "gemv_dense")
     return out
+
+
+def gemv_dense_smem_bytes(d: int, n: int, nb: int, num_sms: int) -> int:
+    """Shared memory of a dense GEMV launch of nb tokens over a [d][n] matrix; the kernel refuses more than 227 KB."""
+    return cl.lib().dl_gemv_dense_smem_bytes(d, n, nb, num_sms)
 
 
 def repack_q40(raw: torch.Tensor, rows: int, n_cols: int, dst: DeviceQ40, *, src_row_pitch: Optional[int] = None,
@@ -80,16 +85,66 @@ def repack_q40(raw: torch.Tensor, rows: int, n_cols: int, dst: DeviceQ40, *, src
              "repack_q40")
 
 
+GEMV_IMPLS = {"auto": 0, "ldg": 1, "tma": 2}
+
+
 def gemv_q40(w: DeviceQ40, x: torch.Tensor, *, pro: int, epi: int, out: torch.Tensor, norm_w: Optional[torch.Tensor] = None,
-             eps: float = 1e-5, num_sms: int = 0, pdl: bool = False, impl: str = "auto") -> torch.Tensor:
-    """x: f32 [nb, n]; out: f32 [nb, d] (STORE / RESIDUAL in place) or [nb, d/2] (SWIGLU)."""
+             eps: float = 1e-5, num_sms: int = 0, pdl: bool = False, impl: str = "auto", act_fn: int = 0) -> torch.Tensor:
+    """x: f32 [nb, n]; out: f32 [nb, d] (STORE / RESIDUAL in place) or [nb, d/2] (SWIGLU). impl "tma" raises (code 1) when the
+    shape does not fit the TMA kernel. act_fn: gate activation of the SwiGLU epilogue (0 = SiLU, 1 = tanh-GELU)."""
     nb = x.shape[0]
     if num_sms == 0:
         num_sms = torch.cuda.get_device_properties(x.device).multi_processor_count
     cl.check(cl.lib().dl_gemv_q40(pro, epi, nb, w.qs.data_ptr(), w.scales.data_ptr(), w.d, w.n, x.data_ptr(), x.stride(0),
                                   norm_w.data_ptr() if norm_w is not None else None, eps, out.data_ptr(), out.stride(0),
-                                  num_sms, cl.stream_ptr(), 1 if pdl else 0, {"auto": 0, "ldg": 1, "tma": 2}[impl]), "gemv_q40")
+                                  num_sms, cl.stream_ptr(), 1 if pdl else 0, GEMV_IMPLS[impl], act_fn), "gemv_q40")
     return out
+
+
+@dataclass(frozen=True)
+class GemvPlan:
+    """What gemv_q40 runs for a one-rank launch (dl_gemv_q40_plan). kernel: 1 per-thread loads ("ldg"), 2 TMA ring ("tma");
+    stage_rows / n_stages: the ring (0 for kernel 1); launches > 1: the batch runs as that many launches of nb / launches tokens,
+    the other fields describing one of them. rc 1: impl "tma" and the shape does not fit it; rc < 0: refused."""
+    rc: int
+    kernel: int
+    grid: int
+    max_tile_rows: int
+    stage_rows: int
+    n_stages: int
+    smem_bytes: int
+    launches: int
+
+
+def gemv_q40_plan(pro: int, epi: int, nb: int, d: int, n: int, *, num_sms: int, impl: str = "auto") -> GemvPlan:
+    """The dispatch decision of gemv_q40; launches nothing."""
+    out = (ctypes.c_int * 8)()
+    cl.lib().dl_gemv_q40_plan(pro, epi, nb, d, n, num_sms, GEMV_IMPLS[impl], out)
+    return GemvPlan(*out)
+
+
+def gemv_q40_argmax(w: DeviceQ40, x: torch.Tensor, *, norm_w: torch.Tensor, eps: float, out: torch.Tensor, arg_val: torch.Tensor,
+                    arg_idx: torch.Tensor, arg_counter: torch.Tensor, token: torch.Tensor, pos: torch.Tensor,
+                    history: Optional[torch.Tensor], history_cap: int, row_offset: int = 0, vocab_limit: int = 0,
+                    num_sms: int = 0) -> None:
+    """Fused logits + greedy token of one token on the TMA kernel: out [d] = logits of rmsnorm(x) [n]; token[0] = lowest-index
+    maximum among rows with row_offset + r < vocab_limit (0: all); pos[0] += 1; history[pos] = token while pos < history_cap.
+    arg_val / arg_idx: one entry per CTA; arg_counter: zero, left at zero."""
+    if num_sms == 0:
+        num_sms = torch.cuda.get_device_properties(x.device).multi_processor_count
+    cl.check(cl.lib().dl_gemv_q40_argmax(w.qs.data_ptr(), w.scales.data_ptr(), w.d, w.n, x.data_ptr(), norm_w.data_ptr(), eps, out.data_ptr(),
+                                         arg_val.data_ptr(), arg_idx.data_ptr(), arg_counter.data_ptr(), token.data_ptr(), pos.data_ptr(),
+                                         history.data_ptr() if history is not None else None, history_cap, row_offset, vocab_limit,
+                                         num_sms, cl.stream_ptr()), "gemv_q40_argmax")
+
+
+def argmax_advance(logits: torch.Tensor, vocab: int, token: torch.Tensor, pos: torch.Tensor, history: Optional[torch.Tensor],
+                   history_cap: int) -> None:
+    """Stand-alone greedy token: token[0] = lowest index among the maxima of logits[:vocab]; pos[0] += 1; history[pos] = token
+    while pos < history_cap."""
+    cl.check(cl.lib().dl_argmax_advance(logits.data_ptr(), vocab, token.data_ptr(), pos.data_ptr(),
+                                        history.data_ptr() if history is not None else None, history_cap, cl.stream_ptr()),
+             "argmax_advance")
 
 
 GEMM_VARIANTS = {"auto": 0, "ldg": 1, "tma": 2}

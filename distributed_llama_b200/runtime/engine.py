@@ -44,6 +44,18 @@ def logprobs_rows(logits: torch.Tensor, chosen: torch.Tensor, k: Sequence[int], 
     return out
 
 
+def dense_max_batch(max_batch: int, dim: int, ff_dim: int, q_dim: int) -> int:
+    """Largest power-of-two batch <= max_batch that the dense-weight GEMV holds: it stages the f32 activations of all tokens of a
+    launch in shared memory (gemv_dense.cu), so the widest matrix row (dim, ff_dim or q_dim values) bounds it."""
+    widest = max(dim, ff_dim, q_dim)
+    cap = (200 * 1024) // (4 * widest)
+    if cap < 1:
+        raise ValueError("matrix rows too wide for the dense-weight kernels on one GPU; use more ranks")
+    while max_batch > cap:
+        max_batch //= 2
+    return max_batch
+
+
 class Engine:
     def __init__(self, weights: DeviceWeights, max_batch: int = 8, n_splits: int = 0, use_pdl: bool = True,
                  seq_len: Optional[int] = None, comm=None, max_prefill: int = 192, collectives: str = "auto",
@@ -60,13 +72,7 @@ class Engine:
             max_batch = 1          # the MoE kernels route one token per launch
         self.dense = getattr(w, "weight_kind", 0) != 0
         if self.dense:
-            # f32 activations of all tokens of a launch are staged in shared memory (gemv_dense.cu)
-            widest = max(h.dim, w.ff_dim, w.n_heads * h.head_dim)
-            cap = (200 * 1024) // (4 * widest)
-            if cap < 1:
-                raise ValueError("matrix rows too wide for the dense-weight kernels on one GPU; use more ranks")
-            while max_batch > cap:
-                max_batch //= 2
+            max_batch = dense_max_batch(max_batch, h.dim, w.ff_dim, w.n_heads * h.head_dim)
         self.max_batch = max_batch
         props = torch.cuda.get_device_properties(dev)
         self.num_sms = props.multi_processor_count

@@ -1,7 +1,8 @@
-"""Float64 reference helpers shared by the tensor-core GEMM tests (tests/test_gpu_gemm_tc.py, tests/test_gpu_moe.py).
+"""Float64 reference helpers shared by the q40 matrix tests (tests/test_gpu_gemm_tc.py, tests/test_gpu_moe.py, tests/test_gpu_gemv.py).
 
 * Random q40 matrices as raw 18-byte blocks (f16 scale + 16 bytes of nibbles) and their device layout.
 * The weights the tensor-core dequant warps build from them: rn_bf16(rn_bf16(f16 scale) * (q - 8)).
+* The q80 grid of decode activations, with the ambiguity of a rounding whose input is only known within an interval.
 * Checks of a kernel's values against a float64 reference with a per-element bound, or against the bf16 roundings of the two ends
   of an interval.
 """
@@ -106,3 +107,38 @@ def assert_bracketed(got, lo, hi, what):
     bad = (got < lo) | (got > hi)
     assert not bad.any(), (f"{what}: {int(bad.sum())} of {bad.numel()} values outside the rounding interval "
                            f"(max distance {torch.maximum(lo - got, got - hi).max().item():.3g})")
+
+
+# ---- decode activations --------------------------------------------------------------------------------------------------
+C_SILU = 2.0 ** -19    # SiLU with __expf and fast division, relative
+
+
+def q80_ref(v, rel):
+    """q80 grid of f64 activations v [..., n] (blocks of 32: d = f16(amax / 127), q = rint(x / d)) and, per element, the most the
+    kernel's grid value can differ when its input is within `rel` (relative) of v."""
+    shp = v.shape
+    g = v.reshape(-1, 32)
+    d = g.abs().amax(1, keepdim=True) / 127.0
+
+    def f16(t):
+        return t.float().half().double()
+
+    dq, dlo, dhi = f16(d), f16(d * (1 - rel)), f16(d * (1 + rel))
+    t = torch.where(d > 0, g / d.clamp_min(1e-300), torch.zeros_like(g))
+    q, qlo, qhi = torch.round(t), torch.round(t - t.abs() * rel), torch.round(t + t.abs() * rel)
+    a = q * dq
+    amb = torch.stack([(x * y - a).abs() for x in (qlo, qhi) for y in (dlo, dhi)]).amax(0)
+    return a.reshape(shp), amb.reshape(shp)
+
+
+def silu(x):
+    return x / (1.0 + torch.exp(-x))
+
+
+def swiglu_ref(gu, e_gu):
+    """h = silu(gate) * up from interleaved rows (gate even, up odd) and the bound on the kernel's f32 h."""
+    g, u, eg, eu = gu[..., 0::2], gu[..., 1::2], e_gu[..., 0::2], e_gu[..., 1::2]
+    s = silu(g)
+    h = s * u
+    # |d silu / dx| <= 1.1
+    return h, 1.1 * eg * u.abs() + s.abs() * eu + 1.1 * eg * eu + C_SILU * h.abs()

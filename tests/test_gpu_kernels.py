@@ -1,4 +1,5 @@
-"""Numerics of the hand-written CUDA kernels against plain PyTorch f32 references of the same op."""
+"""Device q40 repack (csrc/cuda/repack.cu) against the CPU dequantisation of the same blocks. The decode GEMVs are tested in
+tests/test_gpu_gemv.py."""
 import numpy as np
 import pytest
 import torch
@@ -53,77 +54,3 @@ def test_repack_column_slice_and_interleave():
     ref = wq.reshape(d // hd, hd, n)
     np.testing.assert_array_equal(got[:, 0::2], ref[:, : hd // 2])
     np.testing.assert_array_equal(got[:, 1::2], ref[:, hd // 2:])
-
-
-def _q80(x):
-    from distributed_llama_b200.models.reference import q80_round
-    return q80_round(x)
-
-
-@pytest.mark.parametrize("impl", ["ldg", "tma"])
-@pytest.mark.parametrize("nb", [1, 2, 4, 8])
-@pytest.mark.parametrize("d,n", [(256, 256), (6144, 4096), (4096, 1792), (1000, 2176), (128, 96 * 8), (16032, 4096), (402, 14336)])
-def test_gemv_rmsnorm_store(nb, d, n, impl):
-    from distributed_llama_b200 import ops
-    raw, wq = _rand_q40(d, n, seed=3)
-    w = _device_q40(raw, d, n)
-    torch.manual_seed(0)
-    x = torch.randn(nb, n, device="cuda") * 2.0
-    nw = 1.0 + 0.1 * torch.randn(n, device="cuda")
-    out = torch.empty(nb, d, device="cuda")
-    ops.gemv_q40(w, x, pro=ops.PRO_RMSNORM, epi=ops.EPI_STORE, out=out, norm_w=nw, eps=1e-5, impl=impl)
-    y = nw * (x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + 1e-5))
-    ref_q = _q80(y) @ torch.from_numpy(wq).cuda().T       # same activation grid as the kernel
-    ref_f = y @ torch.from_numpy(wq).cuda().T             # un-quantised activations
-    torch.testing.assert_close(out, ref_q, rtol=2e-3, atol=2e-3)
-    assert (out - ref_f).abs().max() < 0.08 * ref_f.abs().max() + 0.05
-
-
-@pytest.mark.parametrize("impl", ["ldg", "tma"])
-@pytest.mark.parametrize("nb", [1, 4])
-def test_gemv_residual_and_swiglu(nb, impl):
-    from distributed_llama_b200 import ops
-    d, n = 512, 1024
-    raw, wq = _rand_q40(d, n, seed=4)
-    w = _device_q40(raw, d, n)
-    wt = torch.from_numpy(wq).cuda()
-    torch.manual_seed(1)
-    z = torch.randn(nb, n, device="cuda")
-    x = torch.randn(nb, d, device="cuda")
-    x0 = x.clone()
-    ops.gemv_q40(w, z, pro=ops.PRO_PLAIN, epi=ops.EPI_RESIDUAL, out=x, impl=impl)
-    torch.testing.assert_close(x, x0 + _q80(z) @ wt.T, rtol=2e-3, atol=2e-3)
-    # swiglu: rows interleaved (gate_i, up_i)
-    nw = torch.ones(n, device="cuda")
-    hbuf = torch.empty(nb, d // 2, device="cuda")
-    ops.gemv_q40(w, z, pro=ops.PRO_RMSNORM, epi=ops.EPI_SWIGLU, out=hbuf, norm_w=nw, eps=1e-6, impl=impl)
-    y = _q80(z * torch.rsqrt(z.pow(2).mean(-1, keepdim=True) + 1e-6))
-    full = y @ wt.T
-    ref = torch.nn.functional.silu(full[:, 0::2]) * full[:, 1::2]
-    torch.testing.assert_close(hbuf, ref, rtol=3e-3, atol=3e-3)
-
-
-@pytest.mark.parametrize("dtype", [torch.float32, torch.float16])
-@pytest.mark.parametrize("nb", [1, 4])
-def test_gemv_dense_f32_f16_weights(dtype, nb):
-    """Dense-weight GEMV (f32 / f16 `.m` files): rmsnorm prologue and store / residual / SwiGLU epilogues vs PyTorch f32."""
-    from distributed_llama_b200.ops import DeviceDense, gemv_dense, PRO_RMSNORM, PRO_PLAIN, EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU
-    torch.manual_seed(3)
-    d, n = 640, 1032 if dtype == torch.float32 else 1024          # n not a multiple of the unrolled chunk stride
-    w = (torch.randn(d, n, device="cuda") / n ** 0.5).to(dtype)
-    W = DeviceDense(w, d, n)
-    x = torch.randn(nb, n, device="cuda")
-    nw = torch.rand(n, device="cuda") + 0.5
-    wf = w.float()
-    xn = nw * x * torch.rsqrt((x * x).mean(-1, keepdim=True) + 1e-5)
-    out = torch.zeros(nb, d, device="cuda")
-    gemv_dense(W, x, pro=PRO_RMSNORM, epi=EPI_STORE, out=out, norm_w=nw, eps=1e-5)
-    torch.testing.assert_close(out, xn @ wf.T, rtol=1e-4, atol=1e-4)
-    res = torch.randn(nb, d, device="cuda")
-    out = res.clone()
-    gemv_dense(W, x, pro=PRO_PLAIN, epi=EPI_RESIDUAL, out=out)
-    torch.testing.assert_close(out, res + x @ wf.T, rtol=1e-4, atol=1e-4)
-    out = torch.zeros(nb, d // 2, device="cuda")
-    gemv_dense(W, x, pro=PRO_RMSNORM, epi=EPI_SWIGLU, out=out, norm_w=nw, eps=1e-5)
-    y = xn @ wf.T
-    torch.testing.assert_close(out, torch.nn.functional.silu(y[:, 0::2]) * y[:, 1::2], rtol=1e-4, atol=1e-4)

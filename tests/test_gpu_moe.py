@@ -42,7 +42,7 @@ import math
 import pytest
 import torch
 
-from q40_ref import Experts, assert_bracketed, assert_within, bf16_bracket, f64_to_bf16
+from q40_ref import Experts, assert_bracketed, assert_within, bf16_bracket, f64_to_bf16, q80_ref, swiglu_ref
 from q40_ref import gen as _gen, seed_of as _seed
 
 pytestmark = pytest.mark.gpu
@@ -50,7 +50,6 @@ pytestmark = pytest.mark.gpu
 SILU = 0
 EPS = 1e-6
 C_ACC = 2.0 ** -18     # f32 accumulation, per unit of S
-C_ACT = 2.0 ** -19     # SiLU (__expf, fast division), relative
 C_SUM = 2.0 ** -22     # residual add, slot / pair sums
 REL_NORM = 2.0 ** -18  # kernel's rmsnorm'd f32 activations vs float64, relative
 REL_H = 2.0 ** -20     # q80 of the kernel's own h: reciprocal and division only
@@ -74,37 +73,6 @@ def _i32(t):
 
 
 # ---- float64 reference helpers ---------------------------------------------------------------------------------------
-def q80_ref(v, rel):
-    """q80 grid of f64 activations v [..., n] (blocks of 32: d = f16(amax / 127), q = rint(x / d)) and, per element, the most the
-    kernel's grid value can differ when its input is within `rel` (relative) of v."""
-    shp = v.shape
-    g = v.reshape(-1, 32)
-    d = g.abs().amax(1, keepdim=True) / 127.0
-
-    def f16(t):
-        return t.float().half().double()
-
-    dq, dlo, dhi = f16(d), f16(d * (1 - rel)), f16(d * (1 + rel))
-    t = torch.where(d > 0, g / d.clamp_min(1e-300), torch.zeros_like(g))
-    q, qlo, qhi = torch.round(t), torch.round(t - t.abs() * rel), torch.round(t + t.abs() * rel)
-    a = q * dq
-    amb = torch.stack([(x * y - a).abs() for x in (qlo, qhi) for y in (dlo, dhi)]).amax(0)
-    return a.reshape(shp), amb.reshape(shp)
-
-
-def silu(x):
-    return x / (1.0 + torch.exp(-x))
-
-
-def swiglu_ref(gu, e_gu):
-    """h = silu(gate) * up from interleaved rows (gate even, up odd) and the bound on the kernel's f32 h."""
-    g, u, eg, eu = gu[..., 0::2], gu[..., 1::2], e_gu[..., 0::2], e_gu[..., 1::2]
-    s = silu(g)
-    h = s * u
-    # |d silu / dx| <= 1.1
-    return h, 1.1 * eg * u.abs() + s.abs() * eu + 1.1 * eg * eu + C_ACT * h.abs()
-
-
 def rms_ref(x, w):
     x = x.double()
     return w.double() * (x * torch.rsqrt(x.pow(2).mean(-1, keepdim=True) + EPS))
