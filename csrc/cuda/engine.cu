@@ -1008,35 +1008,104 @@ DL_EXPORT int dl_moe_decode_ffn_dense(int wtype, const float *x, float *out, con
     return dl::moeDecodeFfn(m, stream, false);
 }
 
-// A prompt of n tokens (host memory) at positions p0 .. p0 + n - 1, staged chunk by chunk on `stream`; logits of the last
-// token with wantLogits. A chunk of up to maxPrefill tokens runs on the tensor cores while at least prefillMinTc tokens remain
-// and the shape allows it: q40 matrices; MoE: dim and ff multiples of 256 (grouped GEMMs); tensor parallel: per-rank qDim, ff and
-// dim multiples of 256 (prefill all-reduce). Otherwise the largest power-of-two GEMV batch <= min(remaining, maxBatch) runs.
-// slot >= 0: into KV-cache slot `slot`, every chunk on the tensor cores.
-DL_EXPORT int dl_engine_prefill(void *h, const int32_t *hostTokens, uint32_t n, uint32_t p0, int slot, int wantLogits, cudaStream_t stream) {
-    Engine &e = *(Engine *)h;
-    const dl::EngineConfig &c = e.cfg;
-    if (slot >= 0 && e.slots < 2) return -64;
-    if ((uint64_t)p0 + n > (slot >= 0 ? e.slotLen : c.seqLen)) return -60;
-    const bool tpOk = e.comm.nRanks <= 1 || ((c.nHeads * c.headDim) % 256 == 0 && c.ffDim % 256 == 0 && c.dim % 256 == 0);
-    const bool moeOk = c.nExperts == 0 || (c.dim % 256 == 0 && c.ffDim % 256 == 0);
-    const bool tc = e.prefillMinTc > 0 && c.wType == 0 && tpOk && moeOk;
-    std::vector<int32_t> pos(n);
-    for (uint32_t i = 0; i < n; i++) pos[i] = (int32_t)(p0 + i);
+namespace dl {
+
+struct PrefillChunk { uint32_t T, p0, onTc; };
+
+// The chunks of a prompt of n tokens at positions p0 .. p0 + n - 1 in a cache of `rows` rows. A chunk of up to maxPrefill tokens
+// runs on the tensor cores while at least minTc (0: never) tokens remain and tcAllowed; otherwise the largest power-of-two GEMV
+// batch <= min(remaining, maxBatch) runs. slot >= 0 (a KV-cache slot of `slots`): every chunk on the tensor cores.
+// -64: slot prefill without slots; -60: the prompt runs past the cache.
+static int planPrefill(uint32_t n, uint32_t p0, int slot, uint32_t slots, uint32_t rows, uint32_t maxPrefill, uint32_t maxBatch,
+                       uint32_t minTc, bool tcAllowed, std::vector<PrefillChunk> &out) {
+    out.clear();
+    if (slot >= 0 && slots < 2) return -64;
+    if ((uint64_t)p0 + n > rows) return -60;
+    if (maxPrefill < 1) return -11;
+    const bool tc = minTc > 0 && tcAllowed;
     for (uint32_t i = 0; i < n;) {
         const uint32_t rem = n - i;
-        const bool onTc = slot >= 0 || (tc && rem >= e.prefillMinTc);
+        const bool onTc = slot >= 0 || (tc && rem >= minTc);
         uint32_t T = 1;
-        if (onTc) T = std::min(rem, c.maxPrefill);
-        else while (T * 2 <= std::min(rem, c.maxBatch)) T *= 2;
-        const bool logits = wantLogits && i + T == n;
-        // pageable sources: each copy has read its host bytes when the call returns
-        DL_CUDA_CHECK(cudaMemcpyAsync(onTc ? e.g.pTokens : e.g.tokens, hostTokens + i, T * 4, cudaMemcpyHostToDevice, stream));
-        DL_CUDA_CHECK(cudaMemcpyAsync(onTc ? e.g.pPos : e.g.pos, pos.data() + i, T * 4, cudaMemcpyHostToDevice, stream));
-        if (onTc) DL_TRY(dl::enginePrefill(e, T, p0 + i, logits, stream, slot));
-        else DL_TRY(dl::engineForward(e, (int)T, logits ? 1 : 0, false, stream));
+        if (onTc) T = std::min(rem, maxPrefill);
+        else while (T * 2 <= std::min(rem, maxBatch)) T *= 2;
+        out.push_back({T, p0 + i, onTc ? 1u : 0u});
         i += T;
     }
+    return 0;
+}
+
+// planPrefill with the engine's settings. The tensor cores take q40 matrices; MoE: dim and ff multiples of 256 (grouped GEMMs);
+// tensor parallel: per-rank qDim, ff and dim multiples of 256 (prefill all-reduce).
+static int planEnginePrefill(const Engine &e, uint32_t n, uint32_t p0, int slot, std::vector<PrefillChunk> &out) {
+    const EngineConfig &c = e.cfg;
+    const bool tpOk = e.comm.nRanks <= 1 || ((c.nHeads * c.headDim) % 256 == 0 && c.ffDim % 256 == 0 && c.dim % 256 == 0);
+    const bool moeOk = c.nExperts == 0 || (c.dim % 256 == 0 && c.ffDim % 256 == 0);
+    return planPrefill(n, p0, slot, e.slots, slot >= 0 ? e.slotLen : c.seqLen, c.maxPrefill, c.maxBatch, e.prefillMinTc,
+                       c.wType == 0 && tpOk && moeOk, out);
+}
+
+static int copyPlan(int rc, const std::vector<PrefillChunk> &chunks, uint32_t *out, uint32_t cap) {
+    if (rc != 0) return rc;
+    for (size_t i = 0; i < chunks.size() && i < cap; i++) {
+        out[3 * i] = chunks[i].T; out[3 * i + 1] = chunks[i].p0; out[3 * i + 2] = chunks[i].onTc;
+    }
+    return (int)chunks.size();
+}
+
+}  // namespace dl
+
+// The prefill schedule without an engine or a device (see planPrefill): writes up to `cap` chunks as (T, p0, on tensor cores)
+// triples and returns the number of chunks, or a negative error.
+DL_EXPORT int dl_prefill_plan(uint32_t n, uint32_t p0, int slot, uint32_t slots, uint32_t rows, uint32_t maxPrefill, uint32_t maxBatch,
+                              uint32_t minTc, int tcAllowed, uint32_t *out, uint32_t cap) {
+    std::vector<dl::PrefillChunk> chunks;
+    return dl::copyPlan(dl::planPrefill(n, p0, slot, slots, rows, maxPrefill, maxBatch, minTc, tcAllowed != 0, chunks), chunks, out, cap);
+}
+
+// The chunks dl_engine_prefill runs for these arguments, as dl_prefill_plan returns them.
+DL_EXPORT int dl_engine_prefill_plan(void *h, uint32_t n, uint32_t p0, int slot, uint32_t *out, uint32_t cap) {
+    std::vector<dl::PrefillChunk> chunks;
+    return dl::copyPlan(dl::planEnginePrefill(*(Engine *)h, n, p0, slot, chunks), chunks, out, cap);
+}
+
+// A prompt of n tokens (host memory) at positions p0 .. p0 + n - 1, staged chunk by chunk (planEnginePrefill) on `stream`;
+// logits of the last token with wantLogits. slot >= 0: into KV-cache slot `slot`.
+DL_EXPORT int dl_engine_prefill(void *h, const int32_t *hostTokens, uint32_t n, uint32_t p0, int slot, int wantLogits, cudaStream_t stream) {
+    Engine &e = *(Engine *)h;
+    std::vector<dl::PrefillChunk> chunks;
+    DL_TRY(dl::planEnginePrefill(e, n, p0, slot, chunks));
+    std::vector<int32_t> pos(n);
+    for (uint32_t i = 0; i < n; i++) pos[i] = (int32_t)(p0 + i);
+    for (const dl::PrefillChunk &ch : chunks) {
+        const uint32_t i = ch.p0 - p0, T = ch.T;
+        const bool logits = wantLogits && i + T == n;
+        // pageable sources: each copy has read its host bytes when the call returns
+        DL_CUDA_CHECK(cudaMemcpyAsync(ch.onTc ? e.g.pTokens : e.g.tokens, hostTokens + i, T * 4, cudaMemcpyHostToDevice, stream));
+        DL_CUDA_CHECK(cudaMemcpyAsync(ch.onTc ? e.g.pPos : e.g.pos, pos.data() + i, T * 4, cudaMemcpyHostToDevice, stream));
+        if (ch.onTc) DL_TRY(dl::enginePrefill(e, T, ch.p0, logits, stream, slot));
+        else DL_TRY(dl::engineForward(e, (int)T, logits ? 1 : 0, false, stream));
+    }
+    return 0;
+}
+
+// Copies the intermediates the last prompt chunk left in the engine's scratch into caller device memory (tests), `rows` rows
+// each; a null destination is skipped. Tensor-core chunk (rows <= maxPrefill): px (f32 [rows][dim], the residual), pqkv (f32
+// [rows][qkvDim], q after QK-norm and RoPE, raw k and v), pxn (bf16 [rows][dim], the last rmsnorm), pzb (bf16 [rows][qDim],
+// attention) and phb (bf16 [rows][ff], SwiGLU). GEMV batch (rows <= maxBatch): qkv (f32 [rows][qkvDim]), z (f32 [rows][qDim],
+// attention) and hF (f32 [rows][ff], SwiGLU); the residual is the client's x. Every buffer holds the last layer's values.
+DL_EXPORT int dl_engine_prefill_scratch(void *h, uint32_t rows, void *px, void *pqkv, void *pxn, void *pzb, void *phb, void *qkv,
+                                        void *z, void *hF, cudaStream_t stream) {
+    Engine &e = *(Engine *)h;
+    const dl::EngineConfig &c = e.cfg;
+    const size_t qDim = (size_t)c.nHeads * c.headDim, qkvDim = qDim + 2 * (size_t)c.nKvHeads * c.headDim;
+    if ((px || pqkv || pxn || pzb || phb) && rows > c.maxPrefill) return -1;
+    if ((qkv || z || hF) && rows > c.maxBatch) return -1;
+    void *dst[8] = {px, pqkv, pxn, pzb, phb, qkv, z, hF};
+    const void *src[8] = {e.g.px, e.g.pqkv, e.g.pxn, e.g.pzb, e.g.phb, e.g.qkv, e.g.z, e.g.h};
+    const size_t bytes[8] = {c.dim * 4, qkvDim * 4, c.dim * 2, qDim * 2, (size_t)c.ffDim * 2, qkvDim * 4, qDim * 4, (size_t)c.ffDim * 4};
+    for (int i = 0; i < 8; i++)
+        if (dst[i]) DL_CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], rows * bytes[i], cudaMemcpyDeviceToDevice, stream));
     return 0;
 }
 

@@ -116,6 +116,13 @@ int dl_engine_forward(void *h, int nb, int logitsMode, int greedyAdvance, cudaSt
 int dl_engine_forward_part(void *h, int nb, uint32_t layer, int part, float *ybuf, cudaStream_t stream);
 // n prompt tokens (host memory) at positions p0 .. p0 + n - 1; slot >= 0: into KV-cache slot `slot`
 int dl_engine_prefill(void *h, const int32_t *hostTokens, uint32_t n, uint32_t p0, int slot, int wantLogits, cudaStream_t stream);
+// the chunks dl_engine_prefill runs, as up to `cap` (T, p0, on tensor cores) triples; returns their number or a negative error
+int dl_engine_prefill_plan(void *h, uint32_t n, uint32_t p0, int slot, uint32_t *out, uint32_t cap);
+int dl_prefill_plan(uint32_t n, uint32_t p0, int slot, uint32_t slots, uint32_t rows, uint32_t maxPrefill, uint32_t maxBatch,
+                    uint32_t minTc, int tcAllowed, uint32_t *out, uint32_t cap);   // the same schedule, no engine or device
+// copies the last prompt chunk's scratch intermediates into device memory (tests); null destinations are skipped
+int dl_engine_prefill_scratch(void *h, uint32_t rows, void *px, void *pqkv, void *pxn, void *pzb, void *phb, void *qkv, void *z,
+                              void *hF, cudaStream_t stream);
 int dl_engine_set_prefill_min_tc(void *h, uint32_t n);   // shortest chunk on the tensor cores (default 9; 0: never)
 int dl_engine_decode_graph(void *h, int nSteps, cudaStream_t stream);   // captures the greedy step on first use
 int dl_engine_graph_captured(void *h);

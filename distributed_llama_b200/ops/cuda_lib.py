@@ -211,6 +211,13 @@ def lib() -> C.CDLL:
     L.dl_engine_forward_part.restype = i32
     L.dl_engine_prefill.argtypes = [vp, ip, u32, u32, i32, i32, vp]
     L.dl_engine_prefill.restype = i32
+    up = C.POINTER(C.c_uint32)
+    L.dl_engine_prefill_plan.argtypes = [vp, u32, u32, i32, up, u32]
+    L.dl_engine_prefill_plan.restype = i32
+    L.dl_prefill_plan.argtypes = [u32, u32, i32, u32, u32, u32, u32, u32, i32, up, u32]
+    L.dl_prefill_plan.restype = i32
+    L.dl_engine_prefill_scratch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.dl_engine_prefill_scratch.restype = i32
     L.dl_engine_set_prefill_min_tc.argtypes = [vp, u32]
     L.dl_engine_set_prefill_min_tc.restype = i32
     L.dl_engine_decode_graph.argtypes = [vp, i32, vp]

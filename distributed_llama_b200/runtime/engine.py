@@ -44,6 +44,26 @@ def logprobs_rows(logits: torch.Tensor, chosen: torch.Tensor, k: Sequence[int], 
     return out
 
 
+def _plan_chunks(call) -> List[tuple]:
+    cap = 64
+    while True:
+        out = (C.c_uint32 * (3 * cap))()
+        n = call(out, cap)
+        cl.check(min(n, 0), "prefill_plan")
+        if n <= cap:
+            return [(int(out[3 * i]), int(out[3 * i + 1]), bool(out[3 * i + 2])) for i in range(n)]
+        cap = n
+
+
+def prefill_plan(n: int, start_pos: int, rows: int, max_prefill: int, max_batch: int, min_tc: int, tensor_cores: bool,
+                 slot: int = -1, slots: int = 1) -> List[tuple]:
+    """The chunks the engine splits a prompt of n tokens at start_pos into (dl_prefill_plan; no device needed), in a cache of `rows`
+    rows: (T, first position, on the tensor cores) per chunk. Raises on a prompt past the cache (code -60) or a slot prefill
+    without slots (-64)."""
+    return _plan_chunks(lambda out, cap: cl.lib().dl_prefill_plan(n, start_pos, slot, slots, rows, max_prefill, max_batch, min_tc,
+                                                                  1 if tensor_cores else 0, out, cap))
+
+
 def dense_max_batch(max_batch: int, dim: int, ff_dim: int, q_dim: int) -> int:
     """Largest power-of-two batch <= max_batch that the dense-weight GEMV holds: it stages the f32 activations of all tokens of a
     launch in shared memory (gemv_dense.cu), so the widest matrix row (dim, ff_dim or q_dim values) bounds it."""
@@ -74,6 +94,7 @@ class Engine:
         if self.dense:
             max_batch = dense_max_batch(max_batch, h.dim, w.ff_dim, w.n_heads * h.head_dim)
         self.max_batch = max_batch
+        self.max_prefill = min(max_prefill, 256)
         props = torch.cuda.get_device_properties(dev)
         self.num_sms = props.multi_processor_count
         if n_splits <= 0:
@@ -108,7 +129,7 @@ class Engine:
                               moeFirstExpert=w.first_expert, moeNumLocal=w.n_local_experts,
                               wType=getattr(w, "weight_kind", 0),
                               hiddenAct=1 if int(h.hidden_act) == 0 else 0,   # header: ACT_GELU = 0, ACT_SILU = 1
-                              kvType=cl.KV_CACHE_TYPES[kv_cache_float_type], maxPrefill=min(max_prefill, 256))
+                              kvType=cl.KV_CACHE_TYPES[kv_cache_float_type], maxPrefill=self.max_prefill)
         self._lib = cl.lib()
         self._h = self._lib.dl_engine_create(C.byref(cfg))
         if not self._h:
@@ -484,16 +505,34 @@ class Engine:
         if not self._parts:
             self._prefill(tokens, start_pos, -1, want_logits)
             return self._full_logits(self.logits[0]) if want_logits else None
-        i = 0
-        while i < len(tokens):
-            rem = len(tokens) - i
-            n = 1
-            while n * 2 <= min(rem, self.max_batch):
-                n *= 2
-            last = i + n == len(tokens)
-            self.forward_batch(tokens[i:i + n], start_pos + i, logits_mode=1 if (last and want_logits) else 0)
-            i += n
+        for T, p, _ in prefill_plan(len(tokens), start_pos, self.seq_len, self.max_prefill, self.max_batch, 0, False):
+            i = p - start_pos
+            last = i + T == len(tokens)
+            self.forward_batch(tokens[i:i + T], p, logits_mode=1 if (last and want_logits) else 0)
         return self._full_logits(self.logits[0]) if want_logits else None
+
+    def prefill_plan(self, n: int, start_pos: int, slot: int = -1) -> List[tuple]:
+        """The chunks prefill() (slot_prefill() for slot >= 0) runs for n tokens at start_pos with the engine's settings:
+        (T, first position, on the tensor cores) per chunk."""
+        if self._parts and slot < 0:
+            return prefill_plan(n, start_pos, self.seq_len, self.max_prefill, self.max_batch, 0, False)
+        return _plan_chunks(lambda out, cap: self._lib.dl_engine_prefill_plan(self._h, n, start_pos, slot, out, cap))
+
+    def prefill_intermediates(self, rows: int, tensor_cores: bool) -> dict:
+        """Copies of what the last prompt chunk of `rows` tokens left in the engine's scratch (its last layer). Tensor-core chunk:
+        "x" (f32 residual), "qkv" (f32: q after QK-norm and RoPE, raw k and v), "xn" (bf16, the post-attention rmsnorm), "z" (bf16
+        attention output), "h" (bf16 SwiGLU output). GEMV batch: "qkv", "z" and "h" in f32 (q is rotated in place for batches of
+        2 or more); its residual is `x`."""
+        w, hd = self.w, self.w.header.head_dim
+        dims = {"x": w.header.dim, "qkv": self.qkv_dim, "xn": w.header.dim, "z": w.n_heads * hd, "h": w.ff_dim}
+        keys = ("x", "qkv", "xn", "z", "h") if tensor_cores else ("qkv", "z", "h")
+        dt = {"x": torch.float32, "qkv": torch.float32}
+        out = {k: torch.empty(rows, dims[k], dtype=dt.get(k, torch.bfloat16 if tensor_cores else torch.float32), device=self.device)
+               for k in keys}
+        ptrs = [_p(out.get(k)) if tensor_cores else None for k in ("x", "qkv", "xn", "z", "h")]
+        ptrs += [None if tensor_cores else _p(out[k]) for k in ("qkv", "z", "h")]
+        cl.check(self._lib.dl_engine_prefill_scratch(self._h, rows, *ptrs, cl.stream_ptr()), "engine_prefill_scratch")
+        return out
 
     def _prefill(self, tokens: List[int], start_pos: int, slot: int, want_logits: bool) -> None:
         arr = (C.c_int32 * len(tokens))(*tokens)

@@ -21,18 +21,17 @@ and the SwiGLU output of that launch must be bitwise those of the normal launch.
 """
 import dataclasses
 import gc
-import math
 import time
 
-import numpy as np
 import pytest
 import torch
+
+from q40_ref import U, Ref, attention, bf16_ulp, dequant, gemv, kv_rows, q80, rms, silu, worst
 
 pytestmark = pytest.mark.gpu
 
 SEQ = 4096
 POSITIONS = [0, 1, 63, 64, 255, 256, 257, 1023, 1024, 2047, 2048, 4095]
-U = 2.0 ** -24                   # unit roundoff of f32
 CONTROL_MIN = 10.0               # a negative control must exceed its bound by this factor
 
 # name: (preset, vocabulary of the synthetic model). Llama-3.1-8B keeps its real vocabulary (970/972-row logits tiles on 132 SMs);
@@ -98,188 +97,6 @@ def tile(P, b):
 
 # ------------------------------------------------------------------ float64 reference ------------------------------------------------------------------
 
-def _interleave_perm(hd):
-    perm = np.empty(hd, dtype=np.int64)
-    perm[0::2] = np.arange(hd // 2)
-    perm[1::2] = np.arange(hd // 2) + hd // 2
-    return torch.from_numpy(perm)
-
-
-def dequant(raw):
-    """q40 file rows [d, n/32, 18] -> (f32 values [d, n] (exact), f32 block scales [d, n/32])."""
-    d = raw[..., :2].contiguous().view(torch.float16).float()        # [d, nb, 1]
-    qs = raw[..., 2:].to(torch.int16)
-    w = torch.cat([(qs & 15) - 8, (qs >> 4) - 8], -1).float().mul_(d)
-    return w.view(raw.shape[0], -1), d.view(raw.shape[0], -1)
-
-
-class Ref:
-    """The model file's q40 matrices as raw file rows on the device, in the engine's row order (q|k|v rows concatenated, q and k rows
-    in adjacent-pair RoPE order for NeoX models, w1/w3 rows interleaved); `gemv` dequantises them chunk by chunk."""
-
-    def __init__(self, path):
-        from distributed_llama_b200 import host
-        from distributed_llama_b200.formats import ModelFile
-        from distributed_llama_b200.models.config import ROPE_FALCON
-        self.mf = mf = ModelFile(path)
-        self.h = h = mf.header
-        self.hd, self.nh, self.nkv, self.dim, self.ff = h.head_dim, h.n_heads, h.n_kv_heads, h.dim, h.ff_dim
-        self.q_dim, self.kv_dim = self.nh * self.hd, self.nkv * self.hd
-        self.eps = float(h.norm_epsilon)
-        perm = _interleave_perm(self.hd).cuda() if h.rope_type == ROPE_FALCON else None
-
-        def heads(t, n_heads):
-            return t if perm is None else t.view(n_heads, self.hd, *t.shape[1:])[:, perm].reshape(t.shape)
-
-        def vec(name, l=0):
-            return torch.from_numpy(np.array(mf.tensor_f32(mf.entry(name, l)))).cuda().double()
-
-        self.layers = []
-        for l in range(h.n_layers):
-            q, k, v = (self._q40(n, l) for n in ("block_matmul_q", "block_matmul_k", "block_matmul_v"))
-            w1, w3 = self._q40("block_matmul_w1", l), self._q40("block_matmul_w3", l)
-            L = dict(qkv=torch.cat([heads(q, self.nh), heads(k, self.nkv), v]), wo=self._q40("block_matmul_wo", l),
-                     w13=torch.stack([w1, w3], 1).reshape(2 * self.ff, self.dim // 32, 18), w2=self._q40("block_matmul_w2", l),
-                     norm0=vec("block_norm_0", l), norm1=vec("block_norm_1", l), q_norm=None, k_norm=None)
-            del q, k, v, w1, w3
-            if h.qk_norm:
-                L["q_norm"], L["k_norm"] = vec("block_norm_q", l), vec("block_norm_k", l)
-                if perm is not None:
-                    L["q_norm"], L["k_norm"] = L["q_norm"][perm], L["k_norm"][perm]
-            self.layers.append(L)
-        self.final_norm = vec("final_norm")
-        self.wcls = self._q40("final_matmul_logits")
-        self.rope = torch.from_numpy(np.asarray(host().build_rope_table(h, h.seq_len))).cuda().double()   # [seq, hd/2, (cos, sin)]
-
-    def _q40(self, name, l=0):
-        e = self.mf.entry(name, l)
-        return torch.from_numpy(np.array(self.mf.raw(e))).cuda().view(e.d, e.n // 32, 18)
-
-    def embedding(self, tok):
-        e = self.mf.entry("embedding")
-        row = np.array(self.mf.data[e.offset + tok * self.dim * 4: e.offset + (tok + 1) * self.dim * 4]).view(np.float32)
-        return torch.from_numpy(row).cuda().double()
-
-
-def rms(x, w, eps):
-    return w * (x / torch.sqrt((x * x).mean(-1, keepdim=True) + eps))
-
-
-def rope(x, row):
-    """Adjacent-pair rotation of the rows of x [.., hd] by a rotary table row [hd/2, (cos, sin)]."""
-    a, b = x[..., 0::2], x[..., 1::2]
-    c, s = row[:, 0], row[:, 1]
-    out = torch.empty_like(x)
-    out[..., 0::2] = a * c - b * s
-    out[..., 1::2] = a * s + b * c
-    return out
-
-
-def q80(v, tol=None, normed=False):
-    """q80 round trip of the float64 vector v, as the kernel's prologue rounds it (d = fp16(amax / 127), q = rn(v / d)), with the
-    alternatives the kernel may take instead. tol: absolute uncertainty of the kernel's input to this prologue (per element, 0 when
-    the input is the kernel's own observed vector). normed: an RMS-norm prologue, whose f32 norm factor scales the whole vector.
-    Returns (xq, alt): one row of alt per alternative the kernel may take instead, holding the change of xq it makes: one grid
-    step of element i where i lies within the kernel's uncertainty of a q tie (bf16 inputs make exact ties common), and the
-    neighbouring fp16 scale of a block whose scale lies at an fp16 tie."""
-    g = v.view(-1, 32)
-    tg = torch.zeros_like(g) if tol is None else tol.view(-1, 32)
-    amax, arg = g.abs().max(1, keepdim=True)
-    dq = amax / 127
-    inv = torch.where(dq > 0, 1 / dq.clamp_min(1e-300), torch.zeros_like(dq))
-    t = g * inv
-    q = torch.round(t)
-    d16 = dq.to(torch.float16).double()
-    rel = tg.gather(1, arg) / amax.clamp_min(1e-300)                 # relative uncertainty of the block maximum from the input
-    # t = v / d: the norm factor cancels; what remains is the f32 rounding of v (2 roundings), d (an approximate division, 2 ulps),
-    # 1/d (an approximate reciprocal, 1 ulp) and v * (1/d): at most 12 half-ulps of t
-    dt = 1e-6 + 16 * U * t.abs() + inv * (tg + g.abs() * rel)
-    at = t.abs()
-    qtie = ((at - at.floor() - 0.5).abs() < dt).view(-1)
-    step = (torch.sign(t - q) * d16).view(-1)                        # towards the other neighbour of t
-    # the fp16 scale also carries the norm factor's f32 error (a sum of n squares)
-    ulp = torch.exp2(torch.floor(torch.log2(dq.clamp_min(2.0 ** -14))) - 10)
-    fr = dq / ulp
-    stie = ((fr - fr.floor() - 0.5).abs() < fr * (rel + 8 * U + (64 * U if normed else 0)) + 1e-6)[:, 0]
-    blocks, elems = stie.nonzero()[:, 0].tolist(), qtie.nonzero()[:, 0].tolist()
-    alt = torch.zeros(len(blocks) + len(elems), v.numel(), dtype=v.dtype, device=v.device)
-    for j, b in enumerate(blocks):
-        alt[j, 32 * b:32 * b + 32] = ulp[b] * q[b]
-    for j, i in enumerate(elems, len(blocks)):
-        alt[j, i] = step[i]
-    return (q * d16).view(-1), alt
-
-
-def gemv(raw, act, bound=True, got=None, chunk=4096):
-    """float64 W @ xq of the q40 rows `raw` and the q80 activation act = q80(..) and, with `bound`, the kernel's error bound of every
-    row: f32 rounding of the per-block dot products (against the block scale x the block's |xq|) and of the segment / row sums
-    (against sum |w x|), plus |W @ alt| for every q80 alternative. With the kernel's output `got`, the alternatives are resolved
-    instead: each one moves every row at once, so the combination the kernel took is the 0/1 least-squares fit of got - W @ xq, and
-    the result is W @ (xq + the chosen alternatives) with the accumulation bound alone. A fault confined to a few rows cannot be
-    absorbed by such a fit."""
-    xq, alt = act
-    nseg = (raw.shape[1] + 31) // 32
-    ax = xq.abs()
-    axb = ax.view(-1, 32).sum(1)
-    ys, bs, alts = [], [], []
-    for r0 in range(0, raw.shape[0], chunk):
-        W, S = dequant(raw[r0:r0 + chunk])
-        w = W.double()
-        del W
-        ys.append(w @ xq)
-        alts.append(w @ alt.T)
-        if bound:
-            w.abs_()
-            bs.append(U * (nseg + 8) * (w @ ax) + 72 * U * (S.double().abs() @ axb))
-        del w
-    y, A = torch.cat(ys), torch.cat(alts)
-    b = torch.cat(bs) if bound else None
-    if A.shape[1]:
-        if got is None:
-            b = b + A.abs().sum(1) if bound else b
-        else:
-            sel = (torch.linalg.pinv(A) @ (got.double() - y)).round().clamp(0, 1)
-            y = y + A @ sel
-    return y, b
-
-
-def silu(g):
-    return g * torch.sigmoid(g)
-
-
-def attention(q_raw, K, V, n_pos, q_norm, rope_row, nh, eps, n_splits, bound=True):
-    """float64 decode attention of the raw q [nh * hd] (QK-norm, RoPE) over rows [0, n_pos) of the bf16 caches K, V [n_kv, seq, hd],
-    and its bound: f32 score error (sum |q k|), __expf error, and the f32 accumulation over the positions one warp walks."""
-    nkv, _, hd = K.shape
-    q = q_raw.view(nh, hd)
-    if q_norm is not None:
-        q = rms(q, q_norm, eps)
-    q = rope(q, rope_row) / math.sqrt(hd)
-    Kh = K[:, :n_pos].double().repeat_interleave(nh // nkv, 0)
-    Vh = V[:, :n_pos].double().repeat_interleave(nh // nkv, 0)
-    s = torch.einsum("hd,hsd->hs", q, Kh)
-    pr = torch.softmax(s, -1)
-    z = torch.einsum("hs,hsd->hd", pr, Vh)
-    if not bound:
-        return z.reshape(-1), None
-    dots = torch.einsum("hd,hsd->hs", q.abs(), Kh.abs())
-    span = (s.amax(-1, keepdim=True) - s.amin(-1, keepdim=True))
-    eps_s = U * (16 * dots + 8 + 4 * (s.amax(-1, keepdim=True) - s + span))
-    eff = max(1, min(n_splits, (n_pos + 255) // 256))
-    depth = math.ceil(math.ceil(n_pos / eff) / 16) + 16 + eff + 8
-    b = torch.einsum("hs,hsd->hd", pr * eps_s, (Vh - z[:, None, :]).abs()) + U * depth * torch.einsum("hs,hsd->hd", pr, Vh.abs())
-    return z.reshape(-1), b.reshape(-1) + U * z.abs().reshape(-1)
-
-
-def bf16_ulp(x):
-    return torch.exp2(torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -126))) - 7)
-
-
-def worst(got, want, bound):
-    r = (got.double() - want).abs() / bound
-    return float(torch.nan_to_num(r, nan=float("inf")).max())
-
-
 def tile_ends(P, grid):
     """The last row of every CTA's tile of a phase."""
     return [sum(tile(P, b)) - 1 for b in range(grid) if tile(P, b)[1]]
@@ -302,14 +119,6 @@ def block_control(got, want, bound, W, xq, rows):
     """Median over `rows` of error / bound when row r loses one 32-column block."""
     c, r = lost_blocks(W, xq, rows)
     return float(((got.double()[r] - (want[r] - c)).abs() / bound[r]).median())
-
-
-def kv_rows(R, L, qkv, rope_row):
-    """float64 K row (QK-norm + RoPE of the raw k) and the V row of the raw q|k|v, [n_kv, hd] each."""
-    k = qkv[R.q_dim:R.q_dim + R.kv_dim].view(R.nkv, R.hd)
-    if L["k_norm"] is not None:
-        k = rms(k, L["k_norm"], R.eps)
-    return rope(k, rope_row), qkv[R.q_dim + R.kv_dim:].view(R.nkv, R.hd)
 
 
 def forward_ref(R, tok, p, K, V, n_splits):
