@@ -101,7 +101,6 @@ struct Engine {
     cudaEvent_t slotStaged = nullptr;  // the uploads of the staged tokens / positions are done: the buffer may be rewritten
     int slotLogprobs[8] = {-1, -1, -1, -1, -1, -1, -1, -1};   // per-slot top_logprobs k (-1: no logprobs), one per slot
     int32_t *slotLpDev = nullptr, *slotLpHost = nullptr;   // [kChoiceRngSlots][kLogprobsWords] results of a slots step (device, pinned)
-    bool prefillFusedAr = false; // TP prefill: GEMM + all-reduce in one kernel (DL_PREFILL_FUSED_AR=1) instead of GEMM, then all-reduce kernel
     bool tcAttn = true;          // prefill attention on the tensor cores (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
     bool fusedAttn = true, fusedArgmax = true, useTma = true;   // debugging switches (DL_NO_FUSED_ATTN / DL_NO_FUSED_ARGMAX / DL_NO_TMA)
 };
@@ -443,13 +442,12 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
             DL_TRY(launchAttnDecode(t, (int)T, stream, pdl));
         }
         // tensor parallel: partial product into the (now free) qkv buffer with all SMs / split-K, then all-reduce + residual over
-        // peer memory as its own kernel (DL_PREFILL_FUSED_AR=1: the one-kernel GEMM + all-reduce epilogue instead)
-        if (tp && !e.prefillFusedAr) {
+        // peer memory as its own kernel
+        if (tp) {
             arP.parity = 0;
             DL_TRY(gemmQ40Tc(GEPI_STORE_F32_, L.woQs, L.woSc, c.dim, qDim, g.pzb, qDim, T, g.pqkv, c.dim, c.numSms, stream, pdl));
             DL_TRY(launchArResidual(g.px, g.pqkv, c.dim, T, arP, stream, pdl));
-        } else if (tp) { arP.parity = 0; DL_TRY(gemmQ40TcAr(L.woQs, L.woSc, c.dim, qDim, g.pzb, qDim, T, g.px, c.dim, c.numSms, stream, arP)); }
-        else DL_TRY(gemmQ40Tc(GEPI_RESIDUAL_, L.woQs, L.woSc, c.dim, qDim, g.pzb, qDim, T, g.px, c.dim, c.numSms, stream, pdl));
+        } else DL_TRY(gemmQ40Tc(GEPI_RESIDUAL_, L.woQs, L.woSc, c.dim, qDim, g.pzb, qDim, T, g.px, c.dim, c.numSms, stream, pdl));
         if (c.nExperts > 0) {
             // mixture of experts: route the whole chunk, sort the (token, expert) pairs, grouped tensor-core GEMMs, weighted combine
             MoePrefillArgs mo{};
@@ -463,12 +461,11 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
         }
         DL_TRY(launchRmsNormBf16(g.px, c.dim, L.norm1, g.pxn, c.dim, c.dim, c.eps, T, stream, pdl));
         DL_TRY(gemmQ40Tc(GEPI_SWIGLU_BF16_, L.w13Qs, L.w13Sc, 2 * c.ffDim, c.dim, g.pxn, c.dim, T, g.phb, c.ffDim, c.numSms, stream, pdl));
-        if (tp && !e.prefillFusedAr) {
+        if (tp) {
             arP.parity = 1;
             DL_TRY(gemmQ40Tc(GEPI_STORE_F32_, L.w2Qs, L.w2Sc, c.dim, c.ffDim, g.phb, c.ffDim, T, g.pqkv, c.dim, c.numSms, stream, pdl));
             DL_TRY(launchArResidual(g.px, g.pqkv, c.dim, T, arP, stream, pdl));
-        } else if (tp) { arP.parity = 1; DL_TRY(gemmQ40TcAr(L.w2Qs, L.w2Sc, c.dim, c.ffDim, g.phb, c.ffDim, T, g.px, c.dim, c.numSms, stream, arP)); }
-        else DL_TRY(gemmQ40Tc(GEPI_RESIDUAL_, L.w2Qs, L.w2Sc, c.dim, c.ffDim, g.phb, c.ffDim, T, g.px, c.dim, c.numSms, stream, pdl));
+        } else DL_TRY(gemmQ40Tc(GEPI_RESIDUAL_, L.w2Qs, L.w2Sc, c.dim, c.ffDim, g.phb, c.ffDim, T, g.px, c.dim, c.numSms, stream, pdl));
     }
     if (wantLogits) {
         GemvArgs a{};
@@ -549,7 +546,6 @@ DL_EXPORT void *dl_engine_create(const dl::EngineConfig *cfg) {
     e->fusedArgmax = std::getenv("DL_NO_FUSED_ARGMAX") == nullptr;
     e->useTma = std::getenv("DL_NO_TMA") == nullptr;
     e->tcAttn = std::getenv("DL_NO_TC_ATTN") == nullptr;
-    e->prefillFusedAr = std::getenv("DL_PREFILL_FUSED_AR") != nullptr;
     if (e->cfg.numSms == 0) {
         int dev = 0, sms = 0;
         cudaGetDevice(&dev);

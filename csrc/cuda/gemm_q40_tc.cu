@@ -34,13 +34,10 @@ constexpr int kGmConsumerWarps = 4;
 // accumulator staging for the epilogue: per consumer warp 32 rows x 16 tokens f32, row stride 17 (conflict-free row reads)
 constexpr int kGmStgStride = 17;
 constexpr int kGmStgBytes = kGmConsumerWarps * 32 * kGmStgStride * 4;
-// DL_GEMM_DEBUG bit 9 (512): CTA 0 records %clock64 stamps of its pipeline events (tools/trace_gemm.py)
-__device__ unsigned long long gGemmTrace[4096];
-__device__ __forceinline__ unsigned long long gmClock() { unsigned long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)); return t; }
 constexpr int kGmATileBytes = kGmBlockM * kGmBlockK * 2;   // 16 KB
 constexpr int kGmBTileBytes = kGmTokTile * kGmBlockK * 2;  // 8 KB
 
-enum { GEPI_STORE_F32 = 0, GEPI_RESIDUAL = 1, GEPI_SWIGLU_BF16 = 2, GEPI_STORE_BF16 = 3, GEPI_RESIDUAL_AR = 4 };
+enum { GEPI_STORE_F32 = 0, GEPI_RESIDUAL = 1, GEPI_SWIGLU_BF16 = 2 };
 
 struct GemmArgs {
     const uint32_t *qs;
@@ -55,12 +52,7 @@ struct GemmArgs {
     float *splitScratch;   // [splitK][T][d] f32 partial accumulators
     uint32_t clusterSplit;  // TMA-staged variant: the splitK CTAs of a row tile form a thread-block cluster and reduce over distributed shared memory
     unsigned int *splitCounters;   // [row tiles x token tiles x 4][2], zero-initialised, self-resetting (arrived / done, per consumer warp)
-    ArArgs ar;             // GEPI_RESIDUAL_AR: tensor-parallel all-reduce fused into the epilogue (LL words over peer memory)
     uint32_t rawStages;    // TMA-staged variant: depth of the raw q40 ring (2 or 3)
-    // DL_GEMM_DEBUG (timing experiments and the pipeline trace of the TMA-staged variant; never set in production):
-    //   1 skip the proxy fence · 2 skip the A-tile stores · 4 release raw stages late
-    //   64 no q40 -> bf16 conversion · 256 contiguous raw loads (wrong results) · 512 CTA 0 records %clock64 stamps (tools/trace_gemm.py)
-    uint32_t debugFlags;
     uint32_t act;          // gate activation of GEPI_SWIGLU_BF16 (gHiddenAct)
     // Grouped (mixture-of-experts) mode, TMA-staged variant only: the weight matrix is nGroups stacked [grpRows][n] matrices, the
     // activation / output rows are sorted by group; group g owns rows [grpOffset[g], grpOffset[g] + grpCount[g]) (device arrays
@@ -140,6 +132,28 @@ __device__ __forceinline__ void gmLoadAcc(float *stgW, const float (&acc0)[32], 
     __syncwarp();
 #pragma unroll
     for (int j = 0; j < 16; j++) r[j] = __float_as_uint(stgW[lane * kGmStgStride + j]);
+}
+
+// ---- epilogue of one output element, shared by every reduce path -----------------------------------------------------------
+// GEPI_RESIDUAL: the residual values of tokens [c0, c0 + N) (rows rowOff + c0 + j), all loaded before any store of the group so
+// the read-modify-writes do not form a serialised chain. Tokens at or past `end` and features past the matrix read nothing.
+template <int EPI, int N>
+__device__ __forceinline__ void gmLoadResid(const GemmArgs &a, uint32_t rowOff, uint32_t c0, uint32_t end, uint32_t f, bool fOk,
+                                            float (&resid)[N]) {
+#pragma unroll
+    for (int j = 0; j < N; j++)
+        resid[j] = (EPI == GEPI_RESIDUAL && c0 + j < end && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(rowOff + c0 + j) * a.outStride + f) : 0.f;
+}
+// Stores the finished value v of feature f into the output row starting at orow. Every lane of the warp calls it: SwiGLU pairs
+// the gate (even row) with its up value (odd row, lane ^ 1) by a shuffle and the even lane stores the bf16 product.
+template <int EPI>
+__device__ __forceinline__ void gmStore(const GemmArgs &a, size_t orow, uint32_t f, float v, float resid, bool ok, uint32_t lane) {
+    if (EPI == GEPI_SWIGLU_BF16) {
+        const float other = __shfl_xor_sync(0xffffffffu, v, 1);   // rows (2i, 2i+1) = (gate_i, up_i)
+        if (ok && !(lane & 1)) reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
+    } else if (ok) {
+        reinterpret_cast<float *>(a.out)[orow + f] = EPI == GEPI_RESIDUAL ? v + resid : v;
+    }
 }
 
 // One k-slice (64 wide) of the 128 x 64 tile: 4 x 2 wgmma (K = 16 each, +32 B per slice inside the swizzle atom; rows 64..127 of
@@ -230,27 +244,11 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcKernel(const __grid_co
             for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
                 uint32_t r[16];
                 float resid[16];
-                if (EPI == GEPI_RESIDUAL) {   // issue all residual loads of the 16-column group before any store (no serialised RMW chain)
-#pragma unroll
-                    for (int j = 0; j < 16; j++)
-                        resid[j] = (c0 + j < Teff && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(tok0 + c0 + j) * a.outStride + f) : 0.f;
-                }
+                gmLoadResid<EPI>(a, tok0, c0, Teff, f, fOk, resid);
                 gmLoadAcc(stgW, acc0, acc1, lane, c0, r);
 #pragma unroll
-                for (int j = 0; j < 16; j++) {
-                    const uint32_t tok = c0 + j;
-                    const size_t orow = (size_t)(tok0 + tok) * a.outStride;
-                    const float v = __uint_as_float(r[j]);
-                    if (EPI == GEPI_SWIGLU_BF16) {
-                        const float other = __shfl_xor_sync(0xffffffffu, v, 1);   // rows (2i, 2i+1) = (gate_i, up_i)
-                        if (tok < Teff && fOk && !(lane & 1))
-                            reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
-                    } else if (tok < Teff && fOk) {
-                        if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[orow + f] = v;
-                        if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[orow + f] = v + resid[j];
-                        if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + f] = __float2bfloat16_rn(v);
-                    }
-                }
+                for (int j = 0; j < 16; j++)
+                    gmStore<EPI>(a, (size_t)(tok0 + c0 + j) * a.outStride, f, __uint_as_float(r[j]), resid[j], c0 + j < Teff && fOk, lane);
             }
         }
     } else if (warp >= 8) {
@@ -408,13 +406,8 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                     gmBarWait(&rawEmpty[rs], ph ^ 1);
                     uint8_t *dst = rawBase + (size_t)rs * kGmRawStageBytes;
                     gmBarExpectTx(&rawFull[rs], kGmRawStageBytes);
-                    if (a.debugFlags & 256u) {   // timing experiment (wrong results): the same bytes as contiguous 16 KB + 2 KB blocks
-                        tmaLoad2d(dst, &tmapQ, 0, (tile * nkq + kq) * kGmBlockM, &rawFull[rs]);
-                        tmaLoad2d(dst + kGmRawQsBytes, &tmapS, 0, (tile * nkq + kq) * kGmBlockM, &rawFull[rs]);
-                    } else {
-                        tmaLoad2d(dst, &tmapQ, kq * 128, wRow, &rawFull[rs]);                 // nibbles: 128 B per row
-                        tmaLoad2d(dst + kGmRawQsBytes, &tmapS, kq * 16, wRow, &rawFull[rs]);   // scales: 16 B per row
-                    }
+                    tmaLoad2d(dst, &tmapQ, kq * 128, wRow, &rawFull[rs]);                 // nibbles: 128 B per row
+                    tmaLoad2d(dst + kGmRawQsBytes, &tmapS, kq * 16, wRow, &rawFull[rs]);   // scales: 16 B per row
                     if (++rs == a.rawStages) { rs = 0; ph ^= 1u; }
                 }
             }
@@ -461,12 +454,8 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                 const uint32_t s = it & aMask, ph = (it >> aShift) & 1;
                 const uint32_t sb = sbM, phb = phbM;
                 if (++sbM == a.bStages) { sbM = 0; phbM ^= 1u; }
-                const bool trc = (a.debugFlags & 512u) && blockIdx.x == 0 && q == 0 && lane == 0 && it < 256;
-                if (trc) gGemmTrace[it * 4 + 0] = gmClock();
                 gmBarWait(&bFull[sb], phb);
-                if (trc) gGemmTrace[it * 4 + 1] = gmClock();
                 gmBarWait(&fullBar[s], ph);
-                if (trc) gGemmTrace[it * 4 + 2] = gmClock();
                 const uint64_t descA = wgDesc(sAddr(smem + (size_t)s * kGmATileBytes));
                 const uint64_t descB = wgDesc(sAddr(bBase + (size_t)sb * kGmBTileBytes));
                 wgFence();
@@ -478,7 +467,6 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                     if (lane == 0) gmBarArrive(&emptyBar[prevSlot]);
                 }
                 prevSlot = s;
-                if (trc) gGemmTrace[it * 4 + 3] = gmClock();
             }
             wgWait<0>();
             wgFenceAcc(acc0);
@@ -523,27 +511,16 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                     uint32_t own[16];
                     loadAcc(c0, own);
                     float resid[16];
-#pragma unroll
-                    for (int j = 0; j < 16; j++)
-                        resid[j] = (EPI == GEPI_RESIDUAL && c0 + j < tEnd && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(rowOff + c0 + j) * a.outStride + f) : 0.f;
+                    gmLoadResid<EPI>(a, rowOff, c0, tEnd, f, fOk, resid);
 #pragma unroll
                     for (int j = 0; j < 16; j++) {
                         const uint32_t tok = c0 + j;
-                        const size_t orow = (size_t)(rowOff + tok) * a.outStride;
                         float v = 0.f;
                         for (uint32_t r = 0; r < splitK; r++) {                        // rank order, own partial at position ks
                             if (r == ks) v += __uint_as_float(own[j]);
                             else if (tok < tEnd) v += recv[(((r < ks ? r : r - 1) * per) + (tok - tBeg)) * kGmBlockM + row];
                         }
-                        if (EPI == GEPI_SWIGLU_BF16) {
-                            const float other = __shfl_xor_sync(0xffffffffu, v, 1);
-                            if (fOk && tok < tEnd && !(lane & 1))
-                                reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
-                        } else if (fOk && tok < tEnd) {
-                            if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[orow + f] = v;
-                            if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[orow + f] = resid[j] + v;
-                            if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + f] = __float2bfloat16_rn(v);
-                        }
+                        gmStore<EPI>(a, (size_t)(rowOff + tok) * a.outStride, f, v, resid[j], fOk && tok < tEnd, lane);
                     }
                 }
                 continue;
@@ -583,24 +560,15 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
 #pragma unroll
                         for (int k2 = 0; k2 < 4; k2++)
                             part[j][k2] = (ok && (uint32_t)k2 < splitK) ? __ldcg(a.splitScratch + ((size_t)k2 * a.T + rowOff + tok0 + j) * a.d + f) : 0.f;
-                        res[j] = (EPI == GEPI_RESIDUAL && ok) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(rowOff + tok0 + j) * a.outStride + f) : 0.f;
                     }
+                    gmLoadResid<EPI>(a, rowOff, tok0, tEnd, f, fOk, res);
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
                         const uint32_t tok = tok0 + j;
-                        const size_t orow = (size_t)(rowOff + tok) * a.outStride;
                         float v = 0.f;
 #pragma unroll
                         for (int k2 = 0; k2 < 4; k2++) v += part[j][k2];          // fixed order -> deterministic
-                        if (EPI == GEPI_SWIGLU_BF16) {
-                            const float other = __shfl_xor_sync(0xffffffffu, v, 1);
-                            if (fOk && tok < tEnd && !(lane & 1))
-                                reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
-                        } else if (fOk && tok < tEnd) {
-                            if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[orow + f] = v;
-                            if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[orow + f] = res[j] + v;
-                            if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + f] = __float2bfloat16_rn(v);
-                        }
+                        gmStore<EPI>(a, (size_t)(rowOff + tok) * a.outStride, f, v, res[j], fOk && tok < tEnd, lane);
                     }
                 }
                 __syncwarp();
@@ -610,85 +578,14 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                 }
                 continue;
             }
-            if (EPI == GEPI_RESIDUAL_AR) {
-                // ---- GEMM + all-reduce in one kernel: the accumulator tile goes from registers straight into LL words of
-                // every rank's slot[myRank] (NVLink peer stores); then the same threads poll the slots of all source ranks for their
-                // (token, feature) cells, sum them in rank order, add the residual and clear the words.
-                const ArArgs &ar = a.ar;
-                const size_t slotBase = (size_t)(ar.parity * ar.nRanks + ar.rank) * ar.slotStride;
-                for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
-                    uint32_t r[16];
-                    loadAcc(c0, r);
-#pragma unroll
-                    for (int j = 0; j < 16; j++) {
-                        const uint32_t tok = rowOff + c0 + j;
-                        if (c0 + j < Teff && fOk) {
-                            const size_t off = slotBase + (size_t)tok * ar.dim + f;
-#pragma unroll 1
-                            for (uint32_t p = 0; p < ar.nRanks; p++) stLL(ar.slots[(ar.rank + p) % ar.nRanks] + off, r[j], 1u);
-                        }
-                    }
-                }
-                if (fOk) {
-                    uint64_t *mine = ar.slots[ar.rank];
-                    for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
-                        const uint32_t tok0 = rowOff + c0;
-                        float sum[16];
-#pragma unroll
-                        for (int j = 0; j < 16; j++) sum[j] = 0.f;
-                        for (uint32_t sr = 0; sr < ar.nRanks; sr++) {
-                            uint64_t *base = mine + (size_t)(ar.parity * ar.nRanks + sr) * ar.slotStride + f;
-                            uint2 v[16];
-                            bool all;
-                            do {   // 16 independent loads in flight per poll round
-                                all = true;
-#pragma unroll
-                                for (int j = 0; j < 16; j++) {
-                                    v[j] = (c0 + j < Teff) ? ldLL(base + (size_t)(tok0 + j) * ar.dim) : make_uint2(0u, 1u);
-                                    all = all && v[j].y != 0u;
-                                }
-                            } while (!all);
-#pragma unroll
-                            for (int j = 0; j < 16; j++) {
-                                sum[j] += __uint_as_float(v[j].x);
-                                if (c0 + j < Teff) stLL(base + (size_t)(tok0 + j) * ar.dim, 0u, 0u);
-                            }
-                        }
-#pragma unroll
-                        for (int j = 0; j < 16; j++) {
-                            if (c0 + j < Teff) {
-                                float *o = reinterpret_cast<float *>(a.out) + (size_t)(tok0 + j) * a.outStride + f;
-                                *o = __ldcg(o) + sum[j];
-                            }
-                        }
-                    }
-                }
-                continue;
-            }
             for (uint32_t c0 = 0; c0 < Teff; c0 += 16) {
                 uint32_t r[16];
                 float resid[16];
-                if (EPI == GEPI_RESIDUAL) {   // issue all residual loads of the 16-column group before any store (no serialised RMW chain)
-#pragma unroll
-                    for (int j = 0; j < 16; j++)
-                        resid[j] = (c0 + j < Teff && fOk) ? __ldcg(reinterpret_cast<const float *>(a.out) + (size_t)(rowOff + c0 + j) * a.outStride + f) : 0.f;
-                }
+                gmLoadResid<EPI>(a, rowOff, c0, Teff, f, fOk, resid);
                 loadAcc(c0, r);
 #pragma unroll
-                for (int j = 0; j < 16; j++) {
-                    const uint32_t tok = c0 + j;
-                    const size_t orow = (size_t)(rowOff + tok) * a.outStride;
-                    const float v = __uint_as_float(r[j]);
-                    if (EPI == GEPI_SWIGLU_BF16) {
-                        const float other = __shfl_xor_sync(0xffffffffu, v, 1);
-                        if (tok < Teff && fOk && !(lane & 1))
-                            reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + (f >> 1)] = __float2bfloat16_rn(gateAct(v, a.act) * other);
-                    } else if (tok < Teff && fOk) {
-                        if (EPI == GEPI_STORE_F32) reinterpret_cast<float *>(a.out)[orow + f] = v;
-                        if (EPI == GEPI_RESIDUAL) reinterpret_cast<float *>(a.out)[orow + f] = v + resid[j];
-                        if (EPI == GEPI_STORE_BF16) reinterpret_cast<__nv_bfloat16 *>(a.out)[orow + f] = __float2bfloat16_rn(v);
-                    }
-                }
+                for (int j = 0; j < 16; j++)
+                    gmStore<EPI>(a, (size_t)(rowOff + c0 + j) * a.outStride, f, __uint_as_float(r[j]), resid[j], c0 + j < Teff && fOk, lane);
             }
         }
     } else if (warp >= 8) {
@@ -708,11 +605,7 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
             for (uint32_t kq = kqBegin(ks); kq < kqBegin(ks + 1); kq++, itR++) {
                 const uint32_t rs = rsD, rph = rphD;
                 if (++rsD == a.rawStages) { rsD = 0; rphD ^= 1u; }
-                const bool trd = (a.debugFlags & 512u) && blockIdx.x == 0 && lane == 0 && !(warp & 1) && itR < 64;
-                unsigned long long *tq = gGemmTrace + 1024 + (grp * 64 + itR) * 8;
-                if (trd) tq[0] = gmClock();
                 gmBarWait(&rawFull[rs], rph);
-                if (trd) tq[1] = gmClock();
                 const uint8_t *rbase = rawBase + (size_t)rs * kGmRawStageBytes;
                 uint4 qv[2][2];
                 uint16_t sv[2][2];
@@ -727,19 +620,14 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                     }
                 }
                 // the raw chunk now lives in registers: hand the stage back to the TMA producer before the (long) conversion
-                const bool lateRelease = (a.debugFlags & 4u) != 0;
-                if (!lateRelease) {
-                    __syncwarp();
-                    if (lane == 0) gmBarArrive(&rawEmpty[rs]);
-                }
+                __syncwarp();
+                if (lane == 0) gmBarArrive(&rawEmpty[rs]);
                 const uint32_t itA = itR * 4 + grp;
                 const uint32_t s = itA & aMask, ph = (itA >> aShift) & 1;
-                if (trd) tq[2] = gmClock();
                 gmBarWait(&emptyBar[s], ph ^ 1);
-                if (trd) tq[3] = gmClock();
                 uint8_t *aTile = smem + (size_t)s * kGmATileBytes;
 #pragma unroll
-                for (int rr = 0; rr < 2 && !(a.debugFlags & 64u); rr++) {
+                for (int rr = 0; rr < 2; rr++) {
                     const uint32_t row = j + 64 * rr;
                     const uint32_t swz = row & 7;
 #pragma unroll
@@ -761,18 +649,13 @@ __global__ void __launch_bounds__(kGmThreads, 1) gemmQ40TcTmaKernel(const __grid
                                 o[sft] = *reinterpret_cast<uint32_t *>(&v);
                             }
                             const uint32_t chunk = (uint32_t)(b * 4 + c) ^ swz;
-                            if (!(a.debugFlags & 2u)) *reinterpret_cast<uint4 *>(aTile + row * 128 + chunk * 16) = make_uint4(o[0], o[1], o[2], o[3]);
+                            *reinterpret_cast<uint4 *>(aTile + row * 128 + chunk * 16) = make_uint4(o[0], o[1], o[2], o[3]);
                         }
                     }
                 }
-                if (trd) tq[4] = gmClock();
-                if (!(a.debugFlags & 1u)) asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
                 __syncwarp();
-                if (trd) tq[5] = gmClock();
-                if (lane == 0) {
-                    gmBarArrive(&fullBar[s]);
-                    if (lateRelease) gmBarArrive(&rawEmpty[rs]);
-                }
+                if (lane == 0) gmBarArrive(&fullBar[s]);
             }
         }
     }
@@ -801,7 +684,7 @@ static int launchGemm(const CUtensorMap &mapB, const CUtensorMap *mapQ, const CU
     const int variant = mapQ ? 1 : 0;
     if (smemBytes > configured[variant]) {
         if (variant) DL_CUDA_CHECK(cudaFuncSetAttribute(gemmQ40TcTmaKernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
-        else DL_CUDA_CHECK(cudaFuncSetAttribute(gemmQ40TcKernel<(EPI == GEPI_RESIDUAL_AR ? GEPI_RESIDUAL : EPI)>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
+        else DL_CUDA_CHECK(cudaFuncSetAttribute(gemmQ40TcKernel<EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
         configured[variant] = smemBytes;
     }
     cudaLaunchConfig_t cfg{};
@@ -820,7 +703,7 @@ static int launchGemm(const CUtensorMap &mapB, const CUtensorMap *mapQ, const CU
         cfg.numAttrs = 2;
     }
     if (variant) DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemmQ40TcTmaKernel<EPI>, mapB, *mapQ, *mapS, a));
-    else DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemmQ40TcKernel<(EPI == GEPI_RESIDUAL_AR ? GEPI_RESIDUAL : EPI)>, mapB, a));
+    else DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, gemmQ40TcKernel<EPI>, mapB, a));
     return 0;
 }
 
@@ -842,13 +725,6 @@ static size_t tmaGeometry(GemmArgs &a) {
     // Candidates in order of preference: {A slices, raw stages, minimum B slices}: the deeper A ring (two slices per dequant group)
     // first, then >= 4 k-slices of activations in flight.
     static const uint32_t cand[6][3] = {{8, 3, 4}, {8, 2, 4}, {4, 3, 4}, {4, 2, 4}, {8, 2, 2}, {4, 2, 2}};
-    if (const char *ea = getenv("DL_GEMM_GEOM")) {   // experiment: "A,raw,B"
-        unsigned ga = 0, gr = 0, gb = 0;
-        if (sscanf(ea, "%u,%u,%u", &ga, &gr, &gb) == 3 && (ga == 4 || ga == 8) && gr >= 2 && gr <= (unsigned)kGmRawStagesMax && gb >= 2 && gb <= ga) {
-            const size_t need = (size_t)ga * kGmATileBytes + (size_t)gr * kGmRawStageBytes + gb * bTile;
-            if (need <= budget) { a.stages = ga; a.rawStages = gr; a.bStages = gb; return need + 1024 + 1024 + kGmStgBytes; }
-        }
-    }
     for (int i = 0; i < 6; i++) {
         const uint32_t nA = cand[i][0], nRaw = cand[i][1], minB = cand[i][2];
         const size_t fixed = (size_t)nA * kGmATileBytes + (size_t)nRaw * kGmRawStageBytes;
@@ -862,7 +738,7 @@ static size_t tmaGeometry(GemmArgs &a) {
 }
 
 // Dispatch decision of gemmQ40TcV: kernel, shared-memory geometry, split-K and reduce scheme, grid. Pure host code (reads only the
-// DL_GEMM_GEOM / DL_GEMM_CLUSTER / DL_GEMM_SPLITK switches), so dl_gemm_q40_tc_plan can report what a launch with the same
+// DL_GEMM_CLUSTER / DL_GEMM_SPLITK switches), so dl_gemm_q40_tc_plan can report what a launch with the same
 // arguments runs. rc != 0: the launcher's return code for a shape it does not cover.
 struct GemmPlan {
     int rc;
@@ -900,15 +776,13 @@ static GemmPlan planGemmQ40Tc(int epi, uint32_t d, uint32_t n, uint32_t T, uint3
         if (p.stages < 2) return p;
         p.smemBytes = p.stages * stageBytes + 1024 + 512 + kGmStgBytes;
     }
-    p.rc = -10;
-    if (epi == GEPI_RESIDUAL_AR && !p.tma) return p;
     p.rc = -5;
-    if (epi < GEPI_STORE_F32 || epi > GEPI_RESIDUAL_AR) return p;
+    if (epi < GEPI_STORE_F32 || epi > GEPI_SWIGLU_BF16) return p;
     p.rc = 0;
     const uint32_t nTilesM = (d + kGmBlockM - 1) / kGmBlockM;
     const uint32_t nTT = (T + kGmTokTile - 1) / kGmTokTile;
     p.splitK = 1;
-    if (p.tma && epi != GEPI_RESIDUAL_AR) {
+    if (p.tma) {
         // small-d matrices (qkv, wo, w2) leave most SMs idle with one CTA per work item: cut K so that ~all SMs get an item
         const uint32_t nkq = n / 256;
         uint32_t sk = (uint32_t)numSms / (nTilesM * nTT);
@@ -944,31 +818,23 @@ static unsigned int *gSplitCounters = nullptr;
 static size_t gSplitScratchBytes = 0;
 
 int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride, uint32_t T,
-               void *out, uint32_t outStride, int numSms, cudaStream_t stream, bool pdl, int variant, const ArArgs *ar) {
+               void *out, uint32_t outStride, int numSms, cudaStream_t stream, bool pdl, int variant) {
     const GemmPlan p = planGemmQ40Tc(epi, d, n, T, actStride, numSms, variant);
     if (p.rc) return p.rc;
-    if (epi == GEPI_RESIDUAL_AR && !ar) return -10;
     EncodeTiledFn enc = encodeTiled();
     if (!enc) return -2;
     GemmArgs a{};
     a.act = gHiddenAct;
     a.qs = (const uint32_t *)qs; a.scales = (const __half *)scales; a.d = d; a.n = n; a.T = T;
     a.out = out; a.outStride = outStride;
-    if (ar) a.ar = *ar;
-    { const char *dbg = getenv("DL_GEMM_DEBUG"); a.debugFlags = dbg ? (uint32_t)atoi(dbg) : 0u; }
     a.stages = p.stages; a.rawStages = p.rawStages; a.bStages = p.bStages;
 
     CUtensorMap mapB, mapQ, mapS;
     if (!encode2d(enc, &mapB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, act, n, T, (uint64_t)actStride * 2, kGmBlockK, kGmTokTile, CU_TENSOR_MAP_SWIZZLE_128B))
         return -4;
     if (p.tma) {
-        if (a.debugFlags & 256u) {
-            if (!encode2d(enc, &mapQ, CU_TENSOR_MAP_DATA_TYPE_UINT8, qs, 128, (uint64_t)d * (n / 2) / 128, 128, 128, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_128B)) return -7;
-            if (!encode2d(enc, &mapS, CU_TENSOR_MAP_DATA_TYPE_UINT8, scales, 16, (uint64_t)d * (n / 16) / 16, 16, 16, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_NONE)) return -8;
-        } else {
         if (!encode2d(enc, &mapQ, CU_TENSOR_MAP_DATA_TYPE_UINT8, qs, n / 2, d, n / 2, 128, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_128B)) return -7;
         if (!encode2d(enc, &mapS, CU_TENSOR_MAP_DATA_TYPE_UINT8, scales, n / 16, d, n / 16, 16, kGmBlockM, CU_TENSOR_MAP_SWIZZLE_NONE)) return -8;
-        }
     }
     a.splitK = p.splitK;
     if (p.splitK >= 2) {
@@ -991,8 +857,6 @@ int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t
         case GEPI_STORE_F32: return launchGemm<GEPI_STORE_F32>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
         case GEPI_RESIDUAL: return launchGemm<GEPI_RESIDUAL>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
         case GEPI_SWIGLU_BF16: return launchGemm<GEPI_SWIGLU_BF16>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
-        case GEPI_STORE_BF16: return launchGemm<GEPI_STORE_BF16>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
-        case GEPI_RESIDUAL_AR: return launchGemm<GEPI_RESIDUAL_AR>(mapB, pq, ps, a, grid, p.smemBytes, stream, pdl);
     }
     return -5;
 }
@@ -1003,7 +867,7 @@ int gemmQ40TcV(int epi, const void *qs, const void *scales, uint32_t d, uint32_t
 int gemmQ40TcGrouped(int epi, const void *qs, const void *scales, uint32_t nGroups, uint32_t grpRows, uint32_t n, const void *act,
                      uint32_t actStride, uint32_t rowsTotal, uint32_t maxTokens, const int *grpCount, const int *grpOffset, void *out,
                      uint32_t outStride, int numSms, cudaStream_t stream) {
-    if (maxTokens == 0 || maxTokens > 256 || n % 256 || grpRows % 2 || (epi != GEPI_STORE_F32 && epi != GEPI_SWIGLU_BF16 && epi != GEPI_STORE_BF16)) return 1;
+    if (maxTokens == 0 || maxTokens > 256 || n % 256 || grpRows % 2 || (epi != GEPI_STORE_F32 && epi != GEPI_SWIGLU_BF16)) return 1;
     EncodeTiledFn enc = encodeTiled();
     if (!enc) return -2;
     GemmArgs a{};
@@ -1023,19 +887,13 @@ int gemmQ40TcGrouped(int epi, const void *qs, const void *scales, uint32_t nGrou
     switch (epi) {
         case GEPI_STORE_F32: return launchGemm<GEPI_STORE_F32>(mapB, &mapQ, &mapS, a, grid, smemBytes, stream, false);
         case GEPI_SWIGLU_BF16: return launchGemm<GEPI_SWIGLU_BF16>(mapB, &mapQ, &mapS, a, grid, smemBytes, stream, false);
-        case GEPI_STORE_BF16: return launchGemm<GEPI_STORE_BF16>(mapB, &mapQ, &mapS, a, grid, smemBytes, stream, false);
     }
     return -5;
 }
 
 int gemmQ40Tc(int epi, const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride, uint32_t T,
               void *out, uint32_t outStride, int numSms, cudaStream_t stream, bool pdl) {
-    return gemmQ40TcV(epi, qs, scales, d, n, act, actStride, T, out, outStride, numSms, stream, pdl, 0, nullptr);
-}
-
-int gemmQ40TcAr(const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride, uint32_t T, void *out,
-                uint32_t outStride, int numSms, cudaStream_t stream, const ArArgs &ar) {
-    return gemmQ40TcV(GEPI_RESIDUAL_AR, qs, scales, d, n, act, actStride, T, out, outStride, numSms, stream, false, 2, &ar);
+    return gemmQ40TcV(epi, qs, scales, d, n, act, actStride, T, out, outStride, numSms, stream, pdl, 0);
 }
 
 // ---- rmsnorm -> bf16 (activation operand producer) ------------------------------------------------------------------
@@ -1074,15 +932,11 @@ int launchRmsNormBf16(const float *x, uint32_t xStride, const float *w, void *y,
 
 }  // namespace dl
 
-DL_EXPORT int dl_gemm_trace_read(unsigned long long *host) {
-    return (int)cudaMemcpyFromSymbol(host, dl::gGemmTrace, sizeof(unsigned long long) * 4096);
-}
-
 // Stand-alone entry point (tests, tools): the gate activation of GEPI_SWIGLU_BF16 is passed explicitly (0 = SiLU, 1 = GELU).
 DL_EXPORT int dl_gemm_q40_tc(int epi, const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride,
                              uint32_t T, void *out, uint32_t outStride, int numSms, uint32_t hiddenAct, cudaStream_t stream, int pdl, int variant) {
     const dl::HiddenActScope a(hiddenAct);
-    return dl::gemmQ40TcV(epi, qs, scales, d, n, act, actStride, T, out, outStride, numSms, stream, pdl != 0, variant, nullptr);
+    return dl::gemmQ40TcV(epi, qs, scales, d, n, act, actStride, T, out, outStride, numSms, stream, pdl != 0, variant);
 }
 
 // What dl_gemm_q40_tc would run for these arguments (and the current DL_GEMM_* switches), without launching or allocating:

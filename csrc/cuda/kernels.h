@@ -436,11 +436,9 @@ inline uint32_t megaTraceRowSlots(uint32_t nLayers) { return megaTraceProdSlot(n
 int launchMegaDecode(MegaArgs m, int numSms, cudaStream_t stream);
 
 // tensor-core prefill GEMM (gemm_q40_tc.cu, wgmma)
-enum { GEPI_STORE_F32_ = 0, GEPI_RESIDUAL_ = 1, GEPI_SWIGLU_BF16_ = 2, GEPI_STORE_BF16_ = 3 };
+enum { GEPI_STORE_F32_ = 0, GEPI_RESIDUAL_ = 1, GEPI_SWIGLU_BF16_ = 2 };
 int gemmQ40Tc(int epi, const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride, uint32_t T,
               void *out, uint32_t outStride, int numSms, cudaStream_t stream, bool pdl);
-int gemmQ40TcAr(const void *qs, const void *scales, uint32_t d, uint32_t n, const void *act, uint32_t actStride, uint32_t T, void *out,
-                uint32_t outStride, int numSms, cudaStream_t stream, const ArArgs &ar);   // GEMM + fused all-reduce + residual
 int gemmQ40TcGrouped(int epi, const void *qs, const void *scales, uint32_t nGroups, uint32_t grpRows, uint32_t n, const void *act,
                      uint32_t actStride, uint32_t rowsTotal, uint32_t maxTokens, const int *grpCount, const int *grpOffset, void *out,
                      uint32_t outStride, int numSms, cudaStream_t stream);   // 1: shape not covered

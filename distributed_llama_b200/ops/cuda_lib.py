@@ -270,4 +270,4 @@ def decode_logprobs(words) -> tuple:
 
 PRO_RMSNORM, PRO_PLAIN = 0, 1
 EPI_STORE, EPI_RESIDUAL, EPI_SWIGLU, EPI_ARGMAX = 0, 1, 2, 3
-GEPI_STORE_F32, GEPI_RESIDUAL, GEPI_SWIGLU_BF16, GEPI_STORE_BF16 = 0, 1, 2, 3
+GEPI_STORE_F32, GEPI_RESIDUAL, GEPI_SWIGLU_BF16 = 0, 1, 2

@@ -13,8 +13,8 @@ S = sum_k |a_k w_k| of that output:
   about sqrt(1792) = 42 half-ulps of S, 2^-18.6 * S; 2^-18 * S is 64 ulps.
 * Split-K partial sums, added in f32 in rank order from 0, and the residual add: 2^-22 of the magnitudes added (at most four
   roundings of sums no larger than S + |residual| + |result|).
-* STORE_BF16 and SwiGLU store bf16: the reference rounds both ends of the interval the kernel's f32 value lies in (bf16_bracket);
-  the kernel's value must lie between them.
+* SwiGLU stores bf16: the reference rounds both ends of the interval the kernel's f32 value lies in (bf16_bracket); the
+  kernel's value must lie between them.
 * SiLU (__expf, fast division): 2^-19 relative. tanh-GELU (tanhf, f32 polynomial argument): 2^-20 * (|gelu(g)| + |g|); the
   absolute term covers the cancellation in 1 + tanh(u) for negative g. The bound on g and up carries through the derivatives
   |silu'| <= 1.1 and |gelu'| <= 1.13.
@@ -47,9 +47,8 @@ NAN_F32 = 0x7FC0DEAD          # payload written around the outputs: must survive
 NAN_BF16 = 0x7FD5
 
 # gemm_q40_tc.cu GEPI_*
-F32, RESID, SWIGLU, BF16 = 0, 1, 2, 3
-EPILOGUES = {"f32": (F32, SILU), "residual": (RESID, SILU), "swiglu-silu": (SWIGLU, SILU), "swiglu-gelu": (SWIGLU, GELU),
-             "bf16": (BF16, SILU)}
+F32, RESID, SWIGLU = 0, 1, 2
+EPILOGUES = {"f32": (F32, SILU), "residual": (RESID, SILU), "swiglu-silu": (SWIGLU, SILU), "swiglu-gelu": (SWIGLU, GELU)}
 
 T_EDGES = [1, 16, 63, 64, 65, 127, 128, 129, 192, 255, 256]
 
@@ -202,10 +201,7 @@ def check_output(epi, act_fn, got, ref, S, x0, what):
     if epi == RESID:
         r = x0.double() + ref
         return assert_within(got, r, tol + C_SUM * (x0.double().abs() + r.abs()), what)
-    if epi == BF16:
-        lo, hi = bf16_bracket(ref, tol)
-    else:
-        lo, hi = bf16_bracket(*_glu_ref(ref, tol, act_fn))
+    lo, hi = bf16_bracket(*_glu_ref(ref, tol, act_fn))
     assert_bracketed(got, lo, hi, what)
     return None
 
@@ -392,7 +388,7 @@ def test_forced_paths(path, epi_name, monkeypatch):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("epi_name", ["f32", "residual", "swiglu-gelu", "bf16"])
+@pytest.mark.parametrize("epi_name", ["f32", "residual", "swiglu-gelu"])
 def test_cross_path_identity(epi_name, monkeypatch):
     """ldg and tma without a split issue the same wgmma sequence on the same tiles; the cluster and global-scratch reduces add the
     same partials in the same order from 0. Each pair must agree bitwise."""
@@ -420,7 +416,7 @@ SHAPES = [   # (d, n, variant, num_sms or 0 = device, expected kernel)
 def test_shapes(d, n, variant, sms, kernel):
     sms = sms or _device_sms()
     c = case(d, n, 1)
-    for epi_name in ("f32", "residual", "swiglu-silu", "swiglu-gelu", "bf16"):
+    for epi_name in ("f32", "residual", "swiglu-silu", "swiglu-gelu"):
         epi, act_fn = EPILOGUES[epi_name]
         for T in (1, 63, 65, 129, 200, 256):
             p = _ops().gemm_q40_tc_plan(epi, d, n, T, num_sms=sms, variant=variant)
@@ -450,19 +446,20 @@ def test_split_scratch_reuse_and_growth(monkeypatch):
 
 @pytest.mark.gpu
 def test_unsupported_shapes_launch_nothing():
-    """Return codes of shapes the launcher rejects, with the output untouched: T = 0 and 257, n % 64 != 0, odd d, the TMA
-    variant with n % 256 != 0, actStride not a multiple of 8."""
+    """Return codes of calls the launcher rejects, with the output untouched: T = 0 and 257, n % 64 != 0, odd d, the TMA
+    variant with n % 256 != 0, actStride not a multiple of 8, an unknown epilogue (3)."""
     ops = _ops()
     cl = ops.cuda_lib
     W = Experts(1, 256, 512, 3)
     w = W.device()
     act = torch.randn(257, 520, device="cuda").bfloat16()
-    for what, d, n, T, stride, variant, rc in [("T=0", 256, 512, 0, 512, 0, -1), ("T=257", 256, 512, 257, 512, 0, -1),
-                                               ("n=480", 256, 480, 16, 512, 0, -1), ("d=255", 255, 512, 16, 512, 0, -1),
-                                               ("tma n=320", 256, 320, 16, 512, 2, -6), ("actStride=516", 256, 512, 16, 516, 0, -4)]:
+    for what, epi, d, n, T, stride, variant, rc in [("T=0", F32, 256, 512, 0, 512, 0, -1), ("T=257", F32, 256, 512, 257, 512, 0, -1),
+                                                    ("n=480", F32, 256, 480, 16, 512, 0, -1), ("d=255", F32, 255, 512, 16, 512, 0, -1),
+                                                    ("tma n=320", F32, 256, 320, 16, 512, 2, -6),
+                                                    ("actStride=516", F32, 256, 512, 16, 516, 0, -4), ("epi=3", 3, 256, 512, 16, 512, 0, -5)]:
         out = torch.full((260, 256), NAN_F32, dtype=torch.int32, device="cuda")
-        p = ops.gemm_q40_tc_plan(F32, d, n, T, act_stride=stride, num_sms=_device_sms(), variant=["auto", "ldg", "tma"][variant])
-        got = cl.lib().dl_gemm_q40_tc(F32, w.qs.data_ptr(), w.scales.data_ptr(), d, n, act.data_ptr(), stride, T, out.data_ptr(), 256,
+        p = ops.gemm_q40_tc_plan(epi, d, n, T, act_stride=stride, num_sms=_device_sms(), variant=["auto", "ldg", "tma"][variant])
+        got = cl.lib().dl_gemm_q40_tc(epi, w.qs.data_ptr(), w.scales.data_ptr(), d, n, act.data_ptr(), stride, T, out.data_ptr(), 256,
                                       _device_sms(), SILU, cl.stream_ptr(), 0, variant)
         torch.cuda.synchronize()
         assert p.rc == rc and got == rc, f"{what}: plan rc {p.rc}, launch rc {got}, expected {rc}"
