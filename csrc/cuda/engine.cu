@@ -102,7 +102,7 @@ struct Engine {
     int slotLogprobs[8] = {-1, -1, -1, -1, -1, -1, -1, -1};   // per-slot top_logprobs k (-1: no logprobs), one per slot
     int32_t *slotLpDev = nullptr, *slotLpHost = nullptr;   // [kChoiceRngSlots][kLogprobsWords] results of a slots step (device, pinned)
     bool tcAttn = true;          // prefill attention on the tensor cores (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
-    bool fusedAttn = true, fusedArgmax = true, useTma = true;   // debugging switches (DL_NO_FUSED_ATTN / DL_NO_FUSED_ARGMAX / DL_NO_TMA)
+    bool fusedAttn = true;       // debugging switch (DL_NO_FUSED_ATTN)
 };
 
 #define DL_TRY(expr)                    \
@@ -140,7 +140,7 @@ static int gemvSel(const Engine &e, int pro, int epi, int nb, const GemvArgs &a,
         const int r = gemvQ40Tma(pro, epi, nb, a, numSms, stream, pdl);
         return r == 1 ? -30 : r;
     }
-    return e.useTma ? gemvQ40Auto(pro, epi, nb, a, numSms, stream, pdl) : gemvQ40(pro, epi, nb, a, numSms, stream, pdl);
+    return gemvQ40Run(pro, epi, nb, a, numSms, stream, pdl, 0);
 }
 
 // Mixture-of-experts feed-forward of one token, all buffers explicit (the engine's and those of tests/test_gpu_moe.py).
@@ -365,7 +365,7 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
         if (logitsMode == 1) {
             a.in = e.g.x + (size_t)(nb - 1) * c.dim;
             int r = 1;
-            if (greedyAdvance && e.fusedArgmax && c.wType == 0) {
+            if (greedyAdvance && c.wType == 0) {
                 // logits + greedy sampling + position advance in one launch
                 a.argVal = e.g.argVal; a.argIdx = e.g.argIdx; a.argCounter = e.g.argCounter;
                 a.tokenOut = e.g.tokens; a.posInOut = e.g.pos; a.history = e.g.history; a.historyCap = c.seqLen;
@@ -543,8 +543,6 @@ DL_EXPORT void *dl_engine_create(const dl::EngineConfig *cfg) {
     dl::gHiddenAct = cfg->hiddenAct;
     e->layers.resize(cfg->nLayers);
     e->fusedAttn = std::getenv("DL_NO_FUSED_ATTN") == nullptr;
-    e->fusedArgmax = std::getenv("DL_NO_FUSED_ARGMAX") == nullptr;
-    e->useTma = std::getenv("DL_NO_TMA") == nullptr;
     e->tcAttn = std::getenv("DL_NO_TC_ATTN") == nullptr;
     if (e->cfg.numSms == 0) {
         int dev = 0, sms = 0;

@@ -6,7 +6,7 @@
 // 1..8 tokens per launch, one persistent CTA per SM owning a contiguous pair-aligned row tile. The weight stream is
 // 4-8x larger than q40, so the kernel is a pure streaming loop: every lane keeps kUnroll 16-byte loads in flight
 // (64 KB per SM), activations are staged once per CTA in shared memory, row sums are reduced in a fixed order.
-#include "kernels.h"
+#include "gemv_common.cuh"
 
 namespace dl {
 
@@ -34,17 +34,6 @@ template <> struct Chunk<__half> {
         }
     }
 };
-
-__device__ __forceinline__ float blockSumDense(float v, float *red) {
-    v = warpSum(v);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    float t = (lane < kDenseWarps) ? red[lane] : 0.f;
-    t = warpSum(t);
-    __syncthreads();
-    return t;
-}
 
 template <typename WT, int PRO, int EPI, int NB>
 __global__ void __launch_bounds__(kDenseThreads, 1) gemvDenseKernel(GemvArgs a) {
@@ -78,16 +67,13 @@ __global__ void __launch_bounds__(kDenseThreads, 1) gemvDenseKernel(GemvArgs a) 
                     const float4 v = x4[i];
                     ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
                 }
-                ss = blockSumDense(ss, red);
+                ss = blockSum512(ss, red);
                 inv = rsqrtf(ss / (float)a.n + a.eps);
             }
             float4 *dst = reinterpret_cast<float4 *>(xs + (size_t)t * a.n);
             for (uint32_t i = tid; i < nVec; i += kDenseThreads) {
                 float4 v = x4[i];
-                if (PRO == PRO_RMSNORM_) {
-                    const float4 w = reinterpret_cast<const float4 *>(a.normW)[i];
-                    v.x = w.x * (v.x * inv); v.y = w.y * (v.y * inv); v.z = w.z * (v.z * inv); v.w = w.w * (v.w * inv);
-                }
+                if (PRO == PRO_RMSNORM_) v = rmsScale(v, reinterpret_cast<const float4 *>(a.normW)[i], inv);
                 dst[i] = v;
             }
         }
@@ -203,16 +189,13 @@ __global__ void __launch_bounds__(kDenseThreads, 1) gemvDenseMoeKernel(GemvArgs 
                 const float4 v = x4[i];
                 ss += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
             }
-            ss = blockSumDense(ss, red);
+            ss = blockSum512(ss, red);
             inv = rsqrtf(ss / (float)a.n + a.eps);
         }
         float4 *dst = reinterpret_cast<float4 *>(xs);
         for (uint32_t i = tid; i < nVec; i += kDenseThreads) {
             float4 v = x4[i];
-            if (PRO == PRO_RMSNORM_) {
-                const float4 w = reinterpret_cast<const float4 *>(a.normW)[i];
-                v.x = w.x * (v.x * inv); v.y = w.y * (v.y * inv); v.z = w.z * (v.z * inv); v.w = w.w * (v.w * inv);
-            }
+            if (PRO == PRO_RMSNORM_) v = rmsScale(v, reinterpret_cast<const float4 *>(a.normW)[i], inv);
             dst[i] = v;
         }
         __syncthreads();
@@ -293,36 +276,17 @@ __global__ void __launch_bounds__(kDenseThreads, 1) gemvDenseMoeKernel(GemvArgs 
     }
 }
 
-template <typename Kernel>
-int launchDenseKernel(Kernel kernel, size_t &configured, const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
-    if (smemBytes > configured) {
-        DL_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
-        configured = smemBytes;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kDenseThreads);
-    cfg.dynamicSmemBytes = smemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, a));
+template <auto Kernel>
+int launchDense(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
+    DL_CUDA_CHECK(raiseSmemLimit<Kernel>(smemBytes));
+    DL_CUDA_CHECK(launchPdl(Kernel, dim3(grid), dim3(kDenseThreads), smemBytes, stream, pdl, a));
     return 0;
-}
-
-template <typename WT, int PRO, int EPI, int RPW>
-int launchDenseMoe(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
-    static size_t configured = 0;   // per instantiation
-    return launchDenseKernel(gemvDenseMoeKernel<WT, PRO, EPI, RPW>, configured, a, grid, smemBytes, stream, pdl);
 }
 
 template <typename WT>
 int dispatchDenseMoe(int pro, int epi, int rpw, const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
 #define DL_MOE_CASE(P, E, R) \
-    if (pro == P && epi == E && rpw == R) return launchDenseMoe<WT, P, E, R>(a, grid, smemBytes, stream, pdl);
+    if (pro == P && epi == E && rpw == R) return launchDense<gemvDenseMoeKernel<WT, P, E, R>>(a, grid, smemBytes, stream, pdl);
 #define DL_MOE_RPW(P, E) DL_MOE_CASE(P, E, 1) DL_MOE_CASE(P, E, 2)
     DL_MOE_RPW(PRO_RMSNORM_, EPI_SWIGLU_)
     DL_MOE_RPW(PRO_PLAIN_, EPI_MOE_DOWN_)
@@ -335,16 +299,10 @@ int dispatchDenseMoe(int pro, int epi, int rpw, const GemvArgs &a, int grid, siz
     return -3;
 }
 
-template <typename WT, int PRO, int EPI, int NB>
-int launchDense(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
-    static size_t configured = 0;   // per instantiation
-    return launchDenseKernel(gemvDenseKernel<WT, PRO, EPI, NB>, configured, a, grid, smemBytes, stream, pdl);
-}
-
 template <typename WT>
 int dispatchDense(int pro, int epi, int nb, const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
 #define DL_DENSE_CASE(P, E, N) \
-    if (pro == P && epi == E && nb == N) return launchDense<WT, P, E, N>(a, grid, smemBytes, stream, pdl);
+    if (pro == P && epi == E && nb == N) return launchDense<gemvDenseKernel<WT, P, E, N>>(a, grid, smemBytes, stream, pdl);
 #define DL_DENSE_NB(P, E) DL_DENSE_CASE(P, E, 1) DL_DENSE_CASE(P, E, 2) DL_DENSE_CASE(P, E, 4) DL_DENSE_CASE(P, E, 8)
     DL_DENSE_NB(PRO_RMSNORM_, EPI_STORE_)
     DL_DENSE_NB(PRO_PLAIN_, EPI_RESIDUAL_)

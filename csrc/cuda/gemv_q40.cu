@@ -16,27 +16,13 @@
 //   * the activation vector is normalised + quantised once per CTA into shared memory in a dp4a-friendly
 //     plane layout (conflict-free 16 B reads per lane);
 //   * deterministic reduction: per-(row,segment) partials in shared memory, summed in fixed order.
-#include "kernels.h"
+#include "gemv_common.cuh"
 
 namespace dl {
-
-enum { PRO_RMSNORM = 0, PRO_PLAIN = 1 };
-enum { EPI_STORE = 0, EPI_RESIDUAL = 1, EPI_SWIGLU = 2 };
 
 constexpr int kGemvThreads = 512;
 constexpr int kGemvWarps = kGemvThreads / 32;
 constexpr int kGemvUnroll = 8;
-
-__device__ __forceinline__ float blockSum512(float v, float *red) {
-    v = warpSum(v);
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (lane == 0) red[warp] = v;
-    __syncthreads();
-    float t = (lane < kGemvWarps) ? red[lane] : 0.f;
-    t = warpSum(t);
-    __syncthreads();
-    return t;
-}
 
 template <int PRO, int EPI, int NB>
 __global__ void __launch_bounds__(kGemvThreads, 1) gemvQ40Kernel(GemvArgs a) {
@@ -63,11 +49,6 @@ __global__ void __launch_bounds__(kGemvThreads, 1) gemvQ40Kernel(GemvArgs a) {
 
     pdlLaunchDependents();
 
-    const uint32_t *qsBase = a.qs;
-    const __half *scBase = a.scales;
-    // Expert-indexed weights need the router output -> no prefetch before the dependency wait.
-    const bool moe = a.expertIdx != nullptr;
-
     uint4 q[kGemvUnroll];
     uint16_t sc[kGemvUnroll];
     auto loadGroup = [&](uint32_t s0) {
@@ -81,22 +62,15 @@ __global__ void __launch_bounds__(kGemvThreads, 1) gemvQ40Kernel(GemvArgs a) {
                 const uint32_t blk = seg * 32 + lane;
                 if (blk < nblk) {
                     const uint64_t off = (uint64_t)(rowBase + r) * nblk + blk;
-                    q[u] = ldgStream16(qsBase + off * 4);
-                    sc[u] = ldgStreamU16(scBase + off);
+                    q[u] = ldgStream16(a.qs + off * 4);
+                    sc[u] = ldgStreamU16(a.scales + off);
                 }
             }
         }
     };
 
-    if (!moe) loadGroup(warp);
+    loadGroup(warp);
     pdlWait();
-    if (moe) {
-        // one expert per launch slot; NB == 1 on this path
-        const int e = a.expertIdx[a.slot];
-        qsBase += (uint64_t)e * a.expertQsStride;
-        scBase += (uint64_t)e * a.expertScaleStride;
-        loadGroup(warp);
-    }
 
     // ---- prologue: (rmsnorm) + q80 quantisation of the activation vector(s) into shared memory ----
     {
@@ -105,7 +79,7 @@ __global__ void __launch_bounds__(kGemvThreads, 1) gemvQ40Kernel(GemvArgs a) {
         for (int t = 0; t < NB; t++) {
             const float4 *x4 = reinterpret_cast<const float4 *>(a.in + (size_t)t * a.inStride);
             float inv = 1.f;
-            if (PRO == PRO_RMSNORM) {
+            if (PRO == PRO_RMSNORM_) {
                 float ss = 0.f;
                 for (uint32_t i = tid; i < nVec; i += kGemvThreads) {
                     const float4 v = x4[i];
@@ -122,34 +96,8 @@ __global__ void __launch_bounds__(kGemvThreads, 1) gemvQ40Kernel(GemvArgs a) {
                 const uint32_t i = base + tid;
                 const bool act = i < nVec;
                 float4 v = act ? x4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-                if (PRO == PRO_RMSNORM && act) {
-                    const float4 w = reinterpret_cast<const float4 *>(a.normW)[i];
-                    v.x = w.x * (v.x * inv); v.y = w.y * (v.y * inv); v.z = w.z * (v.z * inv); v.w = w.w * (v.w * inv);
-                }
-                float amax = fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w)));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
-                const float d = amax / 127.f;
-                const float id = d != 0.f ? 1.f / d : 0.f;
-                const int q0 = __float2int_rn(v.x * id), q1 = __float2int_rn(v.y * id);
-                const int q2 = __float2int_rn(v.z * id), q3 = __float2int_rn(v.w * id);
-                int qsum = q0 + q1 + q2 + q3;
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 1);
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 2);
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 4);
-                if (act) {
-                    const uint32_t b = i >> 3, sub = i & 7, k = sub >> 1, odd = sub & 1;
-                    uint8_t *wa = pa + (size_t)b * 16 + k * 4 + odd;
-                    uint8_t *wb = pb + (size_t)b * 16 + k * 4 + odd;
-                    wa[0] = (uint8_t)(int8_t)q0; wa[2] = (uint8_t)(int8_t)q1;
-                    wb[0] = (uint8_t)(int8_t)q2; wb[2] = (uint8_t)(int8_t)q3;
-                    if (sub == 0) {
-                        const float dq = __half2float(__float2half_rn(d));
-                        dxs[(size_t)t * nblk + b] = dq;
-                        dx8[(size_t)t * nblk + b] = dq * 8.f * (float)qsum;
-                    }
-                }
+                if (PRO == PRO_RMSNORM_ && act) v = rmsScale(v, reinterpret_cast<const float4 *>(a.normW)[i], inv);
+                q80Pack(v, i, act, pa, pb, dxs + (size_t)t * nblk, dx8 + (size_t)t * nblk);
             }
         }
     }
@@ -168,24 +116,10 @@ __global__ void __launch_bounds__(kGemvThreads, 1) gemvQ40Kernel(GemvArgs a) {
                 for (int t = 0; t < NB; t++) acc[t] = 0.f;
                 if (blk < nblk) {
                     const float dw = __half2float(__ushort_as_half(sc[u]));
-                    const uint32_t m = 0x0f0f0f0fu;
-                    const uint32_t l0 = q[u].x & m, h0 = (q[u].x >> 4) & m;
-                    const uint32_t l1 = q[u].y & m, h1 = (q[u].y >> 4) & m;
-                    const uint32_t l2 = q[u].z & m, h2 = (q[u].z >> 4) & m;
-                    const uint32_t l3 = q[u].w & m, h3 = (q[u].w >> 4) & m;
 #pragma unroll
                     for (int t = 0; t < NB; t++) {
-                        const uint4 A = planeA[(size_t)t * nblk + blk];
-                        const uint4 B = planeB[(size_t)t * nblk + blk];
-                        int dot = dp4a(l0, A.x, 0);
-                        dot = dp4a(h0, B.x, dot);
-                        dot = dp4a(l1, A.y, dot);
-                        dot = dp4a(h1, B.y, dot);
-                        dot = dp4a(l2, A.z, dot);
-                        dot = dp4a(h2, B.z, dot);
-                        dot = dp4a(l3, A.w, dot);
-                        dot = dp4a(h3, B.w, dot);
-                        acc[t] = dw * (dxs[(size_t)t * nblk + blk] * (float)dot - dx8[(size_t)t * nblk + blk]);
+                        const size_t tb = (size_t)t * nblk + blk;
+                        acc[t] = dw * (dxs[tb] * (float)q40q80Dot(q[u], planeA[tb], planeB[tb]) - dx8[tb]);
                     }
                 }
 #pragma unroll
@@ -202,29 +136,20 @@ __global__ void __launch_bounds__(kGemvThreads, 1) gemvQ40Kernel(GemvArgs a) {
     __syncthreads();
 
     // ---- epilogue: fixed-order segment sum + fused op ----
-    if (EPI == EPI_SWIGLU) {
+    if (EPI == EPI_SWIGLU_) {
         const uint32_t tilePairs = tileRows / 2;
         for (uint32_t i = tid; i < tilePairs * NB; i += kGemvThreads) {
             const uint32_t p = i / NB, t = i - p * NB;
-            float g = 0.f, up = 0.f;
-            for (uint32_t sg = 0; sg < nseg; sg++) {
-                g += partial[((size_t)(2 * p) * nseg + sg) * NB + t];
-                up += partial[((size_t)(2 * p + 1) * nseg + sg) * NB + t];
-            }
-            a.out[(size_t)t * a.outStride + pairBegin + p] = gateAct(g, a.act) * up;
+            a.out[(size_t)t * a.outStride + pairBegin + p] =
+                gateAct(segRowSum<NB>(partial, 2 * p, t, nseg), a.act) * segRowSum<NB>(partial, 2 * p + 1, t, nseg);
         }
     } else {
         for (uint32_t i = tid; i < tileRows * NB; i += kGemvThreads) {
             const uint32_t r = i / NB, t = i - r * NB;
-            float v = 0.f;
-            for (uint32_t sg = 0; sg < nseg; sg++) v += partial[((size_t)r * nseg + sg) * NB + t];
+            const float v = segRowSum<NB>(partial, r, t, nseg);
             float *o = a.out + (size_t)t * a.outStride + rowBase + r;
-            if (EPI == EPI_RESIDUAL) {
-                if (a.expertWeight) v *= a.expertWeight[t * a.kActive + a.slot];
-                *o += v;
-            } else {
-                *o = v;
-            }
+            if (EPI == EPI_RESIDUAL_) *o += v;
+            else *o = v;
         }
     }
 }
@@ -234,43 +159,17 @@ size_t gemvSmemBytes(uint32_t n, uint32_t maxTileRows, int nb) {
     return (size_t)nb * nblk * (16 + 16 + 4 + 4) + (size_t)maxTileRows * nseg * nb * 4 + 16 * 4 + 16;
 }
 
-template <int PRO, int EPI, int NB>
-static int launchGemv(const GemvArgs &a, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
-    auto kernel = gemvQ40Kernel<PRO, EPI, NB>;
-    static size_t configured = 0;   // per instantiation
-    if (smemBytes > configured) {
-        DL_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
-        configured = smemBytes;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kGemvThreads);
-    cfg.dynamicSmemBytes = smemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, a));
-    return 0;
-}
-
 int launchGemvQ40Ldg(int pro, int epi, int nb, GemvArgs a, const GemvQ40Plan &p, cudaStream_t stream, bool pdl) {
     a.act = gHiddenAct;
     a.maxTileRows = p.maxTileRows;
-    const int grid = (int)p.grid;
-    const size_t smemBytes = p.smemBytes;
-#define DL_GEMV_CASE(P, E, N) \
-    if (pro == P && epi == E && nb == N) return launchGemv<P, E, N>(a, grid, smemBytes, stream, pdl);
-#define DL_GEMV_NB(P, E) DL_GEMV_CASE(P, E, 1) DL_GEMV_CASE(P, E, 2) DL_GEMV_CASE(P, E, 4) DL_GEMV_CASE(P, E, 8)
-    DL_GEMV_NB(PRO_RMSNORM, EPI_STORE)
-    DL_GEMV_NB(PRO_PLAIN, EPI_RESIDUAL)
-    DL_GEMV_NB(PRO_RMSNORM, EPI_SWIGLU)
-    DL_GEMV_NB(PRO_PLAIN, EPI_STORE)
-    DL_GEMV_CASE(PRO_PLAIN, EPI_SWIGLU, 1)
-#undef DL_GEMV_NB
-#undef DL_GEMV_CASE
+#define DL_LAUNCH(P, E, N)                                                                                                  \
+    if (pro == P && epi == E && nb == N) {                                                                                  \
+        DL_CUDA_CHECK((raiseSmemLimit<gemvQ40Kernel<P, E, N>>(p.smemBytes)));                                               \
+        DL_CUDA_CHECK((launchPdl(gemvQ40Kernel<P, E, N>, dim3(p.grid), dim3(kGemvThreads), p.smemBytes, stream, pdl, a)));  \
+        return 0;                                                                                                           \
+    }
+    DL_GEMV_Q40_LDG_INSTANCES(DL_LAUNCH)
+#undef DL_LAUNCH
     return -3;
 }
 
@@ -317,5 +216,5 @@ DL_EXPORT int dl_gemv_q40_argmax(const void *qs, const void *scales, uint32_t d,
     a.argVal = argVal; a.argIdx = argIdx; a.argCounter = argCounter;
     a.tokenOut = tokenOut; a.posInOut = pos; a.history = history; a.historyCap = historyCap;
     a.rowOffsetGlobal = rowOffsetGlobal; a.vocabLimit = vocabLimit;
-    return dl::gemvQ40Tma(dl::PRO_RMSNORM, dl::EPI_ARGMAX_, 1, a, numSms, stream, false);
+    return dl::gemvQ40Tma(dl::PRO_RMSNORM_, dl::EPI_ARGMAX_, 1, a, numSms, stream, false);
 }

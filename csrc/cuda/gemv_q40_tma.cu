@@ -11,13 +11,9 @@
 //     of each lane is read once and reused for the 4 rows (dp4a), 4 partial sums are reduced with a 6-shuffle
 //     transposing butterfly, per-(row,segment) partials are summed in fixed order (deterministic);
 //   * full/empty mbarrier pairs recycle stages when the tile is larger than the ring (w13, logits).
-#include "kernels.h"
-#include "tma_common.cuh"
+#include "gemv_common.cuh"
 
 namespace dl {
-
-enum { PRO_RMSNORM = 0, PRO_PLAIN = 1 };
-enum { EPI_STORE = 0, EPI_RESIDUAL = 1, EPI_SWIGLU = 2, EPI_ARGMAX = 3, EPI_MOE_DOWN = 4 };
 
 struct TmaGemvGeom {
     uint32_t stageRows, nStages, stageBytes, maxTileRows;
@@ -100,7 +96,7 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
 
     // =============================== consumers ===============================
     // norm weights are constants: pull them towards L2 while we wait for the predecessor
-    if (PRO == PRO_RMSNORM) {
+    if (PRO == PRO_RMSNORM_) {
         for (uint32_t i = tid * 32; i < a.n; i += kConsumerThreads * 32)
             asm volatile("prefetch.global.L2 [%0];" ::"l"(a.normW + i));
     }
@@ -116,7 +112,7 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
         for (int t = 0; t < NB; t++) {
             const float4 *x4 = reinterpret_cast<const float4 *>(inBase + (size_t)t * a.inStride);
             float inv = 1.f;
-            if (PRO == PRO_RMSNORM) {
+            if (PRO == PRO_RMSNORM_) {
                 float ss = 0.f;
                 for (uint32_t i = tid; i < nVec; i += kConsumerThreads) {
                     const float4 v = x4[i];
@@ -131,34 +127,8 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
                 const uint32_t i = base + tid;
                 const bool act = i < nVec;
                 float4 v = act ? x4[i] : make_float4(0.f, 0.f, 0.f, 0.f);
-                if (PRO == PRO_RMSNORM && act) {
-                    const float4 w = reinterpret_cast<const float4 *>(a.normW)[i];
-                    v.x = w.x * (v.x * inv); v.y = w.y * (v.y * inv); v.z = w.z * (v.z * inv); v.w = w.w * (v.w * inv);
-                }
-                float amax = fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w)));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
-                const float d = amax / 127.f;
-                const float id = d != 0.f ? 1.f / d : 0.f;
-                const int q0 = __float2int_rn(v.x * id), q1 = __float2int_rn(v.y * id);
-                const int q2 = __float2int_rn(v.z * id), q3 = __float2int_rn(v.w * id);
-                int qsum = q0 + q1 + q2 + q3;
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 1);
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 2);
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 4);
-                if (act) {
-                    const uint32_t b = i >> 3, sub = i & 7, k = sub >> 1, odd = sub & 1;
-                    uint8_t *wa = pa + (size_t)b * 16 + k * 4 + odd;
-                    uint8_t *wb = pb + (size_t)b * 16 + k * 4 + odd;
-                    wa[0] = (uint8_t)(int8_t)q0; wa[2] = (uint8_t)(int8_t)q1;
-                    wb[0] = (uint8_t)(int8_t)q2; wb[2] = (uint8_t)(int8_t)q3;
-                    if (sub == 0) {
-                        const float dq = __half2float(__float2half_rn(d));
-                        dxs[(size_t)t * nblk + b] = dq;
-                        dx8[(size_t)t * nblk + b] = dq * 8.f * (float)qsum;
-                    }
-                }
+                if (PRO == PRO_RMSNORM_ && act) v = rmsScale(v, reinterpret_cast<const float4 *>(a.normW)[i], inv);
+                q80Pack(v, i, act, pa, pb, dxs + (size_t)t * nblk, dx8 + (size_t)t * nblk);
             }
         }
     }
@@ -191,48 +161,7 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
             const uint32_t blk = seg * 32 + lane;
             const uint32_t rl = g * kRowsPerStep;                  // first row of the group inside the stage
             float acc[kRowsPerStep][NB];
-#pragma unroll
-            for (int r = 0; r < kRowsPerStep; r++)
-#pragma unroll
-                for (int t = 0; t < NB; t++) acc[r][t] = 0.f;
-            if (blk < nblk) {
-                uint4 A[NB], B[NB];
-                float dxv[NB], dx8v[NB];
-#pragma unroll
-                for (int t = 0; t < NB; t++) {
-                    A[t] = planeA[t * nblk + blk];
-                    B[t] = planeB[t * nblk + blk];
-                    dxv[t] = dxs[t * nblk + blk];
-                    dx8v[t] = dx8[t * nblk + blk];
-                }
-                // Rows past the end of a short last stage read stale ring bytes (always inside the stage buffer because
-                // stageRows % 4 == 0); their sums are simply not stored below, so no branch is needed here.
-                const uint4 *qp = sq + rl * nblk + blk;
-                const uint16_t *sp = ss + rl * nblk + blk;
-#pragma unroll
-                for (int r = 0; r < kRowsPerStep; r++) {
-                    const uint4 q = qp[r * nblk];
-                    const float dw = __half2float(__ushort_as_half(sp[r * nblk]));
-                    // low nibbles: q & 0x0f0f0f0f; high nibbles are used in place (q & 0xf0f0f0f0 = 16 * nibble), the factor
-                    // 16 is removed with one shift after the dot product (exact: the partial sum is a multiple of 16)
-                    const uint32_t ml = 0x0f0f0f0fu, mh = 0xf0f0f0f0u;
-                    const uint32_t l0 = q.x & ml, h0 = q.x & mh, l1 = q.y & ml, h1 = q.y & mh;
-                    const uint32_t l2 = q.z & ml, h2 = q.z & mh, l3 = q.w & ml, h3 = q.w & mh;
-#pragma unroll
-                    for (int t = 0; t < NB; t++) {
-                        int lo = dp4a(l0, A[t].x, 0);
-                        int hi = dp4a(h0, B[t].x, 0);
-                        lo = dp4a(l1, A[t].y, lo);
-                        hi = dp4a(h1, B[t].y, hi);
-                        lo = dp4a(l2, A[t].z, lo);
-                        hi = dp4a(h2, B[t].z, hi);
-                        lo = dp4a(l3, A[t].w, lo);
-                        hi = dp4a(h3, B[t].w, hi);
-                        const int dot = lo + (hi >> 4);
-                        acc[r][t] = dw * (dxv[t] * (float)dot - dx8v[t]);
-                    }
-                }
-            }
+            stageStepDot<NB>(sq, ss, rl, blk, nblk, planeA, planeB, dxs, dx8, acc);
 #pragma unroll
             for (int t = 0; t < NB; t++) {
                 const float v = reduce4(acc[0][t], acc[1][t], acc[2][t], acc[3][t], lane);
@@ -252,21 +181,17 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
     consumerBarrier();
 
     // ---- epilogue ----
-    auto rowSum = [&](uint32_t r, uint32_t t) {
-        float v = 0.f;
-        for (uint32_t sg = 0; sg < nseg; sg++) v += partial[((size_t)r * nseg + sg) * NB + t];
-        return v;
-    };
-    if (EPI == EPI_SWIGLU) {
+    auto rowSum = [&](uint32_t r, uint32_t t) { return segRowSum<NB>(partial, r, t, nseg); };
+    if (EPI == EPI_SWIGLU_) {
         const uint32_t tilePairs = tileRows / 2;
         float *outBase = a.out + (size_t)slot * a.outSlotStride;
         for (uint32_t i = tid; i < tilePairs * NB; i += kConsumerThreads) {
             const uint32_t p = i / NB, t = i - p * NB;
             outBase[(size_t)t * a.outStride + pairBegin + p] = active ? gateAct(rowSum(2 * p, t), a.act) * rowSum(2 * p + 1, t) : 0.f;
         }
-    } else if (EPI == EPI_RESIDUAL || EPI == EPI_MOE_DOWN) {
+    } else if (EPI == EPI_RESIDUAL_ || EPI == EPI_MOE_DOWN_) {
         __shared__ bool sLastSlot;
-        if (EPI == EPI_MOE_DOWN) {
+        if (EPI == EPI_MOE_DOWN_) {
             // every routing slot leaves its weighted product in the scratch; the last slot CTA of a row tile sums the
             // slots in fixed order (deterministic) and carries on with the residual add / all-reduce
             const float wgt = active ? a.expertWeight[slot] : 0.f;
@@ -284,7 +209,7 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
             __threadfence();
         }
         auto value = [&](uint32_t r, uint32_t t) {
-            if (EPI == EPI_MOE_DOWN) {
+            if (EPI == EPI_MOE_DOWN_) {
                 float v = 0.f;
                 for (uint32_t j = 0; j < a.kActive; j++) v += __ldcg(a.moeScratch + (size_t)j * a.d + rowBase + r);
                 return v;
@@ -332,91 +257,28 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
             const uint32_t r = i / NB, t = i - r * NB;
             const float v = rowSum(r, t);
             a.out[(size_t)t * a.outStride + rowBase + r] = v;
-            if (EPI == EPI_ARGMAX && v > best && a.rowOffsetGlobal + rowBase + r < a.vocabLimit) { best = v; bestIdx = (int)(a.rowOffsetGlobal + rowBase + r); }   // rows ascend per thread
+            if (EPI == EPI_ARGMAX_ && v > best && a.rowOffsetGlobal + rowBase + r < a.vocabLimit) { best = v; bestIdx = (int)(a.rowOffsetGlobal + rowBase + r); }   // rows ascend per thread
         }
-        if (EPI == EPI_ARGMAX) {
-            // greedy sampling fused into the logits kernel: CTA-level arg-max, then the last CTA to finish reduces
-            // the per-CTA candidates, publishes the next token and advances the position (all on the device)
-            auto better = [](float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); };
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, o);
-                if (better(ov, oi, best, bestIdx)) { best = ov; bestIdx = oi; }
-            }
-            float *sv = red;                                   // 16 floats
-            int *si = reinterpret_cast<int *>(red + 16);
-            consumerBarrier();
-            if (lane == 0) { sv[warp] = best; si[warp] = bestIdx; }
-            consumerBarrier();
-            __shared__ bool lastCta;
-            if (warp == 0) {
-                best = lane < kConsumerWarps ? sv[lane] : -INFINITY;
-                bestIdx = lane < kConsumerWarps ? si[lane] : 0x7fffffff;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, o);
-                    if (better(ov, oi, best, bestIdx)) { best = ov; bestIdx = oi; }
-                }
-                if (lane == 0) {
-                    a.argVal[blockIdx.x] = best;
-                    a.argIdx[blockIdx.x] = bestIdx;
-                    __threadfence();
-                    const unsigned int prev = atomicAdd(a.argCounter, 1u);
-                    lastCta = prev == gridDim.x - 1;
-                    if (lastCta) *a.argCounter = 0;
-                }
-            }
-            consumerBarrier();
-            if (lastCta && warp == 0) {
-                __threadfence();
-                best = -INFINITY;
-                bestIdx = 0x7fffffff;
-                for (uint32_t i = lane; i < gridDim.x; i += 32) {
-                    const float v = __ldcg(a.argVal + i);
-                    const int ix = __ldcg(a.argIdx + i);
-                    if (better(v, ix, best, bestIdx)) { best = v; bestIdx = ix; }
-                }
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, o);
-                    if (better(ov, oi, best, bestIdx)) { best = ov; bestIdx = oi; }
-                }
-                if (a.ar.nRanks > 1) {
-                    // vocabulary-parallel logits: exchange the per-rank winners over peer memory; every rank then
-                    // picks the same global token, so no token broadcast is needed afterwards
-                    const ArArgs &ar = a.ar;
-                    if (lane < ar.nRanks) stLL(ar.cand[lane] + ar.rank, __float_as_uint(best), (uint32_t)bestIdx + 1u);
-                    if (lane < ar.nRanks) {
-                        uint64_t *w = ar.cand[ar.rank] + lane;
-                        uint2 v = ldLL(w);
-                        while (v.y == 0u) v = ldLL(w);
-                        best = __uint_as_float(v.x);
-                        bestIdx = (int)(v.y - 1u);
-                        stLL(w, 0u, 0u);
-                    } else {
-                        best = -INFINITY;
-                        bestIdx = 0x7fffffff;
-                    }
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) {
-                        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                        const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, o);
-                        if (better(ov, oi, best, bestIdx)) { best = ov; bestIdx = oi; }
-                    }
-                }
-                if (lane == 0) {
-                    a.tokenOut[0] = bestIdx;
-                    const int p = a.posInOut[0] + 1;
-                    a.posInOut[0] = p;
-                    if (a.history && (uint32_t)p < a.historyCap) a.history[p] = bestIdx;
-                }
-            }
+        if (EPI == EPI_ARGMAX_) {
+            // greedy sampling fused into the logits kernel: the next token and the position advance stay on the device
+            const ArgMaxOut o{a.argVal, a.argIdx, a.argCounter, a.tokenOut, a.posInOut, a.history, a.historyCap};
+            argMaxEpilogue(best, bestIdx, red, o, a.ar, tid, [] { return false; });
         }
     }
     traceStamp(a.trace, 3);
+}
+
+// Whether gemvQ40TmaKernel (tma) or gemvQ40Kernel is compiled for (pro, epi, nb).
+static bool instantiated(bool tma, int pro, int epi, int nb) {
+#define DL_LISTED(P, E, N) \
+    if (pro == P && epi == E && nb == N) return true;
+    if (tma) {
+        DL_GEMV_Q40_TMA_INSTANCES(DL_LISTED)
+    } else {
+        DL_GEMV_Q40_LDG_INSTANCES(DL_LISTED)
+    }
+#undef DL_LISTED
+    return false;
 }
 
 // TMA-ring plan of one launch; rc 1 when the shape cannot use the TMA path.
@@ -451,10 +313,7 @@ static GemvQ40Plan planTma(int pro, int epi, int nb, uint32_t d, uint32_t n, int
     if (stages > need) stages = need;
     if (stages > kMaxStages) stages = kMaxStages;
     if (stages < 1) { p.rc = 1; return p; }
-    const bool inst = ((pro == PRO_RMSNORM && (epi == EPI_STORE || epi == EPI_SWIGLU)) || (pro == PRO_PLAIN && (epi == EPI_RESIDUAL || epi == EPI_STORE)))
-                          ? (nb == 1 || nb == 2 || nb == 4 || nb == 8)
-                          : nb == 1 && ((pro == PRO_PLAIN && (epi == EPI_SWIGLU || epi == EPI_MOE_DOWN)) || (pro == PRO_RMSNORM && epi == EPI_ARGMAX));
-    if (!inst) { p.rc = -3; return p; }
+    if (!instantiated(true, pro, epi, nb)) { p.rc = -3; return p; }
     p.kernel = 2;
     p.grid = grid;
     p.maxTileRows = maxTileRows;
@@ -479,7 +338,7 @@ GemvQ40Plan planGemvQ40(int pro, int epi, int nb, uint32_t d, uint32_t n, int nu
     const size_t smemBytes = gemvSmemBytes(n, p.maxTileRows, nb);
     if (smemBytes > 227 * 1024) {
         // no kernel holds nb tokens: the tokens of STORE / RESIDUAL / SWIGLU are independent, so two launches of nb / 2 are exact
-        if (split && nb > 1 && moeCtasPerSlot == 0 && (epi == EPI_STORE || epi == EPI_RESIDUAL || epi == EPI_SWIGLU)) {
+        if (split && nb > 1 && moeCtasPerSlot == 0 && (epi == EPI_STORE_ || epi == EPI_RESIDUAL_ || epi == EPI_SWIGLU_)) {
             GemvQ40Plan h = planGemvQ40(pro, epi, nb / 2, d, n, numSms, impl, split);
             if (h.rc == 0) {
                 h.launches *= 2;
@@ -489,35 +348,10 @@ GemvQ40Plan planGemvQ40(int pro, int epi, int nb, uint32_t d, uint32_t n, int nu
         p.rc = -2;
         return p;
     }
-    const bool inst = (pro == PRO_RMSNORM && (epi == EPI_STORE || epi == EPI_SWIGLU)) || (pro == PRO_PLAIN && (epi == EPI_RESIDUAL || epi == EPI_STORE))
-                          ? (nb == 1 || nb == 2 || nb == 4 || nb == 8)
-                          : nb == 1 && pro == PRO_PLAIN && epi == EPI_SWIGLU;
-    if (!inst) { p.rc = -3; return p; }
+    if (!instantiated(false, pro, epi, nb)) { p.rc = -3; return p; }
     p.kernel = 1;
     p.smemBytes = (uint32_t)smemBytes;
     return p;
-}
-
-template <int PRO, int EPI, int NB>
-static int launchTma(const GemvArgs &a, const TmaGemvGeom &geo, int grid, size_t smemBytes, cudaStream_t stream, bool pdl) {
-    auto kernel = gemvQ40TmaKernel<PRO, EPI, NB>;
-    static size_t configured = 0;
-    if (smemBytes > configured) {
-        DL_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
-        configured = smemBytes;
-    }
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kTmaThreads);
-    cfg.dynamicSmemBytes = smemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    DL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, a, geo));
-    return 0;
 }
 
 int launchGemvQ40Tma(int pro, int epi, int nb, GemvArgs a, const GemvQ40Plan &p, cudaStream_t stream, bool pdl) {
@@ -528,20 +362,14 @@ int launchGemvQ40Tma(int pro, int epi, int nb, GemvArgs a, const GemvQ40Plan &p,
     geo.stageRows = p.stageRows;
     geo.nStages = p.nStages;
     geo.stageBytes = (p.stageRows * (a.n / 32) * 18 + 127) / 128 * 128;
-    const int grid = (int)p.grid;
-    const size_t smemBytes = p.smemBytes;
-#define DL_TMA_CASE(P, E, N) \
-    if (pro == P && epi == E && nb == N) return launchTma<P, E, N>(a, geo, grid, smemBytes, stream, pdl);
-#define DL_TMA_NB(P, E) DL_TMA_CASE(P, E, 1) DL_TMA_CASE(P, E, 2) DL_TMA_CASE(P, E, 4) DL_TMA_CASE(P, E, 8)
-    DL_TMA_NB(PRO_RMSNORM, EPI_STORE)
-    DL_TMA_NB(PRO_PLAIN, EPI_RESIDUAL)
-    DL_TMA_NB(PRO_RMSNORM, EPI_SWIGLU)
-    DL_TMA_NB(PRO_PLAIN, EPI_STORE)
-    DL_TMA_CASE(PRO_PLAIN, EPI_SWIGLU, 1)
-    DL_TMA_CASE(PRO_RMSNORM, EPI_ARGMAX, 1)
-    DL_TMA_CASE(PRO_PLAIN, EPI_MOE_DOWN, 1)
-#undef DL_TMA_NB
-#undef DL_TMA_CASE
+#define DL_LAUNCH(P, E, N)                                                                                                        \
+    if (pro == P && epi == E && nb == N) {                                                                                        \
+        DL_CUDA_CHECK((raiseSmemLimit<gemvQ40TmaKernel<P, E, N>>(p.smemBytes)));                                                  \
+        DL_CUDA_CHECK((launchPdl(gemvQ40TmaKernel<P, E, N>, dim3(p.grid), dim3(kTmaThreads), p.smemBytes, stream, pdl, a, geo))); \
+        return 0;                                                                                                                 \
+    }
+    DL_GEMV_Q40_TMA_INSTANCES(DL_LAUNCH)
+#undef DL_LAUNCH
     return -3;
 }
 

@@ -39,7 +39,7 @@ struct GemvArgs {
     uint32_t inStride, outStride;
     uint32_t maxTileRows;
     const int *expertIdx;
-    uint32_t slot, kActive;
+    uint32_t kActive;
     uint64_t expertQsStride, expertScaleStride;
     const float *expertWeight;
     // EPI_ARGMAX (TMA kernel, nb == 1): logits are stored and the greedy token is selected in the same launch
@@ -79,14 +79,8 @@ int launchGemvQ40Tma(int pro, int epi, int nb, GemvArgs a, const GemvQ40Plan &p,
 // Plans and launches. A batch is split only on one rank (ar.nRanks <= 1), outside expert launches and for the STORE, RESIDUAL and
 // SWIGLU epilogues, whose tokens are independent; the in-kernel all-reduce indexes its slots per token.
 int gemvQ40Run(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl, int impl);
-inline int gemvQ40(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl) {       // per-thread loads
-    return gemvQ40Run(pro, epi, nb, a, numSms, stream, pdl, 1);
-}
 inline int gemvQ40Tma(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl) {    // 1: shape unsupported
     return gemvQ40Run(pro, epi, nb, a, numSms, stream, pdl, 2);
-}
-inline int gemvQ40Auto(int pro, int epi, int nb, const GemvArgs &a, int numSms, cudaStream_t stream, bool pdl) {
-    return gemvQ40Run(pro, epi, nb, a, numSms, stream, pdl, 0);
 }
 
 // f32 / f16 weight files (gemv_dense.cu): wtype 1 = f32, 2 = f16; a.qs is the row-major [d][n] matrix
@@ -465,6 +459,15 @@ inline cudaError_t launchPdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, si
     attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
     cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
+}
+// Raises Kernel's dynamic shared-memory limit to `bytes` when a launch needs more than any earlier one (one record per kernel).
+template <auto Kernel>
+inline cudaError_t raiseSmemLimit(size_t bytes) {
+    static size_t configured = 0;
+    if (bytes <= configured) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e == cudaSuccess) configured = bytes;
+    return e;
 }
 
 int launchArResidual(float *x, const float *partial, uint32_t dim, uint32_t T, const ArArgs &ar, cudaStream_t stream, bool pdl = false);   // x += all-reduce(partial)

@@ -22,8 +22,7 @@
 // The kernel takes over the roles of NnExecutor's step loop + barriers (reference src/nn/nn-executor.cpp:137-175) on the GPU.
 #include <type_traits>
 
-#include "kernels.h"
-#include "tma_common.cuh"
+#include "gemv_common.cuh"
 
 namespace dl {
 
@@ -283,34 +282,8 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
                 if (vecBase + k * kConsumerThreads >= nVec) break;     // block-uniform
                 const bool act = i < nVec;
                 float4 v = xv[k];
-                if (PRO == PRO_RMSNORM_ && act) {
-                    const float4 w = wv[PRO == PRO_RMSNORM_ ? k : 0];
-                    v.x = w.x * (v.x * inv); v.y = w.y * (v.y * inv); v.z = w.z * (v.z * inv); v.w = w.w * (v.w * inv);
-                }
-                float amax = fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w)));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 1));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 2));
-                amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, 4));
-                const float dq = amax / 127.f;
-                const float id = dq != 0.f ? 1.f / dq : 0.f;
-                const int q0 = __float2int_rn(v.x * id), q1 = __float2int_rn(v.y * id);
-                const int q2 = __float2int_rn(v.z * id), q3 = __float2int_rn(v.w * id);
-                int qsum = q0 + q1 + q2 + q3;
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 1);
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 2);
-                qsum += __shfl_xor_sync(0xffffffffu, qsum, 4);
-                if (act) {
-                    const uint32_t b = i >> 3, sub = i & 7, kk = sub >> 1, odd = sub & 1;
-                    uint8_t *wa = pa + (size_t)b * 16 + kk * 4 + odd;
-                    uint8_t *wb = pb + (size_t)b * 16 + kk * 4 + odd;
-                    wa[0] = (uint8_t)(int8_t)q0; wa[2] = (uint8_t)(int8_t)q1;
-                    wb[0] = (uint8_t)(int8_t)q2; wb[2] = (uint8_t)(int8_t)q3;
-                    if (sub == 0) {
-                        const float dr = __half2float(__float2half_rn(dq));
-                        dxs[b] = dr;
-                        dx8[b] = dr * 8.f * (float)qsum;
-                    }
-                }
+                if (PRO == PRO_RMSNORM_ && act) v = rmsScale(v, wv[PRO == PRO_RMSNORM_ ? k : 0], inv);
+                q80Pack(v, i, act, pa, pb, dxs, dx8);
             }
         }
     }
@@ -332,28 +305,8 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
         uint32_t g = (firstStep * P.recipNseg) >> 16, seg = firstStep - g * nseg;   // firstStep / nseg, firstStep % nseg
         mbarWait(&sm.fullBar[st], ring.par);
         // two steps are processed together (independent dependency chains -> the LDS/IDP/SHFL latencies overlap)
-        auto stepDot = [&](uint32_t g_, uint32_t seg_, float (&acc)[kRowsPerStep]) {
-            const uint32_t blk = seg_ * 32 + lane;
-            const uint32_t rl = g_ * kRowsPerStep;
-#pragma unroll
-            for (int r = 0; r < kRowsPerStep; r++) acc[r] = 0.f;
-            if (blk < nblk) {
-                const uint4 A = planeA[blk], B = planeB[blk];
-                const float dxv = dxs[blk], dx8v = dx8[blk];
-                const uint4 *qp = sq + rl * nblk + blk;
-                const uint16_t *sp = ss + rl * nblk + blk;
-#pragma unroll
-                for (int r = 0; r < kRowsPerStep; r++) {
-                    const uint4 q = qp[r * nblk];
-                    const float dw = __half2float(__ushort_as_half(sp[r * nblk]));
-                    const uint32_t ml = 0x0f0f0f0fu, mh = 0xf0f0f0f0u;
-                    int lo = dp4a(q.x & ml, A.x, 0), hi = dp4a(q.x & mh, B.x, 0);
-                    lo = dp4a(q.y & ml, A.y, lo); hi = dp4a(q.y & mh, B.y, hi);
-                    lo = dp4a(q.z & ml, A.z, lo); hi = dp4a(q.z & mh, B.z, hi);
-                    lo = dp4a(q.w & ml, A.w, lo); hi = dp4a(q.w & mh, B.w, hi);
-                    acc[r] = dw * (dxv * (float)(lo + (hi >> 4)) - dx8v);
-                }
-            }
+        auto stepDot = [&](uint32_t g_, uint32_t seg_, float (&acc)[kRowsPerStep][1]) {
+            stageStepDot<1>(sq, ss, g_ * kRowsPerStep, seg_ * 32 + lane, nblk, planeA, planeB, dxs, dx8, acc);
         };
         auto stepStore = [&](uint32_t g_, uint32_t seg_, float v) {
             const uint32_t rl = g_ * kRowsPerStep;
@@ -371,20 +324,20 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
         for (; s + kConsumerWarps < nSteps; s += 2 * kConsumerWarps) {
             uint32_t g2 = g, seg2 = seg;
             advance(g2, seg2);
-            float a0[kRowsPerStep], a1[kRowsPerStep];
+            float a0[kRowsPerStep][1], a1[kRowsPerStep][1];
             stepDot(g, seg, a0);
             stepDot(g2, seg2, a1);
-            const float v0 = reduce4(a0[0], a0[1], a0[2], a0[3], lane);
-            const float v1 = reduce4(a1[0], a1[1], a1[2], a1[3], lane);
+            const float v0 = reduce4(a0[0][0], a0[1][0], a0[2][0], a0[3][0], lane);
+            const float v1 = reduce4(a1[0][0], a1[1][0], a1[2][0], a1[3][0], lane);
             stepStore(g, seg, v0);
             stepStore(g2, seg2, v1);
             g = g2; seg = seg2;
             advance(g, seg);
         }
         if (s < nSteps) {
-            float a0[kRowsPerStep];
+            float a0[kRowsPerStep][1];
             stepDot(g, seg, a0);
-            stepStore(g, seg, reduce4(a0[0], a0[1], a0[2], a0[3], lane));
+            stepStore(g, seg, reduce4(a0[0][0], a0[1][0], a0[2][0], a0[3][0], lane));
         }
         __syncwarp();
         if (lane == 0) mbarArrive(&sm.emptyBar[st]);
@@ -394,11 +347,7 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
     stamp();   // main loop done
 
     // ---- epilogue ----
-    auto rowSum = [&](uint32_t r) {
-        float v = 0.f;
-        for (uint32_t sg = 0; sg < nseg; sg++) v += partial[r * nseg + sg];
-        return v;
-    };
+    auto rowSum = [&](uint32_t r) { return segRowSum<1>(partial, r, 0, nseg); };
     if (EPI == EPI_SWIGLU_) {
         for (uint32_t p = tid; p < tileRows / 2; p += kConsumerThreads) outF[pairBegin + p] = gateAct(rowSum(2 * p), m.act) * rowSum(2 * p + 1);
     } else if (EPI == EPI_STORE_) {
@@ -447,82 +396,9 @@ __device__ void megaGemv(const MegaArgs &m, const MegaSmem &sm, const MegaPhase 
             if (EPI == EPI_ARGMAX_ && v > best && m.rowOffsetGlobal + rowBase + r < m.vocabLimit) { best = v; bestIdx = (int)(m.rowOffsetGlobal + rowBase + r); }
         }
         if (EPI == EPI_ARGMAX_) {
-            auto better = [](float v, int i, float bv, int bi) { return v > bv || (v == bv && i < bi); };
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, o);
-                if (better(ov, oi, best, bestIdx)) { best = ov; bestIdx = oi; }
-            }
-            float *sv = red;
-            int *si = reinterpret_cast<int *>(red + 16);
-            consumerBarrier();
-            if (lane == 0) { sv[warp] = best; si[warp] = bestIdx; }
-            consumerBarrier();
-            __shared__ bool lastCta;
-            if (warp == 0) {
-                best = lane < kConsumerWarps ? sv[lane] : -INFINITY;
-                bestIdx = lane < kConsumerWarps ? si[lane] : 0x7fffffff;
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, o);
-                    if (better(ov, oi, best, bestIdx)) { best = ov; bestIdx = oi; }
-                }
-                if (lane == 0) {
-                    m.argVal[blockIdx.x] = best;
-                    m.argIdx[blockIdx.x] = bestIdx;
-                    __threadfence();
-                    const unsigned int prev = atomicAdd(m.argCounter, 1u);
-                    lastCta = prev == gridDim.x - 1;
-                    if (lastCta) *m.argCounter = 0;
-                }
-            }
-            consumerBarrier();
-            if (lastCta && warp == 0) {
-                __threadfence();
-                best = -INFINITY;
-                bestIdx = 0x7fffffff;
-                for (uint32_t i = lane; i < gridDim.x; i += 32) {
-                    const float v = __ldcg(m.argVal + i);
-                    const int ix = __ldcg(m.argIdx + i);
-                    if (better(v, ix, best, bestIdx)) { best = v; bestIdx = ix; }
-                }
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                    const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, o);
-                    if (better(ov, oi, best, bestIdx)) { best = ov; bestIdx = oi; }
-                }
-                if (m.ar.nRanks > 1) {
-                    const ArArgs &ar = m.ar;
-                    if (lane < ar.nRanks) stLL(ar.cand[lane] + ar.rank, __float_as_uint(best), (uint32_t)bestIdx + 1u);
-                    if (lane < ar.nRanks) {
-                        uint64_t *w = ar.cand[ar.rank] + lane;
-                        uint2 v = ldLL(w);
-                        SpinGuard g(m.abortFlag);
-                        while (v.y == 0u && !g.tick()) v = ldLL(w);
-                        best = __uint_as_float(v.x);
-                        bestIdx = (int)(v.y - 1u);
-                        stLL(w, 0u, 0u);
-                    } else {
-                        best = -INFINITY;
-                        bestIdx = 0x7fffffff;
-                    }
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) {
-                        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
-                        const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, o);
-                        if (better(ov, oi, best, bestIdx)) { best = ov; bestIdx = oi; }
-                    }
-                }
-                if (lane == 0 && m.greedyAdvance) {
-                    m.tokens[0] = bestIdx;
-                    const int p = m.pos[0] + 1;
-                    m.pos[0] = p;
-                    if (m.history && (uint32_t)p < m.seqLen) m.history[p] = bestIdx;
-                }
-            }
+            const ArgMaxOut o{m.argVal, m.argIdx, m.argCounter, m.greedyAdvance ? m.tokens : nullptr, m.pos, m.history, m.seqLen};
+            SpinGuard g(m.abortFlag);
+            argMaxEpilogue(best, bestIdx, red, o, m.ar, tid, [&g] { return g.tick(); });
         }
     }
 }
