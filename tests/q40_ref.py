@@ -6,6 +6,8 @@ and the model-level tests (tests/test_gpu_mega_shapes.py, tests/test_gpu_prefill
 * The q80 grid of decode activations, with the ambiguity of a rounding whose input is only known within an interval.
 * Checks of a kernel's values against a float64 reference with a per-element bound, or against the bf16 roundings of the two ends
   of an interval.
+* Engine-level pieces of the model tests (test_gpu_prefill_chain.py, test_gpu_batched_steps.py): random K/V caches with NaN rows,
+  the caches as the attention kernels read them, the stored K/V rows against float64, and the per-stage error / bound report.
 """
 import math
 import zlib
@@ -14,6 +16,8 @@ import numpy as np
 import torch
 
 U = 2.0 ** -24                   # unit roundoff of f32
+REL_NORM = 2.0 ** -18
+CONTROL_MIN = 10.0
 
 
 def seed_of(*key):
@@ -294,6 +298,52 @@ def gemv(raw, act, bound=True, got=None, chunk=4096):
     return y, b
 
 
+def gemv_rows(raw, acts, gots=None, chunk=4096):
+    """gemv over the rows of a batch, every chunk of the matrix dequantised once for all of them: acts holds one q80(..) per row,
+    gots (optional) the kernel's output per row. Returns one (y, bound) per row, as gemv(raw, act, got=got) computes them, except
+    that where the rounded least-squares choice of up to 10 alternatives leaves the row outside its bound, the combination that
+    fits best in every element is taken, and where none fits, the row keeps every alternative in its bound (gemv without `got`)."""
+    X = torch.stack([xq for xq, _ in acts])
+    AX = X.abs()
+    AXB = AX.view(len(acts), -1, 32).sum(2)
+    ALT = torch.cat([alt for _, alt in acts])
+    nseg = (raw.shape[1] + 31) // 32
+    ys, bs, alts = [], [], []
+    for r0 in range(0, raw.shape[0], chunk):
+        W, S = dequant(raw[r0:r0 + chunk])
+        w = W.double()
+        del W
+        ys.append(w @ X.T)
+        alts.append(w @ ALT.T)
+        w.abs_()
+        bs.append(U * (nseg + 8) * (w @ AX.T) + 72 * U * (S.double().abs() @ AXB.T))
+        del w
+    Y, A, B = torch.cat(ys), torch.cat(alts), torch.cat(bs)
+    out, k0 = [], 0
+    for i, (_, alt) in enumerate(acts):
+        a, y, b = A[:, k0:k0 + alt.shape[0]], Y[:, i], B[:, i]
+        k0 += alt.shape[0]
+        if a.shape[1]:
+            if gots is None:
+                b = b + a.abs().sum(1)
+            else:
+                d = gots[i].double() - y
+                sel = (torch.linalg.pinv(a) @ d).round().clamp(0, 1)
+                if a.shape[1] <= 10 and float(((d - a @ sel).abs() / b).max()) > 1:
+                    # the rounded least-squares fit can miss among a few alternatives of similar effect: try every combination
+                    combos = torch.tensor([[(c >> k) & 1 for k in range(a.shape[1])] for c in range(1 << a.shape[1])],
+                                          dtype=a.dtype, device=a.device)
+                    worst = torch.stack([((d - a @ c).abs() / b).max() for c in combos])
+                    sel = combos[int(worst.argmin())]
+                    if float(worst.min()) > 1:
+                        # no listed combination explains the row: keep every alternative in the bound, as gemv(got=None)
+                        out.append((y, b + a.abs().sum(1)))
+                        continue
+                y = y + a @ sel
+        out.append((y, b))
+    return out
+
+
 def attention(q_raw, K, V, n_pos, q_norm, rope_row, nh, eps, n_splits, bound=True):
     """float64 decode attention of the raw q [nh * hd] (QK-norm, RoPE) over rows [0, n_pos) of the bf16 caches K, V [n_kv, seq, hd],
     and its bound: f32 score error (sum |q k|), __expf error, and the f32 accumulation over the positions one warp walks."""
@@ -333,3 +383,143 @@ def kv_rows(R, L, qkv, rope_row):
     if L["k_norm"] is not None:
         k = rms(k, L["k_norm"], R.eps)
     return rope(k, rope_row), qkv[R.q_dim + R.kv_dim:].view(R.nkv, R.hd)
+
+
+# ---- engine-level stage checks (test_gpu_prefill_chain.py, test_gpu_batched_steps.py) -----------------------------------------
+def rope_rows(x, rows):
+    """x [T, H, hd] rotated per token by rows [T, hd/2, 2]."""
+    a, b = x[..., 0::2], x[..., 1::2]
+    c, s = rows[:, None, :, 0], rows[:, None, :, 1]
+    out = torch.empty_like(x)
+    out[..., 0::2] = a * c - b * s
+    out[..., 1::2] = a * s + b * c
+    return out
+
+
+def norm_rope(y, b, w, rows, eps):
+    """QK-norm (w, or None) and RoPE of y [T, H, hd] with error bound b, returning (value, bound): the norm carries b through its
+    derivative plus 2^-18 relative for the f32 norm; a rotated pair takes the bounds of both inputs plus 4 f32 roundings."""
+    hd = y.shape[-1]
+    if w is not None:
+        ms = (y * y).mean(-1, keepdim=True) + eps
+        yn = w * y / ms.sqrt()
+        b = w.abs() / ms.sqrt() * (b + y.abs() * (y.abs() * b).sum(-1, keepdim=True) / (hd * ms)) + REL_NORM * yn.abs()
+        y = yn
+    pair = b[..., 0::2] + b[..., 1::2] + 4 * U * (y[..., 0::2].abs() + y[..., 1::2].abs())
+    return rope_rows(y, rows), pair.repeat_interleave(2, -1)
+
+
+
+def ratio(got, want, bound):
+    r = (got.double() - want).abs() / bound
+    return float(torch.nan_to_num(r, nan=float("inf")).max())
+
+
+
+def k_rows_ok(got_k, k, kn):
+    """K rows against bf16 of the f64 rotation k of the normalised raw k `kn`: within 1 bf16 ulp plus the f32 rounding of the
+    rotation (4 roundings of the pair's magnitude, which cancellation can make exceed an ulp of the result) and, with QK-norm,
+    2^-18 of it; at most 1 in 64 off the nearest. Returns (worst error / bound, count ok)."""
+    kb = k.to(torch.bfloat16).double()
+    off = (got_k.double() - kb).abs()
+    pair = (kn[..., 0::2].abs() + kn[..., 1::2].abs()).repeat_interleave(2, -1)
+    worst_r = float((off / (bf16_ulp(kb) + (4 * U + REL_NORM) * pair)).max())
+    n_off = int((off != 0).sum())
+    return worst_r, n_off <= max(4, k.numel() // 64)
+
+
+
+def _random_caches(eng, seed):
+    """Random starting caches in the engine's storage: bf16 N(0, 1), or q80 ints in [-127, 127] with f16 scales of 0.005 .. 0.015
+    (values of about the same spread) as (K values, V values, K scales, V scales)."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    if eng.kv_cache_float_type == "bf16":
+        return ([torch.randn(c.shape, generator=g, device="cuda").to(c.dtype) for c in eng.k_cache],
+                [torch.randn(c.shape, generator=g, device="cuda").to(c.dtype) for c in eng.v_cache])
+    vals = [torch.randint(-127, 128, c.shape, generator=g, device="cuda", dtype=torch.int8) for c in eng.k_cache + eng.v_cache]
+    scales = [(torch.rand(s.shape, generator=g, device="cuda") * 0.01 + 0.005).half() for s in eng.k_scale + eng.v_scale]
+    n = len(eng.k_cache)
+    return vals[:n], vals[n:], scales[:n], scales[n:]
+
+
+def _scale_rows(eng, s):
+    """A q80 scale plane as [nKv, seq, hd / 32] (without its tail padding)."""
+    nkv, seq, hd = eng.k_cache[0].shape
+    return s[:nkv * seq * hd // 32].view(nkv, seq, hd // 32)
+
+
+def _load(eng, caches, poison_from=None):
+    """Copies the caches in; from row poison_from on, bf16 values or q80 scales hold NaN."""
+    q8 = eng.kv_cache_float_type == "q80"
+    for d, s in zip(eng.k_cache + eng.v_cache, caches[0] + caches[1]):
+        d.copy_(s)
+        if poison_from is not None and not q8:
+            d[:, poison_from:] = float("nan")
+    if q8:
+        for d, s in zip(eng.k_scale + eng.v_scale, caches[2] + caches[3]):
+            d.copy_(s)
+            if poison_from is not None:
+                _scale_rows(eng, d)[:, poison_from:] = float("nan")
+
+
+
+def attn_operands(eng, tc):
+    """Layer 0's K and V as the attention kernels multiply them: the bf16 cache as stored; q80: the tensor-core tiles widened to
+    bf16(f32(int8) x f32(f16 scale)), or the exact dequantisation the CUDA-core kernels use (f64)."""
+    if eng.kv_cache_float_type == "bf16":
+        return eng.k_cache[0], eng.v_cache[0]
+    out = []
+    for vals, sc in ((eng.k_cache[0], eng.k_scale[0]), (eng.v_cache[0], eng.v_scale[0])):
+        nkv, seq, hd = vals.shape
+        x = vals.float().view(nkv, seq, hd // 32, 32) * _scale_rows(eng, sc).float()[..., None]
+        out.append(x.view(nkv, seq, hd).bfloat16() if tc else x.view(nkv, seq, hd).double())
+    return out
+
+
+def check_kv_rows(eng, st, tag, p, k, kn, v):
+    """The K/V rows layer 0 stored at p .. p + T - 1 against the f64 K rows k (the rotation of the normalised raw k `kn`) and the
+    raw V rows v, each [T, nKv, hd]. bf16: k_rows_ok, V exactly bf16(v). q80: every 32-block's f16 scale within one f16 step of
+    f16(amax / 127), every int within 0.5 of x / (amax / 127), plus 1e-3 and, for K, the f32 rounding of the rotation in units
+    of the scale; the ratio is the worst int distance over that bound."""
+    T = k.shape[0]
+    if eng.kv_cache_float_type == "bf16":
+        Kc, Vc = eng.k_cache[0], eng.v_cache[0]
+        r, ok = k_rows_ok(Kc[:, p:p + T].transpose(0, 1), k, kn)
+        assert ok, f"{tag} p={p}: K rows off the nearest bf16 too often"
+        st.r(f"{tag} k rows", r)
+        assert torch.equal(Vc[:, p:p + T].transpose(0, 1), v.float().to(torch.bfloat16)), f"{tag} p={p}: V rows are not bf16(v)"
+        return
+    pair = (kn[..., 0::2].abs() + kn[..., 1::2].abs()).repeat_interleave(2, -1)
+    for name, x, err, vals, sc in (("k", k, (4 * U + REL_NORM) * pair, eng.k_cache[0], eng.k_scale[0]),
+                                   ("v", v, torch.zeros_like(v), eng.v_cache[0], eng.v_scale[0])):
+        xb = x.reshape(T, -1, 32)
+        d = xb.abs().amax(-1, keepdim=True) / 127
+        got_s = _scale_rows(eng, sc)[:, p:p + T].transpose(0, 1).reshape(T, -1, 1).double()
+        want_s = d.half().double()
+        st.r(f"{tag} q80 {name} scales", ratio(got_s, want_s, want_s * 2.0 ** -10 + 1e-30))
+        q = vals[:, p:p + T].transpose(0, 1).reshape(T, -1, 32).double()
+        t = torch.where(d > 0, xb / d.clamp_min(1e-300), torch.zeros_like(xb))
+        slack = 1e-3 + torch.where(d > 0, err.reshape(T, -1, 32) / d.clamp_min(1e-300), torch.zeros_like(xb))
+        st.r(f"{tag} q80 {name} ints", ratio(q, t, 0.5 + slack))
+
+
+
+class Stats:
+    def __init__(self):
+        self.ratios, self.controls = {}, {}
+
+    def r(self, k, v):
+        self.ratios[k] = max(self.ratios.get(k, 0.0), v)
+
+    def c(self, k, v):
+        """A negative control counts where it lands furthest: the check fails by that factor if the kernel has that fault."""
+        self.controls[k] = max(self.controls.get(k, 0.0), v)
+
+    def report(self, tag):
+        print(f"\n[{tag}] worst error / bound: " + ", ".join(f"{k} {v:.3f}" for k, v in self.ratios.items()))
+        if self.controls:
+            print(f"[{tag}] negative control / bound: " + ", ".join(f"{k} {v:.0f}" for k, v in self.controls.items()))
+        for k, v in self.ratios.items():
+            assert v <= 1.0, f"{tag}: {k} exceeds its bound ({v:.3f})"
+        for k, v in self.controls.items():
+            assert v >= CONTROL_MIN, f"{tag}: the negative control '{k}' is only {v:.1f}x its bound"

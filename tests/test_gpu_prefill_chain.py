@@ -55,18 +55,17 @@ import time
 import pytest
 import torch
 
-from q40_ref import (U, Ref, attention, bf16_ulp, f64_to_bf16, gemv, kv_rows, q40_parts, q80, rms, silu, swiglu_ref,
+from q40_ref import (REL_NORM, U, Ref, Stats, _load, _random_caches, _scale_rows, attention, attn_operands, bf16_ulp,
+                     check_kv_rows, f64_to_bf16, gemv, kv_rows, norm_rope, q40_parts, q80, ratio, rms, rope_rows, silu, swiglu_ref,
                      w_tc_of)
 
 SEQ = 4096
 C_ACC = 2.0 ** -18
 K_ACC = 12288                      # the accumulation bound grows linearly with K beyond this many columns (see the docstring)
 C_SUM = 2.0 ** -22
-REL_NORM = 2.0 ** -18
 TOL_TC = 2.0 ** -9 + 2.0 ** -14
 TOL_FALLBACK = 2e-4
 LOG2E = 1.4426950408889634
-CONTROL_MIN = 10.0
 
 SHAPES = {
     "llama-3.1-8b": ("llama-3.1-8b", 128256),
@@ -202,29 +201,6 @@ def tc_mm(W, a, extra=None):
     return torch.cat(ys, 1), torch.cat(ss, 1), (torch.cat(es, 1) if extra is not None else 0)
 
 
-def rope_rows(x, rows):
-    """x [T, H, hd] rotated per token by rows [T, hd/2, 2]."""
-    a, b = x[..., 0::2], x[..., 1::2]
-    c, s = rows[:, None, :, 0], rows[:, None, :, 1]
-    out = torch.empty_like(x)
-    out[..., 0::2] = a * c - b * s
-    out[..., 1::2] = a * s + b * c
-    return out
-
-
-def norm_rope(y, b, w, rows, eps):
-    """QK-norm (w, or None) and RoPE of y [T, H, hd] with error bound b, returning (value, bound): the norm carries b through its
-    derivative plus 2^-18 relative for the f32 norm; a rotated pair takes the bounds of both inputs plus 4 f32 roundings."""
-    hd = y.shape[-1]
-    if w is not None:
-        ms = (y * y).mean(-1, keepdim=True) + eps
-        yn = w * y / ms.sqrt()
-        b = w.abs() / ms.sqrt() * (b + y.abs() * (y.abs() * b).sum(-1, keepdim=True) / (hd * ms)) + REL_NORM * yn.abs()
-        y = yn
-    pair = b[..., 0::2] + b[..., 1::2] + 4 * U * (y[..., 0::2].abs() + y[..., 1::2].abs())
-    return rope_rows(y, rows), pair.repeat_interleave(2, -1)
-
-
 def attn_ref(q, K, V, p0, c, shift=0):
     """softmax(c q . K^T) V of token t over positions 0 .. p0 + t + shift; q [T, H, hd], K, V [nkv, >= p0 + T, hd]. Returns
     f64 [T, H, hd] and max|V| over the visible rows [T, H]."""
@@ -251,11 +227,6 @@ def q_tc(q, hd):
     return (q.float() * s.to(q.device)).bfloat16()
 
 
-def ratio(got, want, bound):
-    r = (got.double() - want).abs() / bound
-    return float(torch.nan_to_num(r, nan=float("inf")).max())
-
-
 def bracket_ratio(got, lo, hi):
     """<= 1 iff every value lies in [lo, hi]: |got - mid| / half-width (an empty interval: 0 if equal)."""
     g = got.double()
@@ -267,18 +238,6 @@ def bracket_ratio(got, lo, hi):
 
 def bf16_bracket_rel(r, rel):
     return f64_to_bf16(r - r.abs() * rel), f64_to_bf16(r + r.abs() * rel)
-
-
-def k_rows_ok(got_k, k, kn):
-    """K rows against bf16 of the f64 rotation k of the normalised raw k `kn`: within 1 bf16 ulp plus the f32 rounding of the
-    rotation (4 roundings of the pair's magnitude, which cancellation can make exceed an ulp of the result) and, with QK-norm,
-    2^-18 of it; at most 1 in 64 off the nearest. Returns (worst error / bound, count ok)."""
-    kb = k.to(torch.bfloat16).double()
-    off = (got_k.double() - kb).abs()
-    pair = (kn[..., 0::2].abs() + kn[..., 1::2].abs()).repeat_interleave(2, -1)
-    worst_r = float((off / (bf16_ulp(kb) + (4 * U + REL_NORM) * pair)).max())
-    n_off = int((off != 0).sum())
-    return worst_r, n_off <= max(4, k.numel() // 64)
 
 
 # ------------------------------------------------------------------ engines and models ------------------------------------------------------------------
@@ -327,84 +286,11 @@ def _engine(weights, monkeypatch, no_tc_attn=False, **kw):
     return eng
 
 
-def _random_caches(eng, seed):
-    """Random starting caches in the engine's storage: bf16 N(0, 1), or q80 ints in [-127, 127] with f16 scales of 0.005 .. 0.015
-    (values of about the same spread) as (K values, V values, K scales, V scales)."""
-    g = torch.Generator(device="cuda").manual_seed(seed)
-    if eng.kv_cache_float_type == "bf16":
-        return ([torch.randn(c.shape, generator=g, device="cuda").to(c.dtype) for c in eng.k_cache],
-                [torch.randn(c.shape, generator=g, device="cuda").to(c.dtype) for c in eng.v_cache])
-    vals = [torch.randint(-127, 128, c.shape, generator=g, device="cuda", dtype=torch.int8) for c in eng.k_cache + eng.v_cache]
-    scales = [(torch.rand(s.shape, generator=g, device="cuda") * 0.01 + 0.005).half() for s in eng.k_scale + eng.v_scale]
-    n = len(eng.k_cache)
-    return vals[:n], vals[n:], scales[:n], scales[n:]
-
-
-def _scale_rows(eng, s):
-    """A q80 scale plane as [nKv, seq, hd / 32] (without its tail padding)."""
-    nkv, seq, hd = eng.k_cache[0].shape
-    return s[:nkv * seq * hd // 32].view(nkv, seq, hd // 32)
-
-
-def _load(eng, caches, poison_from=None):
-    """Copies the caches in; from row poison_from on, bf16 values or q80 scales hold NaN."""
-    q8 = eng.kv_cache_float_type == "q80"
-    for d, s in zip(eng.k_cache + eng.v_cache, caches[0] + caches[1]):
-        d.copy_(s)
-        if poison_from is not None and not q8:
-            d[:, poison_from:] = float("nan")
-    if q8:
-        for d, s in zip(eng.k_scale + eng.v_scale, caches[2] + caches[3]):
-            d.copy_(s)
-            if poison_from is not None:
-                _scale_rows(eng, d)[:, poison_from:] = float("nan")
-
-
 def _poison_planes(eng):
     """The planes that carry the NaN rows past a prompt: bf16 values, or q80 scales."""
     if eng.kv_cache_float_type == "q80":
         return [_scale_rows(eng, s) for s in eng.k_scale + eng.v_scale]
     return eng.k_cache + eng.v_cache
-
-
-def attn_operands(eng, tc):
-    """Layer 0's K and V as the attention kernels multiply them: the bf16 cache as stored; q80: the tensor-core tiles widened to
-    bf16(f32(int8) x f32(f16 scale)), or the exact dequantisation the CUDA-core kernels use (f64)."""
-    if eng.kv_cache_float_type == "bf16":
-        return eng.k_cache[0], eng.v_cache[0]
-    out = []
-    for vals, sc in ((eng.k_cache[0], eng.k_scale[0]), (eng.v_cache[0], eng.v_scale[0])):
-        nkv, seq, hd = vals.shape
-        x = vals.float().view(nkv, seq, hd // 32, 32) * _scale_rows(eng, sc).float()[..., None]
-        out.append(x.view(nkv, seq, hd).bfloat16() if tc else x.view(nkv, seq, hd).double())
-    return out
-
-
-def check_kv_rows(eng, st, tag, p, k, kn, v):
-    """The K/V rows layer 0 stored at p .. p + T - 1 against the f64 K rows k (the rotation of the normalised raw k `kn`) and the
-    raw V rows v, each [T, nKv, hd]. bf16: k_rows_ok, V exactly bf16(v). q80: every 32-block's f16 scale within one f16 step of
-    f16(amax / 127), every int within 0.5 of x / (amax / 127), plus 1e-3 and, for K, the f32 rounding of the rotation in units
-    of the scale; the ratio is the worst int distance over that bound."""
-    T = k.shape[0]
-    if eng.kv_cache_float_type == "bf16":
-        Kc, Vc = eng.k_cache[0], eng.v_cache[0]
-        r, ok = k_rows_ok(Kc[:, p:p + T].transpose(0, 1), k, kn)
-        assert ok, f"{tag} p={p}: K rows off the nearest bf16 too often"
-        st.r(f"{tag} k rows", r)
-        assert torch.equal(Vc[:, p:p + T].transpose(0, 1), v.float().to(torch.bfloat16)), f"{tag} p={p}: V rows are not bf16(v)"
-        return
-    pair = (kn[..., 0::2].abs() + kn[..., 1::2].abs()).repeat_interleave(2, -1)
-    for name, x, err, vals, sc in (("k", k, (4 * U + REL_NORM) * pair, eng.k_cache[0], eng.k_scale[0]),
-                                   ("v", v, torch.zeros_like(v), eng.v_cache[0], eng.v_scale[0])):
-        xb = x.reshape(T, -1, 32)
-        d = xb.abs().amax(-1, keepdim=True) / 127
-        got_s = _scale_rows(eng, sc)[:, p:p + T].transpose(0, 1).reshape(T, -1, 1).double()
-        want_s = d.half().double()
-        st.r(f"{tag} q80 {name} scales", ratio(got_s, want_s, want_s * 2.0 ** -10 + 1e-30))
-        q = vals[:, p:p + T].transpose(0, 1).reshape(T, -1, 32).double()
-        t = torch.where(d > 0, xb / d.clamp_min(1e-300), torch.zeros_like(xb))
-        slack = 1e-3 + torch.where(d > 0, err.reshape(T, -1, 32) / d.clamp_min(1e-300), torch.zeros_like(xb))
-        st.r(f"{tag} q80 {name} ints", ratio(q, t, 0.5 + slack))
 
 
 def _tokens(n, p0, vocab):
@@ -419,27 +305,6 @@ def _run_chunk(eng, toks, p, want):
 
 
 # ------------------------------------------------------------------ stage checks ------------------------------------------------------------------
-class Stats:
-    def __init__(self):
-        self.ratios, self.controls = {}, {}
-
-    def r(self, k, v):
-        self.ratios[k] = max(self.ratios.get(k, 0.0), v)
-
-    def c(self, k, v):
-        """A negative control counts where it lands furthest: the check fails by that factor if the kernel has that fault."""
-        self.controls[k] = max(self.controls.get(k, 0.0), v)
-
-    def report(self, tag):
-        print(f"\n[{tag}] worst error / bound: " + ", ".join(f"{k} {v:.3f}" for k, v in self.ratios.items()))
-        if self.controls:
-            print(f"[{tag}] negative control / bound: " + ", ".join(f"{k} {v:.0f}" for k, v in self.controls.items()))
-        for k, v in self.ratios.items():
-            assert v <= 1.0, f"{tag}: {k} exceeds its bound ({v:.3f})"
-        for k, v in self.controls.items():
-            assert v >= CONTROL_MIN, f"{tag}: the negative control '{k}' is only {v:.1f}x its bound"
-
-
 def check_tc_chunk(M, eng, st, toks, p, I1, I, logits, tag, tc_attn=True, second=False):
     """Stage checks of a tensor-core chunk of T = len(toks) tokens at p from its scratch (I1: the run with W2 zeroed)."""
     R, L, W = M["ref"], M["ref"].layers[0], M["tc"]
