@@ -10,6 +10,7 @@
 #include <cctype>
 #include <condition_variable>
 #include <deque>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <thread>
@@ -707,6 +708,7 @@ struct SlotJob {
     std::vector<uint32_t> slots;
     uint32_t P = 0, nPrompt = 0, limit = 0, live = 0;
     std::vector<std::vector<int32_t>> out;
+    std::map<std::pair<uint32_t, size_t>, uint32_t> promptLens;   // paged: P by (slot, cached messages), computed once
     SlotJob(HttpRequest r, ChatRequest c, const Tokenizer &tok, const std::vector<std::string> &stops)
         : req(std::move(r)), chat(std::move(c)), resp(req, chat, tok, stops) {}
 };
@@ -774,11 +776,37 @@ void ApiServer::serveParallel(int srv) {
 
     std::vector<std::shared_ptr<SlotJob>> owner(N);
     std::vector<SlotRow> rows(N);
+    // paged slots: when each slot's cache was last left idle (eviction order)
+    const bool paged = backend_.paged();
+    constexpr uint32_t kPage = 64;
+    std::vector<uint64_t> finished(N, 0);
+    uint64_t clock = 0;
     const auto release = [&](const std::shared_ptr<SlotJob> &job) {
-        for (uint32_t s : job->slots) if (owner[s] == job) { owner[s].reset(); rows[s] = SlotRow(); }
+        for (uint32_t s : job->slots)
+            if (owner[s] == job) { owner[s].reset(); rows[s] = SlotRow(); finished[s] = ++clock; }
+    };
+    // Evicts idle caches, least recently finished first and none of `keep`, until `pages` pages are free; false (nothing evicted) if
+    // even all of them would not do.
+    const auto evictFor = [&](uint32_t pages, const std::vector<uint32_t> &keep) {
+        std::vector<uint32_t> idle;
+        uint32_t avail = backend_.freePages();
+        for (uint32_t s = 0; s < N; s++)
+            if (!owner[s] && std::find(keep.begin(), keep.end(), s) == keep.end() && backend_.slotPageCount(s) > 0) {
+                idle.push_back(s);
+                avail += backend_.slotPageCount(s);
+            }
+        if (avail < pages) return false;
+        std::stable_sort(idle.begin(), idle.end(), [&](uint32_t a, uint32_t b) { return finished[a] < finished[b]; });
+        for (uint32_t s : idle) {
+            if (backend_.freePages() >= pages) break;
+            backend_.slotRelease(s);
+            caches[s].clear();
+        }
+        return true;
     };
     const auto fail = [&](const std::shared_ptr<SlotJob> &job, const std::exception &e) {
         for (uint32_t s : job->slots) caches[s].clear();   // their rows may not match what their caches say
+        if (paged) for (uint32_t s : job->slots) backend_.slotRelease(s);
         std::printf("Socket error: %s\n", e.what());
         std::fflush(stdout);
         closeConn(job->req.fd);
@@ -802,6 +830,20 @@ void ApiServer::serveParallel(int srv) {
         for (uint32_t s : free) { const size_t n = caches[s].coveredPrefix(c.messages); if (n > best) { best = n; first = s; } }
         j.slots = {first};
         for (uint32_t s : free) if (s != first && j.slots.size() < need) j.slots.push_back(s);
+        if (paged) {
+            // every slot holds rows [0, P + 64) and no more; P as preparePrompt will find it, from a copy of the cache
+            const auto key = std::make_pair(first, caches[first].coveredPrefix(c.messages));
+            if (!j.promptLens.count(key)) { NaiveCache probe = caches[first]; j.promptLens[key] = preparePrompt(gen_, tok_, probe, c.messages, L).P; }
+            const uint32_t want = std::min(L, j.promptLens[key] + kPage), pages = (want + kPage - 1) / kPage;
+            if (pages * j.slots.size() > L / kPage)
+                throw std::runtime_error("the request needs " + std::to_string(pages * j.slots.size()) + " KV-cache pages, more than the pool's " +
+                                         std::to_string(L / kPage));
+            int64_t net = 0;   // free pages the admission takes once its slots give back what they hold beyond `want`
+            for (uint32_t s : j.slots) net += (int64_t)pages - (int64_t)backend_.slotPageCount(s);
+            if (!evictFor((uint32_t)std::max<int64_t>(0, net), j.slots)) return false;
+            for (uint32_t s : j.slots) backend_.slotTrim(s, want);
+            for (uint32_t s : j.slots) backend_.slotReserve(s, want);   // cannot fail: the pages are free
+        }
         const Prompt p = preparePrompt(gen_, tok_, caches[first], c.messages, L);
         j.P = p.P;
         j.nPrompt = p.nPrompt;
@@ -818,7 +860,7 @@ void ApiServer::serveParallel(int srv) {
         }
         j.limit = L - j.P;
         if (c.maxTokens > 0) j.limit = std::min<uint32_t>(j.limit, (uint32_t)c.maxTokens);
-        if (j.limit == 0) { finish(job); return; }
+        if (j.limit == 0) { finish(job); return true; }
         j.live = (uint32_t)j.slots.size();
         for (size_t k = 0; k < j.slots.size(); k++) {
             SlotRow &r = rows[j.slots[k]];
@@ -828,6 +870,32 @@ void ApiServer::serveParallel(int srv) {
             if (need == 1) for (uint32_t i = 0; i < c.n; i++) r.choices.push_back(i);
             else r.choices.push_back((uint32_t)k);
             r.done.assign(r.choices.size(), false);
+        }
+        return true;
+    };
+    // Slot s's row has finished every completion it serves; the request finishes with its last row.
+    const auto rowDone = [&](uint32_t s) {
+        const std::shared_ptr<SlotJob> job = rows[s].job;
+        rows[s] = SlotRow();
+        if (--job->live == 0) {
+            release(job);
+            try { finish(job); } catch (const std::exception &e) { fail(job, e); }
+        }
+    };
+    // Paged: every row about to write a row past its pages reserves the next page (evicting idle caches); one that cannot ends.
+    const auto grow = [&] {
+        for (uint32_t s = 0; s < N; s++) {
+            SlotRow &r = rows[s];
+            if (!r.job) continue;
+            const uint32_t need = (uint32_t)r.pos + 1, have = backend_.slotPageCount(s);
+            const uint32_t shortPages = (need + kPage - 1) / kPage > have ? (need + kPage - 1) / kPage - have : 0;
+            if (shortPages == 0) continue;
+            std::vector<uint32_t> busy;
+            for (uint32_t t = 0; t < N; t++) if (rows[t].job) busy.push_back(t);
+            if (evictFor(shortPages, busy) && backend_.slotReserve(s, need)) continue;
+            for (size_t c = 0; c < r.choices.size(); c++) r.done[c] = true;
+            r.nDone = (uint32_t)r.choices.size();
+            rowDone(s);
         }
     };
 
@@ -847,14 +915,16 @@ void ApiServer::serveParallel(int srv) {
             const std::shared_ptr<SlotJob> job = waiting.front();
             const uint32_t need = job->chat.temperature == 0.f ? 1 : job->chat.n;
             if (free.size() < need) break;
-            waiting.pop_front();
             try {
-                admit(job, free, need);
+                if (!admit(job, free, need)) break;   // paged: its pages are not there yet; it and everything behind it wait
+                waiting.pop_front();
             } catch (const std::exception &e) {
+                waiting.pop_front();
                 release(job);
                 fail(job, e);
             }
         }
+        if (paged) grow();
         std::vector<int32_t> tokens(N, 0), pos(N, 0);
         uint32_t active = 0;
         for (uint32_t s = 0; s < N; s++)
@@ -884,13 +954,7 @@ void ApiServer::serveParallel(int srv) {
                 fail(job, e);
                 continue;
             }
-            if (r.nDone == r.choices.size()) {
-                rows[s] = SlotRow();
-                if (--j.live == 0) {
-                    release(job);
-                    try { finish(job); } catch (const std::exception &e) { fail(job, e); }
-                }
-            }
+            if (r.nDone == r.choices.size()) rowDone(s);
         }
     }
     acceptor.join();

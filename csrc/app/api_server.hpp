@@ -49,6 +49,15 @@ struct InferenceBackend {
     virtual uint32_t slotLen() const { return 0; }
     virtual void slotPrefill(uint32_t /*slot*/, const std::vector<int32_t> & /*tokens*/, uint32_t /*pos*/) { throw std::runtime_error("slots unsupported"); }
     virtual void slotCopy(uint32_t /*src*/, uint32_t /*dst*/, uint32_t /*P*/) { throw std::runtime_error("slots unsupported"); }
+    // Paged slots (paged() true: the slots share the cache as one pool of 64-row pages, csrc/cuda/engine.cu): slotReserve grows a slot
+    // to cover rows [0, rows) (false, nothing changed, when the pool is short), slotTrim keeps the pages of rows [0, rows) and frees
+    // the rest, slotRelease frees every page of a slot; freePages and slotPageCount report the pool.
+    virtual bool paged() const { return false; }
+    virtual bool slotReserve(uint32_t /*slot*/, uint32_t /*rows*/) { throw std::runtime_error("paged slots unsupported"); }
+    virtual void slotTrim(uint32_t /*slot*/, uint32_t /*rows*/) { throw std::runtime_error("paged slots unsupported"); }
+    virtual void slotRelease(uint32_t /*slot*/) { throw std::runtime_error("paged slots unsupported"); }
+    virtual uint32_t freePages() const { return 0; }
+    virtual uint32_t slotPageCount(uint32_t /*slot*/) const { return 0; }
     // seeds slot `slot`'s generator, zeroes its counts and sets its temperature (0: arg-max), top-p, penalties and logit bias
     virtual void slotSampling(uint32_t /*slot*/, uint64_t /*seed*/, float /*temperature*/, float /*topp*/, float /*presence*/, float /*frequency*/,
                               const std::vector<std::pair<int32_t, float>> & /*bias*/) { throw std::runtime_error("slots unsupported"); }

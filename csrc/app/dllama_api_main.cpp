@@ -47,6 +47,13 @@ struct EngineBackend : InferenceBackend {
     uint32_t slotLen() const override { return e.slotLen(); }
     void slotPrefill(uint32_t slot, const std::vector<int32_t> &tokens, uint32_t pos) override { e.slotPrefill(slot, tokens, pos); }
     void slotCopy(uint32_t src, uint32_t dst, uint32_t P) override { e.slotCopy(src, dst, P); }
+    bool pagedSlots = false;
+    bool paged() const override { return pagedSlots; }
+    bool slotReserve(uint32_t slot, uint32_t rows) override { return e.slotReserve(slot, rows); }
+    void slotTrim(uint32_t slot, uint32_t rows) override { e.slotTrim(slot, rows); }
+    void slotRelease(uint32_t slot) override { e.slotRelease(slot); }
+    uint32_t freePages() const override { return e.freePages(); }
+    uint32_t slotPageCount(uint32_t slot) const override { return e.slotPageCount(slot); }
     void slotSampling(uint32_t slot, uint64_t seed, float temperature, float topp, float presence, float frequency,
                       const std::vector<std::pair<int32_t, float>> &bias) override {
         e.slotSampling(slot, seed, temperature, topp, presence, frequency, bias);
@@ -83,8 +90,9 @@ struct ParallelRefused : std::runtime_error {
     using std::runtime_error::runtime_error;
 };
 
-// Why --parallel `parallel` cannot run here (empty: it can); the rules of distributed_llama_b200.api.parallel_refusal.
-std::string parallelRefusal(uint32_t parallel, uint32_t nRanks, uint32_t nExperts) {
+// Why --parallel `parallel` with slot layout `cache` cannot run here (empty: it can); the rules of distributed_llama_b200.api.parallel_refusal.
+std::string parallelRefusal(uint32_t parallel, uint32_t nRanks, uint32_t nExperts, const std::string &cache) {
+    if (cache != "split" && cache != "paged") return "--parallel-cache must be split or paged, not '" + cache + "'";
     if (parallel < 1 || parallel > kMaxChoices) return "--parallel must be from 1 to 8";
     if (parallel == 1) return "";
     if (nRanks > 1) return "--parallel > 1 runs on one GPU only (workers cannot mirror slot steps yet)";
@@ -103,12 +111,13 @@ const char *kUsage =
     "        [--kv-cache-float-type {bf16|q80}]  KV-cache storage (default bf16; q80 = int8 blocks of 32 + f16 scale)\n"
     "        [--parallel <n>]  decode up to n (1..8) chat requests together, each in its own KV-cache slot of floor(context / n)\n"
     "                       tokens; one GPU and dense models only\n"
+    "        [--parallel-cache {split|paged}]  paged: the slots share the KV cache as one pool of 64-token pages (default split)\n"
     "        [--gpus <n>]   tensor parallel over n GPUs: a supervisor forks one process per GPU (rank 0 serves HTTP) and restarts\n"
     "                       the whole job 3 s after any rank fails\n";
 
 // One attempt of rank 0 of a job (or the only process on one GPU): engine + tokenizer + HTTP server until --max-requests is reached.
 int serveOnce(const std::string &model, const std::string &tokenizer, uint32_t maxSeqLen, int gpu, const ApiConfig &cfg, TpJob &job,
-              uint32_t kvType) {
+              uint32_t kvType, const std::string &parallelCache) {
     NativeEngine engine(model, maxSeqLen, gpu, 0, job.nRanks, job.tag, [&job] { job.barrier(); }, kvType);
     Tokenizer tok(tokenizer);
     if (job.nRanks > 1) job.barrier();   // every rank has its weights
@@ -118,11 +127,12 @@ int serveOnce(const std::string &model, const std::string &tokenizer, uint32_t m
                     engine.multicast() ? "the NVSwitch multicast mapping (multimem.st)" : "NVLink peer memory");
     std::printf("💿 Weights loaded\n");
     EngineBackend backend(engine, job);
-    const std::string why = parallelRefusal(cfg.parallel, job.nRanks, engine.header().nExperts);
+    const std::string why = parallelRefusal(cfg.parallel, job.nRanks, engine.header().nExperts, parallelCache);
     if (!why.empty()) throw ParallelRefused(why);
     if (cfg.parallel > 1) {
-        engine.setSlots(cfg.parallel);
+        engine.setSlots(cfg.parallel, parallelCache == "paged");
         backend.slotCount = cfg.parallel;
+        backend.pagedSlots = parallelCache == "paged";
     }
     ApiServer server(backend, tok, cfg);
     server.serve();
@@ -138,6 +148,7 @@ int main(int argc, char **argv) {
     uint32_t maxSeqLen = 0, kvType = 0;
     int gpu = 0;
     uint32_t gpus = 1, workers = 0;
+    std::string parallelCache = "split";
     try {
         for (int i = 1; i < argc;) {
             const std::string name = argv[i];
@@ -163,6 +174,7 @@ int main(int argc, char **argv) {
             else if (name == "--gpus") gpus = (uint32_t)std::max(1, std::stoi(v));
             else if (name == "--max-requests") cfg.maxRequests = std::stoi(v);
             else if (name == "--parallel") cfg.parallel = (uint32_t)std::max(0, std::stoi(v));
+            else if (name == "--parallel-cache") parallelCache = v;
             else if (name == "--buffer-float-type" || name == "--nthreads" || name == "--net-turbo" || name == "--gpu-segments") {}
             else throw std::runtime_error("Unknown option: " + name);
             i += 2;
@@ -174,7 +186,7 @@ int main(int argc, char **argv) {
         return 1;
     }
     {
-        const std::string why = parallelRefusal(cfg.parallel, gpus + workers, 0);
+        const std::string why = parallelRefusal(cfg.parallel, gpus + workers, 0, parallelCache);
         if (!why.empty()) { std::fprintf(stderr, "%s\n", why.c_str()); return 1; }
     }
     const size_t slash = model.find_last_of("/\\");
@@ -184,7 +196,7 @@ int main(int argc, char **argv) {
         while (true) {
             try {
                 TpJob job;
-                return serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType);
+                return serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType, parallelCache);
             } catch (const ParallelRefused &e) {
                 std::fprintf(stderr, "%s\n", e.what());
                 return 1;
@@ -215,7 +227,7 @@ int main(int argc, char **argv) {
                 int rc = 1;
                 if (r == 0) {
                     try {
-                        rc = serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType);
+                        rc = serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType, parallelCache);
                         job.sendExit();
                     } catch (const std::exception &e) {
                         job.fail(e.what());

@@ -436,9 +436,25 @@ std::vector<int32_t> NativeEngine::choicesStep(const std::vector<int32_t> &token
     return out;
 }
 
-void NativeEngine::setSlots(uint32_t n) {
+void NativeEngine::setSlots(uint32_t n, bool paged) {
+    engCheck(dl_engine_set_slot_cache(impl_->engine, paged ? 1 : 0), "dl_engine_set_slot_cache");
     engCheck(dl_engine_set_slots(impl_->engine, n), "dl_engine_set_slots");
     slots_ = n;
+}
+
+bool NativeEngine::slotReserve(uint32_t slot, uint32_t rows) {
+    const int rc = dl_engine_slot_reserve(impl_->engine, slot, rows);
+    if (rc == dl::kEngineErrPoolShort) return false;
+    engCheck(rc, "dl_engine_slot_reserve");
+    return true;
+}
+
+void NativeEngine::slotTrim(uint32_t slot, uint32_t rows) { engCheck(dl_engine_slot_trim(impl_->engine, slot, rows), "dl_engine_slot_trim"); }
+void NativeEngine::slotRelease(uint32_t slot) { engCheck(dl_engine_slot_release(impl_->engine, slot), "dl_engine_slot_release"); }
+uint32_t NativeEngine::freePages() const { return dl_engine_free_pages(impl_->engine); }
+uint32_t NativeEngine::slotPageCount(uint32_t slot) const {
+    const int n = dl_engine_slot_pages(impl_->engine, slot, nullptr, 0);
+    return n > 0 ? (uint32_t)n : 0u;
 }
 
 uint32_t NativeEngine::slotLen() const { return dl_engine_slot_len(impl_->engine); }

@@ -84,8 +84,15 @@ public:
                                      float topp);
     // KV-cache slots (csrc/cuda/attn_decode.cu): n <= 8 independent sequences, each in its own floor(seqLen / n) rows of the cache, decoded
     // together by slotsStep. Single GPU, dense q40 models. Row b of a step is slot b (activeMask bit b); inactive rows return -1.
-    void setSlots(uint32_t n);
+    // paged: the slots share the cache as one pool of 64-row pages instead (engine_api.h: dl_engine_set_slot_cache); slotLen() is
+    // then 64 * floor(seqLen / 64) and a slot's rows are reserved before they are written.
+    void setSlots(uint32_t n, bool paged = false);
     uint32_t slotLen() const;
+    bool slotReserve(uint32_t slot, uint32_t rows);   // false: the pool is short (nothing changed)
+    void slotTrim(uint32_t slot, uint32_t rows);
+    void slotRelease(uint32_t slot);
+    uint32_t freePages() const;
+    uint32_t slotPageCount(uint32_t slot) const;
     void slotPrefill(uint32_t slot, const std::vector<int32_t> &tokens, uint32_t pos);
     void slotCopy(uint32_t src, uint32_t dst, uint32_t P);
     void slotSampling(uint32_t slot, uint64_t seed, float temperature, float topp, float presence, float frequency,

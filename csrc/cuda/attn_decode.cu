@@ -26,6 +26,10 @@
 // element offset s * slotStride, slotStride = nKvHeads * L * headDim. Row b of the step is slot b; its token sits at position pos[b]
 // and its K/V row pos[b] was written by ropeKvKernel (RopeKvArgs::slotStride) before slotAttnKernel runs. Row b attends to rows
 // [0, pos[b]] of its own slot and nothing else.
+//
+// Paged slots (SlotAttnArgs::pageTable): every layer plane is one pool of 64-row pages, and slot b's logical row r lives at physical
+// row table[b][r / 64] * 64 + r % 64 of the plane. slotAttnKernel stages the same 32-row tiles as for a contiguous slot, each row from
+// its own page, so a step computes bit for bit what it computes in the contiguous layout.
 #include <type_traits>
 
 #include "kernels.h"
@@ -196,22 +200,45 @@ struct TileSmem {
     }
 };
 
+// The cache row of logical row r where rows are where they are (every layout but paged slots).
+struct SameRow {
+    __device__ __forceinline__ SameRow tile(uint32_t, uint32_t) const { return *this; }
+    __device__ __forceinline__ uint32_t operator()(uint32_t r) const { return r; }
+};
+// The physical rows of a tile of a paged slot: its (at most two) pages, looked up once for the whole tile.
+struct TilePages {
+    uint32_t page0, row0, row1;   // the first row's logical page; physical row 0 of that page and of the next
+    __device__ __forceinline__ uint32_t operator()(uint32_t r) const { return (r / kPageRows == page0 ? row0 : row1) + r % kPageRows; }
+};
+// The pages of a paged slot.
+struct PagedRows {
+    const int32_t *table;
+    // rows [first, first + n)
+    __device__ __forceinline__ TilePages tile(uint32_t first, uint32_t n) const {
+        const uint32_t p0 = first / kPageRows, row0 = (uint32_t)__ldg(table + p0) * kPageRows;
+        return {p0, row0, (first + n - 1) / kPageRows != p0 ? (uint32_t)__ldg(table + p0 + 1) * kPageRows : row0};
+    }
+};
+
 // Query rows [r0, r1) attend to cache rows [row0, row0 + n) of one KV head (kHead / vHead, and kSc / vSc for Q8, point at its row 0).
-// The rows are staged kTile at a time; inside a tile lane i scores row i, and the query rows go to the warps round robin.
-template <int HD, bool Q8>
+// The rows are staged kTile at a time; inside a tile lane i scores row i, and the query rows go to the warps round robin. The rows
+// of a tile are read from cache rows rowOf.tile(...)(row): a paged slot stages the same tiles from wherever its pages are (a tile
+// may span two pages: splits need not start on a page edge), so the arithmetic does not depend on the layout.
+template <int HD, bool Q8, typename RowOf = SameRow>
 __device__ __forceinline__ void attendTiles(const TileSmem<HD, Q8> &sm, const void *kHead, const void *vHead, const __half *kSc,
-                                            const __half *vSc, uint32_t row0, uint32_t n, uint32_t r0, uint32_t r1) {
+                                            const __half *vSc, uint32_t row0, uint32_t n, uint32_t r0, uint32_t r1, RowOf rowOf = {}) {
     constexpr int DPL = HD / 32, RP = TileSmem<HD, Q8>::kRowPad;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (uint32_t t0 = 0; t0 < n; t0 += kTile) {
         const uint32_t len = min((uint32_t)kTile, n - t0);
+        const auto tileRow = rowOf.tile(row0 + t0, len);
         __syncthreads();   // the previous tile (and the caller's initialisation) is complete
         if constexpr (Q8) {
             for (uint32_t i = threadIdx.x; i < kTile * (HD / 4); i += blockDim.x) {
                 const uint32_t rr = i / (HD / 4), c = i % (HD / 4);
                 float kf[4] = {0.f, 0.f, 0.f, 0.f}, vf[4] = {0.f, 0.f, 0.f, 0.f};
                 if (rr < len) {
-                    const size_t off = (size_t)(row0 + t0 + rr) * HD + 4 * c;
+                    const size_t off = (size_t)tileRow(row0 + t0 + rr) * HD + 4 * c;
                     loadKv<4, true>(kHead, kSc, off, kf);
                     loadKv<4, true>(vHead, vSc, off, vf);
                 }
@@ -223,7 +250,7 @@ __device__ __forceinline__ void attendTiles(const TileSmem<HD, Q8> &sm, const vo
                 const uint32_t rr = i / (HD / 2), c = i % (HD / 2);
                 __nv_bfloat162 kv = __floats2bfloat162_rn(0.f, 0.f), vv = kv;
                 if (rr < len) {
-                    const size_t off = (size_t)(row0 + t0 + rr) * HD + 2 * c;
+                    const size_t off = (size_t)tileRow(row0 + t0 + rr) * HD + 2 * c;
                     kv = *reinterpret_cast<const __nv_bfloat162 *>(reinterpret_cast<const __nv_bfloat16 *>(kHead) + off);
                     vv = *reinterpret_cast<const __nv_bfloat162 *>(reinterpret_cast<const __nv_bfloat16 *>(vHead) + off);
                 }
@@ -507,8 +534,10 @@ __global__ void __launch_bounds__(128) choiceAttnKernel(ChoiceAttnArgs a) {
 
 // ---- slots step: grid (nKvHeads, nSplits, B), block 128 (4 warps) -----------------------------------------------------------------
 // CTA (kvh, split, b) runs the kvMul q-heads of the KV head over its chunk of row b's slot (one q-head per warp, round robin).
-template <int HD, bool Q8>
-__global__ void __launch_bounds__(128) slotAttnKernel(SlotAttnArgs a) {
+// PAGED: the slot's rows are read through its page table from planes of planeRows rows per KV head; the tiles and splits are those
+// of the contiguous slot.
+template <int HD, bool Q8, bool PAGED>
+__global__ void __launch_bounds__(128) slotAttnKernel(typename std::conditional<PAGED, PagedSlotAttnArgs, SlotAttnArgs>::type a) {
     pdlLaunchDependents();
     pdlWait();
     const uint32_t kvh = blockIdx.x, split = blockIdx.y, b = blockIdx.z;
@@ -527,9 +556,15 @@ __global__ void __launch_bounds__(128) slotAttnKernel(SlotAttnArgs a) {
     for (uint32_t i = threadIdx.x; i < R * HD; i += blockDim.x) { sm.q[i] = qRow[i] * scale; sm.acc[i] = 0.f; }
     for (uint32_t r = threadIdx.x; r < R; r += blockDim.x) { sm.m[r] = -INFINITY; sm.l[r] = 0.f; }
 
-    const size_t headOff = (size_t)b * a.slotStride + (size_t)kvh * a.L * HD;
-    attendTiles(sm, kvPlane<Q8>(a.kCache, headOff), kvPlane<Q8>(a.vCache, headOff), Q8 ? a.kScale + headOff / 32 : nullptr,
-                Q8 ? a.vScale + headOff / 32 : nullptr, sp.begin, sp.end - sp.begin, 0, R);
+    if constexpr (PAGED) {
+        const size_t headOff = (size_t)kvh * a.planeRows * HD;
+        attendTiles(sm, kvPlane<Q8>(a.kCache, headOff), kvPlane<Q8>(a.vCache, headOff), Q8 ? a.kScale + headOff / 32 : nullptr,
+                    Q8 ? a.vScale + headOff / 32 : nullptr, sp.begin, sp.end - sp.begin, 0, R, PagedRows{a.pageTable + (size_t)b * a.pageStride});
+    } else {
+        const size_t headOff = (size_t)b * a.slotStride + (size_t)kvh * a.L * HD;
+        attendTiles(sm, kvPlane<Q8>(a.kCache, headOff), kvPlane<Q8>(a.vCache, headOff), Q8 ? a.kScale + headOff / 32 : nullptr,
+                    Q8 ? a.vScale + headOff / 32 : nullptr, sp.begin, sp.end - sp.begin, 0, R);
+    }
     __syncthreads();
 
     float *outRow = a.out + (size_t)b * a.outStride + (size_t)kvh * R * HD;
@@ -587,19 +622,27 @@ int launchChoiceAttn(const ChoiceAttnArgs &a, cudaStream_t stream, bool pdl) {
     return -1;
 }
 
-int launchSlotAttn(const SlotAttnArgs &a, cudaStream_t stream, bool pdl) {
+template <bool PAGED, typename Args>
+static int launchSlotAttnAs(const Args &a, cudaStream_t stream, bool pdl) {
     if (a.nKvHeads == 0 || a.nHeads % a.nKvHeads || a.nSplits < 1 || a.L < 1 || a.B < 1 || a.B > 32) return -1;
     if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
     const uint32_t R = a.nHeads / a.nKvHeads;
     const dim3 grid(a.nKvHeads, a.nSplits, a.B);
     if (a.kScale) {
-        if (a.headDim == 128) return launchTiles<slotAttnKernel<128, true>>(grid, TileSmem<128, true>::bytes(R), stream, pdl, a);
-        if (a.headDim == 64) return launchTiles<slotAttnKernel<64, true>>(grid, TileSmem<64, true>::bytes(R), stream, pdl, a);
+        if (a.headDim == 128) return launchTiles<slotAttnKernel<128, true, PAGED>>(grid, TileSmem<128, true>::bytes(R), stream, pdl, a);
+        if (a.headDim == 64) return launchTiles<slotAttnKernel<64, true, PAGED>>(grid, TileSmem<64, true>::bytes(R), stream, pdl, a);
         return -1;
     }
-    if (a.headDim == 128) return launchTiles<slotAttnKernel<128, false>>(grid, TileSmem<128, false>::bytes(R), stream, pdl, a);
-    if (a.headDim == 64) return launchTiles<slotAttnKernel<64, false>>(grid, TileSmem<64, false>::bytes(R), stream, pdl, a);
+    if (a.headDim == 128) return launchTiles<slotAttnKernel<128, false, PAGED>>(grid, TileSmem<128, false>::bytes(R), stream, pdl, a);
+    if (a.headDim == 64) return launchTiles<slotAttnKernel<64, false, PAGED>>(grid, TileSmem<64, false>::bytes(R), stream, pdl, a);
     return -1;
+}
+
+int launchSlotAttn(const SlotAttnArgs &a, cudaStream_t stream, bool pdl) { return launchSlotAttnAs<false>(a, stream, pdl); }
+
+int launchSlotAttnPaged(const PagedSlotAttnArgs &a, cudaStream_t stream, bool pdl) {
+    if (!a.pageTable || a.pageStride < (a.L + kPageRows - 1) / kPageRows || a.planeRows < a.L) return -1;
+    return launchSlotAttnAs<true>(a, stream, pdl);
 }
 
 }  // namespace dl
@@ -716,4 +759,19 @@ DL_EXPORT int dl_slot_attn_q80(const float *qkv, uint32_t qkvStride, const int *
     a.slotStride = (uint64_t)nKvHeads * L * headDim; a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.L = L;
     a.nSplits = nSplits; a.B = B; a.inactiveMask = inactiveMask; a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride;
     return dl::launchSlotAttn(a, stream, false);
+}
+
+// slotAttnKernel over paged slots (tests/test_gpu_paged_slots.py): the planes hold planeRows rows per KV head, row b's logical row r
+// is at physical row pageTable[b * pageStride + r / 64] * 64 + r % 64 (pageTable: device int32). kScale / vScale null: bf16 planes.
+DL_EXPORT int dl_slot_attn_paged(const float *qkv, uint32_t qkvStride, const int *pos, const void *kCache, const void *vCache, const void *kScale,
+                                 const void *vScale, const int32_t *pageTable, uint32_t pageStride, uint32_t planeRows, uint32_t nHeads,
+                                 uint32_t nKvHeads, uint32_t headDim, uint32_t L, uint32_t nSplits, uint32_t B, uint32_t inactiveMask,
+                                 float *partial, unsigned int *counters, float *out, uint32_t outStride, cudaStream_t stream) {
+    dl::PagedSlotAttnArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.pos = pos; a.kCache = kCache; a.vCache = vCache;
+    a.kScale = (const __half *)kScale; a.vScale = (const __half *)vScale;
+    a.pageTable = pageTable; a.pageStride = pageStride; a.planeRows = planeRows;
+    a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.L = L;
+    a.nSplits = nSplits; a.B = B; a.inactiveMask = inactiveMask; a.partial = partial; a.counters = counters; a.out = out; a.outStride = outStride;
+    return dl::launchSlotAttnPaged(a, stream, false);
 }

@@ -3,6 +3,7 @@
 // The maps are 3-D, {headDim, p0 + T, nKvHeads}, so TMA fills the rows of a tile at or past p0 + T with zeros: the kernel reads only
 // rows [0, p0 + T) of its own head, never a later (not yet written, or a previous request's) row or the next head's rows. Those rows
 // are masked to P = 0, but 0 * NaN is NaN on the tensor core as anywhere else.
+// A paged slot (PAGED kernels) reads its rows through its page table instead, and zeroes the rows past p0 + T itself.
 //
 // Work item (one CTA) = one KV head x one query tile. The `kvMul` query heads that share the KV head (GQA) are packed on the
 // MMA M dimension: a tile holds tq = 128 / kvMul consecutive prompt tokens x kvMul heads = up to 128 query rows, so every K / V
@@ -18,6 +19,8 @@
 // Replaces (reference): OP_MULTIHEAD_ATT over a prompt chunk, multiheadAtt_F32 + softmax_F32 per (head, batch row)
 // (src/nn/nn-cpu-ops.cpp:753-788,1260-1286) and the round-1 fallback that ran the decode kernel once per (head, token).
 #include <cuda.h>
+
+#include <type_traits>
 
 #include "kernels.h"
 #include "wgmma.cuh"
@@ -64,16 +67,32 @@ struct AttnPrefillKArgs {
     const __half *kScale, *vScale;
 };
 
+// The arguments of the PAGED kernels (derived, so that the others keep their argument layout and their code).
+struct PagedPrefillKArgs : AttnPrefillKArgs {
+    const __nv_bfloat16 *vBf16; // bf16: the V plane (the tile past the chunk's last row is copied, not loaded by TMA)
+    const int32_t *pageTable;   // the slot's page table (logical row r at physical row table[r / 64] * 64 + r % 64)
+};
+template <bool PAGED> using PrefillKArgs = typename std::conditional<PAGED, PagedPrefillKArgs, AttnPrefillKArgs>::type;
+template <typename A>
+__device__ __forceinline__ const int32_t *pagesOf(const A &a) {
+    if constexpr (std::is_same<A, PagedPrefillKArgs>::value) return a.pageTable;
+    else return nullptr;
+}
+
 // Q8: one 128-position K or V tile of a q80 cache, widened to bf16 by the 128 threads of warps 0..3 into the SWIZZLE_128B layout
 // ([NA][128 rows][128 B], 16-byte chunk c of row r at ((c ^ (r & 7)) << 4)). Rows at or past `rowEnd` (not yet written) are zero.
-template <int HD>
-__device__ __forceinline__ void apWidenTile(uint8_t *dst, const int8_t *q, const __half *sc, uint32_t kvRow0, uint32_t pos0, uint32_t rowEnd) {
+// PAGED: logical row pos0 + r is read from its page.
+template <int HD, bool PAGED>
+__device__ __forceinline__ void apWidenTile(uint8_t *dst, const int8_t *q, const __half *sc, uint32_t kvRow0, uint32_t pos0, uint32_t rowEnd,
+                                            const int32_t *table) {
     constexpr uint32_t CPR = HD / 8;   // 16-byte bf16 chunks per row
     for (uint32_t u = threadIdx.x; u < 128 * CPR; u += 128) {
         const uint32_t r = u / CPR, cc = u % CPR;
         uint4 packed = make_uint4(0u, 0u, 0u, 0u);
         if (pos0 + r < rowEnd) {
-            const size_t e = (size_t)(kvRow0 + pos0 + r) * HD + cc * 8;
+            size_t e;
+            if constexpr (PAGED) e = (size_t)(kvRow0 + pagedRow(table, pos0 + r)) * HD + cc * 8;
+            else e = (size_t)(kvRow0 + pos0 + r) * HD + cc * 8;
             const float d = __half2float(sc[e / 32]);
             const uint2 w = *reinterpret_cast<const uint2 *>(q + e);
             packed = make_uint4(apPack(q8ToFloat(w.x, 0) * d, q8ToFloat(w.x, 1) * d), apPack(q8ToFloat(w.x, 2) * d, q8ToFloat(w.x, 3) * d),
@@ -85,9 +104,28 @@ __device__ __forceinline__ void apWidenTile(uint8_t *dst, const int8_t *q, const
     __syncwarp();
 }
 
-template <int HD, bool Q8>
+// PAGED bf16: the V tile that holds rows at or past `rowEnd`, copied by the 32 lanes of warp 0 into the SWIZZLE_128B layout. Those rows
+// of a page may hold anything (another request's rows, or NaN); they get P = 0, and 0 * NaN would still be NaN, so they are zeroed.
+template <int HD>
+__device__ __forceinline__ void apCopyTailTile(uint8_t *dst, const __nv_bfloat16 *plane, uint32_t kvRow0, uint32_t pos0, uint32_t rowEnd,
+                                               const int32_t *table) {
+    constexpr uint32_t CPR = HD / 8;
+    for (uint32_t u = threadIdx.x & 31; u < 128 * CPR; u += 32) {
+        const uint32_t r = u / CPR, cc = u % CPR;
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (pos0 + r < rowEnd) v = *reinterpret_cast<const uint4 *>(plane + (size_t)(kvRow0 + pagedRow(table, pos0 + r)) * HD + cc * 8);
+        *reinterpret_cast<uint4 *>(dst + (cc >> 3) * kApAtomBytes + r * 128 + (((cc & 7) ^ (r & 7)) << 4)) = v;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncwarp();
+}
+
+// PAGED: the slot's rows are read through its page table (AttnPrefillKArgs::pageTable) from a map over the whole layer plane: a
+// 128-position K tile is two 64-row TMA boxes at the pages' physical rows, and the last V tile of a query tile comes through
+// apCopyTailTile. The tiles, and so the arithmetic, are those of a contiguous cache.
+template <int HD, bool Q8, bool PAGED>
 __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __grid_constant__ CUtensorMap tmapK,
-                                                                     const __grid_constant__ CUtensorMap tmapV, AttnPrefillKArgs a) {
+                                                                     const __grid_constant__ CUtensorMap tmapV, PrefillKArgs<PAGED> a) {
     constexpr uint32_t NA = HD / 64;                    // 64-wide atom columns along headDim
     constexpr uint32_t kTileBytes = NA * kApAtomBytes;  // one K or V tile: 128 positions x HD
     extern __shared__ __align__(1024) uint8_t apSmemRaw[];
@@ -128,17 +166,54 @@ __global__ void __launch_bounds__(kApThreads, 1) attnPrefillTcKernel(const __gri
             for (uint32_t j = 0; j < nKv; j++, itK++) {
                 const uint32_t st = itK & 1, ph = (itK >> 1) & 1;
                 apBarWait(&kEmpty[st], ph ^ 1);
-                apWidenTile<HD>(Ks + st * kTileBytes, a.kQ8, a.kScale, kvRow0, j * 128, rowEnd);
+                apWidenTile<HD, PAGED>(Ks + st * kTileBytes, a.kQ8, a.kScale, kvRow0, j * 128, rowEnd, pagesOf(a));
                 if (lane == 0) apBarArrive(&kFull[st]);
                 if (pass == 1) {
                     const uint32_t vs = j & 1, vph = (j >> 1) & 1;
                     apBarWait(&vEmpty[vs], vph ^ 1);
-                    apWidenTile<HD>(Vs + vs * kTileBytes, a.vQ8, a.vScale, kvRow0, j * 128, rowEnd);
+                    apWidenTile<HD, PAGED>(Vs + vs * kTileBytes, a.vQ8, a.vScale, kvRow0, j * 128, rowEnd, pagesOf(a));
                     if (lane == 0) apBarArrive(&vFull[vs]);
                 }
             }
         }
-    } else if (!Q8 && warp == 0) {
+    } else if (!Q8 && PAGED && warp == 0) {
+        // ============================ TMA producer, paged: warp 0 ============================
+        if constexpr (PAGED) {
+        const uint32_t rowEnd = a.p0 + a.T;
+        uint32_t itK = 0;
+        for (uint32_t pass = 0; pass < 2; pass++) {
+            for (uint32_t j = 0; j < nKv; j++, itK++) {
+                const uint32_t st = itK & 1, ph = (itK >> 1) & 1;
+                apBarWait(&kEmpty[st], ph ^ 1);
+                if (lane == 0) {
+                    // page 2j holds a row below rowEnd; a page 2j + 1 past it is loaded as page 2j again (masked like any row past rowEnd)
+                    const uint32_t r0 = (uint32_t)__ldg(a.pageTable + 2 * j) * 64;
+                    const uint32_t r1 = j * 128 + 64 < rowEnd ? (uint32_t)__ldg(a.pageTable + 2 * j + 1) * 64 : r0;
+                    apBarExpectTx(&kFull[st], kTileBytes);
+                    for (uint32_t c = 0; c < NA; c++) {
+                        apTmaLoad3d(Ks + st * kTileBytes + c * kApAtomBytes, &tmapK, c * 64, r0, kvh, &kFull[st]);
+                        apTmaLoad3d(Ks + st * kTileBytes + c * kApAtomBytes + 8192, &tmapK, c * 64, r1, kvh, &kFull[st]);
+                    }
+                }
+                if (pass == 1) {
+                    const uint32_t vs = j & 1, vph = (j >> 1) & 1;
+                    apBarWait(&vEmpty[vs], vph ^ 1);
+                    if (j * 128 + 128 > rowEnd) {
+                        apCopyTailTile<HD>(Vs + vs * kTileBytes, a.vBf16, kvRow0, j * 128, rowEnd, a.pageTable);
+                        if (lane == 0) apBarArrive(&vFull[vs]);
+                    } else if (lane == 0) {
+                        const uint32_t r0 = (uint32_t)__ldg(a.pageTable + 2 * j) * 64, r1 = (uint32_t)__ldg(a.pageTable + 2 * j + 1) * 64;
+                        apBarExpectTx(&vFull[vs], kTileBytes);
+                        for (uint32_t c = 0; c < NA; c++) {
+                            apTmaLoad3d(Vs + vs * kTileBytes + c * kApAtomBytes, &tmapV, c * 64, r0, kvh, &vFull[vs]);
+                            apTmaLoad3d(Vs + vs * kTileBytes + c * kApAtomBytes + 8192, &tmapV, c * 64, r1, kvh, &vFull[vs]);
+                        }
+                    }
+                }
+            }
+        }
+        }
+    } else if (!Q8 && !PAGED && warp == 0) {
         // ================================ TMA producer ================================
         // expect_tx counts the whole box: TMA delivers the zero-filled rows past p0 + T like the loaded ones
         if (lane == 0) {
@@ -321,29 +396,46 @@ ApEncodeFn apEncode() {
     return fn;
 }
 
-// Rows [0, rows) of every head of a [nKvHeads][seqLen][hd] bf16 cache; a box is 64 columns x 128 rows of one head.
-bool apCacheMap(CUtensorMap *map, const void *cache, uint32_t hd, uint32_t rows, uint32_t nKvHeads, uint32_t seqLen) {
+// Rows [0, rows) of every head of a [nKvHeads][seqLen][hd] bf16 cache; a box is 64 columns x boxRows rows of one head.
+bool apCacheMap(CUtensorMap *map, const void *cache, uint32_t hd, uint32_t rows, uint32_t nKvHeads, uint32_t seqLen, uint32_t boxRows = 128) {
     ApEncodeFn enc = apEncode();
     if (!enc) return false;
     const cuuint64_t dims[3] = {hd, rows, nKvHeads};
     const cuuint64_t strides[2] = {(cuuint64_t)hd * 2, (cuuint64_t)hd * 2 * seqLen};
-    const cuuint32_t box[3] = {64, 128, 1};
+    const cuuint32_t box[3] = {64, boxRows, 1};
     const cuuint32_t estr[3] = {1, 1, 1};
     return enc(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(cache), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int HD, bool Q8>
-int apLaunch(const CUtensorMap &mk, const CUtensorMap &mv, const AttnPrefillKArgs &k, uint32_t grid, cudaStream_t stream, bool pdl) {
+template <int HD, bool Q8, bool PAGED>
+int apLaunch(const CUtensorMap &mk, const CUtensorMap &mv, const PrefillKArgs<PAGED> &k, uint32_t grid, cudaStream_t stream, bool pdl) {
     constexpr size_t smemBytes = (size_t)(HD / 64) * kApAtomBytes * 5 + 256 + 1024;
     static bool configured = false;
     if (!configured) {
-        DL_CUDA_CHECK(cudaFuncSetAttribute(attnPrefillTcKernel<HD, Q8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
+        DL_CUDA_CHECK(cudaFuncSetAttribute(attnPrefillTcKernel<HD, Q8, PAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smemBytes));
         configured = true;
     }
-    DL_CUDA_CHECK(launchPdl(attnPrefillTcKernel<HD, Q8>, dim3(grid), dim3(kApThreads), smemBytes, stream, pdl, mk, mv, k));
+    DL_CUDA_CHECK(launchPdl(attnPrefillTcKernel<HD, Q8, PAGED>, dim3(grid), dim3(kApThreads), smemBytes, stream, pdl, mk, mv, k));
     DL_CUDA_CHECK(cudaGetLastError());
     return 0;
+}
+
+// A paged slot's chunk: q80 widened through the table; bf16 over maps of the whole layer plane in 64-row boxes (one page each).
+int launchPaged(const AttnPrefillArgs &a, const AttnPrefillKArgs &base, uint32_t grid, cudaStream_t stream, bool pdl) {
+    PagedPrefillKArgs k{};
+    static_cast<AttnPrefillKArgs &>(k) = base;
+    k.pageTable = a.pageTable;
+    if (a.kScale) {
+        CUtensorMap none{};
+        k.kQ8 = (const int8_t *)a.kCache; k.vQ8 = (const int8_t *)a.vCache; k.kScale = a.kScale; k.vScale = a.vScale;
+        return a.headDim == 128 ? apLaunch<128, true, true>(none, none, k, grid, stream, pdl) : apLaunch<64, true, true>(none, none, k, grid, stream, pdl);
+    }
+    CUtensorMap mk, mv;
+    if (!apCacheMap(&mk, a.kCache, a.headDim, a.seqLen, a.nKvHeads, a.seqLen, 64) || !apCacheMap(&mv, a.vCache, a.headDim, a.seqLen, a.nKvHeads, a.seqLen, 64))
+        return -2;
+    k.vBf16 = (const __nv_bfloat16 *)a.vCache;
+    return a.headDim == 128 ? apLaunch<128, false, true>(mk, mv, k, grid, stream, pdl) : apLaunch<64, false, true>(mk, mv, k, grid, stream, pdl);
 }
 
 }  // namespace
@@ -362,16 +454,17 @@ int launchAttnPrefillTc(const AttnPrefillArgs &a, cudaStream_t stream, bool pdl)
     k.scaleLog2 = 1.4426950408889634f / sqrtf((float)a.headDim);
     const uint32_t grid = a.nKvHeads * k.nQTiles;
     if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
+    if (a.pageTable) return launchPaged(a, k, grid, stream, pdl);
     if (a.kScale) {   // q80: widened by the kernel itself, no tensor maps
         CUtensorMap none{};
         k.kQ8 = (const int8_t *)a.kCache; k.vQ8 = (const int8_t *)a.vCache; k.kScale = a.kScale; k.vScale = a.vScale;
-        return a.headDim == 128 ? apLaunch<128, true>(none, none, k, grid, stream, pdl) : apLaunch<64, true>(none, none, k, grid, stream, pdl);
+        return a.headDim == 128 ? apLaunch<128, true, false>(none, none, k, grid, stream, pdl) : apLaunch<64, true, false>(none, none, k, grid, stream, pdl);
     }
     CUtensorMap mk, mv;
     const uint32_t rows = a.p0 + a.T;   // rows of each head this chunk may read; TMA zero-fills the rest of the last tile
     if (!apCacheMap(&mk, a.kCache, a.headDim, rows, a.nKvHeads, a.seqLen) || !apCacheMap(&mv, a.vCache, a.headDim, rows, a.nKvHeads, a.seqLen))
         return -2;
-    return a.headDim == 128 ? apLaunch<128, false>(mk, mv, k, grid, stream, pdl) : apLaunch<64, false>(mk, mv, k, grid, stream, pdl);
+    return a.headDim == 128 ? apLaunch<128, false, false>(mk, mv, k, grid, stream, pdl) : apLaunch<64, false, false>(mk, mv, k, grid, stream, pdl);
 }
 
 }  // namespace dl
@@ -393,6 +486,19 @@ DL_EXPORT int dl_attn_prefill_tc_q80(const float *qkv, uint32_t qkvStride, uint3
     dl::AttnPrefillArgs a{};
     a.qkv = qkv; a.qkvStride = qkvStride; a.T = T; a.p0 = p0; a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen;
     a.kCache = kCache; a.vCache = vCache; a.kScale = (const __half *)kScale; a.vScale = (const __half *)vScale;
+    a.out = (__nv_bfloat16 *)out; a.outStride = outStride;
+    return dl::launchAttnPrefillTc(a, stream);
+}
+
+// Tensor-core prefill attention of one paged slot's chunk (tests/test_gpu_paged_slots.py): kCache / vCache are whole layer planes of
+// seqLen rows per KV head (seqLen a multiple of 64), pageTable (device int32) maps the slot's logical page i to physical page
+// pageTable[i]; kScale / vScale null: bf16 planes, else q80 scale planes.
+DL_EXPORT int dl_attn_prefill_tc_paged(const float *qkv, uint32_t qkvStride, uint32_t T, uint32_t p0, uint32_t nHeads, uint32_t nKvHeads,
+                                       uint32_t headDim, uint32_t seqLen, const void *kCache, const void *vCache, const void *kScale,
+                                       const void *vScale, const int32_t *pageTable, void *out, uint32_t outStride, cudaStream_t stream) {
+    dl::AttnPrefillArgs a{};
+    a.qkv = qkv; a.qkvStride = qkvStride; a.T = T; a.p0 = p0; a.nHeads = nHeads; a.nKvHeads = nKvHeads; a.headDim = headDim; a.seqLen = seqLen;
+    a.kCache = kCache; a.vCache = vCache; a.kScale = (const __half *)kScale; a.vScale = (const __half *)vScale; a.pageTable = pageTable;
     a.out = (__nv_bfloat16 *)out; a.outStride = outStride;
     return dl::launchAttnPrefillTc(a, stream);
 }

@@ -5,6 +5,8 @@
 // (llm.cpp:322-346), OP_ROPE (nn-cpu-ops.cpp:843-885), OP_SHIFT (:1419-1441), host argmax (tokenizer.cpp:392-403).
 // Differences by design: KV cache is bf16 and head-major [kvHead][pos][headDim] (reference: f32 [pos][kvDim]);
 // both rotary conventions run as adjacent-pair rotation because NeoX-style heads are re-ordered at load.
+#include <type_traits>
+
 #include "kernels.h"
 
 namespace dl {
@@ -24,9 +26,9 @@ __global__ void __launch_bounds__(256) embeddingKernel(const EmbTable table, con
 
 // ---- QK-norm + RoPE + KV write -------------------------------------------------------------------------
 // grid (nHeads + 2*nKvHeads, nb), block headDim/2: thread j rotates pair (2j, 2j+1). Q8: the cache is q80 (a 32-value block is
-// the pairs of 16 neighbouring threads).
-template <bool Q8>
-__global__ void __launch_bounds__(128) ropeKvKernel(RopeKvArgs a) {
+// the pairs of 16 neighbouring threads). PAGED: the row goes to its physical row through the token's page table.
+template <bool Q8, bool PAGED>
+__global__ void __launch_bounds__(128) ropeKvKernel(typename std::conditional<PAGED, PagedRopeKvArgs, RopeKvArgs>::type a) {
     pdlLaunchDependents();
     pdlWait();
     __shared__ float red[4];
@@ -56,7 +58,9 @@ __global__ void __launch_bounds__(128) ropeKvKernel(RopeKvArgs a) {
         const float x1 = v.x * cs.y + v.y * cs.x;
         v.x = x0; v.y = x1;
     }
-    const uint32_t cacheRow = (uint32_t)p + t * a.rowStride;
+    uint32_t cacheRow;
+    if constexpr (PAGED) cacheRow = pagedRow(a.pageTable + (size_t)t * a.pageTableStride, (uint32_t)p);
+    else cacheRow = (uint32_t)p + t * a.rowStride;
     const bool inactive = t < 32 && ((a.inactiveMask >> t) & 1u);
     if (isQ) {
         reinterpret_cast<float2 *>(row)[j] = v;
@@ -213,8 +217,17 @@ int launchRopeKv(const RopeKvArgs &a, int nb, cudaStream_t stream, bool pdl) {
     if (a.headDim != 64 && a.headDim != 128 && a.headDim != 256) return -1;
     if ((a.kScale == nullptr) != (a.vScale == nullptr)) return -1;
     const dim3 grid(a.nHeads + 2 * a.nKvHeads, nb), block(a.headDim / 2);
-    if (a.kScale) DL_CUDA_CHECK(launchPdl(ropeKvKernel<true>, grid, block, 0, stream, pdl, a));
-    else DL_CUDA_CHECK(launchPdl(ropeKvKernel<false>, grid, block, 0, stream, pdl, a));
+    if (a.kScale) DL_CUDA_CHECK(launchPdl(ropeKvKernel<true, false>, grid, block, 0, stream, pdl, a));
+    else DL_CUDA_CHECK(launchPdl(ropeKvKernel<false, false>, grid, block, 0, stream, pdl, a));
+    return 0;
+}
+
+int launchRopeKvPaged(const PagedRopeKvArgs &a, int nb, cudaStream_t stream, bool pdl) {
+    if (a.headDim != 64 && a.headDim != 128 && a.headDim != 256) return -1;
+    if ((a.kScale == nullptr) != (a.vScale == nullptr) || !a.pageTable || a.slotStride || a.rowStride) return -1;
+    const dim3 grid(a.nHeads + 2 * a.nKvHeads, nb), block(a.headDim / 2);
+    if (a.kScale) DL_CUDA_CHECK(launchPdl(ropeKvKernel<true, true>, grid, block, 0, stream, pdl, a));
+    else DL_CUDA_CHECK(launchPdl(ropeKvKernel<false, true>, grid, block, 0, stream, pdl, a));
     return 0;
 }
 

@@ -101,6 +101,16 @@ struct Engine {
     cudaEvent_t slotStaged = nullptr;  // the uploads of the staged tokens / positions are done: the buffer may be rewritten
     int slotLogprobs[8] = {-1, -1, -1, -1, -1, -1, -1, -1};   // per-slot top_logprobs k (-1: no logprobs), one per slot
     int32_t *slotLpDev = nullptr, *slotLpHost = nullptr;   // [kChoiceRngSlots][kLogprobsWords] results of a slots step (device, pinned)
+    // Paged slots (dl_engine_set_slot_cache): every layer plane is a pool of nPages 64-row pages shared by the slots; slot s maps its
+    // logical page i to physical page pageHost[s * nPages + i] (i < slotPages[s]; -1 past them). The device copy is refreshed on the
+    // stream of the next call that reads it (uploadPages).
+    bool pagedSlots = false;
+    uint32_t nPages = 0;
+    int32_t *pageDev = nullptr, *pageHost = nullptr;   // [kChoiceRngSlots][nPages] (device, pinned)
+    std::vector<uint32_t> slotPages;
+    std::vector<uint8_t> pageUsed;
+    bool pagesDirty = false;
+    cudaEvent_t pagesStaged = nullptr;   // the last upload has read pageHost
     bool tcAttn = true;          // prefill attention on the tensor cores (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
     bool fusedAttn = true;       // debugging switch (DL_NO_FUSED_ATTN)
 };
@@ -292,15 +302,27 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
         DL_TRY(gemvSel(e, PRO_RMSNORM_, EPI_STORE_, nb, a, c.numSms, stream, pdl));
         if (sl) {
             // 2+3. qk-norm + rope + K/V append at row pos[b] of slot b, then attention of each row over its own slot
-            RopeKvArgs r = layerRopeKv(e, L, e.g.qkv, e.g.pos, 0, e.slotLen);
-            r.slotStride = slotElems(e); r.inactiveMask = sl->inactiveMask;
-            DL_TRY(launchRopeKv(r, nb, stream, pdl));
+            RopeKvArgs r = layerRopeKv(e, L, e.g.qkv, e.g.pos, 0, e.pagedSlots ? c.seqLen : e.slotLen);
+            if (!e.pagedSlots) r.slotStride = slotElems(e);
+            r.inactiveMask = sl->inactiveMask;
             SlotAttnArgs t{};
             t.qkv = e.g.qkv; t.qkvStride = qkvDim; t.pos = e.g.pos; t.kCache = r.kCache; t.vCache = r.vCache; t.kScale = r.kScale; t.vScale = r.vScale; t.slotStride = r.slotStride;
             t.nHeads = c.nHeads; t.nKvHeads = c.nKvHeads; t.headDim = c.headDim; t.L = e.slotLen; t.nSplits = c.nSplits;
             t.B = (uint32_t)nb; t.inactiveMask = sl->inactiveMask;
             t.partial = e.g.attnPartial; t.counters = e.g.attnCounters; t.out = e.g.z; t.outStride = qDim;
-            DL_TRY(launchSlotAttn(t, stream, pdl));
+            if (e.pagedSlots) {
+                PagedRopeKvArgs pr{};
+                static_cast<RopeKvArgs &>(pr) = r;
+                pr.pageTable = e.pageDev; pr.pageTableStride = e.nPages;
+                DL_TRY(launchRopeKvPaged(pr, nb, stream, pdl));
+                PagedSlotAttnArgs pt{};
+                static_cast<SlotAttnArgs &>(pt) = t;
+                pt.pageTable = e.pageDev; pt.pageStride = e.nPages; pt.planeRows = c.seqLen;
+                DL_TRY(launchSlotAttnPaged(pt, stream, pdl));
+            } else {
+                DL_TRY(launchRopeKv(r, nb, stream, pdl));
+                DL_TRY(launchSlotAttn(t, stream, pdl));
+            }
         } else if (ch) {
             // 2+3. qk-norm + rope + K/V append at the choices' own rows, then attention over the shared prompt + own rows
             RopeKvArgs r = layerRopeKv(e, L, e.g.qkv, e.g.pos, 0, c.seqLen);
@@ -405,9 +427,12 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
     const uint32_t qDim = c.nHeads * c.headDim, kvDim = c.nKvHeads * c.headDim, qkvDim = qDim + 2 * kvDim;
     if (T < 1 || T > c.maxPrefill) return -11;
     if (c.wType != 0) return -35;   // tensor-core path: q40 matrices
-    const uint32_t seqLen = slot >= 0 ? e.slotLen : c.seqLen;
-    const uint64_t cacheOff = slot >= 0 ? (uint64_t)slot * slotElems(e) : 0;
-    if (slot >= 0 && ((uint32_t)slot >= e.slots || p0 + T > seqLen)) return -60;
+    const bool paged = slot >= 0 && e.pagedSlots;
+    const uint32_t seqLen = slot >= 0 && !paged ? e.slotLen : c.seqLen;   // rows a KV head's plane holds
+    const uint64_t cacheOff = slot >= 0 && !paged ? (uint64_t)slot * slotElems(e) : 0;
+    if (slot >= 0 && ((uint32_t)slot >= e.slots || p0 + T > (paged ? e.slotPages[slot] * kPageRows : seqLen))) return -60;
+    if (paged && !e.tcAttn) return -69;
+    const int32_t *pages = paged ? e.pageDev + (size_t)slot * e.nPages : nullptr;
     const bool tp = e.comm.nRanks > 1;
     ArArgs arP{};
     if (tp) {
@@ -423,16 +448,22 @@ static int enginePrefill(Engine &e, uint32_t T, uint32_t p0, int wantLogits, cud
         DL_TRY(launchRmsNormBf16(g.px, c.dim, L.norm0, g.pxn, c.dim, c.dim, c.eps, T, stream, pdl));
         DL_TRY(gemmQ40Tc(GEPI_STORE_F32_, L.qkvQs, L.qkvSc, qkvDim, c.dim, g.pxn, c.dim, T, g.pqkv, qkvDim, c.numSms, stream, pdl));
         const RopeKvArgs r = layerRopeKv(e, L, g.pqkv, g.pPos, cacheOff, seqLen);
-        DL_TRY(launchRopeKv(r, (int)T, stream, pdl));
+        if (paged) {
+            PagedRopeKvArgs pr{};
+            static_cast<RopeKvArgs &>(pr) = r;
+            pr.pageTable = pages;
+            DL_TRY(launchRopeKvPaged(pr, (int)T, stream, pdl));
+        } else DL_TRY(launchRopeKv(r, (int)T, stream, pdl));
         int attnRc = 1;
         if (e.tcAttn) {
             // tensor-core attention over the whole chunk: the tokens of a chunk sit at consecutive positions p0 .. p0 + T - 1
             AttnPrefillArgs ap{};
             ap.qkv = g.pqkv; ap.qkvStride = qkvDim; ap.T = T; ap.p0 = p0; ap.nHeads = c.nHeads; ap.nKvHeads = c.nKvHeads;
             ap.headDim = c.headDim; ap.seqLen = seqLen; ap.kCache = r.kCache; ap.vCache = r.vCache; ap.kScale = r.kScale; ap.vScale = r.vScale;
-            ap.out = (__nv_bfloat16 *)g.pzb; ap.outStride = qDim;
+            ap.out = (__nv_bfloat16 *)g.pzb; ap.outStride = qDim; ap.pageTable = pages;
             attnRc = launchAttnPrefillTc(ap, stream, pdl);
             if (attnRc < 0) return attnRc;
+            if (attnRc == 1 && paged) return -69;
         }
         if (attnRc == 1) {
             AttnArgs t{};
@@ -576,6 +607,9 @@ DL_EXPORT void dl_engine_destroy(void *h) {
     if (e->slotStaged) cudaEventDestroy(e->slotStaged);
     if (e->slotLpDev) cudaFree(e->slotLpDev);
     if (e->slotLpHost) cudaFreeHost(e->slotLpHost);
+    if (e->pageDev) cudaFree(e->pageDev);
+    if (e->pageHost) cudaFreeHost(e->pageHost);
+    if (e->pagesStaged) cudaEventDestroy(e->pagesStaged);
     if (e->scratch) cudaFree(e->scratch);
     delete e;
 }
@@ -698,6 +732,22 @@ static int ensureCounts(Engine *e, cudaStream_t stream) {
         DL_CUDA_CHECK(cudaMalloc(&e->ctlCounts, bytes));
         DL_CUDA_CHECK(cudaMemsetAsync(e->ctlCounts, 0, bytes, stream));
     }
+    return 0;
+}
+
+// Paged slots: copies the host page table to the device on `stream` if it changed since the last upload.
+static int uploadPages(Engine *e, cudaStream_t stream) {
+    if (!e->pagesDirty) return 0;
+    DL_CUDA_CHECK(cudaMemcpyAsync(e->pageDev, e->pageHost, (size_t)kChoiceRngSlots * e->nPages * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
+    DL_CUDA_CHECK(cudaEventRecord(e->pagesStaged, stream));
+    e->pagesDirty = false;
+    return 0;
+}
+
+// Paged slots: the host page table may be rewritten once the last upload has read it.
+static int editPages(Engine *e) {
+    DL_CUDA_CHECK(cudaEventSynchronize(e->pagesStaged));
+    e->pagesDirty = true;
     return 0;
 }
 
@@ -1069,6 +1119,10 @@ DL_EXPORT int dl_engine_prefill(void *h, const int32_t *hostTokens, uint32_t n, 
     Engine &e = *(Engine *)h;
     std::vector<dl::PrefillChunk> chunks;
     DL_TRY(dl::planEnginePrefill(e, n, p0, slot, chunks));
+    if (slot >= 0 && e.pagedSlots) {
+        if ((uint64_t)p0 + n > (uint64_t)e.slotPages[slot] * dl::kPageRows) return -60;   // reserve the rows first (dl_engine_slot_reserve)
+        DL_TRY(uploadPages(&e, stream));
+    }
     std::vector<int32_t> pos(n);
     for (uint32_t i = 0; i < n; i++) pos[i] = (int32_t)(p0 + i);
     for (const dl::PrefillChunk &ch : chunks) {
@@ -1139,8 +1193,24 @@ DL_EXPORT void dl_abi_struct_sizes(uint32_t out[4]) {
 
 // ---- KV-cache slots: up to 8 independent sequences decoded together (attn_decode.cu) -------------------------------------------------
 
+// The layout of the next dl_engine_set_slots: 0 = split (every slot owns floor(seqLen / n) contiguous rows), 1 = paged (the slots
+// share every layer plane as one pool of floor(seqLen / 64) pages of 64 rows; a slot holds the pages dl_engine_slot_reserve gave it).
+// -64 once slots are set.
+DL_EXPORT int dl_engine_set_slot_cache(void *h, int paged) {
+    Engine *e = (Engine *)h;
+    if (e->slots > 1) return -64;
+    if (paged && e->cfg.seqLen < dl::kPageRows) return -61;
+    // a paged slot's prompt runs on the tensor-core prefill attention only (launchAttnPrefillTc: head dim 64 or 128, <= 128 q-heads per KV head)
+    const dl::EngineConfig &c = e->cfg;
+    const bool tcShape = (c.headDim == 64 || c.headDim == 128) && c.nKvHeads && c.nHeads % c.nKvHeads == 0 && c.nHeads / c.nKvHeads <= 128;
+    if (paged && (!e->tcAttn || !tcShape)) return -69;
+    e->pagedSlots = paged != 0;
+    return 0;
+}
+
 // Splits every layer's K/V cache into n equal slots of floor(seqLen / n) rows (no extra memory) and allocates the per-slot sampling
-// state. Single GPU, dense (non-MoE) q40 layers only. n = 1 leaves the engine exactly as it was.
+// state; paged (dl_engine_set_slot_cache): n slots over one pool of pages, every page free. Single GPU, dense (non-MoE) q40 layers
+// only. n = 1 leaves the engine exactly as it was.
 DL_EXPORT int dl_engine_set_slots(void *h, uint32_t n) {
     Engine *e = (Engine *)h;
     const dl::EngineConfig &c = e->cfg;
@@ -1150,8 +1220,22 @@ DL_EXPORT int dl_engine_set_slots(void *h, uint32_t n) {
     while (nb < n) nb *= 2;
     if (nb > c.maxBatch) return -63;
     e->slots = n;
-    e->slotLen = c.seqLen / n;
+    e->slotLen = e->pagedSlots && n > 1 ? c.seqLen / dl::kPageRows * dl::kPageRows : c.seqLen / n;
     if (n == 1) return 0;
+    if (e->pagedSlots) {
+        const uint32_t pages = c.seqLen / dl::kPageRows;
+        if (!e->pageDev) {
+            DL_CUDA_CHECK(cudaMalloc(&e->pageDev, (size_t)kChoiceRngSlots * pages * sizeof(int32_t)));
+            DL_CUDA_CHECK(cudaHostAlloc((void **)&e->pageHost, (size_t)kChoiceRngSlots * pages * sizeof(int32_t), cudaHostAllocDefault));
+            DL_CUDA_CHECK(cudaEventCreateWithFlags(&e->pagesStaged, cudaEventDisableTiming));
+        }
+        DL_CUDA_CHECK(cudaEventSynchronize(e->pagesStaged));
+        e->nPages = pages;
+        std::fill(e->pageHost, e->pageHost + (size_t)kChoiceRngSlots * pages, -1);
+        e->slotPages.assign(kChoiceRngSlots, 0);
+        e->pageUsed.assign(pages, 0);
+        e->pagesDirty = true;
+    }
     DL_TRY(ensureSampler(e));
     DL_TRY(ensureCounts(e, 0));
     const uint32_t full = c.vocab;
@@ -1174,12 +1258,43 @@ DL_EXPORT uint32_t dl_engine_slot_len(void *h) {
     return e->slots > 1 ? e->slotLen : e->cfg.seqLen;
 }
 
-// Copies rows [0, P) of slot src into slot dst, every layer and KV head (several completions of one prompt).
+DL_EXPORT int dl_engine_slot_reserve(void *h, uint32_t slot, uint32_t rows);
+
+// Paged slots: copies rows [0, P) of slot src into the pages of slot dst (reserved first; -68 and nothing copied when the pool is
+// short), one copy per run of pages that are consecutive in both slots.
+static int slotCopyPaged(Engine *e, uint32_t src, uint32_t dst, uint32_t P, cudaStream_t stream) {
+    const dl::EngineConfig &c = e->cfg;
+    if ((uint64_t)P > (uint64_t)e->slotPages[src] * dl::kPageRows) return -60;
+    DL_TRY(dl_engine_slot_reserve(e, dst, P));
+    const int32_t *ts = e->pageHost + (size_t)src * e->nPages, *td = e->pageHost + (size_t)dst * e->nPages;
+    const bool q8 = c.kvType != 0;
+    const size_t rowBytes[2] = {(size_t)c.headDim * (q8 ? 1 : sizeof(__nv_bfloat16)), (size_t)c.headDim / 16};
+    const uint32_t pages = (P + dl::kPageRows - 1) / dl::kPageRows;
+    for (uint32_t i = 0; i < pages;) {
+        uint32_t n = 1;
+        while (i + n < pages && ts[i + n] == ts[i] + (int32_t)n && td[i + n] == td[i] + (int32_t)n) n++;
+        const size_t rows = std::min<size_t>((size_t)n * dl::kPageRows, P - (size_t)i * dl::kPageRows);
+        for (const dl::LayerPtrs &L : e->layers)
+            for (int plane = 0; plane < (q8 ? 2 : 1); plane++) {
+                const size_t pitch = (size_t)c.seqLen * rowBytes[plane];
+                for (void *cache : {plane ? L.kScale : L.kCache, plane ? L.vScale : L.vCache})
+                    DL_CUDA_CHECK(cudaMemcpy2DAsync((uint8_t *)cache + (size_t)td[i] * dl::kPageRows * rowBytes[plane], pitch,
+                                                    (const uint8_t *)cache + (size_t)ts[i] * dl::kPageRows * rowBytes[plane], pitch,
+                                                    rows * rowBytes[plane], c.nKvHeads, cudaMemcpyDeviceToDevice, stream));
+            }
+        i += n;
+    }
+    return 0;
+}
+
+// Copies rows [0, P) of slot src into slot dst, every layer and KV head (several completions of one prompt). Paged slots: into
+// dst's own pages, reserved first (-68 when the pool is short).
 DL_EXPORT int dl_engine_slot_copy(void *h, uint32_t src, uint32_t dst, uint32_t P, cudaStream_t stream) {
     Engine *e = (Engine *)h;
     const dl::EngineConfig &c = e->cfg;
     if (e->slots < 2 || src >= e->slots || dst >= e->slots || P > e->slotLen) return -64;
     if (src == dst || P == 0) return 0;
+    if (e->pagedSlots) return slotCopyPaged(e, src, dst, P, stream);
     // bf16: one plane per cache; q80: the int8 values (headDim bytes a row) and the scales (headDim / 16 bytes a row)
     const bool q8 = c.kvType != 0;
     const size_t rowBytes[2] = {(size_t)c.headDim * (q8 ? 1 : sizeof(__nv_bfloat16)), (size_t)c.headDim / 16};
@@ -1255,12 +1370,14 @@ DL_EXPORT int dl_engine_slots_forward(void *h, const int32_t *tokens, const int3
     for (int b = 0; b < nb; b++) {
         const bool on = !((mask >> b) & 1u);
         if (on && (pos[b] < 0 || (uint32_t)pos[b] >= e->slotLen)) return -66;
+        if (on && e->pagedSlots && (uint32_t)pos[b] >= e->slotPages[b] * dl::kPageRows) return -66;   // not reserved
         tok[b] = on ? tokens[b] : 0;
         ps[b] = on ? pos[b] : 0;
     }
     DL_CUDA_CHECK(cudaMemcpyAsync(e->g.tokens, tok, nb * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
     DL_CUDA_CHECK(cudaMemcpyAsync(e->g.pos, ps, nb * sizeof(int32_t), cudaMemcpyHostToDevice, stream));
     DL_CUDA_CHECK(cudaEventRecord(e->slotStaged, stream));
+    if (e->pagedSlots) DL_TRY(uploadPages(e, stream));
     const dl::SlotStep sl{mask};
     return dl::engineForward(*e, nb, 2, false, stream, nullptr, &sl);
 }
@@ -1316,4 +1433,64 @@ DL_EXPORT int dl_engine_slots_step_logprobs(void *h, const int32_t *tokens, cons
 
 DL_EXPORT int dl_engine_slots_step(void *h, const int32_t *tokens, const int32_t *pos, uint32_t inactiveMask, int32_t *out, cudaStream_t stream) {
     return dl_engine_slots_step_logprobs(h, tokens, pos, inactiveMask, out, nullptr, stream);
+}
+
+// ---- paged slots: the page allocator (dl_engine_set_slot_cache) -------------------------------------------------------------------
+
+// Grows slot `slot`'s pages to cover rows [0, rows), free pages taken lowest index first. -68 when the pool has too few free pages
+// (nothing changes then); -60 past the slot length.
+DL_EXPORT int dl_engine_slot_reserve(void *h, uint32_t slot, uint32_t rows) {
+    Engine *e = (Engine *)h;
+    if (!e->pagedSlots || e->slots < 2 || slot >= e->slots) return -64;
+    if (rows > e->slotLen) return -60;
+    const uint32_t need = (rows + dl::kPageRows - 1) / dl::kPageRows;
+    uint32_t &have = e->slotPages[slot];
+    if (need <= have) return 0;
+    if ((uint32_t)std::count(e->pageUsed.begin(), e->pageUsed.end(), 0) < need - have) return -68;
+    DL_TRY(editPages(e));
+    int32_t *row = e->pageHost + (size_t)slot * e->nPages;
+    for (uint32_t p = 0; p < e->nPages && have < need; p++)
+        if (!e->pageUsed[p]) { e->pageUsed[p] = 1; row[have++] = (int32_t)p; }
+    return 0;
+}
+
+// Returns every page of slot `slot` to the pool.
+DL_EXPORT int dl_engine_slot_release(void *h, uint32_t slot) {
+    Engine *e = (Engine *)h;
+    if (!e->pagedSlots || e->slots < 2 || slot >= e->slots) return -64;
+    if (e->slotPages[slot] == 0) return 0;
+    DL_TRY(editPages(e));
+    int32_t *row = e->pageHost + (size_t)slot * e->nPages;
+    for (uint32_t i = 0; i < e->slotPages[slot]; i++) { e->pageUsed[row[i]] = 0; row[i] = -1; }
+    e->slotPages[slot] = 0;
+    return 0;
+}
+
+// Shrinks slot `slot` to the pages that cover rows [0, rows) and returns the rest to the pool (a slot taken by a request that needs
+// fewer rows than its previous occupant left).
+DL_EXPORT int dl_engine_slot_trim(void *h, uint32_t slot, uint32_t rows) {
+    Engine *e = (Engine *)h;
+    if (!e->pagedSlots || e->slots < 2 || slot >= e->slots) return -64;
+    const uint32_t keep = (rows + dl::kPageRows - 1) / dl::kPageRows;
+    if (keep >= e->slotPages[slot]) return 0;
+    DL_TRY(editPages(e));
+    int32_t *row = e->pageHost + (size_t)slot * e->nPages;
+    for (uint32_t i = keep; i < e->slotPages[slot]; i++) { e->pageUsed[row[i]] = 0; row[i] = -1; }
+    e->slotPages[slot] = keep;
+    return 0;
+}
+
+// Free pages of the pool (0 without paged slots).
+DL_EXPORT uint32_t dl_engine_free_pages(void *h) {
+    Engine *e = (Engine *)h;
+    if (!e->pagedSlots || e->slots < 2) return 0;
+    return (uint32_t)std::count(e->pageUsed.begin(), e->pageUsed.end(), 0);
+}
+
+// Slot `slot`'s physical pages in logical order into out[0..cap); returns how many it holds (negative: not paged).
+DL_EXPORT int dl_engine_slot_pages(void *h, uint32_t slot, int32_t *out, uint32_t cap) {
+    Engine *e = (Engine *)h;
+    if (!e->pagedSlots || e->slots < 2 || slot >= e->slots) return -64;
+    for (uint32_t i = 0; i < e->slotPages[slot] && i < cap; i++) out[i] = e->pageHost[(size_t)slot * e->nPages + i];
+    return (int)e->slotPages[slot];
 }

@@ -10,6 +10,7 @@ constexpr int kApiMaxRanks = 8;
 constexpr int kApiLogprobsWords = 44;   // int32 words of one row's log-probabilities (dl_engine_logprobs)
 constexpr int kApiLogprobsMaxTop = 20;
 constexpr int kLogprobsControlled = 1, kLogprobsSharedRow = 2;   // dl_engine_logprobs flags
+constexpr int kEngineErrPoolShort = -68;   // dl_engine_slot_reserve / dl_engine_slot_copy: too few free pages, nothing changed
 
 struct EngineConfig {   // mirrored by ctypes in distributed_llama_b200/ops/cuda_lib.py
     uint32_t dim, nLayers, nHeads, nKvHeads, headDim, ffDim, vocab, seqLen;   // per-rank (sliced) head/ff/vocab counts
@@ -92,6 +93,16 @@ int dl_engine_choices_forward(void *h, int nb, uint32_t P, uint32_t C, uint32_t 
 // KV-cache slots (csrc/cuda/attn_decode.cu): n <= 8 independent sequences, slot s = rows [0, floor(seqLen / n)) of its own cache block
 int dl_engine_set_slots(void *h, uint32_t n);
 uint32_t dl_engine_slot_len(void *h);
+// Paged slots: set paged = 1 before dl_engine_set_slots and the slots share every layer plane as one pool of floor(seqLen / 64)
+// 64-row pages; dl_engine_slot_len is then 64 * floor(seqLen / 64). A slot's rows must be reserved before a step or prefill writes
+// them. dl_engine_slot_reserve returns kEngineErrPoolShort, changing nothing, when the pool has too few free pages; pages are taken
+// lowest index first.
+int dl_engine_set_slot_cache(void *h, int paged);
+int dl_engine_slot_reserve(void *h, uint32_t slot, uint32_t rows);
+int dl_engine_slot_release(void *h, uint32_t slot);
+int dl_engine_slot_trim(void *h, uint32_t slot, uint32_t rows);   // keeps the pages of rows [0, rows), frees the rest
+uint32_t dl_engine_free_pages(void *h);
+int dl_engine_slot_pages(void *h, uint32_t slot, int32_t *out, uint32_t cap);
 int dl_engine_slot_copy(void *h, uint32_t src, uint32_t dst, uint32_t P, cudaStream_t stream);
 int dl_engine_slot_sampling(void *h, uint32_t slot, unsigned long long seed, float temperature, float topp, float presence, float frequency,
                             const int32_t *ids, const float *vals, int nBias, cudaStream_t stream);

@@ -9,6 +9,12 @@ enum { EPI_STORE_ = 0, EPI_RESIDUAL_ = 1, EPI_SWIGLU_ = 2, EPI_ARGMAX_ = 3, EPI_
 
 // In-kernel one-shot all-reduce over NVLink peer memory (see the EPI_RESIDUAL epilogue of gemv_q40_tma.cu).
 constexpr int kMaxRanks = 8;
+// Rows of a KV-cache page of the paged slot layout (engine.cu: dl_engine_set_slot_cache).
+constexpr uint32_t kPageRows = 64;
+// Physical row of logical row `row` through a slot's page table.
+__device__ __forceinline__ uint32_t pagedRow(const int32_t *table, uint32_t row) {
+    return (uint32_t)__ldg(table + row / kPageRows) * kPageRows + row % kPageRows;
+}
 extern uint32_t gHiddenAct;   // process-wide gate activation (0 = SiLU, 1 = GELU), set by dl_engine_create from the model header
 
 // Sets gHiddenAct for the launches of one stand-alone entry point and restores the engine's value afterwards (the launchers read
@@ -195,6 +201,14 @@ struct RopeKvArgs {
     uint64_t slotStride;
 };
 int launchRopeKv(const RopeKvArgs &a, int nb, cudaStream_t stream, bool pdl);
+// Paged slots (slotStride 0, seqLen = the rows of the whole layer plane): token t stores its logical row pos[t] at physical row
+// pageTable[t * pageTableStride + pos / 64] * 64 + pos % 64 (stride 0: every token through one slot's table). The paged kernels take
+// these derived structs so that the others keep their argument layout, and with it their code.
+struct PagedRopeKvArgs : RopeKvArgs {
+    const int32_t *pageTable;
+    uint32_t pageTableStride;
+};
+int launchRopeKvPaged(const PagedRopeKvArgs &a, int nb, cudaStream_t stream, bool pdl);
 
 // Attention of B choices that share the prompt rows [0, P] of the cache (attn_decode.cu). Query row b (choice b, rotary position
 // P + 1 + j, already normalised and rotated by ropeKvKernel) attends to [0, P] and to its own rows [P + 1 + b * C, P + 1 + b * C + j].
@@ -233,6 +247,13 @@ struct SlotAttnArgs {
     uint32_t outStride;
 };
 int launchSlotAttn(const SlotAttnArgs &a, cudaStream_t stream, bool pdl);
+// Paged slots (slotStride unused): every layer plane holds planeRows rows per KV head, and row b's logical row r lives at physical
+// row pageTable[b * pageStride + r / 64] * 64 + r % 64. L is the longest a slot may grow.
+struct PagedSlotAttnArgs : SlotAttnArgs {
+    const int32_t *pageTable;
+    uint32_t pageStride, planeRows;
+};
+int launchSlotAttnPaged(const PagedSlotAttnArgs &a, cudaStream_t stream, bool pdl);
 
 struct AttnArgs {
     const float *qkv;
@@ -259,6 +280,9 @@ struct AttnPrefillArgs {
     const __half *kScale, *vScale;          // q80 scale planes; null: bf16 cache
     __nv_bfloat16 *out;          // [T][outStride], head h at columns h * headDim
     uint32_t outStride;
+    // Paged slot (set): seqLen is the rows of the whole layer plane, and logical row r lives at physical row
+    // pageTable[r / 64] * 64 + r % 64; pages up to row p0 + T - 1 must be mapped.
+    const int32_t *pageTable;
 };
 int launchAttnPrefillTc(const AttnPrefillArgs &a, cudaStream_t stream, bool pdl = false);   // 1: shape not covered
 

@@ -21,6 +21,7 @@ import torch
 
 from . import host
 from .formats.model_file import ModelFile
+from .ops.cuda_lib import PAGE_ROWS, SLOT_CACHE_LAYOUTS
 from .parallel.control import (OP_CHOICES_FIRST, OP_CHOICES_SEED, OP_CHOICES_STEP, OP_CONTROLS, OP_DECODE_N, OP_FILTERS, OP_PREFILL,
                                OP_SEED, OP_STEP_GREEDY, OP_STEP_LOGITS, OP_STEP_SAMPLE, _active_mask, _f32_bits, _split_seed)
 
@@ -344,8 +345,11 @@ class ParallelRefused(ValueError):
     """A --parallel value this configuration cannot serve (see parallel_refusal)."""
 
 
-def parallel_refusal(parallel: int, n_ranks: int = 1, n_experts: int = 0) -> Optional[str]:
-    """Why `parallel` concurrent sequences (KV-cache slots) cannot run in this configuration, or None if they can."""
+def parallel_refusal(parallel: int, n_ranks: int = 1, n_experts: int = 0, cache: str = "split") -> Optional[str]:
+    """Why `parallel` concurrent sequences (KV-cache slots) in layout `cache` cannot run in this configuration, or None if
+    they can."""
+    if cache not in SLOT_CACHE_LAYOUTS:
+        return f"--parallel-cache must be split or paged, not {cache!r}"
     if not 1 <= parallel <= MAX_CHOICES:
         return f"--parallel must be from 1 to {MAX_CHOICES}"
     if parallel == 1:
@@ -384,6 +388,11 @@ class SlotRequest:
         """How many of the request's messages slot `slot`'s prompt cache covers (slot choice; ties go to the lowest index)."""
         return 0
 
+    def prompt_len(self, slot: int) -> int:
+        """P, the position of the prompt's last token, as prepare(slot) would return it, without changing anything (paged slots:
+        what the request reserves before it is admitted)."""
+        raise NotImplementedError
+
     def prepare(self, slot: int):
         """Resolves the prompt against slot `slot`'s cache: (tokens to prefill, their start position, last prompt token, P)
         with P = the last prompt token's position."""
@@ -413,16 +422,30 @@ class SlotScheduler:
     end of sequence or after min(max_tokens, slot_len - P) tokens. If on_token raises (a client went away), the request ends
     and frees its slots; the other requests continue.
 
+    Paged slots (backend.paged: the slots share the KV cache as one pool of 64-row pages): a request is admitted, still first in,
+    first out, only when every slot it takes can hold rows [0, P + 64) (P = prompt_len(slot), capped at slot_len); otherwise it
+    and everything behind it wait. Each slot it takes keeps exactly the pages of those rows: pages a previous occupant left beyond
+    them go back to the pool (the rows it reuses, [0, P), lie inside). A running row reserves its next page when its position reaches a page boundary. A finished slot
+    keeps its pages as its prompt cache; when an admission or a growing row needs pages, idle slots' caches are evicted whole, least
+    recently finished first (backend.slot_release, then on_evict(slot): the server forgets that slot's prompt cache). A row that
+    cannot get a page ends there, as if it had reached its length limit. A request that needs more pages than the pool holds fails.
+
     `backend` provides slots, slot_len, slot_prefill(slot, tokens, pos), slot_copy(src, dst, P),
     slot_sampling(slot, seed, temperature, topp, presence, frequency, bias, top_k=.., min_p=..) (the filters are passed only
     when one is on) and slots_step(tokens, pos, active) (InferenceSession(parallel=N)); for requests with logprobs also slot_logprobs(slot, k) and slots_step_logprobs(tokens, pos,
     active) -> (draws, per-slot entries), used only while such a request holds a slot."""
 
-    def __init__(self, backend, seed_source: Callable[[], int]):
+    def __init__(self, backend, seed_source: Callable[[], int], on_evict: Optional[Callable[[int], None]] = None):
+        """Paged backends (backend.paged true) also provide slot_reserve(slot, rows) -> bool, slot_trim(slot, rows),
+        slot_release(slot), free_pages() and slot_pages(slot)."""
         self.backend = backend
         self.seed_source = seed_source
+        self.on_evict = on_evict
         self.queue: "queue.Queue" = queue.Queue()
         self.owner: List[Optional[object]] = [None] * backend.slots
+        self.paged = bool(getattr(backend, "paged", False))
+        self._finished = [0] * backend.slots   # paged: when each slot's cache was last left idle (eviction order)
+        self._clock = 0
         self._stop = threading.Event()
 
     def submit(self, req: SlotRequest) -> None:
@@ -436,15 +459,64 @@ class SlotScheduler:
         self._stop.set()
         self.queue.put(None)
 
-    def _admit(self, req: SlotRequest, free: List[int], rows: List[dict]) -> None:
+    # ---- paged slots: pages per slot, eviction ----
+    def _pages(self, slot: int) -> int:
+        return len(self.backend.slot_pages(slot))
+
+    def _evict_for(self, pages: int, keep) -> bool:
+        """Evicts idle caches, least recently finished first and none of `keep`, until `pages` pages are free. False (nothing
+        evicted) if even all of them would not do."""
+        be = self.backend
+        idle = sorted((s for s in range(be.slots) if self.owner[s] is None and s not in keep and self._pages(s) > 0),
+                      key=lambda s: self._finished[s])
+        if be.free_pages() + sum(self._pages(s) for s in idle) < pages:
+            return False
+        for s in idle:
+            if be.free_pages() >= pages:
+                break
+            be.slot_release(s)
+            if self.on_evict is not None:
+                self.on_evict(s)
+        return True
+
+    def _reserve(self, slot: int, rows: int, keep) -> bool:
+        """Grows `slot` to cover rows [0, rows), evicting idle caches if the pool is short."""
+        be = self.backend
+        short = -(-rows // PAGE_ROWS) - self._pages(slot)
+        if short <= 0:
+            return True
+        return self._evict_for(short, keep) and be.slot_reserve(slot, rows)
+
+    def _admit(self, req: SlotRequest, free: List[int], rows: List[dict]) -> bool:
+        """Starts `req` in free slots; False when paged slots cannot reserve its pages yet (nothing changed)."""
         be = self.backend
         rows_needed = 1 if req.temperature == 0.0 else req.n
         first = max(free, key=lambda s: (req.cached_prefix(s), -s))
         slots = [first] + [s for s in free if s != first][:rows_needed - 1]
         try:
+            if self.paged:
+                want = min(be.slot_len, req.prompt_len(first) + PAGE_ROWS)
+                pages = -(-want // PAGE_ROWS)
+                if pages * len(slots) > be.slot_len // PAGE_ROWS:
+                    raise ValueError(f"the request needs {pages * len(slots)} KV-cache pages, more than the pool's {be.slot_len // PAGE_ROWS}")
+                # free pages the admission takes once its slots give back what they hold beyond `want`
+                if not self._evict_for(max(0, sum(pages - self._pages(s) for s in slots)), slots):
+                    return False
+                for s in slots:
+                    be.slot_trim(s, want)
+                for s in slots:
+                    be.slot_reserve(s, want)   # cannot fail: the pages are free
             self._start(req, slots, rows, rows_needed)
         except Exception as e:   # e.g. the client went away while its prompt was prepared
+            self._drop_pages(slots)
             req.fail(e, slots)
+        return True
+
+    def _drop_pages(self, slots) -> None:
+        """Paged: slots whose rows no longer match a prompt cache give their pages back."""
+        if self.paged:
+            for s in slots:
+                self.backend.slot_release(s)
 
     def _start(self, req: SlotRequest, slots: List[int], rows: List[dict], rows_needed: int) -> None:
         be, first = self.backend, slots[0]
@@ -478,6 +550,8 @@ class SlotScheduler:
             if self.owner[s] is job:
                 self.owner[s] = None
                 rows[s] = None
+                self._clock += 1
+                self._finished[s] = self._clock
 
     def run(self) -> None:
         """The engine loop; returns after stop()."""
@@ -498,9 +572,11 @@ class SlotScheduler:
             while waiting:
                 free = [s for s in range(N) if self.owner[s] is None]
                 need = 1 if waiting[0].temperature == 0.0 else waiting[0].n
-                if len(free) < need:
+                if len(free) < need or not self._admit(waiting[0], free, rows):
                     break
-                self._admit(waiting.pop(0), free, rows)
+                waiting.pop(0)
+            if self.paged:
+                self._grow(rows)
             active = [r is not None for r in rows]
             if not any(active):
                 continue
@@ -528,17 +604,35 @@ class SlotScheduler:
                             r["done"].add(i)
                 except Exception as e:
                     self._release(job, rows)
+                    self._drop_pages(job["slots"])
                     req.fail(e, job["slots"])
                     continue
                 if len(r["done"]) == len(r["choices"]):
-                    rows[s] = None
-                    job["live"] -= 1
-                    if job["live"] == 0:
-                        self._release(job, rows)
-                        try:
-                            req.finish(job["out"], job["slots"], job["P"])
-                        except Exception as e:
-                            req.fail(e, job["slots"])
+                    self._row_done(s, rows)
+
+    def _row_done(self, s: int, rows: List[Optional[dict]]) -> None:
+        """Slot s's row has finished every completion it serves; the request finishes with its last row."""
+        job = rows[s]["job"]
+        req = job["req"]
+        rows[s] = None
+        job["live"] -= 1
+        if job["live"] == 0:
+            self._release(job, rows)
+            try:
+                req.finish(job["out"], job["slots"], job["P"])
+            except Exception as e:
+                self._drop_pages(job["slots"])
+                req.fail(e, job["slots"])
+
+    def _grow(self, rows: List[Optional[dict]]) -> None:
+        """Paged: every row about to write a row past its pages reserves the next page; one that cannot get a page ends."""
+        for s in range(len(rows)):
+            r = rows[s]
+            if r is None:
+                continue
+            if not self._reserve(s, r["pos"] + 1, {t for t, x in enumerate(rows) if x is not None}):
+                r["done"].update(r["choices"])
+                self._row_done(s, rows)
 
 
 class InferenceSession(TokenSteps):
@@ -546,20 +640,22 @@ class InferenceSession(TokenSteps):
                  temperature: float = 0.0, topp: float = 0.9, seed: int = 12345, device: Optional[str] = None,
                  max_batch: int = 8, use_pdl: bool = True, comm=None, moe_mode: str = "auto", presence_penalty: float = 0.0,
                  frequency_penalty: float = 0.0, logit_bias: Optional[dict] = None, parallel: int = 1,
-                 kv_cache_float_type: str = "bf16", top_k: int = 0, min_p: float = 0.0):
+                 kv_cache_float_type: str = "bf16", top_k: int = 0, min_p: float = 0.0, parallel_cache: str = "split"):
         """presence_penalty, frequency_penalty and logit_bias ({token id: value}) are the sampling controls of every
         completion (host Sampler.set_controls; they may be changed later through self.sampler.set_controls, which restarts the
         counts of the current completion). top_k and min_p are the sampling filters of every sampled draw (host
         Sampler.set_filters, 0: off; self.sampler.set_filters changes them). parallel > 1 splits the KV cache into that many slots for SlotScheduler
         (slot_prefill, slot_copy, slot_sampling, slots_step); the single-sequence calls then must not be used.
-        kv_cache_float_type: "bf16" or "q80" (runtime.engine.Engine)."""
+        kv_cache_float_type: "bf16" or "q80" (runtime.engine.Engine). parallel_cache: the layout of the slots, "split" (each
+        slot owns floor(context / parallel) rows) or "paged" (the slots share the cache as one pool of 64-row pages, so one
+        request may use the whole context; see SlotScheduler for the rules)."""
         from .models.loader import load_device_weights
         from .runtime.engine import Engine
 
         self.model_file = ModelFile(model_path, max_seq_len)
         self.header = self.model_file.header
         self.comm = comm
-        why = parallel_refusal(parallel, comm.world_size if comm is not None else 1, self.header.n_experts)
+        why = parallel_refusal(parallel, comm.world_size if comm is not None else 1, self.header.n_experts, parallel_cache)
         if why:
             raise ParallelRefused(why)
         rank = comm.rank if comm is not None else 0
@@ -580,8 +676,9 @@ class InferenceSession(TokenSteps):
         self.pos = 0
         self.slots = parallel
         if parallel > 1:
-            self.engine.set_slots(parallel)
+            self.engine.set_slots(parallel, parallel_cache)
         self.slot_len = self.engine.slot_len
+        self.paged = self.engine.paged
 
     # ---- KV-cache slots (SlotScheduler) ----
     def slot_prefill(self, slot: int, tokens: Sequence[int], pos: int) -> None:
@@ -589,6 +686,21 @@ class InferenceSession(TokenSteps):
 
     def slot_copy(self, src: int, dst: int, P: int) -> None:
         self.engine.slot_copy(src, dst, P)
+
+    def slot_reserve(self, slot: int, rows: int) -> bool:
+        return self.engine.slot_reserve(slot, rows)
+
+    def slot_release(self, slot: int) -> None:
+        self.engine.slot_release(slot)
+
+    def slot_trim(self, slot: int, rows: int) -> None:
+        self.engine.slot_trim(slot, rows)
+
+    def free_pages(self) -> int:
+        return self.engine.free_pages()
+
+    def slot_pages(self, slot: int) -> List[int]:
+        return self.engine.slot_pages(slot)
 
     def slot_sampling(self, slot: int, seed: int, temperature: float, topp: float, presence: float, frequency: float, bias, *,
                       top_k: int = 0, min_p: float = 0.0) -> None:

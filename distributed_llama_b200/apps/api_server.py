@@ -449,12 +449,21 @@ class ApiServer:
         chat = parse_chat(req.json, self.ctx.args, self.ctx.sampler.vocab_size, n_slots, 1)   # --parallel > 1 runs on one GPU
         resp = ChatResponse(self, req, chat)
         api, slot_len, messages = self, self.slot_len, chat.messages
+        lens = {}   # prompt_len by (start position, cached messages)
 
         class Chat(SlotRequest):
             def cached_prefix(self, slot):
                 items = caches[slot].items
                 ok = len(messages) > len(items) and all(items[i][1] == messages[i] for i in range(len(items)))
                 return len(items) if ok else 0
+
+            def prompt_len(self, slot):
+                n = self.cached_prefix(slot)
+                start = caches[slot].items[n - 1][0] if n else 0
+                if (start, n) not in lens:   # the head of a blocked queue asks again before every step
+                    content, _ = api.gen.generate(messages[n:], True)
+                    lens[(start, n)] = min(start + len(api.ctx.tokenizer.encode(content, start == 0, True)) - 1, slot_len)
+                return lens[(start, n)]
 
             def prepare(self, slot):
                 prefill, start, token, P, self.n_prompt, public = api.prepare_prompt(caches[slot], messages, slot_len)
@@ -494,7 +503,7 @@ def serve_parallel(ctx: AppContext, srv: socket.socket, api: ApiServer, n_slots:
     backend = ctx.sess if ctx.sess is not None else ctx.inference
     api.slot_len = backend.slot_len
     caches = [NaiveCache() for _ in range(n_slots)]
-    sched = SlotScheduler(backend, ctx.sampler.next_seed)
+    sched = SlotScheduler(backend, ctx.sampler.next_seed, on_evict=lambda s: caches[s].clear())
     pending = threading.Semaphore(0)   # one release per finished connection
 
     def handle(conn):
@@ -578,8 +587,11 @@ USAGE = """Usage: dllama-api {--model <path>} {--tokenizer <path>} [--host <addr
         [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>] [--gpus <n>] [--workers <ip:port> ...]
         [--temperature <temp>] [--topp <t>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]
         [--top-k <k>] [--min-p <p>] [--chat-template {llama2|llama3|deepSeek3|chatml}] [--parallel <n>]
+        [--parallel-cache {split|paged}]
         --parallel <n>: decode up to n (1..8) chat requests together, each in its own KV-cache slot of
                         floor(context / n) tokens; single GPU and dense models only
+        --parallel-cache paged: the slots share the KV cache as one pool of 64-token pages instead, so a request
+                        may use the whole context while the pool has room (default split)
 """
 
 
@@ -590,7 +602,7 @@ def main(argv=None) -> int:
     if args.help:
         sys.stderr.write(USAGE)
         return 0
-    why = parallel_refusal(args.parallel, max(args.gpus, 1, int(os.environ.get("WORLD_SIZE", "1"))) + len(args.workers))
+    why = parallel_refusal(args.parallel, max(args.gpus, 1, int(os.environ.get("WORLD_SIZE", "1"))) + len(args.workers), 0, args.parallel_cache)
     if why:
         sys.stderr.write(why + "\n")
         return 1

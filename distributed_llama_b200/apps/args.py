@@ -43,6 +43,7 @@ class AppArgs:
     gpus: int = 0            # spawn this many local ranks (0 = use the current torch.distributed world / single GPU)
     moe_mode: str = "auto"   # tp | ep | auto
     parallel: int = 1        # dllama-api: chat requests decoded together, one KV-cache slot each (1..8)
+    parallel_cache: str = "split"   # dllama-api: the slots' KV-cache layout: split (floor(context / n) rows each) | paged (shared 64-row pages)
     kv_cache_float_type: str = "bf16"   # KV-cache storage: bf16 | q80 (int8 blocks of 32 with an f16 scale)
 
 
@@ -140,6 +141,8 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
             a.kv_cache_float_type = value
         elif name == "--parallel" and not require_mode:   # dllama-api only; its range is checked by api.parallel_refusal
             a.parallel = int(value)
+        elif name == "--parallel-cache" and not require_mode:   # dllama-api only; checked by api.parallel_refusal
+            a.parallel_cache = value
         else:
             raise ValueError(f"Unknown option: {name}")
         i += 2

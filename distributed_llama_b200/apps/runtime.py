@@ -185,7 +185,8 @@ def run_inference_app(args: AppArgs, handler: Callable[[AppContext], None]) -> N
     sess = InferenceSession(args.model, args.tokenizer, max_seq_len=args.max_seq_len, temperature=args.temperature,
                             topp=args.topp, seed=args.seed, comm=comm, moe_mode=getattr(args, "moe_mode", "auto") or "auto",
                             presence_penalty=args.presence_penalty, frequency_penalty=args.frequency_penalty,
-                            parallel=getattr(args, "parallel", 1), kv_cache_float_type=args.kv_cache_float_type,
+                            parallel=getattr(args, "parallel", 1), parallel_cache=getattr(args, "parallel_cache", "split"),
+                            kv_cache_float_type=args.kv_cache_float_type,
                             top_k=getattr(args, "top_k", 0), min_p=getattr(args, "min_p", 0.0))
     chan = open_control_channel(comm)
     if rank != 0:

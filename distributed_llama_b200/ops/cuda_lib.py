@@ -175,6 +175,22 @@ def lib() -> C.CDLL:
     L.dl_engine_set_slots.restype = i32
     L.dl_engine_slot_len.argtypes = [vp]
     L.dl_engine_slot_len.restype = u32
+    L.dl_engine_set_slot_cache.argtypes = [vp, i32]
+    L.dl_engine_set_slot_cache.restype = i32
+    L.dl_engine_slot_reserve.argtypes = [vp, u32, u32]
+    L.dl_engine_slot_reserve.restype = i32
+    L.dl_engine_slot_trim.argtypes = [vp, u32, u32]
+    L.dl_engine_slot_trim.restype = i32
+    L.dl_engine_slot_release.argtypes = [vp, u32]
+    L.dl_engine_slot_release.restype = i32
+    L.dl_engine_free_pages.argtypes = [vp]
+    L.dl_engine_free_pages.restype = u32
+    L.dl_engine_slot_pages.argtypes = [vp, u32, ip, u32]
+    L.dl_engine_slot_pages.restype = i32
+    L.dl_slot_attn_paged.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, u32, u32, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, u32, vp]
+    L.dl_slot_attn_paged.restype = i32
+    L.dl_attn_prefill_tc_paged.argtypes = [vp, u32, u32, u32, u32, u32, u32, u32, vp, vp, vp, vp, vp, vp, u32, vp]
+    L.dl_attn_prefill_tc_paged.restype = i32
     L.dl_engine_slot_copy.argtypes = [vp, u32, u32, u32, vp]
     L.dl_engine_slot_copy.restype = i32
     L.dl_engine_slot_sampling.argtypes = [vp, u32, C.c_uint64, f32, f32, f32, f32, ip, C.POINTER(f32), i32, vp]
@@ -239,7 +255,14 @@ _ERRORS = {
     -40: "the dense-weight GEMV has no in-kernel all-reduce (dense weight files use library collectives under tensor parallelism)",
     -41: "expert-routed dense-weight GEMV needs one token, the routing slots' expert indices and k >= 1",
     -53: "logit_bias token id outside the sampled vocabulary",
+    -66: "a slot position past the rows the slot holds",
+    -68: "the KV-cache page pool has too few free pages",
+    -69: "paged KV-cache slots need the tensor-core prefill attention",
 }
+
+POOL_SHORT = -68   # dl_engine_slot_reserve / dl_engine_slot_copy: too few free pages, nothing changed
+PAGE_ROWS = 64     # rows of a KV-cache page (paged slots)
+SLOT_CACHE_LAYOUTS = ("split", "paged")   # --parallel-cache
 
 
 def check(code: int, what: str) -> None:

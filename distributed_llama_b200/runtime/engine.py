@@ -164,7 +164,7 @@ class Engine:
         self.mega = False
         if h.n_experts == 0 and not self.dense and not self._parts and os.environ.get("DL_NO_MEGA") is None:
             self.enable_mega(True)     # persistent decode kernel by default; the engine falls back per call if a shape is unsupported
-        self.slots, self.slot_len = 1, self.seq_len
+        self.slots, self.slot_len, self.paged = 1, self.seq_len, False
         self._stage_tok = torch.zeros(max_batch, dtype=torch.int32).pin_memory()
         self._stage_pos = torch.zeros(max_batch, dtype=torch.int32).pin_memory()
 
@@ -282,12 +282,49 @@ class Engine:
         return out
 
     # -- KV-cache slots: up to 8 independent sequences decoded together (csrc/cuda/attn_decode.cu) --
-    def set_slots(self, n: int) -> None:
-        """Splits every layer's KV cache into n slots of floor(seq_len / n) rows. Single GPU, dense q40 layers only; n = 1 is
-        the ordinary single-sequence engine."""
+    def set_slots(self, n: int, layout: str = "split") -> None:
+        """Splits every layer's KV cache into n slots of floor(seq_len / n) rows (layout "split"), or lets n slots share it as
+        one pool of 64-row pages (layout "paged": slot_len is 64 * floor(seq_len / 64), and a slot's rows must be reserved with
+        slot_reserve before a step or prefill writes them). Single GPU, dense q40 layers only; n = 1 is the ordinary
+        single-sequence engine."""
+        if layout not in cl.SLOT_CACHE_LAYOUTS:
+            raise ValueError(f"unknown KV-cache slot layout {layout!r} (expected split or paged)")
+        if self.slots > 1:   # the layout is chosen while the cache is not split
+            cl.check(self._lib.dl_engine_set_slots(self._h, 1), "engine_set_slots")
+        cl.check(self._lib.dl_engine_set_slot_cache(self._h, 1 if layout == "paged" else 0), "engine_set_slot_cache")
         cl.check(self._lib.dl_engine_set_slots(self._h, int(n)), "engine_set_slots")
         self.slots = int(n)
+        self.paged = layout == "paged" and n > 1
         self.slot_len = int(self._lib.dl_engine_slot_len(self._h))
+
+    def slot_reserve(self, slot: int, rows: int) -> bool:
+        """Paged slots: grows slot `slot`'s pages to cover rows [0, rows), lowest free pages first. False, with nothing changed,
+        when the pool has too few free pages."""
+        rc = self._lib.dl_engine_slot_reserve(self._h, int(slot), int(rows))
+        if rc == cl.POOL_SHORT:
+            return False
+        cl.check(rc, "engine_slot_reserve")
+        return True
+
+    def slot_trim(self, slot: int, rows: int) -> None:
+        """Paged slots: keeps the pages of rows [0, rows) of slot `slot` and returns the rest to the pool."""
+        cl.check(self._lib.dl_engine_slot_trim(self._h, int(slot), int(rows)), "engine_slot_trim")
+
+    def slot_release(self, slot: int) -> None:
+        """Paged slots: returns slot `slot`'s pages to the pool."""
+        cl.check(self._lib.dl_engine_slot_release(self._h, int(slot)), "engine_slot_release")
+
+    def free_pages(self) -> int:
+        return int(self._lib.dl_engine_free_pages(self._h))
+
+    def slot_pages(self, slot: int) -> List[int]:
+        """Paged slots: slot `slot`'s physical pages in logical order."""
+        cap = max(1, self.seq_len // cl.PAGE_ROWS)
+        out = (C.c_int32 * cap)()
+        n = self._lib.dl_engine_slot_pages(self._h, int(slot), out, cap)
+        if n < 0:
+            cl.check(n, "engine_slot_pages")
+        return list(out[:n])
 
     def slot_prefill(self, slot: int, tokens: Sequence[int], start_pos: int) -> None:
         """Feeds tokens at positions start_pos.. into slot `slot` (tensor-core prefill kernels with the slot's cache). No logits."""
@@ -297,7 +334,8 @@ class Engine:
         self._prefill(tokens, start_pos, int(slot), False)
 
     def slot_copy(self, src: int, dst: int, P: int) -> None:
-        """Copies rows [0, P) of slot src into slot dst (every layer and KV head)."""
+        """Copies rows [0, P) of slot src into slot dst (every layer and KV head); paged slots: into dst's own pages, reserved
+        first (RuntimeError with code -68 when the pool is short)."""
         cl.check(self._lib.dl_engine_slot_copy(self._h, int(src), int(dst), int(P), cl.stream_ptr()), "engine_slot_copy")
 
     def slot_sampling(self, slot: int, seed: int, temperature: float, topp: float, presence: float = 0.0, frequency: float = 0.0,
