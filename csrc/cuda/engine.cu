@@ -1157,6 +1157,31 @@ DL_EXPORT int dl_engine_prefill_scratch(void *h, uint32_t rows, void *px, void *
     return 0;
 }
 
+// The mixture-of-experts stages of the last prompt chunk's last layer (tests), a null destination skipped. Tensor-core chunk of
+// `rows` tokens (the process-wide MoE prefill scratch; -1 unless its last call had this engine's shape and `rows` tokens): router logits f32
+// [rows][nExperts], expert ids and weights [rows][k], and the SwiGLU output of every (token, slot) pair, bf16 [rows][k][ff]. One-token
+// step (rows = 1): router logits [nExperts], ids and weights [k], and h f32 [k][ff]. The MoE rmsnorm output and the residual are
+// those of dl_engine_prefill_scratch.
+DL_EXPORT int dl_engine_moe_scratch(void *h, uint32_t rows, int tensorCores, void *logits, void *ids, void *weights, void *hPairs,
+                                    cudaStream_t stream) {
+    Engine &e = *(Engine *)h;
+    const dl::EngineConfig &c = e.cfg;
+    const uint32_t k = c.nActiveExperts;
+    if (c.nExperts == 0) return -1;
+    if (tensorCores) {
+        if (rows > c.maxPrefill) return -1;
+        return dl::moePrefillScratchRead(rows, k, c.nExperts, c.ffDim, (float *)logits, (int *)ids, (float *)weights,
+                                         (__nv_bfloat16 *)hPairs, stream);
+    }
+    if (rows != 1) return -1;
+    void *dst[4] = {logits, ids, weights, hPairs};
+    const void *src[4] = {e.g.routerLogits, e.g.expertIdx, e.g.expertWeight, e.g.h};
+    const size_t bytes[4] = {(size_t)c.nExperts * 4, (size_t)k * 4, (size_t)k * 4, (size_t)k * c.ffDim * 4};
+    for (int i = 0; i < 4; i++)
+        if (dst[i]) DL_CUDA_CHECK(cudaMemcpyAsync(dst[i], src[i], bytes[i], cudaMemcpyDeviceToDevice, stream));
+    return 0;
+}
+
 DL_EXPORT int dl_engine_set_prefill_min_tc(void *h, uint32_t n) { ((Engine *)h)->prefillMinTc = n; return 0; }
 
 // Captures one greedy decode step (forward of 1 token + argmax + position advance) into a graph, after a warm-up forward on

@@ -472,6 +472,9 @@ struct MoePrefillArgs {
     ArArgs ar;                    // nRanks > 1: partial sums are all-reduced over peer memory inside the combine kernel
 };
 int moePrefillFfn(const MoePrefillArgs &a, cudaStream_t stream);   // 1: shape not covered
+// Test read-back of the last moePrefillFfn call's routing and per-pair SwiGLU output (see moe_prefill.cu); -1: scratch too small
+int moePrefillScratchRead(uint32_t T, uint32_t k, uint32_t nExperts, uint32_t ff, float *logits, int *ids, float *weights,
+                          __nv_bfloat16 *hPairs, cudaStream_t stream);
 // Launch with the programmatic-dependent-launch attribute: the kernel may start while its predecessor in the stream is still running
 // and must execute griddepcontrol.wait (pdlWait) before touching anything the predecessor produces or still reads.
 template <typename... KArgs, typename... Args>

@@ -141,6 +141,7 @@ struct MoeScratch {
     __nv_bfloat16 *xs = nullptr, *hs = nullptr;
     float *ys = nullptr;
     size_t capPairs = 0, capDim = 0, capFf = 0, capExperts = 0, capTokens = 0;
+    uint32_t lastT = 0, lastK = 0, lastExperts = 0, lastFf = 0;   // shape of the call whose data the scratch holds (moePrefillScratchRead)
 };
 MoeScratch gMoe;
 
@@ -169,7 +170,33 @@ int moeEnsureScratch(uint32_t nPairs, uint32_t dim, uint32_t ff, uint32_t nExper
     return 0;
 }
 
+// out[p][:] = hs[slotOfPair[p]][:] (bf16 rows in pair order; a pair of another rank's expert gets zeros)
+__global__ void __launch_bounds__(256) moePairRowsKernel(const __nv_bfloat16 *__restrict__ hs, uint32_t ff, const int *__restrict__ slotOfPair,
+                                                          __nv_bfloat16 *__restrict__ out) {
+    const uint32_t p = blockIdx.x;
+    const int s = slotOfPair[p];
+    for (uint32_t i = threadIdx.x; i < ff; i += blockDim.x)
+        out[(size_t)p * ff + i] = s >= 0 ? hs[(size_t)s * ff + i] : __float2bfloat16(0.f);
+}
+
 }  // namespace
+
+// What the last moePrefillFfn call of the process left in its scratch, for T tokens of k routing slots (tests): router logits
+// [T][nExperts] f32, expert ids and weights [T][k], and the SwiGLU output of every (token, slot) pair [T][k][ff] bf16 in pair order.
+// A null destination is skipped; -1 unless the last call had exactly this T, k, nExperts and ff.
+int moePrefillScratchRead(uint32_t T, uint32_t k, uint32_t nExperts, uint32_t ff, float *logits, int *ids, float *weights,
+                          __nv_bfloat16 *hPairs, cudaStream_t stream) {
+    const MoeScratch &m = gMoe;
+    if (T == 0 || T != m.lastT || k != m.lastK || nExperts != m.lastExperts || ff != m.lastFf) return -1;
+    if (logits) DL_CUDA_CHECK(cudaMemcpyAsync(logits, m.routerLogits, (size_t)T * nExperts * 4, cudaMemcpyDeviceToDevice, stream));
+    if (ids) DL_CUDA_CHECK(cudaMemcpyAsync(ids, m.expertIdx, (size_t)T * k * 4, cudaMemcpyDeviceToDevice, stream));
+    if (weights) DL_CUDA_CHECK(cudaMemcpyAsync(weights, m.expertWeight, (size_t)T * k * 4, cudaMemcpyDeviceToDevice, stream));
+    if (hPairs) {
+        moePairRowsKernel<<<T * k, 256, 0, stream>>>(m.hs, ff, m.slotOfPair, hPairs);
+        DL_CUDA_CHECK(cudaGetLastError());
+    }
+    return 0;
+}
 
 int launchArResidual(float *x, const float *partial, uint32_t dim, uint32_t T, const ArArgs &ar, cudaStream_t stream, bool pdl) {
     DL_CUDA_CHECK(launchPdl(arResidualKernel, dim3((dim + 255) / 256, T), dim3(256), 0, stream, pdl, x, partial, dim, T, ar));
@@ -184,6 +211,7 @@ int moePrefillFfn(const MoePrefillArgs &a, cudaStream_t stream) {
     if (nPairs * 4 + (a.nLocal + 1) * 4 > 40 * 1024) return 1;
     { const int r = moeEnsureScratch(nPairs, a.dim, a.ff, a.nExperts, a.T); if (r != 0) return r; }
     MoeScratch &m = gMoe;
+    m.lastT = a.T; m.lastK = a.k; m.lastExperts = a.nExperts; m.lastFf = a.ff;
     RouterArgs ro{};
     ro.x = a.x; ro.normW = a.norm; ro.gate = a.gate; ro.eps = a.eps; ro.dim = a.dim; ro.nExperts = a.nExperts; ro.k = a.k;
     ro.logits = m.routerLogits; ro.counter = m.routerCounter; ro.expertIdx = m.expertIdx; ro.expertWeight = m.expertWeight;
@@ -221,4 +249,11 @@ DL_EXPORT int dl_moe_prefill_ffn(float *x, void *xnScratch, const float *norm, c
     DL_CUDA_CHECK(cudaMemcpyAsync(expertIdxOut, dl::gMoe.expertIdx, (size_t)T * k * sizeof(int), cudaMemcpyDeviceToDevice, stream));
     DL_CUDA_CHECK(cudaMemcpyAsync(expertWeightOut, dl::gMoe.expertWeight, (size_t)T * k * sizeof(float), cudaMemcpyDeviceToDevice, stream));
     return 0;
+}
+
+// The capacities of the MoE prefill scratch (tests): pairs, dim, ff, experts, tokens. They only grow; a call beyond any of them
+// reallocates every buffer.
+DL_EXPORT void dl_moe_scratch_caps(uint64_t out[5]) {
+    const dl::MoeScratch &m = dl::gMoe;
+    out[0] = m.capPairs; out[1] = m.capDim; out[2] = m.capFf; out[3] = m.capExperts; out[4] = m.capTokens;
 }

@@ -234,6 +234,10 @@ def lib() -> C.CDLL:
     L.dl_prefill_plan.restype = i32
     L.dl_engine_prefill_scratch.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.dl_engine_prefill_scratch.restype = i32
+    L.dl_engine_moe_scratch.argtypes = [vp, u32, i32, vp, vp, vp, vp, vp]
+    L.dl_engine_moe_scratch.restype = i32
+    L.dl_moe_scratch_caps.argtypes = [vp]
+    L.dl_moe_scratch_caps.restype = None
     L.dl_engine_set_prefill_min_tc.argtypes = [vp, u32]
     L.dl_engine_set_prefill_min_tc.restype = i32
     L.dl_engine_decode_graph.argtypes = [vp, i32, vp]

@@ -572,6 +572,21 @@ class Engine:
         cl.check(self._lib.dl_engine_prefill_scratch(self._h, rows, *ptrs, cl.stream_ptr()), "engine_prefill_scratch")
         return out
 
+    def moe_intermediates(self, rows: int, tensor_cores: bool) -> dict:
+        """The mixture-of-experts stages of the last prompt chunk of `rows` tokens (its last layer). Tensor-core chunk: "logits"
+        (f32 router logits [rows][E]), "ids" (int32 [rows][k]), "weights" (f32 [rows][k]) and "h" (bf16 SwiGLU output of every
+        (token, slot) pair [rows][k][ff]). One-token step (rows = 1): "logits" [E], "ids" and "weights" [k], "h" f32 [k][ff].
+        The MoE rmsnorm output and the residual are "xn" and "x" of prefill_intermediates."""
+        h, k, dev = self.w.header, self.w.header.n_active_experts, self.device
+        lead = (rows,) if tensor_cores else ()
+        out = {"logits": torch.empty(*lead, h.n_experts, dtype=torch.float32, device=dev),
+               "ids": torch.empty(*lead, k, dtype=torch.int32, device=dev),
+               "weights": torch.empty(*lead, k, dtype=torch.float32, device=dev),
+               "h": torch.empty(*lead, k, self.w.ff_dim, dtype=torch.bfloat16 if tensor_cores else torch.float32, device=dev)}
+        cl.check(self._lib.dl_engine_moe_scratch(self._h, rows, 1 if tensor_cores else 0, *(_p(out[n]) for n in ("logits", "ids", "weights", "h")),
+                                                 cl.stream_ptr()), "engine_moe_scratch")
+        return out
+
     def _prefill(self, tokens: List[int], start_pos: int, slot: int, want_logits: bool) -> None:
         arr = (C.c_int32 * len(tokens))(*tokens)
         cl.check(self._lib.dl_engine_prefill(self._h, arr, len(tokens), start_pos, slot, 1 if want_logits else 0, cl.stream_ptr()),

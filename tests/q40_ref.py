@@ -1,5 +1,5 @@
 """Float64 reference helpers shared by the q40 matrix tests (tests/test_gpu_gemm_tc.py, tests/test_gpu_moe.py, tests/test_gpu_gemv.py)
-and the model-level tests (tests/test_gpu_mega_shapes.py, tests/test_gpu_prefill_chain.py).
+and the model-level tests (tests/test_gpu_mega_shapes.py, tests/test_gpu_prefill_chain.py, tests/test_gpu_moe_chain.py).
 
 * Random q40 matrices as raw 18-byte blocks (f16 scale + 16 bytes of nibbles) and their device layout.
 * The weights the tensor-core dequant warps build from them: rn_bf16(rn_bf16(f16 scale) * (q - 8)).
@@ -46,6 +46,19 @@ def w_tc_of(sc, q):
     return (sb * q.float()).bfloat16().double()
 
 
+def q40_exact(raw, rows, n):
+    """raw blocks of a [rows][n] matrix dequantised exactly (the decode GEMV's weights), f64 [rows][n], and |w| + 8 |scale| (its
+    f32 error scale: the GEMV multiplies unsigned nibbles and subtracts 8 x scale x sum(q) afterwards)."""
+    sc, q = q40_parts(raw, rows, n)
+    s = sc.double().repeat_interleave(32, dim=1)
+    return s * q, s.abs() * (q.abs() + 8)
+
+
+def q40_tc(raw, rows, n):
+    """raw blocks of a [rows][n] matrix as the tensor-core dequant builds it (w_tc_of), f64."""
+    return w_tc_of(*q40_parts(raw, rows, n))
+
+
 class Experts:
     """E stacked random q40 matrices [rows][n] (raw 18-byte blocks + the device layout). Row r of matrix e is stack row e * rows + r.
     Scales are +-(0.5 .. 1.5) / (4 sqrt(n)), so a dot product with unit-variance activations is of order 1."""
@@ -73,19 +86,17 @@ class Experts:
             self._dev[first, count] = dst
         return self._dev[first, count]
 
-    def _parts(self, e):
+    def _raw(self, e):
         blk = self.n // 32
-        return q40_parts(self.raw[e * self.rows * blk:(e + 1) * self.rows * blk], self.rows, self.n)
+        return self.raw[e * self.rows * blk:(e + 1) * self.rows * blk]
 
     def w_exact(self, e):
-        """Matrix e dequantised exactly (the decode GEMV's weights), f64 [rows][n], and |w| + 8 |scale| (its f32 error scale)."""
-        sc, q = self._parts(e)
-        s = sc.double().repeat_interleave(32, dim=1)
-        return s * q, s.abs() * (q.abs() + 8)
+        """Matrix e dequantised exactly (q40_exact)."""
+        return q40_exact(self._raw(e), self.rows, self.n)
 
     def w_tc(self, e=0):
         """Matrix e as the tensor-core dequant builds it."""
-        return w_tc_of(*self._parts(e))
+        return q40_tc(self._raw(e), self.rows, self.n)
 
 
 # ---- comparisons ---------------------------------------------------------------------------------------------------------
@@ -170,7 +181,9 @@ def dequant(raw):
 
 class Ref:
     """The model file's q40 matrices as raw file rows on the device, in the engine's row order (q|k|v rows concatenated, q and k rows
-    in adjacent-pair RoPE order for NeoX models, w1/w3 rows interleaved); `gemv` dequantises them chunk by chunk."""
+    in adjacent-pair RoPE order for NeoX models, w1/w3 rows interleaved); `gemv` dequantises them chunk by chunk. Mixture-of-experts
+    files: the f32 router gate ("moe_gate", [E][dim]) and every expert's w13 / w2 stacked on a leading expert index, dequantised per
+    expert on demand by expert_exact and expert_tc."""
 
     def __init__(self, path):
         from distributed_llama_b200 import host
@@ -189,14 +202,25 @@ class Ref:
         def vec(name, l=0):
             return torch.from_numpy(np.array(mf.tensor_f32(mf.entry(name, l)))).cuda().double()
 
+        self.n_experts, self.k = h.n_experts, h.n_active_experts
         self.layers = []
         for l in range(h.n_layers):
             q, k, v = (self._q40(n, l) for n in ("block_matmul_q", "block_matmul_k", "block_matmul_v"))
-            w1, w3 = self._q40("block_matmul_w1", l), self._q40("block_matmul_w3", l)
             L = dict(qkv=torch.cat([heads(q, self.nh), heads(k, self.nkv), v]), wo=self._q40("block_matmul_wo", l),
-                     w13=torch.stack([w1, w3], 1).reshape(2 * self.ff, self.dim // 32, 18), w2=self._q40("block_matmul_w2", l),
                      norm0=vec("block_norm_0", l), norm1=vec("block_norm_1", l), q_norm=None, k_norm=None)
-            del q, k, v, w1, w3
+            if self.n_experts:
+                # per expert, as the engine holds them: w13 [E][2 ff][dim / 32][18] (gate / up rows interleaved), w2 [E][dim][ff / 32][18]
+                L["moe_gate"] = torch.from_numpy(np.array(mf.tensor_f32(mf.entry("block_moe_gate", l)))).cuda().double().view(
+                    self.n_experts, self.dim)
+                L["w13"] = torch.stack([torch.stack([self._q40("block_matmul_w1", l, e), self._q40("block_matmul_w3", l, e)], 1)
+                                        .reshape(2 * self.ff, self.dim // 32, 18) for e in range(self.n_experts)])
+                L["w2"] = torch.stack([self._q40("block_matmul_w2", l, e) for e in range(self.n_experts)])
+            else:
+                w1, w3 = self._q40("block_matmul_w1", l), self._q40("block_matmul_w3", l)
+                L["w13"] = torch.stack([w1, w3], 1).reshape(2 * self.ff, self.dim // 32, 18)
+                L["w2"] = self._q40("block_matmul_w2", l)
+                del w1, w3
+            del q, k, v
             if h.qk_norm:
                 L["q_norm"], L["k_norm"] = vec("block_norm_q", l), vec("block_norm_k", l)
                 if perm is not None:
@@ -206,9 +230,19 @@ class Ref:
         self.wcls = self._q40("final_matmul_logits")
         self.rope = torch.from_numpy(np.asarray(host().build_rope_table(h, h.seq_len))).cuda().double()   # [seq, hd/2, (cos, sin)]
 
-    def _q40(self, name, l=0):
-        e = self.mf.entry(name, l)
+    def _q40(self, name, l=0, expert=0):
+        e = self.mf.entry(name, l, expert)
         return torch.from_numpy(np.array(self.mf.raw(e))).cuda().view(e.d, e.n // 32, 18)
+
+    def expert_exact(self, l, name, e):
+        """MoE file: expert e's "w13" or "w2" of layer l dequantised exactly (q40_exact)."""
+        raw = self.layers[l][name][e]
+        return q40_exact(raw.reshape(-1, 18), raw.shape[0], raw.shape[1] * 32)
+
+    def expert_tc(self, l, name, e):
+        """MoE file: expert e's "w13" or "w2" of layer l as the tensor-core dequant builds it (q40_tc), bf16 [rows][n] (exact)."""
+        raw = self.layers[l][name][e]
+        return q40_tc(raw.reshape(-1, 18), raw.shape[0], raw.shape[1] * 32).bfloat16()
 
     def embedding(self, tok):
         e = self.mf.entry("embedding")

@@ -308,6 +308,28 @@ def _run_chunk(eng, toks, p, want):
 def check_tc_chunk(M, eng, st, toks, p, I1, I, logits, tag, tc_attn=True, second=False):
     """Stage checks of a tensor-core chunk of T = len(toks) tokens at p from its scratch (I1: the run with W2 zeroed)."""
     R, L, W = M["ref"], M["ref"].layers[0], M["tc"]
+    x1k = check_tc_attn(M, eng, st, toks, p, I1, I, tag, tc_attn, second)
+    # post-attention rmsnorm, bracketed
+    lo, hi = bf16_bracket_rel(rms(x1k, L["norm1"], R.eps), REL_NORM)
+    st.r(f"{tag} rmsnorm1 (bracket)", bracket_ratio(I["xn"], lo, hi))
+    # W1|W3 + SwiGLU, bracketed to bf16
+    gu, S, _ = tc_mm(W(0, "w13"), I["xn"])
+    h, e = swiglu_ref(gu, c_acc(W(0, "w13")) * S)
+    lo, hi = f64_to_bf16(h - e), f64_to_bf16(h + e)
+    st.r(f"{tag} w13+swiglu (bracket)", bracket_ratio(I["h"], lo, hi))
+    # W2 residual
+    x2k = I["x"].double()
+    y, S, _ = tc_mm(W(0, "w2"), I["h"])
+    x2 = x1k + y
+    b = c_acc(W(0, "w2")) * S + C_SUM * (S + x1k.abs() + x2.abs())
+    st.r(f"{tag} w2+residual", ratio(x2k, x2, b))
+    check_logits(M, st, logits, x2k, tag)
+
+
+def check_tc_attn(M, eng, st, toks, p, I1, I, tag, tc_attn=True, second=False):
+    """The stages of a tensor-core chunk up to and including the WO residual: QKV, q after QK-norm and RoPE, the K/V rows,
+    attention and WO. I1: the run whose final residual is the WO residual x1; returns x1 as float64."""
+    R, L, W = M["ref"], M["ref"].layers[0], M["tc"]
     T, hd, nh, nkv, qd, kvd = len(toks), R.hd, R.nh, R.nkv, R.q_dim, R.kv_dim
     rows = R.rope[p:p + T]
     x0 = torch.stack([R.embedding(t) for t in toks])
@@ -359,21 +381,7 @@ def check_tc_chunk(M, eng, st, toks, p, I1, I, logits, tag, tc_attn=True, second
     if T >= 2:
         xbad = x0[1:] + y[:-1]
         st.c("WO residual from token t+1", float(((x1k[:-1] - xbad).abs() / b[:-1]).amax(1).median()))
-    # post-attention rmsnorm, bracketed
-    lo, hi = bf16_bracket_rel(rms(x1k, L["norm1"], R.eps), REL_NORM)
-    st.r(f"{tag} rmsnorm1 (bracket)", bracket_ratio(I["xn"], lo, hi))
-    # W1|W3 + SwiGLU, bracketed to bf16
-    gu, S, _ = tc_mm(W(0, "w13"), I["xn"])
-    h, e = swiglu_ref(gu, c_acc(W(0, "w13")) * S)
-    lo, hi = f64_to_bf16(h - e), f64_to_bf16(h + e)
-    st.r(f"{tag} w13+swiglu (bracket)", bracket_ratio(I["h"], lo, hi))
-    # W2 residual
-    x2k = I["x"].double()
-    y, S, _ = tc_mm(W(0, "w2"), I["h"])
-    x2 = x1k + y
-    b = c_acc(W(0, "w2")) * S + C_SUM * (S + x1k.abs() + x2.abs())
-    st.r(f"{tag} w2+residual", ratio(x2k, x2, b))
-    check_logits(M, st, logits, x2k, tag)
+    return x1k
 
 
 def check_logits(M, st, logits, xk, tag):
@@ -389,35 +397,8 @@ def check_logits(M, st, logits, xk, tag):
 def check_gemv_batch(M, eng, st, toks, p, I, x1k, x2k, logits, tag):
     """Stage checks of a GEMV batch of nb = len(toks) tokens at p (q is rotated in place for nb >= 2, raw for nb = 1)."""
     R, L = M["ref"], M["ref"].layers[0]
-    nb, hd, nh, qd, kvd = len(toks), R.hd, R.nh, R.q_dim, R.kv_dim
-    Kc, Vc = attn_operands(eng, False)
-    ident = torch.stack([torch.ones(hd // 2), torch.zeros(hd // 2)], -1).double().cuda()
     for i, tok in enumerate(toks):
-        pos = p + i
-        x0 = R.embedding(tok)
-        act = q80(rms(x0, L["norm0"], R.eps), normed=True)
-        qkv = I["qkv"][i].double()
-        ykv, bkv = gemv(L["qkv"][qd:], act, got=qkv[qd:])
-        st.r(f"{tag} qkv k|v", ratio(qkv[qd:], ykv, bkv))
-        if nb == 1:
-            yq, bq = gemv(L["qkv"][:qd], act, got=qkv[:qd])
-            st.r(f"{tag} q", ratio(qkv[:qd], yq, bq))
-        else:
-            yq, bq = gemv(L["qkv"][:qd], act)
-            q_ref, q_b = norm_rope(yq.view(1, nh, hd), bq.view(1, nh, hd), L["q_norm"], R.rope[pos:pos + 1], R.eps)
-            st.r(f"{tag} q (norm+rope)", ratio(qkv[:qd].view(1, nh, hd), q_ref, q_b))
-        k, v = kv_rows(R, L, qkv, R.rope[pos])
-        kn = qkv[qd:qd + kvd].view(R.nkv, hd)
-        check_kv_rows(eng, st, tag, pos, k[None], (kn if L["k_norm"] is None else rms(kn, L["k_norm"], R.eps))[None], v[None])
-        zk = I["z"][i].double()
-        if nb == 1:
-            z, b = attention(qkv[:qd], Kc, Vc, pos + 1, L["q_norm"], R.rope[pos], nh, R.eps, eng.n_splits)
-        else:
-            z, b = attention(qkv[:qd], Kc, Vc, pos + 1, None, ident, nh, R.eps, eng.n_splits)
-        st.r(f"{tag} attention", ratio(zk, z, b))
-        y, b = gemv(L["wo"], q80(zk), got=x1k[i] - x0)
-        x1 = x0 + y
-        st.r(f"{tag} wo+residual", ratio(x1k[i], x1, b + U * x1.abs()))
+        check_gemv_attn(M, eng, st, tok, p + i, len(toks), I["qkv"][i], I["z"][i], x1k[i], tag)
         y13, b13 = gemv(L["w13"], q80(rms(x1k[i], L["norm1"], R.eps), normed=True))
         g, u = y13[0::2], y13[1::2]
         sg = torch.sigmoid(g)
@@ -428,6 +409,39 @@ def check_gemv_batch(M, eng, st, toks, p, I, x1k, x2k, logits, tag):
         x2 = x1k[i] + y2
         st.r(f"{tag} w2+residual", ratio(x2k[i], x2, b2 + U * x2.abs()))
     check_logits(M, st, logits, x2k, tag)
+
+
+def check_gemv_attn(M, eng, st, tok, pos, nb, qkv, zk, x1k, tag):
+    """The stages of token `tok` at `pos` in a GEMV batch of nb up to and including the WO residual x1k (f64 [dim]): QKV, q
+    (raw for nb = 1, after QK-norm and RoPE for nb >= 2), the K/V rows, attention and WO; qkv, zk: its rows of the scratch."""
+    R, L = M["ref"], M["ref"].layers[0]
+    hd, nh, qd, kvd = R.hd, R.nh, R.q_dim, R.kv_dim
+    Kc, Vc = attn_operands(eng, False)
+    ident = torch.stack([torch.ones(hd // 2), torch.zeros(hd // 2)], -1).double().cuda()
+    x0 = R.embedding(tok)
+    act = q80(rms(x0, L["norm0"], R.eps), normed=True)
+    qkv = qkv.double()
+    ykv, bkv = gemv(L["qkv"][qd:], act, got=qkv[qd:])
+    st.r(f"{tag} qkv k|v", ratio(qkv[qd:], ykv, bkv))
+    if nb == 1:
+        yq, bq = gemv(L["qkv"][:qd], act, got=qkv[:qd])
+        st.r(f"{tag} q", ratio(qkv[:qd], yq, bq))
+    else:
+        yq, bq = gemv(L["qkv"][:qd], act)
+        q_ref, q_b = norm_rope(yq.view(1, nh, hd), bq.view(1, nh, hd), L["q_norm"], R.rope[pos:pos + 1], R.eps)
+        st.r(f"{tag} q (norm+rope)", ratio(qkv[:qd].view(1, nh, hd), q_ref, q_b))
+    k, v = kv_rows(R, L, qkv, R.rope[pos])
+    kn = qkv[qd:qd + kvd].view(R.nkv, hd)
+    check_kv_rows(eng, st, tag, pos, k[None], (kn if L["k_norm"] is None else rms(kn, L["k_norm"], R.eps))[None], v[None])
+    zk = zk.double()
+    if nb == 1:
+        z, b = attention(qkv[:qd], Kc, Vc, pos + 1, L["q_norm"], R.rope[pos], nh, R.eps, eng.n_splits)
+    else:
+        z, b = attention(qkv[:qd], Kc, Vc, pos + 1, None, ident, nh, R.eps, eng.n_splits)
+    st.r(f"{tag} attention", ratio(zk, z, b))
+    y, b = gemv(L["wo"], q80(zk), got=x1k - x0)
+    x1 = x0 + y
+    st.r(f"{tag} wo+residual", ratio(x1k, x1, b + U * x1.abs()))
 
 
 def run_prompt(M, eng, st, n, p0, caches, tag, tc_attn=True):
