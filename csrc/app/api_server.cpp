@@ -1,4 +1,5 @@
 #include "api_server.hpp"
+#include "../host/slot_scheduler.hpp"
 
 #include <arpa/inet.h>
 #include <netinet/in.h>
@@ -9,7 +10,6 @@
 #include <algorithm>
 #include <cctype>
 #include <condition_variable>
-#include <deque>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -19,6 +19,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <ctime>
+#include <optional>
 #include <stdexcept>
 
 namespace dl {
@@ -601,12 +602,10 @@ private:
     std::vector<std::string> pending_, buffers_;
 };
 
-// A prompt resolved against a NaiveCache: the tokens to prefill from `start`, the last prompt token at P, the prompt's token count
+// A prompt resolved against a NaiveCache (the tokens to prefill from `start`, the last prompt token at P), the prompt's token count
 // and its public part.
-struct Prompt {
-    std::vector<int32_t> prefill;
-    uint32_t start = 0, P = 0, nPrompt = 0;
-    int32_t token = 0;
+struct Prompt : SlotPrompt {
+    uint32_t nPrompt = 0;
     std::string publicPrompt;
 };
 
@@ -697,45 +696,111 @@ void ApiServer::models(HttpRequest &req) const {
     req.writeJson("{\"object\": \"list\", \"data\": [{\"id\": " + jsonEscape(cfg_.modelName) + ", \"object\": \"model\", \"created\": 0, \"owned_by\": \"user\"}]}");
 }
 
-// ---- concurrent requests (--parallel): the rules of distributed_llama_b200.api.SlotScheduler --------------------------------
+// ---- concurrent requests (--parallel): SlotScheduler (csrc/host/slot_scheduler.hpp) over SlotJobs ------------------------------
 
 namespace {
-// One validated chat completion and, once admitted, its slots and progress.
+// What the slots' requests share: the slots' prompt caches, the prompt tools and the connection count's close.
+struct SlotServer {
+    const ChatTemplateGenerator &gen;
+    const Tokenizer &tok;
+    std::vector<NaiveCache> caches;
+    uint32_t slotLen;
+    std::function<void(int)> close;   // closes a connection and counts it finished
+};
+
+// One validated chat completion: SlotScheduler's request, answered on its connection.
 struct SlotJob {
+    SlotServer &srv;
     HttpRequest req;
     ChatRequest chat;
     ChatResponse resp;
-    std::vector<uint32_t> slots;
-    uint32_t P = 0, nPrompt = 0, limit = 0, live = 0;
-    std::vector<std::vector<int32_t>> out;
+    uint32_t nPrompt = 0;
     std::map<std::pair<uint32_t, size_t>, uint32_t> promptLens;   // paged: P by (slot, cached messages), computed once
-    SlotJob(HttpRequest r, ChatRequest c, const Tokenizer &tok, const std::vector<std::string> &stops)
-        : req(std::move(r)), chat(std::move(c)), resp(req, chat, tok, stops) {}
+    SlotJob(SlotServer &s, HttpRequest r, ChatRequest c, const std::vector<std::string> &stops)
+        : srv(s), req(std::move(r)), chat(std::move(c)), resp(req, chat, s.tok, stops) {}
+
+    uint32_t n() const { return chat.n; }
+    bool greedy() const { return chat.temperature == 0.f; }
+    std::optional<uint64_t> seed() const { return chat.hasSeed ? std::optional<uint64_t>(chat.seed) : std::nullopt; }
+    int64_t maxTokens() const { return chat.maxTokens; }
+    int logprobs() const { return chat.logprobs; }
+    size_t cachedPrefix(uint32_t slot) const { return srv.caches[slot].coveredPrefix(chat.messages); }
+    uint32_t promptLen(uint32_t slot) {
+        const auto key = std::make_pair(slot, cachedPrefix(slot));
+        if (!promptLens.count(key)) { NaiveCache probe = srv.caches[slot]; promptLens[key] = preparePrompt(srv.gen, srv.tok, probe, chat.messages, srv.slotLen).P; }
+        return promptLens[key];
+    }
+    SlotPrompt prepare(uint32_t slot) {
+        const Prompt p = preparePrompt(srv.gen, srv.tok, srv.caches[slot], chat.messages, srv.slotLen);
+        nPrompt = p.nPrompt;
+        resp.start(p.publicPrompt);
+        return p;
+    }
+    void onLogprobs(uint32_t i, const TokenLogprobs &e) { resp.onLogprobs(i, e); }
+    bool onToken(uint32_t i, int32_t t) { return resp.onToken(i, t); }
+    void finish(const std::vector<std::vector<int32_t>> &out, const std::vector<uint32_t> &slots, uint32_t P) {
+        NaiveCache &cache = srv.caches[slots[0]];
+        if (chat.n == 1 && !resp.stopped(0)) rememberAnswer(cache, P, out[0].size(), resp.text(0), srv.slotLen);
+        for (size_t k = 1; k < slots.size(); k++) srv.caches[slots[k]].copyFrom(cache);   // they hold a copy of the prompt rows
+        resp.finish(out, nPrompt);
+        std::printf("🔶 slot %u%s\n", slots[0], chat.n > 1 ? (" (" + std::to_string(chat.n) + " choices)").c_str() : "");
+        std::fflush(stdout);
+        srv.close(req.fd);
+    }
+    void fail(std::exception_ptr error, const std::vector<uint32_t> &slots) {
+        for (uint32_t s : slots) srv.caches[s].clear();   // their rows may not match what their caches say
+        try {
+            std::rethrow_exception(error);
+        } catch (const std::exception &e) {
+            std::printf("Socket error: %s\n", e.what());
+        } catch (...) {
+            std::printf("Socket error: unknown error\n");
+        }
+        std::fflush(stdout);
+        srv.close(req.fd);
+    }
 };
 
-struct SlotRow {
-    std::shared_ptr<SlotJob> job;
-    int32_t token = 0, pos = 0;
-    std::vector<uint32_t> choices;   // completions this row serves (all n for a greedy request)
-    std::vector<bool> done;
-    uint32_t nDone = 0;
+// InferenceBackend's slot calls as SlotScheduler makes them.
+struct SlotBackend {
+    using Request = std::shared_ptr<SlotJob>;
+    using Entry = TokenLogprobs;
+    InferenceBackend &be;
+    uint32_t slots() const { return be.slots(); }
+    uint32_t slotLen() const { return be.slotLen(); }
+    bool paged() const { return be.paged(); }
+    void slotPrefill(uint32_t slot, const std::vector<int32_t> &tokens, uint32_t pos) { be.slotPrefill(slot, tokens, pos); }
+    void slotCopy(uint32_t src, uint32_t dst, uint32_t P) { be.slotCopy(src, dst, P); }
+    void slotSampling(uint32_t slot, uint64_t seed, const Request &r) {
+        const ChatRequest &c = r->chat;
+        be.slotSampling(slot, seed, c.temperature, c.topp, c.presence, c.frequency, c.bias);
+        if (c.topK || c.minP > 0.f) be.slotFilters(slot, c.topK, c.minP);
+    }
+    void slotLogprobs(uint32_t slot, int k) { be.slotLogprobs(slot, k); }
+    std::vector<int32_t> slotsStep(const std::vector<int32_t> &t, const std::vector<int32_t> &pos, uint32_t active) { return be.slotsStep(t, pos, active); }
+    std::vector<int32_t> slotsStepLogprobs(const std::vector<int32_t> &t, const std::vector<int32_t> &pos, uint32_t active, std::vector<Entry> &e) {
+        return be.slotsStepLogprobs(t, pos, active, e);
+    }
+    bool slotReserve(uint32_t slot, uint32_t rows) { return be.slotReserve(slot, rows); }
+    void slotTrim(uint32_t slot, uint32_t rows) { be.slotTrim(slot, rows); }
+    void slotRelease(uint32_t slot) { be.slotRelease(slot); }
+    uint32_t freePages() const { return be.freePages(); }
+    uint32_t slotPageCount(uint32_t slot) const { return be.slotPageCount(slot); }
+    template <class F> void asleep(const F &ready) const { while (!ready()) {} }
 };
 }  // namespace
 
 void ApiServer::serveParallel(int srv) {
-    const uint32_t N = cfg_.parallel, L = backend_.slotLen();
-    std::vector<NaiveCache> caches(N);
     std::mutex mu;
     std::condition_variable cv;
-    std::deque<std::shared_ptr<SlotJob>> queue;
-    int open = 0;           // connections accepted and not yet finished
-    bool accepting = true;
-    const auto closeConn = [&](int fd) {
+    int open = 0;   // connections accepted and not yet finished
+    SlotServer slots{gen_, tok_, std::vector<NaiveCache>(cfg_.parallel), backend_.slotLen(), [&](int fd) {
         ::close(fd);
         std::lock_guard<std::mutex> lk(mu);
         open--;
         cv.notify_all();
-    };
+    }};
+    SlotScheduler<SlotBackend> sched(SlotBackend{backend_}, [this] { return sampler_.nextSeed(); }, [&](uint32_t s) { slots.caches[s].clear(); });
     // Reads and validates one connection; chat completions go to the engine thread, which closes them when they end.
     const auto handle = [&](int fd) {
         try {
@@ -743,11 +808,8 @@ void ApiServer::serveParallel(int srv) {
             std::printf("🔷 %s %s\n", req.method.c_str(), req.path.c_str());
             std::fflush(stdout);
             if (req.method == "POST" && req.path == "/v1/chat/completions") {
-                ChatRequest chat = parseChat(req.json, cfg_, sampler_.vocabSize(), N);   // --parallel > 1 runs on one GPU
-                auto job = std::make_shared<SlotJob>(std::move(req), std::move(chat), tok_, stops_);
-                std::lock_guard<std::mutex> lk(mu);
-                queue.push_back(job);
-                cv.notify_all();
+                ChatRequest chat = parseChat(req.json, cfg_, sampler_.vocabSize(), cfg_.parallel);   // --parallel > 1 runs on one GPU
+                sched.submit(std::make_shared<SlotJob>(slots, std::move(req), std::move(chat), stops_));
                 return;
             }
             if (req.method == "OPTIONS") req.writeCors();
@@ -757,8 +819,9 @@ void ApiServer::serveParallel(int srv) {
             std::printf("Socket error: %s\n", e.what());
             std::fflush(stdout);
         }
-        closeConn(fd);
+        slots.close(fd);
     };
+    // Once it has served maxRequests connections and every one is finished, the engine thread stops.
     std::thread acceptor([&] {
         int one = 1, served = 0;
         while (cfg_.maxRequests == 0 || served < cfg_.maxRequests) {
@@ -769,194 +832,13 @@ void ApiServer::serveParallel(int srv) {
             std::thread(handle, fd).detach();
             served++;
         }
-        std::lock_guard<std::mutex> lk(mu);
-        accepting = false;
-        cv.notify_all();
-    });
-
-    std::vector<std::shared_ptr<SlotJob>> owner(N);
-    std::vector<SlotRow> rows(N);
-    // paged slots: when each slot's cache was last left idle (eviction order)
-    const bool paged = backend_.paged();
-    constexpr uint32_t kPage = 64;
-    std::vector<uint64_t> finished(N, 0);
-    uint64_t clock = 0;
-    const auto release = [&](const std::shared_ptr<SlotJob> &job) {
-        for (uint32_t s : job->slots)
-            if (owner[s] == job) { owner[s].reset(); rows[s] = SlotRow(); finished[s] = ++clock; }
-    };
-    // Evicts idle caches, least recently finished first and none of `keep`, until `pages` pages are free; false (nothing evicted) if
-    // even all of them would not do.
-    const auto evictFor = [&](uint32_t pages, const std::vector<uint32_t> &keep) {
-        std::vector<uint32_t> idle;
-        uint32_t avail = backend_.freePages();
-        for (uint32_t s = 0; s < N; s++)
-            if (!owner[s] && std::find(keep.begin(), keep.end(), s) == keep.end() && backend_.slotPageCount(s) > 0) {
-                idle.push_back(s);
-                avail += backend_.slotPageCount(s);
-            }
-        if (avail < pages) return false;
-        std::stable_sort(idle.begin(), idle.end(), [&](uint32_t a, uint32_t b) { return finished[a] < finished[b]; });
-        for (uint32_t s : idle) {
-            if (backend_.freePages() >= pages) break;
-            backend_.slotRelease(s);
-            caches[s].clear();
-        }
-        return true;
-    };
-    const auto fail = [&](const std::shared_ptr<SlotJob> &job, const std::exception &e) {
-        for (uint32_t s : job->slots) caches[s].clear();   // their rows may not match what their caches say
-        if (paged) for (uint32_t s : job->slots) backend_.slotRelease(s);
-        std::printf("Socket error: %s\n", e.what());
-        std::fflush(stdout);
-        closeConn(job->req.fd);
-    };
-    const auto finish = [&](const std::shared_ptr<SlotJob> &job) {
-        SlotJob &j = *job;
-        NaiveCache &cache = caches[j.slots[0]];
-        if (j.chat.n == 1 && !j.resp.stopped(0)) rememberAnswer(cache, j.P, j.out[0].size(), j.resp.text(0), L);
-        for (size_t k = 1; k < j.slots.size(); k++) caches[j.slots[k]].copyFrom(cache);   // they hold a copy of the prompt rows
-        j.resp.finish(j.out, j.nPrompt);
-        std::printf("🔶 slot %u%s\n", j.slots[0], j.chat.n > 1 ? (" (" + std::to_string(j.chat.n) + " choices)").c_str() : "");
-        std::fflush(stdout);
-        closeConn(j.req.fd);
-    };
-    // Admission: the free slot whose cache covers most of the messages (lowest index on ties), then the lowest other free slots.
-    const auto admit = [&](const std::shared_ptr<SlotJob> &job, const std::vector<uint32_t> &free, uint32_t need) {
-        SlotJob &j = *job;
-        const ChatRequest &c = j.chat;
-        uint32_t first = free[0];
-        size_t best = caches[first].coveredPrefix(c.messages);
-        for (uint32_t s : free) { const size_t n = caches[s].coveredPrefix(c.messages); if (n > best) { best = n; first = s; } }
-        j.slots = {first};
-        for (uint32_t s : free) if (s != first && j.slots.size() < need) j.slots.push_back(s);
-        if (paged) {
-            // every slot holds rows [0, P + 64) and no more; P as preparePrompt will find it, from a copy of the cache
-            const auto key = std::make_pair(first, caches[first].coveredPrefix(c.messages));
-            if (!j.promptLens.count(key)) { NaiveCache probe = caches[first]; j.promptLens[key] = preparePrompt(gen_, tok_, probe, c.messages, L).P; }
-            const uint32_t want = std::min(L, j.promptLens[key] + kPage), pages = (want + kPage - 1) / kPage;
-            if (pages * j.slots.size() > L / kPage)
-                throw std::runtime_error("the request needs " + std::to_string(pages * j.slots.size()) + " KV-cache pages, more than the pool's " +
-                                         std::to_string(L / kPage));
-            int64_t net = 0;   // free pages the admission takes once its slots give back what they hold beyond `want`
-            for (uint32_t s : j.slots) net += (int64_t)pages - (int64_t)backend_.slotPageCount(s);
-            if (!evictFor((uint32_t)std::max<int64_t>(0, net), j.slots)) return false;
-            for (uint32_t s : j.slots) backend_.slotTrim(s, want);
-            for (uint32_t s : j.slots) backend_.slotReserve(s, want);   // cannot fail: the pages are free
-        }
-        const Prompt p = preparePrompt(gen_, tok_, caches[first], c.messages, L);
-        j.P = p.P;
-        j.nPrompt = p.nPrompt;
-        j.out.assign(c.n, {});
-        j.resp.start(p.publicPrompt);
-        if (!p.prefill.empty()) backend_.slotPrefill(first, p.prefill, p.start);
-        for (size_t k = 1; k < j.slots.size(); k++) backend_.slotCopy(first, j.slots[k], j.P);
-        const uint64_t seed = c.hasSeed ? c.seed : (c.temperature != 0.f ? sampler_.nextSeed() : 0);
-        for (size_t k = 0; k < j.slots.size(); k++)
-        {
-            backend_.slotSampling(j.slots[k], c.n == 1 ? seed : choiceSeed(seed, (uint32_t)k), c.temperature, c.topp, c.presence, c.frequency, c.bias);
-            if (c.topK || c.minP > 0.f) backend_.slotFilters(j.slots[k], c.topK, c.minP);
-            if (c.logprobs >= 0) backend_.slotLogprobs(j.slots[k], c.logprobs);
-        }
-        j.limit = L - j.P;
-        if (c.maxTokens > 0) j.limit = std::min<uint32_t>(j.limit, (uint32_t)c.maxTokens);
-        if (j.limit == 0) { finish(job); return true; }
-        j.live = (uint32_t)j.slots.size();
-        for (size_t k = 0; k < j.slots.size(); k++) {
-            SlotRow &r = rows[j.slots[k]];
-            owner[j.slots[k]] = job;
-            r.job = job; r.token = p.token; r.pos = (int32_t)j.P; r.nDone = 0;
-            r.choices.clear();
-            if (need == 1) for (uint32_t i = 0; i < c.n; i++) r.choices.push_back(i);
-            else r.choices.push_back((uint32_t)k);
-            r.done.assign(r.choices.size(), false);
-        }
-        return true;
-    };
-    // Slot s's row has finished every completion it serves; the request finishes with its last row.
-    const auto rowDone = [&](uint32_t s) {
-        const std::shared_ptr<SlotJob> job = rows[s].job;
-        rows[s] = SlotRow();
-        if (--job->live == 0) {
-            release(job);
-            try { finish(job); } catch (const std::exception &e) { fail(job, e); }
-        }
-    };
-    // Paged: every row about to write a row past its pages reserves the next page (evicting idle caches); one that cannot ends.
-    const auto grow = [&] {
-        for (uint32_t s = 0; s < N; s++) {
-            SlotRow &r = rows[s];
-            if (!r.job) continue;
-            const uint32_t need = (uint32_t)r.pos + 1, have = backend_.slotPageCount(s);
-            const uint32_t shortPages = (need + kPage - 1) / kPage > have ? (need + kPage - 1) / kPage - have : 0;
-            if (shortPages == 0) continue;
-            std::vector<uint32_t> busy;
-            for (uint32_t t = 0; t < N; t++) if (rows[t].job) busy.push_back(t);
-            if (evictFor(shortPages, busy) && backend_.slotReserve(s, need)) continue;
-            for (size_t c = 0; c < r.choices.size(); c++) r.done[c] = true;
-            r.nDone = (uint32_t)r.choices.size();
-            rowDone(s);
-        }
-    };
-
-    std::deque<std::shared_ptr<SlotJob>> waiting;
-    while (true) {
-        bool busy = false;
-        for (const SlotRow &r : rows) busy = busy || r.job != nullptr;
         {
             std::unique_lock<std::mutex> lk(mu);
-            if (!busy && waiting.empty()) cv.wait(lk, [&] { return !queue.empty() || (!accepting && open == 0); });
-            while (!queue.empty()) { waiting.push_back(queue.front()); queue.pop_front(); }
-            if (!busy && waiting.empty() && !accepting && open == 0) break;
+            cv.wait(lk, [&] { return open == 0; });
         }
-        while (!waiting.empty()) {
-            std::vector<uint32_t> free;
-            for (uint32_t s = 0; s < N; s++) if (!owner[s]) free.push_back(s);
-            const std::shared_ptr<SlotJob> job = waiting.front();
-            const uint32_t need = job->chat.temperature == 0.f ? 1 : job->chat.n;
-            if (free.size() < need) break;
-            try {
-                if (!admit(job, free, need)) break;   // paged: its pages are not there yet; it and everything behind it wait
-                waiting.pop_front();
-            } catch (const std::exception &e) {
-                waiting.pop_front();
-                release(job);
-                fail(job, e);
-            }
-        }
-        if (paged) grow();
-        std::vector<int32_t> tokens(N, 0), pos(N, 0);
-        uint32_t active = 0;
-        for (uint32_t s = 0; s < N; s++)
-            if (rows[s].job) { tokens[s] = rows[s].token; pos[s] = rows[s].pos; active |= 1u << s; }
-        if (!active) continue;
-        bool wantLp = false;
-        for (uint32_t s = 0; s < N; s++) wantLp = wantLp || (rows[s].job && rows[s].job->chat.logprobs >= 0);
-        std::vector<TokenLogprobs> entries;
-        const std::vector<int32_t> drawn = wantLp ? backend_.slotsStepLogprobs(tokens, pos, active, entries) : backend_.slotsStep(tokens, pos, active);
-        for (uint32_t s = 0; s < N; s++) {
-            SlotRow &r = rows[s];
-            if (!r.job) continue;
-            const std::shared_ptr<SlotJob> job = r.job;
-            SlotJob &j = *job;
-            r.token = drawn[s];
-            r.pos++;
-            try {
-                for (size_t c = 0; c < r.choices.size(); c++) {
-                    if (r.done[c]) continue;
-                    const uint32_t i = r.choices[c];
-                    j.out[i].push_back(drawn[s]);
-                    if (j.chat.logprobs >= 0) j.resp.onLogprobs(i, entries.at(s));
-                    if (j.resp.onToken(i, drawn[s]) || j.out[i].size() >= j.limit) { r.done[c] = true; r.nDone++; }
-                }
-            } catch (const std::exception &e) {
-                release(job);
-                fail(job, e);
-                continue;
-            }
-            if (r.nDone == r.choices.size()) rowDone(s);
-        }
-    }
+        sched.stop();
+    });
+    sched.run();
     acceptor.join();
     ::close(srv);
 }

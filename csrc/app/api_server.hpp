@@ -171,7 +171,7 @@ public:
     void models(HttpRequest &req) const;
     void serve();          // accept loop (parallel > 1: serveParallel)
 private:
-    void serveParallel(int srv);   // one engine thread, a reader thread per connection; same rules as api.SlotScheduler
+    void serveParallel(int srv);   // one engine thread running SlotScheduler (host/slot_scheduler.hpp), a reader thread per connection
     InferenceBackend &backend_;
     Tokenizer &tok_;
     ApiConfig cfg_;

@@ -5,6 +5,7 @@
 
 #include "model_format.hpp"
 #include "quants.hpp"
+#include "slot_scheduler.hpp"
 #include "text.hpp"
 
 namespace py = pybind11;
@@ -14,6 +15,121 @@ using F32Array = py::array_t<float, py::array::c_style | py::array::forcecast>;
 using U8Array = py::array_t<uint8_t, py::array::c_style | py::array::forcecast>;
 
 static py::bytes asBytes(const std::string &s) { return py::bytes(s.data(), s.size()); }
+
+// SlotScheduler over Python objects (distributed_llama_b200.api.SlotScheduler). run() holds the GIL except while it sleeps, so
+// every hook and backend call below runs with it.
+namespace {
+// A Python int as the engine takes a seed: modulo 2^64.
+uint64_t seed64(const py::handle &v) {
+    const unsigned long long s = PyLong_AsUnsignedLongLongMask(v.ptr());
+    if (PyErr_Occurred()) throw py::error_already_set();
+    return s;
+}
+
+// A distributed_llama_b200.api.SlotRequest: its fields and hooks.
+struct PySlotRequest {
+    py::object o;
+    uint32_t n() const { return o.attr("n").cast<uint32_t>(); }
+    bool greedy() const { return o.attr("temperature").cast<double>() == 0.0; }
+    std::optional<uint64_t> seed() const {
+        const py::object s = o.attr("seed");
+        return s.is_none() ? std::nullopt : std::optional<uint64_t>(seed64(s));
+    }
+    int64_t maxTokens() const {   // past int64: no limit but the slot's
+        int over = 0;
+        const long long v = PyLong_AsLongLongAndOverflow(o.attr("max_tokens").ptr(), &over);
+        if (PyErr_Occurred()) throw py::error_already_set();
+        return over ? (over > 0 ? INT64_MAX : -1) : v;
+    }
+    int logprobs() const {
+        const py::object k = o.attr("logprobs");
+        return k.is_none() ? -1 : k.cast<int>();
+    }
+    size_t cachedPrefix(uint32_t slot) const { return o.attr("cached_prefix")(slot).cast<size_t>(); }
+    uint32_t promptLen(uint32_t slot) const { return o.attr("prompt_len")(slot).cast<uint32_t>(); }
+    SlotPrompt prepare(uint32_t slot) const {
+        const py::tuple t(o.attr("prepare")(slot));
+        return {t[0].cast<std::vector<int32_t>>(), t[1].cast<uint32_t>(), t[2].cast<int32_t>(), t[3].cast<uint32_t>()};
+    }
+    void onLogprobs(uint32_t i, const py::object &entry) const { o.attr("on_logprobs")(i, entry); }
+    bool onToken(uint32_t i, int32_t token) const { return py::bool_(o.attr("on_token")(i, token)).cast<bool>(); }
+    void finish(const std::vector<std::vector<int32_t>> &out, const std::vector<uint32_t> &slots, uint32_t P) const {
+        o.attr("finish")(out, slots, P);
+    }
+    // A hook's exception goes on as the same object; the scheduler's own refusals as ValueError.
+    void fail(std::exception_ptr error, const std::vector<uint32_t> &slots) const {
+        py::object e;
+        try {
+            std::rethrow_exception(error);
+        } catch (const py::error_already_set &x) {
+            if (!x.matches(PyExc_Exception)) throw;   // KeyboardInterrupt, SystemExit: out of run()
+            e = x.value();
+        } catch (const std::exception &x) {
+            e = py::reinterpret_borrow<py::object>(PyExc_ValueError)(x.what());
+        }
+        o.attr("fail")(e, slots);
+    }
+};
+
+// The slot calls of a Python backend (InferenceSession(parallel=N) or a stub).
+struct PySlotBackend {
+    using Request = std::shared_ptr<PySlotRequest>;
+    using Entry = py::object;
+    py::object b;
+    uint32_t slots() const { return b.attr("slots").cast<uint32_t>(); }
+    uint32_t slotLen() const { return b.attr("slot_len").cast<uint32_t>(); }
+    bool paged() const { return py::bool_(py::getattr(b, "paged", py::bool_(false))).cast<bool>(); }
+    void slotPrefill(uint32_t slot, const std::vector<int32_t> &tokens, uint32_t pos) { b.attr("slot_prefill")(slot, tokens, pos); }
+    void slotCopy(uint32_t src, uint32_t dst, uint32_t P) { b.attr("slot_copy")(src, dst, P); }
+    void slotSampling(uint32_t slot, uint64_t seed, const Request &r) {
+        const py::object &q = r->o;
+        const py::object topK = q.attr("top_k"), minP = q.attr("min_p"), f = b.attr("slot_sampling");
+        const auto args = py::make_tuple(slot, seed, q.attr("temperature"), q.attr("topp"), q.attr("presence"), q.attr("frequency"), q.attr("bias"));
+        if (py::bool_(topK).cast<bool>() || py::bool_(minP).cast<bool>()) f(*args, py::arg("top_k") = topK, py::arg("min_p") = minP);
+        else f(*args);
+    }
+    void slotLogprobs(uint32_t slot, int k) { b.attr("slot_logprobs")(slot, k); }
+    std::vector<int32_t> slotsStep(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t active) {
+        return b.attr("slots_step")(tokens, pos, activeList(active)).cast<std::vector<int32_t>>();
+    }
+    std::vector<int32_t> slotsStepLogprobs(const std::vector<int32_t> &tokens, const std::vector<int32_t> &pos, uint32_t active,
+                                           std::vector<py::object> &entries) {
+        const py::tuple r(b.attr("slots_step_logprobs")(tokens, pos, activeList(active)));
+        entries = r[1].cast<std::vector<py::object>>();
+        return r[0].cast<std::vector<int32_t>>();
+    }
+    bool slotReserve(uint32_t slot, uint32_t rows) { return py::bool_(b.attr("slot_reserve")(slot, rows)).cast<bool>(); }
+    void slotTrim(uint32_t slot, uint32_t rows) { b.attr("slot_trim")(slot, rows); }
+    void slotRelease(uint32_t slot) { b.attr("slot_release")(slot); }
+    uint32_t freePages() const { return b.attr("free_pages")().cast<uint32_t>(); }
+    uint32_t slotPageCount(uint32_t slot) const { return (uint32_t)py::len(b.attr("slot_pages")(slot)); }
+    // Waits without the GIL. On the main thread, which alone receives signals, a pending signal's handler runs between slices and
+    // its exception (KeyboardInterrupt) leaves run(). Another thread does not take the GIL back until a request comes, so that a
+    // daemon thread never asks for it while the interpreter shuts down.
+    template <class F> void asleep(const F &ready) const {
+        const py::module_ threading = py::module_::import("threading");
+        if (!threading.attr("current_thread")().is(threading.attr("main_thread")())) {
+            py::gil_scoped_release nogil;
+            while (!ready()) {}
+            return;
+        }
+        while (true) {
+            {
+                py::gil_scoped_release nogil;
+                if (ready()) return;
+            }
+            if (PyErr_CheckSignals() != 0) throw py::error_already_set();
+        }
+    }
+private:
+    std::vector<bool> activeList(uint32_t mask) const {
+        std::vector<bool> a(slots());
+        for (size_t i = 0; i < a.size(); i++) a[i] = (mask >> i) & 1u;
+        return a;
+    }
+};
+using PySlotScheduler = SlotScheduler<PySlotBackend>;
+}  // namespace
 
 PYBIND11_MODULE(_host, m) {
     m.doc() = "distributed_llama_b200 host library: .m/.t formats, q40/q80 codecs, TP slicers, tokenizer, sampler";
@@ -179,6 +295,16 @@ PYBIND11_MODULE(_host, m) {
         .def("decode", [](TokenDecoder &d, const Tokenizer &t, int32_t token) { return asBytes(t.decodeWith(d.pending, token)); })
         .def("reset", [](TokenDecoder &d) { d.pending.clear(); });
     m.def("choice_seed", &choiceSeed, py::arg("seed"), py::arg("index"));
+
+    py::class_<PySlotScheduler>(m, "SlotScheduler")
+        .def(py::init([](py::object backend, py::object seedSource, py::object onEvict) {
+            std::function<void(uint32_t)> evict;
+            if (!onEvict.is_none()) evict = [onEvict](uint32_t s) { onEvict(s); };
+            return new PySlotScheduler(PySlotBackend{std::move(backend)}, [seedSource] { return seed64(seedSource()); }, evict);
+        }), py::arg("backend"), py::arg("seed_source"), py::arg("on_evict") = py::none())
+        .def("submit", [](PySlotScheduler &s, py::object req) { s.submit(std::make_shared<PySlotRequest>(PySlotRequest{std::move(req)})); })
+        .def("stop", &PySlotScheduler::stop)
+        .def("run", &PySlotScheduler::run);
 
     py::class_<Rng>(m, "Rng")
         .def(py::init<uint64_t>())

@@ -10,8 +10,6 @@ src/app.cpp:232-304).
 from __future__ import annotations
 
 import os
-import queue
-import threading
 import time
 from dataclasses import dataclass
 from typing import Callable, List, Optional, Sequence
@@ -21,7 +19,7 @@ import torch
 
 from . import host
 from .formats.model_file import ModelFile
-from .ops.cuda_lib import PAGE_ROWS, SLOT_CACHE_LAYOUTS
+from .ops.cuda_lib import SLOT_CACHE_LAYOUTS
 from .parallel.control import (OP_CHOICES_FIRST, OP_CHOICES_SEED, OP_CHOICES_STEP, OP_CONTROLS, OP_DECODE_N, OP_FILTERS, OP_PREFILL,
                                OP_SEED, OP_STEP_GREEDY, OP_STEP_LOGITS, OP_STEP_SAMPLE, _active_mask, _f32_bits, _split_seed)
 
@@ -411,228 +409,31 @@ class SlotRequest:
 
 
 class SlotScheduler:
-    """Serves SlotRequests on the KV-cache slots of a backend: one engine thread owns the GPU and decodes every busy slot in one
-    batched step per token.
-
-    Between steps it admits waiting requests first-in, first-out into free slots: a request takes n slots (one when greedy:
-    every greedy completion is the same), the free slot whose prompt cache covers most of its messages first. It prefills the
-    request's delta prompt into that slot (the running rows wait for this prefill), copies the prompt rows into its other slots
-    and seeds each slot: completion i with choice_seed(seed, i) when n > 1, the seed itself when n = 1; a request without a seed
-    takes seed_source() in admission order. The prompt's last token then enters the next batched step. A completion stops at
-    end of sequence or after min(max_tokens, slot_len - P) tokens. If on_token raises (a client went away), the request ends
-    and frees its slots; the other requests continue.
-
-    Paged slots (backend.paged: the slots share the KV cache as one pool of 64-row pages): a request is admitted, still first in,
-    first out, only when every slot it takes can hold rows [0, P + 64) (P = prompt_len(slot), capped at slot_len); otherwise it
-    and everything behind it wait. Each slot it takes keeps exactly the pages of those rows: pages a previous occupant left beyond
-    them go back to the pool (the rows it reuses, [0, P), lie inside). A running row reserves its next page when its position reaches a page boundary. A finished slot
-    keeps its pages as its prompt cache; when an admission or a growing row needs pages, idle slots' caches are evicted whole, least
-    recently finished first (backend.slot_release, then on_evict(slot): the server forgets that slot's prompt cache). A row that
-    cannot get a page ends there, as if it had reached its length limit. A request that needs more pages than the pool holds fails.
+    """Serves SlotRequests on the KV-cache slots of a backend by the rules both API servers share (csrc/host/slot_scheduler.hpp):
+    run() is the engine loop until stop(); submit and stop may be called from any thread; on_evict(slot) follows the eviction of a
+    paged slot's idle cache. A hook's exception reaches the request's fail as it is, the scheduler's own refusals as ValueError.
 
     `backend` provides slots, slot_len, slot_prefill(slot, tokens, pos), slot_copy(src, dst, P),
     slot_sampling(slot, seed, temperature, topp, presence, frequency, bias, top_k=.., min_p=..) (the filters are passed only
-    when one is on) and slots_step(tokens, pos, active) (InferenceSession(parallel=N)); for requests with logprobs also slot_logprobs(slot, k) and slots_step_logprobs(tokens, pos,
-    active) -> (draws, per-slot entries), used only while such a request holds a slot."""
+    when one is on) and slots_step(tokens, pos, active) (InferenceSession(parallel=N)); for requests with logprobs also
+    slot_logprobs(slot, k) and slots_step_logprobs(tokens, pos, active) -> (draws, per-slot entries), used only while such a
+    request holds a slot. Paged backends (backend.paged true) also provide slot_reserve(slot, rows) -> bool,
+    slot_trim(slot, rows), slot_release(slot), free_pages() and slot_pages(slot)."""
 
     def __init__(self, backend, seed_source: Callable[[], int], on_evict: Optional[Callable[[int], None]] = None):
-        """Paged backends (backend.paged true) also provide slot_reserve(slot, rows) -> bool, slot_trim(slot, rows),
-        slot_release(slot), free_pages() and slot_pages(slot)."""
-        self.backend = backend
-        self.seed_source = seed_source
-        self.on_evict = on_evict
-        self.queue: "queue.Queue" = queue.Queue()
-        self.owner: List[Optional[object]] = [None] * backend.slots
-        self.paged = bool(getattr(backend, "paged", False))
-        self._finished = [0] * backend.slots   # paged: when each slot's cache was last left idle (eviction order)
-        self._clock = 0
-        self._stop = threading.Event()
+        self._core = host().SlotScheduler(backend, seed_source, on_evict)
 
     def submit(self, req: SlotRequest) -> None:
-        """Queues the request; one that needs more slots than there are is refused at once (fail with no slots)."""
-        if req.temperature != 0.0 and req.n > self.backend.slots:
-            req.fail(ValueError(f"n = {req.n} needs more than the {self.backend.slots} slots"), [])
-            return
-        self.queue.put(req)
+        """Queues the request; one for no completions or for more completions than there are slots fails at once (no slots)."""
+        self._core.submit(req)
 
     def stop(self) -> None:
-        self._stop.set()
-        self.queue.put(None)
-
-    # ---- paged slots: pages per slot, eviction ----
-    def _pages(self, slot: int) -> int:
-        return len(self.backend.slot_pages(slot))
-
-    def _evict_for(self, pages: int, keep) -> bool:
-        """Evicts idle caches, least recently finished first and none of `keep`, until `pages` pages are free. False (nothing
-        evicted) if even all of them would not do."""
-        be = self.backend
-        idle = sorted((s for s in range(be.slots) if self.owner[s] is None and s not in keep and self._pages(s) > 0),
-                      key=lambda s: self._finished[s])
-        if be.free_pages() + sum(self._pages(s) for s in idle) < pages:
-            return False
-        for s in idle:
-            if be.free_pages() >= pages:
-                break
-            be.slot_release(s)
-            if self.on_evict is not None:
-                self.on_evict(s)
-        return True
-
-    def _reserve(self, slot: int, rows: int, keep) -> bool:
-        """Grows `slot` to cover rows [0, rows), evicting idle caches if the pool is short."""
-        be = self.backend
-        short = -(-rows // PAGE_ROWS) - self._pages(slot)
-        if short <= 0:
-            return True
-        return self._evict_for(short, keep) and be.slot_reserve(slot, rows)
-
-    def _admit(self, req: SlotRequest, free: List[int], rows: List[dict]) -> bool:
-        """Starts `req` in free slots; False when paged slots cannot reserve its pages yet (nothing changed)."""
-        be = self.backend
-        rows_needed = 1 if req.temperature == 0.0 else req.n
-        first = max(free, key=lambda s: (req.cached_prefix(s), -s))
-        slots = [first] + [s for s in free if s != first][:rows_needed - 1]
-        try:
-            if self.paged:
-                want = min(be.slot_len, req.prompt_len(first) + PAGE_ROWS)
-                pages = -(-want // PAGE_ROWS)
-                if pages * len(slots) > be.slot_len // PAGE_ROWS:
-                    raise ValueError(f"the request needs {pages * len(slots)} KV-cache pages, more than the pool's {be.slot_len // PAGE_ROWS}")
-                # free pages the admission takes once its slots give back what they hold beyond `want`
-                if not self._evict_for(max(0, sum(pages - self._pages(s) for s in slots)), slots):
-                    return False
-                for s in slots:
-                    be.slot_trim(s, want)
-                for s in slots:
-                    be.slot_reserve(s, want)   # cannot fail: the pages are free
-            self._start(req, slots, rows, rows_needed)
-        except Exception as e:   # e.g. the client went away while its prompt was prepared
-            self._drop_pages(slots)
-            req.fail(e, slots)
-        return True
-
-    def _drop_pages(self, slots) -> None:
-        """Paged: slots whose rows no longer match a prompt cache give their pages back."""
-        if self.paged:
-            for s in slots:
-                self.backend.slot_release(s)
-
-    def _start(self, req: SlotRequest, slots: List[int], rows: List[dict], rows_needed: int) -> None:
-        be, first = self.backend, slots[0]
-        prefill, start, token, P = req.prepare(first)
-        if prefill:
-            be.slot_prefill(first, prefill, start)
-        for s in slots[1:]:
-            be.slot_copy(first, s, P)
-        seed = req.seed if req.seed is not None else (self.seed_source() if req.temperature != 0.0 else 0)
-        seeds = [seed] if req.n == 1 else [host().choice_seed(seed, i) for i in range(len(slots))]
-        for s, sd in zip(slots, seeds):
-            filters = {"top_k": req.top_k, "min_p": req.min_p} if (req.top_k or req.min_p) else {}
-            be.slot_sampling(s, sd, req.temperature, req.topp, req.presence, req.frequency, req.bias, **filters)
-            if req.logprobs is not None:
-                be.slot_logprobs(s, req.logprobs)
-        limit = be.slot_len - P
-        if req.max_tokens > 0:
-            limit = min(limit, req.max_tokens)
-        job = {"req": req, "slots": slots, "P": P, "out": [[] for _ in range(req.n)], "limit": limit, "live": len(slots)}
-        if limit <= 0:
-            req.finish(job["out"], slots, P)
-            return
-        for k, s in enumerate(slots):
-            self.owner[s] = job
-            # completion k of the request; a greedy request's only row serves all n completions
-            rows[s] = {"job": job, "k": k, "token": token, "pos": P,
-                       "choices": list(range(req.n)) if rows_needed == 1 else [k], "done": set()}
-
-    def _release(self, job, rows) -> None:
-        for s in job["slots"]:
-            if self.owner[s] is job:
-                self.owner[s] = None
-                rows[s] = None
-                self._clock += 1
-                self._finished[s] = self._clock
+        """run() returns before its next step."""
+        self._core.stop()
 
     def run(self) -> None:
-        """The engine loop; returns after stop()."""
-        be = self.backend
-        N = be.slots
-        rows: List[Optional[dict]] = [None] * N
-        waiting: List[SlotRequest] = []
-        while not self._stop.is_set():
-            busy = any(r is not None for r in rows)
-            try:
-                while True:
-                    item = self.queue.get(block=not busy and not waiting, timeout=None)
-                    if item is None:
-                        return
-                    waiting.append(item)
-            except queue.Empty:
-                pass
-            while waiting:
-                free = [s for s in range(N) if self.owner[s] is None]
-                need = 1 if waiting[0].temperature == 0.0 else waiting[0].n
-                if len(free) < need or not self._admit(waiting[0], free, rows):
-                    break
-                waiting.pop(0)
-            if self.paged:
-                self._grow(rows)
-            active = [r is not None for r in rows]
-            if not any(active):
-                continue
-            args = ([r["token"] if r else 0 for r in rows], [r["pos"] if r else 0 for r in rows], active)
-            entries = None
-            if any(r is not None and r["job"]["req"].logprobs is not None for r in rows):
-                drawn, entries = be.slots_step_logprobs(*args)
-            else:
-                drawn = be.slots_step(*args)
-            for s in range(N):
-                r = rows[s]
-                if r is None:
-                    continue
-                job, req = r["job"], r["job"]["req"]
-                tok = drawn[s]
-                r["token"], r["pos"] = tok, r["pos"] + 1
-                try:
-                    for i in r["choices"]:
-                        if i in r["done"]:
-                            continue
-                        job["out"][i].append(tok)
-                        if entries is not None and req.logprobs is not None:
-                            req.on_logprobs(i, entries[s])
-                        if req.on_token(i, tok) or len(job["out"][i]) >= job["limit"]:
-                            r["done"].add(i)
-                except Exception as e:
-                    self._release(job, rows)
-                    self._drop_pages(job["slots"])
-                    req.fail(e, job["slots"])
-                    continue
-                if len(r["done"]) == len(r["choices"]):
-                    self._row_done(s, rows)
-
-    def _row_done(self, s: int, rows: List[Optional[dict]]) -> None:
-        """Slot s's row has finished every completion it serves; the request finishes with its last row."""
-        job = rows[s]["job"]
-        req = job["req"]
-        rows[s] = None
-        job["live"] -= 1
-        if job["live"] == 0:
-            self._release(job, rows)
-            try:
-                req.finish(job["out"], job["slots"], job["P"])
-            except Exception as e:
-                self._drop_pages(job["slots"])
-                req.fail(e, job["slots"])
-
-    def _grow(self, rows: List[Optional[dict]]) -> None:
-        """Paged: every row about to write a row past its pages reserves the next page; one that cannot get a page ends."""
-        for s in range(len(rows)):
-            r = rows[s]
-            if r is None:
-                continue
-            if not self._reserve(s, r["pos"] + 1, {t for t, x in enumerate(rows) if x is not None}):
-                r["done"].update(r["choices"])
-                self._row_done(s, rows)
+        """The engine loop, until stop(). While idle it still raises what a signal handler raises (Ctrl-C: KeyboardInterrupt)."""
+        self._core.run()
 
 
 class InferenceSession(TokenSteps):

@@ -178,6 +178,67 @@ def test_request_larger_than_the_pool_fails():
     assert r.error is not None and "pages" in str(r.error)
 
 
+def test_hook_error_reaches_fail_as_the_same_object():
+    """An exception a request's hook raises reaches its fail as the same object and frees its pages, while the other request
+    finishes; the scheduler's own refusal of a request arrives as ValueError."""
+    stub, log, caches = PagedStub(3, 6), [], [None] * 3
+    gone = ConnectionError("the client went away")
+    a, b = Req(log, "a", _prompt(20, 1), 10, caches), Req(log, "b", _prompt(20, 2), 10, caches)
+    wide = Req(log, "wide", _prompt(20, 3), 5, caches, n=4, temperature=0.7)   # 4 completions, 3 slots
+    none = Req(log, "none", _prompt(20, 4), 5, caches, n=0)
+
+    def on_token(i, tok):
+        raise gone
+    a.on_token = on_token
+    _run(stub, caches, [[a, b, wide, none]])
+    assert a.error is gone and a.out is None
+    slot = [e for e in log if e[:2] == ("admit", "a")][0][2]
+    assert ("release", slot) in stub.log                       # a's slot gives its pages back
+    assert b.error is None and len(b.out[0]) == 10
+    assert type(wide.error) is ValueError and str(wide.error) == "n = 4 needs more than the 3 slots"
+    assert type(none.error) is ValueError and str(none.error) == "n must be at least 1"
+
+
+def test_seeds_are_taken_modulo_2_64():
+    """A request's seed reaches the slots as the engine takes it, modulo 2^64: itself for one completion, choice_seed of it for
+    several, so a negative seed serves n > 1 too."""
+    from distributed_llama_b200 import host
+
+    class SeedStub(PagedStub):
+        def slot_sampling(self, slot, seed, temperature, topp, presence, frequency, bias, **filters):
+            self.log.append(("seed", slot, seed))
+
+    stub, log, caches = SeedStub(3, 6), [], [None] * 3
+    one, two = Req(log, "one", _prompt(20, 1), 3, caches, temperature=0.7), Req(log, "two", _prompt(20, 2), 3, caches, n=2, temperature=0.7)
+    one.seed = two.seed = -5
+    _run(stub, caches, [[one], [two]])
+    assert one.error is None and two.error is None
+    seeds = [e[2] for e in stub.log if e[0] == "seed"]
+    assert seeds == [2**64 - 5] + [host().choice_seed(2**64 - 5, i) for i in range(2)]
+
+
+def test_idle_run_stops_on_sigint():
+    """run() on the main thread with nothing to do raises KeyboardInterrupt on Ctrl-C, without waiting for a request."""
+    import signal
+    import time
+    from distributed_llama_b200.api import SlotScheduler
+    sched = SlotScheduler(PagedStub(2, 4), lambda: 1)
+    old = signal.signal(signal.SIGINT, signal.default_int_handler)
+    interrupt = threading.Timer(0.3, lambda: os.kill(os.getpid(), signal.SIGINT))
+    watchdog = threading.Timer(10, sched.stop)   # a run() that misses the signal returns here, too late
+    try:
+        interrupt.start()
+        watchdog.start()
+        t0 = time.monotonic()
+        with pytest.raises(KeyboardInterrupt):
+            sched.run()
+        assert time.monotonic() - t0 < 5
+    finally:
+        interrupt.cancel()
+        watchdog.cancel()
+        signal.signal(signal.SIGINT, old)
+
+
 def test_pages_are_taken_lowest_first():
     stub = PagedStub(2, 6)
     assert stub.slot_reserve(0, 65) and stub.slot_reserve(1, 1)
