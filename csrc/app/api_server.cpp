@@ -370,14 +370,21 @@ std::vector<std::vector<int32_t>> runChoices(InferenceBackend &backend, int32_t 
         uint32_t pos = P;
         std::vector<bool> done(n, false);
         uint32_t nDone = 0;
+        // a single greedy completion with a draft model takes speculative rounds of several tokens (the same tokens)
+        const bool spec = n == 1 && !onLogprobs && backend.speculates(smp);
         while (out[first].size() < limit) {
-            tok = backend.next(tok, pos++, smp);
+            const std::vector<int32_t> toks = spec ? backend.specRound(tok, pos) : std::vector<int32_t>{backend.next(tok, pos, smp)};
             const TokenLogprobs entry = onLogprobs ? backend.lastLogprobs().at(0) : TokenLogprobs();
-            for (uint32_t i = first; i <= last; i++) {
-                if (done[i]) continue;
-                out[i].push_back(tok);
-                if (onLogprobs) onLogprobs(i, entry);
-                if (onToken(i, tok)) { done[i] = true; nDone++; }
+            for (const int32_t t : toks) {
+                tok = t;
+                pos++;
+                for (uint32_t i = first; i <= last; i++) {
+                    if (done[i]) continue;
+                    out[i].push_back(tok);
+                    if (onLogprobs) onLogprobs(i, entry);
+                    if (onToken(i, tok)) { done[i] = true; nDone++; }
+                }
+                if (nDone == last - first + 1 || out[first].size() >= limit) break;
             }
             if (nDone == last - first + 1) break;
         }

@@ -31,6 +31,10 @@ struct InferenceBackend {
     virtual void setVocabLimit(uint32_t) {}   // greedy decoding never returns ids >= limit (tokenizer vocabulary)
     virtual void prefill(const std::vector<int32_t> &tokens, uint32_t pos) = 0;
     virtual int32_t next(int32_t token, uint32_t pos, Sampler &sampler) = 0;   // greedy on the device when temperature == 0
+    // Greedy speculative decoding with a draft model (--draft-model): whether a single completion with the sampler's settings
+    // decodes in rounds (plain greedy only), and one round from the last emitted token at `pos`: the tokens greedy decoding emits next.
+    virtual bool speculates(const Sampler & /*sampler*/) const { return false; }
+    virtual std::vector<int32_t> specRound(int32_t /*token*/, uint32_t /*pos*/) { throw std::runtime_error("no draft model"); }
     // Several completions of one prompt (runChoices). Without a batched path the choices run one after another through next().
     virtual bool batchedChoices(uint32_t /*n*/) const { return false; }
     virtual void seedChoices(const std::vector<uint64_t> & /*seeds*/) {}

@@ -3,6 +3,7 @@
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
+#include <memory>
 #include <ctime>
 #include <stdexcept>
 #include <string>
@@ -25,9 +26,22 @@ struct EngineBackend : InferenceBackend {
     EngineBackend(NativeEngine &engine, TpJob &job) : e(engine), tp{engine, job} {}
     uint32_t seqLen() const override { return e.seqLen(); }
     uint32_t vocabSize() const override { return e.header().vocabSize; }
-    void setVocabLimit(uint32_t limit) override { e.setVocabLimit(limit); }
-    void prefill(const std::vector<int32_t> &tokens, uint32_t pos) override { if (!tokens.empty()) tp.prefill(tokens, pos); }
+    void setVocabLimit(uint32_t limit) override {
+        e.setVocabLimit(limit);
+        if (draft) draft->setVocabLimit(limit);
+    }
+    void prefill(const std::vector<int32_t> &tokens, uint32_t pos) override {
+        if (tokens.empty()) return;
+        tp.prefill(tokens, pos);
+        if (draft) draft->prefill(tokens, pos);   // the draft follows every prefill, prompt-cache continuations included
+    }
     int32_t next(int32_t token, uint32_t pos, Sampler &sampler) override { return tp.next(token, pos, sampler); }
+    // --draft-model (one GPU): greedy single completions decode in speculative rounds
+    NativeEngine *draft = nullptr;
+    uint32_t draftTokens = 3;
+    SpecStats specStats;
+    bool speculates(const Sampler &sampler) const override { return draft && sampler.temperature() == 0.f && !sampler.controlsActive(); }
+    std::vector<int32_t> specRound(int32_t token, uint32_t pos) override { return e.specRound(*draft, token, pos, draftTokens, specStats); }
     // choices: one batched step per token on dense models; the sequential fallback (MoE) keeps the device generator's stream
     bool batchedChoices(uint32_t n) const override { return e.supportsChoices(n); }
     void seedChoices(const std::vector<uint64_t> &seeds) override { tp.seedChoices(seeds); }
@@ -112,12 +126,14 @@ const char *kUsage =
     "        [--parallel <n>]  decode up to n (1..8) chat requests together, each in its own KV-cache slot of floor(context / n)\n"
     "                       tokens; one GPU and dense models only\n"
     "        [--parallel-cache {split|paged}]  paged: the slots share the KV cache as one pool of 64-token pages (default split)\n"
+    "        [--draft-model <path>] [--draft-tokens {1|3|7}]  greedy single completions decode in speculative rounds: the draft\n"
+    "                       (same tokenizer, dense q40) proposes k tokens (default 3), the model checks them in one forward\n"
     "        [--gpus <n>]   tensor parallel over n GPUs: a supervisor forks one process per GPU (rank 0 serves HTTP) and restarts\n"
     "                       the whole job 3 s after any rank fails\n";
 
 // One attempt of rank 0 of a job (or the only process on one GPU): engine + tokenizer + HTTP server until --max-requests is reached.
 int serveOnce(const std::string &model, const std::string &tokenizer, uint32_t maxSeqLen, int gpu, const ApiConfig &cfg, TpJob &job,
-              uint32_t kvType, const std::string &parallelCache) {
+              uint32_t kvType, const std::string &parallelCache, const std::string &draftModel, uint32_t draftTokens) {
     NativeEngine engine(model, maxSeqLen, gpu, 0, job.nRanks, job.tag, [&job] { job.barrier(); }, kvType);
     Tokenizer tok(tokenizer);
     if (job.nRanks > 1) job.barrier();   // every rank has its weights
@@ -129,6 +145,16 @@ int serveOnce(const std::string &model, const std::string &tokenizer, uint32_t m
     EngineBackend backend(engine, job);
     const std::string why = parallelRefusal(cfg.parallel, job.nRanks, engine.header().nExperts, parallelCache);
     if (!why.empty()) throw ParallelRefused(why);
+    std::unique_ptr<NativeEngine> draft;
+    if (!draftModel.empty()) {
+        // the draft gets the target's context length and KV-cache storage; refused in one line before its weights load
+        const ModelHeader dh = loadModelHeader(draftModel, engine.seqLen());
+        const std::string whyDraft = draftRefusal(draftTokens, job.nRanks, cfg.parallel, &engine.header(), &dh);
+        if (!whyDraft.empty()) throw ParallelRefused(whyDraft);
+        draft.reset(new NativeEngine(draftModel, engine.seqLen(), gpu, 0, 1, std::string(), std::function<void()>(), kvType));
+        backend.draft = draft.get();
+        backend.draftTokens = draftTokens;
+    }
     if (cfg.parallel > 1) {
         engine.setSlots(cfg.parallel, parallelCache == "paged");
         backend.slotCount = cfg.parallel;
@@ -148,7 +174,8 @@ int main(int argc, char **argv) {
     uint32_t maxSeqLen = 0, kvType = 0;
     int gpu = 0;
     uint32_t gpus = 1, workers = 0;
-    std::string parallelCache = "split";
+    std::string parallelCache = "split", draftModel;
+    uint32_t draftTokens = 3;
     try {
         for (int i = 1; i < argc;) {
             const std::string name = argv[i];
@@ -175,6 +202,8 @@ int main(int argc, char **argv) {
             else if (name == "--max-requests") cfg.maxRequests = std::stoi(v);
             else if (name == "--parallel") cfg.parallel = (uint32_t)std::max(0, std::stoi(v));
             else if (name == "--parallel-cache") parallelCache = v;
+            else if (name == "--draft-model") draftModel = v;
+            else if (name == "--draft-tokens") draftTokens = (uint32_t)std::max(0, std::stoi(v));
             else if (name == "--buffer-float-type" || name == "--nthreads" || name == "--net-turbo" || name == "--gpu-segments") {}
             else throw std::runtime_error("Unknown option: " + name);
             i += 2;
@@ -186,7 +215,8 @@ int main(int argc, char **argv) {
         return 1;
     }
     {
-        const std::string why = parallelRefusal(cfg.parallel, gpus + workers, 0, parallelCache);
+        std::string why = parallelRefusal(cfg.parallel, gpus + workers, 0, parallelCache);
+        if (why.empty() && !draftModel.empty()) why = draftRefusal(draftTokens, gpus + workers, cfg.parallel);
         if (!why.empty()) { std::fprintf(stderr, "%s\n", why.c_str()); return 1; }
     }
     const size_t slash = model.find_last_of("/\\");
@@ -196,7 +226,7 @@ int main(int argc, char **argv) {
         while (true) {
             try {
                 TpJob job;
-                return serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType, parallelCache);
+                return serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType, parallelCache, draftModel, draftTokens);
             } catch (const ParallelRefused &e) {
                 std::fprintf(stderr, "%s\n", e.what());
                 return 1;
@@ -227,7 +257,7 @@ int main(int argc, char **argv) {
                 int rc = 1;
                 if (r == 0) {
                     try {
-                        rc = serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType, parallelCache);
+                        rc = serveOnce(model, tokenizer, maxSeqLen, gpu, cfg, job, kvType, parallelCache, draftModel, draftTokens);
                         job.sendExit();
                     } catch (const std::exception &e) {
                         job.fail(e.what());

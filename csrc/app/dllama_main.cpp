@@ -49,7 +49,9 @@ struct Args {
     float minP = 0.f;
     uint64_t seed = (uint64_t)std::time(nullptr);
     int gpuIndex = 0;
-    uint32_t gpus = 1;
+    uint32_t gpus = 1, workers = 0;
+    std::string draftModel;   // --draft-model: greedy speculative decoding with this smaller model (one GPU)
+    uint32_t draftTokens = 3;
 };
 
 const char *kUsage =
@@ -59,6 +61,7 @@ const char *kUsage =
     "        [--seed <s>] [--max-seq-len <n>] [--kv-cache-float-type {bf16|q80}]\n"
     "        [--chat-template {llama2|llama3|deepSeek3|chatml}] [--buffer-float-type q80] [--gpu-index <i>]\n"
     "        [--gpus <n>]   tensor parallel over GPUs gpu-index .. gpu-index + n - 1 of this machine (one process per GPU)\n"
+    "        [--draft-model <path>] [--draft-tokens {1|3|7}]  greedy speculative decoding: the draft proposes k tokens a round (default 3)\n"
     "        (accepted for drop-in compatibility and ignored: --nthreads --net-turbo --gpu-segments --workers --host --port)\n";
 
 Args parse(int argc, char **argv) {
@@ -70,7 +73,7 @@ Args parse(int argc, char **argv) {
         if (name == "--help" || name == "-h" || name == "--usage") { a.help = true; return a; }
         if (name == "--workers") {   // variadic until the next flag
             i++;
-            while (i < argc && argv[i][0] != '-') i++;
+            while (i < argc && argv[i][0] != '-') { i++; a.workers++; }
             continue;
         }
         if (i + 1 >= argc) throw std::runtime_error("Missing value for " + name);
@@ -92,6 +95,8 @@ Args parse(int argc, char **argv) {
         else if (name == "--buffer-float-type") a.bufferFloatType = value;
         else if (name == "--gpu-index") a.gpuIndex = std::max(0, std::stoi(value));
         else if (name == "--gpus") a.gpus = (uint32_t)std::max(1, std::stoi(value));
+        else if (name == "--draft-model") a.draftModel = value;
+        else if (name == "--draft-tokens") a.draftTokens = (uint32_t)std::max(0, std::stoi(value));
         else if (name == "--nthreads" || name == "--net-turbo" || name == "--gpu-segments" || name == "--host" || name == "--port") {}
         else throw std::runtime_error("Unknown option: " + name);
         i += 2;
@@ -111,6 +116,8 @@ struct App {
     Tokenizer tokenizer;
     Sampler sampler;
     TpEngine tp;
+    std::unique_ptr<NativeEngine> draft;   // --draft-model: the target's context length and KV-cache storage
+    SpecStats specStats;
     App(const Args &a, TpJob &j)
         : args(a), job(j), engine(a.model, a.maxSeqLen, a.gpuIndex + (int)j.rank, j.rank, j.nRanks, j.tag, [&j] { j.barrier(); }, a.kvType),
           tokenizer(a.tokenizer),
@@ -119,11 +126,28 @@ struct App {
         engine.setVocabLimit(tokenizer.vocabSize());
         sampler.setControls(a.presencePenalty, a.frequencyPenalty, {});
         sampler.setFilters(a.topK, a.minP);
+        if (!a.draftModel.empty()) {
+            const ModelHeader dh = loadModelHeader(a.draftModel, engine.seqLen());
+            const std::string why = draftRefusal(a.draftTokens, j.nRanks, 1, &engine.header(), &dh);
+            if (!why.empty()) throw std::runtime_error(why);
+            draft.reset(new NativeEngine(a.draftModel, engine.seqLen(), a.gpuIndex, 0, 1, std::string(), std::function<void()>(), a.kvType));
+            draft->setVocabLimit(tokenizer.vocabSize());
+        }
     }
 
-    void prefill(const std::vector<int32_t> &tokens, uint32_t pos) { tp.prefill(tokens, pos); }
+    void prefill(const std::vector<int32_t> &tokens, uint32_t pos) {
+        tp.prefill(tokens, pos);
+        if (draft && !tokens.empty()) draft->prefill(tokens, pos);
+    }
 
     int32_t next(int32_t token, uint32_t pos) { return tp.next(token, pos, sampler); }
+
+    // the tokens of one step: a speculative round for plain greedy decoding with a draft, else one token
+    std::vector<int32_t> nextTokens(int32_t token, uint32_t pos) {
+        if (draft && sampler.temperature() == 0.f && !sampler.controlsActive())
+            return engine.specRound(*draft, token, pos, args.draftTokens, specStats);
+        return {next(token, pos)};
+    }
 };
 
 void inference(App &app) {
@@ -160,18 +184,24 @@ void inference(App &app) {
     while (pos < maxPos) {
         const double t0 = nowMs();
         const uint64_t sync0 = app.engine.syncNs();
-        token = app.next(token, pos);
+        // a speculative round emits several tokens: each line shows its share of the round's time
+        const std::vector<int32_t> toks = app.nextTokens(token, pos);
         const double dt = nowMs() - t0;
         predMs += dt;
         syncMs += (double)(app.engine.syncNs() - sync0) * 1e-6;
-        uint64_t sent = 0, recv = 0;
-        app.engine.linkBytes(1, sent, recv);
-        const std::string piece = app.tokenizer.decode(token);
-        std::printf("🔶 Pred%5d ms Sync%5d ms | Sent%6d kB Recv%6d kB | %s\n", (int)dt, (int)((double)(app.engine.syncNs() - sync0) * 1e-6),
-                    (int)(sent / 1024), (int)(recv / 1024), piece.empty() ? "~" : piece.c_str());
-        std::fflush(stdout);
-        pos++;
-        nPred++;
+        for (const int32_t t : toks) {
+            token = t;
+            uint64_t sent = 0, recv = 0;
+            app.engine.linkBytes(1, sent, recv);
+            const std::string piece = app.tokenizer.decode(token);
+            std::printf("🔶 Pred%5d ms Sync%5d ms | Sent%6d kB Recv%6d kB | %s\n", (int)(dt / (double)toks.size()),
+                        (int)((double)(app.engine.syncNs() - sync0) * 1e-6), (int)(sent / 1024), (int)(recv / 1024),
+                        piece.empty() ? "~" : piece.c_str());
+            std::fflush(stdout);
+            pos++;
+            nPred++;
+            if (pos >= maxPos) break;
+        }
     }
     const uint32_t nEval = nIn - 1;
     std::printf("\nEvaluation\n   nBatches: %u\n    nTokens: %u\n", chunk, nEval);
@@ -179,6 +209,7 @@ void inference(App &app) {
     std::printf("Prediction\n    nTokens: %u\n", nPred);
     if (nPred > 0 && predMs > 0) std::printf("   tokens/s: %3.2f (%3.2f ms/tok)\n", nPred * 1000.0 / predMs, predMs / nPred);
     if (app.job.nRanks > 1 && nPred > 0) std::printf("   syncTime: %3.3f ms/tok waiting for peers inside the fused all-reduces\n", syncMs / nPred);
+    if (app.draft) std::printf("%s\n", app.specStats.line().c_str());
 }
 
 void perplexity(App &app) {
@@ -245,21 +276,26 @@ void chat(App &app) {
         app.sampler.beginCompletion();
         std::printf("\n🤖 Assistant\n");
         if (!g.publicPrompt.empty()) std::printf("%s", g.publicPrompt.c_str());
-        while (pos < h.seqLen) {
-            token = app.next(token, pos);
-            const std::string piece = app.tokenizer.decode(token);
-            const EosDetectorResult kind = det.append(token, piece);
-            if (kind == NOT_EOS || kind == EOS) {
-                const std::string delta = det.getDelta();
-                if (!delta.empty()) { std::printf("%s", delta.c_str()); std::fflush(stdout); }
-                det.reset();
+        bool eos = false;
+        while (pos < h.seqLen && !eos) {
+            for (const int32_t t : app.nextTokens(token, pos)) {
+                token = t;
+                const std::string piece = app.tokenizer.decode(token);
+                const EosDetectorResult kind = det.append(token, piece);
+                if (kind == NOT_EOS || kind == EOS) {
+                    const std::string delta = det.getDelta();
+                    if (!delta.empty()) { std::printf("%s", delta.c_str()); std::fflush(stdout); }
+                    det.reset();
+                }
+                pos++;
+                eos = kind == EOS;
+                if (eos || pos >= h.seqLen) break;
             }
-            pos++;
-            if (kind == EOS) break;
         }
         items.clear();
     }
     std::printf("(end of context)\n");
+    if (app.draft) std::printf("%s\n", app.specStats.line().c_str());
 }
 
 }  // namespace
@@ -274,6 +310,10 @@ int main(int argc, char **argv) {
         if (a.model.empty()) throw std::runtime_error("Model is required");
         if (a.tokenizer.empty()) throw std::runtime_error("Tokenizer is required");
         if (a.bufferFloatType != "q80") throw std::runtime_error("This version supports only Q40 weights with Q80 sync type");
+        if (!a.draftModel.empty()) {   // refused before any process or GPU work
+            const std::string why = draftRefusal(a.draftTokens, a.gpus + a.workers, 1);
+            if (!why.empty()) throw std::runtime_error(why);
+        }
         // ---- tensor-parallel job: fork the workers before CUDA exists in this process ----
         TpJob job;
         job.create(a.gpus);

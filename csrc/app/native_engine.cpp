@@ -350,6 +350,20 @@ std::vector<int32_t> NativeEngine::decodeGreedy(int32_t firstToken, uint32_t pos
     return out;
 }
 
+std::vector<int32_t> NativeEngine::specRound(NativeEngine &draft, int32_t token, uint32_t pos, uint32_t k, SpecStats &stats) {
+    constexpr uint32_t kWords = 12, kHead = 4;
+    if (dl_spec_result_words() != kWords) throw std::runtime_error("speculative result block size differs from the library's");
+    draft.synchronize();   // the draft's prefills ran on its own stream; the round runs on this engine's
+    int32_t out[kWords];
+    engCheck(dl_spec_round(impl_->engine, draft.impl_->engine, token, (int)pos, (int)k, 1, out, impl_->stream), "dl_spec_round");
+    const uint32_t n = (uint32_t)out[1];
+    stats.rounds++;
+    stats.drafted += (uint32_t)out[2];
+    stats.accepted += (uint32_t)out[0];
+    stats.emitted += n;
+    return std::vector<int32_t>(out + kHead, out + kHead + n);
+}
+
 int32_t NativeEngine::stepGreedy(int32_t token, uint32_t pos) {
     if (pos >= seqLen_) throw std::runtime_error("position beyond the context length");
     Impl &I = *impl_;

@@ -7,6 +7,9 @@
 // that do not want an interpreter link against.
 #pragma once
 #include <cstdint>
+#include <cstdio>
+#include <cstdlib>
+#include <utility>
 #include <functional>
 #include <stdexcept>
 #include <string>
@@ -29,6 +32,45 @@ inline uint64_t kvCacheBytes(const ModelHeader &h, uint32_t nRanks, uint32_t kvT
     const uint64_t values = 2ull * h.nLayers * h.seqLen * kvHeads * h.headDim;
     return kvType == 0 ? 2 * values : values + values / 16;
 }
+
+// Greedy speculative decoding (--draft-model): why `draftTokens` drafts a round cannot run in this configuration, empty when they
+// can (the rules of distributed_llama_b200.api.draft_refusal). target / draft: the model headers once read, the draft's read with
+// the target's context length.
+inline std::string draftRefusal(uint32_t draftTokens, uint32_t nRanks, uint32_t parallel, const ModelHeader *target = nullptr,
+                                const ModelHeader *draft = nullptr) {
+    if (draftTokens != 1 && draftTokens != 3 && draftTokens != 7) return "--draft-tokens must be 1, 3 or 7";
+    if (nRanks > 1) return "--draft-model runs on one GPU only (no --gpus > 1 or --workers)";
+    const char *c = std::getenv("DL_COLLECTIVES");
+    if (c && std::string(c) == "nccl") return "--draft-model does not support DL_COLLECTIVES=nccl";
+    if (parallel > 1) return "--draft-model does not combine with --parallel > 1";
+    if (!target || !draft) return "";
+    const std::pair<const char *, const ModelHeader *> models[2] = {{"target model", target}, {"draft model", draft}};
+    for (const auto &m : models) {
+        if (m.second->nExperts > 0)
+            return std::string("--draft-model needs dense models: the ") + m.first + " is mixture-of-experts (no batched verify step)";
+        if (m.second->weightType != F_Q40)
+            return std::string("--draft-model needs q40 weights: the ") + m.first + " has " + floatTypeName(m.second->weightType) + " weights";
+    }
+    if (target->vocabSize != draft->vocabSize)
+        return "--draft-model needs the target's vocabulary: " + std::to_string(target->vocabSize) + " tokens against " +
+               std::to_string(draft->vocabSize);
+    if (draft->seqLen < target->seqLen)
+        return "--draft-model needs a context of at least " + std::to_string(target->seqLen) + " tokens: the draft model has " +
+               std::to_string(draft->seqLen);
+    return "";
+}
+
+// Counters of speculative rounds and the CLIs' summary line.
+struct SpecStats {
+    uint64_t rounds = 0, drafted = 0, accepted = 0, emitted = 0;
+    std::string line() const {
+        char buf[160];
+        std::snprintf(buf, sizeof(buf), "Speculative: %llu rounds, %llu drafted, %llu accepted (%.1f %%), %.2f tokens/round",
+                      (unsigned long long)rounds, (unsigned long long)drafted, (unsigned long long)accepted,
+                      drafted ? 100.0 * (double)accepted / (double)drafted : 0.0, rounds ? (double)emitted / (double)rounds : 0.0);
+        return buf;
+    }
+};
 
 class NativeEngine {
 public:
@@ -114,6 +156,10 @@ public:
                                            std::vector<int32_t> &blocks);
     // n greedy steps back to back on the device without host round trips; returns the generated tokens.
     std::vector<int32_t> decodeGreedy(int32_t firstToken, uint32_t pos, uint32_t nSteps);
+    // One round of greedy speculative decoding with this engine as the target (dl_spec_round): `token` is the last emitted token at
+    // `pos`, both engines hold every row before it; the draft proposes k (1, 3, 7; fewer near the end of the context) tokens.
+    // Returns the tokens greedy decoding emits next (1 to k + 1) and adds the round to `stats`.
+    std::vector<int32_t> specRound(NativeEngine &draft, int32_t token, uint32_t pos, uint32_t k, SpecStats &stats);
     void synchronize();
     // Traffic / synchronisation accounting of the reference's Eval / Pred lines (src/dllama.cpp:59-66): cumulative ns this rank's
     // decode kernel waited for its peers inside the fused all-reduces, and (sent, received) NVLink bytes of a forward over nTokens

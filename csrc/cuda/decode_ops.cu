@@ -206,6 +206,47 @@ __global__ void __launch_bounds__(1024) argmaxAdvanceKernel(const float *__restr
     }
 }
 
+// One CTA per logits row: row b's arg-max over ids [0, vocab), lowest id among equal maxima, into out[b]. The verify step of a
+// speculative round uses it after a STORE logits GEMV where the fused per-row arg-max does not fit shared memory.
+__global__ void __launch_bounds__(1024) argmaxRowsKernel(const float *__restrict__ logits, uint32_t stride, uint32_t vocab, int *out) {
+    pdlLaunchDependents();
+    pdlWait();
+    __shared__ float sv[32];
+    __shared__ int si[32];
+    const float *row = logits + (size_t)blockIdx.x * stride;
+    float best = -INFINITY;
+    int bi = 0x7fffffff;
+    for (uint32_t i = threadIdx.x; i < vocab; i += blockDim.x) {
+        const float v = row[i];
+        if (v > best || bi == 0x7fffffff) { best = v; bi = (int)i; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+    }
+    if ((threadIdx.x & 31) == 0) { sv[threadIdx.x >> 5] = best; si[threadIdx.x >> 5] = bi; }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        best = sv[threadIdx.x];
+        bi = si[threadIdx.x];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (ov > best || (ov == best && oi < bi)) { best = ov; bi = oi; }
+        }
+        if (threadIdx.x == 0) out[blockIdx.x] = bi;
+    }
+}
+
+int launchArgmaxRows(const float *logits, uint32_t stride, uint32_t vocab, int nb, int *out, cudaStream_t stream, bool pdl) {
+    if (nb < 1 || vocab < 1) return -1;
+    DL_CUDA_CHECK(launchPdl(argmaxRowsKernel, dim3(nb), dim3(1024), 0, stream, pdl, logits, stride, vocab, out));
+    return 0;
+}
+
 int launchEmbedding(const EmbTable &table, const int *tokens, float *x, uint32_t dim, uint32_t xStride, uint32_t vocab, int nb,
                     cudaStream_t stream) {
     embeddingKernel<<<nb, 256, 0, stream>>>(table, tokens, x, dim, xStride, vocab);
@@ -282,4 +323,9 @@ DL_EXPORT int dl_moe_router(const float *x, const float *normW, const float *gat
     a.x = x; a.normW = normW; a.gate = gate; a.eps = eps; a.dim = dim; a.nExperts = nExperts; a.k = k;
     a.logits = logits; a.counter = counter; a.expertIdx = expertIdx; a.expertWeight = expertWeight;
     return dl::launchMoeRouter(a, T, stream, false);
+}
+
+// Per-row arg-max of nb logits rows (tests/test_gpu_speculative.py): row b = logits + b * stride, ids [0, vocab), into out[b].
+DL_EXPORT int dl_argmax_rows(const float *logits, uint32_t stride, uint32_t vocab, int nb, int *out, cudaStream_t stream) {
+    return dl::launchArgmaxRows(logits, stride, vocab, nb, out, stream, false);
 }

@@ -113,6 +113,23 @@ struct Engine {
     cudaEvent_t pagesStaged = nullptr;   // the last upload has read pageHost
     bool tcAttn = true;          // prefill attention on the tensor cores (DL_NO_TC_ATTN=1: per-token CUDA-core kernel)
     bool fusedAttn = true;       // debugging switch (DL_NO_FUSED_ATTN)
+    uint64_t serial = 0;         // unique per engine of the process (a round graph names its draft by it)
+    uint32_t graphGen = 0;       // bumped whenever captured launches of this engine go stale (dropGraph)
+    struct Spec *spec = nullptr; // speculative rounds with this engine as the target (dl_spec_round), allocated on first use
+};
+
+// The target's state of speculative rounds: per-row arg-max scratch of the verify GEMV, its tokens, the accept kernel's result
+// block, a pinned staging block and one round graph per draft length.
+struct Spec {
+    uint8_t *dev = nullptr;            // one allocation: argVal [8][256], argIdx [8][256], counter, verify tokens [8], result block
+    float *argVal = nullptr;
+    int *argIdx = nullptr;
+    unsigned int *argCounter = nullptr;
+    int *verifyTok = nullptr, *result = nullptr;
+    int32_t *stage = nullptr;          // pinned: [0] token, [1] position in; [kSpecResultHead..] the result block out
+    cudaGraphExec_t graph[kSpecMaxDraft + 1] = {};
+    uint64_t graphDraft[kSpecMaxDraft + 1] = {};          // serial of the draft engine the graph was captured with
+    uint32_t graphGen[kSpecMaxDraft + 1][2] = {};         // graphGen of the target and the draft at capture
 };
 
 #define DL_TRY(expr)                    \
@@ -270,7 +287,8 @@ static RopeKvArgs layerRopeKv(const Engine &e, const LayerPtrs &L, float *qkv, c
     return r;
 }
 
-// logitsMode: 0 = none (prefill chunk), 1 = logits of the last token in the batch into logits[0], 2 = all tokens.
+// logitsMode: 0 = none (prefill chunk), 1 = logits of the last token in the batch into logits[0], 2 = all tokens, 3 = all tokens
+// and the arg-max of every row into spec->verifyTok (the verify step of a speculative round: nb >= 2, one rank, dense q40).
 // ch: a choices step instead of a batch of consecutive tokens (logitsMode 2, dense layers only); sl: a slots step (same limits).
 static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, cudaStream_t stream, const ChoiceStep *ch = nullptr,
                          const SlotStep *sl = nullptr) {
@@ -280,6 +298,7 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
     if (nb < 1 || (uint32_t)nb > c.maxBatch || (nb & (nb - 1))) return -10;
     e.lastDecodeMega = false;
     if ((ch || sl) && (c.nExperts > 0 || logitsMode != 2 || greedyAdvance)) return -14;
+    if (logitsMode == 3 && (nb < 2 || !e.spec || greedyAdvance || c.wType != 0 || c.nExperts > 0 || e.comm.nRanks > 1)) return -73;
     if (nb == 1 && logitsMode == 1 && e.useMega) {
         const int r = engineDecodeMega(e, greedyAdvance, stream);
         if (r != 1) { e.lastDecodeMega = r == 0; return r; }
@@ -405,6 +424,19 @@ static int engineForward(Engine &e, int nb, int logitsMode, bool greedyAdvance, 
                 DL_TRY(gemvSel(e, PRO_RMSNORM_, EPI_STORE_, 1, a, c.numSms, stream, pdl));
                 if (greedyAdvance)
                     DL_TRY(launchArgmaxAdvance(e.g.logits, localVocabLimit(e), e.g.tokens, e.g.pos, e.g.history, c.seqLen, stream, pdl));
+            }
+        } else if (logitsMode == 3) {
+            a.in = e.g.x;
+            a.argVal = e.spec->argVal; a.argIdx = e.spec->argIdx; a.argCounter = e.spec->argCounter; a.tokenOut = e.spec->verifyTok;
+            a.vocabLimit = e.vocabLimit;
+            const int r = gemvQ40Tma(PRO_RMSNORM_, EPI_ARGMAX_ROWS_, nb, a, c.numSms, stream, pdl);
+            if (r < 0) return r;
+            if (r == 1) {
+                // the fused per-row arg-max needs all nb rows' partial sums in one CTA's shared memory (Llama-3.3-70B, Qwen3-14B
+                // logits at nb = 8 do not fit): the STORE GEMV, which may split the batch, then one arg-max CTA per row
+                a.argVal = nullptr; a.argIdx = nullptr; a.argCounter = nullptr; a.tokenOut = nullptr;
+                DL_TRY(gemvSel(e, PRO_RMSNORM_, EPI_STORE_, nb, a, c.numSms, stream, pdl));
+                DL_TRY(launchArgmaxRows(e.g.logits, c.vocab, localVocabLimit(e), nb, e.spec->verifyTok, stream, pdl));
             }
         } else {
             a.in = e.g.x;
@@ -556,6 +588,7 @@ static uint64_t arenaLayout(const EngineConfig &c, uint32_t vocabFull, Comm &m) 
 
 static void dropGraph(Engine &e) {
     if (e.decodeGraph) { cudaGraphExecDestroy(e.decodeGraph); e.decodeGraph = nullptr; }
+    e.graphGen++;   // round graphs that hold this engine's launches are captured again
 }
 
 }  // namespace dl
@@ -569,8 +602,10 @@ static_assert(sizeof(Engine::slotLogprobs) == kChoiceRngSlots * sizeof(int), "on
 DL_EXPORT void *dl_engine_create(const dl::EngineConfig *cfg) {
     if (cfg->kvType > 1 || (cfg->kvType == 1 && cfg->headDim % 32)) return nullptr;   // unknown KV-cache storage
     if (cfg->maxPrefill < 1 || cfg->maxPrefill > 256) return nullptr;
+    static uint64_t serials = 0;
     Engine *e = new Engine();
     e->cfg = *cfg;
+    e->serial = ++serials;
     dl::gHiddenAct = cfg->hiddenAct;
     e->layers.resize(cfg->nLayers);
     e->fusedAttn = std::getenv("DL_NO_FUSED_ATTN") == nullptr;
@@ -592,6 +627,12 @@ DL_EXPORT void dl_engine_destroy(void *h) {
     Engine *e = (Engine *)h;
     if (!e) return;
     if (e->decodeGraph) cudaGraphExecDestroy(e->decodeGraph);
+    if (e->spec) {
+        for (cudaGraphExec_t g : e->spec->graph) if (g) cudaGraphExecDestroy(g);
+        if (e->spec->dev) cudaFree(e->spec->dev);
+        if (e->spec->stage) cudaFreeHost(e->spec->stage);
+        delete e->spec;
+    }
     if (e->captureStream) cudaStreamDestroy(e->captureStream);
     if (e->megaLayers) cudaFree(e->megaLayers);
     if (e->megaKvScales) cudaFree(e->megaKvScales);
@@ -1519,3 +1560,129 @@ DL_EXPORT int dl_engine_slot_pages(void *h, uint32_t slot, int32_t *out, uint32_
     for (uint32_t i = 0; i < e->slotPages[slot] && i < cap; i++) out[i] = e->pageHost[(size_t)slot * e->nPages + i];
     return (int)e->slotPages[slot];
 }
+
+// ---- speculative decoding with a draft model (speculative.cu) ------------------------------------------------------------------------
+
+static int ensureSpec(Engine *e) {
+    if (e->spec) return 0;
+    dl::Spec *s = new dl::Spec();
+    const size_t words = 8 * 256;
+    const size_t bytes = words * 4 * 2 + 64 + 32 + dl::kSpecResultWords * 4;
+    if (cudaMalloc(&s->dev, bytes) != cudaSuccess || cudaMemset(s->dev, 0, bytes) != cudaSuccess ||
+        cudaHostAlloc((void **)&s->stage, (dl::kSpecResultHead + dl::kSpecResultWords) * 4, cudaHostAllocDefault) != cudaSuccess) {
+        if (s->dev) cudaFree(s->dev);
+        delete s;
+        return -77;   // out of device or pinned memory; nothing is kept, a later call tries again
+    }
+    s->argVal = (float *)s->dev;
+    s->argIdx = (int *)(s->dev + words * 4);
+    s->argCounter = (unsigned int *)(s->dev + words * 8);
+    s->verifyTok = (int *)(s->dev + words * 8 + 64);
+    s->result = (int *)(s->dev + words * 8 + 96);
+    e->spec = s;
+    return 0;
+}
+
+// Whether `draft` can draft for `target`: two engines on one rank, dense q40 layers, the same vocabulary and KV-cache storage, no slots.
+static int specCheck(const Engine &t, const Engine &d) {
+    if (&t == &d) return -72;
+    for (const Engine *e : {&t, &d})
+        if (e->comm.nRanks > 1 || e->cfg.nExperts > 0 || e->cfg.wType != 0 || e->slots > 1) return -73;
+    if (t.cfg.vocab != d.cfg.vocab || t.g.vocabFull != d.g.vocabFull || t.cfg.kvType != d.cfg.kvType) return -72;
+    return 0;
+}
+
+static dl::SpecAcceptArgs specArgs(Engine &t, Engine &d, uint32_t k) {
+    dl::SpecAcceptArgs a{};
+    a.verifyTokens = t.spec->verifyTok; a.targetTokens = t.g.tokens; a.targetPos = t.g.pos; a.targetHistory = t.g.history;
+    a.historyCap = t.cfg.seqLen; a.draftTokens = d.g.tokens; a.draftPos = d.g.pos; a.draftHistory = d.g.history;
+    a.draftHistoryCap = d.cfg.seqLen; a.k = k; a.result = t.spec->result;
+    return a;
+}
+
+// The launches of one round of k drafts. The draft feeds t, d1..dk (k + 1 greedy steps, the last output unused): so it holds the
+// row of dk when every draft is accepted. The target verifies [t, d1..dk] at p..p+k, the accept kernel keeps g(0..a).
+static int specRoundLaunches(Engine &t, Engine &d, uint32_t k, cudaStream_t stream) {
+    const dl::SpecAcceptArgs a = specArgs(t, d, k);
+    DL_TRY(dl::launchSpecStage(a, stream));
+    for (uint32_t i = 1; i <= k + 1; i++) {
+        DL_TRY(dl::engineForward(d, 1, 1, true, stream));
+        if (i <= k) DL_CUDA_CHECK(cudaMemcpyAsync(t.g.tokens + i, d.g.tokens, 4, cudaMemcpyDeviceToDevice, stream));
+    }
+    DL_TRY(dl::engineForward(t, (int)k + 1, 3, false, stream));
+    return dl::launchSpecAccept(a, stream);
+}
+
+static int captureSpecRound(Engine &t, Engine &d, uint32_t k) {
+    dl::Spec &s = *t.spec;
+    if (s.graph[k]) { cudaGraphExecDestroy(s.graph[k]); s.graph[k] = nullptr; }
+    if (!t.captureStream) DL_CUDA_CHECK(cudaStreamCreateWithFlags(&t.captureStream, cudaStreamNonBlocking));
+    DL_CUDA_CHECK(cudaStreamBeginCapture(t.captureStream, cudaStreamCaptureModeThreadLocal));
+    const int r = specRoundLaunches(t, d, k, t.captureStream);
+    cudaGraph_t graph = nullptr;
+    const cudaError_t endErr = cudaStreamEndCapture(t.captureStream, &graph);
+    if (r != 0) { if (graph) cudaGraphDestroy(graph); return r; }
+    DL_CUDA_CHECK(endErr);
+    DL_CUDA_CHECK(cudaGraphInstantiate(&s.graph[k], graph, 0));
+    cudaGraphDestroy(graph);
+    s.graphDraft[k] = d.serial;
+    s.graphGen[k][0] = t.graphGen;
+    s.graphGen[k][1] = d.graphGen;
+    return 0;
+}
+
+// One round of speculative decoding: the last emitted token `token` sits at position `pos`, and both engines hold valid KV rows for
+// every position before it. k (1, 3 or 7) drafts, fewer where pos + k would reach the end of either cache; at the last row one
+// greedy step of each engine (k = 0). Writes the result block (kSpecResultWords int32, layout in kernels.h) to `out` once the
+// round has finished on `stream`. useGraph: replay the round's graph (captured after the first eager round of each k).
+DL_EXPORT int dl_spec_round(void *target, void *draft, int token, int pos, int k, int useGraph, int32_t *out, cudaStream_t stream) {
+    Engine &t = *(Engine *)target, &d = *(Engine *)draft;
+    DL_TRY(specCheck(t, d));
+    if (k != 1 && k != 3 && k != 7) return -75;
+    const uint32_t seqLen = std::min(t.cfg.seqLen, d.cfg.seqLen);
+    if (pos < 0 || (uint32_t)pos >= seqLen) return -71;
+    while (k > 0 && (uint32_t)(pos + k) >= seqLen) k /= 2;   // 7 -> 3 -> 1 -> 0
+    if ((uint32_t)k + 1 > t.cfg.maxBatch) return -10;
+    DL_TRY(ensureSpec(&t));
+    dl::Spec &s = *t.spec;
+    int32_t *res = s.stage + dl::kSpecResultHead;
+    s.stage[0] = token;
+    s.stage[1] = pos;
+    DL_CUDA_CHECK(cudaMemcpyAsync(t.g.tokens, s.stage, 4, cudaMemcpyHostToDevice, stream));
+    DL_CUDA_CHECK(cudaMemcpyAsync(t.g.pos, s.stage + 1, 4, cudaMemcpyHostToDevice, stream));
+    if (k == 0) {
+        DL_CUDA_CHECK(cudaMemcpyAsync(d.g.tokens, s.stage, 4, cudaMemcpyHostToDevice, stream));
+        DL_CUDA_CHECK(cudaMemcpyAsync(d.g.pos, s.stage + 1, 4, cudaMemcpyHostToDevice, stream));
+        for (Engine *e : {&t, &d}) {
+            if (useGraph) DL_TRY(dl_engine_decode_graph(e, 1, stream));
+            else DL_TRY(dl::engineForward(*e, 1, 1, true, stream));
+        }
+        DL_CUDA_CHECK(cudaMemcpyAsync(res + dl::kSpecResultHead, t.g.tokens, 4, cudaMemcpyDeviceToHost, stream));
+        DL_CUDA_CHECK(cudaStreamSynchronize(stream));
+        res[0] = 0; res[1] = 1; res[2] = 0; res[3] = pos + 1;
+    } else {
+        const bool fresh = s.graph[k] && s.graphDraft[k] == d.serial && s.graphGen[k][0] == t.graphGen && s.graphGen[k][1] == d.graphGen;
+        if (useGraph && fresh) DL_CUDA_CHECK(cudaGraphLaunch(s.graph[k], stream));
+        else DL_TRY(specRoundLaunches(t, d, (uint32_t)k, stream));   // the first round of a k also sets the kernels' attributes
+        DL_CUDA_CHECK(cudaMemcpyAsync(res, s.result, dl::kSpecResultWords * 4, cudaMemcpyDeviceToHost, stream));
+        DL_CUDA_CHECK(cudaStreamSynchronize(stream));
+        if (useGraph && !fresh) DL_TRY(captureSpecRound(t, d, (uint32_t)k));
+    }
+    if (dl_engine_aborted(&t) || dl_engine_aborted(&d)) return -74;
+    std::memcpy(out, res, dl::kSpecResultWords * 4);
+    return 0;
+}
+
+// The verify step alone (tests): nb (2, 4 or 8) tokens staged in tokens[0..nb) at pos[0..nb), logits of every row into logits[0..nb)
+// and the arg-max of row b (ids >= the vocabulary limit ignored, lowest id among ties) into out[b] once the stream has finished.
+DL_EXPORT int dl_engine_verify(void *h, int nb, int32_t *out, cudaStream_t stream) {
+    Engine &e = *(Engine *)h;
+    DL_TRY(ensureSpec(&e));
+    DL_TRY(dl::engineForward(e, nb, 3, false, stream));
+    DL_CUDA_CHECK(cudaMemcpyAsync(e.spec->stage, e.spec->verifyTok, nb * 4, cudaMemcpyDeviceToHost, stream));
+    DL_CUDA_CHECK(cudaStreamSynchronize(stream));
+    std::memcpy(out, e.spec->stage, nb * 4);
+    return 0;
+}
+
+DL_EXPORT uint32_t dl_spec_result_words() { return dl::kSpecResultWords; }

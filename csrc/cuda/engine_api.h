@@ -137,6 +137,9 @@ int dl_engine_prefill_scratch(void *h, uint32_t rows, void *px, void *pqkv, void
 int dl_engine_set_prefill_min_tc(void *h, uint32_t n);   // shortest chunk on the tensor cores (default 9; 0: never)
 int dl_engine_decode_graph(void *h, int nSteps, cudaStream_t stream);   // captures the greedy step on first use
 int dl_engine_graph_captured(void *h);
+// one round of greedy speculative decoding with `draft` (engine.cu): result block of dl_spec_result_words() int32 into `out`
+int dl_spec_round(void *target, void *draft, int token, int pos, int k, int useGraph, int32_t *out, cudaStream_t stream);
+uint32_t dl_spec_result_words();
 void dl_abi_struct_sizes(uint32_t out[4]);   // sizeof EngineConfig, LayerPtrs, GlobalPtrs, CommPtrs
 // symmetric peer-memory arena (csrc/cuda/comm_vmm.cu): create (local, binds the bootstrap socket) -> [job-wide barrier] -> connect
 // (collective: exchanges file descriptors, maps every peer, sets up the NVSwitch multicast mapping)

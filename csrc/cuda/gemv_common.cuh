@@ -15,7 +15,8 @@ namespace dl {
     DL_GEMV_NB(X, PRO_RMSNORM_, EPI_STORE_) DL_GEMV_NB(X, PRO_PLAIN_, EPI_RESIDUAL_) DL_GEMV_NB(X, PRO_RMSNORM_, EPI_SWIGLU_) \
     DL_GEMV_NB(X, PRO_PLAIN_, EPI_STORE_) X(PRO_PLAIN_, EPI_SWIGLU_, 1)
 #define DL_GEMV_Q40_TMA_INSTANCES(X) \
-    DL_GEMV_Q40_LDG_INSTANCES(X) X(PRO_RMSNORM_, EPI_ARGMAX_, 1) X(PRO_PLAIN_, EPI_MOE_DOWN_, 1)
+    DL_GEMV_Q40_LDG_INSTANCES(X) X(PRO_RMSNORM_, EPI_ARGMAX_, 1) X(PRO_PLAIN_, EPI_MOE_DOWN_, 1) \
+    X(PRO_RMSNORM_, EPI_ARGMAX_ROWS_, 2) X(PRO_RMSNORM_, EPI_ARGMAX_ROWS_, 4) X(PRO_RMSNORM_, EPI_ARGMAX_ROWS_, 8)
 
 // Sum over the 512 threads of a block; `red` holds 16 floats.
 __device__ __forceinline__ float blockSum512(float v, float *red) {
@@ -197,6 +198,53 @@ __device__ __forceinline__ void argMaxEpilogue(float best, int bestIdx, float *r
         o.pos[0] = p;
         if (o.history && (uint32_t)p < o.historyCap) o.history[p] = bestIdx;
     }
+}
+
+// Per-row arg-max of an NB-row logits launch (NB > 1, one rank): every consumer thread has reduced its rows of logits row
+// tid % NB to (best, bestIdx). Each CTA leaves row t's candidate at o.val / o.idx [t * grid + cta]; the last CTA to arrive
+// writes row t's winner, the lowest index among equal maxima, to o.token[t]. Positions and history are not touched.
+// `scratch` holds 2 * kConsumerWarps * NB words of shared memory that no consumer reads any more.
+template <int NB>
+__device__ __forceinline__ void argMaxRowsEpilogue(float best, int bestIdx, float *scratch, const ArgMaxOut &o, int tid) {
+    static_assert(NB > 1 && NB <= 8 && (NB & (NB - 1)) == 0, "rows of a batched launch");
+    const int lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+    for (int off = 16; off >= NB; off >>= 1) {   // lanes with the same lane % NB hold the same row
+        const float ov = __shfl_xor_sync(0xffffffffu, best, off);
+        const int oi = __shfl_xor_sync(0xffffffffu, bestIdx, off);
+        argMaxMerge(best, bestIdx, ov, oi);
+    }
+    float *sv = scratch;
+    int *si = reinterpret_cast<int *>(scratch + kConsumerWarps * NB);
+    consumerBarrier();
+    if (lane < NB) { sv[warp * NB + lane] = best; si[warp * NB + lane] = bestIdx; }
+    consumerBarrier();
+    __shared__ bool lastCta;
+    if (warp == 0) {
+        if (lane < NB) {
+            best = -INFINITY;
+            bestIdx = 0x7fffffff;
+            for (int w = 0; w < kConsumerWarps; w++) argMaxMerge(best, bestIdx, sv[w * NB + lane], si[w * NB + lane]);
+            o.val[lane * gridDim.x + blockIdx.x] = best;
+            o.idx[lane * gridDim.x + blockIdx.x] = bestIdx;
+            __threadfence();
+        }
+        __syncwarp();
+        if (lane == 0) {
+            const unsigned int prev = atomicAdd(o.counter, 1u);
+            lastCta = prev == gridDim.x - 1;
+            if (lastCta) *o.counter = 0;
+        }
+    }
+    consumerBarrier();
+    if (!lastCta || warp >= NB) return;
+    __threadfence();
+    best = -INFINITY;
+    bestIdx = 0x7fffffff;
+    for (uint32_t i = lane; i < gridDim.x; i += 32)
+        argMaxMerge(best, bestIdx, __ldcg(o.val + warp * gridDim.x + i), __ldcg(o.idx + warp * gridDim.x + i));
+    warpArgMax(best, bestIdx);
+    if (lane == 0) o.token[warp] = bestIdx;
 }
 
 }  // namespace dl

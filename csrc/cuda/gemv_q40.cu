@@ -218,3 +218,20 @@ DL_EXPORT int dl_gemv_q40_argmax(const void *qs, const void *scales, uint32_t d,
     a.rowOffsetGlobal = rowOffsetGlobal; a.vocabLimit = vocabLimit;
     return dl::gemvQ40Tma(dl::PRO_RMSNORM_, dl::EPI_ARGMAX_, 1, a, numSms, stream, false);
 }
+
+// Logits of nb (2, 4 or 8) activation rows [nb][n] with the per-row fused arg-max (tests): out [nb][d]; row b's lowest-index maximum
+// among ids < vocabLimit (0: no limit) into tokenOut[b]. argVal / argIdx hold nb x grid candidates, argCounter is zeroed and
+// self-resetting. 1: the shape does not fit the TMA kernel at this width.
+DL_EXPORT int dl_gemv_q40_argmax_rows(const void *qs, const void *scales, uint32_t d, uint32_t n, const float *in, const float *normW, float eps,
+                                      float *out, float *argVal, int *argIdx, unsigned int *argCounter, int *tokenOut, uint32_t vocabLimit,
+                                      int nb, int numSms, cudaStream_t stream) {
+    if (nb != 2 && nb != 4 && nb != 8) return -4;
+    dl::GemvArgs a{};
+    a.qs = (const uint32_t *)qs;
+    a.scales = (const __half *)scales;
+    a.d = d; a.n = n;
+    a.in = in; a.inStride = n; a.normW = normW; a.eps = eps;
+    a.out = out; a.outStride = d;
+    a.argVal = argVal; a.argIdx = argIdx; a.argCounter = argCounter; a.tokenOut = tokenOut; a.vocabLimit = vocabLimit;
+    return dl::gemvQ40Tma(dl::PRO_RMSNORM_, dl::EPI_ARGMAX_ROWS_, nb, a, numSms, stream, false);
+}

@@ -257,12 +257,17 @@ __global__ void __launch_bounds__(kTmaThreads, (NB == 1 ? 2 : 1)) gemvQ40TmaKern
             const uint32_t r = i / NB, t = i - r * NB;
             const float v = rowSum(r, t);
             a.out[(size_t)t * a.outStride + rowBase + r] = v;
-            if (EPI == EPI_ARGMAX_ && v > best && a.rowOffsetGlobal + rowBase + r < a.vocabLimit) { best = v; bestIdx = (int)(a.rowOffsetGlobal + rowBase + r); }   // rows ascend per thread
+            if ((EPI == EPI_ARGMAX_ || EPI == EPI_ARGMAX_ROWS_) && v > best && a.rowOffsetGlobal + rowBase + r < a.vocabLimit) { best = v; bestIdx = (int)(a.rowOffsetGlobal + rowBase + r); }   // rows ascend per thread
         }
         if (EPI == EPI_ARGMAX_) {
             // greedy sampling fused into the logits kernel: the next token and the position advance stay on the device
             const ArgMaxOut o{a.argVal, a.argIdx, a.argCounter, a.tokenOut, a.posInOut, a.history, a.historyCap};
             argMaxEpilogue(best, bestIdx, red, o, a.ar, tid, [] { return false; });
+        }
+        if constexpr (EPI == EPI_ARGMAX_ROWS_ && NB > 1) {
+            // a thread's rows all belong to logits row tid % NB; the activation planes are no longer read
+            const ArgMaxOut o{a.argVal, a.argIdx, a.argCounter, a.tokenOut, nullptr, nullptr, 0};
+            argMaxRowsEpilogue<NB>(best, bestIdx, reinterpret_cast<float *>(planeA), o, tid);
         }
     }
     traceStamp(a.trace, 3);

@@ -5,7 +5,8 @@
 namespace dl {
 
 enum { PRO_RMSNORM_ = 0, PRO_PLAIN_ = 1 };
-enum { EPI_STORE_ = 0, EPI_RESIDUAL_ = 1, EPI_SWIGLU_ = 2, EPI_ARGMAX_ = 3, EPI_MOE_DOWN_ = 4 };
+enum { EPI_STORE_ = 0, EPI_RESIDUAL_ = 1, EPI_SWIGLU_ = 2, EPI_ARGMAX_ = 3, EPI_MOE_DOWN_ = 4, EPI_ARGMAX_ROWS_ = 5 };
+// EPI_ARGMAX: one row, the token is fed back (position advance, history); EPI_ARGMAX_ROWS: 2-8 rows, each row's arg-max to tokenOut[row]
 
 // In-kernel one-shot all-reduce over NVLink peer memory (see the EPI_RESIDUAL epilogue of gemv_q40_tma.cu).
 constexpr int kMaxRanks = 8;
@@ -332,6 +333,23 @@ int launchEmbedding(const EmbTable &table, const int *tokens, float *x, uint32_t
                     cudaStream_t stream);
 int launchArgmaxAdvance(const float *logits, uint32_t vocab, int *tokenOut, int *pos, int *history, uint32_t historyCap,
                         cudaStream_t stream, bool pdl);   // single rank only: the index is local to `logits`
+int launchArgmaxRows(const float *logits, uint32_t stride, uint32_t vocab, int nb, int *out, cudaStream_t stream, bool pdl);
+
+// Speculative decoding (speculative.cu). Result block of a round, int32: [0] accepted drafts a, [1] emitted tokens a + 1, [2] drafts k,
+// [3] position of the last emitted token, [kSpecResultHead + i] emitted token i.
+constexpr uint32_t kSpecMaxDraft = 7, kSpecResultHead = 4, kSpecResultWords = kSpecResultHead + kSpecMaxDraft + 1;
+struct SpecAcceptArgs {
+    const int *verifyTokens;            // [k + 1] the target's arg-max after rows t, d1..dk
+    int *targetTokens, *targetPos;      // [k + 1]: t, d1..dk and p (row 0); next round: tokens[0], pos[0]
+    int *targetHistory;                 // history[q] = the token at position q (may be null)
+    uint32_t historyCap;
+    int *draftTokens, *draftPos, *draftHistory;
+    uint32_t draftHistoryCap;
+    uint32_t k;                         // 1 .. kSpecMaxDraft
+    int *result;                        // [kSpecResultWords]
+};
+int launchSpecStage(const SpecAcceptArgs &a, cudaStream_t stream);
+int launchSpecAccept(const SpecAcceptArgs &a, cudaStream_t stream);
 
 // Device-side temperature / top-p sampler and the logits gather that feeds it under tensor parallelism (sampler.cu)
 // Optional per-request controls, applied to every logit before temperature (float32, round to nearest, no contraction):

@@ -86,8 +86,8 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     backend's choice_controls hands them to the batched path). `backend` provides
     next_token(token, pos, sampler), forget_device_seed(), save_sampler() / restore_sampler(saved), and for the batched path
     batched_choices(n), seed_choices(seeds), choice_controls(sampler, n), choices_first(token, P, n, T, topp) and
-    choices_step(tokens, P, C, j, active, T, topp) (TokenSteps: InferenceSession and apps.runtime.RootInference). Returns each
-    choice's tokens.
+    choices_step(tokens, P, C, j, active, T, topp) (TokenSteps: InferenceSession and apps.runtime.RootInference), and with a draft
+    model (backend.draft set) speculates(sampler) and spec_round(token, pos). Returns each choice's tokens.
 
     logprobs = k (0..20): on_logprobs(i, entry) is called right before on_token(i, tok) with the entry of that token,
     (tok, logprob, [(id, logprob), ...] k most likely); the backend's next_token, choices_first and choices_step then take a
@@ -107,19 +107,24 @@ def run_choices(backend, token: int, P: int, n: int, max_tokens: int, seq_len: i
     sampler.begin_completion()
 
     def single(smp, choices):
-        # today's single-sequence path from P; rows past P belong to this sequence until the next one overwrites them
+        # today's single-sequence path from P; rows past P belong to this sequence until the next one overwrites them. A single
+        # greedy completion with a draft model takes speculative rounds of several tokens instead (the same tokens).
         tok, pos, done = token, P, set()
+        spec = n == 1 and not lp and getattr(backend, "draft", None) is not None and backend.speculates(smp)
         while len(out[choices[0]]) < limit:
-            tok = backend.next_token(tok, pos, smp, **lp)
+            toks = backend.spec_round(tok, pos) if spec else [backend.next_token(tok, pos, smp, **lp)]
             entry = backend.last_logprobs()[0] if lp else None
-            pos += 1
-            for i in choices:
-                if i not in done:
-                    out[i].append(tok)
-                    if lp:
-                        on_logprobs(i, entry)
-                    if on_token(i, tok):
-                        done.add(i)
+            for tok in toks:
+                pos += 1
+                for i in choices:
+                    if i not in done:
+                        out[i].append(tok)
+                        if lp:
+                            on_logprobs(i, entry)
+                        if on_token(i, tok):
+                            done.add(i)
+                if len(done) == len(choices) or len(out[choices[0]]) >= limit:
+                    break
             if len(done) == len(choices):
                 break
 
@@ -167,6 +172,60 @@ def _lp_kw(logprobs: Optional[int]) -> dict:
     return {} if logprobs is None else {"logprobs": logprobs}
 
 
+class SpecStats:
+    """Counters of speculative rounds: rounds, drafted and accepted tokens, emitted tokens."""
+
+    def __init__(self):
+        self.rounds = self.drafted = self.accepted = self.emitted = 0
+
+    def add(self, drafted: int, accepted: int, emitted: int) -> None:
+        self.rounds += 1
+        self.drafted += drafted
+        self.accepted += accepted
+        self.emitted += emitted
+
+    def line(self) -> str:
+        """The CLIs' summary line."""
+        rate = 100.0 * self.accepted / self.drafted if self.drafted else 0.0
+        per = self.emitted / self.rounds if self.rounds else 0.0
+        return (f"Speculative: {self.rounds} rounds, {self.drafted} drafted, {self.accepted} accepted ({rate:.1f} %), "
+                f"{per:.2f} tokens/round")
+
+
+DRAFT_TOKENS = (1, 3, 7)   # --draft-tokens: the verify forward runs k + 1 rows, a power of two
+
+
+class DraftRefused(ValueError):
+    """A --draft-model setting this configuration cannot run (see draft_refusal)."""
+
+
+def draft_refusal(draft_tokens: int, n_ranks: int = 1, parallel: int = 1, headers: Sequence = ()) -> Optional[str]:
+    """Why greedy speculative decoding with a draft model of `draft_tokens` drafts per round cannot run here, or None if it can.
+    headers: (name, model header) of the target and the draft, checked once they are read (the draft's with the target's context
+    length: a shorter draft context is refused)."""
+    if draft_tokens not in DRAFT_TOKENS:
+        return "--draft-tokens must be 1, 3 or 7"
+    if n_ranks > 1:
+        return "--draft-model runs on one GPU only (no --gpus > 1 or --workers)"
+    if os.environ.get("DL_COLLECTIVES") == "nccl":
+        return "--draft-model does not support DL_COLLECTIVES=nccl"
+    if parallel > 1:
+        return "--draft-model does not combine with --parallel > 1"
+    H = host() if headers else None
+    for name, h in headers:
+        if h.n_experts > 0:
+            return f"--draft-model needs dense models: the {name} is mixture-of-experts (no batched verify step)"
+        if h.weight_type != H.F_Q40:
+            return f"--draft-model needs q40 weights: the {name} has {H.float_type_name(h.weight_type)} weights"
+    if len(headers) == 2:
+        t, d = headers[0][1], headers[1][1]
+        if t.vocab_size != d.vocab_size:
+            return f"--draft-model needs the target's vocabulary: {t.vocab_size} tokens against {d.vocab_size}"
+        if d.seq_len < t.seq_len:
+            return f"--draft-model needs a context of at least {t.seq_len} tokens: the draft model has {d.seq_len}"
+    return None
+
+
 class TokenSteps:
     """The token steps of one engine, the backend run_choices needs: InferenceSession for the library and
     apps.runtime.RootInference for the CLIs and API server, which announces every engine call to the workers (_send).
@@ -176,10 +235,13 @@ class TokenSteps:
     library's (multi-node) or DL_HOST_SAMPLER is set: then the host sampler draws from logits copied back. The device's
     generator, controls and filters are handed over when the sampler's differ from what the device holds."""
 
-    def __init__(self, engine, device, n_ranks: int):
+    def __init__(self, engine, device, n_ranks: int, draft=None, draft_tokens: int = 3):
         self.engine = engine
         self.device = torch.device(device)
         self.n_ranks = n_ranks
+        self.draft = draft                  # runtime.engine.Engine of the draft model, or None (speculates)
+        self.draft_tokens = draft_tokens
+        self.spec_stats = SpecStats()
         # the caller synchronises every step, so one pinned staging slot is enough (workers enqueue ahead: pageable staging)
         on_gpu = self.device.type == "cuda"
         self._pin_in = torch.zeros(2, dtype=torch.int32).pin_memory() if on_gpu else None
@@ -201,6 +263,8 @@ class TokenSteps:
         if tokens:
             self._send(OP_PREFILL, pos, tokens)
             self.engine.prefill(tokens, pos, want_logits=False)
+            if self.draft is not None:
+                self.draft.prefill(tokens, pos, want_logits=False)
 
     def forward_logits(self, token: int, pos: int) -> torch.Tensor:
         self._send(OP_STEP_LOGITS, pos, [token])
@@ -263,6 +327,18 @@ class TokenSteps:
         self._send(OP_STEP_SAMPLE, pos, [token] + _f32_bits(sampler.temperature, sampler.topp))
         self.engine.step_sampled(token, pos, sampler.temperature, sampler.topp)
         return self._read_token(logprobs, controlled=True)
+
+    def speculates(self, sampler) -> bool:
+        """Whether a single completion with these sampler settings decodes in speculative rounds: a draft model is loaded and
+        the draw is plain greedy (temperature 0, no penalties or logit bias). Requests with logprobs or n > 1 never do."""
+        return self.draft is not None and sampler.temperature == 0.0 and not sampler.controls_active
+
+    def spec_round(self, token: int, pos: int) -> List[int]:
+        """One speculative round from the last emitted token at `pos` (runtime.engine.Engine.spec_round): the tokens greedy
+        decoding emits next, one to draft_tokens + 1 of them."""
+        toks, accepted, drafted = self.engine.spec_round(self.draft, token, pos, self.draft_tokens)
+        self.spec_stats.add(drafted, accepted, len(toks))
+        return toks
 
     def last_logprobs(self) -> list:
         """Per row of the last step that was asked for logprobs (next_token: one row; choices_first / choices_step: one per
@@ -441,7 +517,8 @@ class InferenceSession(TokenSteps):
                  temperature: float = 0.0, topp: float = 0.9, seed: int = 12345, device: Optional[str] = None,
                  max_batch: int = 8, use_pdl: bool = True, comm=None, moe_mode: str = "auto", presence_penalty: float = 0.0,
                  frequency_penalty: float = 0.0, logit_bias: Optional[dict] = None, parallel: int = 1,
-                 kv_cache_float_type: str = "bf16", top_k: int = 0, min_p: float = 0.0, parallel_cache: str = "split"):
+                 kv_cache_float_type: str = "bf16", top_k: int = 0, min_p: float = 0.0, parallel_cache: str = "split",
+                 draft_model: Optional[str] = None, draft_tokens: int = 3):
         """presence_penalty, frequency_penalty and logit_bias ({token id: value}) are the sampling controls of every
         completion (host Sampler.set_controls; they may be changed later through self.sampler.set_controls, which restarts the
         counts of the current completion). top_k and min_p are the sampling filters of every sampled draw (host
@@ -449,7 +526,9 @@ class InferenceSession(TokenSteps):
         (slot_prefill, slot_copy, slot_sampling, slots_step); the single-sequence calls then must not be used.
         kv_cache_float_type: "bf16" or "q80" (runtime.engine.Engine). parallel_cache: the layout of the slots, "split" (each
         slot owns floor(context / parallel) rows) or "paged" (the slots share the cache as one pool of 64-row pages, so one
-        request may use the whole context; see SlotScheduler for the rules)."""
+        request may use the whole context; see SlotScheduler for the rules). draft_model: the `.m` file of a smaller model with the
+        target's tokenizer; single greedy completions then decode in speculative rounds of draft_tokens (1, 3 or 7) drafts that
+        this model checks in one batched forward, with the tokens of plain greedy decoding (DraftRefused where it cannot run)."""
         from .models.loader import load_device_weights
         from .runtime.engine import Engine
 
@@ -461,11 +540,22 @@ class InferenceSession(TokenSteps):
             raise ParallelRefused(why)
         rank = comm.rank if comm is not None else 0
         n_ranks = comm.world_size if comm is not None else 1
+        draft_file = None
+        if draft_model is not None:
+            # the draft follows the target's context length and KV-cache storage
+            draft_file = ModelFile(draft_model, self.header.seq_len)
+            why = draft_refusal(draft_tokens, n_ranks, parallel, (("target model", self.header), ("draft model", draft_file.header)))
+            if why:
+                raise DraftRefused(why)
         if device is None:
             device = f"cuda:{torch.cuda.current_device()}"
         self.weights = load_device_weights(self.model_file, rank, n_ranks, torch.device(device), moe_mode=moe_mode, comm=comm)
+        draft = None
+        if draft_file is not None:
+            draft = Engine(load_device_weights(draft_file, 0, 1, torch.device(device)), max_batch=max_batch, use_pdl=use_pdl,
+                           kv_cache_float_type=kv_cache_float_type)
         super().__init__(Engine(self.weights, max_batch=max_batch, use_pdl=use_pdl, comm=comm, kv_cache_float_type=kv_cache_float_type),
-                         device, n_ranks)
+                         device, n_ranks, draft, draft_tokens)
         H = host()
         self.tokenizer = H.Tokenizer(tokenizer_path) if tokenizer_path else None
         vocab = self.tokenizer.vocab_size if self.tokenizer else self.header.vocab_size
@@ -473,7 +563,9 @@ class InferenceSession(TokenSteps):
         self.sampler.set_controls(presence_penalty, frequency_penalty, sorted((int(k), float(v)) for k, v in (logit_bias or {}).items()))
         self.sampler.set_filters(top_k, min_p)
         if self.tokenizer and self.tokenizer.vocab_size < self.header.vocab_size:
-            self.engine.set_vocab_limit(self.tokenizer.vocab_size)
+            for e in (self.engine, self.draft):
+                if e is not None:
+                    e.set_vocab_limit(self.tokenizer.vocab_size)
         self.pos = 0
         self.slots = parallel
         if parallel > 1:
@@ -581,12 +673,18 @@ class InferenceSession(TokenSteps):
         self.tokenizer.reset_decoder()
         self.sampler.begin_completion()
         out = []
-        while self.pos < min(steps, self.header.seq_len):
-            tok = self.next_token(tok)
-            piece = self.tokenizer.decode(tok).decode("utf-8", errors="replace")
-            out.append(piece)
-            if on_piece:
-                on_piece(piece)
-            if self.tokenizer.is_eos(tok):
-                break
+        limit = min(steps, self.header.seq_len)
+        spec = self.speculates(self.sampler)
+        while self.pos < limit:
+            toks = self.spec_round(tok, self.pos) if spec else [super().next_token(tok, self.pos, self.sampler)]
+            for tok in toks:
+                self.pos += 1
+                piece = self.tokenizer.decode(tok).decode("utf-8", errors="replace")
+                out.append(piece)
+                if on_piece:
+                    on_piece(piece)
+                if self.tokenizer.is_eos(tok):
+                    return "".join(out)
+                if self.pos >= limit:
+                    break
         return "".join(out)

@@ -18,8 +18,8 @@ from types import SimpleNamespace
 from typing import Dict, List, Optional, Tuple
 
 from .. import host
-from ..api import (MAX_CHOICES, MAX_TOP_LOGPROBS, ParallelRefused, SlotRequest, SlotScheduler, check_logprobs, check_stop,
-                   parallel_refusal, run_choices)
+from ..api import (MAX_CHOICES, MAX_TOP_LOGPROBS, DraftRefused, ParallelRefused, SlotRequest, SlotScheduler, check_logprobs,
+                   check_stop, draft_refusal, parallel_refusal, run_choices)
 from .args import AppArgs, parse_args
 from .cli import make_chat_tools
 from .runtime import AppContext, run_inference_app
@@ -587,11 +587,13 @@ USAGE = """Usage: dllama-api {--model <path>} {--tokenizer <path>} [--host <addr
         [--buffer-float-type {f32|f16|q40|q80}] [--max-seq-len <max>] [--gpus <n>] [--workers <ip:port> ...]
         [--temperature <temp>] [--topp <t>] [--presence-penalty <p>] [--frequency-penalty <f>] [--seed <s>]
         [--top-k <k>] [--min-p <p>] [--chat-template {llama2|llama3|deepSeek3|chatml}] [--parallel <n>]
-        [--parallel-cache {split|paged}]
+        [--parallel-cache {split|paged}] [--draft-model <path>] [--draft-tokens {1|3|7}]
         --parallel <n>: decode up to n (1..8) chat requests together, each in its own KV-cache slot of
                         floor(context / n) tokens; single GPU and dense models only
         --parallel-cache paged: the slots share the KV cache as one pool of 64-token pages instead, so a request
                         may use the whole context while the pool has room (default split)
+        --draft-model <path>: greedy single-completion requests decode in speculative rounds: the draft (same
+                        tokenizer, dense q40) proposes --draft-tokens tokens (default 3), the model checks them at once
 """
 
 
@@ -602,7 +604,10 @@ def main(argv=None) -> int:
     if args.help:
         sys.stderr.write(USAGE)
         return 0
-    why = parallel_refusal(args.parallel, max(args.gpus, 1, int(os.environ.get("WORLD_SIZE", "1"))) + len(args.workers), 0, args.parallel_cache)
+    n_ranks = max(args.gpus, 1, int(os.environ.get("WORLD_SIZE", "1"))) + len(args.workers)
+    why = parallel_refusal(args.parallel, n_ranks, 0, args.parallel_cache)
+    if not why and args.draft_model is not None:
+        why = draft_refusal(args.draft_tokens, n_ranks, args.parallel)
     if why:
         sys.stderr.write(why + "\n")
         return 1
@@ -630,7 +635,7 @@ def main(argv=None) -> int:
         try:
             run_inference_app(args, serve)
             return 0
-        except ParallelRefused as e:   # found once the model header is read (mixture of experts)
+        except (ParallelRefused, DraftRefused) as e:   # found once the model headers are read
             sys.stderr.write(f"{e}\n")
             return 1
         except (ConnectionError, RuntimeError) as e:

@@ -45,6 +45,8 @@ class AppArgs:
     parallel: int = 1        # dllama-api: chat requests decoded together, one KV-cache slot each (1..8)
     parallel_cache: str = "split"   # dllama-api: the slots' KV-cache layout: split (floor(context / n) rows each) | paged (shared 64-row pages)
     kv_cache_float_type: str = "bf16"   # KV-cache storage: bf16 | q80 (int8 blocks of 32 with an f16 scale)
+    draft_model: Optional[str] = None   # greedy speculative decoding: a smaller model with the same tokenizer drafts tokens
+    draft_tokens: int = 3               # drafts per round: 1, 3 or 7 (checked by api.draft_refusal)
 
 
 FLOAT_TYPES = ("f32", "f16", "q40", "q80")
@@ -139,6 +141,10 @@ def parse_args(argv: List[str], require_mode: bool) -> AppArgs:
             if value not in KV_CACHE_FLOAT_TYPES:
                 raise ValueError(f"Invalid KV-cache float type: {value} (expected bf16 or q80)")
             a.kv_cache_float_type = value
+        elif name == "--draft-model":
+            a.draft_model = value
+        elif name == "--draft-tokens":
+            a.draft_tokens = int(value)
         elif name == "--parallel" and not require_mode:   # dllama-api only; its range is checked by api.parallel_refusal
             a.parallel = int(value)
         elif name == "--parallel-cache" and not require_mode:   # dllama-api only; checked by api.parallel_refusal
@@ -155,6 +161,8 @@ USAGE = """Usage: dllama {inference|chat|perplexity|worker} {--model <path>} {--
         [--top-k <k>] [--min-p <p>]        sampling filters of sampled draws (default 0 = off)
         [--chat-template {llama2|llama3|deepSeek3|chatml}]
         [--kv-cache-float-type {bf16|q80}] KV-cache storage (default bf16; q80 = int8 blocks of 32 + f16 scale)
+        [--draft-model <path>] [--draft-tokens {1|3|7}]
+                                          greedy speculative decoding: the draft proposes k tokens (default 3) per round
         [--gpus <n>]                      run tensor-parallel on n local GPUs (spawns one process per GPU)
         [--workers <ip:port> ...] [--nthreads <n>] [--net-turbo {0|1}] [--gpu-index <i>] [--gpu-segments <a:b>]
                                           accepted for compatibility with the reference CLI

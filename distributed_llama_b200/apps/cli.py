@@ -12,6 +12,7 @@ import numpy as np
 import torch
 
 from .. import host
+from ..api import DraftRefused, draft_refusal
 from .args import AppArgs, USAGE, parse_args
 from .runtime import AppContext, run_inference_app, init_distributed_from_env
 
@@ -61,23 +62,28 @@ def inference(ctx: AppContext) -> None:
     n_pred = 0
     sync_prev = ctx.sess.engine.sync_ns() if inf.comm is not None else 0
     sync_total_us = 0
+    spec = inf.speculates(ctx.sampler)
     while pos < max_pos:
         torch.cuda.synchronize(dev)
         t0 = time.perf_counter()
-        token = inf.next_token(token, pos, ctx.sampler)
+        # a speculative round emits several tokens: each line shows its share of the round's time
+        toks = inf.spec_round(token, pos) if spec else [inf.next_token(token, pos, ctx.sampler)]
         dt = (time.perf_counter() - t0) * 1000
         pred_ms += dt
-        piece = tok.decode(token).decode("utf-8", errors="replace")
-        sent, recv = ctx.sess.engine.link_bytes(1)
-        sync_now = ctx.sess.engine.sync_ns() if inf.comm is not None else 0
-        sync_us, sync_prev = (sync_now - sync_prev) // 1000, sync_now
-        sync_total_us += sync_us
-        # Sync = time the decode kernel waited for peer ranks inside its fused all-reduces (a token takes ~1 ms: mostly prints 0;
-        # the per-token average in microseconds is part of the summary)
-        print(f"🔶 Pred{int(dt):5d} ms Sync{sync_us // 1000:5d} ms | Sent{sent // 1024:6d} kB Recv{recv // 1024:6d} kB | {piece if piece else '~'}")
-        sys.stdout.flush()
-        pos += 1
-        n_pred += 1
+        for token in toks:
+            piece = tok.decode(token).decode("utf-8", errors="replace")
+            sent, recv = ctx.sess.engine.link_bytes(1)
+            sync_now = ctx.sess.engine.sync_ns() if inf.comm is not None else 0
+            sync_us, sync_prev = (sync_now - sync_prev) // 1000, sync_now
+            sync_total_us += sync_us
+            # Sync = time the decode kernel waited for peer ranks inside its fused all-reduces (a token takes ~1 ms: mostly prints 0;
+            # the per-token average in microseconds is part of the summary)
+            print(f"🔶 Pred{int(dt / len(toks)):5d} ms Sync{sync_us // 1000:5d} ms | Sent{sent // 1024:6d} kB Recv{recv // 1024:6d} kB | {piece if piece else '~'}")
+            sys.stdout.flush()
+            pos += 1
+            n_pred += 1
+            if pos >= max_pos:
+                break
     n_eval = n_in - 1
     print()
     print("Evaluation")
@@ -91,6 +97,8 @@ def inference(ctx: AppContext) -> None:
         print(f"   tokens/s: {n_pred * 1000 / pred_ms:3.2f} ({pred_ms / n_pred:3.2f} ms/tok)")
         if inf.comm is not None:
             print(f"   syncTime: {sync_total_us / n_pred:3.1f} us/tok (waiting for peer ranks inside the fused all-reduces)")
+    if inf.draft is not None:
+        print(inf.spec_stats.line())
 
 
 def perplexity(ctx: AppContext) -> None:
@@ -163,20 +171,24 @@ def chat(ctx: AppContext) -> None:
         print("\n🤖 Assistant")
         if public:
             print(public.decode("utf-8", errors="replace"), end="")
-        while pos < seq_len:
-            token = inf.next_token(token, pos, ctx.sampler)
-            piece = tok.decode(token)
-            kind = det.append(token, piece)
-            if kind in (H.NOT_EOS, H.EOS):
-                delta = det.get_delta()
-                if delta:
-                    print(delta.decode("utf-8", errors="replace"), end="", flush=True)
-                det.reset()
-            pos += 1
-            if kind == H.EOS:
-                break
+        spec = inf.speculates(ctx.sampler)
+        kind = None
+        while pos < seq_len and kind != H.EOS:
+            for token in (inf.spec_round(token, pos) if spec else [inf.next_token(token, pos, ctx.sampler)]):
+                piece = tok.decode(token)
+                kind = det.append(token, piece)
+                if kind in (H.NOT_EOS, H.EOS):
+                    delta = det.get_delta()
+                    if delta:
+                        print(delta.decode("utf-8", errors="replace"), end="", flush=True)
+                    det.reset()
+                pos += 1
+                if kind == H.EOS or pos >= seq_len:
+                    break
         items = []
     print("(end of context)")
+    if inf.draft is not None:
+        print(inf.spec_stats.line())
 
 
 def worker(args: AppArgs) -> None:
@@ -205,6 +217,10 @@ def main(argv=None) -> int:
         if args.help or args.mode is None:
             print(USAGE)
             return 0
+        if args.draft_model is not None:
+            why = draft_refusal(args.draft_tokens, max(args.gpus, 1, int(os.environ.get("WORLD_SIZE", "1"))) + len(args.workers))
+            if why:
+                raise DraftRefused(why)
         if args.gpus > 1 and os.environ.get("DLLAMA_SPAWNED") != "1" and int(os.environ.get("WORLD_SIZE", "1")) == 1:
             return _respawn_with_torchrun(argv, args.gpus)
         if args.mode == "inference":

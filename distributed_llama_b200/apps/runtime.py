@@ -72,7 +72,8 @@ class RootInference(TokenSteps):
     or torch.distributed broadcasts without a channel; the activations never leave the GPUs."""
 
     def __init__(self, sess: InferenceSession, comm, chan=None):
-        super().__init__(sess.engine, sess.device, comm.world_size if comm is not None else 1)
+        super().__init__(sess.engine, sess.device, comm.world_size if comm is not None else 1,
+                         getattr(sess, "draft", None), getattr(sess, "draft_tokens", 3))
         self.comm = comm
         self.chan = chan
         self._ctl = torch.zeros(4, dtype=torch.int64, device=self.device) if (comm is not None and chan is None) else None
@@ -187,7 +188,8 @@ def run_inference_app(args: AppArgs, handler: Callable[[AppContext], None]) -> N
                             presence_penalty=args.presence_penalty, frequency_penalty=args.frequency_penalty,
                             parallel=getattr(args, "parallel", 1), parallel_cache=getattr(args, "parallel_cache", "split"),
                             kv_cache_float_type=args.kv_cache_float_type,
-                            top_k=getattr(args, "top_k", 0), min_p=getattr(args, "min_p", 0.0))
+                            top_k=getattr(args, "top_k", 0), min_p=getattr(args, "min_p", 0.0),
+                            draft_model=args.draft_model, draft_tokens=args.draft_tokens)
     chan = open_control_channel(comm)
     if rank != 0:
         worker_loop(sess, comm, chan)

@@ -244,6 +244,18 @@ def lib() -> C.CDLL:
     L.dl_engine_decode_graph.restype = i32
     L.dl_engine_graph_captured.argtypes = [vp]
     L.dl_engine_graph_captured.restype = i32
+    L.dl_spec_round.argtypes = [vp, vp, i32, i32, i32, i32, ip, vp]
+    L.dl_spec_round.restype = i32
+    L.dl_engine_verify.argtypes = [vp, i32, ip, vp]
+    L.dl_engine_verify.restype = i32
+    L.dl_spec_accept.argtypes = [vp, vp, vp, vp, u32, vp, vp, vp, u32, u32, vp, vp]
+    L.dl_spec_accept.restype = i32
+    L.dl_gemv_q40_argmax_rows.argtypes = [vp, vp, u32, u32, vp, vp, f32, vp, vp, vp, vp, vp, u32, i32, i32, vp]
+    L.dl_gemv_q40_argmax_rows.restype = i32
+    L.dl_argmax_rows.argtypes = [vp, u32, u32, i32, vp, vp]
+    L.dl_argmax_rows.restype = i32
+    if L.dl_spec_result_words() != SPEC_RESULT_WORDS:
+        raise RuntimeError(f"{path}: speculative result block of {L.dl_spec_result_words()} words, expected {SPEC_RESULT_WORDS}")
     _lib = L
     return L
 
@@ -262,7 +274,16 @@ _ERRORS = {
     -66: "a slot position past the rows the slot holds",
     -68: "the KV-cache page pool has too few free pages",
     -69: "paged KV-cache slots need the tensor-core prefill attention",
+    -71: "speculative round at a position past the context",
+    -72: "the draft model must be a second engine with the target's vocabulary and KV-cache float type",
+    -73: "speculative decoding needs one GPU, dense q40 models and no KV-cache slots",
+    -74: "device-side wait timed out during a speculative round",
+    -75: "--draft-tokens must be 1, 3 or 7",
+    -77: "out of device or pinned memory for the speculative-decoding state",
 }
+
+# Speculative rounds (dl_spec_round): int32 result block [accepted, emitted, drafts, position of the last emitted token, tokens...]
+SPEC_RESULT_WORDS, SPEC_RESULT_HEAD = 12, 4
 
 POOL_SHORT = -68   # dl_engine_slot_reserve / dl_engine_slot_copy: too few free pages, nothing changed
 PAGE_ROWS = 64     # rows of a KV-cache page (paged slots)

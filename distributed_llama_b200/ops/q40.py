@@ -192,3 +192,16 @@ def rmsnorm_bf16(x: torch.Tensor, w: Optional[torch.Tensor], eps: float, out: Op
     cl.check(cl.lib().dl_rmsnorm_bf16(x.data_ptr(), x.stride(0), w.data_ptr() if w is not None else None, out.data_ptr(), out.stride(0),
                                       n, eps, T, cl.stream_ptr()), "rmsnorm_bf16")
     return out
+
+
+def gemv_q40_argmax_rows(w: DeviceQ40, x: torch.Tensor, *, norm_w: torch.Tensor, eps: float, out: torch.Tensor, arg_val: torch.Tensor,
+                         arg_idx: torch.Tensor, arg_counter: torch.Tensor, tokens: torch.Tensor, vocab_limit: int = 0,
+                         num_sms: int = 0) -> None:
+    """Fused logits + per-row arg-max of nb = x.shape[0] (2, 4 or 8) rows on the TMA kernel (the verify step of speculative
+    decoding): out [nb][d] = logits of rmsnorm(x[b]); tokens[b] = lowest-index maximum of row b among rows < vocab_limit (0: all).
+    arg_val / arg_idx: nb x grid entries; arg_counter: zero, left at zero. Raises with code 1 where the shape does not fit."""
+    if num_sms == 0:
+        num_sms = torch.cuda.get_device_properties(x.device).multi_processor_count
+    cl.check(cl.lib().dl_gemv_q40_argmax_rows(w.qs.data_ptr(), w.scales.data_ptr(), w.d, w.n, x.data_ptr(), norm_w.data_ptr(), eps,
+                                              out.data_ptr(), arg_val.data_ptr(), arg_idx.data_ptr(), arg_counter.data_ptr(),
+                                              tokens.data_ptr(), vocab_limit, x.shape[0], num_sms, cl.stream_ptr()), "gemv_q40_argmax_rows")

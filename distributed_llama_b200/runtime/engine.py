@@ -661,6 +661,29 @@ class Engine:
         """True while the engine holds a decode graph of its current configuration (captured on the first graph step)."""
         return bool(self._lib.dl_engine_graph_captured(self._h))
 
+    # -- speculative decoding with a draft model (csrc/cuda/speculative.cu) --
+    def spec_round(self, draft: "Engine", token: int, pos: int, k: int, use_graph: bool = True) -> tuple:
+        """One round of greedy speculative decoding with this engine as the target: `token` is the last emitted token at `pos`,
+        both engines hold valid KV rows for every position before it. The draft proposes k (1, 3 or 7; fewer near the end of the
+        context) tokens, this engine checks them in one batched forward. Returns (emitted tokens, accepted drafts, drafts): the
+        accepted drafts followed by this engine's own token after them, the tokens greedy decoding emits from (token, pos)."""
+        out = (C.c_int32 * cl.SPEC_RESULT_WORDS)()
+        cl.check(self._lib.dl_spec_round(self._h, draft._h, int(token), int(pos), int(k), 1 if use_graph else 0, out, cl.stream_ptr()),
+                 "spec_round")
+        n = out[1]
+        return list(out[cl.SPEC_RESULT_HEAD:cl.SPEC_RESULT_HEAD + n]), int(out[0]), int(out[2])
+
+    def verify(self, tokens: Sequence[int], start_pos: int) -> List[int]:
+        """The verify forward of a speculative round over len(tokens) in {2, 4, 8} tokens at consecutive positions: logits of
+        every row in logits[:n] and the arg-max of each row (lowest id among ties, ids at or above the vocabulary limit ignored)."""
+        n = len(tokens)
+        if start_pos + n > self.seq_len:
+            raise ValueError("position beyond the context length")
+        self._set_inputs(tokens, start_pos)
+        out = (C.c_int32 * n)()
+        cl.check(self._lib.dl_engine_verify(self._h, n, out, cl.stream_ptr()), "engine_verify")
+        return list(out)
+
     def decode_greedy(self, first_token: int, start_pos: int, n_steps: int, use_graph: bool = True) -> List[int]:
         """Generates n_steps tokens greedily: step i consumes the token at position start_pos+i and emits the next.
         The loop runs entirely on the device (token + position live in device memory)."""
